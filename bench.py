@@ -1,7 +1,7 @@
 #!/usr/bin/env python3
-"""bench.py -- correspondence + linearisation + reduction throughput of the small_gicp hot path on B200.
+"""bench.py -- correspondence + linearisation + reduction throughput of the small_gicp hot path on H100.
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--points P] [--no-extras]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--points P] [--no-extras] [--dump-outputs DIR]
   python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 ... bench.py --gpus N ...
 
 Headline workload (BASELINE.json configs[1]): synthetic room pair, P = 1,000,000 target points and 1,000,000 source points PER GPU,
@@ -20,9 +20,12 @@ Extras on the same line (the other BASELINE configs on hardware; skipped with --
 `c1`           configs[0]: the bundled PLY pair, ICP, helper align() vs the 1-thread CPU pipeline; per-call latency (N = 1 only).
 `c3`           configs[2]: 120k-ray LiDAR stream, per frame voxel grid / tree + grid / covariances / LM align (N = 1 only).
 `c4`           configs[3]: 10M-point VGICP, LevenbergMarquardt, ONE source strong-sharded over the N GPUs.
-`c5`           configs[4]: linearize over 100k .. 100M points (ONE cloud pair, source strong-sharded over the N GPUs).
+`c5`           configs[4]: linearize over 100k .. 50M points (ONE cloud pair, source strong-sharded over the N GPUs; 50M is the
+               largest size of the sweep whose target, block lists and construction scratch fit one 80 GB H100).
 `allreduce_check_rel`  N > 1: |fused sum - NCCL sum of the per-rank local sums| / |sum| (must be <= 1e-12).
 `comm_wait_us` N > 1: time the finishing CTA waited for its peers per exchange: min over ranks = transport, max - min = skew.
+--dump-outputs DIR  after the timed steps: what the last timed step returned (H, b, e, inlier count) and its correspondences, as
+               DIR/<name>.npy (float64), so that two builds can be compared output for output on identical seeded inputs.
 """
 import argparse
 import json
@@ -41,7 +44,7 @@ if ROOT not in sys.path:
 METRIC = "correspondence+reduction Mpoints/sec per GICP iter"
 UNIT = "Mpoints/s"
 BYTES_PER_POINT = {"ICP": 36, "PLANE_ICP": 52, "GICP": 100, "VGICP": 116}  # SURVEY.md §8(d)
-HBM_FALLBACK_GBS = 6650.0  # /opt/skills/guides/B200_PROFILING.md fallback
+HBM_FALLBACK_GBS = 3350.0  # H100 SXM data sheet (HBM3); not a measured figure
 
 
 def parse_args():
@@ -54,10 +57,11 @@ def parse_args():
     ap.add_argument("--covs", default="knn", choices=["knn", "analytic"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-extras", action="store_true", help="skip c3 / c4 / c5 (profiler runs)")
-    ap.add_argument("--c5-sizes", default="100000,1000000,10000000,100000000")
+    ap.add_argument("--c5-sizes", default="100000,1000000,10000000,50000000")
     ap.add_argument("--c4-points", type=int, default=10_000_000)
     ap.add_argument("--c3-frames", type=int, default=12)
     ap.add_argument("--leaf", type=int, default=0, help="max leaf size of the device kd-tree (0 = library default)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR", help="write the last timed step's outputs to DIR/<name>.npy")
     return ap.parse_args()
 
 
@@ -70,7 +74,7 @@ def hbm_peak():
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs, burst copy)"
     except Exception:
-        return HBM_FALLBACK_GBS, "fallback (B200_PROFILING.md)"
+        return HBM_FALLBACK_GBS, "H100 SXM data sheet (3.35 TB/s), not measured"
 
 
 # ------------------------------------------------------------------------------------------------
@@ -169,7 +173,7 @@ def lm_align(linearize, error, max_iterations=20, max_inner=10, lam=1e-3, lam_fa
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region."""
 
     Q = "index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
 
@@ -466,6 +470,25 @@ class Bench:
             b.record(self.stream)
         self.barrier()
         return self.max_over_ranks([float(np.mean([a.elapsed_time(b) for a, b in ev]))])[0]
+
+
+DUMP_CORR_MAX = 1 << 21  # correspondences dumped in full up to this many source points, else a fixed seeded sample of this size
+
+
+def dump_outputs(path, hbe, corr):
+    """what the timed path returned in its last step: H (6x6), b (6), e and the inlier count (H|b|e|inliers of sgb_linearize), and the
+    correspondences it used (target index per source point, -1 = rejected / none); all float64, at most ~34 MB in all"""
+    os.makedirs(path, exist_ok=True)
+    c = corr.astype(np.float64)
+    c[corr == np.iinfo(np.uint64).max] = -1.0
+    arrays = {"H": hbe[:36].reshape(6, 6), "b": hbe[36:42], "e": hbe[42:43], "inliers": hbe[43:44]}
+    if len(c) > DUMP_CORR_MAX:
+        idx = np.sort(np.random.default_rng(0).choice(len(c), DUMP_CORR_MAX, replace=False))
+        arrays["correspondences_index"] = idx.astype(np.float64)
+        c = c[idx]
+    arrays["correspondences"] = c
+    for name, a in arrays.items():
+        np.save(os.path.join(path, name + ".npy"), np.ascontiguousarray(a, dtype=np.float64))
 
 
 def shard(n, rank, world):
@@ -922,6 +945,8 @@ def run_ours(args):
         ev[i][1].record(stream)
     barrier()
     launches = ctx.kernel_launches - launches0
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, out[:44].cpu().numpy(), ctx.correspondences())
     step_ms = np.array([a.elapsed_time(b) for a, b in ev])
     kern_ms = np.array([a.elapsed_time(b) for a, b in kev])
     total_ms = float(step_ms.sum())

@@ -1,5 +1,5 @@
 // SPDX-License-Identifier: MIT
-// How a user of koide3/small_gicp calls the B200 backend: the three entry levels of the reference's public API -- the one-call
+// How a user of koide3/small_gicp calls the H100 backend: the three entry levels of the reference's public API -- the one-call
 // helper, pre-processing + align, and the Registration<> template -- exercised on a pair of PLY files.  Inside the reference
 // tree the includes would be <small_gicp/...> plus <small_gicp/registration/reduction_cuda.hpp> (INTEGRATION.md); here they
 // come from this repository's Eigen-free mirror of the same surface.  All per-point work (voxel grid, normals / covariances,

@@ -1,6 +1,6 @@
 /* SPDX-License-Identifier: MIT
  *
- * sgicp_b200.h -- C-ABI of the B200-native small_gicp hot path (libsgicp_b200.so).
+ * sgicp_b200.h -- C-ABI of the H100-native small_gicp hot path (libsgicp_b200.so).
  *
  * One context = one GPU = one CUDA stream.  A context is NOT thread-safe; distinct contexts are
  * (the reference runs several align() calls concurrently from TBB flow-graph nodes,

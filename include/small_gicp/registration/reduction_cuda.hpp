@@ -1,7 +1,7 @@
 // SPDX-License-Identifier: MIT
-// include/small_gicp/registration/reduction_cuda.hpp -- the ONE header a maintainer adds to koide3/small_gicp to get the B200
+// include/small_gicp/registration/reduction_cuda.hpp -- the ONE header a maintainer adds to koide3/small_gicp to get the H100
 // backend (plus `target_link_libraries(... sgicp_b200)`).  It is written against the reference's own types and compiled,
-// unmodified, by tests/host_ref/ against /root/reference/include (the reference's headers in place) -- INTEGRATION.md shows
+// unmodified, by tests/host_ref/ against the reference's include/ directory (its headers in place) -- INTEGRATION.md shows
 // this file, not a sketch of it.
 //
 // ParallelReductionCUDA is a peer of SerialReduction / ParallelReductionOMP / ParallelReductionTBB
@@ -137,7 +137,7 @@ struct CloudArrays {
 
 }  // namespace cuda_detail
 
-/// Reduction on a B200 (one CUDA context per object; copies share it).
+/// Reduction on an H100 (one CUDA context per object; copies share it).
 ///
 /// When are the clouds (re)uploaded?  The reference's reductions re-read host memory on every call.  This one mirrors target,
 /// search structure and source to the device at the FIRST linearize() of every align() -- recognised by the freshly constructed

@@ -1,7 +1,7 @@
-"""B200-native small_gicp hot path: ctypes front-end of libsgicp_b200.so (C-ABI in include/sgicp_b200.h).
+"""H100-native small_gicp hot path: ctypes front-end of libsgicp_b200.so (C-ABI in include/sgicp_b200.h).
 
 There is no CPU fallback: importing works anywhere (the library only needs libcudart), but creating a
-Context without a B200 raises, and a missing library raises at import of `capi`.
+Context without an H100 raises, and a missing library raises at import of `capi`.
 """
 from .capi import (  # noqa: F401
     Context,

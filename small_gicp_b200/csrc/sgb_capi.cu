@@ -1,5 +1,5 @@
 // SPDX-License-Identifier: MIT
-// Context + C-ABI (include/sgicp_b200.h) of the B200-native small_gicp hot path.
+// Context + C-ABI (include/sgicp_b200.h) of the H100-native small_gicp hot path.
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -422,8 +422,8 @@ int sgb_create(int device_id, sgb_ctx** out_ctx) {
     g_create_error = std::string("cudaGetDeviceProperties: ") + cudaGetErrorString(e);
     return 2;
   }
-  if (prop.major != 10) {
-    g_create_error = "sgb_create: kernels are built for sm_100a (B200) only; found sm_" + std::to_string(prop.major) + std::to_string(prop.minor);
+  if (prop.major != 9 || prop.minor != 0) {
+    g_create_error = "sgb_create: kernels are built for sm_90a (H100) only; found sm_" + std::to_string(prop.major) + std::to_string(prop.minor);
     return 3;
   }
   sgb_ctx* ctx = new sgb_ctx();
@@ -443,11 +443,11 @@ int sgb_create(int device_id, sgb_ctx** out_ctx) {
     return 2;
   }
   ctx->stream = ctx->own_stream;
-#ifdef SGB_PROFILING  // libsgicp_b200_prof.so only: the A/B switches behind the experiment log in profiles/ (the product library reads no environment variable)
-  if (const char* s = getenv("SGB_SEARCH")) ctx->search_mode = atoi(s);  // profiling switch (profiles/r01): 0 fused, 1 per-thread, 2 packet
+#ifdef SGB_PROFILING  // libsgicp_b200_prof.so only: the A/B switches of the experiments (the product library reads no environment variable)
+  if (const char* s = getenv("SGB_SEARCH")) ctx->search_mode = atoi(s);  // profiling switch: 0 fused, 1 per-thread, 2 packet
   if (const char* s = getenv("SGB_CURVE")) set_source_curve(atoi(s));     // profiling switch: 0 Morton, 1 Hilbert (default)
   if (const char* s = getenv("SGB_GRID")) ctx->use_grid = !(s[0] == '0');  // profiling switch: 0 = tree search only
-  // profiling switches of the grid front end (A/B runs in profiles/, variants exercised by tests/test_gpu_parity.py)
+  // profiling switches of the grid front end (A/B runs, variants exercised by tests/test_gpu_parity.py)
   if (const char* s = getenv("SGB_RING")) ctx->use_ring = !(s[0] == '0');                   // 0 = pending queries always walk the tree
   if (const char* s = getenv("SGB_PENDING_DIV")) ctx->pending_div = std::max(1, atoi(s));   // packet search when more than n / div queries are pending
   if (const char* s = getenv("SGB_GRID_CELL")) {                                            // cell edge in units of the median point spacing

@@ -44,7 +44,7 @@ int build_lbvh(sgb_ctx* ctx, const float4* d_orig_pts, size_t n, const double* d
   CU(launch_gather(perm.as<uint32_t>(), n, d_orig_pts, leaf_pts.as<float4>(), nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, ctx->sm_count, ctx->stream));
   ctx->launches += 5;
   // (Skipping this refinement for small clouds -- its d radix sorts are pure launch latency at 15k points -- was measured and rejected:
-  // the k = 20 searches of the covariance estimation in the unrefined tree cost more than the sorts save, r02j: 6.8 vs 4.1 ms per frame.)
+  // the k = 20 searches of the covariance estimation in the unrefined tree cost more than the sorts save.)
   if (ctx->tree_quality >= 1) {
     // median-split refinement: level by level, sort every node's points along the widest axis of its box; the balanced
     // position boundaries of the next level are then exactly the median splits of a kd-tree (same quality as the host

@@ -50,7 +50,7 @@ struct DevBuf {
 
 struct sgb_ctx {
   int device = 0;
-  int sm_count = 148;
+  int sm_count = 132;
   cudaStream_t own_stream = nullptr;
   cudaStream_t stream = nullptr;
   // second stream + events of the pipelined source upload (sgb_source_set_points): the covariance chunks travel on it while the
@@ -62,7 +62,7 @@ struct sgb_ctx {
   std::string err;
   uint64_t launches = 0;
   // The product library has ONE search path (grid front end + packet / pending search, then the factor kernel).  The fields below that
-  // select anything else are only ever changed by the profiling build (-DSGB_PROFILING, libsgicp_b200_prof.so: A/B runs in profiles/).
+  // select anything else are only ever changed by the profiling build (-DSGB_PROFILING, libsgicp_b200_prof.so: A/B runs).
   int search_mode = 2;  // 2: packet (warp-cooperative) search + factor kernel; [profiling build] 1: per-thread search + factor kernel; 0: single fused kernel
 
   // ---- target ----
@@ -85,7 +85,7 @@ struct sgb_ctx {
   sgb::DevBuf grid_pending_q;  // parallel to the list: transformed query + squared distance of the probe's best candidate
   bool use_ring = true, debug_pending = false;  // profiling switches (sgb_create)
   int pending_div = 16;           // more than n_src / pending_div pending queries: packet search, else a warp per pending query
-  double grid_cell_factor = 2.5;  // cell edge in units of the median point spacing (sweep in profiles/r01: 2 / 2.5 / 3 / 4)
+  double grid_cell_factor = 2.5;  // cell edge in units of the median point spacing (2 / 2.5 / 3 / 4 were compared)
   uint32_t grid_capacity = 0;
   bool pending_clean = false;  // both pending counters are zero / maintained by the probe kernels
   int pending_parity = 0;

@@ -1,5 +1,5 @@
 // SPDX-License-Identifier: MIT
-// Device-side data layout and per-point math of the B200 hot path.  See DESIGN.md §3-4.
+// Device-side data layout and per-point math of the H100 hot path.  See DESIGN.md §3-4.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -218,8 +218,7 @@ __host__ __device__ inline size_t reduction_tickets(size_t grid) { return 1 + (g
 /// Block-wide sum of per-thread accumulators -> partials[blockIdx.x].  The sums of all CTAs are then combined by a
 /// two-level tree of tickets: the last CTA of every group of kFinishGroup consecutive CTAs adds that group's partials,
 /// the last group to finish adds the group sums and writes the (expanded 44-double) result.  Each level is one batch of
-/// independent L2 loads per lane -- a single CTA adding all gridDim.x partials cost ~15-25 us of an otherwise idle GPU
-/// (profiles/r01/p, r01/t).  The order of the additions depends on gridDim.x only: deterministic.
+/// independent L2 loads per lane -- a single CTA adding all gridDim.x partials keeps an otherwise idle GPU waiting.  The order of the additions depends on gridDim.x only: deterministic.
 /// partials: reduction_partials_doubles(gridDim.x) doubles; ticket: reduction_tickets(gridDim.x) zeroed counters (left zeroed).
 /// comm.world > 1: the finishing CTA then exchanges the sums with the other ranks (comm_all_reduce) before writing `out`.
 template <int NACC, bool EXPAND>
@@ -231,7 +230,7 @@ __device__ __forceinline__ void block_reduce_and_finish(double* acc, double* par
   if (NACC > 4) {
     // Transposing butterfly: at every step a lane keeps one half of the values it still owns and hands the other half to its partner,
     // so the 32 lanes end up with ONE fully reduced accumulator each (lane l holds sum l): 16 + 8 + 4 + 2 + 1 = 31 exchanges instead of
-    // 5 per accumulator (145 for the 29 sums of linearize -- 9 % of the factor kernel's instructions, profiles/r01/an).  The order of
+    // 5 per accumulator (145 for the 29 sums of linearize).  The order of
     // the additions is fixed by the lane numbers: deterministic.
     double v[32];
 #pragma unroll

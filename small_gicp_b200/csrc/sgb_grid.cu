@@ -7,15 +7,14 @@
 // it is the exact nearest neighbour and the query is finished -- no tree walk, no dependent pointer chasing.
 // BLOCK LISTS: every target point is stored under the eight blocks that contain its cell, so a block is ONE hash lookup and ONE
 // contiguous run of points (grid_probe_blocks_kernel); 8x the point storage buys the removal of seven lookups and of divergent per-cell
-// scans (round 1 A/B, profiles/r01).  The runs are stored as 32-byte PAIR RECORDS (sgb_grid.cuh: GridPair): one 256-bit load and packed
-// FP32 arithmetic per two points (profiles/r02/b_experiments.md).
+// scans.  The runs are stored as 32-byte PAIR RECORDS (sgb_grid.cuh: GridPair): two points per sector.
 // Queries the probe cannot settle (nothing within c/2: misaligned first iterations, holes, outliers) are appended to a
 // compact pending list -- with the best candidate found so far as an upper bound -- and finished exactly by packet_search_kernel:
 //   * few of them: a warp per query (pending_search_body, sgb_grid.cuh): ring search over the 27 blocks at stride 2 around the query
 //     (everything within 2.5 c), then, only if that radius does not decide it, a walk of the packet tree;
 //   * many of them: the packet walk (sgb_kernels_packet.cu) over the chunk-ordered queries, settled lanes idle.
 // Which of the two runs is decided on the device from the pending counter.  Results are identical to a pure tree search
-// (exact ties aside; tests/test_gpu_parity.py::test_search_structures_agree); evidence and A/B runs: profiles/r01, profiles/r02.
+// (exact ties aside; tests/test_gpu_parity.py::test_search_structures_agree).
 #include <cfloat>
 #include <cstdlib>
 #include <cub/device/device_radix_sort.cuh>
@@ -29,7 +28,7 @@ namespace sgb {
 // Morton (Z-order) code of the three 21-bit offset coordinates: the ORDER in which the lists are laid out in memory.  The table is keyed
 // by the plain packed coordinates (grid_key); only the sort uses the curve, so that the lists a warp of Hilbert-ordered queries needs --
 // a compact patch of ~11 neighbouring blocks -- are neighbours in memory too (DRAM pages, L2 sectors, TLB) instead of being strung along
-// x only (profiles/r02: probe and the 10M - 100M sizes).
+// x only (it matters most for the probe at 10M points and more).
 __device__ __forceinline__ uint64_t grid_spread21(uint64_t x) {
   x &= 0x1fffffull;
   x = (x | x << 32) & 0x1f00000000ffffull;
@@ -143,8 +142,8 @@ __global__ void grid_table_init_kernel(GridSlot* table, uint32_t capacity) {
 // ---------------------------------------------------------------------------------------------------------------
 // probe, block lists: the block anchored at floor(u - 1/2) covers [q - c/2, q + c/2]^3; one lookup, one contiguous scan
 // ---------------------------------------------------------------------------------------------------------------
-// UNROLL pairs of the scan loop are in flight per thread (2: 32 registers = 8 CTAs of 256 threads = full occupancy, measured best: r02aa / r02ab);
-// PREFETCH: the whole list is requested into L2 as soon as its table slot is known (-6 us).  MIN_CTAS / UNROLL / PREFETCH other than the defaults
+// UNROLL pairs of the scan loop are in flight per thread (2: 32 registers = 8 CTAs of 256 threads = full occupancy);
+// PREFETCH: the whole list is requested into L2 as soon as its table slot is known.  MIN_CTAS / UNROLL / PREFETCH other than the defaults
 // exist in the profiling library only (SGB_PROBE_CTAS, SGB_PROBE_UNROLL, SGB_PROBE_PREFETCH).
 template <int MIN_CTAS, int UNROLL = 2, bool PREFETCH = true>
 __global__ void __launch_bounds__(256, MIN_CTAS) grid_probe_blocks_kernel(const __grid_constant__ LinParams P, const GridPair* __restrict__ grid_pairs,
@@ -175,10 +174,9 @@ __global__ void __launch_bounds__(256, MIN_CTAS) grid_probe_blocks_kernel(const 
             bz = static_cast<int>(fminf(fmaxf(az, -1e5f), 1e5f));
   const uint2 e = grid_lookup(table, mask, bx, by, bz);
   {
-    // The list is a contiguous run of ceil(e.y / 2) PAIR RECORDS (32 B: two points, components interleaved).  One 256-bit load
-    // (ld.global.nc.v8.f32 -> LDG.E.256, new with sm_100) brings a pair, and the squared distances of both points come out of packed FP32
-    // arithmetic (add / mul / fma .f32x2 -> FADD2 / FMUL2 / FFMA2, also new with sm_100): half the load instructions -- the scan is bound by
-    // L1 wavefronts, ~11 distinct lists per warp and instruction (profiles/r02/f: l1tex 65 % busy) -- and half the arithmetic per point.
+    // The list is a contiguous run of ceil(e.y / 2) PAIR RECORDS (32 B: two points, components interleaved), read by two 128-bit
+    // loads of one sector (load_pair).  The squared distance is fma(dz, dz, fma(dy, dy, dx * dx)) in FP32 with round-to-nearest for
+    // each point, so the candidate and its distance are bit-identical to a packed f32x2 evaluation of the same expression.
     const GridPair* __restrict__ rec = grid_pairs + e.x;
     const uint32_t npairs = (e.y + 1u) >> 1;
     // pull all of its lines into L2 at once (the scan would otherwise pay one DRAM round trip per batch of loads)
@@ -187,18 +185,19 @@ __global__ void __launch_bounds__(256, MIN_CTAS) grid_probe_blocks_kernel(const 
     if (PREFETCH)
       for (uint32_t off = 128u; off < bytes; off += 128u) asm volatile("prefetch.global.L2 [%0];" ::"l"(lp + off));
     if (PREFETCH && bytes > 128u) asm volatile("prefetch.global.L2 [%0];" ::"l"(lp + bytes - 32u));  // last line of a run that is not 128 B aligned
-    const float2 nfx = make_float2(-fx, -fx), nfy = make_float2(-fy, -fy), nfz = make_float2(-fz, -fz);
 #pragma unroll UNROLL
     for (uint32_t j = 0; j < npairs; j++) {
       const GridPair t = load_pair(rec + j);
-      const float2 dx = __fadd2_rn(make_float2(t.a.x, t.a.y), nfx), dy = __fadd2_rn(make_float2(t.a.z, t.a.w), nfy), dz = __fadd2_rn(make_float2(t.b.x, t.b.y), nfz);
-      const float2 d = __ffma2_rn(dz, dz, __ffma2_rn(dy, dy, __fmul2_rn(dx, dx)));
-      if (d.x < best_d) {  // first point of the pair first: ties keep the scan order
-        best_d = d.x;
+      const float dx0 = __fsub_rn(t.a.x, fx), dy0 = __fsub_rn(t.a.z, fy), dz0 = __fsub_rn(t.b.x, fz);
+      const float dx1 = __fsub_rn(t.a.y, fx), dy1 = __fsub_rn(t.a.w, fy), dz1 = __fsub_rn(t.b.y, fz);
+      const float d0 = __fmaf_rn(dz0, dz0, __fmaf_rn(dy0, dy0, __fmul_rn(dx0, dx0)));
+      const float d1 = __fmaf_rn(dz1, dz1, __fmaf_rn(dy1, dy1, __fmul_rn(dx1, dx1)));
+      if (d0 < best_d) {  // first point of the pair first: ties keep the scan order
+        best_d = d0;
         best = __float_as_uint(t.b.z);
       }
-      if (d.y < best_d) {  // (the pad of an odd list sits at 1e18: ~3e36, never nearest)
-        best_d = d.y;
+      if (d1 < best_d) {  // (the pad of an odd list sits at 1e18: ~3e36, never nearest)
+        best_d = d1;
         best = __float_as_uint(t.b.w);
       }
     }
@@ -223,9 +222,9 @@ __global__ void __launch_bounds__(256, MIN_CTAS) grid_probe_blocks_kernel(const 
   // Pending queries go to a compact list, and -- for the packet search -- the CHUNK (one warp here = one 32-query chunk there) goes into
   // the work list of its cost class = how far its widest search ball reaches (best_d is the squared radius a pending lane starts its
   // walk with).  The packet search takes the wide classes first, so that what is left when the GPU drains are the cheap walks
-  // (profiles/r01/ai: a third of that kernel was a tail of late-starting heavy chunks); chunks without a pending lane are in no list.
+  // (otherwise a long tail of late-starting heavy chunks); chunks without a pending lane are in no list.
   // Both appends are aggregated over the CTA's eight warps: at most four atomics per CTA -- one per warp and list made the hot
-  // counters the probe's own tail (r02d: +9 us at the identity pose).
+  // counters the probe's own tail at the identity pose.
   const bool pend = in_range && !settled;
   const unsigned m = __ballot_sync(0xffffffffu, pend);
   const uint32_t lane = threadIdx.x & 31u, wib = threadIdx.x >> 5;

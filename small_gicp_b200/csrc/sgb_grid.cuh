@@ -13,19 +13,19 @@ namespace sgb {
 // in cell units carries < 1e-3 of rounding error
 constexpr float kGridSlack = 4e-3f;
 
-// One entry of a block list: TWO points, components interleaved so that a 256-bit load brings both and packed FP32 arithmetic (f32x2)
-// computes both squared distances: a = (x0, x1, y0, y1), b = (z0, z1, leaf position 0, leaf position 1).  A list with an odd number of
-// points ends in a pad: coordinates kGridPadCoord (squared distance ~3e36: farther than anything real, still finite), position kNone.
+// One entry of a block list: TWO points in one 32-byte sector, components interleaved: a = (x0, x1, y0, y1), b = (z0, z1, leaf
+// position 0, leaf position 1).  A list with an odd number of points ends in a pad: coordinates kGridPadCoord (squared distance ~3e36:
+// farther than anything real, still finite), position kNone.
 struct __align__(32) GridPair {
   float4 a, b;
 };
 constexpr float kGridPadCoord = 1e18f;
 
+// sm_90 has no 256-bit load: the record is two 128-bit read-only loads (LDG.E.128.CONSTANT) of the same sector
 __device__ __forceinline__ GridPair load_pair(const GridPair* p) {
   GridPair r;
-  asm("ld.global.nc.v8.f32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-      : "=f"(r.a.x), "=f"(r.a.y), "=f"(r.a.z), "=f"(r.a.w), "=f"(r.b.x), "=f"(r.b.y), "=f"(r.b.z), "=f"(r.b.w)
-      : "l"(p));
+  r.a = __ldg(&p->a);
+  r.b = __ldg(&p->b);
   return r;
 }
 
@@ -62,7 +62,7 @@ __device__ __forceinline__ uint2 grid_lookup(const GridSlot* __restrict__ table,
 // Ring phase first (block lists): 27 lookups in parallel, the lists scanned as one flattened run over all lanes, a
 // hardware min -- a handful of memory round trips.  Only if the ring's radius (2.5 cells) does not decide the query does
 // the warp walk the packet records: every step of a single walk is a dependent load, so a thread per query would be
-// pure latency (measured: 300 us for 1000 queries); with a warp per query a leaf's points are fetched by one coalesced
+// pure latency; with a warp per query a leaf's points are fetched by one coalesced
 // load and reduced by a hardware min, and thousands of walks are in flight at once.  Runs (inside packet_search_kernel) when at most N / pending_div queries
 // are pending; with more, the packet search over the chunk-ordered queries takes them.
 // ---------------------------------------------------------------------------------------------------------------
@@ -198,12 +198,16 @@ __device__ __forceinline__ void pending_search_body(const LinParams& P, const fl
         }
         leaf = cn;
       } else {
+        // Every popped descriptor is read (volatile) before the test.  When the read sits behind the test, ptxas of CUDA 12.9 for sm_90a
+        // sinks it out of the loop and addresses desc[sp - 1] -- the entry below, at sp == 0 the bytes before this warp's stack.
         bool got = false;
         __syncwarp();
         while (sp > 0) {
           sp--;
+          const volatile uint2* e = desc + sp;
+          const uint2 c = make_uint2(e->x, e->y);
           if (dist[sp] < best_d) {
-            leaf = desc[sp];
+            leaf = c;
             got = true;
             break;
           }

@@ -179,7 +179,7 @@ bool build_flat_tree(const float* pts_xyzw, size_t n_points, int max_leaf_size, 
     err = "too many points for 32-bit device indices";
     return false;
   }
-  if (max_leaf_size <= 0) max_leaf_size = 32;  // one point per lane in the packet search's leaf scan (profiles/r01: best of 8..64)
+  if (max_leaf_size <= 0) max_leaf_size = 32;  // one point per lane in the packet search's leaf scan (leaf sizes 8..64 were compared)
   if (max_leaf_size > 64) max_leaf_size = 64;
   out.perm.resize(n_points);
   std::iota(out.perm.begin(), out.perm.end(), 0u);

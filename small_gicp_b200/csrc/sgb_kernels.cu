@@ -1,5 +1,5 @@
 // SPDX-License-Identifier: MIT
-// Hot-path kernels (sm_100a): fused transform -> kd-tree NN -> reject -> factor -> reduction, the
+// Hot-path kernels (sm_90a): fused transform -> kd-tree NN -> reject -> factor -> reduction, the
 // error() kernel for the LM inner loop, and the one-off layout kernels (upload conversion, Morton
 // ordering of the source, leaf ordering of the target).  See DESIGN.md §4 for the roofline of each.
 #include "sgb_device.cuh"
@@ -569,7 +569,7 @@ __global__ void kd_keys_kernel(const float4* __restrict__ pts, uint32_t n, uint3
 // (a contiguous position range), keeps its points in shared memory and runs every remaining level there -- per level: node boxes
 // (shared-memory atomics on order-preserving integer images of the floats), key = (node, coordinate along the node's widest axis),
 // bitonic sort of (key, slot), permutation of the points.  Above level0 a level is ~12 launches (boxes, keys, radix sort, gather); for a
-// 16k-point frame that was 9 levels = ~110 launches = 0.9 ms of launch latency, now 3 levels + this kernel.  Same keys, same balanced
+// 16k-point frame that was 9 levels = ~110 launches of pure launch latency, now 3 levels + this kernel.  Same keys, same balanced
 // position boundaries as the per-level path (ties may land differently -- any order is a valid tree).
 constexpr uint32_t kKdSegMax = 2048;
 constexpr uint32_t kKdSegNodes = 128;

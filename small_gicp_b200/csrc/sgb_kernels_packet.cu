@@ -2,7 +2,7 @@
 // Warp-cooperative ("packet") exact nearest-neighbour search -- the search phase of linearize.
 //
 // A warp owns 32 CONSECUTIVE source points of the Morton order, i.e. 32 queries that sit within a small patch of the
-// surface.  Instead of 32 divergent per-thread walks (profiles/r01: 10-14 of 32 lanes active, every lane issuing its own
+// surface.  Instead of 32 divergent per-thread walks (a third of the lanes active, every lane issuing its own
 // node and point loads), the warp walks the tree ONCE with a single shared traversal stack:
 //   * every control-flow decision is a warp vote, so the instruction stream never diverges;
 //   * node and leaf-point addresses are warp-uniform: one 64 B node / one 16 B point is fetched per warp and broadcast;
@@ -27,7 +27,7 @@ constexpr int kPktWarps = kLinBlock / 32;
 // served one by one by the whole warp (~16 instr / lane): break-even ~ points_per_leaf * 10 / 16
 constexpr int kPacketDenseLanes = 18;
 // resident CTAs per SM the kernel is compiled for: the compiler's own 48 registers -> 10 CTAs x 4 warps.  Forcing 12 (40 registers, 8 B
-// of spills) measured slower (r02j: 0.2444 vs 0.2393 ms at the identity pose, 0.184 vs 0.180 ms at T1).
+// of spills) is the profiling library's A/B (SGB_PACKET_CTAS=12).
 constexpr int kPacketCtas = 10;
 
 __device__ __forceinline__ float box_dist2(float qx, float qy, float qz, const float4& lo, const float4& hi) {
@@ -40,8 +40,8 @@ __device__ __forceinline__ float box_dist2(float qx, float qy, float qz, const f
 // ---- TMA staging of a leaf's point block (BASELINE north_star: "TMA bulk loads for the leaf point blocks") ----------------------
 // One elected lane arms the warp's mbarrier with the byte count and issues ONE cp.async.bulk (SASS UBLKCP) for the leaf's contiguous
 // <= 32 x 16 B; the warp waits on the barrier's phase and then reads the points from shared memory.  TMA_LEAF is a compile-time A/B:
-// measured in profiles/r02 (the broadcast __ldg path below serves an L1-resident leaf in ~32 cycles per load, pipelined; the bulk copy
-// always makes the round trip through L2) -- see DESIGN.md §4 for the numbers and which variant ships.
+// kept in the profiling library (the broadcast __ldg path below serves an L1-resident leaf in ~32 cycles per load, pipelined; the bulk copy
+// always makes the round trip through L2) -- DESIGN.md §4 says which variant ships.
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(static_cast<uint32_t>(__cvta_generic_to_shared(bar))), "r"(count));
 }
@@ -72,7 +72,7 @@ __global__ void __launch_bounds__(kLinBlock, MIN_CTAS) packet_search_kernel(cons
                                                                   uint32_t min_pending, uint32_t* queue, uint32_t* queue_next, ChunkClasses cc, RingParams ring) {
   // Work distribution: chunks (32 consecutive queries) differ wildly in cost -- all lanes settled by the grid probe, or 32
   // tree walks through a misaligned wall -- and a static stride left a third of the warps idle for the second half of the
-  // kernel (profiles/r01/ai: 39-52 % achieved occupancy of 75 %).  With `queue` the warps take their first chunk by rank and
+  // kernel (achieved occupancy far below the theoretical).  With `queue` the warps take their first chunk by rank and
   // every further one from a global counter.  Two counters alternate between launches: this launch clears the next one's
   // (launches of one context are stream-ordered, the next user is the packet search of the NEXT linearize).
   if (queue_next && blockIdx.x == 0 && threadIdx.x == 0) *queue_next = 0u;
@@ -83,7 +83,7 @@ __global__ void __launch_bounds__(kLinBlock, MIN_CTAS) packet_search_kernel(cons
   __shared__ __align__(8) uint64_t s_bar[TMA_LEAF ? kPktWarps : 1];
   // Two regimes, picked from the probe's counter: FEW pending queries (holes, borders, outliers at an aligned pose) -> a warp per query
   // (ring phase over the block lists, tree walk only beyond its reach: sgb_grid.cuh); MANY (a misaligned first iteration) -> the packet
-  // walk below.  One launch serves both (round 1: two kernels, one of which exited at once -- 3.5 - 5 us per linearize).
+  // walk below.  One launch serves both (two kernels, one of which exits at once, cost a launch per linearize).
   if (pending_count) {
     const uint32_t pc = *pending_count;
     if (pc <= min_pending) {
@@ -116,7 +116,7 @@ __global__ void __launch_bounds__(kLinBlock, MIN_CTAS) packet_search_kernel(cons
     c1 = c0 + cc.count[1];
     // The lists are in the order the probe's warps happened to finish: neighbouring items are NOT neighbouring chunks, so the warps of
     // an SM no longer share tree nodes through L1.  When nearly every chunk has pending lanes anyway (a grossly misaligned first
-    // iteration: nothing to skip, no cheap tail to save for the end) the curve order wins (r02d: 0.2335 vs 0.2441 ms at T0, 0.1936 vs 0.1795 ms at T1).
+    // iteration: nothing to skip, no cheap tail to save for the end) the curve order wins (threshold: class_fallback_pct).
     const uint32_t listed = c1 + cc.count[2];
     if (listed * 100u > n_items * cc.fallback_pct) cc.lists = nullptr;
     else n_items = listed;

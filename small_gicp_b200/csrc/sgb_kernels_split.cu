@@ -1,5 +1,5 @@
 // SPDX-License-Identifier: MIT
-// The factor / reduction phase of linearize, and the per-thread search kept as a profiling switch (DESIGN.md §4, profiles/r01):
+// The factor / reduction phase of linearize, and the per-thread search kept as a profiling switch (DESIGN.md §4):
 //   nn_search_kernel      (SGB_SEARCH=1) transform + exact kd-tree NN, one query per thread -- the product path searches
 //                         with sgb_grid.cu + sgb_kernels_packet.cu instead
 //   factor_reduce_kernel  streams source + correspondences, gathers the matched target point / covariance with cp.async two
@@ -134,7 +134,7 @@ __global__ void __launch_bounds__(kLinBlock) nn_search_kernel(const __grid_const
 // ---------------------------------------------------------------------------------------------------------------
 // Phase 2.  One point per thread per tile of kLinBlock points.  The gather of the matched target point / covariance
 // depends on the correspondence index, and the FP64 factor algebra holds ~128 registers (4 CTAs / SM), so plain loads
-// left the kernel latency-bound (profiles/r01/k: 24 % issue slots, 1.4 TB/s).  The loads are therefore issued two
+// left the kernel latency-bound (few issue slots used, far from the HBM bandwidth).  The loads are therefore issued two
 // tiles ahead with cp.async into a per-thread landing zone in shared memory:
 //   A(t+2): correspondence index + source point / covariance (coalesced)
 //   B(t+1): target point / normal / covariance gathered through the index A(t+1) brought in
@@ -159,10 +159,10 @@ struct FactorFields {
 constexpr int kFactorStages = 3;
 
 // NREG: register budget per thread = resident CTAs per SM (128 -> 4 CTAs x 4 warps, no spills; 96 -> 5 CTAs; 80 -> 6, both with spills and slower): the algebra is a chain of
-// dependent FP64 operations and the kernel is short of warps, not of FP64 pipe (41 % active) -- A/B in profiles/r02/b_experiments.md.
+// dependent FP64 operations and the kernel is short of warps, not of FP64 pipe.
 // ERR: the same operand pipeline evaluating Reduction::error instead (cached correspondences, trial pose P.T, GICP precision matrix re-derived
 // from the linearisation pose P.Tlin, one sum): the LM inner loop's kernel.  The plain grid-stride version of it (error_kernel, sgb_kernels.cu)
-// waited on two dependent load round trips per point with nothing in flight: 48 us per 1M points against 38 us for the whole linearize algebra.
+// waited on two dependent load round trips per point with nothing in flight: longer than the whole linearize algebra.
 template <int FACTOR, int ROBUST, int NREG, bool ERR = false>
 __global__ void __maxnreg__(NREG) factor_reduce_kernel(const __grid_constant__ LinParams P) {
   using F = FactorFields<FACTOR>;
@@ -278,7 +278,7 @@ static int error_ctas_per_sm() {
 }
 
 // resident CTAs per SM of one instantiation (the grid is sized to exactly one wave: a partial second wave of this
-// register-heavy kernel ran one CTA per SM for a third of the kernel's duration, profiles/r01/r)
+// register-heavy kernel runs one CTA per SM for a good part of the kernel's duration)
 template <int FACTOR, int ROBUST>
 static int factor_ctas_per_sm() {
   static int cached = 0;

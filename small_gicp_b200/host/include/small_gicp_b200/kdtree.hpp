@@ -6,7 +6,7 @@
 // The node array keeps the reference's 24-byte layout because it IS the data contract of
 // sgb_target_set_kdtree(); the construction below is iterative (explicit work list, nodes emitted in
 // pre-order) instead of the reference's recursion, and the search uses an explicit stack.
-// `DeviceKdTree` is the B200-native alternative: no host nodes at all, the context builds the tree.
+// `DeviceKdTree` is the H100-native alternative: no host nodes at all, the context builds the tree.
 #pragma once
 #include <algorithm>
 #include <limits>
@@ -222,7 +222,7 @@ struct KdTree {
   const UnsafeKdTree<PointCloud, Projection> kdtree;
 };
 
-/// B200-native tree handle: nothing is built on the host; ParallelReductionCUDA asks the context to build
+/// H100-native tree handle: nothing is built on the host; ParallelReductionCUDA asks the context to build
 /// its own flattened tree over the target (sgb_target_build_kdtree).
 template <typename PointCloud>
 struct DeviceKdTree {

@@ -1,5 +1,5 @@
 // SPDX-License-Identifier: MIT
-// ParallelReductionCUDA -- the B200 backend as a peer of SerialReduction / ParallelReductionOMP /
+// ParallelReductionCUDA -- the H100 backend as a peer of SerialReduction / ParallelReductionOMP /
 // ParallelReductionTBB (/root/reference/include/small_gicp/registration/reduction.hpp:12-63,
 // reduction_omp.hpp:20-73, reduction_tbb.hpp:114-139): same two const member templates, plain public fields
 // for tunables, default-constructible and copyable (copies share one device context).

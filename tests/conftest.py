@@ -11,12 +11,12 @@ GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a B200 (run with -m gpu under gpurun)")
+    config.addinivalue_line("markers", "gpu: needs an H100 (run with -m gpu)")
 
 
 def pytest_sessionstart(session):
     """A fresh checkout has no built artefacts (they are git-ignored): build them once (nvcc cross-compiles without a GPU).  Only when
-    something is MISSING -- on the GPU box the libraries arrive pre-built with the snapshot and must not be rebuilt because of clock skew."""
+    something is MISSING -- libraries built elsewhere and copied in with the tree must not be rebuilt because of clock skew."""
     needed = [
         os.path.join(ROOT, "small_gicp_b200", "lib", "libsgicp_b200.so"),
         os.path.join(ROOT, "small_gicp_b200", "lib", "libsgicp_b200_prof.so"),

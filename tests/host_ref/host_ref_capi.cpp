@@ -2,7 +2,7 @@
 // tests/host_ref: the REFERENCE's own Registration<> template (headers included in place from /root/reference/include, nothing
 // copied) instantiated with include/small_gicp/registration/reduction_cuda.hpp -- the binding INTEGRATION.md shows -- next to
 // the same template on the reference's ParallelReductionOMP, behind one C entry point for the Python tests.
-// TEST INFRASTRUCTURE: built only where /root/reference exists (this container), shipped as a .so to the GPU box.
+// TEST INFRASTRUCTURE: built only where the reference's sources are at hand (tests/host_ref/Makefile), into oracle/_ref/.
 // Eigen is absent from the image: both arms compile against the API shim of oracle/ref_build/eigen_shim (DESIGN.md §2).
 #include <cstring>
 #include <memory>

@@ -16,13 +16,13 @@ import pytest
 import oracle as O
 from conftest import ROOT, noise_poses, pose_error
 
-LIB = os.path.join(ROOT, "tests", "host_ref", "libsgb_host_ref.so")
+LIB = os.path.join(ROOT, "oracle", "_ref", "libsgb_host_ref.so")
 _dp = C.POINTER(C.c_double)
 
 
 def _lib():
     if not os.path.exists(LIB):
-        pytest.skip("tests/host_ref/libsgb_host_ref.so not built (needs /root/reference: `make -C tests/host_ref`)")
+        pytest.skip("oracle/_ref/libsgb_host_ref.so not built (needs the reference's sources: `make -C tests/host_ref REF=<reference checkout>`)")
     L = C.CDLL(LIB)
     L.href_align.restype = C.c_int
     L.href_align.argtypes = [_dp, C.c_size_t, _dp, _dp, _dp, C.c_size_t, _dp, _dp, _dp, _dp]

@@ -1,7 +1,7 @@
 """Pins the oracle's restatement (oracle/sgicp_oracle.cpp) against the REFERENCE'S OWN CODE: oracle/_ref/libsmallgicp_ref.so is
-/root/reference/include compiled in place against the Eigen API shim (oracle/ref_build) behind the same C API.
+the reference's include/ directory compiled in place against the Eigen API shim (oracle/ref_build) behind the same C API.
 Same inputs -> same outputs: bit-exact for integer / index / structure work, <= 1e-12 relative for floating point (the two differ only
-in summation order inside small fixed-size products).  Skipped where the library has not been built (it needs /root/reference)."""
+in summation order inside small fixed-size products).  Skipped where the library has not been built (it needs the reference's sources)."""
 import numpy as np
 import pytest
 
@@ -9,7 +9,7 @@ import oracle as O
 from conftest import noise_poses
 
 REF = O.reference_lib()
-pytestmark = pytest.mark.skipif(REF is None, reason="oracle/_ref not built (needs /root/reference)")
+pytestmark = pytest.mark.skipif(REF is None, reason="oracle/_ref not built (needs the reference's sources, oracle/ref_build/Makefile)")
 
 
 def both_clouds(xyz, leaf):
