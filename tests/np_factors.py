@@ -8,6 +8,71 @@ import numpy as np
 
 NO = np.uint64(0xFFFFFFFFFFFFFFFF)
 
+# GPU sums against this module evaluated on storage_model() inputs: FP64 algebra on identical operands, only the summation order and
+# fma contraction differ.  One point's share of the sums at 1M points is ~1e-6, so a point given wrong operands misses this by far.
+TIGHT = 1e-10
+
+
+def _f32(a):
+    return np.asarray(a, dtype=np.float64).astype(np.float32).astype(np.float64)
+
+
+def box_centre(pts):
+    """the centre every upload (source, target, voxel means) is stored relative to: 0.5 (min + max) per axis in FP64, 0 if empty"""
+    if len(pts) == 0:
+        return np.zeros(3)
+    return 0.5 * (pts[:, :3].min(0) + pts[:, :3].max(0))
+
+
+def stored_points(pts, centre=None):
+    """convert_kernel: float32(p - c) with round-to-nearest, read back as that + c in FP64; c = box_centre of the whole upload"""
+    c = box_centre(pts) if centre is None else centre
+    out = np.array(pts, dtype=np.float64)
+    out[:, :3] = _f32(out[:, :3] - c) + c
+    return out
+
+
+def stored_normals(normals):
+    out = np.zeros((len(normals), 4))
+    out[:, :3] = _f32(np.asarray(normals)[:, :3])
+    return out
+
+
+def stored_covs(covs):
+    """pack_covA / pack_covB: the upper triangle (0,0) (0,1) (0,2) (1,1) (1,2) (2,2) rounded to FP32 and mirrored; the lower triangle
+    and the fourth row / column are never read"""
+    covs = np.asarray(covs)
+    out = np.zeros((len(covs), 4, 4))
+    for a, b in ((0, 0), (0, 1), (0, 2), (1, 1), (1, 2), (2, 2)):
+        out[:, a, b] = out[:, b, a] = _f32(covs[:, a, b])
+    return out
+
+
+def storage_model(src_pts, src_covs, tgt_pts, tgt_normals, tgt_covs, src_centre=None, tgt_centre=None):
+    """what the device holds for one (source, target) upload, as FP64 arrays for linearize() / error(); absent features stay None.
+    The centres default to the boxes of the arrays given (pass them when the arrays are a subset of what was uploaded)."""
+    return (stored_points(src_pts, src_centre), None if src_covs is None else stored_covs(src_covs), stored_points(tgt_pts, tgt_centre),
+            None if tgt_normals is None else stored_normals(tgt_normals), None if tgt_covs is None else stored_covs(tgt_covs))
+
+
+def orthonormal(T):
+    """T_target_source.txt carries 6 digits: R^T R differs from I by 1e-6.  The source-frame formulation uses R^T R = I (an
+    Isometry3d is a rotation; every pose the optimizers produce is one to 1e-16), so the exact-algebra check needs a true rotation."""
+    U, _, Vt = np.linalg.svd(T[:3, :3])
+    out = T.copy()
+    out[:3, :3] = U @ Vt
+    return out
+
+
+def tight_ratios(got, ref):
+    """(H, b, e) against a reference: relative Frobenius norm of H, relative e, and b per component relative to sqrt(2 e H_kk)
+    (Cauchy-Schwarz scale of b_k); each is held to TIGHT"""
+    (H, b, e), (H0, b0, e0) = got, ref
+    rh = np.linalg.norm(H - H0) / np.linalg.norm(H0)
+    re = abs(e - e0) / e0
+    rb = float((np.abs(b - b0) / np.sqrt(2.0 * e0 * np.diag(H0))).max())
+    return float(rh), float(rb), float(re)
+
 
 def _skew_batch(p):
     S = np.zeros((len(p), 3, 3))

@@ -74,24 +74,10 @@ class Pairs:
 
 
 def storage_model(P):
-    """what the device actually holds: centred coordinates and covariance entries rounded to FP32"""
-    f32 = lambda a: a.astype(np.float32).astype(np.float64)
-    sp, tp = P.sp.copy(), P.tp.copy()
-    sp[:, :3] = f32(P.sp[:, :3] - P.cs) + P.cs
-    tp[:, :3] = f32(P.tp[:, :3] - P.ct) + P.ct
-    return sp, f32(P.sc), tp, f32(P.tn), f32(P.tcv)
+    return NF.storage_model(P.sp, P.sc, P.tp, P.tn, P.tcv, P.cs, P.ct)
 
 
 CASES = [(f, r) for f in (0, 1, 2) for r in (0, 1, 2)]
-
-
-def orthonormal(T):
-    """T_target_source.txt carries 6 digits: R^T R differs from I by 1e-6.  The source-frame formulation uses R^T R = I (an
-    Isometry3d is a rotation; every pose the optimizers produce is one to 1e-16), so the exact-algebra check needs a true rotation."""
-    U, _, Vt = np.linalg.svd(T[:3, :3])
-    out = T.copy()
-    out[:3, :3] = U @ Vt
-    return out
 
 
 @pytest.mark.parametrize("factor,robust", CASES)
@@ -99,7 +85,7 @@ def test_kernel_arithmetic_matches_oracle_and_numpy(hm, golden_prepared, factor,
     g = golden_prepared
     tc, sc = g["target"], g["source"]
     reg = O.Registration(factor=factor, robust=robust, robust_c=0.7, num_threads=0)
-    for T in (np.eye(4), orthonormal(g["T"]), noise_poses()[2]):
+    for T in (np.eye(4), NF.orthonormal(g["T"]), noise_poses()[2]):
         H0, b0, e0 = reg.linearize(tc, g["target_tree"], sc, T)
         corr = reg.correspondences(len(sc))
         P = Pairs(g, corr)

@@ -5,6 +5,8 @@ by raw device pointers (the multi-process wiring over CUDA IPC differs only in h
 import numpy as np
 import pytest
 
+import np_factors as NF
+
 pytestmark = pytest.mark.gpu
 
 
@@ -80,7 +82,19 @@ def test_sharded_contexts_exchange_inside_the_kernel(world):
             np.testing.assert_array_equal(h, ref)  # summed in rank order on every rank: bit-identical
             assert float(errs[r].cpu()[0]) == float(errs[0].cpu()[0])
         H, b, e, ninl = ref[:36].reshape(6, 6), ref[36:42], ref[42], ref[43]
-        # shards re-centre their own source boxes: FP32 roundings differ slightly from the un-sharded run
+        # every shard re-centres its own source box: the exchanged sum is the sum of the per-shard storage models
+        Hm, bm, em, err_m = np.zeros((6, 6)), np.zeros(6), 0.0, 0.0
+        for r, (lo, hi) in enumerate(shards):
+            model = NF.storage_model(src[lo:hi], scov[lo:hi], tgt, None, tcov)
+            corr = ctxs[r].correspondences()
+            Hr, br, er = NF.linearize(pose, corr, 2, 0, 1.0, *model)
+            Hm, bm, em = Hm + Hr, bm + br, em + er
+            err_m += NF.error(pose, pose, corr, 2, 0, 1.0, *model)
+        ratios = NF.tight_ratios((H, b, e), (Hm, bm, em)) + (abs(float(errs[0].cpu()[0]) - err_m) / err_m,)
+        print(f"worst ratio to the per-shard storage models (world {world}, pose {it}): {max(ratios):.2e}")
+        assert max(ratios) <= NF.TIGHT, ("H, b, e, error:", ratios)
+        assert int(ninl) == sum(int((ctxs[r].correspondences() != NF.NO).sum()) for r in range(world))
+        # ... so FP32 roundings differ slightly from the un-sharded run
         assert np.linalg.norm(H - H0) <= 1e-5 * np.linalg.norm(H0)
         assert abs(e - e0) <= 1e-5 * e0 and abs(float(errs[0].cpu()[0]) - err0) <= 1e-5 * err0
         assert abs(ninl - n0) <= 3

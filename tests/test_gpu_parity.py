@@ -4,15 +4,18 @@ Each check is a triangle  oracle <-> numpy <-> GPU  (tests/np_factors.py):
   1. correspondences: GPU == oracle except FP32 near-ties (squared distances equal to 1e-5 rel + 1e-7) and points
      sitting on the rejection boundary (|d2 - max_dist_sq| < 1e-4);
   2. oracle sums == numpy sums over the ORACLE's correspondences to 1e-9 (pins the numpy leg to the oracle);
-  3. GPU sums == numpy sums over the GPU's OWN correspondences within the tolerances below; when (1) found no
-     difference at all the GPU sums are also compared directly with the oracle's.
+  3. GPU sums == numpy sums over the GPU's OWN correspondences, evaluated on the storage model of what the device holds
+     (np_factors.storage_model: centred FP32 coordinates, FP32 normals and covariance entries) to np_factors.TIGHT = 1e-10;
+     when (1) found no difference at all the GPU sums are also compared directly with the oracle's.
 
-Tolerances (FP32 coordinate/covariance storage, FP32 search, FP64 factor algebra and sums; DESIGN.md §5):
+Tolerances against the oracle (FP32 coordinate/covariance storage, FP32 search, FP64 factor algebra and sums; DESIGN.md §5):
   H      : ||H_gpu - H_ref||_F <= 2e-5 ||H_ref||_F
   e      : |e_gpu - e_ref| <= 2e-5 e_ref
   b      : |b_gpu - b_ref|_k <= 2e-5 sqrt(2 e H_kk)           (Cauchy-Schwarz scale of b_k)
   step   : |H^-1 b|_gpu - |H^-1 b|_ref  <= 2e-6 (rad / m)
   pose   : converged SE(3) within 1e-4 rad / 1e-3 m of the oracle (BASELINE.json north_star)
+The model leg needs exact rotations (the kernels work in the source frame, D = R^T M R): the 6-digit golden pose goes through
+np_factors.orthonormal for the oracle and the GPU alike.
 """
 import numpy as np
 import pytest
@@ -55,12 +58,26 @@ def check_linearized(got, ref, tag="", rtol=RTOL):
     assert np.abs(d - d0).max() <= max(2e-6, 100 * rtol * np.abs(d0).max() * 1e-2), (tag, np.abs(d - d0).max())
 
 
+def check_tight(got, ref, tag=""):
+    """GPU sums against numpy on the storage model (np_factors.TIGHT); returns the worst of the three ratios"""
+    r = NF.tight_ratios(got, ref)
+    assert max(r) <= NF.TIGHT, (tag, "H, b, e:", r)
+    return max(r)
+
+
+def check_tight_error(e_gpu, e_model, tag=""):
+    r = abs(e_gpu - e_model) / e_model
+    assert r <= NF.TIGHT, (tag, e_gpu, e_model, r)
+    return r
+
+
 class Arrays:
-    """numpy views of an oracle (target, source) pair"""
+    """numpy views of an oracle (target, source) pair, and the storage model of the same pair uploaded whole"""
 
     def __init__(self, target, source):
         self.tp, self.tn, self.tc = target.points, target.normals, target.covs
         self.sp, self.sc = source.points, source.covs
+        self.model = NF.storage_model(self.sp, self.sc, self.tp, self.tn, self.tc)
 
 
 def triangle(ctx, reg, target, tree, source, arr, T, factor, robust, c, rejector=1, max_d=1.0, tag=""):
@@ -74,10 +91,10 @@ def triangle(ctx, reg, target, tree, source, arr, T, factor, robust, c, rejector
     assert ctx.num_inliers() == int((c_gpu != sg.NO_CORRESPONDENCE).sum())
     args = (factor, robust, c, arr.sp, arr.sc, arr.tp, arr.tn, arr.tc)
     check_linearized(cpu, NF.linearize(T, c_cpu, *args), (tag, "oracle-vs-numpy"), rtol=1e-9)
-    check_linearized(gpu, NF.linearize(T, c_gpu, *args), (tag, "gpu-vs-numpy"))
+    worst = check_tight(gpu, NF.linearize(T, c_gpu, factor, robust, c, *arr.model), (tag, "gpu-vs-model"))
     if nm == 0:
         check_linearized(gpu, cpu, (tag, "gpu-vs-oracle"))
-    return c_cpu, c_gpu, nm
+    return c_cpu, c_gpu, nm, worst
 
 
 FACTORS = [
@@ -105,18 +122,21 @@ def test_linearize_and_error_golden(golden_prepared, golden_ctx, name, factor, r
     ctx = golden_ctx
     arr = Arrays(g["target"], g["source"])
     reg = O.Registration(factor=factor, robust=robust, robust_c=0.7, num_threads=0)
-    for j, T in enumerate([np.eye(4), g["T"]] + noise_poses()[1:3]):
-        c_cpu, c_gpu, nm = triangle(ctx, reg, g["target"], g["target_tree"], g["source"], arr, T, factor, robust, 0.7, tag=(name, j))
+    worst = 0.0
+    for j, T in enumerate([np.eye(4), NF.orthonormal(g["T"])] + noise_poses()[1:3]):
+        c_cpu, c_gpu, nm, w = triangle(ctx, reg, g["target"], g["target_tree"], g["source"], arr, T, factor, robust, 0.7, tag=(name, j))
+        worst = max(worst, w)
         # LM trial poses: cached correspondences, precision matrices frozen at the linearisation pose
         for a in ([0.01, -0.02, 0.005, 0.05, -0.03, 0.02], [0, 0, 0, 0, 0, 0]):
             T2 = T @ O.se3_exp(np.array(a, dtype=float))
             e_gpu = ctx.error(T2)
-            e_np = NF.error(T2, T, c_gpu, factor, robust, 0.7, arr.sp, arr.sc, arr.tp, arr.tn, arr.tc)
-            assert abs(e_gpu - e_np) <= RTOL * e_np, (name, j, e_gpu, e_np)
+            e_np = NF.error(T2, T, c_gpu, factor, robust, 0.7, *arr.model)
+            worst = max(worst, check_tight_error(e_gpu, e_np, (name, j)))
             e_cpu = reg.error(g["target"], g["source"], T2)
             assert abs(e_cpu - NF.error(T2, T, c_cpu, factor, robust, 0.7, arr.sp, arr.sc, arr.tp, arr.tn, arr.tc)) <= 1e-9 * e_cpu
             if nm == 0:
                 assert abs(e_gpu - e_cpu) <= RTOL * e_cpu
+    print(f"worst ratio to the storage model ({name}): {worst:.2e}")
 
 
 def test_null_rejector_and_small_radius(golden_prepared, golden_ctx):
@@ -189,6 +209,7 @@ def test_converged_pose_matches_oracle(golden_prepared, golden_ctx, name, factor
 def test_voxelmap_target(golden_prepared):
     g = golden_prepared
     sg = _sg()
+    worst = 0.0
     for offsets in (1, 7, 27):
         vm = O.GaussianVoxelMap(g["target"], 1.0, offsets)
         coords, means, covs, _ = vm.export()
@@ -196,26 +217,28 @@ def test_voxelmap_target(golden_prepared):
         ctx.set_target_voxelmap(1.0, coords, means, covs, offsets)
         ctx.set_source(g["source"].points, g["source"].covs)
         reg = O.Registration(factor=O.FACTOR_GICP, num_threads=0)
-        for T in (np.eye(4), g["T"]):
+        # the voxel means are one upload of their own: centred on their box, stored like any target point
+        model = NF.storage_model(g["source"].points, g["source"].covs, means, None, covs)
+        for T in (np.eye(4), NF.orthonormal(g["T"])):
             cpu = reg.linearize(vm, None, g["source"], T)
             gpu = ctx.linearize(T, factor=sg.FACTOR_GICP)
             c = reg.correspondences(len(g["source"]))
             cg = ctx.correspondences()
             nm = int((cg != c).sum())
             assert nm <= 2
-            # GPU sums against the numpy leg over the GPU's OWN correspondences (always), and against the oracle when they agree
+            # GPU sums against numpy on the storage model over the GPU's OWN correspondences (always), and against the oracle when they agree
             src = g["source"]
             vox_id = np.where(cg == sg.NO_CORRESPONDENCE, NF.NO, cg >> np.uint64(32))  # calc_index: voxel id << 32 (incremental_voxelmap.hpp:151)
-            args = (2, 0, 1.0, src.points, src.covs, means, None, covs)
-            check_linearized(gpu, NF.linearize(T, vox_id, *args), ("vgicp-numpy", offsets))
+            worst = max(worst, check_tight(gpu, NF.linearize(T, vox_id, 2, 0, 1.0, *model), ("vgicp-model", offsets)))
             T2 = T @ O.se3_exp(np.array([0.01, 0.0, -0.01, 0.02, 0.02, 0.0]))
             e_gpu = ctx.error(T2)
-            e_npy = NF.error(T2, T, vox_id, *args)
-            assert abs(e_gpu - e_npy) <= RTOL * e_npy
+            e_npy = NF.error(T2, T, vox_id, 2, 0, 1.0, src.points, src.covs, means, None, covs)
+            worst = max(worst, check_tight_error(e_gpu, NF.error(T2, T, vox_id, 2, 0, 1.0, *model), ("vgicp-model-error", offsets)))
             if nm == 0:
                 check_linearized(gpu, cpu, ("vgicp", offsets))
                 assert abs(e_gpu - reg.error(vm, g["source"], T2)) <= RTOL * e_npy
         ctx.close()
+    print(f"worst ratio to the storage model (voxel map): {worst:.2e}")
 
 
 def test_device_built_voxelmap_matches_oracle(golden_prepared):
@@ -282,7 +305,7 @@ def test_empty_and_tiny_inputs(golden_prepared):
         tc.set_features(g["target"].normals[:n], g["target"].covs[:n])
         c2 = load_ctx(tc, tt, g["source"])
         reg = O.Registration(factor=O.FACTOR_GICP, rejector=O.REJECT_NONE, num_threads=0)
-        triangle(c2, reg, tc, tt, g["source"], Arrays(tc, g["source"]), g["T"], 2, 0, 1.0, rejector=0, tag=("tiny", n))
+        triangle(c2, reg, tc, tt, g["source"], Arrays(tc, g["source"]), NF.orthonormal(g["T"]), 2, 0, 1.0, rejector=0, tag=("tiny", n))
         c2.close()
     # missing features are an error, not a silent fallback
     ctx.set_target(g["target"].points)
