@@ -160,6 +160,34 @@ int sgb_correspondences(sgb_ctx* ctx, uint64_t* target_index);
 /* count_if(factors, inlier()) of the last linearize (registration/optimizer.hpp:60,146). */
 int sgb_num_inliers(sgb_ctx* ctx, size_t* n);
 
+/* ---- batched registration: many sources against the one target, each at its own pose --------------
+ * The context holds EITHER one source (sgb_source_set_points) OR a batch of sources ("members"); each setter replaces the other.
+ * While a batch is set, sgb_linearize, sgb_error, sgb_correspondences, sgb_num_inliers and the _device variants fail with a
+ * message, and the _batch calls fail while a single source is set.  The batch calls are single-GPU: they fail while
+ * sgb_comm_connect* is active.  Every member is stored exactly as sgb_source_set_points would store it alone (centred on its own
+ * box, FP32, its own curve order), and its results -- H | b | e | inliers, error(), correspondences -- are bit-identical whatever
+ * else is in the batch, wherever it sits and whichever other members are inactive, EXCEPT at exact FP32 distance ties between two
+ * target points: the search returns an exact nearest neighbour, but which of two equidistant ones it returns depends on the
+ * traversal, and that may depend on the other queries of a 32-query chunk (members are not padded to chunks) and on the batch's
+ * total pending count.  sgb_drop_seeds applies to every member.
+ * The upload is not batched: sgb_source_set_batch runs the single-source conversion and sort per non-empty member (5 launches, 7
+ * with covariances), so its cost grows with the member count. */
+#define SGB_BATCH_MAX_MEMBERS 65536
+/* offsets: n_members + 1 ascending entries, offsets[0] = 0; member m = points offsets[m] .. offsets[m+1] (empty members allowed).
+ * points / covariances: all members concatenated, in the layouts above (host, page-locked or device memory). */
+int sgb_source_set_batch(sgb_ctx* ctx, size_t n_members, const size_t* offsets, const double* points_xyz1, const double* covs_4x4 /*or NULL*/);
+/* One linearize per member at its pose T_colmajor16xB[16 m ..]: out44xB[44 m ..] = H(36) | b(6) | e | num_inliers.  active (or NULL =
+ * all): an inactive member costs no search or factor work, gets zeros and keeps its cached correspondences and linearisation pose.
+ * out44xB may be host or device memory; the call returns when the results are there. */
+int sgb_linearize_batch(sgb_ctx* ctx, int factor_kind, int robust_kind, double robust_c, int rejector_kind, double max_dist_sq,
+                        const double* T_colmajor16xB, const uint8_t* active /*or NULL*/, double* out44xB);
+/* error() of every active member at its trial pose with its cached correspondences; GICP precision matrices re-derived from THAT
+ * member's last linearisation pose.  Inactive members: 0. */
+int sgb_error_batch(sgb_ctx* ctx, const double* T_colmajor16xB, const uint8_t* active /*or NULL*/, double* out_e);
+/* Correspondences of every member's last linearize, concatenated in the caller's order (offsets of sgb_source_set_batch), original
+ * target indices; SGB_NO_CORRESPONDENCE = rejected or never linearised. */
+int sgb_correspondences_batch(sgb_ctx* ctx, uint64_t* out);
+
 /* ---- per-cloud preparation on the device (SURVEY.md §8(f); not per-iteration) --------------------
  * sgb_estimate_features replaces estimate_normals / estimate_covariances / estimate_normals_covariances and
  * their _omp / _tbb variants (include/small_gicp/util/normal_estimation.hpp:12-140, normal_estimation_omp.hpp:9-60):

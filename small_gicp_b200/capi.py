@@ -50,6 +50,10 @@ _SIGNATURES = {
     "sgb_error_device": (C.c_int, [_vp, _dp, _vp]),
     "sgb_correspondences": (C.c_int, [_vp, _u64p]),
     "sgb_num_inliers": (C.c_int, [_vp, C.POINTER(C.c_size_t)]),
+    "sgb_source_set_batch": (C.c_int, [_vp, C.c_size_t, C.POINTER(C.c_size_t), _dp, _dp]),
+    "sgb_linearize_batch": (C.c_int, [_vp, C.c_int, C.c_int, C.c_double, C.c_int, C.c_double, _dp, C.POINTER(C.c_uint8), _dp]),
+    "sgb_error_batch": (C.c_int, [_vp, _dp, C.POINTER(C.c_uint8), _dp]),
+    "sgb_correspondences_batch": (C.c_int, [_vp, _u64p]),
     "sgb_estimate_features": (C.c_int, [_vp, C.c_size_t, _dp, C.c_int, _dp, _dp]),
     "sgb_target_estimate_features": (C.c_int, [_vp, C.c_int]),
     "sgb_source_estimate_features": (C.c_int, [_vp, C.c_int]),
@@ -258,6 +262,59 @@ class Context:
         out = np.empty(self.source_size, dtype=np.uint64)
         self._check(self._L.sgb_correspondences(self._h, out.ctypes.data_as(_u64p)))
         return out
+
+    # ---- batched registration: many sources ("members") against the one target, each at its own pose ----
+    def set_source_batch(self, sources, covs=None):
+        """sources: a list of (N_m, 3|4) arrays, or (points (N, 3|4), offsets (B + 1,)) with the members concatenated.
+        covs: None, a list of (N_m, 4, 4) arrays, or one (N, 4, 4) array."""
+        if isinstance(sources, tuple):
+            points, offsets = sources
+            p = _points4(points)
+            offsets = np.ascontiguousarray(offsets, dtype=np.uint64)
+            if offsets.ndim != 1 or offsets.size < 1 or int(offsets[-1]) != p.shape[0]:
+                raise SgbError(f"set_source_batch: offsets must have B + 1 entries ending at the point count {p.shape[0]}")
+        else:
+            members = [_points4(s) for s in sources]
+            offsets = np.zeros(len(members) + 1, dtype=np.uint64)
+            offsets[1:] = np.cumsum([m.shape[0] for m in members])
+            p = np.concatenate(members) if members else np.zeros((0, 4))
+        c = None
+        if covs is not None:
+            c = _f64(covs) if not isinstance(covs, (list, tuple)) else (np.concatenate([_f64(x) for x in covs]) if len(covs) else np.zeros((0, 4, 4)))
+            assert tuple(c.shape) == (p.shape[0], 4, 4)
+        offsets = offsets.astype(np.uintp)
+        self._check(self._L.sgb_source_set_batch(self._h, offsets.size - 1, offsets.ctypes.data_as(C.POINTER(C.c_size_t)), _d(p), _d(c)))
+        self._batch_offsets = offsets.astype(np.int64)
+
+    def _batch_args(self, Ts, active):
+        Ts = np.asarray(Ts, dtype=np.float64)
+        B = self._batch_offsets.size - 1
+        assert Ts.shape == (B, 4, 4), f"need ({B}, 4, 4) poses"
+        Tc = np.ascontiguousarray(Ts.transpose(0, 2, 1))  # each pose column-major
+        a = None if active is None else np.ascontiguousarray(np.asarray(active).astype(np.uint8).reshape(B))
+        return B, Tc, a, (None if a is None else a.ctypes.data_as(C.POINTER(C.c_uint8)))
+
+    def linearize_batch(self, Ts, active=None, factor=FACTOR_GICP, robust=ROBUST_NONE, robust_c=1.0, rejector=REJECT_DISTANCE, max_dist_sq=1.0):
+        """Reduction::linearize of every member at its pose -> (H (B,6,6), b (B,6), e (B,), inliers (B,)); inactive members: zeros"""
+        B, Tc, a, ap = self._batch_args(Ts, active)
+        out = np.zeros((max(B, 1), 44))
+        self._check(self._L.sgb_linearize_batch(self._h, factor, robust, float(robust_c), rejector, float(max_dist_sq), _d(Tc), ap, _d(out)))
+        out = out[:B]
+        return out[:, :36].reshape(B, 6, 6).copy(), out[:, 36:42].copy(), out[:, 42].copy(), out[:, 43].astype(np.int64)
+
+    def error_batch(self, Ts, active=None):
+        """Reduction::error of every active member at its trial pose (cached correspondences) -> (B,)"""
+        B, Tc, a, ap = self._batch_args(Ts, active)
+        out = np.zeros(max(B, 1))
+        self._check(self._L.sgb_error_batch(self._h, _d(Tc), ap, _d(out)))
+        return out[:B].copy()
+
+    def correspondences_batch(self):
+        """list of per-member correspondence arrays (original target indices, NO_CORRESPONDENCE = rejected)"""
+        off = self._batch_offsets
+        out = np.empty(max(int(off[-1]), 1), dtype=np.uint64)
+        self._check(self._L.sgb_correspondences_batch(self._h, out.ctypes.data_as(_u64p)))
+        return [out[off[m] : off[m + 1]].copy() for m in range(off.size - 1)]
 
     # ---- multi-GPU: all-reduce of H|b|e fused into the reduction kernel (peer memory over NVLink) ----
     COMM_HANDLE_BYTES = 64

@@ -1,0 +1,218 @@
+// SPDX-License-Identifier: MIT
+// Batched registration (DESIGN.md §11): B source clouds ("members") against the one target of the context, each at its own pose.
+//   batch_transform_kernel  member pose applied once per point: the FP32 query of every point of the active members, written as a
+//                           "virtual source" (target-centred, identity pose) that the single-source search kernels walk unchanged
+//   batch_factor_kernel     one CTA per 128-point tile of ONE member: FP64 rejector + factor (or error()) at that member's pose,
+//                           voxel-map probe for VGICP, CTA sum -> one partial per tile
+//   batch_segment_kernel    one CTA per member: its tiles' partials in tile order -> H|b|e|inliers (or e) of that member
+// A member's sums depend on its own points, pose and correspondences only, added in an order fixed by its size: bit-identical whatever
+// else is in the batch.
+#include <cfloat>
+
+#include "sgb_batch.h"
+#include "sgb_device.cuh"
+
+namespace sgb {
+
+// CTA sum of per-thread accumulators, thread k < NACC returns sum k: the transposing butterfly of block_reduce_and_finish
+// (sgb_device.cuh), kept apart from it because inlining a shared helper there changed the register allocation of the
+// single-source kernels.
+template <int NACC>
+__device__ __forceinline__ double tile_sum(const double* acc) {
+  __shared__ double s_red[kLinBlock / 32][NACC];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  if (NACC > 4) {
+    double v[32];
+#pragma unroll
+    for (int k = 0; k < 32; k++) v[k] = k < NACC ? acc[k] : 0.0;
+#pragma unroll
+    for (int w = 16; w >= 1; w >>= 1) {
+      const bool upper = (lane & w) != 0;
+#pragma unroll
+      for (int k = 0; k < w; k++) {
+        if (k >= NACC) continue;
+        const double keep = upper ? v[k + w] : v[k];
+        const double send = upper ? v[k] : v[k + w];
+        v[k] = keep + __shfl_xor_sync(0xffffffffu, send, w);
+      }
+    }
+    if (lane < NACC) s_red[warp][lane] = v[0];
+  } else {
+#pragma unroll
+    for (int k = 0; k < NACC; k++) {
+      double v = acc[k];
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) v += __shfl_down_sync(0xffffffffu, v, o);
+      if (lane == 0) s_red[warp][k] = v;
+    }
+  }
+  __syncthreads();
+  double v = 0.0;
+  if (threadIdx.x < NACC) {
+#pragma unroll
+    for (int w = 0; w < kLinBlock / 32; w++) v += s_red[w][threadIdx.x];
+  }
+  return v;
+}
+
+__global__ void __launch_bounds__(kLinBlock) batch_transform_kernel(const __grid_constant__ BatchParams B, float4* vq, uint32_t* vcorr) {
+  const BatchTile t = B.tiles[blockIdx.x];
+  const uint32_t tid = threadIdx.x;
+  if (tid >= t.count) return;
+  const uint32_t i = t.first + tid, v = t.vfirst + tid;
+  // the single-source kernels' transform, term for term (grid_probe_blocks_kernel, packet_search_kernel): the same FP32 query
+  const double* R = B.poses + 12 * static_cast<size_t>(t.member);
+  const double* cs = B.centres + 4 * static_cast<size_t>(t.member);
+  const double csx = cs[0], csy = cs[1], csz = cs[2];
+  const double tpx = R[0] * csx + R[1] * csy + R[2] * csz + R[9] - B.tgt.centre[0];
+  const double tpy = R[3] * csx + R[4] * csy + R[5] * csz + R[10] - B.tgt.centre[1];
+  const double tpz = R[6] * csx + R[7] * csy + R[8] * csz + R[11] - B.tgt.centre[2];
+  const float4 s = __ldg(&B.pts[i]);
+  const double sx = s.x, sy = s.y, sz = s.z;
+  const float fx = static_cast<float>(R[0] * sx + R[1] * sy + R[2] * sz + tpx);
+  const float fy = static_cast<float>(R[3] * sx + R[4] * sy + R[5] * sz + tpy);
+  const float fz = static_cast<float>(R[6] * sx + R[7] * sy + R[8] * sz + tpz);
+  vq[v] = make_float4(fx, fy, fz, 0.f);
+  // the member's previous correspondence seeds the search (seeds only prune: the result does not depend on them)
+  vcorr[v] = (B.members[t.member].z & kMemberSeeded) ? B.corr[i] : kNone;
+}
+
+// ERR = false: linearize (VOX: voxel-map probe here; else vcorr = what the search found); ERR = true: error() with the cached corr[]
+template <int FACTOR, int ROBUST, bool VOX, bool ERR>
+__global__ void __launch_bounds__(kLinBlock, 4) batch_factor_kernel(const __grid_constant__ BatchParams B, const uint32_t* __restrict__ vcorr) {
+  constexpr int NACC = ERR ? 1 : kAcc + 1;
+  double acc[NACC];
+#pragma unroll
+  for (int k = 0; k < NACC; k++) acc[k] = 0.0;
+  const BatchTile t = B.tiles[blockIdx.x];
+  const uint32_t tid = threadIdx.x;
+  if (tid < t.count) {
+    const uint32_t i = t.first + tid;
+    const double* R = B.poses + 12 * static_cast<size_t>(t.member);
+    const double* cs = B.centres + 4 * static_cast<size_t>(t.member);
+    const double csx = cs[0], csy = cs[1], csz = cs[2];
+    const double ctx = B.tgt.centre[0], cty = B.tgt.centre[1], ctz = B.tgt.centre[2];
+    const double tpx = R[0] * csx + R[1] * csy + R[2] * csz + R[9] - ctx;
+    const double tpy = R[3] * csx + R[4] * csy + R[5] * csz + R[10] - cty;
+    const double tpz = R[6] * csx + R[7] * csy + R[8] * csz + R[11] - ctz;
+    const float4 sp = __ldg(&B.pts[i]);
+    const float4 z = make_float4(0.f, 0.f, 0.f, 0.f);
+    const float4 sA = FACTOR == 2 ? __ldg(&B.covA[i]) : z, sB = FACTOR == 2 ? __ldg(&B.covB[i]) : z;
+    if (ERR) {
+      const uint32_t k = B.corr[i];
+      if (k != kNone) {
+        const float4 tq = __ldg(&B.tgt.pts[k]);
+        const float4 t1 = FACTOR == 1 ? __ldg(&B.tgt.normals[k]) : (FACTOR == 2 ? __ldg(&B.tgt.covA[k]) : z);
+        const float4 t2 = FACTOR == 2 ? __ldg(&B.tgt.covB[k]) : z;
+        // GICP: precision matrix re-derived from THIS member's linearisation pose (gicp_factor.hpp:81-89)
+        acc[0] += point_error<FACTOR, ROBUST>(R, tpx, tpy, tpz, B.lin_poses + 12 * static_cast<size_t>(t.member), B.robust_c, sp, sA, sB, tq, t1, t2);
+      }
+    } else if (VOX) {
+      // linearize_vox_kernel's per-point work at this member's pose
+      const double sx = sp.x, sy = sp.y, sz = sp.z;
+      const double qx = R[0] * sx + R[1] * sy + R[2] * sz + tpx;
+      const double qy = R[3] * sx + R[4] * sy + R[5] * sz + tpy;
+      const double qz = R[6] * sx + R[7] * sy + R[8] * sz + tpz;
+      double brx = 0, bry = 0, brz = 0;
+      const uint32_t best = vox_nearest(B.tgt, qx, qy, qz, ctx, cty, ctz, B.max_dist_sq_d, brx, bry, brz);
+      B.corr[i] = best;
+      if (best != kNone) {
+        Sym3 M;
+        if (FACTOR == 2) {
+          M = gicp_precision(R, sA, sB, __ldg(&B.tgt.covA[best]), __ldg(&B.tgt.covB[best]));
+        } else {
+          M = Sym3{1.0, 0.0, 0.0, 1.0, 0.0, 1.0};
+        }
+        accumulate_factor<ROBUST>(R, M, brx, bry, brz, csx + sx, csy + sy, csz + sz, B.robust_c, acc);
+        acc[kAcc] += 1.0;
+      }
+    } else {
+      // factor_reduce_kernel's per-point work at this member's pose
+      uint32_t best = vcorr[t.vfirst + tid];
+      if (best != kNone) {
+        const float4 tq = __ldg(&B.tgt.pts[best]);
+        const float4 t1 = FACTOR == 1 ? __ldg(&B.tgt.normals[best]) : (FACTOR == 2 ? __ldg(&B.tgt.covA[best]) : z);
+        const float4 t2 = FACTOR == 2 ? __ldg(&B.tgt.covB[best]) : z;
+        if (!point_linearize_source<FACTOR, ROBUST>(R, tpx, tpy, tpz, csx, csy, csz, B.max_dist_sq_d, B.robust_c, sp, &sA, &sB, tq, &t1, &t2, acc))
+          best = kNone;  // rejected: error() and the correspondences must not see it
+      }
+      B.corr[i] = best;
+    }
+  }
+  const double v = tile_sum<NACC>(acc);
+  if (tid < NACC) B.tile_partials[static_cast<size_t>(blockIdx.x) * kPartialStride + tid] = v;
+}
+
+// One CTA per member: warp w adds tiles w, w + 8, ... of the member in order, then the 8 warp sums are added in warp order.  The order
+// depends on the member's tile count only.  Members without tiles (inactive or empty) get zeros.  LIN: the member's pose becomes its
+// linearisation pose (read by later error() calls).
+constexpr int kSegWarps = 8;
+template <int NACC, bool LIN>
+__global__ void __launch_bounds__(kSegWarps * 32) batch_segment_kernel(const __grid_constant__ BatchParams B, double* out) {
+  __shared__ double s_sum[kSegWarps][NACC];
+  const uint32_t m = blockIdx.x, lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
+  const uint4 mem = B.members[m];
+  if (lane < static_cast<uint32_t>(NACC)) {
+    double v = 0.0;
+    for (uint32_t t = warp; t < mem.y; t += kSegWarps) v += __ldcg(&B.tile_partials[static_cast<size_t>(mem.x + t) * kPartialStride + lane]);
+    s_sum[warp][lane] = v;
+  }
+  __syncthreads();
+  if (threadIdx.x < static_cast<uint32_t>(NACC)) {
+    double v = 0.0;
+#pragma unroll
+    for (int w = 0; w < kSegWarps; w++) v += s_sum[w][threadIdx.x];
+    if (LIN) {
+      double* o = out + 44 * static_cast<size_t>(m);
+      int p0, p1;
+      if (expand_positions(threadIdx.x, p0, p1) == 2) o[p1] = v;
+      o[p0] = v;
+    } else {
+      out[m] = v;
+    }
+  }
+  if (LIN && (mem.z & kMemberActive) && threadIdx.x < 12) B.lin_poses[12 * static_cast<size_t>(m) + threadIdx.x] = B.poses[12 * static_cast<size_t>(m) + threadIdx.x];
+}
+
+cudaError_t launch_batch_transform(const BatchParams& B, uint32_t n_tiles, float4* vq, uint32_t* vcorr, cudaStream_t st) {
+  batch_transform_kernel<<<n_tiles, kLinBlock, 0, st>>>(B, vq, vcorr);
+  return cudaGetLastError();
+}
+
+template <int FACTOR, int ROBUST>
+static cudaError_t launch_bf(const BatchParams& B, uint32_t n_tiles, bool voxel, bool err, const uint32_t* vcorr, cudaStream_t st) {
+  if (err)
+    batch_factor_kernel<FACTOR, ROBUST, false, true><<<n_tiles, kLinBlock, 0, st>>>(B, vcorr);
+  else if (voxel)
+    batch_factor_kernel<(FACTOR == 1 ? 0 : FACTOR), ROBUST, true, false><<<n_tiles, kLinBlock, 0, st>>>(B, vcorr);
+  else
+    batch_factor_kernel<FACTOR, ROBUST, false, false><<<n_tiles, kLinBlock, 0, st>>>(B, vcorr);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_batch_factor(const BatchParams& B, int factor, int robust, uint32_t n_tiles, bool voxel, bool err, const uint32_t* vcorr,
+                                cudaStream_t st) {
+  if (voxel && factor == 1 && !err) return cudaErrorInvalidValue;
+  switch (factor * 3 + robust) {
+    case 0: return launch_bf<0, 0>(B, n_tiles, voxel, err, vcorr, st);
+    case 1: return launch_bf<0, 1>(B, n_tiles, voxel, err, vcorr, st);
+    case 2: return launch_bf<0, 2>(B, n_tiles, voxel, err, vcorr, st);
+    case 3: return launch_bf<1, 0>(B, n_tiles, voxel, err, vcorr, st);
+    case 4: return launch_bf<1, 1>(B, n_tiles, voxel, err, vcorr, st);
+    case 5: return launch_bf<1, 2>(B, n_tiles, voxel, err, vcorr, st);
+    case 6: return launch_bf<2, 0>(B, n_tiles, voxel, err, vcorr, st);
+    case 7: return launch_bf<2, 1>(B, n_tiles, voxel, err, vcorr, st);
+    case 8: return launch_bf<2, 2>(B, n_tiles, voxel, err, vcorr, st);
+    default: return cudaErrorInvalidValue;
+  }
+}
+
+cudaError_t launch_batch_segment(const BatchParams& B, uint32_t n_members, bool linearize, double* out, cudaStream_t st) {
+  if (linearize)
+    batch_segment_kernel<kAcc + 1, true><<<n_members, kSegWarps * 32, 0, st>>>(B, out);
+  else
+    batch_segment_kernel<1, false><<<n_members, kSegWarps * 32, 0, st>>>(B, out);
+  return cudaGetLastError();
+}
+
+}  // namespace sgb

@@ -1,0 +1,40 @@
+// SPDX-License-Identifier: MIT
+// Batched registration: device-side layout and launchers (sgb_batch.cu; C-ABI in sgb_capi_batch.cu).
+#pragma once
+#include <cuda_runtime.h>
+#include <stdint.h>
+
+#include "sgb_device.cuh"
+
+namespace sgb {
+
+/// 128 consecutive points (or fewer, at the end of a member) of ONE member: `first` = position in the member-concatenated storage,
+/// `vfirst` = position in the virtual source of this call (the active members' points, concatenated)
+struct __align__(16) BatchTile {
+  uint32_t member, first, count, vfirst;
+};
+/// per member: x = first tile of this call, y = tile count (0: inactive or empty), z = flags
+constexpr uint32_t kMemberActive = 1u, kMemberSeeded = 2u;
+
+struct BatchParams {
+  DevTarget tgt;
+  const float4* pts;   // members concatenated, each centred on its own box and in its own curve order (as sgb_source_set_points stores one cloud)
+  const float4* covA;
+  const float4* covB;
+  const double* centres;  // [members][4]
+  const double* poses;    // [members][12] row-major R | t of this call
+  double* lin_poses;      // [members][12] pose of each member's last linearize
+  const BatchTile* tiles;
+  const uint4* members;
+  uint32_t* corr;         // per stored point: leaf-order position / voxel id of its correspondence, or kNone
+  double max_dist_sq_d;
+  double robust_c;
+  double* tile_partials;  // [tiles][kPartialStride]
+};
+
+cudaError_t launch_batch_transform(const BatchParams& B, uint32_t n_tiles, float4* vq, uint32_t* vcorr, cudaStream_t st);
+cudaError_t launch_batch_factor(const BatchParams& B, int factor, int robust, uint32_t n_tiles, bool voxel, bool err, const uint32_t* vcorr, cudaStream_t st);
+/// out: [members][44] (linearize) or [members] (error)
+cudaError_t launch_batch_segment(const BatchParams& B, uint32_t n_members, bool linearize, double* out, cudaStream_t st);
+
+}  // namespace sgb

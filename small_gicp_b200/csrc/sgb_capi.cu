@@ -87,7 +87,9 @@ int upload_tree(sgb_ctx* ctx, const FlatTree& tree, const float* host_pts_xyzw) 
   return build_grid(ctx);
 }
 
-int fill_params(sgb_ctx* ctx, LinParams& P, const double* T_colmajor16) {
+}  // namespace
+
+int sgb::fill_params(sgb_ctx* ctx, LinParams& P, const double* T_colmajor16) {
   std::memset(&P, 0, sizeof(P));
   P.tgt.pts = ctx->tgt_pts.as<float4>();
   P.tgt.normals = ctx->tgt_normals.as<float4>();
@@ -120,6 +122,8 @@ int fill_params(sgb_ctx* ctx, LinParams& P, const double* T_colmajor16) {
   }
   return 0;
 }
+
+namespace {
 
 int do_linearize_impl(sgb_ctx* ctx, int factor, int robust, double robust_c, int rejector, double max_dist_sq, const double* T, double* d_out) {
   if (factor < 0 || factor > 2 || robust < 0 || robust > 2 || rejector < 0 || rejector > 1) return fail(ctx, 1, "sgb_linearize: invalid factor/robust/rejector kind");
@@ -189,93 +193,13 @@ int do_linearize_impl(sgb_ctx* ctx, int factor, int robust, double robust_c, int
 #endif
   if (split_path) {
     // phase 1: search at high occupancy; phase 2: factor algebra + reduction (sgb_kernels_split.cu)
-    const uint32_t chunk_pts = 32u * ctx->src_run;
-    const size_t n_chunks = (ctx->n_src + chunk_pts - 1) / chunk_pts;
-    int sgrid = static_cast<int>((n_chunks * 32 + kLinBlock - 1) / kLinBlock);
     if (packet_path) {
-      const int scap = ctx->sm_count * packet_occupancy(depth);
-      if (sgrid > scap) sgrid = scap;
-      const uint8_t* settled = nullptr;
-      const uint32_t* pending_count = nullptr;
-      ChunkClasses cc = {};
-      PendingParams pp = {};
-      // more pending queries than this: packet search over the chunk-ordered queries, else a warp per pending query
-      const uint32_t pending_split = static_cast<uint32_t>(ctx->n_src / static_cast<size_t>(ctx->pending_div));
-      if (ctx->grid_ready) {
-        // grid front end: settles every query whose nearest neighbour lies within half a cell (sgb_grid.cu)
-        CU(ctx->grid_state.reserve(ctx->n_src));
-        GridParams g;
-        for (int a = 0; a < 3; a++) g.origin[a] = ctx->grid_origin[a];
-        g.inv_cell = ctx->grid_inv_cell;
-        g.settle_d2 = ctx->grid_settle_d2;
-        // [0], [1]: two pending counters that alternate between calls (each probe clears the other one), [2..]: the list
-        const void* before = ctx->grid_pending.p;
-        CU(ctx->grid_pending.reserve((ctx->n_src + 2) * sizeof(uint32_t)));
-        if (ctx->grid_pending.p != before || !ctx->pending_clean) {
-          CU(cudaMemsetAsync(ctx->grid_pending.p, 0, 2 * sizeof(uint32_t), ctx->stream));
-          ctx->pending_clean = true;
-        }
-        uint32_t* pbase = ctx->grid_pending.as<uint32_t>();
-        uint32_t* pc = pbase + ctx->pending_parity;
-        uint32_t* plist = pbase + 2;
-        if (ctx->grid_blocks && ctx->use_chunk_classes) {
-          // work lists of the packet search by cost class; counters alternate like the pending counters (sized in sgb_source_set_points)
-          const uint32_t nck = static_cast<uint32_t>((ctx->n_src + 31) / 32);
-          const void* cb = ctx->chunk_lists.p;
-          CU(ctx->chunk_lists.reserve((8 + static_cast<size_t>(kChunkClasses) * nck) * sizeof(uint32_t)));
-          if (ctx->chunk_lists.p != cb || !ctx->chunk_lists_clean) {
-            CU(cudaMemsetAsync(ctx->chunk_lists.p, 0, 8 * sizeof(uint32_t), ctx->stream));
-            ctx->chunk_lists_clean = true;
-          }
-          uint32_t* cbase = ctx->chunk_lists.as<uint32_t>();
-          cc.count = cbase + 4 * ctx->pending_parity;
-          cc.count_next = cbase + 4 * (ctx->pending_parity ^ 1);
-          cc.lists = cbase + 8;
-          cc.n_chunks = nck;
-          const float cell = ctx->grid_cell;
-          cc.wide_r2 = ctx->class_wide_cells * ctx->class_wide_cells * cell * cell;  // search balls wider than two cells / one cell
-          cc.mid_r2 = cell * cell;
-          cc.fallback_pct = ctx->class_fallback_pct;
-        }
-        CU(ctx->grid_pending_q.reserve(ctx->n_src * sizeof(float4)));
-        CU(launch_grid_probe(P, ctx->grid_pts.as<float4>(), ctx->grid_table.as<GridSlot>(), ctx->grid_capacity, g, ctx->grid_state.as<uint8_t>(), pc,
-                             plist, ctx->grid_pending_q.as<float4>(), pbase + (ctx->pending_parity ^ 1), cc, ctx->stream));
-        ctx->pending_parity ^= 1;
-        // the finishing kernel (below) serves both regimes: few pending queries warp-per-query, many through the packet walk
-        pp.list = plist;
-        pp.q = ctx->grid_pending_q.as<float4>();
-        pp.grid_pts = ctx->grid_pts.as<float4>();
-        pp.table = (ctx->grid_blocks && ctx->use_ring) ? ctx->grid_table.as<GridSlot>() : nullptr;
-        pp.capacity = ctx->grid_capacity;
-        pp.g = g;
-        ctx->launches += 1;
-        settled = ctx->grid_state.as<uint8_t>();
-        pending_count = pc;
-      }
-      // many pending queries: the packet search walks the tree
-      {
-      uint32_t *queue = nullptr, *queue_next = nullptr;
-      if (ctx->use_packet_queue) {
-        if (!ctx->packet_queue.p) {  // first use: two zeroed counters (afterwards every launch clears the other one)
-          CU(ctx->packet_queue.reserve(2 * sizeof(uint32_t)));
-          CU(cudaMemsetAsync(ctx->packet_queue.p, 0, 2 * sizeof(uint32_t), ctx->stream));
-        }
-        queue = ctx->packet_queue.as<uint32_t>() + ctx->packet_parity;
-        queue_next = ctx->packet_queue.as<uint32_t>() + (ctx->packet_parity ^ 1);
-        ctx->packet_parity ^= 1;
-      }
-      CU(launch_packet_search(P, ctx->tgt_pnodes.as<float4>(), sgrid, depth, settled, pending_count, pending_split, queue, queue_next, cc, pp, ctx->tma_leaf, ctx->stream));
-      }
-#ifdef SGB_PROFILING
-      if (ctx->debug_pending && pending_count) {  // profiling aid: synchronises
-        uint32_t h = 0;
-        CU(cudaMemcpyAsync(&h, pending_count, sizeof(h), cudaMemcpyDeviceToHost, ctx->stream));
-        CU(cudaStreamSynchronize(ctx->stream));
-        std::fprintf(stderr, "[sgb] grid front end: %u of %zu queries pending (cell %.4g)\n", h, ctx->n_src, ctx->grid_cell);
-      }
-#endif
+      if (int rc = launch_point_search(ctx, P, depth)) return rc;
     } else {
 #ifdef SGB_PROFILING
+      const uint32_t chunk_pts = 32u * ctx->src_run;
+      const size_t n_chunks = (ctx->n_src + chunk_pts - 1) / chunk_pts;
+      int sgrid = static_cast<int>((n_chunks * 32 + kLinBlock - 1) / kLinBlock);
       const int scap = ctx->sm_count * search_occupancy(depth);
       if (sgrid > scap) sgrid = scap;
       CU(launch_search(P, sgrid, depth, ctx->stream));
@@ -303,6 +227,95 @@ int do_linearize_impl(sgb_ctx* ctx, int factor, int robust, double robust_c, int
   std::memcpy(ctx->Tlin, P.T, sizeof(P.T));
   return 0;
 }
+}  // namespace
+
+// The search of a point target over P.src (P.src.n queries): grid probe, then the packet search / warp-per-query finish.  Fills P.corr.
+int sgb::launch_point_search(sgb_ctx* ctx, const LinParams& P, int depth) {
+  const size_t n = P.src.n;
+  int sgrid = static_cast<int>((((n + 31) / 32) * 32 + kLinBlock - 1) / kLinBlock);
+  const int scap = ctx->sm_count * packet_occupancy(depth);
+  if (sgrid > scap) sgrid = scap;
+  const uint8_t* settled = nullptr;
+  const uint32_t* pending_count = nullptr;
+  ChunkClasses cc = {};
+  PendingParams pp = {};
+  // more pending queries than this: packet search over the chunk-ordered queries, else a warp per pending query
+  const uint32_t pending_split = static_cast<uint32_t>(n / static_cast<size_t>(ctx->pending_div));
+  if (ctx->grid_ready) {
+    // grid front end: settles every query whose nearest neighbour lies within half a cell (sgb_grid.cu)
+    CU(ctx->grid_state.reserve(n));
+    GridParams g;
+    for (int a = 0; a < 3; a++) g.origin[a] = ctx->grid_origin[a];
+    g.inv_cell = ctx->grid_inv_cell;
+    g.settle_d2 = ctx->grid_settle_d2;
+    // [0], [1]: two pending counters that alternate between calls (each probe clears the other one), [2..]: the list
+    const void* before = ctx->grid_pending.p;
+    CU(ctx->grid_pending.reserve((n + 2) * sizeof(uint32_t)));
+    if (ctx->grid_pending.p != before || !ctx->pending_clean) {
+      CU(cudaMemsetAsync(ctx->grid_pending.p, 0, 2 * sizeof(uint32_t), ctx->stream));
+      ctx->pending_clean = true;
+    }
+    uint32_t* pbase = ctx->grid_pending.as<uint32_t>();
+    uint32_t* pc = pbase + ctx->pending_parity;
+    uint32_t* plist = pbase + 2;
+    if (ctx->grid_blocks && ctx->use_chunk_classes) {
+      // work lists of the packet search by cost class; counters alternate like the pending counters (sized in sgb_source_set_points)
+      const uint32_t nck = static_cast<uint32_t>((n + 31) / 32);
+      const void* cb = ctx->chunk_lists.p;
+      CU(ctx->chunk_lists.reserve((8 + static_cast<size_t>(kChunkClasses) * nck) * sizeof(uint32_t)));
+      if (ctx->chunk_lists.p != cb || !ctx->chunk_lists_clean) {
+        CU(cudaMemsetAsync(ctx->chunk_lists.p, 0, 8 * sizeof(uint32_t), ctx->stream));
+        ctx->chunk_lists_clean = true;
+      }
+      uint32_t* cbase = ctx->chunk_lists.as<uint32_t>();
+      cc.count = cbase + 4 * ctx->pending_parity;
+      cc.count_next = cbase + 4 * (ctx->pending_parity ^ 1);
+      cc.lists = cbase + 8;
+      cc.n_chunks = nck;
+      const float cell = ctx->grid_cell;
+      cc.wide_r2 = ctx->class_wide_cells * ctx->class_wide_cells * cell * cell;  // search balls wider than two cells / one cell
+      cc.mid_r2 = cell * cell;
+      cc.fallback_pct = ctx->class_fallback_pct;
+    }
+    CU(ctx->grid_pending_q.reserve(n * sizeof(float4)));
+    CU(launch_grid_probe(P, ctx->grid_pts.as<float4>(), ctx->grid_table.as<GridSlot>(), ctx->grid_capacity, g, ctx->grid_state.as<uint8_t>(), pc,
+                         plist, ctx->grid_pending_q.as<float4>(), pbase + (ctx->pending_parity ^ 1), cc, ctx->stream));
+    ctx->pending_parity ^= 1;
+    // the finishing kernel (below) serves both regimes: few pending queries warp-per-query, many through the packet walk
+    pp.list = plist;
+    pp.q = ctx->grid_pending_q.as<float4>();
+    pp.grid_pts = ctx->grid_pts.as<float4>();
+    pp.table = (ctx->grid_blocks && ctx->use_ring) ? ctx->grid_table.as<GridSlot>() : nullptr;
+    pp.capacity = ctx->grid_capacity;
+    pp.g = g;
+    ctx->launches += 1;
+    settled = ctx->grid_state.as<uint8_t>();
+    pending_count = pc;
+  }
+  // many pending queries: the packet search walks the tree
+  uint32_t *queue = nullptr, *queue_next = nullptr;
+  if (ctx->use_packet_queue) {
+    if (!ctx->packet_queue.p) {  // first use: two zeroed counters (afterwards every launch clears the other one)
+      CU(ctx->packet_queue.reserve(2 * sizeof(uint32_t)));
+      CU(cudaMemsetAsync(ctx->packet_queue.p, 0, 2 * sizeof(uint32_t), ctx->stream));
+    }
+    queue = ctx->packet_queue.as<uint32_t>() + ctx->packet_parity;
+    queue_next = ctx->packet_queue.as<uint32_t>() + (ctx->packet_parity ^ 1);
+    ctx->packet_parity ^= 1;
+  }
+  CU(launch_packet_search(P, ctx->tgt_pnodes.as<float4>(), sgrid, depth, settled, pending_count, pending_split, queue, queue_next, cc, pp, ctx->tma_leaf, ctx->stream));
+#ifdef SGB_PROFILING
+  if (ctx->debug_pending && pending_count) {  // profiling aid: synchronises
+    uint32_t h = 0;
+    CU(cudaMemcpyAsync(&h, pending_count, sizeof(h), cudaMemcpyDeviceToHost, ctx->stream));
+    CU(cudaStreamSynchronize(ctx->stream));
+    std::fprintf(stderr, "[sgb] grid front end: %u of %zu queries pending (cell %.4g)\n", h, n, ctx->grid_cell);
+  }
+#endif
+  return 0;
+}
+
+namespace {
 
 int do_error_impl(sgb_ctx* ctx, const double* T, double* d_out) {
   if (!T) return fail(ctx, 1, "sgb_error: null pose");
@@ -367,6 +380,7 @@ int comm_poison(sgb_ctx* ctx, const double* T, double* d_out, bool linearize) {
 }
 
 int do_linearize(sgb_ctx* ctx, int factor, int robust, double robust_c, int rejector, double max_dist_sq, const double* T, double* d_out) {
+  if (ctx->src_is_batch) return fail(ctx, 1, "sgb_linearize: the context holds a batch of sources (sgb_source_set_batch); use sgb_linearize_batch");
   if (ctx->comm_failed) return fail(ctx, 5, "sgb_linearize: an earlier multi-GPU exchange of this context failed; call sgb_comm_connect again");
   const unsigned long long seq0 = ctx->comm_seq;
   const int rc = do_linearize_impl(ctx, factor, robust, robust_c, rejector, max_dist_sq, T, d_out);
@@ -375,6 +389,7 @@ int do_linearize(sgb_ctx* ctx, int factor, int robust, double robust_c, int reje
 }
 
 int do_error(sgb_ctx* ctx, const double* T, double* d_out) {
+  if (ctx->src_is_batch) return fail(ctx, 1, "sgb_error: the context holds a batch of sources (sgb_source_set_batch); use sgb_error_batch");
   if (ctx->comm_failed) return fail(ctx, 5, "sgb_error: an earlier multi-GPU exchange of this context failed; call sgb_comm_connect again");
   const unsigned long long seq0 = ctx->comm_seq;
   const int rc = do_error_impl(ctx, T, d_out);
@@ -822,6 +837,7 @@ int sgb_source_set_points(sgb_ctx* ctx, size_t n, const double* points, const do
   if (n && !points) return fail(ctx, 1, "sgb_source_set_points: null points");
   if (n >= (1ull << 31)) return fail(ctx, 1, "sgb_source_set_points: too many points");
   CU(cudaSetDevice(ctx->device));
+  ctx->src_is_batch = false;
   ctx->n_src = n;
   ctx->src_has_covs = covs != nullptr;
   ctx->have_lin = false;
@@ -967,6 +983,7 @@ int sgb_error(sgb_ctx* ctx, const double* T, double* out_e) {
 
 int sgb_correspondences(sgb_ctx* ctx, uint64_t* target_index) {
   if (!ctx) return 1;
+  if (ctx->src_is_batch) return fail(ctx, 1, "sgb_correspondences: the context holds a batch of sources (sgb_source_set_batch); use sgb_correspondences_batch");
   if (!ctx->have_lin) return fail(ctx, 1, "sgb_correspondences: no preceding sgb_linearize");
   if (ctx->n_src == 0) return 0;
   if (!target_index) return fail(ctx, 1, "sgb_correspondences: null output");
@@ -982,6 +999,7 @@ int sgb_correspondences(sgb_ctx* ctx, uint64_t* target_index) {
 
 int sgb_num_inliers(sgb_ctx* ctx, size_t* n) {
   if (!ctx || !n) return 1;
+  if (ctx->src_is_batch) return fail(ctx, 1, "sgb_num_inliers: the context holds a batch of sources (sgb_source_set_batch); sgb_linearize_batch returns each member's count");
   if (!ctx->have_lin || !ctx->last_out) return fail(ctx, 1, "sgb_num_inliers: no preceding sgb_linearize");
   CU(cudaSetDevice(ctx->device));
   if (ctx->last_out == ctx->h_out_dev) {  // sgb_linearize left the count in the mapped host slot

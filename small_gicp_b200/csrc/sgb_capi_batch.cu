@@ -1,0 +1,316 @@
+// SPDX-License-Identifier: MIT
+// C-ABI of batched registration (include/sgicp_b200.h: sgb_source_set_batch, sgb_{linearize,error,correspondences}_batch).
+// Kernels in sgb_batch.cu; DESIGN.md §11.
+#include <cuda_runtime.h>
+
+#include <algorithm>
+#include <cfloat>
+#include <cmath>
+#include <cstring>
+#include <string>
+#include <vector>
+
+#include "../../include/sgicp_b200.h"
+#include "sgb_batch.h"
+#include "sgb_context.hpp"
+#include "sgb_kernels.h"
+
+using namespace sgb;
+
+namespace {
+
+constexpr double kIdentity[16] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1};
+
+size_t batch_points(const sgb_ctx* ctx) { return ctx->b_offsets.empty() ? 0 : ctx->b_offsets.back(); }
+size_t batch_members(const sgb_ctx* ctx) { return ctx->b_offsets.empty() ? 0 : ctx->b_offsets.size() - 1; }
+size_t max_tiles(const sgb_ctx* ctx) { return batch_points(ctx) / kLinBlock + batch_members(ctx) + 1; }
+
+int batch_check(sgb_ctx* ctx, const char* who, const double* T) {
+  if (!ctx->src_is_batch) return fail(ctx, 1, std::string(who) + ": the context holds no batch of sources (call sgb_source_set_batch)");
+  if (ctx->comm_world > 1) return fail(ctx, 1, std::string(who) + ": batched calls are single-GPU only (call sgb_comm_disconnect first)");
+  if (!T) return fail(ctx, 1, std::string(who) + ": null poses");
+  return 0;
+}
+
+// The tables of one call: every active non-empty member's points cut into tiles of kLinBlock (the virtual source concatenates the
+// active members in member order), each member's pose (row-major R | t).  Uploaded on the context's stream.
+int batch_tables(sgb_ctx* ctx, const double* T, const uint8_t* active, bool seeds, uint32_t* n_tiles, uint32_t* n_virtual) {
+  const size_t B = batch_members(ctx);
+  std::vector<double> poses(12 * B);
+  std::vector<BatchTile> tiles;
+  std::vector<uint4> members(B);
+  uint32_t v = 0;
+  for (size_t m = 0; m < B; m++) {
+    const double* Tm = T + 16 * m;
+    for (int i = 0; i < 3; i++) {
+      for (int j = 0; j < 3; j++) poses[12 * m + i * 3 + j] = Tm[j * 4 + i];
+      poses[12 * m + 9 + i] = Tm[12 + i];
+    }
+    const bool act = !active || active[m];
+    const uint32_t first = static_cast<uint32_t>(ctx->b_offsets[m]), n = static_cast<uint32_t>(ctx->b_offsets[m + 1] - ctx->b_offsets[m]);
+    const uint32_t t0 = static_cast<uint32_t>(tiles.size());
+    if (act) {
+      for (uint32_t j = 0; j < n; j += kLinBlock) tiles.push_back(BatchTile{static_cast<uint32_t>(m), first + j, std::min<uint32_t>(kLinBlock, n - j), v + j});
+      v += n;
+    }
+    members[m] = make_uint4(t0, static_cast<uint32_t>(tiles.size()) - t0, (act ? kMemberActive : 0u) | (seeds && ctx->b_seeded[m] ? kMemberSeeded : 0u), 0u);
+  }
+  // pageable host memory: the copies are staged before cudaMemcpyAsync returns
+  CU(cudaMemcpyAsync(ctx->b_poses.p, poses.data(), poses.size() * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
+  CU(cudaMemcpyAsync(ctx->b_members.p, members.data(), members.size() * sizeof(uint4), cudaMemcpyHostToDevice, ctx->stream));
+  if (!tiles.empty()) CU(cudaMemcpyAsync(ctx->b_tiles.p, tiles.data(), tiles.size() * sizeof(BatchTile), cudaMemcpyHostToDevice, ctx->stream));
+  *n_tiles = static_cast<uint32_t>(tiles.size());
+  *n_virtual = v;
+  return 0;
+}
+
+BatchParams batch_params(sgb_ctx* ctx, const LinParams& P) {
+  BatchParams B = {};
+  B.tgt = P.tgt;
+  B.pts = ctx->src_pts.as<float4>();
+  B.covA = ctx->src_covA.as<float4>();
+  B.covB = ctx->src_covB.as<float4>();
+  B.centres = ctx->b_centres.as<double>();
+  B.poses = ctx->b_poses.as<double>();
+  B.lin_poses = ctx->b_lin_poses.as<double>();
+  B.tiles = ctx->b_tiles.as<BatchTile>();
+  B.members = ctx->b_members.as<uint4>();
+  B.corr = ctx->b_corr.as<uint32_t>();
+  B.tile_partials = ctx->b_partials.as<double>();
+  return B;
+}
+
+int copy_out(sgb_ctx* ctx, double* out, size_t doubles) {
+  CU(cudaMemcpyAsync(out, ctx->b_out.p, doubles * sizeof(double), cudaMemcpyDefault, ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));
+  return 0;
+}
+
+}  // namespace
+
+extern "C" {
+
+int sgb_source_set_batch(sgb_ctx* ctx, size_t n_members, const size_t* offsets, const double* points, const double* covs) {
+  if (!ctx) return 1;
+  if (n_members > SGB_BATCH_MAX_MEMBERS)
+    return fail(ctx, 1, "sgb_source_set_batch: " + std::to_string(n_members) + " members, at most " + std::to_string(SGB_BATCH_MAX_MEMBERS));
+  if (!offsets) return fail(ctx, 1, "sgb_source_set_batch: null offsets");
+  if (offsets[0] != 0) return fail(ctx, 1, "sgb_source_set_batch: offsets[0] must be 0");
+  size_t largest = 0;
+  for (size_t m = 0; m < n_members; m++) {
+    if (offsets[m + 1] < offsets[m]) return fail(ctx, 1, "sgb_source_set_batch: offsets must be ascending (member " + std::to_string(m) + ")");
+    largest = std::max(largest, offsets[m + 1] - offsets[m]);
+  }
+  const size_t n = offsets[n_members];
+  if (n >= (1ull << 31)) return fail(ctx, 1, "sgb_source_set_batch: too many points");
+  if (n && !points) return fail(ctx, 1, "sgb_source_set_batch: null points");
+  CU(cudaSetDevice(ctx->device));
+  // from here on the context holds this batch (and no single source)
+  ctx->src_is_batch = true;
+  ctx->n_src = 0;
+  ctx->src_has_covs = covs != nullptr;
+  ctx->have_lin = false;
+  ctx->corr_seeds = false;
+  ctx->src_orig_valid = ctx->src_tree_valid = ctx->src_cov_orig_valid = ctx->src_has_lo = false;
+  ctx->b_offsets.assign(offsets, offsets + n_members + 1);
+  ctx->b_lin.assign(n_members, 0);
+  ctx->b_seeded.assign(n_members, 0);
+  const size_t B = std::max<size_t>(n_members, 1), nn = std::max<size_t>(n, 1);
+  CU(ctx->b_centres.reserve(B * 4 * sizeof(double)));
+  CU(ctx->b_bounds.reserve(B * 6 * sizeof(double)));
+  CU(ctx->b_poses.reserve(B * 12 * sizeof(double)));
+  CU(ctx->b_lin_poses.reserve(B * 12 * sizeof(double)));
+  CU(ctx->b_members.reserve(B * sizeof(uint4)));
+  CU(ctx->b_tiles.reserve(max_tiles(ctx) * sizeof(BatchTile)));
+  CU(ctx->b_partials.reserve(max_tiles(ctx) * kPartialStride * sizeof(double)));
+  CU(ctx->b_out.reserve(B * 44 * sizeof(double)));
+  CU(ctx->b_corr.reserve(nn * sizeof(uint32_t)));
+  CU(ctx->b_vq.reserve(nn * sizeof(float4)));
+  CU(ctx->b_vcorr.reserve(nn * sizeof(uint32_t)));
+  CU(cudaMemsetAsync(ctx->b_corr.p, 0xFF, nn * sizeof(uint32_t), ctx->stream));  // no correspondences before the first linearize
+  // per-query scratch of the search, sized here so that the batch calls never (re)allocate (as sgb_source_set_points does)
+  CU(ctx->grid_state.reserve(nn));
+  {
+    const void* before = ctx->grid_pending.p;
+    CU(ctx->grid_pending.reserve((nn + 2) * sizeof(uint32_t)));
+    if (ctx->grid_pending.p != before) ctx->pending_clean = false;
+    CU(ctx->grid_pending_q.reserve(nn * sizeof(float4)));
+  }
+  {
+    const void* before = ctx->chunk_lists.p;
+    CU(ctx->chunk_lists.reserve((8 + static_cast<size_t>(kChunkClasses) * ((nn + 31) / 32)) * sizeof(uint32_t)));
+    if (ctx->chunk_lists.p != before) ctx->chunk_lists_clean = false;
+  }
+  if (n == 0) return 0;
+  CU(ctx->stage_pts.reserve(n * 4 * sizeof(double)));
+  CU(ctx->tmp_pts.reserve(n * sizeof(float4)));
+  CU(ctx->src_pts.reserve(n * sizeof(float4)));
+  CU(ctx->keys_in.reserve(n * sizeof(uint64_t)));
+  CU(ctx->keys_out.reserve(n * sizeof(uint64_t)));
+  CU(ctx->vals_in.reserve(n * sizeof(uint32_t)));
+  CU(ctx->src_perm.reserve(n * sizeof(uint32_t)));
+  CU(ctx->src_rank.reserve(n * sizeof(uint32_t)));
+  CU(cudaMemcpyAsync(ctx->stage_pts.p, points, n * 4 * sizeof(double), cudaMemcpyDefault, ctx->stream));
+  if (covs) {
+    CU(ctx->stage_covs.reserve(n * 16 * sizeof(double)));
+    CU(ctx->src_covA.reserve(n * sizeof(float4)));
+    CU(ctx->src_covB.reserve(n * sizeof(float4)));
+    CU(cudaMemcpyAsync(ctx->stage_covs.p, covs, n * 16 * sizeof(double), cudaMemcpyDefault, ctx->stream));
+  }
+  size_t temp_bytes = 0;
+  CU(sort_pairs_u64_u32(nullptr, temp_bytes, ctx->keys_in.as<uint64_t>(), ctx->keys_out.as<uint64_t>(), ctx->vals_in.as<uint32_t>(),
+                        ctx->src_perm.as<uint32_t>(), largest, ctx->stream));
+  CU(ctx->sort_temp.reserve(temp_bytes));
+  // Every member is stored exactly as sgb_source_set_points stores one cloud: centred on its own box, rounded to FP32, sorted along the
+  // curve within itself, covariances packed into its search order.  Its slice of the storage is contiguous.
+  for (size_t m = 0; m < n_members; m++) {
+    const size_t off = offsets[m], nm = offsets[m + 1] - offsets[m];
+    if (nm == 0) continue;
+    double* centre = ctx->b_centres.as<double>() + 4 * m;
+    CU(launch_bounds_centre(ctx->stage_pts.as<double>() + 4 * off, nm, ctx->b_bounds.as<double>() + 6 * m, centre, ctx->sm_count, ctx->stream));
+    CU(launch_convert(ctx->stage_pts.as<double>() + 4 * off, nullptr, nullptr, nm, centre, ctx->tmp_pts.as<float4>() + off, nullptr, nullptr, nullptr,
+                      ctx->keys_in.as<uint64_t>() + off, ctx->vals_in.as<uint32_t>() + off, ctx->sm_count, ctx->stream));
+    CU(sort_pairs_u64_u32(ctx->sort_temp.p, temp_bytes, ctx->keys_in.as<uint64_t>() + off, ctx->keys_out.as<uint64_t>() + off,
+                          ctx->vals_in.as<uint32_t>() + off, ctx->src_perm.as<uint32_t>() + off, nm, ctx->stream));
+    CU(launch_gather(ctx->src_perm.as<uint32_t>() + off, nm, ctx->tmp_pts.as<float4>() + off, ctx->src_pts.as<float4>() + off, nullptr, nullptr, nullptr,
+                     nullptr, nullptr, nullptr, ctx->sm_count, ctx->stream));
+    ctx->launches += 5;
+    if (covs) {
+      CU(launch_inverse_perm(ctx->src_perm.as<uint32_t>() + off, nm, ctx->src_rank.as<uint32_t>() + off, ctx->sm_count, ctx->stream));
+      CU(launch_convert_cov_scatter(ctx->stage_covs.as<double>() + 16 * off, 0, nm, ctx->src_rank.as<uint32_t>() + off, ctx->src_covA.as<float4>() + off,
+                                    ctx->src_covB.as<float4>() + off, nullptr, nullptr, ctx->sm_count, ctx->stream));
+      ctx->launches += 2;
+    }
+  }
+  return 0;
+}
+
+int sgb_linearize_batch(sgb_ctx* ctx, int factor, int robust, double robust_c, int rejector, double max_dist_sq, const double* T, const uint8_t* active,
+                        double* out44) {
+  if (!ctx) return 1;
+  if (int rc = batch_check(ctx, "sgb_linearize_batch", T)) return rc;
+  if (factor < 0 || factor > 2 || robust < 0 || robust > 2 || rejector < 0 || rejector > 1) return fail(ctx, 1, "sgb_linearize_batch: invalid factor/robust/rejector kind");
+  if (!out44) return fail(ctx, 1, "sgb_linearize_batch: null output");
+  const size_t B = batch_members(ctx);
+  if (B == 0) return 0;
+  if (batch_points(ctx) && ctx->n_tgt) {
+    if (!ctx->tgt_ready) return fail(ctx, 1, "sgb_linearize_batch: target has no search structure (call sgb_target_set_kdtree / _build_kdtree / _set_voxelmap)");
+    if (factor == SGB_FACTOR_PLANE_ICP && (!ctx->tgt_has_normals || ctx->tgt_is_voxel)) return fail(ctx, 1, "sgb_linearize_batch: point-to-plane needs target normals");
+    if (factor == SGB_FACTOR_GICP && (!ctx->tgt_has_covs || !ctx->src_has_covs)) return fail(ctx, 1, "sgb_linearize_batch: GICP needs target and source covariances");
+  }
+  CU(cudaSetDevice(ctx->device));
+  // a new target (or none linearised yet) invalidates every member's cached state; sgb_drop_seeds only the seeds
+  if (!ctx->have_lin) std::fill(ctx->b_lin.begin(), ctx->b_lin.end(), 0);
+  if (!ctx->corr_seeds) std::fill(ctx->b_seeded.begin(), ctx->b_seeded.end(), 0);
+  uint32_t n_tiles = 0, n_virtual = 0;
+  if (int rc = batch_tables(ctx, T, active, !ctx->tgt_is_voxel, &n_tiles, &n_virtual)) return rc;
+  LinParams P;
+  fill_params(ctx, P, kIdentity);
+  BatchParams Bp = batch_params(ctx, P);
+  Bp.max_dist_sq_d = rejector == SGB_REJECT_DISTANCE ? max_dist_sq : DBL_MAX;
+  Bp.robust_c = robust_c;
+  if (ctx->n_tgt == 0) {  // nothing to match: every active member's points are unmatched, its sums zero
+    n_tiles = 0;
+    for (size_t m = 0; m < B; m++) {
+      const size_t nm = ctx->b_offsets[m + 1] - ctx->b_offsets[m];
+      if ((!active || active[m]) && nm) CU(cudaMemsetAsync(ctx->b_corr.as<uint32_t>() + ctx->b_offsets[m], 0xFF, nm * sizeof(uint32_t), ctx->stream));
+    }
+    std::vector<uint4> none(B, make_uint4(0, 0, 0, 0));
+    for (size_t m = 0; m < B; m++) none[m].z = (!active || active[m]) ? kMemberActive : 0u;
+    CU(cudaMemcpyAsync(ctx->b_members.p, none.data(), B * sizeof(uint4), cudaMemcpyHostToDevice, ctx->stream));
+  }
+  if (n_tiles && !ctx->tgt_is_voxel) {
+    // the search runs over the virtual source: the active members' queries, already transformed into the target's frame
+    CU(launch_batch_transform(Bp, n_tiles, ctx->b_vq.as<float4>(), ctx->b_vcorr.as<uint32_t>(), ctx->stream));
+    ctx->launches += 1;
+    P.src.pts = ctx->b_vq.as<float4>();
+    P.src.covA = P.src.covB = nullptr;
+    P.src.centre = ctx->tgt_centre.as<double>();  // identity pose, source centre = target centre: the search takes the stored query as is
+    P.src.n = n_virtual;
+    P.src.run = 1;
+    P.corr = ctx->b_vcorr.as<uint32_t>();
+    P.use_prev = 1;  // per member: its previous correspondences, or kNone
+    float bound = FLT_MAX;
+    if (rejector == SGB_REJECT_DISTANCE) {  // the single-source path's FP32 search bound
+      bound = nextafterf(static_cast<float>(max_dist_sq * (1.0 + 4e-6) + 1e-12), INFINITY);
+      if (!(bound < FLT_MAX)) bound = FLT_MAX;
+    }
+    P.max_dist_sq = bound;
+    if (int rc = launch_point_search(ctx, P, ctx->tree_depth > 0 ? ctx->tree_depth : 1)) return rc;
+    ctx->launches += 1;
+  }
+  if (n_tiles) {
+    CU(launch_batch_factor(Bp, factor, robust, n_tiles, ctx->tgt_is_voxel, false, ctx->b_vcorr.as<uint32_t>(), ctx->stream));
+    ctx->launches += 1;
+  }
+  CU(launch_batch_segment(Bp, static_cast<uint32_t>(B), true, ctx->b_out.as<double>(), ctx->stream));
+  ctx->launches += 1;
+  for (size_t m = 0; m < B; m++) {
+    if (active && !active[m]) continue;
+    ctx->b_lin[m] = 1;
+    ctx->b_seeded[m] = 1;
+  }
+  ctx->have_lin = true;
+  ctx->corr_seeds = true;
+  ctx->lin_factor = factor;
+  ctx->lin_robust = robust;
+  ctx->lin_c = robust_c;
+  return copy_out(ctx, out44, 44 * B);
+}
+
+int sgb_error_batch(sgb_ctx* ctx, const double* T, const uint8_t* active, double* out_e) {
+  if (!ctx) return 1;
+  if (int rc = batch_check(ctx, "sgb_error_batch", T)) return rc;
+  if (!out_e) return fail(ctx, 1, "sgb_error_batch: null output");
+  const size_t B = batch_members(ctx);
+  if (B == 0) return 0;
+  if (!ctx->have_lin) return fail(ctx, 1, "sgb_error_batch: no preceding sgb_linearize_batch (the correspondences are cached there)");
+  for (size_t m = 0; m < B; m++)
+    if ((!active || active[m]) && !ctx->b_lin[m])
+      return fail(ctx, 1, "sgb_error_batch: member " + std::to_string(m) + " is active but has not been linearised against the current target");
+  CU(cudaSetDevice(ctx->device));
+  uint32_t n_tiles = 0, n_virtual = 0;
+  if (int rc = batch_tables(ctx, T, active, false, &n_tiles, &n_virtual)) return rc;
+  LinParams P;
+  fill_params(ctx, P, kIdentity);
+  BatchParams Bp = batch_params(ctx, P);
+  Bp.robust_c = ctx->lin_c;
+  if (n_tiles && ctx->n_tgt) {
+    CU(launch_batch_factor(Bp, ctx->lin_factor, ctx->lin_robust, n_tiles, ctx->tgt_is_voxel, true, nullptr, ctx->stream));
+    ctx->launches += 1;
+  } else {
+    n_tiles = 0;
+    std::vector<uint4> none(B, make_uint4(0, 0, 0, 0));
+    CU(cudaMemcpyAsync(ctx->b_members.p, none.data(), B * sizeof(uint4), cudaMemcpyHostToDevice, ctx->stream));
+  }
+  CU(launch_batch_segment(Bp, static_cast<uint32_t>(B), false, ctx->b_out.as<double>(), ctx->stream));
+  ctx->launches += 1;
+  return copy_out(ctx, out_e, B);
+}
+
+int sgb_correspondences_batch(sgb_ctx* ctx, uint64_t* out) {
+  if (!ctx) return 1;
+  if (int rc = batch_check(ctx, "sgb_correspondences_batch", kIdentity)) return rc;
+  const size_t n = batch_points(ctx);
+  if (n == 0) return 0;
+  if (!out) return fail(ctx, 1, "sgb_correspondences_batch: null output");
+  CU(cudaSetDevice(ctx->device));
+  CU(ctx->corr64.reserve(n * sizeof(uint64_t)));
+  for (size_t m = 0; m + 1 < ctx->b_offsets.size(); m++) {
+    const size_t off = ctx->b_offsets[m], nm = ctx->b_offsets[m + 1] - off;
+    if (nm == 0) continue;
+    // not linearised against the current target (never, or before the target changed: have_lin is cleared with it): no correspondences
+    if (!ctx->have_lin || !ctx->b_lin[m]) {
+      CU(cudaMemsetAsync(ctx->corr64.as<uint64_t>() + off, 0xFF, nm * sizeof(uint64_t), ctx->stream));
+      continue;
+    }
+    CU(launch_correspondences(ctx->b_corr.as<uint32_t>() + off, ctx->src_perm.as<uint32_t>() + off, nm, ctx->tgt_pts.as<float4>(), ctx->tgt_is_voxel ? 1 : 0,
+                              ctx->corr64.as<uint64_t>() + off, ctx->sm_count, ctx->stream));
+    ctx->launches += 1;
+  }
+  CU(cudaMemcpyAsync(out, ctx->corr64.p, n * sizeof(uint64_t), cudaMemcpyDefault, ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));
+  return 0;
+}
+
+}  // extern "C"

@@ -218,6 +218,7 @@ int sgb_target_estimate_features(sgb_ctx* ctx, int num_neighbors) {
 int sgb_source_estimate_features(sgb_ctx* ctx, int num_neighbors) {
   if (!ctx) return 1;
   if (num_neighbors < 1 || num_neighbors > 32) return fail(ctx, 1, "sgb_source_estimate_features: num_neighbors must be in 1..32");
+  if (ctx->src_is_batch) return fail(ctx, 1, "sgb_source_estimate_features: the context holds a batch of sources; pass each member's covariances to sgb_source_set_batch");
   const size_t n = ctx->n_src;
   ctx->src_has_covs = true;
   ctx->have_lin = false;

@@ -5,6 +5,7 @@
 #include <stdint.h>
 
 #include <string>
+#include <vector>
 
 namespace sgb {
 
@@ -149,6 +150,17 @@ struct sgb_ctx {
   double Tlin[12] = {1, 0, 0, 0, 1, 0, 0, 0, 1, 0, 0, 0};
   const double* last_out = nullptr;  // device pointer holding H|b|e|inliers of the last linearize
   int lin_grid = 0;
+
+  // ---- batch of sources (sgb_source_set_batch, sgb_capi_batch.cu): members concatenated in src_pts / src_covA / src_covB / src_perm ----
+  bool src_is_batch = false;
+  std::vector<size_t> b_offsets;           // members + 1
+  std::vector<uint8_t> b_lin, b_seeded;    // per member: linearised against the current target / correspondences usable as search seeds
+  sgb::DevBuf b_centres, b_bounds;         // [members][4] / [members][6]
+  sgb::DevBuf b_poses, b_lin_poses;        // [members][12]: this call's poses / each member's last linearisation pose
+  sgb::DevBuf b_tiles, b_members;          // BatchTile / uint4 tables of the current call
+  sgb::DevBuf b_corr;                      // per stored point: cached correspondence
+  sgb::DevBuf b_vq, b_vcorr;               // virtual source of the search: transformed queries of the active members and what the search found
+  sgb::DevBuf b_partials, b_out;           // per-tile partial sums, per-member results
 };
 
 namespace sgb {
@@ -162,6 +174,12 @@ inline int fail(sgb_ctx* c, int code, const std::string& msg) {
 int build_lbvh(sgb_ctx* ctx, const float4* d_orig_pts, size_t n, const double* d_centre4, DevBuf& perm, DevBuf& leaf_pts, DevBuf& pnodes, int* depth);
 /// uniform grid over the current (leaf-ordered) target for the search front end; no-op unless enabled
 int build_grid(sgb_ctx* ctx);
+
+struct LinParams;
+/// kernel parameters of the current target and source at pose T (sgb_capi.cu)
+int fill_params(sgb_ctx* ctx, LinParams& P, const double* T_colmajor16);
+/// nearest-neighbour search of the P.src.n queries of P.src in a point target: grid probe, then the packet search (sgb_capi.cu)
+int launch_point_search(sgb_ctx* ctx, const LinParams& P, int depth);
 
 }  // namespace sgb
 

@@ -4,6 +4,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <cfloat>
+
 #include "sgb_math.cuh"
 
 namespace sgb {
@@ -92,6 +94,60 @@ __device__ __forceinline__ uint32_t vox_hash(int x, int y, int z) {
   h *= 0x2c1b3c6du;
   h ^= h >> 12;
   return h;
+}
+
+// Gaussian-voxel-map target (VGICP): hash probe of 1 / 7 / 27 voxels in the reference's offset order
+// (incremental_voxelmap.hpp:157-186), nearest voxel mean wins, first-found wins ties (knn_result.hpp:81-83).
+__device__ __forceinline__ void vox_offset(int num, int o, int& dx, int& dy, int& dz) {
+  if (num == 27) {  // for i, j, k in -1..1 (lexicographic)
+    dx = o / 9 - 1;
+    dy = (o / 3) % 3 - 1;
+    dz = o % 3 - 1;
+  } else {  // 1 or 7: centre, +x, +y, +z, -x, -y, -z
+    const int s = o == 0 ? 0 : (o <= 3 ? 1 : -1);
+    const int a = o == 0 ? -1 : (o - 1) % 3;
+    dx = a == 0 ? s : 0;
+    dy = a == 1 ? s : 0;
+    dz = a == 2 ? s : 0;
+  }
+}
+
+/// Nearest voxel mean of the (target-centred, FP64) query q, or kNone; DistanceRejector applied (d2 > max_d rejects).
+/// (brx, bry, brz) = mean - q of the winner.  A copy of linearize_vox_kernel's probe loop (sgb_kernels.cu): keep the two equal.
+__device__ __forceinline__ uint32_t vox_nearest(const DevTarget& tgt, double qx, double qy, double qz, double ctx, double cty, double ctz, double max_d,
+                                                double& brx, double& bry, double& brz) {
+  // voxel coordinate of the un-centred point, fast_floor semantics == floor (util/fast_floor.hpp:12-15)
+  const int cx = static_cast<int>(floor((qx + ctx) * tgt.vox_inv_leaf));
+  const int cy = static_cast<int>(floor((qy + cty) * tgt.vox_inv_leaf));
+  const int cz = static_cast<int>(floor((qz + ctz) * tgt.vox_inv_leaf));
+  double best_d = DBL_MAX;
+  uint32_t best = kNone;
+  for (int o = 0; o < tgt.vox_num_offsets; o++) {
+    int ox, oy, oz;
+    vox_offset(tgt.vox_num_offsets, o, ox, oy, oz);
+    const int vx = cx + ox, vy = cy + oy, vz = cz + oz;
+    uint32_t slot = vox_hash(vx, vy, vz) & tgt.vox_mask;
+    for (;;) {
+      const int4 e = __ldg(&tgt.vox_table[slot]);
+      if (e.w < 0) break;
+      if (e.x == vx && e.y == vy && e.z == vz) {
+        const float4 m = __ldg(&tgt.pts[e.w]);
+        const double dx = static_cast<double>(m.x) - qx, dy = static_cast<double>(m.y) - qy, dz = static_cast<double>(m.z) - qz;
+        const double d = dx * dx + dy * dy + dz * dz;
+        if (d < best_d) {
+          best_d = d;
+          best = static_cast<uint32_t>(e.w);
+          brx = dx;
+          bry = dy;
+          brz = dz;
+        }
+        break;
+      }
+      slot = (slot + 1u) & tgt.vox_mask;
+    }
+  }
+  if (best != kNone && best_d > max_d) best = kNone;  // DistanceRejector, rejector.hpp:23-25
+  return best;
 }
 
 // Sym3, the factor algebra and the per-point helpers live in sgb_math.cuh (also compiled for the host by tests/host_math).
@@ -221,6 +277,7 @@ __host__ __device__ inline size_t reduction_tickets(size_t grid) { return 1 + (g
 /// independent L2 loads per lane -- a single CTA adding all gridDim.x partials keeps an otherwise idle GPU waiting.  The order of the additions depends on gridDim.x only: deterministic.
 /// partials: reduction_partials_doubles(gridDim.x) doubles; ticket: reduction_tickets(gridDim.x) zeroed counters (left zeroed).
 /// comm.world > 1: the finishing CTA then exchanges the sums with the other ranks (comm_all_reduce) before writing `out`.
+/// tile_sum (sgb_batch.cu) is a copy of the CTA butterfly below: keep the two equal (sharing it changes this function's register allocation).
 template <int NACC, bool EXPAND>
 __device__ __forceinline__ void block_reduce_and_finish(double* acc, double* partials, unsigned int* ticket, double* out, const CommParams& comm) {
   static_assert(NACC <= 32, "one lane per accumulator");

@@ -103,22 +103,9 @@ __global__ void __launch_bounds__(kLinBlock) linearize_kd_kernel(const __grid_co
 
 #endif  // SGB_PROFILING
 
-// Gaussian-voxel-map target (VGICP): hash probe of 1 / 7 / 27 voxels in the reference's offset order
-// (incremental_voxelmap.hpp:157-186), nearest voxel mean wins, first-found wins ties (knn_result.hpp:81-83).
-__device__ __forceinline__ void vox_offset(int num, int o, int& dx, int& dy, int& dz) {
-  if (num == 27) {  // for i, j, k in -1..1 (lexicographic)
-    dx = o / 9 - 1;
-    dy = (o / 3) % 3 - 1;
-    dz = o % 3 - 1;
-  } else {  // 1 or 7: centre, +x, +y, +z, -x, -y, -z
-    const int s = o == 0 ? 0 : (o <= 3 ? 1 : -1);
-    const int a = o == 0 ? -1 : (o - 1) % 3;
-    dx = a == 0 ? s : 0;
-    dy = a == 1 ? s : 0;
-    dz = a == 2 ? s : 0;
-  }
-}
-
+// Gaussian-voxel-map target (VGICP): hash probe of 1 / 7 / 27 voxels (vox_offset, sgb_device.cuh), nearest voxel mean wins, first-found
+// wins ties (knn_result.hpp:81-83).  vox_nearest (sgb_device.cuh, used by the batch kernels) is a copy of the probe loop below: keep the two
+// equal (calling it from here changes this kernel's SASS).
 template <int FACTOR, int ROBUST>
 __global__ void __launch_bounds__(kLinBlock) linearize_vox_kernel(const __grid_constant__ LinParams P) {
   double acc[kAcc + 1];
