@@ -22,13 +22,6 @@ namespace {
 
 thread_local std::string g_create_error;
 
-inline void pose_from_colmajor(const double* T, double out12[12]) {
-  for (int i = 0; i < 3; i++) {
-    for (int j = 0; j < 3; j++) out12[i * 3 + j] = T[j * 4 + i];
-    out12[9 + i] = T[12 + i];
-  }
-}
-
 uint32_t host_vox_hash(int x, int y, int z) {  // must equal vox_hash() in sgb_device.cuh
   uint32_t h = static_cast<uint32_t>(x) * 73856093u ^ static_cast<uint32_t>(y) * 19349669u ^ static_cast<uint32_t>(z) * 83492791u;
   h ^= h >> 15;
@@ -44,7 +37,6 @@ int ensure_reduction_buffers(sgb_ctx* ctx, int grid) {
     CU(ctx->ticket.reserve(ticket_bytes));
     CU(cudaMemsetAsync(ctx->ticket.p, 0, ctx->ticket.cap, ctx->stream));
   }
-  CU(ctx->out44.reserve(64 * sizeof(double)));
   return 0;
 }
 
@@ -62,29 +54,34 @@ int upload_tree(sgb_ctx* ctx, const FlatTree& tree, const float* host_pts_xyzw) 
   CU(cudaMemcpyAsync(ctx->tgt_nodes.p, tree.nodes.data(), tree.nodes.size() * sizeof(FlatNode), cudaMemcpyHostToDevice, ctx->stream));
 #endif
   CU(cudaMemcpyAsync(ctx->tgt_perm.p, tree.perm.data(), tree.perm.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
-  const size_t n = ctx->n_tgt;
-  CU(ctx->tgt_pts.reserve(n * sizeof(float4)));
-  if (ctx->tgt_has_normals) CU(ctx->tgt_normals.reserve(n * sizeof(float4)));
-  if (ctx->tgt_has_covs) {
-    CU(ctx->tgt_covA.reserve(n * sizeof(float4)));
-    CU(ctx->tgt_covB.reserve(n * sizeof(float4)));
-  }
-  CU(launch_gather(ctx->tgt_perm.as<uint32_t>(), n, ctx->tgt_orig_pts.as<float4>(), ctx->tgt_pts.as<float4>(),
-                   ctx->tgt_has_normals ? ctx->tgt_orig_normals.as<float4>() : nullptr, ctx->tgt_normals.as<float4>(),
-                   ctx->tgt_has_covs ? ctx->tgt_orig_covA.as<float4>() : nullptr, ctx->tgt_covA.as<float4>(),
-                   ctx->tgt_has_covs ? ctx->tgt_orig_covB.as<float4>() : nullptr, ctx->tgt_covB.as<float4>(), ctx->sm_count, ctx->stream));
-  ctx->launches += 1;
+  if (int rc = gather_target_features(ctx, true)) return rc;
   // the host vectors go out of scope when the caller returns: make sure the async copies are done
   CU(cudaStreamSynchronize(ctx->stream));
-  ctx->tree_depth = tree.depth;
-  ctx->tgt_has_kd = true;
-  ctx->tgt_is_voxel = false;
-  ctx->tgt_ready = true;
-  ctx->tgt_feats_leaf_only = false;
+  return install_tree(ctx, tree.depth, pnodes.size());
+}
+
+// the answer of linearize / error() over an empty cloud (helper_test.cpp:53-59: empty clouds must not crash): a sum over nothing
+int zero_result(sgb_ctx* ctx, const double* T, double* d_out, bool linearize) {
+  const size_t at = linearize ? 0 : 48, doubles = linearize ? 44 : 1;  // slots of the mapped host result (sgb_linearize / sgb_error)
+  if (ctx->comm_world > 1) {  // an empty shard still takes part in the exchange: contribute zeros
+    if (int rc = ensure_reduction_buffers(ctx, 1)) return rc;
+    LinParams P0;
+    fill_params(ctx, P0, T);
+    P0.out = d_out;
+    CU(launch_reduce_nothing(P0, linearize, ctx->stream));
+    ctx->launches += 1;
+  } else if (d_out == ctx->h_out_dev + at) {  // the mapped host slot: clear it from the host side, in stream order
+    CU(cudaStreamSynchronize(ctx->stream));
+    std::memset(ctx->h_out + at, 0, doubles * sizeof(double));
+  } else {
+    CU(cudaMemsetAsync(d_out, 0, doubles * sizeof(double), ctx->stream));
+  }
+  return 0;
+}
+
+void forget_linearisation(sgb_ctx* ctx) {
   ctx->have_lin = false;
   ctx->corr_seeds = false;
-  ctx->n_pnodes = pnodes.size();
-  return build_grid(ctx);
 }
 
 }  // namespace
@@ -123,6 +120,153 @@ int sgb::fill_params(sgb_ctx* ctx, LinParams& P, const double* T_colmajor16) {
   return 0;
 }
 
+void sgb::pose_from_colmajor(const double* T, double out12[12]) {
+  for (int i = 0; i < 3; i++) {
+    for (int j = 0; j < 3; j++) out12[i * 3 + j] = T[j * 4 + i];
+    out12[9 + i] = T[12 + i];
+  }
+}
+
+// ---- transitions ----
+int sgb::begin_point_target(sgb_ctx* ctx, size_t n, bool normals, bool covs, bool lo) {
+  ctx->tgt_state = TargetState::Points;
+  ctx->n_tgt = n;
+  ctx->tgt_has_normals = normals;
+  ctx->tgt_has_covs = covs;
+  ctx->tgt_has_lo = lo;
+  ctx->grid_ready = false;
+  forget_linearisation(ctx);
+  CU(ctx->tgt_centre.reserve(4 * sizeof(double)));
+  CU(ctx->tgt_bounds.reserve(6 * sizeof(double)));
+  return 0;
+}
+
+int sgb::begin_voxel_target(sgb_ctx* ctx, size_t n, bool covs, double leaf_size, int search_offsets) {
+  ctx->tgt_state = TargetState::VoxelMap;
+  ctx->n_tgt = n;
+  ctx->tgt_has_normals = false;
+  ctx->tgt_has_covs = covs;
+  ctx->grid_ready = false;
+  forget_linearisation(ctx);
+  ctx->vox_offsets = search_offsets;
+  ctx->vox_inv_leaf = 1.0 / leaf_size;
+  CU(ctx->tgt_centre.reserve(4 * sizeof(double)));
+  CU(ctx->tgt_bounds.reserve(6 * sizeof(double)));
+  return 0;
+}
+
+int sgb::install_tree(sgb_ctx* ctx, int depth, size_t n_pnodes) {
+  ctx->tgt_state = TargetState::Tree;
+  ctx->tree_depth = depth;
+  ctx->n_pnodes = n_pnodes;
+  forget_linearisation(ctx);
+  return build_grid(ctx);
+}
+
+void sgb::begin_source(sgb_ctx* ctx, SourceState state, size_t n, bool covs) {
+  ctx->src_state = state;
+  ctx->n_src = n;
+  ctx->src_has_covs = covs;
+  ctx->src_has_lo = ctx->src_tree_valid = ctx->src_cov_orig_valid = false;
+  forget_linearisation(ctx);
+}
+
+void sgb::features_changed(sgb_ctx* ctx, bool target) {
+  if (target)
+    ctx->tgt_has_normals = ctx->tgt_has_covs = true;
+  else
+    ctx->src_has_covs = true;
+  forget_linearisation(ctx);
+}
+
+// ---- steps shared by the entry points ----
+int sgb::gather_target_features(sgb_ctx* ctx, bool points) {
+  const size_t n = ctx->n_tgt;
+  if (points) CU(ctx->tgt_pts.reserve(n * sizeof(float4)));
+  if (ctx->tgt_has_normals) CU(ctx->tgt_normals.reserve(n * sizeof(float4)));
+  if (ctx->tgt_has_covs) {
+    CU(ctx->tgt_covA.reserve(n * sizeof(float4)));
+    CU(ctx->tgt_covB.reserve(n * sizeof(float4)));
+  }
+  if (!points && !ctx->tgt_has_normals && !ctx->tgt_has_covs) return 0;
+  CU(launch_gather(ctx->tgt_perm.as<uint32_t>(), n, points ? ctx->tgt_orig_pts.as<float4>() : nullptr, ctx->tgt_pts.as<float4>(),
+                   ctx->tgt_has_normals ? ctx->tgt_orig_normals.as<float4>() : nullptr, ctx->tgt_normals.as<float4>(),
+                   ctx->tgt_has_covs ? ctx->tgt_orig_covA.as<float4>() : nullptr, ctx->tgt_covA.as<float4>(),
+                   ctx->tgt_has_covs ? ctx->tgt_orig_covB.as<float4>() : nullptr, ctx->tgt_covB.as<float4>(), ctx->sm_count, ctx->stream));
+  ctx->launches += 1;
+  return 0;
+}
+
+int sgb::reserve_query_scratch(sgb_ctx* ctx, size_t n) {
+  CU(ctx->grid_state.reserve(n));
+  const void* before = ctx->grid_pending.p;
+  CU(ctx->grid_pending.reserve((n + 2) * sizeof(uint32_t)));
+  if (ctx->grid_pending.p != before) ctx->pending_clean = false;
+  CU(ctx->grid_pending_q.reserve(n * sizeof(float4)));
+  before = ctx->chunk_lists.p;
+  CU(ctx->chunk_lists.reserve((8 + static_cast<size_t>(kChunkClasses) * ((n + 31) / 32)) * sizeof(uint32_t)));
+  if (ctx->chunk_lists.p != before) ctx->chunk_lists_clean = false;
+  return 0;
+}
+
+// The n points at stage_pts[off..] become one source cloud: centred on its own box (centre / bounds), rounded to FP32 (tmp_pts[off..]:
+// original order, w = index; lo: the rounding residuals, or nullptr), Hilbert-sorted within itself (src_perm[off..]: search order ->
+// original index; sort_bytes of sort_temp suffice for n) and gathered into src_pts[off..].  With cov_chunks > 0 the covariances at
+// stage_covs[off..] are packed into the search order in cov_chunks pieces, piece k once arrived[k] has fired (arrived = nullptr: they are
+// already there).  run > 1 (profiling build only): the chunk-transposed order of the per-thread search.
+int sgb::store_source(sgb_ctx* ctx, size_t off, size_t n, double* centre, double* bounds, float4* lo, size_t sort_bytes, uint32_t run, int cov_chunks,
+                      const cudaEvent_t* arrived) {
+  const double* pts = ctx->stage_pts.as<double>() + 4 * off;
+  uint32_t* perm = ctx->src_perm.as<uint32_t>() + off;
+  CU(launch_bounds_centre(pts, n, bounds, centre, ctx->sm_count, ctx->stream));
+  CU(launch_convert(pts, nullptr, nullptr, n, centre, ctx->tmp_pts.as<float4>() + off, nullptr, nullptr, nullptr, ctx->keys_in.as<uint64_t>() + off,
+                    ctx->vals_in.as<uint32_t>() + off, ctx->sm_count, ctx->stream, lo));
+  // Hilbert order: consecutive lanes get spatially adjacent queries (coherent tree paths, coalesced gathers)
+  CU(sort_pairs_u64_u32(ctx->sort_temp.p, sort_bytes, ctx->keys_in.as<uint64_t>() + off, ctx->keys_out.as<uint64_t>() + off,
+                        ctx->vals_in.as<uint32_t>() + off, perm, n, ctx->stream));
+#ifdef SGB_PROFILING
+  // chunk-transposed order of the per-thread search (A/B): a lane walks K consecutive points of the curve, warp loads stay coalesced
+  if (run > 1) {
+    CU(launch_chunk_transpose(perm, ctx->vals_in.as<uint32_t>() + off, n, run, ctx->sm_count, ctx->stream));
+    CU(cudaMemcpyAsync(perm, ctx->vals_in.as<uint32_t>() + off, n * sizeof(uint32_t), cudaMemcpyDeviceToDevice, ctx->stream));
+    ctx->launches += 1;
+  }
+#else
+  (void)run;
+#endif
+  CU(launch_gather(perm, n, ctx->tmp_pts.as<float4>() + off, ctx->src_pts.as<float4>() + off, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr,
+                   ctx->sm_count, ctx->stream));
+  ctx->launches += 5;
+  if (cov_chunks == 0) return 0;
+  uint32_t* rank = ctx->src_rank.as<uint32_t>() + off;
+  CU(launch_inverse_perm(perm, n, rank, ctx->sm_count, ctx->stream));
+  ctx->launches += 1;
+  const size_t per_chunk = (n + cov_chunks - 1) / cov_chunks;
+  for (int k = 0; k < cov_chunks; k++) {
+    const size_t first = static_cast<size_t>(k) * per_chunk, cnt = std::min(per_chunk, n - first);
+    if (arrived) CU(cudaStreamWaitEvent(ctx->stream, arrived[k], 0));
+    CU(launch_convert_cov_scatter(ctx->stage_covs.as<double>() + 16 * off, first, cnt, rank, ctx->src_covA.as<float4>() + off, ctx->src_covB.as<float4>() + off,
+                                  nullptr, nullptr, ctx->sm_count, ctx->stream));
+    ctx->launches += 1;
+  }
+  return 0;
+}
+
+int sgb::check_target(sgb_ctx* ctx, const char* who, int factor) {
+  if (ctx->tgt_state != TargetState::Tree && ctx->tgt_state != TargetState::VoxelMap)
+    return fail(ctx, 1, std::string(who) + ": target has no search structure (call sgb_target_set_kdtree / _build_kdtree / _set_voxelmap)");
+  if (factor == SGB_FACTOR_PLANE_ICP && (!ctx->tgt_has_normals || ctx->tgt_state == TargetState::VoxelMap))
+    return fail(ctx, 1, std::string(who) + ": point-to-plane needs target normals");
+  if (factor == SGB_FACTOR_GICP && (!ctx->tgt_has_covs || !ctx->src_has_covs)) return fail(ctx, 1, std::string(who) + ": GICP needs target and source covariances");
+  return 0;
+}
+
+float sgb::search_bound(int rejector, double max_dist_sq) {
+  if (rejector != SGB_REJECT_DISTANCE) return FLT_MAX;
+  const float bound = nextafterf(static_cast<float>(max_dist_sq * (1.0 + 4e-6) + 1e-12), INFINITY);
+  return bound < FLT_MAX ? bound : FLT_MAX;
+}
+
 namespace {
 
 int do_linearize_impl(sgb_ctx* ctx, int factor, int robust, double robust_c, int rejector, double max_dist_sq, const double* T, double* d_out) {
@@ -130,20 +274,8 @@ int do_linearize_impl(sgb_ctx* ctx, int factor, int robust, double robust_c, int
   if (!T) return fail(ctx, 1, "sgb_linearize: null pose");
   CU(cudaSetDevice(ctx->device));
   ctx->last_out = d_out;
-  if (ctx->n_src == 0 || ctx->n_tgt == 0) {  // empty clouds must not crash (helper_test.cpp:53-59): sum over nothing
-    if (ctx->comm_world > 1) {  // an empty shard still takes part in the exchange: contribute zeros
-      if (int rc = ensure_reduction_buffers(ctx, 1)) return rc;
-      LinParams P0;
-      fill_params(ctx, P0, T);
-      P0.out = d_out;
-      CU(launch_reduce_nothing(P0, true, ctx->stream));
-      ctx->launches += 1;
-    } else if (d_out == ctx->h_out_dev) {  // the mapped host slot of sgb_linearize: clear it from the host side, in stream order
-      CU(cudaStreamSynchronize(ctx->stream));
-      std::memset(ctx->h_out, 0, 44 * sizeof(double));
-    } else {
-      CU(cudaMemsetAsync(d_out, 0, 44 * sizeof(double), ctx->stream));
-    }
+  if (ctx->n_src == 0 || ctx->n_tgt == 0) {
+    if (int rc = zero_result(ctx, T, d_out, true)) return rc;
     if (ctx->n_src) {
       CU(ctx->corr.reserve(ctx->n_src * sizeof(uint32_t)));
       CU(cudaMemsetAsync(ctx->corr.p, 0xFF, ctx->n_src * sizeof(uint32_t), ctx->stream));
@@ -155,11 +287,10 @@ int do_linearize_impl(sgb_ctx* ctx, int factor, int robust, double robust_c, int
     pose_from_colmajor(T, ctx->Tlin);
     return 0;
   }
-  if (!ctx->tgt_ready) return fail(ctx, 1, "sgb_linearize: target has no search structure (call sgb_target_set_kdtree / _build_kdtree / _set_voxelmap)");
-  if (factor == SGB_FACTOR_PLANE_ICP && (!ctx->tgt_has_normals || ctx->tgt_is_voxel)) return fail(ctx, 1, "sgb_linearize: point-to-plane needs target normals");
-  if (factor == SGB_FACTOR_GICP && (!ctx->tgt_has_covs || !ctx->src_has_covs)) return fail(ctx, 1, "sgb_linearize: GICP needs target and source covariances");
+  if (int rc = check_target(ctx, "sgb_linearize", factor)) return rc;
+  const bool voxel = ctx->tgt_state == TargetState::VoxelMap;
 
-  const int depth = ctx->tgt_is_voxel ? 0 : (ctx->tree_depth > 0 ? ctx->tree_depth : 1);
+  const int depth = voxel ? 0 : (ctx->tree_depth > 0 ? ctx->tree_depth : 1);
   const int occ = linearize_occupancy(depth);
   int grid = static_cast<int>((ctx->n_src + kLinBlock - 1) / kLinBlock);
   const int cap = ctx->sm_count * occ;
@@ -173,22 +304,16 @@ int do_linearize_impl(sgb_ctx* ctx, int factor, int robust, double robust_c, int
   fill_params(ctx, P, T);
   std::memcpy(P.Tlin, P.T, sizeof(P.T));
   // FP32 search bound a hair above the threshold; the rejector itself (d2 > max, rejector.hpp:24) is applied to the FP64 residual
-  float bound = FLT_MAX;
-  P.max_dist_sq_d = DBL_MAX;
-  if (rejector == SGB_REJECT_DISTANCE) {
-    bound = nextafterf(static_cast<float>(max_dist_sq * (1.0 + 4e-6) + 1e-12), INFINITY);
-    if (!(bound < FLT_MAX)) bound = FLT_MAX;
-    P.max_dist_sq_d = max_dist_sq;
-  }
-  P.max_dist_sq = bound;
-  P.use_prev = (ctx->corr_seeds && !ctx->tgt_is_voxel) ? 1 : 0;
+  P.max_dist_sq = search_bound(rejector, max_dist_sq);
+  P.max_dist_sq_d = rejector == SGB_REJECT_DISTANCE ? max_dist_sq : DBL_MAX;
+  P.use_prev = (ctx->corr_seeds && !voxel) ? 1 : 0;
   P.robust_c = robust_c;
   P.out = d_out;
 #ifdef SGB_PROFILING
-  const bool split_path = ctx->search_mode != 0 && !ctx->tgt_is_voxel;
+  const bool split_path = ctx->search_mode != 0 && !voxel;
   const bool packet_path = ctx->search_mode == 2 && ctx->src_run == 1;
 #else
-  const bool split_path = !ctx->tgt_is_voxel;
+  const bool split_path = !voxel;
   const bool packet_path = true;
 #endif
   if (split_path) {
@@ -215,7 +340,7 @@ int do_linearize_impl(sgb_ctx* ctx, int factor, int robust, double robust_c, int
     CU(launch_factor_reduce(P, factor, robust, fgrid, ctx->stream));
     ctx->launches += 2;
   } else {
-    CU(launch_linearize(P, factor, robust, ctx->tgt_is_voxel, grid, depth, ctx->stream));
+    CU(launch_linearize(P, factor, robust, voxel, grid, depth, ctx->stream));
     ctx->launches += 1;
   }
   ctx->have_lin = true;
@@ -223,7 +348,6 @@ int do_linearize_impl(sgb_ctx* ctx, int factor, int robust, double robust_c, int
   ctx->lin_factor = factor;
   ctx->lin_robust = robust;
   ctx->lin_c = robust_c;
-  ctx->lin_grid = grid;
   std::memcpy(ctx->Tlin, P.T, sizeof(P.T));
   return 0;
 }
@@ -258,7 +382,7 @@ int sgb::launch_point_search(sgb_ctx* ctx, const LinParams& P, int depth) {
     uint32_t* pbase = ctx->grid_pending.as<uint32_t>();
     uint32_t* pc = pbase + ctx->pending_parity;
     uint32_t* plist = pbase + 2;
-    if (ctx->grid_blocks && ctx->use_chunk_classes) {
+    if (ctx->use_chunk_classes) {
       // work lists of the packet search by cost class; counters alternate like the pending counters (sized in sgb_source_set_points)
       const uint32_t nck = static_cast<uint32_t>((n + 31) / 32);
       const void* cb = ctx->chunk_lists.p;
@@ -285,7 +409,7 @@ int sgb::launch_point_search(sgb_ctx* ctx, const LinParams& P, int depth) {
     pp.list = plist;
     pp.q = ctx->grid_pending_q.as<float4>();
     pp.grid_pts = ctx->grid_pts.as<float4>();
-    pp.table = (ctx->grid_blocks && ctx->use_ring) ? ctx->grid_table.as<GridSlot>() : nullptr;
+    pp.table = ctx->use_ring ? ctx->grid_table.as<GridSlot>() : nullptr;
     pp.capacity = ctx->grid_capacity;
     pp.g = g;
     ctx->launches += 1;
@@ -321,25 +445,10 @@ int do_error_impl(sgb_ctx* ctx, const double* T, double* d_out) {
   if (!T) return fail(ctx, 1, "sgb_error: null pose");
   if (!ctx->have_lin) return fail(ctx, 1, "sgb_error: no preceding sgb_linearize (the correspondences are cached there)");
   CU(cudaSetDevice(ctx->device));
-  if (ctx->n_src == 0 || ctx->n_tgt == 0) {
-    if (ctx->comm_world > 1) {
-      if (int rc = ensure_reduction_buffers(ctx, 1)) return rc;
-      LinParams P0;
-      fill_params(ctx, P0, T);
-      P0.out = d_out;
-      CU(launch_reduce_nothing(P0, false, ctx->stream));
-      ctx->launches += 1;
-    } else if (d_out == ctx->h_out_dev + 48) {
-      CU(cudaStreamSynchronize(ctx->stream));
-      ctx->h_out[48] = 0.0;
-    } else {
-      CU(cudaMemsetAsync(d_out, 0, sizeof(double), ctx->stream));
-    }
-    return 0;
-  }
+  if (ctx->n_src == 0 || ctx->n_tgt == 0) return zero_result(ctx, T, d_out, false);
   // point targets: the factor kernel's operand pipeline (one wave of CTAs looping over tiles); voxel-map targets and the profiling switch
   // SGB_ERROR_PIPE=0: the plain grid-stride kernel
-  const bool pipelined = !ctx->tgt_is_voxel && ctx->error_pipelined;
+  const bool pipelined = ctx->tgt_state != TargetState::VoxelMap && ctx->error_pipelined;
   int grid = static_cast<int>((ctx->n_src + kLinBlock - 1) / kLinBlock);
   const int cap = ctx->sm_count * (pipelined ? error_pipelined_occupancy(ctx->lin_factor, ctx->lin_robust) : 8);
   if (grid > cap) grid = cap;
@@ -380,7 +489,7 @@ int comm_poison(sgb_ctx* ctx, const double* T, double* d_out, bool linearize) {
 }
 
 int do_linearize(sgb_ctx* ctx, int factor, int robust, double robust_c, int rejector, double max_dist_sq, const double* T, double* d_out) {
-  if (ctx->src_is_batch) return fail(ctx, 1, "sgb_linearize: the context holds a batch of sources (sgb_source_set_batch); use sgb_linearize_batch");
+  if (ctx->src_state == SourceState::Batch) return fail(ctx, 1, "sgb_linearize: the context holds a batch of sources (sgb_source_set_batch); use sgb_linearize_batch");
   if (ctx->comm_failed) return fail(ctx, 5, "sgb_linearize: an earlier multi-GPU exchange of this context failed; call sgb_comm_connect again");
   const unsigned long long seq0 = ctx->comm_seq;
   const int rc = do_linearize_impl(ctx, factor, robust, robust_c, rejector, max_dist_sq, T, d_out);
@@ -389,7 +498,7 @@ int do_linearize(sgb_ctx* ctx, int factor, int robust, double robust_c, int reje
 }
 
 int do_error(sgb_ctx* ctx, const double* T, double* d_out) {
-  if (ctx->src_is_batch) return fail(ctx, 1, "sgb_error: the context holds a batch of sources (sgb_source_set_batch); use sgb_error_batch");
+  if (ctx->src_state == SourceState::Batch) return fail(ctx, 1, "sgb_error: the context holds a batch of sources (sgb_source_set_batch); use sgb_error_batch");
   if (ctx->comm_failed) return fail(ctx, 5, "sgb_error: an earlier multi-GPU exchange of this context failed; call sgb_comm_connect again");
   const unsigned long long seq0 = ctx->comm_seq;
   const int rc = do_error_impl(ctx, T, d_out);
@@ -660,16 +769,9 @@ int sgb_target_set_points(sgb_ctx* ctx, size_t n, const double* points, const do
   if (n && !points) return fail(ctx, 1, "sgb_target_set_points: null points");
   if (n >= (1ull << 31)) return fail(ctx, 1, "sgb_target_set_points: too many points");
   CU(cudaSetDevice(ctx->device));
-  ctx->n_tgt = n;
-  ctx->tgt_has_normals = normals != nullptr;
-  ctx->tgt_has_covs = covs != nullptr;
-  ctx->tgt_ready = false;
-  ctx->grid_ready = false;
-  ctx->tgt_is_voxel = false;
-  ctx->have_lin = false;
-  ctx->corr_seeds = false;
-  CU(ctx->tgt_centre.reserve(4 * sizeof(double)));
-  CU(ctx->tgt_bounds.reserve(6 * sizeof(double)));
+  // without normals or covariances, features may still be estimated on the device (sgb_target_estimate_features): keep the rounding residuals
+  const bool keep_lo = !normals || !covs;
+  if (int rc = begin_point_target(ctx, n, normals != nullptr, covs != nullptr, keep_lo)) return rc;
   if (n == 0) return 0;
   CU(ctx->stage_pts.reserve(n * 4 * sizeof(double)));
   CU(cudaMemcpyAsync(ctx->stage_pts.p, points, n * 4 * sizeof(double), cudaMemcpyDefault, ctx->stream));
@@ -685,16 +787,11 @@ int sgb_target_set_points(sgb_ctx* ctx, size_t n, const double* points, const do
     CU(ctx->tgt_orig_covB.reserve(n * sizeof(float4)));
   }
   CU(ctx->tgt_orig_pts.reserve(n * sizeof(float4)));
-  float4* lo = nullptr;
-  if (!normals || !covs) {  // features may still be estimated on the device (sgb_target_estimate_features): keep the rounding residuals
-    CU(ctx->tgt_orig_lo.reserve(n * sizeof(float4)));
-    lo = ctx->tgt_orig_lo.as<float4>();
-  }
-  ctx->tgt_has_lo = lo != nullptr;
+  if (keep_lo) CU(ctx->tgt_orig_lo.reserve(n * sizeof(float4)));
   CU(launch_bounds_centre(ctx->stage_pts.as<double>(), n, ctx->tgt_bounds.as<double>(), ctx->tgt_centre.as<double>(), ctx->sm_count, ctx->stream));
   CU(launch_convert(ctx->stage_pts.as<double>(), normals ? ctx->stage_normals.as<double>() : nullptr, covs ? ctx->stage_covs.as<double>() : nullptr, n,
                     ctx->tgt_centre.as<double>(), ctx->tgt_orig_pts.as<float4>(), ctx->tgt_orig_normals.as<float4>(), ctx->tgt_orig_covA.as<float4>(),
-                    ctx->tgt_orig_covB.as<float4>(), nullptr, nullptr, ctx->sm_count, ctx->stream, lo));
+                    ctx->tgt_orig_covB.as<float4>(), nullptr, nullptr, ctx->sm_count, ctx->stream, keep_lo ? ctx->tgt_orig_lo.as<float4>() : nullptr));
   ctx->launches += 4;
   // pageable host memory: the async copies above are staged synchronously, nothing else borrows the inputs
   return 0;
@@ -702,8 +799,9 @@ int sgb_target_set_points(sgb_ctx* ctx, size_t n, const double* points, const do
 
 int sgb_target_set_kdtree(sgb_ctx* ctx, const void* nodes24, size_t n_nodes, uint32_t root, const uint64_t* indices) {
   if (!ctx) return 1;
+  if (ctx->tgt_state == TargetState::VoxelMap) return fail(ctx, 1, "sgb_target_set_kdtree: the target is a voxel map; call sgb_target_set_points first");
   if (ctx->n_tgt == 0) {
-    ctx->tgt_ready = true;
+    ctx->tgt_state = TargetState::Tree;  // nothing to search
     return 0;
   }
   if (!nodes24 || !indices) return fail(ctx, 1, "sgb_target_set_kdtree: null tree");
@@ -722,8 +820,9 @@ int sgb_target_set_kdtree(sgb_ctx* ctx, const void* nodes24, size_t n_nodes, uin
 
 int sgb_target_build_kdtree(sgb_ctx* ctx, int max_leaf_size) {
   if (!ctx) return 1;
+  if (ctx->tgt_state == TargetState::VoxelMap) return fail(ctx, 1, "sgb_target_build_kdtree: the target is a voxel map; call sgb_target_set_points first");
   if (ctx->n_tgt == 0) {
-    ctx->tgt_ready = true;
+    ctx->tgt_state = TargetState::Tree;  // nothing to search
     return 0;
   }
   CU(cudaSetDevice(ctx->device));
@@ -739,26 +838,8 @@ int sgb_target_build_kdtree(sgb_ctx* ctx, int max_leaf_size) {
     int depth = 1;
     if (int rc = build_lbvh(ctx, ctx->tgt_orig_pts.as<float4>(), n, ctx->tgt_centre.as<double>(), ctx->tgt_perm, ctx->tgt_pts, ctx->tgt_pnodes, &depth)) return rc;
     if (depth > 40) return fail(ctx, 1, "sgb_target_build_kdtree: tree too deep");
-    if (ctx->tgt_has_normals) CU(ctx->tgt_normals.reserve(n * sizeof(float4)));
-    if (ctx->tgt_has_covs) {
-      CU(ctx->tgt_covA.reserve(n * sizeof(float4)));
-      CU(ctx->tgt_covB.reserve(n * sizeof(float4)));
-    }
-    if (ctx->tgt_has_normals || ctx->tgt_has_covs) {
-      CU(launch_gather(ctx->tgt_perm.as<uint32_t>(), n, nullptr, nullptr, ctx->tgt_has_normals ? ctx->tgt_orig_normals.as<float4>() : nullptr,
-                       ctx->tgt_normals.as<float4>(), ctx->tgt_has_covs ? ctx->tgt_orig_covA.as<float4>() : nullptr, ctx->tgt_covA.as<float4>(),
-                       ctx->tgt_has_covs ? ctx->tgt_orig_covB.as<float4>() : nullptr, ctx->tgt_covB.as<float4>(), ctx->sm_count, ctx->stream));
-      ctx->launches += 1;
-    }
-    ctx->tree_depth = depth;
-    ctx->tgt_has_kd = false;
-    ctx->tgt_is_voxel = false;
-    ctx->tgt_ready = true;
-    ctx->tgt_feats_leaf_only = false;
-    ctx->have_lin = false;
-    ctx->corr_seeds = false;
-    ctx->n_pnodes = (static_cast<size_t>(1) << (depth - 1)) - 1;  // P - 1 records of the implicit tree (depth = log2(P) + 1)
-    return build_grid(ctx);
+    if (int rc = gather_target_features(ctx, false)) return rc;
+    return install_tree(ctx, depth, (static_cast<size_t>(1) << (depth - 1)) - 1);  // P - 1 records of the implicit tree (depth = log2(P) + 1)
   }
 #ifndef SGB_PROFILING
   return fail(ctx, 1, "sgb_target_build_kdtree: unreachable");
@@ -780,18 +861,7 @@ int sgb_target_set_voxelmap(sgb_ctx* ctx, double leaf_size, size_t n_voxels, con
   if (n_voxels && (!coords || !means)) return fail(ctx, 1, "sgb_target_set_voxelmap: null input");
   if (n_voxels >= (1ull << 30)) return fail(ctx, 1, "sgb_target_set_voxelmap: too many voxels");
   CU(cudaSetDevice(ctx->device));
-  ctx->n_tgt = n_voxels;
-  ctx->tgt_has_normals = false;
-  ctx->tgt_has_covs = covs != nullptr;
-  ctx->tgt_is_voxel = true;
-  ctx->grid_ready = false;
-  ctx->tgt_ready = true;
-  ctx->have_lin = false;
-  ctx->corr_seeds = false;
-  ctx->vox_offsets = search_offsets;
-  ctx->vox_inv_leaf = 1.0 / leaf_size;
-  CU(ctx->tgt_centre.reserve(4 * sizeof(double)));
-  CU(ctx->tgt_bounds.reserve(6 * sizeof(double)));
+  if (int rc = begin_voxel_target(ctx, n_voxels, covs != nullptr, leaf_size, search_offsets)) return rc;
   if (n_voxels == 0) return 0;
   const size_t n = n_voxels;
   CU(ctx->stage_pts.reserve(n * 4 * sizeof(double)));
@@ -837,13 +907,7 @@ int sgb_source_set_points(sgb_ctx* ctx, size_t n, const double* points, const do
   if (n && !points) return fail(ctx, 1, "sgb_source_set_points: null points");
   if (n >= (1ull << 31)) return fail(ctx, 1, "sgb_source_set_points: too many points");
   CU(cudaSetDevice(ctx->device));
-  ctx->src_is_batch = false;
-  ctx->n_src = n;
-  ctx->src_has_covs = covs != nullptr;
-  ctx->have_lin = false;
-  ctx->corr_seeds = false;
-  ctx->src_orig_valid = n > 0;  // tmp_pts (filled below) holds this source in original order
-  ctx->src_tree_valid = ctx->src_cov_orig_valid = false;
+  begin_source(ctx, SourceState::Single, n, covs != nullptr);
   CU(ctx->src_centre.reserve(4 * sizeof(double)));
   CU(ctx->src_bounds.reserve(6 * sizeof(double)));
   if (n == 0) return 0;
@@ -855,22 +919,12 @@ int sgb_source_set_points(sgb_ctx* ctx, size_t n, const double* points, const do
   }
   CU(ctx->tmp_pts.reserve(n * sizeof(float4)));
   CU(ctx->src_pts.reserve(n * sizeof(float4)));
-  // per-query scratch of linearize, sized here so that linearize itself never (re)allocates -- a cudaFree there would
-  // synchronise the device in the middle of an asynchronous call
   CU(ctx->corr.reserve(n * sizeof(uint32_t)));
-  CU(ctx->grid_state.reserve(n));
-  {
-    const void* before = ctx->grid_pending.p;
-    CU(ctx->grid_pending.reserve((n + 2) * sizeof(uint32_t)));
-    if (ctx->grid_pending.p != before) ctx->pending_clean = false;
-    CU(ctx->grid_pending_q.reserve(n * sizeof(float4)));
-  }
+  if (int rc = reserve_query_scratch(ctx, n)) return rc;
   if (int rc = ensure_reduction_buffers(ctx, ctx->sm_count * 8)) return rc;
-  {
-    const void* before = ctx->chunk_lists.p;
-    CU(ctx->chunk_lists.reserve((8 + static_cast<size_t>(kChunkClasses) * ((n + 31) / 32)) * sizeof(uint32_t)));
-    if (ctx->chunk_lists.p != before) ctx->chunk_lists_clean = false;
-  }
+  // without covariances, they may still be estimated on the device (sgb_source_estimate_features): keep the rounding residuals
+  if (!covs) CU(ctx->tmp_lo.reserve(n * sizeof(float4)));
+  ctx->src_has_lo = !covs;
   CU(ctx->keys_in.reserve(n * sizeof(uint64_t)));
   CU(ctx->keys_out.reserve(n * sizeof(uint64_t)));
   CU(ctx->vals_in.reserve(n * sizeof(uint32_t)));
@@ -890,7 +944,7 @@ int sgb_source_set_points(sgb_ctx* ctx, size_t n, const double* points, const do
   CU(cudaStreamWaitEvent(ctx->copy_stream, ctx->ev_entry, 0));  // ... precedes the first chunk
   CU(cudaMemcpyAsync(ctx->stage_pts.p, points, n * 4 * sizeof(double), cudaMemcpyDefault, ctx->stream));
   const int n_chunks = covs ? static_cast<int>(std::min<size_t>(sgb_ctx::kUploadChunks, (n + 65535) / 65536)) : 0;
-  const size_t per_chunk = n_chunks ? (n + n_chunks - 1) / n_chunks : 0;
+  const size_t per_chunk = n_chunks ? (n + n_chunks - 1) / n_chunks : 0;  // as store_source cuts them
   if (covs) {
     // the chunks queue up behind the points on the same DMA engine: wait for the points' copy to have been ISSUED first
     CU(cudaEventRecord(ctx->ev_entry, ctx->stream));
@@ -901,45 +955,14 @@ int sgb_source_set_points(sgb_ctx* ctx, size_t n, const double* points, const do
       CU(cudaEventRecord(ctx->ev_upload[k], ctx->copy_stream));
     }
   }
-  CU(launch_bounds_centre(ctx->stage_pts.as<double>(), n, ctx->src_bounds.as<double>(), ctx->src_centre.as<double>(), ctx->sm_count, ctx->stream));
-  float4* lo = nullptr;
-  if (!covs) {  // covariances may still be estimated on the device (sgb_source_estimate_features): keep the rounding residuals
-    CU(ctx->tmp_lo.reserve(n * sizeof(float4)));
-    lo = ctx->tmp_lo.as<float4>();
-  }
-  ctx->src_has_lo = lo != nullptr;
-  CU(launch_convert(ctx->stage_pts.as<double>(), nullptr, nullptr, n, ctx->src_centre.as<double>(), ctx->tmp_pts.as<float4>(), nullptr, nullptr, nullptr,
-                    ctx->keys_in.as<uint64_t>(), ctx->vals_in.as<uint32_t>(), ctx->sm_count, ctx->stream, lo));
-  // Hilbert order: consecutive lanes get spatially adjacent queries (coherent tree paths, coalesced gathers)
-  CU(sort_pairs_u64_u32(ctx->sort_temp.p, temp_bytes, ctx->keys_in.as<uint64_t>(), ctx->keys_out.as<uint64_t>(), ctx->vals_in.as<uint32_t>(),
-                        ctx->src_perm.as<uint32_t>(), n, ctx->stream));
   uint32_t K = 1;
 #ifdef SGB_PROFILING
-  // chunk-transposed order of the per-thread search (A/B): a lane walks K consecutive points of the curve, warp loads stay coalesced
   if (const char* s = getenv("SGB_RUN")) K = static_cast<uint32_t>(atoi(s)) > 0 ? static_cast<uint32_t>(atoi(s)) : 1;
   while (K > 1 && n / (32ull * K) < static_cast<size_t>(ctx->sm_count) * 16) K >>= 1;
-  if (K > 1) {
-    CU(launch_chunk_transpose(ctx->src_perm.as<uint32_t>(), ctx->vals_in.as<uint32_t>(), n, K, ctx->sm_count, ctx->stream));
-    CU(cudaMemcpyAsync(ctx->src_perm.p, ctx->vals_in.p, n * sizeof(uint32_t), cudaMemcpyDeviceToDevice, ctx->stream));
-    ctx->launches += 1;
-  }
 #endif
   ctx->src_run = K;
-  CU(launch_gather(ctx->src_perm.as<uint32_t>(), n, ctx->tmp_pts.as<float4>(), ctx->src_pts.as<float4>(), nullptr, nullptr, nullptr, nullptr, nullptr, nullptr,
-                   ctx->sm_count, ctx->stream));
-  ctx->launches += 5;
-  if (covs) {
-    CU(launch_inverse_perm(ctx->src_perm.as<uint32_t>(), n, ctx->src_rank.as<uint32_t>(), ctx->sm_count, ctx->stream));
-    ctx->launches += 1;
-    for (int k = 0; k < n_chunks; k++) {
-      const size_t first = static_cast<size_t>(k) * per_chunk, cnt = std::min(per_chunk, n - first);
-      CU(cudaStreamWaitEvent(ctx->stream, ctx->ev_upload[k], 0));
-      CU(launch_convert_cov_scatter(ctx->stage_covs.as<double>(), first, cnt, ctx->src_rank.as<uint32_t>(), ctx->src_covA.as<float4>(), ctx->src_covB.as<float4>(),
-                                    nullptr, nullptr, ctx->sm_count, ctx->stream));
-      ctx->launches += 1;
-    }
-  }
-  return 0;
+  return store_source(ctx, 0, n, ctx->src_centre.as<double>(), ctx->src_bounds.as<double>(), covs ? nullptr : ctx->tmp_lo.as<float4>(), temp_bytes, K,
+                      n_chunks, ctx->ev_upload);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -983,14 +1006,14 @@ int sgb_error(sgb_ctx* ctx, const double* T, double* out_e) {
 
 int sgb_correspondences(sgb_ctx* ctx, uint64_t* target_index) {
   if (!ctx) return 1;
-  if (ctx->src_is_batch) return fail(ctx, 1, "sgb_correspondences: the context holds a batch of sources (sgb_source_set_batch); use sgb_correspondences_batch");
+  if (ctx->src_state == SourceState::Batch) return fail(ctx, 1, "sgb_correspondences: the context holds a batch of sources (sgb_source_set_batch); use sgb_correspondences_batch");
   if (!ctx->have_lin) return fail(ctx, 1, "sgb_correspondences: no preceding sgb_linearize");
   if (ctx->n_src == 0) return 0;
   if (!target_index) return fail(ctx, 1, "sgb_correspondences: null output");
   CU(cudaSetDevice(ctx->device));
   CU(ctx->corr64.reserve(ctx->n_src * sizeof(uint64_t)));
-  CU(launch_correspondences(ctx->corr.as<uint32_t>(), ctx->src_perm.as<uint32_t>(), ctx->n_src, ctx->tgt_pts.as<float4>(), ctx->tgt_is_voxel ? 1 : 0,
-                            ctx->corr64.as<uint64_t>(), ctx->sm_count, ctx->stream));
+  CU(launch_correspondences(ctx->corr.as<uint32_t>(), ctx->src_perm.as<uint32_t>(), ctx->n_src, ctx->tgt_pts.as<float4>(),
+                            ctx->tgt_state == TargetState::VoxelMap ? 1 : 0, ctx->corr64.as<uint64_t>(), ctx->sm_count, ctx->stream));
   ctx->launches += 1;
   CU(cudaMemcpyAsync(target_index, ctx->corr64.p, ctx->n_src * sizeof(uint64_t), cudaMemcpyDefault, ctx->stream));
   CU(cudaStreamSynchronize(ctx->stream));
@@ -999,7 +1022,7 @@ int sgb_correspondences(sgb_ctx* ctx, uint64_t* target_index) {
 
 int sgb_num_inliers(sgb_ctx* ctx, size_t* n) {
   if (!ctx || !n) return 1;
-  if (ctx->src_is_batch) return fail(ctx, 1, "sgb_num_inliers: the context holds a batch of sources (sgb_source_set_batch); sgb_linearize_batch returns each member's count");
+  if (ctx->src_state == SourceState::Batch) return fail(ctx, 1, "sgb_num_inliers: the context holds a batch of sources (sgb_source_set_batch); sgb_linearize_batch returns each member's count");
   if (!ctx->have_lin || !ctx->last_out) return fail(ctx, 1, "sgb_num_inliers: no preceding sgb_linearize");
   CU(cudaSetDevice(ctx->device));
   if (ctx->last_out == ctx->h_out_dev) {  // sgb_linearize left the count in the mapped host slot

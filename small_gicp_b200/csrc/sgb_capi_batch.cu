@@ -5,7 +5,6 @@
 
 #include <algorithm>
 #include <cfloat>
-#include <cmath>
 #include <cstring>
 #include <string>
 #include <vector>
@@ -26,7 +25,7 @@ size_t batch_members(const sgb_ctx* ctx) { return ctx->b_offsets.empty() ? 0 : c
 size_t max_tiles(const sgb_ctx* ctx) { return batch_points(ctx) / kLinBlock + batch_members(ctx) + 1; }
 
 int batch_check(sgb_ctx* ctx, const char* who, const double* T) {
-  if (!ctx->src_is_batch) return fail(ctx, 1, std::string(who) + ": the context holds no batch of sources (call sgb_source_set_batch)");
+  if (ctx->src_state != SourceState::Batch) return fail(ctx, 1, std::string(who) + ": the context holds no batch of sources (call sgb_source_set_batch)");
   if (ctx->comm_world > 1) return fail(ctx, 1, std::string(who) + ": batched calls are single-GPU only (call sgb_comm_disconnect first)");
   if (!T) return fail(ctx, 1, std::string(who) + ": null poses");
   return 0;
@@ -41,11 +40,7 @@ int batch_tables(sgb_ctx* ctx, const double* T, const uint8_t* active, bool seed
   std::vector<uint4> members(B);
   uint32_t v = 0;
   for (size_t m = 0; m < B; m++) {
-    const double* Tm = T + 16 * m;
-    for (int i = 0; i < 3; i++) {
-      for (int j = 0; j < 3; j++) poses[12 * m + i * 3 + j] = Tm[j * 4 + i];
-      poses[12 * m + 9 + i] = Tm[12 + i];
-    }
+    pose_from_colmajor(T + 16 * m, poses.data() + 12 * m);
     const bool act = !active || active[m];
     const uint32_t first = static_cast<uint32_t>(ctx->b_offsets[m]), n = static_cast<uint32_t>(ctx->b_offsets[m + 1] - ctx->b_offsets[m]);
     const uint32_t t0 = static_cast<uint32_t>(tiles.size());
@@ -105,13 +100,7 @@ int sgb_source_set_batch(sgb_ctx* ctx, size_t n_members, const size_t* offsets, 
   if (n >= (1ull << 31)) return fail(ctx, 1, "sgb_source_set_batch: too many points");
   if (n && !points) return fail(ctx, 1, "sgb_source_set_batch: null points");
   CU(cudaSetDevice(ctx->device));
-  // from here on the context holds this batch (and no single source)
-  ctx->src_is_batch = true;
-  ctx->n_src = 0;
-  ctx->src_has_covs = covs != nullptr;
-  ctx->have_lin = false;
-  ctx->corr_seeds = false;
-  ctx->src_orig_valid = ctx->src_tree_valid = ctx->src_cov_orig_valid = ctx->src_has_lo = false;
+  begin_source(ctx, SourceState::Batch, 0, covs != nullptr);
   ctx->b_offsets.assign(offsets, offsets + n_members + 1);
   ctx->b_lin.assign(n_members, 0);
   ctx->b_seeded.assign(n_members, 0);
@@ -128,19 +117,7 @@ int sgb_source_set_batch(sgb_ctx* ctx, size_t n_members, const size_t* offsets, 
   CU(ctx->b_vq.reserve(nn * sizeof(float4)));
   CU(ctx->b_vcorr.reserve(nn * sizeof(uint32_t)));
   CU(cudaMemsetAsync(ctx->b_corr.p, 0xFF, nn * sizeof(uint32_t), ctx->stream));  // no correspondences before the first linearize
-  // per-query scratch of the search, sized here so that the batch calls never (re)allocate (as sgb_source_set_points does)
-  CU(ctx->grid_state.reserve(nn));
-  {
-    const void* before = ctx->grid_pending.p;
-    CU(ctx->grid_pending.reserve((nn + 2) * sizeof(uint32_t)));
-    if (ctx->grid_pending.p != before) ctx->pending_clean = false;
-    CU(ctx->grid_pending_q.reserve(nn * sizeof(float4)));
-  }
-  {
-    const void* before = ctx->chunk_lists.p;
-    CU(ctx->chunk_lists.reserve((8 + static_cast<size_t>(kChunkClasses) * ((nn + 31) / 32)) * sizeof(uint32_t)));
-    if (ctx->chunk_lists.p != before) ctx->chunk_lists_clean = false;
-  }
+  if (int rc = reserve_query_scratch(ctx, nn)) return rc;
   if (n == 0) return 0;
   CU(ctx->stage_pts.reserve(n * 4 * sizeof(double)));
   CU(ctx->tmp_pts.reserve(n * sizeof(float4)));
@@ -166,21 +143,8 @@ int sgb_source_set_batch(sgb_ctx* ctx, size_t n_members, const size_t* offsets, 
   for (size_t m = 0; m < n_members; m++) {
     const size_t off = offsets[m], nm = offsets[m + 1] - offsets[m];
     if (nm == 0) continue;
-    double* centre = ctx->b_centres.as<double>() + 4 * m;
-    CU(launch_bounds_centre(ctx->stage_pts.as<double>() + 4 * off, nm, ctx->b_bounds.as<double>() + 6 * m, centre, ctx->sm_count, ctx->stream));
-    CU(launch_convert(ctx->stage_pts.as<double>() + 4 * off, nullptr, nullptr, nm, centre, ctx->tmp_pts.as<float4>() + off, nullptr, nullptr, nullptr,
-                      ctx->keys_in.as<uint64_t>() + off, ctx->vals_in.as<uint32_t>() + off, ctx->sm_count, ctx->stream));
-    CU(sort_pairs_u64_u32(ctx->sort_temp.p, temp_bytes, ctx->keys_in.as<uint64_t>() + off, ctx->keys_out.as<uint64_t>() + off,
-                          ctx->vals_in.as<uint32_t>() + off, ctx->src_perm.as<uint32_t>() + off, nm, ctx->stream));
-    CU(launch_gather(ctx->src_perm.as<uint32_t>() + off, nm, ctx->tmp_pts.as<float4>() + off, ctx->src_pts.as<float4>() + off, nullptr, nullptr, nullptr,
-                     nullptr, nullptr, nullptr, ctx->sm_count, ctx->stream));
-    ctx->launches += 5;
-    if (covs) {
-      CU(launch_inverse_perm(ctx->src_perm.as<uint32_t>() + off, nm, ctx->src_rank.as<uint32_t>() + off, ctx->sm_count, ctx->stream));
-      CU(launch_convert_cov_scatter(ctx->stage_covs.as<double>() + 16 * off, 0, nm, ctx->src_rank.as<uint32_t>() + off, ctx->src_covA.as<float4>() + off,
-                                    ctx->src_covB.as<float4>() + off, nullptr, nullptr, ctx->sm_count, ctx->stream));
-      ctx->launches += 2;
-    }
+    if (int rc = store_source(ctx, off, nm, ctx->b_centres.as<double>() + 4 * m, ctx->b_bounds.as<double>() + 6 * m, nullptr, temp_bytes, 1, covs ? 1 : 0, nullptr))
+      return rc;
   }
   return 0;
 }
@@ -194,16 +158,15 @@ int sgb_linearize_batch(sgb_ctx* ctx, int factor, int robust, double robust_c, i
   const size_t B = batch_members(ctx);
   if (B == 0) return 0;
   if (batch_points(ctx) && ctx->n_tgt) {
-    if (!ctx->tgt_ready) return fail(ctx, 1, "sgb_linearize_batch: target has no search structure (call sgb_target_set_kdtree / _build_kdtree / _set_voxelmap)");
-    if (factor == SGB_FACTOR_PLANE_ICP && (!ctx->tgt_has_normals || ctx->tgt_is_voxel)) return fail(ctx, 1, "sgb_linearize_batch: point-to-plane needs target normals");
-    if (factor == SGB_FACTOR_GICP && (!ctx->tgt_has_covs || !ctx->src_has_covs)) return fail(ctx, 1, "sgb_linearize_batch: GICP needs target and source covariances");
+    if (int rc = check_target(ctx, "sgb_linearize_batch", factor)) return rc;
   }
   CU(cudaSetDevice(ctx->device));
+  const bool voxel = ctx->tgt_state == TargetState::VoxelMap;
   // a new target (or none linearised yet) invalidates every member's cached state; sgb_drop_seeds only the seeds
   if (!ctx->have_lin) std::fill(ctx->b_lin.begin(), ctx->b_lin.end(), 0);
   if (!ctx->corr_seeds) std::fill(ctx->b_seeded.begin(), ctx->b_seeded.end(), 0);
   uint32_t n_tiles = 0, n_virtual = 0;
-  if (int rc = batch_tables(ctx, T, active, !ctx->tgt_is_voxel, &n_tiles, &n_virtual)) return rc;
+  if (int rc = batch_tables(ctx, T, active, !voxel, &n_tiles, &n_virtual)) return rc;
   LinParams P;
   fill_params(ctx, P, kIdentity);
   BatchParams Bp = batch_params(ctx, P);
@@ -219,7 +182,7 @@ int sgb_linearize_batch(sgb_ctx* ctx, int factor, int robust, double robust_c, i
     for (size_t m = 0; m < B; m++) none[m].z = (!active || active[m]) ? kMemberActive : 0u;
     CU(cudaMemcpyAsync(ctx->b_members.p, none.data(), B * sizeof(uint4), cudaMemcpyHostToDevice, ctx->stream));
   }
-  if (n_tiles && !ctx->tgt_is_voxel) {
+  if (n_tiles && !voxel) {
     // the search runs over the virtual source: the active members' queries, already transformed into the target's frame
     CU(launch_batch_transform(Bp, n_tiles, ctx->b_vq.as<float4>(), ctx->b_vcorr.as<uint32_t>(), ctx->stream));
     ctx->launches += 1;
@@ -230,17 +193,12 @@ int sgb_linearize_batch(sgb_ctx* ctx, int factor, int robust, double robust_c, i
     P.src.run = 1;
     P.corr = ctx->b_vcorr.as<uint32_t>();
     P.use_prev = 1;  // per member: its previous correspondences, or kNone
-    float bound = FLT_MAX;
-    if (rejector == SGB_REJECT_DISTANCE) {  // the single-source path's FP32 search bound
-      bound = nextafterf(static_cast<float>(max_dist_sq * (1.0 + 4e-6) + 1e-12), INFINITY);
-      if (!(bound < FLT_MAX)) bound = FLT_MAX;
-    }
-    P.max_dist_sq = bound;
+    P.max_dist_sq = search_bound(rejector, max_dist_sq);
     if (int rc = launch_point_search(ctx, P, ctx->tree_depth > 0 ? ctx->tree_depth : 1)) return rc;
     ctx->launches += 1;
   }
   if (n_tiles) {
-    CU(launch_batch_factor(Bp, factor, robust, n_tiles, ctx->tgt_is_voxel, false, ctx->b_vcorr.as<uint32_t>(), ctx->stream));
+    CU(launch_batch_factor(Bp, factor, robust, n_tiles, voxel, false, ctx->b_vcorr.as<uint32_t>(), ctx->stream));
     ctx->launches += 1;
   }
   CU(launch_batch_segment(Bp, static_cast<uint32_t>(B), true, ctx->b_out.as<double>(), ctx->stream));
@@ -276,7 +234,7 @@ int sgb_error_batch(sgb_ctx* ctx, const double* T, const uint8_t* active, double
   BatchParams Bp = batch_params(ctx, P);
   Bp.robust_c = ctx->lin_c;
   if (n_tiles && ctx->n_tgt) {
-    CU(launch_batch_factor(Bp, ctx->lin_factor, ctx->lin_robust, n_tiles, ctx->tgt_is_voxel, true, nullptr, ctx->stream));
+    CU(launch_batch_factor(Bp, ctx->lin_factor, ctx->lin_robust, n_tiles, ctx->tgt_state == TargetState::VoxelMap, true, nullptr, ctx->stream));
     ctx->launches += 1;
   } else {
     n_tiles = 0;
@@ -304,8 +262,8 @@ int sgb_correspondences_batch(sgb_ctx* ctx, uint64_t* out) {
       CU(cudaMemsetAsync(ctx->corr64.as<uint64_t>() + off, 0xFF, nm * sizeof(uint64_t), ctx->stream));
       continue;
     }
-    CU(launch_correspondences(ctx->b_corr.as<uint32_t>() + off, ctx->src_perm.as<uint32_t>() + off, nm, ctx->tgt_pts.as<float4>(), ctx->tgt_is_voxel ? 1 : 0,
-                              ctx->corr64.as<uint64_t>() + off, ctx->sm_count, ctx->stream));
+    CU(launch_correspondences(ctx->b_corr.as<uint32_t>() + off, ctx->src_perm.as<uint32_t>() + off, nm, ctx->tgt_pts.as<float4>(),
+                              ctx->tgt_state == TargetState::VoxelMap ? 1 : 0, ctx->corr64.as<uint64_t>() + off, ctx->sm_count, ctx->stream));
     ctx->launches += 1;
   }
   CU(cudaMemcpyAsync(out, ctx->corr64.p, n * sizeof(uint64_t), cudaMemcpyDefault, ctx->stream));

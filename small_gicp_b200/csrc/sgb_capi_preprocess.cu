@@ -83,7 +83,7 @@ int build_lbvh(sgb_ctx* ctx, const float4* d_orig_pts, size_t n, const double* d
 int build_grid(sgb_ctx* ctx) {
   ctx->grid_ready = false;
   const size_t n = ctx->n_tgt;
-  if (!ctx->use_grid || ctx->search_mode != 2 || ctx->tgt_is_voxel || n < 1024 || ctx->n_pnodes == 0) return 0;
+  if (!ctx->use_grid || ctx->search_mode != 2 || ctx->tgt_state != TargetState::Tree || n < 1024 || ctx->n_pnodes == 0) return 0;
   // spacing estimate from the leaf boxes + the target box (one small D2H, construction is a per-target one-off)
   const size_t m = ctx->n_pnodes * 2;
   CU(ctx->grid_spacing.reserve(m * sizeof(float)));
@@ -139,7 +139,6 @@ int build_grid(sgb_ctx* ctx) {
   CU(launch_grid_fill(ctx->keys_out.as<uint64_t>(), ctx->pre_vals_out.as<uint32_t>(), ctx->tgt_pts.as<float4>(), static_cast<uint32_t>(n_ent), ctx->vals_in.as<uint32_t>(),
                       ctx->keys_in.as<uint32_t>(), ctx->sort_temp.p, tb, ctx->grid_pts.as<float4>(), ctx->grid_table.as<GridSlot>(), capacity, ctx->grid_curve_order,
                       ctx->stream));
-  ctx->grid_blocks = true;
   ctx->launches += 5;
   for (int a = 0; a < 3; a++) ctx->grid_origin[a] = g.origin[a];
   ctx->grid_inv_cell = g.inv_cell;
@@ -151,6 +150,34 @@ int build_grid(sgb_ctx* ctx) {
 }
 
 }  // namespace sgb
+
+namespace {
+
+// Sorts the n points at stage_pts into voxels of edge 1 / inv_leaf: keys_out / pre_vals_out = voxel keys / point indices in key order,
+// pre_heads[j] = 1 where a voxel starts, pre_slots = their exclusive scan (pre_slots[n] = voxel count).  7 launches.
+int sort_into_voxels(sgb_ctx* ctx, size_t n, double inv_leaf) {
+  CU(ctx->keys_in.reserve(n * sizeof(uint64_t)));
+  CU(ctx->keys_out.reserve(n * sizeof(uint64_t)));
+  CU(ctx->vals_in.reserve(n * sizeof(uint32_t)));
+  CU(ctx->pre_vals_out.reserve(n * sizeof(uint32_t)));
+  CU(ctx->pre_heads.reserve((n + 1) * sizeof(uint32_t)));
+  CU(ctx->pre_slots.reserve((n + 1) * sizeof(uint32_t)));
+  CU(launch_voxel_keys(ctx->stage_pts.as<double>(), n, inv_leaf, ctx->keys_in.as<uint64_t>(), ctx->vals_in.as<uint32_t>(), ctx->sm_count, ctx->stream));
+  size_t temp_bytes = 0, scan_bytes = 0;
+  CU(sort_pairs_u64_u32(nullptr, temp_bytes, ctx->keys_in.as<uint64_t>(), ctx->keys_out.as<uint64_t>(), ctx->vals_in.as<uint32_t>(),
+                        ctx->pre_vals_out.as<uint32_t>(), n, ctx->stream));
+  CU(exclusive_sum_u32(nullptr, scan_bytes, ctx->pre_heads.as<uint32_t>(), ctx->pre_slots.as<uint32_t>(), n + 1, ctx->stream));
+  CU(ctx->sort_temp.reserve(temp_bytes > scan_bytes ? temp_bytes : scan_bytes));
+  CU(sort_pairs_u64_u32(ctx->sort_temp.p, temp_bytes, ctx->keys_in.as<uint64_t>(), ctx->keys_out.as<uint64_t>(), ctx->vals_in.as<uint32_t>(),
+                        ctx->pre_vals_out.as<uint32_t>(), n, ctx->stream));
+  CU(cudaMemsetAsync(ctx->pre_heads.p, 0, (n + 1) * sizeof(uint32_t), ctx->stream));
+  CU(launch_voxel_heads(ctx->keys_out.as<uint64_t>(), n, ctx->pre_heads.as<uint32_t>(), ctx->sm_count, ctx->stream));
+  CU(exclusive_sum_u32(ctx->sort_temp.p, scan_bytes, ctx->pre_heads.as<uint32_t>(), ctx->pre_slots.as<uint32_t>(), n + 1, ctx->stream));
+  ctx->launches += 7;
+  return 0;
+}
+
+}  // namespace
 
 extern "C" {
 
@@ -190,11 +217,9 @@ int sgb_estimate_features(sgb_ctx* ctx, size_t n, const double* points, int num_
 int sgb_target_estimate_features(sgb_ctx* ctx, int num_neighbors) {
   if (!ctx) return 1;
   if (num_neighbors < 1 || num_neighbors > 32) return fail(ctx, 1, "sgb_target_estimate_features: num_neighbors must be in 1..32");
-  if (ctx->tgt_is_voxel || !ctx->tgt_ready) return fail(ctx, 1, "sgb_target_estimate_features: needs a point target with its kd-tree (set points, then set/build the tree)");
+  if (ctx->tgt_state != TargetState::Tree) return fail(ctx, 1, "sgb_target_estimate_features: needs a point target with its kd-tree (set points, then set/build the tree)");
   const size_t n = ctx->n_tgt;
-  ctx->tgt_has_normals = ctx->tgt_has_covs = true;
-  ctx->have_lin = false;
-  ctx->corr_seeds = false;
+  features_changed(ctx, true);
   if (n == 0) return 0;
   CU(cudaSetDevice(ctx->device));
   CU(ctx->tgt_normals.reserve(n * sizeof(float4)));
@@ -218,15 +243,12 @@ int sgb_target_estimate_features(sgb_ctx* ctx, int num_neighbors) {
 int sgb_source_estimate_features(sgb_ctx* ctx, int num_neighbors) {
   if (!ctx) return 1;
   if (num_neighbors < 1 || num_neighbors > 32) return fail(ctx, 1, "sgb_source_estimate_features: num_neighbors must be in 1..32");
-  if (ctx->src_is_batch) return fail(ctx, 1, "sgb_source_estimate_features: the context holds a batch of sources; pass each member's covariances to sgb_source_set_batch");
+  if (ctx->src_state == SourceState::Batch) return fail(ctx, 1, "sgb_source_estimate_features: the context holds a batch of sources; pass each member's covariances to sgb_source_set_batch");
   const size_t n = ctx->n_src;
-  ctx->src_has_covs = true;
-  ctx->have_lin = false;
-  ctx->corr_seeds = false;
+  features_changed(ctx, false);
   if (n == 0) return 0;
   CU(cudaSetDevice(ctx->device));
-  // tmp_pts still holds the source in ORIGINAL order (centred FP32, w = index) from sgb_source_set_points
-  if (!ctx->src_orig_valid) return fail(ctx, 1, "sgb_source_estimate_features: no source points (call sgb_source_set_points first)");
+  // a single source of n > 0 points: tmp_pts holds it in ORIGINAL order (centred FP32, w = index)
   int depth = 0;
   ctx->src_tree_valid = false;
   if (int rc = build_lbvh(ctx, ctx->tmp_pts.as<float4>(), n, ctx->src_centre.as<double>(), ctx->pre_perm, ctx->pre_leaf_pts, ctx->pre_nodes, &depth)) return rc;
@@ -256,28 +278,11 @@ int sgb_voxelgrid_sampling(sgb_ctx* ctx, size_t n, const double* points, double 
   CU(cudaSetDevice(ctx->device));
   CU(ctx->stage_pts.reserve(n * 4 * sizeof(double)));
   CU(cudaMemcpyAsync(ctx->stage_pts.p, points, n * 4 * sizeof(double), cudaMemcpyDefault, ctx->stream));
-  CU(ctx->keys_in.reserve(n * sizeof(uint64_t)));
-  CU(ctx->keys_out.reserve(n * sizeof(uint64_t)));
-  CU(ctx->vals_in.reserve(n * sizeof(uint32_t)));
-  CU(ctx->pre_vals_out.reserve(n * sizeof(uint32_t)));
-  CU(ctx->pre_heads.reserve((n + 1) * sizeof(uint32_t)));
-  CU(ctx->pre_slots.reserve((n + 1) * sizeof(uint32_t)));
+  if (int rc = sort_into_voxels(ctx, n, 1.0 / leaf_size)) return rc;
   CU(ctx->stage_covs.reserve(n * 4 * sizeof(double)));  // output staging (re-uses a scratch buffer)
-  CU(launch_voxel_keys(ctx->stage_pts.as<double>(), n, 1.0 / leaf_size, ctx->keys_in.as<uint64_t>(), ctx->vals_in.as<uint32_t>(), ctx->sm_count, ctx->stream));
-  size_t temp_bytes = 0;
-  CU(sort_pairs_u64_u32(nullptr, temp_bytes, ctx->keys_in.as<uint64_t>(), ctx->keys_out.as<uint64_t>(), ctx->vals_in.as<uint32_t>(),
-                        ctx->pre_vals_out.as<uint32_t>(), n, ctx->stream));
-  size_t scan_bytes = 0;
-  CU(exclusive_sum_u32(nullptr, scan_bytes, ctx->pre_heads.as<uint32_t>(), ctx->pre_slots.as<uint32_t>(), n + 1, ctx->stream));
-  CU(ctx->sort_temp.reserve(temp_bytes > scan_bytes ? temp_bytes : scan_bytes));
-  CU(sort_pairs_u64_u32(ctx->sort_temp.p, temp_bytes, ctx->keys_in.as<uint64_t>(), ctx->keys_out.as<uint64_t>(), ctx->vals_in.as<uint32_t>(),
-                        ctx->pre_vals_out.as<uint32_t>(), n, ctx->stream));
-  CU(cudaMemsetAsync(ctx->pre_heads.p, 0, (n + 1) * sizeof(uint32_t), ctx->stream));
-  CU(launch_voxel_heads(ctx->keys_out.as<uint64_t>(), n, ctx->pre_heads.as<uint32_t>(), ctx->sm_count, ctx->stream));
-  CU(exclusive_sum_u32(ctx->sort_temp.p, scan_bytes, ctx->pre_heads.as<uint32_t>(), ctx->pre_slots.as<uint32_t>(), n + 1, ctx->stream));
   CU(launch_voxel_means(ctx->keys_out.as<uint64_t>(), ctx->pre_vals_out.as<uint32_t>(), ctx->pre_heads.as<uint32_t>(), ctx->pre_slots.as<uint32_t>(), n,
                         ctx->stage_pts.as<double>(), ctx->stage_covs.as<double>(), ctx->sm_count, ctx->stream));
-  ctx->launches += 8;
+  ctx->launches += 1;
   uint32_t count = 0;
   CU(cudaMemcpyAsync(&count, ctx->pre_slots.as<uint32_t>() + n, sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
   CU(cudaStreamSynchronize(ctx->stream));
@@ -293,7 +298,7 @@ int sgb_voxelgrid_sampling(sgb_ctx* ctx, size_t n, const double* points, double 
 // the source of this align() is the target of the next one.  Everything that already exists on the device is taken over, not rebuilt.
 int sgb_target_adopt_source(sgb_ctx* ctx) {
   if (!ctx) return 1;
-  if (!ctx->src_orig_valid || ctx->n_src == 0) return fail(ctx, 1, "sgb_target_adopt_source: no source points (call sgb_source_set_points first)");
+  if (ctx->src_state != SourceState::Single || ctx->n_src == 0) return fail(ctx, 1, "sgb_target_adopt_source: no source points (call sgb_source_set_points first)");
   CU(cudaSetDevice(ctx->device));
   const size_t n = ctx->n_src;
   const bool covs = ctx->src_has_covs;
@@ -306,7 +311,6 @@ int sgb_target_adopt_source(sgb_ctx* ctx) {
     ctx->launches += 1;
   }
   ctx->tgt_orig_pts.swap(ctx->tmp_pts);
-  ctx->tgt_has_lo = ctx->src_has_lo;
   if (ctx->src_has_lo) ctx->tgt_orig_lo.swap(ctx->tmp_lo);
   if (covs) {
     ctx->tgt_orig_covA.swap(ctx->tmp_covA);
@@ -316,17 +320,12 @@ int sgb_target_adopt_source(sgb_ctx* ctx) {
   ctx->tgt_bounds.swap(ctx->src_bounds);
   CU(ctx->src_centre.reserve(4 * sizeof(double)));
   CU(ctx->src_bounds.reserve(6 * sizeof(double)));
-  ctx->n_tgt = n;
-  ctx->tgt_has_normals = false;
-  ctx->tgt_has_covs = covs;
-  ctx->tgt_is_voxel = false;
-  ctx->tgt_has_kd = false;
-  ctx->tgt_feats_leaf_only = false;
-  ctx->grid_ready = false;
-  ctx->have_lin = false;
-  ctx->corr_seeds = false;
+  const bool src_tree = ctx->src_tree_valid;
   int depth = ctx->src_tree_depth;
-  if (ctx->src_tree_valid) {
+  if (int rc = begin_point_target(ctx, n, false, covs, ctx->src_has_lo)) return rc;
+  // the context has no source until the next sgb_source_set_points (its buffers now belong to the target)
+  begin_source(ctx, SourceState::None, 0, false);
+  if (src_tree) {
     ctx->tgt_perm.swap(ctx->pre_perm);
     ctx->tgt_pts.swap(ctx->pre_leaf_pts);
     ctx->tgt_pnodes.swap(ctx->pre_nodes);
@@ -334,20 +333,8 @@ int sgb_target_adopt_source(sgb_ctx* ctx) {
     return rc;
   }
   if (depth > 40) return fail(ctx, 1, "sgb_target_adopt_source: tree too deep");
-  if (covs) {
-    CU(ctx->tgt_covA.reserve(n * sizeof(float4)));
-    CU(ctx->tgt_covB.reserve(n * sizeof(float4)));
-    CU(launch_gather(ctx->tgt_perm.as<uint32_t>(), n, nullptr, nullptr, nullptr, nullptr, ctx->tgt_orig_covA.as<float4>(), ctx->tgt_covA.as<float4>(),
-                     ctx->tgt_orig_covB.as<float4>(), ctx->tgt_covB.as<float4>(), ctx->sm_count, ctx->stream));
-    ctx->launches += 1;
-  }
-  ctx->tree_depth = depth;
-  ctx->n_pnodes = (static_cast<size_t>(1) << (depth - 1)) - 1;
-  ctx->tgt_ready = true;
-  // the context has no source until the next sgb_source_set_points (its buffers now belong to the target)
-  ctx->n_src = 0;
-  ctx->src_has_covs = ctx->src_orig_valid = ctx->src_tree_valid = ctx->src_cov_orig_valid = ctx->src_has_lo = false;
-  return build_grid(ctx);
+  if (int rc = gather_target_features(ctx, false)) return rc;
+  return install_tree(ctx, depth, (static_cast<size_t>(1) << (depth - 1)) - 1);
 }
 
 // Gaussian voxel map built on the device (SURVEY §8f row 3): replaces IncrementalVoxelMap<GaussianVoxel>::insert
@@ -359,19 +346,7 @@ int sgb_target_build_voxelmap(sgb_ctx* ctx, size_t n, const double* points, cons
   if (n >= (1ull << 31)) return fail(ctx, 1, "sgb_target_build_voxelmap: too many points");
   if (search_offsets != 1 && search_offsets != 7 && search_offsets != 27) search_offsets = 1;  // incremental_voxelmap.hpp:159-163
   CU(cudaSetDevice(ctx->device));
-  ctx->tgt_has_normals = false;
-  ctx->tgt_has_covs = covs != nullptr;
-  ctx->tgt_is_voxel = true;
-  ctx->tgt_has_kd = false;
-  ctx->grid_ready = false;
-  ctx->tgt_ready = true;
-  ctx->have_lin = false;
-  ctx->corr_seeds = false;
-  ctx->vox_offsets = search_offsets;
-  ctx->vox_inv_leaf = 1.0 / leaf_size;
-  ctx->n_tgt = 0;
-  CU(ctx->tgt_centre.reserve(4 * sizeof(double)));
-  CU(ctx->tgt_bounds.reserve(6 * sizeof(double)));
+  if (int rc = begin_voxel_target(ctx, 0, covs != nullptr, leaf_size, search_offsets)) return rc;  // n_tgt = the voxel count once known
   if (n == 0) return 0;
   CU(ctx->stage_pts.reserve(n * 4 * sizeof(double)));
   CU(cudaMemcpyAsync(ctx->stage_pts.p, points, n * 4 * sizeof(double), cudaMemcpyDefault, ctx->stream));
@@ -379,32 +354,15 @@ int sgb_target_build_voxelmap(sgb_ctx* ctx, size_t n, const double* points, cons
     CU(ctx->stage_covs.reserve(n * 16 * sizeof(double)));
     CU(cudaMemcpyAsync(ctx->stage_covs.p, covs, n * 16 * sizeof(double), cudaMemcpyDefault, ctx->stream));
   }
-  CU(ctx->keys_in.reserve(n * sizeof(uint64_t)));
-  CU(ctx->keys_out.reserve(n * sizeof(uint64_t)));
-  CU(ctx->vals_in.reserve(n * sizeof(uint32_t)));
-  CU(ctx->pre_vals_out.reserve(n * sizeof(uint32_t)));
-  CU(ctx->pre_heads.reserve((n + 1) * sizeof(uint32_t)));
-  CU(ctx->pre_slots.reserve((n + 1) * sizeof(uint32_t)));
-  CU(launch_voxel_keys(ctx->stage_pts.as<double>(), n, 1.0 / leaf_size, ctx->keys_in.as<uint64_t>(), ctx->vals_in.as<uint32_t>(), ctx->sm_count, ctx->stream));
-  size_t temp_bytes = 0, scan_bytes = 0;
-  CU(sort_pairs_u64_u32(nullptr, temp_bytes, ctx->keys_in.as<uint64_t>(), ctx->keys_out.as<uint64_t>(), ctx->vals_in.as<uint32_t>(),
-                        ctx->pre_vals_out.as<uint32_t>(), n, ctx->stream));
-  CU(exclusive_sum_u32(nullptr, scan_bytes, ctx->pre_heads.as<uint32_t>(), ctx->pre_slots.as<uint32_t>(), n + 1, ctx->stream));
-  CU(ctx->sort_temp.reserve(temp_bytes > scan_bytes ? temp_bytes : scan_bytes));
-  CU(sort_pairs_u64_u32(ctx->sort_temp.p, temp_bytes, ctx->keys_in.as<uint64_t>(), ctx->keys_out.as<uint64_t>(), ctx->vals_in.as<uint32_t>(),
-                        ctx->pre_vals_out.as<uint32_t>(), n, ctx->stream));
-  CU(cudaMemsetAsync(ctx->pre_heads.p, 0, (n + 1) * sizeof(uint32_t), ctx->stream));
-  CU(launch_voxel_heads(ctx->keys_out.as<uint64_t>(), n, ctx->pre_heads.as<uint32_t>(), ctx->sm_count, ctx->stream));
-  CU(exclusive_sum_u32(ctx->sort_temp.p, scan_bytes, ctx->pre_heads.as<uint32_t>(), ctx->pre_slots.as<uint32_t>(), n + 1, ctx->stream));
+  if (int rc = sort_into_voxels(ctx, n, 1.0 / leaf_size)) return rc;
   uint32_t n_vox = 0;
   CU(cudaMemcpyAsync(&n_vox, ctx->pre_slots.as<uint32_t>() + n, sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
   CU(cudaStreamSynchronize(ctx->stream));
-  ctx->launches += 7;
   if (n_vox == 0) return 0;  // every point outside the 21-bit voxel range
   // per-voxel mean / covariance / integer coordinates (FP64), then the same device-side conversion as sgb_target_set_voxelmap
   CU(ctx->pre_out_normals.reserve(static_cast<size_t>(n_vox) * 4 * sizeof(double)));
   if (covs) CU(ctx->pre_out_covs.reserve(static_cast<size_t>(n_vox) * 16 * sizeof(double)));
-  CU(ctx->pre_vox_coords.reserve(static_cast<size_t>(n_vox) * sizeof(int4)));  // NOT tmp_pts: that buffer holds the source in original order
+  CU(ctx->pre_vox_coords.reserve(static_cast<size_t>(n_vox) * sizeof(int4)));
   CU(launch_voxel_stats(ctx->keys_out.as<uint64_t>(), ctx->pre_vals_out.as<uint32_t>(), ctx->pre_heads.as<uint32_t>(), ctx->pre_slots.as<uint32_t>(), n,
                         ctx->stage_pts.as<double>(), covs ? ctx->stage_covs.as<double>() : nullptr, ctx->pre_out_normals.as<double>(),
                         covs ? ctx->pre_out_covs.as<double>() : nullptr, ctx->pre_vox_coords.as<int4>(), ctx->sm_count, ctx->stream));
@@ -432,7 +390,7 @@ int sgb_target_batch_knn(sgb_ctx* ctx, size_t n_queries, const double* queries, 
   if (k < 1 || k > 32) return fail(ctx, 1, "sgb_target_batch_knn: k must be in 1..32");
   if (n_queries && (!queries || !out_indices || !out_sq_dists)) return fail(ctx, 1, "sgb_target_batch_knn: null buffer");
   if (n_queries >= (1ull << 31) / static_cast<size_t>(k)) return fail(ctx, 1, "sgb_target_batch_knn: too many queries");
-  if (ctx->tgt_is_voxel || !ctx->tgt_ready) return fail(ctx, 1, "sgb_target_batch_knn: needs a point target with its kd-tree (set points, then set/build the tree)");
+  if (ctx->tgt_state != TargetState::Tree) return fail(ctx, 1, "sgb_target_batch_knn: needs a point target with its kd-tree (set points, then set/build the tree)");
   if (n_queries == 0) return 0;
   CU(cudaSetDevice(ctx->device));
   const size_t n = n_queries, nk = n * static_cast<size_t>(k);

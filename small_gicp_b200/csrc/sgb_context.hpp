@@ -1,5 +1,5 @@
 // SPDX-License-Identifier: MIT
-// The context behind the opaque sgb_ctx handle of include/sgicp_b200.h (shared by sgb_capi.cu / sgb_capi_preprocess.cu).
+// The context behind the opaque sgb_ctx handle of include/sgicp_b200.h (shared by sgb_capi.cu / sgb_capi_preprocess.cu / sgb_capi_batch.cu).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -47,6 +47,13 @@ struct DevBuf {
   }
 };
 
+/// What the target is.  Points: tgt_orig_* hold n_tgt points in original order, no search structure yet.  Tree: the points are still
+/// resident, and tgt_perm / tgt_pts / tgt_pnodes (+ the grid front end when grid_ready) are their search structure.  VoxelMap: tgt_pts /
+/// tgt_cov* hold n_tgt voxels and vox_table indexes them; tgt_orig_* belong to no one.
+enum class TargetState { None, Points, Tree, VoxelMap };
+/// What the source is.  Single: one cloud of n_src points.  Batch: b_offsets.size() - 1 members concatenated (n_src = 0).
+enum class SourceState { None, Single, Batch };
+
 }  // namespace sgb
 
 struct sgb_ctx {
@@ -67,21 +74,23 @@ struct sgb_ctx {
   int search_mode = 2;  // 2: packet (warp-cooperative) search + factor kernel; [profiling build] 1: per-thread search + factor kernel; 0: single fused kernel
 
   // ---- target ----
+  // tgt_state and src_state are written by the transitions in sgb_capi.cu (begin_point_target, begin_voxel_target, install_tree,
+  // begin_source, features_changed), which are also the only places that drop the last linearisation (have_lin, corr_seeds).
+  // (A tree over an empty target only sets tgt_state = Tree: there is nothing to install and nothing is dropped.)
+  sgb::TargetState tgt_state = sgb::TargetState::None;
   size_t n_tgt = 0;
   bool tgt_has_normals = false, tgt_has_covs = false;
-  bool tgt_is_voxel = false, tgt_ready = false;
-  sgb::DevBuf tgt_orig_pts, tgt_orig_normals, tgt_orig_covA, tgt_orig_covB;  // original order
+  sgb::DevBuf tgt_orig_pts, tgt_orig_normals, tgt_orig_covA, tgt_orig_covB;  // original order (Points / Tree)
   sgb::DevBuf tgt_orig_lo, tmp_lo, pre_lo;  // what the FP32 rounding of the coordinates dropped (target / source / scratch cloud, original order): feature estimation only
   sgb::DevBuf tgt_pts, tgt_normals, tgt_covA, tgt_covB;                      // leaf order (or voxel order)
-  sgb::DevBuf tgt_nodes, tgt_perm, tgt_pnodes;  // kd nodes (8 B), leaf permutation, packet records (64 B / inner node)
+  sgb::DevBuf tgt_nodes, tgt_perm, tgt_pnodes;  // kd nodes (8 B, profiling build only), leaf permutation, packet records (64 B / inner node)
   int tree_depth = 0;
-  bool tgt_has_kd = false;  // 8-byte kd nodes present (adopted / host-built trees); device-built trees only have packet records
   bool host_tree = false;   // profiling switch: sgb_target_build_kdtree builds a median-split kd-tree on the host
   int tree_quality = 1;     // device construction: 1 = Hilbert order + per-level median-split refinement (kd quality), 0 = Hilbert order only (linear BVH)
   sgb::DevBuf pre_boxes;
   size_t n_pnodes = 0;      // packet records of the current target tree
   // uniform-grid front end of the search (sgb_grid.cu)
-  bool use_grid = true, grid_ready = false, grid_blocks = true;  // grid_blocks: the front end holds 2 x 2 x 2 block lists (one lookup per query)
+  bool use_grid = true, grid_ready = false;  // the front end holds 2 x 2 x 2 block lists (one lookup per query)
   sgb::DevBuf grid_pts, grid_table, grid_state, grid_spacing, grid_pending;  // grid_pending: [0], [1] = alternating counters, [2..] = pending query positions
   sgb::DevBuf grid_pending_q;  // parallel to the list: transformed query + squared distance of the probe's best candidate
   bool use_ring = true, debug_pending = false;  // profiling switches (sgb_create)
@@ -110,27 +119,30 @@ struct sgb_ctx {
   double vox_inv_leaf = 1.0;
 
   // ---- source ----
+  sgb::SourceState src_state = sgb::SourceState::None;
   size_t n_src = 0;
   bool src_has_covs = false;
-  sgb::DevBuf src_pts, src_covA, src_covB, src_perm, src_rank, src_centre, src_bounds;
+  sgb::DevBuf src_pts, src_covA, src_covB, src_perm, src_rank, src_centre, src_bounds;  // search order (src_perm: search order -> original index)
   uint32_t src_run = 1;  // K of the chunk-transposed source layout (DevSource::run)
+  // Buffers of the single source that outlive a call, read by sgb_source_estimate_features and taken over by sgb_target_adopt_source.
+  // begin_source clears their flags; only sgb_estimate_features also writes one of them (its scratch tree goes to pre_*).
+  sgb::DevBuf tmp_pts;  // the source in original order (centred FP32, w = index)
+  bool tgt_has_lo = false, src_has_lo = false;  // tgt_orig_lo / tmp_lo hold the residuals of the current target / single source
+  bool src_tree_valid = false;  // pre_perm / pre_leaf_pts / pre_nodes hold the source's tree (sgb_source_estimate_features built it), depth src_tree_depth
+  sgb::DevBuf tmp_covA, tmp_covB;
+  bool src_cov_orig_valid = false;  // tmp_covA / tmp_covB hold the source's covariances in original order (estimated on the device)
+  int src_tree_depth = 0;
 
-  // ---- scratch ----
+  // ---- scratch: contents do not outlive the call that writes them ----
   sgb::DevBuf stage_pts, stage_normals, stage_covs;  // raw double uploads
-  sgb::DevBuf tmp_pts, tmp_covA, tmp_covB, keys_in, keys_out, vals_in, sort_temp;
-  sgb::DevBuf corr, partials, ticket, out44, corr64;
+  sgb::DevBuf keys_in, keys_out, vals_in, sort_temp;
+  sgb::DevBuf corr, partials, ticket, corr64;
   double* h_out = nullptr;      // page-locked AND mapped, 64 doubles: [0,44) H|b|e|inliers, [48] error(), [56] scratch, [60] comm status
   double* h_out_dev = nullptr;  // device address of the same memory (the reduction's finishing CTA writes into it)
 
   // ---- preprocessing scratch (sgb_capi_preprocess.cu) ----
   sgb::DevBuf pre_pts, pre_leaf_pts, pre_nodes, pre_perm, pre_centre, pre_bounds, pre_out_normals, pre_out_covs, pre_heads, pre_slots, pre_vals_out;
-  sgb::DevBuf pre_vox_coords;  // integer voxel coordinates of sgb_target_build_voxelmap (its own scratch: tmp_pts belongs to the source)
-  bool tgt_has_lo = false, src_has_lo = false;  // tgt_orig_lo / tmp_lo hold the residuals of the current target / source
-  bool src_tree_valid = false;  // pre_perm / pre_leaf_pts / pre_nodes hold the SOURCE's tree (sgb_source_estimate_features built it), depth src_tree_depth
-  bool src_cov_orig_valid = false;  // tmp_covA / tmp_covB hold the source's covariances in original order (estimated on the device)
-  int src_tree_depth = 0;
-  bool src_orig_valid = false;  // tmp_pts holds the current source in original order (sgb_source_estimate_features needs it)
-  bool tgt_feats_leaf_only = false;  // normals / covariances were estimated on the device into the leaf-ordered streams only
+  sgb::DevBuf pre_vox_coords;  // integer voxel coordinates of sgb_target_build_voxelmap
 
   // ---- multi-GPU exchange fused into the reduction's finishing CTA (sgb_comm_*, CommParams in sgb_device.cuh) ----
   sgb::DevBuf comm_mail;                  // this rank's mailbox (zeroed at allocation)
@@ -149,10 +161,8 @@ struct sgb_ctx {
   double lin_c = 1.0;
   double Tlin[12] = {1, 0, 0, 0, 1, 0, 0, 0, 1, 0, 0, 0};
   const double* last_out = nullptr;  // device pointer holding H|b|e|inliers of the last linearize
-  int lin_grid = 0;
 
   // ---- batch of sources (sgb_source_set_batch, sgb_capi_batch.cu): members concatenated in src_pts / src_covA / src_covB / src_perm ----
-  bool src_is_batch = false;
   std::vector<size_t> b_offsets;           // members + 1
   std::vector<uint8_t> b_lin, b_seeded;    // per member: linearised against the current target / correspondences usable as search seeds
   sgb::DevBuf b_centres, b_bounds;         // [members][4] / [members][6]
@@ -174,6 +184,33 @@ inline int fail(sgb_ctx* c, int code, const std::string& msg) {
 int build_lbvh(sgb_ctx* ctx, const float4* d_orig_pts, size_t n, const double* d_centre4, DevBuf& perm, DevBuf& leaf_pts, DevBuf& pnodes, int* depth);
 /// uniform grid over the current (leaf-ordered) target for the search front end; no-op unless enabled
 int build_grid(sgb_ctx* ctx);
+
+// ---- transitions (sgb_capi.cu) ----
+/// a target of n points (with normals / covariances / FP32 rounding residuals as flagged) replaces the target; no search structure yet
+int begin_point_target(sgb_ctx* ctx, size_t n, bool normals, bool covs, bool lo);
+/// a voxel map of n voxels replaces the target (the caller fills tgt_pts / tgt_cov* and vox_table)
+int begin_voxel_target(sgb_ctx* ctx, size_t n, bool covs, double leaf_size, int search_offsets);
+/// the point target's tree in tgt_perm / tgt_pts / tgt_pnodes (depth, n_pnodes packet records) becomes its search structure; builds the grid
+int install_tree(sgb_ctx* ctx, int depth, size_t n_pnodes);
+/// a single cloud of n points, a batch (n = 0) or nothing replaces the source
+void begin_source(sgb_ctx* ctx, SourceState state, size_t n, bool covs);
+/// normals and covariances (target) or covariances (source) were estimated on the device
+void features_changed(sgb_ctx* ctx, bool target);
+
+// ---- steps shared by the entry points (sgb_capi.cu) ----
+void pose_from_colmajor(const double* T, double out12[12]);
+/// gathers the target's normals / covariances (and with points its FP32 points) from original into leaf order: 0 or 1 launch
+int gather_target_features(sgb_ctx* ctx, bool points);
+/// sizes the per-query scratch of the search for n queries, so that the linearize calls never (re)allocate: a cudaFree there would
+/// synchronise the device in the middle of an asynchronous call
+int reserve_query_scratch(sgb_ctx* ctx, size_t n);
+/// stores stage_pts[off, off + n) as one source cloud in src_*[off..] (see the definition); 5 launches, + 1 + cov_chunks with covariances
+int store_source(sgb_ctx* ctx, size_t off, size_t n, double* centre, double* bounds, float4* lo, size_t sort_bytes, uint32_t run, int cov_chunks,
+                 const cudaEvent_t* arrived);
+/// the target can serve `factor` (who names the caller in the message)
+int check_target(sgb_ctx* ctx, const char* who, int factor);
+/// FP32 search bound a hair above the rejector's threshold (FLT_MAX without a distance rejector)
+float search_bound(int rejector, double max_dist_sq);
 
 struct LinParams;
 /// kernel parameters of the current target and source at pose T (sgb_capi.cu)
