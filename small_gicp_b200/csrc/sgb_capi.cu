@@ -580,7 +580,6 @@ int sgb_create(int device_id, sgb_ctx** out_ctx) {
   }
   if (const char* s = getenv("SGB_PACKET_QUEUE")) ctx->use_packet_queue = !(s[0] == '0');   // 0 = chunks assigned to warps by a static stride
   if (const char* s = getenv("SGB_CHUNK_CLASSES")) ctx->use_chunk_classes = !(s[0] == '0');  // 0 = no work lists by cost class: chunks in curve order
-  if (const char* s = getenv("SGB_GRID_ORDER")) ctx->grid_curve_order = !(s[0] == '0');  // 0 = block lists in raster order of the packed block coordinates
   if (const char* s = getenv("SGB_KD_SMEM")) ctx->kd_smem_refine = !(s[0] == '0');  // 0 = kd refinement with one radix sort per level all the way down
   if (const char* s = getenv("SGB_ERROR_PIPE")) ctx->error_pipelined = !(s[0] == '0');  // 0 = Reduction::error through the plain grid-stride kernel
   if (const char* s = getenv("SGB_TMA_LEAF")) ctx->tma_leaf = (s[0] == '1');  // 1 = dense leaf scans read a cp.async.bulk (TMA) staged copy of the leaf

@@ -2,6 +2,7 @@
 // C-ABI entry points of the per-cloud preparation steps (SURVEY.md §8(f)): normal / covariance estimation and
 // voxel-grid down-sampling on the device.  Kernels: sgb_preprocess.cu.
 #include <algorithm>
+#include <cmath>
 #include <cstdlib>
 #include <cstring>
 #include <limits>
@@ -109,37 +110,47 @@ int build_grid(sgb_ctx* ctx) {
   g.inv_cell = static_cast<float>(1.0 / cell);
   const double settle = (0.5 - 4e-3) * cell;  // margin for the FP32 cell-coordinate arithmetic (kGridSlack cells, sgb_grid.cu)
   g.settle_d2 = static_cast<float>(settle * settle);
-  const size_t n_ent = n * 8;  // block lists hold every point under its eight enclosing 2 x 2 x 2 blocks
-  if (n_ent >= (1ull << 31)) return 0;
-  CU(ctx->keys_in.reserve(n_ent * sizeof(uint64_t)));
-  CU(ctx->keys_out.reserve(n_ent * sizeof(uint64_t)));
-  CU(ctx->vals_in.reserve(n_ent * sizeof(uint32_t)));
-  CU(ctx->pre_vals_out.reserve(n_ent * sizeof(uint32_t)));
+  if (n >= (1ull << 28)) return 0;  // eight anchor entries per point must stay below 2^31
+  // compact sort keys: B bits per axis hold every cell and anchor coordinate (-2 .. cells along the widest axis + 1, biased by 2) with the
+  // all-ones pad left over; at most 13 bits (cell indices < 2^13)
+  const double cells_axis = std::ceil(ext / cell) + 2.0;
+  int bits = 1;
+  while (static_cast<double>((1ull << bits) - 1ull) <= cells_axis + 4.0) bits++;
+  const size_t m_ent = n * 8;  // anchor entries: eight per point, real ones at the first point of each cell
+  CU(ctx->keys_in.reserve(m_ent * sizeof(uint64_t)));
+  CU(ctx->keys_out.reserve(m_ent * sizeof(uint64_t)));
+  CU(ctx->vals_in.reserve(m_ent * sizeof(uint32_t)));
+  CU(ctx->pre_vals_out.reserve(m_ent * sizeof(uint32_t)));
+  CU(ctx->pre_heads.reserve(n * sizeof(uint32_t)));
+  CU(ctx->grid_pts.reserve(n * sizeof(float4)));
   CU(ctx->grid_pending.reserve(2 * sizeof(uint32_t)));
   size_t tb = 0;
-  CU(sort_pairs_u64_u32(nullptr, tb, ctx->keys_in.as<uint64_t>(), ctx->keys_out.as<uint64_t>(), ctx->vals_in.as<uint32_t>(), ctx->pre_vals_out.as<uint32_t>(), n_ent,
-                        ctx->stream));
+  CU(sort_pairs_u64_u32_bits(nullptr, tb, ctx->keys_in.as<uint64_t>(), ctx->keys_out.as<uint64_t>(), ctx->vals_in.as<uint32_t>(), ctx->pre_vals_out.as<uint32_t>(),
+                             m_ent, 3 * bits, ctx->stream));
   CU(ctx->sort_temp.reserve(tb));
-  uint32_t* d_distinct = ctx->grid_pending.as<uint32_t>();  // the two pending counters double as scratch during construction
-  CU(launch_grid_sort(ctx->tgt_pts.as<float4>(), static_cast<uint32_t>(n), g, ctx->keys_in.as<uint64_t>(), ctx->keys_out.as<uint64_t>(),
-                      ctx->vals_in.as<uint32_t>(), ctx->pre_vals_out.as<uint32_t>(), ctx->sort_temp.p, tb, d_distinct, ctx->grid_curve_order, ctx->stream));
+  uint32_t* d_counters = ctx->grid_pending.as<uint32_t>();  // the two pending counters double as scratch during construction
+  CU(launch_grid_build(ctx->tgt_pts.as<float4>(), static_cast<uint32_t>(n), g, bits, ctx->keys_in.as<uint64_t>(), ctx->keys_out.as<uint64_t>(),
+                       ctx->vals_in.as<uint32_t>(), ctx->pre_vals_out.as<uint32_t>(), ctx->sort_temp.p, tb, ctx->grid_pts.as<float4>(), ctx->pre_heads.as<uint32_t>(),
+                       d_counters, ctx->stream));
   ctx->pending_clean = false;  // the two counters of the construction live in the pending counters
-  uint32_t counters[2] = {0, 0};  // runs (= lists), longest run
-  CU(cudaMemcpyAsync(counters, d_distinct, sizeof(counters), cudaMemcpyDeviceToHost, ctx->stream));
+  uint32_t counters[2] = {0, 0};  // distinct anchors (= non-empty blocks), largest block
+  CU(cudaMemcpyAsync(counters, d_counters, sizeof(counters), cudaMemcpyDeviceToHost, ctx->stream));
   CU(cudaStreamSynchronize(ctx->stream));
-  const uint32_t distinct = counters[0], max_list = counters[1];
-  ctx->launches += 4;
-  if (ctx->debug_pending) std::fprintf(stderr, "[sgb] grid front end: cell %.4g, %u distinct lists, longest %u points\n", cell, distinct, max_list);
-  if (max_list > kGridMaxList) return 0;  // degenerate density (see kGridMaxList): the tree search alone stays exact and bounded
+  const uint32_t distinct = counters[0], max_block = counters[1];
+  ctx->launches += 7;
   uint32_t capacity = 1024;
   while (capacity < 2ull * distinct) capacity <<= 1;  // load factor <= 1/2
+  if (ctx->debug_pending)
+    std::fprintf(stderr, "[sgb] grid front end: cell %.9g (origin %a %a %a, inv_cell %a), %d key bits, %u blocks, largest block %u points, %.1f B/point%s\n", cell,
+                 g.origin[0], g.origin[1], g.origin[2], g.inv_cell, 3 * bits, distinct, max_block,
+                 (16.0 * static_cast<double>(n) + static_cast<double>(capacity) * sizeof(GridSlot)) / static_cast<double>(n),
+                 max_block > kGridMaxList ? ", dropped" : "");
+  if (max_block > kGridMaxList) return 0;  // degenerate density (see kGridMaxList): the tree search alone stays exact and bounded
+  // one slot per non-empty block
   CU(ctx->grid_table.reserve(static_cast<size_t>(capacity) * sizeof(GridSlot)));
-  // lists are stored as pair records (two points each, sgb_grid.cuh): a list of odd length carries one pad
-  CU(ctx->grid_pts.reserve((n_ent + distinct + 2) * sizeof(float4)));
-  CU(launch_grid_fill(ctx->keys_out.as<uint64_t>(), ctx->pre_vals_out.as<uint32_t>(), ctx->tgt_pts.as<float4>(), static_cast<uint32_t>(n_ent), ctx->vals_in.as<uint32_t>(),
-                      ctx->keys_in.as<uint32_t>(), ctx->sort_temp.p, tb, ctx->grid_pts.as<float4>(), ctx->grid_table.as<GridSlot>(), capacity, ctx->grid_curve_order,
-                      ctx->stream));
-  ctx->launches += 5;
+  CU(launch_grid_fill(ctx->keys_out.as<uint64_t>(), ctx->pre_vals_out.as<uint32_t>(), static_cast<uint32_t>(m_ent), ctx->pre_heads.as<uint32_t>(), bits,
+                      ctx->grid_table.as<GridSlot>(), capacity, ctx->stream));
+  ctx->launches += 2;
   for (int a = 0; a < 3; a++) ctx->grid_origin[a] = g.origin[a];
   ctx->grid_inv_cell = g.inv_cell;
   ctx->grid_settle_d2 = g.settle_d2;

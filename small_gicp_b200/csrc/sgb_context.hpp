@@ -90,7 +90,7 @@ struct sgb_ctx {
   sgb::DevBuf pre_boxes;
   size_t n_pnodes = 0;      // packet records of the current target tree
   // uniform-grid front end of the search (sgb_grid.cu)
-  bool use_grid = true, grid_ready = false;  // the front end holds 2 x 2 x 2 block lists (one lookup per query)
+  bool use_grid = true, grid_ready = false;  // the front end holds the cell-ordered points + block table (one lookup per query)
   sgb::DevBuf grid_pts, grid_table, grid_state, grid_spacing, grid_pending;  // grid_pending: [0], [1] = alternating counters, [2..] = pending query positions
   sgb::DevBuf grid_pending_q;  // parallel to the list: transformed query + squared distance of the probe's best candidate
   bool use_ring = true, debug_pending = false;  // profiling switches (sgb_create)
@@ -104,7 +104,6 @@ struct sgb_ctx {
   bool chunk_lists_clean = false;
   uint32_t class_fallback_pct = 85;  // more than this share of the chunks listed (pending lanes almost everywhere): curve order instead of the lists
   float class_wide_cells = 2.0f;     // search radius (in cells) from which a chunk counts as wide
-  bool grid_curve_order = true;  // block lists laid out along a Morton curve (profiling switch SGB_GRID_ORDER=0: raster order of the packed coordinates)
   bool kd_smem_refine = true;    // subtrees of <= 2048 points refined in shared memory by one launch (profiling switch SGB_KD_SMEM=0: one radix sort per level)
   bool error_pipelined = true;   // Reduction::error through the factor kernel's cp.async operand pipeline (profiling switch SGB_ERROR_PIPE=0: plain kernel)
   bool tma_leaf = false;         // profiling switch SGB_TMA_LEAF=1 (A/B of the north-star's TMA leaf staging)

@@ -5,9 +5,11 @@
 // spacing away.  The 2 x 2 x 2 block of grid cells (cell edge c) anchored at floor(u - 1/2) covers the cube
 // [q - c/2, q + c/2]^3, i.e. it holds EVERY target point within c/2 of q: if the closest point of the block is within c/2
 // it is the exact nearest neighbour and the query is finished -- no tree walk, no dependent pointer chasing.
-// BLOCK LISTS: every target point is stored under the eight blocks that contain its cell, so a block is ONE hash lookup and ONE
-// contiguous run of points (grid_probe_blocks_kernel); 8x the point storage buys the removal of seven lookups and of divergent per-cell
-// scans.  The runs are stored as 32-byte PAIR RECORDS (sgb_grid.cuh: GridPair): two points per sector.
+// CELL ORDER + BLOCK TABLE: the target is held once more, sorted by cell in raster order (x fastest), one float4 per point
+// (x, y, z, leaf position).  In that order the block anchored at (x, y, z) is exactly FOUR contiguous runs, one per (y, z) row pair,
+// each run being cells x and x + 1; a table slot per non-empty block (one 32-byte sector: sgb_kernels.h GridSlot) holds the four
+// runs, so a block is ONE hash lookup and four independent scans (grid_probe_blocks_kernel).  Every point is stored once (16 B)
+// and the blocks of neighbouring queries share their points in L2.
 // Queries the probe cannot settle (nothing within c/2: misaligned first iterations, holes, outliers) are appended to a
 // compact pending list -- with the best candidate found so far as an upper bound -- and finished exactly by packet_search_kernel:
 //   * few of them: a warp per query (pending_search_body, sgb_grid.cuh): ring search over the 27 blocks at stride 2 around the query
@@ -16,7 +18,6 @@
 // Which of the two runs is decided on the device from the pending counter.  Results are identical to a pure tree search
 // (exact ties aside; tests/test_gpu_parity.py::test_search_structures_agree).
 #include <cfloat>
-#include <cstdlib>
 #include <cub/device/device_radix_sort.cuh>
 
 #include "sgb_device.cuh"
@@ -25,131 +26,129 @@
 
 namespace sgb {
 
-// Morton (Z-order) code of the three 21-bit offset coordinates: the ORDER in which the lists are laid out in memory.  The table is keyed
-// by the plain packed coordinates (grid_key); only the sort uses the curve, so that the lists a warp of Hilbert-ordered queries needs --
-// a compact patch of ~11 neighbouring blocks -- are neighbours in memory too (DRAM pages, L2 sectors, TLB) instead of being strung along
-// x only (it matters most for the probe at 10M points and more).
-__device__ __forceinline__ uint64_t grid_spread21(uint64_t x) {
-  x &= 0x1fffffull;
-  x = (x | x << 32) & 0x1f00000000ffffull;
-  x = (x | x << 16) & 0x1f0000ff0000ffull;
-  x = (x | x << 8) & 0x100f00f00f00f00full;
-  x = (x | x << 4) & 0x10c30c30c30c30c3ull;
-  x = (x | x << 2) & 0x1249249249249249ull;
-  return x;
+// Construction sorts by a COMPACT raster key: B bits per axis (build_grid picks B from the number of cells along the widest axis),
+// coordinate + 2, x in the lowest bits -- the same order as grid_key, in 3 B bits instead of 63, so the radix sorts make fewer passes.
+// All-ones (grid_sort_pad) is never a real cell or anchor: it pads the anchor entries of points that do not start a cell.
+__device__ __forceinline__ uint64_t grid_sort_key(int ix, int iy, int iz, int bits) {
+  return static_cast<uint64_t>(ix + 2) | (static_cast<uint64_t>(iy + 2) << bits) | (static_cast<uint64_t>(iz + 2) << (2 * bits));
 }
-__device__ __forceinline__ uint64_t grid_compact21(uint64_t x) {
-  x &= 0x1249249249249249ull;
-  x = (x | x >> 2) & 0x10c30c30c30c30c3ull;
-  x = (x | x >> 4) & 0x100f00f00f00f00full;
-  x = (x | x >> 8) & 0x1f0000ff0000ffull;
-  x = (x | x >> 16) & 0x1f00000000ffffull;
-  x = (x | x >> 32) & 0x1fffffull;
-  return x;
+__device__ __forceinline__ void grid_sort_coords(uint64_t k, int bits, int& ix, int& iy, int& iz) {
+  const uint64_t m = (1ull << bits) - 1ull;
+  ix = static_cast<int>(k & m) - 2;
+  iy = static_cast<int>((k >> bits) & m) - 2;
+  iz = static_cast<int>((k >> (2 * bits)) & m) - 2;
 }
-__device__ __forceinline__ uint64_t grid_order_key(int ix, int iy, int iz, bool curve) {
-  if (!curve) return grid_key(ix, iy, iz);
-  return grid_spread21(static_cast<uint32_t>(ix + (1 << 20))) | (grid_spread21(static_cast<uint32_t>(iy + (1 << 20))) << 1) |
-         (grid_spread21(static_cast<uint32_t>(iz + (1 << 20))) << 2);
-}
-/// sort key -> table key (packed coordinates)
-__device__ __forceinline__ uint64_t grid_table_key(uint64_t k, bool curve) {
-  if (!curve) return k;
-  return grid_compact21(k) | (grid_compact21(k >> 1) << 21) | (grid_compact21(k >> 2) << 42);
-}
+__device__ __forceinline__ uint64_t grid_sort_pad(int bits) { return (1ull << (3 * bits)) - 1ull; }
 
-// cell key of every target point (leaf-ordered, centred FP32); value = leaf position.
-// BLOCKS: every point is entered under the eight 2 x 2 x 2 cell blocks that contain its cell (block anchor = lowest cell),
-// so that a query finds every point of the block around it in ONE contiguous run (8x the points, one lookup, one loop).
-__global__ void grid_keys_kernel(const float4* __restrict__ pts, uint32_t n, GridParams g, uint64_t* keys, uint32_t* vals, bool curve) {
-  const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
-  const uint32_t i = t >> 3, o = t & 7u;
+// cell key of every target point (leaf-ordered, centred FP32); value = leaf position
+__global__ void grid_cell_keys_kernel(const float4* __restrict__ pts, uint32_t n, GridParams g, int bits, uint64_t* keys, uint32_t* vals) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   const float4 p = pts[i];
   const int ix = __float2int_rd((p.x - g.origin[0]) * g.inv_cell), iy = __float2int_rd((p.y - g.origin[1]) * g.inv_cell),
             iz = __float2int_rd((p.z - g.origin[2]) * g.inv_cell);
-  keys[t] = grid_order_key(ix - static_cast<int>(o & 1u), iy - static_cast<int>((o >> 1) & 1u), iz - static_cast<int>(o >> 2), curve);
-  vals[t] = i;
+  keys[i] = grid_sort_key(ix, iy, iz, bits);
+  vals[i] = i;
 }
 
-// after the sort: one table entry per run of equal keys, and the run's points as PAIR RECORDS (sgb_grid.cuh: GridPair).
-// pass 1 (heads): length of every run -> its number of records at the head's position (0 elsewhere); counters[0] = number of runs
-// (sizes the hash table and, with m, the record array), counters[1] = longest run
-__global__ void grid_heads_kernel(const uint64_t* __restrict__ keys, uint32_t m, uint32_t* pairs, uint32_t* counters) {
+// after the (stable) sort: the points in cell order -- within a cell in ascending leaf position -- and, at position j, the eight
+// anchor entries of the cell that starts at j: every cell c is part of the blocks anchored at c - o, o in {0, 1}^3, in run
+// r = oy + 2 oz of each (value 4 j + r).  cnt[j] = points of that cell (measured up to kGridMaxList + 1: beyond it build_grid drops
+// the front end anyway).  Positions that start no cell write eight pads.
+__global__ void grid_cell_heads_kernel(const uint64_t* __restrict__ keys, const uint32_t* __restrict__ leaf_pos, const float4* __restrict__ leaf_pts, uint32_t n,
+                                       int bits, float4* grid_pts, uint32_t* cnt, uint64_t* akeys, uint32_t* avals) {
+  const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= n) return;
+  const uint32_t l = leaf_pos[j];
+  const float4 p = leaf_pts[l];
+  grid_pts[j] = make_float4(p.x, p.y, p.z, __uint_as_float(l));
+  const uint64_t k = keys[j];
+  if (j != 0 && keys[j - 1] == k) {
+#pragma unroll
+    for (uint32_t o = 0; o < 8u; o++) {
+      akeys[8u * j + o] = grid_sort_pad(bits);
+      avals[8u * j + o] = 0u;
+    }
+    return;
+  }
+  uint32_t c = 1;
+  while (j + c < n && c <= kGridMaxList && keys[j + c] == k) c++;
+  cnt[j] = c;
+  int ix, iy, iz;
+  grid_sort_coords(k, bits, ix, iy, iz);
+#pragma unroll
+  for (uint32_t o = 0; o < 8u; o++) {
+    akeys[8u * j + o] = grid_sort_key(ix - static_cast<int>(o & 1u), iy - static_cast<int>((o >> 1) & 1u), iz - static_cast<int>(o >> 2), bits);
+    avals[8u * j + o] = 4u * j + ((o >> 1) & 3u);
+  }
+}
+
+// after sorting the anchor entries (pads last): the first entry of every distinct anchor adds up its block (at most 8 cells);
+// counters[0] = distinct anchors (sizes the table), counters[1] = largest block (build_grid drops the front end beyond kGridMaxList)
+__global__ void grid_anchor_heads_kernel(const uint64_t* __restrict__ akeys, const uint32_t* __restrict__ avals, uint32_t m, const uint32_t* __restrict__ cnt,
+                                         int bits, uint32_t* counters) {
   const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-  uint32_t np = 0;
   bool head = false;
   if (i < m) {
-    const uint64_t k = keys[i];
-    head = i == 0 || keys[i - 1] != k;
+    const uint64_t k = akeys[i];
+    head = k != grid_sort_pad(bits) && (i == 0 || akeys[i - 1] != k);
     if (head) {
-      uint32_t cnt = 1;
-      // (a run longer than the front end accepts is only measured up to the limit: build_grid drops the grid before anything reads the records)
-      while (i + cnt < m && cnt <= kGridMaxList && keys[i + cnt] == k) cnt++;
-      np = (cnt + 1u) >> 1;
-      atomicMax(counters + 1, cnt);  // longest list: build_grid drops the front end when one query would have to scan thousands of points
+      uint32_t total = 0;
+      for (uint32_t e = i; e < m && akeys[e] == k; e++) total += cnt[avals[e] >> 2];
+      atomicMax(counters + 1, total);
     }
-    pairs[i] = np;
   }
   const unsigned b = __ballot_sync(0xffffffffu, head);
   if ((threadIdx.x & 31u) == 0 && b) atomicAdd(counters, static_cast<uint32_t>(__popc(b)));
 }
-// pass 2 (after an exclusive scan of `pairs` -> first record of every run): the head of a run writes its records -- two points per
-// record, components interleaved; an odd run is padded with a point at infinity that can never be nearest -- and claims the table slot
-__global__ void grid_fill_kernel(const uint64_t* __restrict__ keys, const uint32_t* __restrict__ leaf_pos, const float4* __restrict__ leaf_pts, uint32_t m,
-                                 const uint32_t* __restrict__ pair_start, GridPair* grid_pairs, GridSlot* table, uint32_t mask, bool curve) {
+
+// the first entry of every distinct anchor writes its slot: run r holds the cells with ox = 0 then ox = 1 (adjacent in raster
+// order, so the run starts at the first point of whichever is non-empty and counts both)
+__global__ void grid_fill_kernel(const uint64_t* __restrict__ akeys, const uint32_t* __restrict__ avals, uint32_t m, const uint32_t* __restrict__ cnt, int bits,
+                                 GridSlot* table, uint32_t mask) {
   const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= m) return;
-  const uint64_t k = keys[i];
-  if (i != 0 && keys[i - 1] == k) return;
-  uint32_t cnt = 1;
-  while (i + cnt < m && keys[i + cnt] == k) cnt++;
-  const uint32_t first = pair_start[i];
-  for (uint32_t e = 0; e < cnt; e += 2u) {
-    const uint32_t l0 = leaf_pos[i + e];
-    const float4 p0 = leaf_pts[l0];
-    float4 p1 = make_float4(kGridPadCoord, kGridPadCoord, kGridPadCoord, 0.f);
-    uint32_t l1 = kNone;
-    if (e + 1u < cnt) {
-      l1 = leaf_pos[i + e + 1u];
-      p1 = leaf_pts[l1];
-    }
-    GridPair r;
-    r.a = make_float4(p0.x, p1.x, p0.y, p1.y);
-    r.b = make_float4(p0.z, p1.z, __uint_as_float(l0), __uint_as_float(l1));
-    grid_pairs[first + (e >> 1)] = r;
+  const uint64_t k = akeys[i];
+  if (k == grid_sort_pad(bits) || (i != 0 && akeys[i - 1] == k)) return;
+  uint32_t start[4] = {~0u, ~0u, ~0u, ~0u}, count[4] = {0u, 0u, 0u, 0u};
+  for (uint32_t e = i; e < m && akeys[e] == k; e++) {
+    const uint32_t v = avals[e], s = v >> 2, r = v & 3u;
+    start[r] = min(start[r], s);
+    count[r] += cnt[s];
   }
-  const uint64_t tk = grid_table_key(k, curve);
-  uint32_t slot = grid_hash_of_key(tk) & mask;
+  int ix, iy, iz;
+  grid_sort_coords(k, bits, ix, iy, iz);
+  const unsigned long long tk = grid_key(ix, iy, iz);
+  uint32_t slot = grid_hash(ix, iy, iz) & mask;
   for (;;) {
-    const unsigned long long prev = atomicCAS(reinterpret_cast<unsigned long long*>(&table[slot].key), ~0ull, static_cast<unsigned long long>(tk));
+    const unsigned long long prev = atomicCAS(&table[slot].key, ~0ull, tk);
     if (prev == ~0ull) break;
     slot = (slot + 1u) & mask;
   }
-  table[slot].start = first;  // in records
-  table[slot].count = cnt;    // in points
+  uint4* w = reinterpret_cast<uint4*>(&table[slot]);
+  // (the key half of the first 16 bytes is already in place; an empty run keeps start 0)
+  w[0].z = count[0] ? start[0] : 0u;
+  w[0].w = count[1] ? start[1] : 0u;
+  w[1] = make_uint4(count[2] ? start[2] : 0u, count[3] ? start[3] : 0u, count[0] | (count[1] << 16), count[2] | (count[3] << 16));
 }
 
 __global__ void grid_table_init_kernel(GridSlot* table, uint32_t capacity) {
   const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < capacity) {
-    table[i].key = ~0ull;
-    table[i].start = 0u;
-    table[i].count = 0u;
+    uint4* w = reinterpret_cast<uint4*>(&table[i]);
+    w[0] = make_uint4(~0u, ~0u, 0u, 0u);
+    w[1] = make_uint4(0u, 0u, 0u, 0u);
   }
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// probe, block lists: the block anchored at floor(u - 1/2) covers [q - c/2, q + c/2]^3; one lookup, one contiguous scan
+// probe: the block anchored at floor(u - 1/2) covers [q - c/2, q + c/2]^3; one lookup, then its four contiguous runs
 // ---------------------------------------------------------------------------------------------------------------
-// UNROLL pairs of the scan loop are in flight per thread (2: 32 registers = 8 CTAs of 256 threads = full occupancy);
-// PREFETCH: the whole list is requested into L2 as soon as its table slot is known.  MIN_CTAS / UNROLL / PREFETCH other than the defaults
-// exist in the profiling library only (SGB_PROBE_CTAS, SGB_PROBE_UNROLL, SGB_PROBE_PREFETCH).
-template <int MIN_CTAS, int UNROLL = 2, bool PREFETCH = true>
-__global__ void __launch_bounds__(256, MIN_CTAS) grid_probe_blocks_kernel(const __grid_constant__ LinParams P, const GridPair* __restrict__ grid_pairs,
-                                                               const GridSlot* __restrict__ table, uint32_t mask, GridParams g, uint8_t* state,
-                                                               uint32_t* pending_count, uint32_t* pending_list, float4* pending_q, uint32_t* next_count,
-                                                               ChunkClasses cc) {
+// 32 registers, no spills: 8 CTAs of 256 threads = full occupancy.
+__global__ void __launch_bounds__(256, 8) grid_probe_blocks_kernel(const __grid_constant__ LinParams P, const float4* __restrict__ grid_pts,
+                                                                   const GridSlot* __restrict__ table, uint32_t mask, GridParams g, uint8_t* state,
+                                                                   uint32_t* pending_count, uint32_t* pending_list, float4* pending_q, uint32_t* next_count,
+                                                                   ChunkClasses cc) {
   const uint32_t gi = blockIdx.x * blockDim.x + threadIdx.x;
   const bool in_range = gi < P.src.n;
   if (gi == 0u) *next_count = 0u;  // the counter of the NEXT linearize (two counters alternate: no memset between launches)
@@ -165,42 +164,34 @@ __global__ void __launch_bounds__(256, MIN_CTAS) grid_probe_blocks_kernel(const 
   const float fx = static_cast<float>(R[0] * sx + R[1] * sy + R[2] * sz + tpx);
   const float fy = static_cast<float>(R[3] * sx + R[4] * sy + R[5] * sz + tpy);
   const float fz = static_cast<float>(R[6] * sx + R[7] * sy + R[8] * sz + tpz);
-  float best_d = P.max_dist_sq;
-  uint32_t best = kNone;
   const float ax = floorf((fx - g.origin[0]) * g.inv_cell - 0.5f), ay = floorf((fy - g.origin[1]) * g.inv_cell - 0.5f),
               az = floorf((fz - g.origin[2]) * g.inv_cell - 0.5f);
   // queries far outside the target's box cannot be settled anyway; clamping keeps the integer cell coordinates in range
   const int bx = static_cast<int>(fminf(fmaxf(ax, -1e5f), 1e5f)), by = static_cast<int>(fminf(fmaxf(ay, -1e5f), 1e5f)),
             bz = static_cast<int>(fminf(fmaxf(az, -1e5f), 1e5f));
-  const uint2 e = grid_lookup(table, mask, bx, by, bz);
+  const GridRuns e = grid_lookup(table, mask, bx, by, bz);
+  // The four runs are scanned as one sequence (run r starts at position p_r = count[0] + ... + count[r - 1], and o_r maps a position
+  // of run r to its point), unrolled by four so that four independent loads are in flight per thread.  The squared distance is
+  // fma(dz, dz, fma(dy, dy, dx * dx)) in FP32 with round-to-nearest, and the candidate is the lexicographic minimum of (distance, leaf
+  // position) -- within one block the same point the scan of a leaf-position-ordered list with a strict < keeps.
+  uint64_t best_key = grid_cand_key(P.max_dist_sq, 0u);
   {
-    // The list is a contiguous run of ceil(e.y / 2) PAIR RECORDS (32 B: two points, components interleaved), read by two 128-bit
-    // loads of one sector (load_pair).  The squared distance is fma(dz, dz, fma(dy, dy, dx * dx)) in FP32 with round-to-nearest for
-    // each point, so the candidate and its distance are bit-identical to a packed f32x2 evaluation of the same expression.
-    const GridPair* __restrict__ rec = grid_pairs + e.x;
-    const uint32_t npairs = (e.y + 1u) >> 1;
-    // pull all of its lines into L2 at once (the scan would otherwise pay one DRAM round trip per batch of loads)
-    const char* lp = reinterpret_cast<const char*>(rec);
-    const uint32_t bytes = npairs * 32u;
-    if (PREFETCH)
-      for (uint32_t off = 128u; off < bytes; off += 128u) asm volatile("prefetch.global.L2 [%0];" ::"l"(lp + off));
-    if (PREFETCH && bytes > 128u) asm volatile("prefetch.global.L2 [%0];" ::"l"(lp + bytes - 32u));  // last line of a run that is not 128 B aligned
-#pragma unroll UNROLL
-    for (uint32_t j = 0; j < npairs; j++) {
-      const GridPair t = load_pair(rec + j);
-      const float dx0 = __fsub_rn(t.a.x, fx), dy0 = __fsub_rn(t.a.z, fy), dz0 = __fsub_rn(t.b.x, fz);
-      const float dx1 = __fsub_rn(t.a.y, fx), dy1 = __fsub_rn(t.a.w, fy), dz1 = __fsub_rn(t.b.y, fz);
-      const float d0 = __fmaf_rn(dz0, dz0, __fmaf_rn(dy0, dy0, __fmul_rn(dx0, dx0)));
-      const float d1 = __fmaf_rn(dz1, dz1, __fmaf_rn(dy1, dy1, __fmul_rn(dx1, dx1)));
-      if (d0 < best_d) {  // first point of the pair first: ties keep the scan order
-        best_d = d0;
-        best = __float_as_uint(t.b.z);
-      }
-      if (d1 < best_d) {  // (the pad of an odd list sits at 1e18: ~3e36, never nearest)
-        best_d = d1;
-        best = __float_as_uint(t.b.w);
-      }
+    const uint32_t p1 = e.count[0], p2 = p1 + e.count[1], p3 = p2 + e.count[2], total = p3 + e.count[3];
+    const uint32_t o0 = e.start[0], o1 = e.start[1] - p1, o2 = e.start[2] - p2, o3 = e.start[3] - p3;
+#pragma unroll 4
+    for (uint32_t j = 0; j < total; j++) {
+      const uint32_t idx = j + (j >= p3 ? o3 : j >= p2 ? o2 : j >= p1 ? o1 : o0);
+      const float4 t = __ldg(&grid_pts[idx]);
+      const float dx = __fsub_rn(t.x, fx), dy = __fsub_rn(t.y, fy), dz = __fsub_rn(t.z, fz);
+      const uint64_t key = grid_cand_key(__fmaf_rn(dz, dz, __fmaf_rn(dy, dy, __fmul_rn(dx, dx))), __float_as_uint(t.w));
+      best_key = key < best_key ? key : best_key;
     }
+  }
+  float best_d = P.max_dist_sq;
+  uint32_t best = kNone;
+  if (best_key != grid_cand_key(P.max_dist_sq, 0u)) {
+    best_d = __uint_as_float(static_cast<uint32_t>(best_key >> 32));
+    best = static_cast<uint32_t>(best_key);
   }
   const bool settled = best != kNone && best_d <= g.settle_d2;
   if (!settled && P.use_prev) {  // keep the better of (grid candidate, previous correspondence) as the tree search's seed
@@ -295,28 +286,27 @@ cudaError_t launch_grid_spacing(const float4* pnodes, uint32_t n_inner, float* o
   return cudaGetLastError();
 }
 
-cudaError_t launch_grid_sort(const float4* leaf_pts, uint32_t n, const GridParams& g, uint64_t* keys_in, uint64_t* keys_out, uint32_t* vals_in, uint32_t* vals_out,
-                             void* sort_temp, size_t sort_temp_bytes, uint32_t* d_counters, bool curve, cudaStream_t st) {
+cudaError_t launch_grid_build(const float4* leaf_pts, uint32_t n, const GridParams& g, int bits, uint64_t* keys_a, uint64_t* keys_b, uint32_t* vals_a, uint32_t* vals_b,
+                              void* sort_temp, size_t sort_temp_bytes, float4* grid_pts, uint32_t* cnt, uint32_t* d_counters, cudaStream_t st) {
+  const int end_bit = 3 * bits;
   const uint32_t m = n * 8u;
-  grid_keys_kernel<<<(m + 255u) / 256u, 256, 0, st>>>(leaf_pts, n, g, keys_in, vals_in, curve);
-  cudaError_t e = cub::DeviceRadixSort::SortPairs(sort_temp, sort_temp_bytes, keys_in, keys_out, vals_in, vals_out, static_cast<int>(m), 0, 63, st);
+  grid_cell_keys_kernel<<<(n + 255u) / 256u, 256, 0, st>>>(leaf_pts, n, g, bits, keys_a, vals_a);
+  cudaError_t e = cub::DeviceRadixSort::SortPairs(sort_temp, sort_temp_bytes, keys_a, keys_b, vals_a, vals_b, static_cast<int>(n), 0, end_bit, st);
+  if (e != cudaSuccess) return e;
+  // the cell-sorted keys / positions are read from keys_b / vals_b; the anchor entries go to keys_a / vals_a and are sorted back into b
+  grid_cell_heads_kernel<<<(n + 255u) / 256u, 256, 0, st>>>(keys_b, vals_b, leaf_pts, n, bits, grid_pts, cnt, keys_a, vals_a);
+  e = cub::DeviceRadixSort::SortPairs(sort_temp, sort_temp_bytes, keys_a, keys_b, vals_a, vals_b, static_cast<int>(m), 0, end_bit, st);
   if (e != cudaSuccess) return e;
   e = cudaMemsetAsync(d_counters, 0, 2 * sizeof(uint32_t), st);
   if (e != cudaSuccess) return e;
-  grid_heads_kernel<<<(m + 255u) / 256u, 256, 0, st>>>(keys_out, m, vals_in, d_counters);  // the sort's value input is free again: records per run
+  grid_anchor_heads_kernel<<<(m + 255u) / 256u, 256, 0, st>>>(keys_b, vals_b, m, cnt, bits, d_counters);
   return cudaGetLastError();
 }
 
-cudaError_t launch_grid_fill(const uint64_t* keys_sorted, const uint32_t* vals_sorted, const float4* leaf_pts, uint32_t m, const uint32_t* pairs, uint32_t* pair_start,
-                             void* scan_temp, size_t scan_temp_bytes, float4* grid_pts, GridSlot* table, uint32_t capacity, bool curve, cudaStream_t st) {
-  size_t need = 0;
-  cudaError_t e = exclusive_sum_u32(nullptr, need, pairs, pair_start, m, st);
-  if (e != cudaSuccess) return e;
-  if (need > scan_temp_bytes) return cudaErrorInvalidValue;  // (the radix sort's scratch, which the caller hands over, is far larger)
-  e = exclusive_sum_u32(scan_temp, need, pairs, pair_start, m, st);
-  if (e != cudaSuccess) return e;
+cudaError_t launch_grid_fill(const uint64_t* akeys, const uint32_t* avals, uint32_t m, const uint32_t* cnt, int bits, GridSlot* table, uint32_t capacity,
+                             cudaStream_t st) {
   grid_table_init_kernel<<<(capacity + 255u) / 256u, 256, 0, st>>>(table, capacity);
-  grid_fill_kernel<<<(m + 255u) / 256u, 256, 0, st>>>(keys_sorted, vals_sorted, leaf_pts, m, pair_start, reinterpret_cast<GridPair*>(grid_pts), table, capacity - 1u, curve);
+  grid_fill_kernel<<<(m + 255u) / 256u, 256, 0, st>>>(akeys, avals, m, cnt, bits, table, capacity - 1u);
   return cudaGetLastError();
 }
 
@@ -324,24 +314,7 @@ cudaError_t launch_grid_probe(const LinParams& P, const float4* grid_pts, const 
                               uint32_t* pending_count, uint32_t* pending_list, float4* pending_q, uint32_t* next_count, const ChunkClasses& cc, cudaStream_t st) {
   // *pending_count must be zero on entry: the previous probe (or the context) cleared it
   const uint32_t grid = (P.src.n + 255u) / 256u;
-  const GridPair* pairs = reinterpret_cast<const GridPair*>(grid_pts);
-#ifdef SGB_PROFILING
-  static const int ctas = std::getenv("SGB_PROBE_CTAS") ? std::atoi(std::getenv("SGB_PROBE_CTAS")) : 5;
-  static const int unroll = std::getenv("SGB_PROBE_UNROLL") ? std::atoi(std::getenv("SGB_PROBE_UNROLL")) : 2;
-#define SGB_PROBE_VARIANT(C, U)                                                                                                                        \
-  if (ctas == C && unroll == U) {                                                                                                                      \
-    grid_probe_blocks_kernel<C, U><<<grid, 256, 0, st>>>(P, pairs, table, capacity - 1u, g, state, pending_count, pending_list, pending_q, next_count, cc); \
-    return cudaGetLastError();                                                                                                                         \
-  }
-  static const bool prefetch = !(std::getenv("SGB_PROBE_PREFETCH") && std::getenv("SGB_PROBE_PREFETCH")[0] == '0');
-  if (!prefetch) {
-    grid_probe_blocks_kernel<5, 2, false><<<grid, 256, 0, st>>>(P, pairs, table, capacity - 1u, g, state, pending_count, pending_list, pending_q, next_count, cc);
-    return cudaGetLastError();
-  }
-  SGB_PROBE_VARIANT(5, 1) SGB_PROBE_VARIANT(5, 3) SGB_PROBE_VARIANT(5, 4) SGB_PROBE_VARIANT(6, 1) SGB_PROBE_VARIANT(6, 2) SGB_PROBE_VARIANT(6, 3) SGB_PROBE_VARIANT(8, 2)
-#undef SGB_PROBE_VARIANT
-#endif
-  grid_probe_blocks_kernel<5><<<grid, 256, 0, st>>>(P, pairs, table, capacity - 1u, g, state, pending_count, pending_list, pending_q, next_count, cc);
+  grid_probe_blocks_kernel<<<grid, 256, 0, st>>>(P, grid_pts, table, capacity - 1u, g, state, pending_count, pending_list, pending_q, next_count, cc);
   return cudaGetLastError();
 }
 

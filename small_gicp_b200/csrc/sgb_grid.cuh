@@ -1,6 +1,6 @@
 // SPDX-License-Identifier: MIT
 // Device-side pieces of the grid front end that more than one kernel uses: the block-table lookup and the warp-per-query search of
-// the pending queries (ring phase over the block lists, then -- only beyond the ring's reach -- a warp-cooperative walk of the packet
+// the pending queries (ring phase over the block table, then -- only beyond the ring's reach -- a warp-cooperative walk of the packet
 // records).  The latter runs inside packet_search_kernel (sgb_kernels_packet.cu), which picks the regime from the probe's counter:
 // one launch for both, where round 1 launched two kernels of which one exited at once.
 #pragma once
@@ -13,22 +13,6 @@ namespace sgb {
 // in cell units carries < 1e-3 of rounding error
 constexpr float kGridSlack = 4e-3f;
 
-// One entry of a block list: TWO points in one 32-byte sector, components interleaved: a = (x0, x1, y0, y1), b = (z0, z1, leaf
-// position 0, leaf position 1).  A list with an odd number of points ends in a pad: coordinates kGridPadCoord (squared distance ~3e36:
-// farther than anything real, still finite), position kNone.
-struct __align__(32) GridPair {
-  float4 a, b;
-};
-constexpr float kGridPadCoord = 1e18f;
-
-// sm_90 has no 256-bit load: the record is two 128-bit read-only loads (LDG.E.128.CONSTANT) of the same sector
-__device__ __forceinline__ GridPair load_pair(const GridPair* p) {
-  GridPair r;
-  r.a = __ldg(&p->a);
-  r.b = __ldg(&p->b);
-  return r;
-}
-
 __device__ __forceinline__ uint64_t grid_key(int ix, int iy, int iz) {
   return (static_cast<uint64_t>(static_cast<uint32_t>(ix + (1 << 20)) & 0x1fffffu)) | (static_cast<uint64_t>(static_cast<uint32_t>(iy + (1 << 20)) & 0x1fffffu) << 21) |
          (static_cast<uint64_t>(static_cast<uint32_t>(iz + (1 << 20)) & 0x1fffffu) << 42);
@@ -38,28 +22,48 @@ __device__ __forceinline__ uint32_t grid_hash(int ix, int iy, int iz) {
   h ^= h >> 15;
   return h;
 }
-__device__ __forceinline__ uint32_t grid_hash_of_key(uint64_t k) {
-  const int ix = static_cast<int>(k & 0x1fffffu) - (1 << 20), iy = static_cast<int>((k >> 21) & 0x1fffffu) - (1 << 20),
-            iz = static_cast<int>((k >> 42) & 0x1fffffu) - (1 << 20);
-  return grid_hash(ix, iy, iz);
-}
 
-__device__ __forceinline__ uint2 grid_lookup(const GridSlot* __restrict__ table, uint32_t mask, int ix, int iy, int iz) {
+/// The four runs of one block (sgb_kernels.h: GridSlot); all counts zero when the block is empty.
+struct GridRuns {
+  uint32_t start[4], count[4];
+};
+
+/// One slot = one sector, read by two 128-bit loads issued together.
+__device__ __forceinline__ GridRuns grid_lookup(const GridSlot* __restrict__ table, uint32_t mask, int ix, int iy, int iz) {
   const uint64_t k = grid_key(ix, iy, iz);
   uint32_t slot = grid_hash(ix, iy, iz) & mask;
+  GridRuns r;
   for (;;) {
-    const uint4 e = __ldg(reinterpret_cast<const uint4*>(&table[slot]));
-    const uint64_t ek = static_cast<uint64_t>(e.x) | (static_cast<uint64_t>(e.y) << 32);
-    if (ek == k) return make_uint2(e.z, e.w);
-    if (ek == ~0ull) return make_uint2(0u, 0u);
+    const uint4* p = reinterpret_cast<const uint4*>(&table[slot]);
+    const uint4 a = __ldg(p), b = __ldg(p + 1);
+    const uint64_t ek = static_cast<uint64_t>(a.x) | (static_cast<uint64_t>(a.y) << 32);
+    if (ek == k) {
+      r.start[0] = a.z;
+      r.start[1] = a.w;
+      r.start[2] = b.x;
+      r.start[3] = b.y;
+      r.count[0] = b.z & 0xffffu;
+      r.count[1] = b.z >> 16;
+      r.count[2] = b.w & 0xffffu;
+      r.count[3] = b.w >> 16;
+      return r;
+    }
+    if (ek == ~0ull) {
+#pragma unroll
+      for (int j = 0; j < 4; j++) r.start[j] = r.count[j] = 0u;
+      return r;
+    }
     slot = (slot + 1u) & mask;
   }
 }
 
+/// Lexicographic minimum of (squared distance, leaf position): the key of a candidate is its distance's bits (non-negative floats
+/// order like their bits) above its leaf position.  Starting from (bits(bound), 0) only points strictly closer than the bound enter.
+__device__ __forceinline__ uint64_t grid_cand_key(float d, uint32_t pos) { return (static_cast<uint64_t>(__float_as_uint(d)) << 32) | pos; }
 
 // ---------------------------------------------------------------------------------------------------------------
 // Few pending queries (holes, outliers, borders: a few per mille to a few per cent, scattered): one WARP per query.
-// Ring phase first (block lists): 27 lookups in parallel, the lists scanned as one flattened run over all lanes, a
+// Ring phase first (block table): 27 lookups in parallel, their 108 runs scanned as one flattened run over all lanes, a
 // hardware min -- a handful of memory round trips.  Only if the ring's radius (2.5 cells) does not decide the query does
 // the warp walk the packet records: every step of a single walk is a dependent load, so a thread per query would be
 // pure latency; with a warp per query a leaf's points are fetched by one coalesced
@@ -80,7 +84,7 @@ __device__ __forceinline__ float grid_box_dist2(float qx, float qy, float qz, co
 struct RingParams {
   const uint32_t* list;     // pending list: source positions, [*count] entries
   const float4* q;          // parallel to it: transformed query (x, y, z) and the squared distance of the probe's best candidate (w)
-  const GridPair* grid_pairs;  // block lists (pair records)
+  const float4* grid_pts;   // target points in cell (raster) order: (x, y, z, leaf position)
   const GridSlot* table;    // block table (null: no ring phase, every pending query walks the tree)
   uint32_t mask;
   GridParams g;
@@ -101,13 +105,15 @@ __device__ __forceinline__ void pending_search_body(const LinParams& P, const fl
     float best_d = rec.w;
     uint32_t best = kNone;  // "nothing closer than the probe's candidate found (yet)"
     if (R.table) {
-      // Ring phase (block lists): the 3 x 3 x 3 blocks at stride 2 around the query's own block tile the cells
-      // [a - 2, a + 4)^3, i.e. they hold every target point within 2.5 cells of q.  One lookup and one list scan per lane,
-      // all 27 in parallel, then a warp min: a handful of memory round trips instead of the ~45 of a tree walk.
+      // Ring phase (block table): the 3 x 3 x 3 blocks at stride 2 around the query's own block tile the cells
+      // [a - 2, a + 4)^3, i.e. they hold every target point within 2.5 cells of q.  One lookup per lane, all 27 in parallel, their
+      // 4 runs each scanned together, then a warp min: a handful of memory round trips instead of the ~45 of a tree walk.
       const float ux = (qx - R.g.origin[0]) * R.g.inv_cell, uy = (qy - R.g.origin[1]) * R.g.inv_cell, uz = (qz - R.g.origin[2]) * R.g.inv_cell;
       const int ax = static_cast<int>(fminf(fmaxf(floorf(ux - 0.5f), -1e5f), 1e5f)), ay = static_cast<int>(fminf(fmaxf(floorf(uy - 0.5f), -1e5f), 1e5f)),
                 az = static_cast<int>(fminf(fmaxf(floorf(uz - 0.5f), -1e5f), 1e5f));
-      uint2 e = make_uint2(0u, 0u);
+      GridRuns e;
+#pragma unroll
+      for (int r = 0; r < 4; r++) e.start[r] = e.count[r] = 0u;
       if (lane < 27u) {
         const int bx = ax + 2 * (static_cast<int>(lane % 3u) - 1), by = ay + 2 * (static_cast<int>((lane / 3u) % 3u) - 1),
                   bz = az + 2 * (static_cast<int>(lane / 9u) - 1);
@@ -116,10 +122,11 @@ __device__ __forceinline__ void pending_search_body(const LinParams& P, const fl
         const float ez = fmaxf(fmaxf(static_cast<float>(bz) - uz, uz - static_cast<float>(bz + 2)) - kGridSlack, 0.0f);
         if ((ex * ex + ey * ey + ez * ez) * R.cell * R.cell < best_d) e = grid_lookup(R.table, R.mask, bx, by, bz);
       }
-      // The (typically ~9 non-empty) lists are scanned as ONE flattened run spread over all 32 lanes: point j of the
-      // concatenation (of pair records) goes to lane j mod 32, which finds its list by a shuffle binary search over the exclusive prefix
-      // sums of the counts.  A lane per list would walk up to ~40 points in dependent batches; this is ~7 loads per lane.
-      const uint32_t np = (e.y + 1u) >> 1;  // records of this lane's list (two points each)
+      // The (typically ~9 non-empty) blocks' up to 108 runs are scanned as ONE flattened run spread over all 32 lanes: point j of the
+      // concatenation goes to lane j mod 32, which finds the block by a shuffle binary search over the exclusive prefix sums of the
+      // blocks' sizes, then the run within it from the block's partial sums.  off[r] = start of run r minus the points before it.
+      const uint32_t p1 = e.count[0], p2 = p1 + e.count[1], p3 = p2 + e.count[2], np = p3 + e.count[3];
+      const uint32_t off0 = e.start[0], off1 = e.start[1] - p1, off2 = e.start[2] - p2, off3 = e.start[3] - p3;  // (mod 2^32)
       uint32_t incl = np;
 #pragma unroll
       for (int o = 1; o < 32; o <<= 1) {
@@ -127,39 +134,36 @@ __device__ __forceinline__ void pending_search_body(const LinParams& P, const fl
         if (lane >= static_cast<uint32_t>(o)) incl += t;
       }
       const uint32_t excl = incl - np, total = __shfl_sync(0xffffffffu, incl, 31);
-      float my_d = best_d;
-      uint32_t my_best = kNone;
+      const uint64_t bound = grid_cand_key(best_d, 0u);
+      uint64_t mine = bound;
 #pragma unroll 2
       for (uint32_t base = 0; base < total; base += 32u) {
         const uint32_t j = base + lane;
-        uint32_t owner = 0;  // largest lane whose exclusive prefix is <= j (empty lists share their successor's prefix and lose)
+        uint32_t owner = 0;  // largest lane whose exclusive prefix is <= j (empty blocks share their successor's prefix and lose)
 #pragma unroll
         for (uint32_t step = 16u; step >= 1u; step >>= 1) {
           const uint32_t cand = owner + step;
           const uint32_t ex = __shfl_sync(0xffffffffu, excl, cand & 31u);
           if (cand < 32u && ex <= j) owner = cand;
         }
-        const uint32_t st = __shfl_sync(0xffffffffu, e.x, owner), ex0 = __shfl_sync(0xffffffffu, excl, owner);
+        const uint32_t ex0 = __shfl_sync(0xffffffffu, excl, owner);
+        const uint32_t q1 = __shfl_sync(0xffffffffu, p1, owner), q2 = __shfl_sync(0xffffffffu, p2, owner), q3 = __shfl_sync(0xffffffffu, p3, owner);
+        const uint32_t o0 = __shfl_sync(0xffffffffu, off0, owner), o1 = __shfl_sync(0xffffffffu, off1, owner);
+        const uint32_t o2 = __shfl_sync(0xffffffffu, off2, owner), o3 = __shfl_sync(0xffffffffu, off3, owner);
         if (j < total) {
-          const GridPair t = load_pair(R.grid_pairs + st + (j - ex0));
-          const float dx0 = t.a.x - qx, dy0 = t.a.z - qy, dz0 = t.b.x - qz;
-          const float dx1 = t.a.y - qx, dy1 = t.a.w - qy, dz1 = t.b.y - qz;
-          const float d0 = dx0 * dx0 + dy0 * dy0 + dz0 * dz0, d1 = dx1 * dx1 + dy1 * dy1 + dz1 * dz1;
-          if (d0 < my_d) {
-            my_d = d0;
-            my_best = __float_as_uint(t.b.z);
-          }
-          if (d1 < my_d) {  // (a pad never is: ~3e36)
-            my_d = d1;
-            my_best = __float_as_uint(t.b.w);
-          }
+          const uint32_t local = j - ex0;
+          const uint32_t idx = local + (local >= q3 ? o3 : local >= q2 ? o2 : local >= q1 ? o1 : o0);
+          const float4 t = __ldg(&R.grid_pts[idx]);
+          const float dx = t.x - qx, dy = t.y - qy, dz = t.z - qz;
+          const uint64_t key = grid_cand_key(dx * dx + dy * dy + dz * dz, __float_as_uint(t.w));
+          mine = key < mine ? key : mine;
         }
       }
-      const uint32_t dbits = my_best != kNone ? __float_as_uint(my_d) : 0x7f800000u;
+      // warp minimum of (distance, leaf position): the smallest distance first, then the lowest position among the lanes holding it
+      const uint32_t dbits = mine != bound ? static_cast<uint32_t>(mine >> 32) : 0x7f800000u;
       const uint32_t dmin = __reduce_min_sync(0xffffffffu, dbits);
       if (dmin != 0x7f800000u) {
-        const unsigned who = __ballot_sync(0xffffffffu, dbits == dmin);
-        best = __shfl_sync(0xffffffffu, my_best, __ffs(who) - 1);
+        best = __reduce_min_sync(0xffffffffu, dbits == dmin ? static_cast<uint32_t>(mine) : kNone);
         best_d = __uint_as_float(dmin);
       }
       const float cover = (2.5f - kGridSlack) * R.cell;

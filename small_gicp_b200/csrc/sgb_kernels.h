@@ -85,15 +85,18 @@ struct GridParams {
   float inv_cell;   // 1 / cell edge
   float settle_d2;  // a candidate within this squared distance is provably the nearest neighbour ((cell/2 - margin)^2)
 };
-struct __align__(16) GridSlot {
-  unsigned long long key;  // packed cell coordinates, ~0 = empty
-  uint32_t start, count;   // run of the cell's points in the cell-ordered copy of the target
+/// One slot of the block table = one 32-byte sector: the 2 x 2 x 2 block anchored at cell (x, y, z) is, in the raster-ordered copy
+/// of the target, four contiguous runs -- run r = cells (x, y + (r & 1), z + (r >> 1)) and (x + 1, same y, same z).
+struct __align__(32) GridSlot {
+  unsigned long long key;  // packed anchor coordinates (grid_key), ~0 = empty
+  uint32_t start[4];       // first point of each run (cell-ordered copy)
+  uint16_t count[4];       // points of each run (a kept block holds at most kGridMaxList)
 };
 /// What the warp-per-query search of few pending queries needs (it runs inside packet_search_kernel; see sgb_grid.cuh)
 struct PendingParams {
   const uint32_t* list;    // pending list (source positions)
   const float4* q;         // parallel: transformed query + squared distance of the probe's best candidate
-  const float4* grid_pts;  // block lists (pair records, sgb_grid.cuh)
+  const float4* grid_pts;  // target points in cell (raster) order: (x, y, z, leaf position)
   const GridSlot* table;   // block table, or null: no ring phase
   uint32_t capacity;
   GridParams g;
@@ -103,14 +106,15 @@ struct PendingParams {
 cudaError_t launch_packet_search(const LinParams& P, const float4* pnodes, int grid, int max_depth, const uint8_t* settled, const uint32_t* pending_count,
                                  uint32_t min_pending, uint32_t* queue, uint32_t* queue_next, const ChunkClasses& cc, const PendingParams& pp, bool tma_leaf, cudaStream_t st);
 cudaError_t launch_grid_spacing(const float4* pnodes, uint32_t n_inner, float* out, cudaStream_t st);
-/// Block lists as PAIR RECORDS (sgb_grid.cuh: GridPair).  sort: keys of the 8 n entries, radix sort, then records per run at the run heads
-/// (into vals_in) and d_counters[0] = runs, [1] = longest run.  fill: exclusive scan (pairs -> pair_start), table, records.
-/// grid_pts must hold (m + runs) / 2 records of 32 B, i.e. (m + runs) float4.
-cudaError_t launch_grid_sort(const float4* leaf_pts, uint32_t n, const GridParams& g, uint64_t* keys_in, uint64_t* keys_out, uint32_t* vals_in, uint32_t* vals_out,
-                             void* sort_temp, size_t sort_temp_bytes, uint32_t* d_counters, bool curve, cudaStream_t st);
-cudaError_t launch_grid_fill(const uint64_t* keys_sorted, const uint32_t* vals_sorted, const float4* leaf_pts, uint32_t m, const uint32_t* pairs, uint32_t* pair_start,
-                             void* scan_temp, size_t scan_temp_bytes, float4* grid_pts, GridSlot* table, uint32_t capacity, bool curve, cudaStream_t st);
-/// longest list (points) the grid front end accepts: beyond it a single query's scan would dominate (a cluster of near-duplicate
+/// Cell-ordered points + block table (sgb_grid.cu), sorted by compact raster keys of 3 `bits` bits.  build: cell keys of the n
+/// leaf-ordered points, radix sort, the points in cell order into grid_pts (n float4), cell sizes into cnt (n), the eight block anchors
+/// of every cell (8 n entries, padded), radix sort; then d_counters[0] = distinct anchors, [1] = largest block (points).  keys_a / b and
+/// vals_a / b hold 8 n entries; the sorted anchors end in keys_b / vals_b.  fill: table of `capacity` slots from the sorted anchors.
+cudaError_t launch_grid_build(const float4* leaf_pts, uint32_t n, const GridParams& g, int bits, uint64_t* keys_a, uint64_t* keys_b, uint32_t* vals_a, uint32_t* vals_b,
+                              void* sort_temp, size_t sort_temp_bytes, float4* grid_pts, uint32_t* cnt, uint32_t* d_counters, cudaStream_t st);
+cudaError_t launch_grid_fill(const uint64_t* akeys, const uint32_t* avals, uint32_t m, const uint32_t* cnt, int bits, GridSlot* table, uint32_t capacity,
+                             cudaStream_t st);
+/// largest block (points, the sum of its four runs) the grid front end accepts: beyond it a single query's scan would dominate (a cluster of near-duplicate
 /// points, or a few far outliers stretching the box so that the cell-count bound inflates the cell) and the exact tree search alone is used
 constexpr uint32_t kGridMaxList = 2048;
 cudaError_t launch_grid_probe(const LinParams& P, const float4* grid_pts, const GridSlot* table, uint32_t capacity, const GridParams& g, uint8_t* state,

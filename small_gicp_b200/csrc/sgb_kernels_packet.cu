@@ -82,7 +82,7 @@ __global__ void __launch_bounds__(kLinBlock, MIN_CTAS) packet_search_kernel(cons
   __shared__ __align__(128) float4 s_leaf[TMA_LEAF ? kPktWarps : 1][32];  // TMA landing zone of the warp's current leaf
   __shared__ __align__(8) uint64_t s_bar[TMA_LEAF ? kPktWarps : 1];
   // Two regimes, picked from the probe's counter: FEW pending queries (holes, borders, outliers at an aligned pose) -> a warp per query
-  // (ring phase over the block lists, tree walk only beyond its reach: sgb_grid.cuh); MANY (a misaligned first iteration) -> the packet
+  // (ring phase over the block table, tree walk only beyond its reach: sgb_grid.cuh); MANY (a misaligned first iteration) -> the packet
   // walk below.  One launch serves both (two kernels, one of which exits at once, cost a launch per linearize).
   if (pending_count) {
     const uint32_t pc = *pending_count;
@@ -300,7 +300,7 @@ cudaError_t launch_packet_search(const LinParams& P, const float4* pnodes, int g
   RingParams ring;
   ring.list = pp.list;
   ring.q = pp.q;
-  ring.grid_pairs = reinterpret_cast<const GridPair*>(pp.grid_pts);
+  ring.grid_pts = pp.grid_pts;
   ring.table = pp.table;
   ring.mask = pp.capacity ? pp.capacity - 1u : 0u;
   ring.g = pp.g;
