@@ -188,6 +188,32 @@ int sgb_error_batch(sgb_ctx* ctx, const double* T_colmajor16xB, const uint8_t* a
  * target indices; SGB_NO_CORRESPONDENCE = rejected or never linearised. */
 int sgb_correspondences_batch(sgb_ctx* ctx, uint64_t* out);
 
+/* Batched align(): Registration<Factor, ..., GeneralFactor, Rejector, Optimizer>::align (registration.hpp:17-54, optimizer.hpp:10-158) of
+ * every member from its own initial pose, in lockstep.  A round is one sgb_linearize_batch over the members still iterating or, for
+ * Levenberg-Marquardt, one sgb_error_batch over the members with a pending trial (until none has one), followed by one kernel in which
+ * each member solves its damped 6x6 system, updates its pose, lambda and convergence exactly as the reference's optimizer does, and
+ * writes its next pose on the device.  Per round the host reads one byte per member.  A member's results depend only on its own cloud,
+ * initial pose and the options (the exact-FP32-tie caveat above applies).  Afterwards sgb_correspondences_batch returns each member's
+ * correspondences of its last linearize. */
+enum sgb_optimizer_kind { SGB_OPT_GAUSS_NEWTON = 0, SGB_OPT_LEVENBERG_MARQUARDT = 1 };
+typedef struct sgb_align_options {
+  int factor_kind, robust_kind; /* sgb_factor_kind, sgb_robust_kind */
+  double robust_c;
+  int rejector_kind; /* sgb_rejector_kind */
+  double max_dist_sq;
+  int optimizer_kind;       /* sgb_optimizer_kind */
+  int max_iterations;       /* 20 */
+  double gn_lambda;         /* 1e-6: GaussNewtonOptimizer::lambda */
+  int max_inner_iterations; /* 10 */
+  double init_lambda, lambda_factor; /* 1e-3, 10 */
+  double rotation_eps, translation_eps; /* 0.1 deg [rad], 1e-3 [m]: TerminationCriteria */
+  double dof_mask[6]; /* RestrictDoFFactor (rx ry rz tx ty tz; 0 = frozen): H(i,i) += 1e9 |mask_i - 1|.  All 1 = NullFactor */
+} sgb_align_options;
+/* init_T16xB / out_T16xB: column-major 4x4 per member; inputs and outputs in host memory.  out_info4xB = converged, iterations, num_inliers, error per member;
+ * out_Hb42xB (or NULL) = H(36) | b(6) per member (RegistrationResult).  max_iterations <= 0 returns the initial poses, not converged. */
+int sgb_align_batch(sgb_ctx* ctx, const sgb_align_options* options, const double* init_T16xB, double* out_T16xB, double* out_info4xB,
+                    double* out_Hb42xB /*or NULL*/);
+
 /* ---- per-cloud preparation on the device (SURVEY.md §8(f); not per-iteration) --------------------
  * sgb_estimate_features replaces estimate_normals / estimate_covariances / estimate_normals_covariances and
  * their _omp / _tbb variants (include/small_gicp/util/normal_estimation.hpp:12-140, normal_estimation_omp.hpp:9-60):

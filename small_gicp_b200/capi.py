@@ -11,12 +11,34 @@ _ROOT = os.path.dirname(_HERE)
 FACTOR_ICP, FACTOR_PLANE_ICP, FACTOR_GICP = 0, 1, 2
 ROBUST_NONE, ROBUST_HUBER, ROBUST_CAUCHY = 0, 1, 2
 REJECT_NONE, REJECT_DISTANCE = 0, 1
+OPT_GAUSS_NEWTON, OPT_LEVENBERG_MARQUARDT = 0, 1
 NO_CORRESPONDENCE = np.uint64(0xFFFFFFFFFFFFFFFF)
 
 _dp = C.POINTER(C.c_double)
 _u64p = C.POINTER(C.c_uint64)
 _i32p = C.POINTER(C.c_int32)
 _vp = C.c_void_p
+
+
+class AlignOptions(C.Structure):
+    """sgb_align_options"""
+
+    _fields_ = [
+        ("factor_kind", C.c_int),
+        ("robust_kind", C.c_int),
+        ("robust_c", C.c_double),
+        ("rejector_kind", C.c_int),
+        ("max_dist_sq", C.c_double),
+        ("optimizer_kind", C.c_int),
+        ("max_iterations", C.c_int),
+        ("gn_lambda", C.c_double),
+        ("max_inner_iterations", C.c_int),
+        ("init_lambda", C.c_double),
+        ("lambda_factor", C.c_double),
+        ("rotation_eps", C.c_double),
+        ("translation_eps", C.c_double),
+        ("dof_mask", C.c_double * 6),
+    ]
 
 # name -> (restype, argtypes): every symbol include/sgicp_b200.h declares
 _SIGNATURES = {
@@ -54,6 +76,7 @@ _SIGNATURES = {
     "sgb_linearize_batch": (C.c_int, [_vp, C.c_int, C.c_int, C.c_double, C.c_int, C.c_double, _dp, C.POINTER(C.c_uint8), _dp]),
     "sgb_error_batch": (C.c_int, [_vp, _dp, C.POINTER(C.c_uint8), _dp]),
     "sgb_correspondences_batch": (C.c_int, [_vp, _u64p]),
+    "sgb_align_batch": (C.c_int, [_vp, C.POINTER(AlignOptions), _dp, _dp, _dp, _dp]),
     "sgb_estimate_features": (C.c_int, [_vp, C.c_size_t, _dp, C.c_int, _dp, _dp]),
     "sgb_target_estimate_features": (C.c_int, [_vp, C.c_int]),
     "sgb_source_estimate_features": (C.c_int, [_vp, C.c_int]),
@@ -64,6 +87,20 @@ _SIGNATURES = {
 
 class SgbError(RuntimeError):
     pass
+
+
+class BatchAlignResult:
+    """per-member RegistrationResult fields of a batched align, from T16 (column-major), info4 and H|b 42 rows"""
+
+    def __init__(self, T16, info4, Hb42):
+        B = T16.shape[0]
+        self.T_target_source = np.ascontiguousarray(T16.reshape(B, 4, 4).transpose(0, 2, 1))
+        self.converged = info4[:, 0] != 0
+        self.iterations = info4[:, 1].astype(np.int64)
+        self.num_inliers = info4[:, 2].astype(np.int64)
+        self.error = info4[:, 3].copy()
+        self.H = np.ascontiguousarray(Hb42[:, :36].reshape(B, 6, 6).transpose(0, 2, 1))
+        self.b = Hb42[:, 36:42].copy()
 
 
 def library_path(profiling=False):
@@ -315,6 +352,21 @@ class Context:
         out = np.empty(max(int(off[-1]), 1), dtype=np.uint64)
         self._check(self._L.sgb_correspondences_batch(self._h, out.ctypes.data_as(_u64p)))
         return [out[off[m] : off[m + 1]].copy() for m in range(off.size - 1)]
+
+    def align_batch(self, init_Ts, factor=FACTOR_GICP, robust=ROBUST_NONE, robust_c=1.0, rejector=REJECT_DISTANCE, max_dist_sq=1.0,
+                    optimizer=OPT_LEVENBERG_MARQUARDT, max_iterations=20, gn_lambda=1e-6, max_inner_iterations=10, init_lambda=1e-3,
+                    lambda_factor=10.0, rotation_eps=0.1 * np.pi / 180.0, translation_eps=1e-3, dof_mask=None):
+        """Registration<...>::align of every member from its initial pose (sgb_align_batch) -> a Result with per-member arrays
+        T_target_source (B,4,4), converged (B,) bool, iterations (B,), num_inliers (B,), error (B,), H (B,6,6), b (B,6)"""
+        B, Tc, _, _ = self._batch_args(init_Ts, None)
+        o = AlignOptions(int(factor), int(robust), float(robust_c), int(rejector), float(max_dist_sq), int(optimizer), int(max_iterations), float(gn_lambda),
+                         int(max_inner_iterations), float(init_lambda), float(lambda_factor), float(rotation_eps), float(translation_eps))
+        o.dof_mask[:] = [1.0] * 6 if dof_mask is None else [float(x) for x in dof_mask]
+        T = np.zeros((max(B, 1), 16))
+        info = np.zeros((max(B, 1), 4))
+        Hb = np.zeros((max(B, 1), 42))
+        self._check(self._L.sgb_align_batch(self._h, C.byref(o), _d(Tc), _d(T), _d(info), _d(Hb)))
+        return BatchAlignResult(T[:B], info[:B], Hb[:B])
 
     # ---- multi-GPU: all-reduce of H|b|e fused into the reduction kernel (peer memory over NVLink) ----
     COMM_HANDLE_BYTES = 64

@@ -6,6 +6,8 @@
 //   batch_factor_kernel     one CTA per 128-point tile of ONE member: FP64 rejector + factor (or error()) at that member's pose,
 //                           voxel-map probe for VGICP (vox_nearest, as in linearize_vox_kernel), CTA sum -> one partial per tile
 //   batch_segment_kernel    one CTA per member: its tiles' partials in tile order -> H|b|e|inliers (or e) of that member
+//   batch_step_kernel       batched align(): one thread per member, its Gauss-Newton / Levenberg-Marquardt step (sgb_math.cuh) after a
+//                           round, its next pose and phase
 // A member's sums depend on its own points, pose and correspondences only, added in an order fixed by its size: bit-identical whatever
 // else is in the batch.
 #include <cfloat>
@@ -162,6 +164,35 @@ __global__ void __launch_bounds__(kSegWarps * 32) batch_segment_kernel(const __g
     }
   }
   if (LIN && (mem.z & kMemberActive) && threadIdx.x < 12) B.lin_poses[12 * static_cast<size_t>(m) + threadIdx.x] = B.poses[12 * static_cast<size_t>(m) + threadIdx.x];
+}
+
+// One thread per member: the step is a sequential 6x6 solve and a few 4x4 products (about 2k FP64 operations), and at the 65536-member
+// limit that is 512 CTAs of 128 threads.  The state stays in global memory; only the solve's matrix is copied (to local memory: the
+// pivot indexes it at run time).
+constexpr int kStepBlock = 128;
+__global__ void __launch_bounds__(kStepBlock) batch_step_kernel(const __grid_constant__ AlignOptions o, uint32_t n_members, bool linearize,
+                                                                const double* __restrict__ out, MemberState* __restrict__ state,
+                                                                double* __restrict__ poses, uint8_t* __restrict__ phase) {
+  const uint32_t m = blockIdx.x * kStepBlock + threadIdx.x;
+  if (m >= n_members) return;
+  MemberState& s = state[m];
+  if (linearize && s.phase == kPhaseLinearize)
+    align_after_linearize(o, s, out + 44 * static_cast<size_t>(m));
+  else if (!linearize && s.phase == kPhaseTrial)
+    align_after_error(o, s, out[m]);
+  const double* T = s.phase == kPhaseTrial ? s.cand : s.T;
+  double* p = poses + 12 * static_cast<size_t>(m);
+  for (int i = 0; i < 3; i++) {  // pose_from_colmajor
+    for (int j = 0; j < 3; j++) p[i * 3 + j] = T[j * 4 + i];
+    p[9 + i] = T[12 + i];
+  }
+  phase[m] = static_cast<uint8_t>(s.phase);
+}
+
+cudaError_t launch_batch_step(const AlignOptions& o, uint32_t n_members, bool linearize, const double* out, MemberState* state, double* poses,
+                              uint8_t* phase, cudaStream_t st) {
+  batch_step_kernel<<<(n_members + kStepBlock - 1) / kStepBlock, kStepBlock, 0, st>>>(o, n_members, linearize, out, state, poses, phase);
+  return cudaGetLastError();
 }
 
 cudaError_t launch_batch_transform(const BatchParams& B, uint32_t n_tiles, float4* vq, uint32_t* vcorr, cudaStream_t st) {

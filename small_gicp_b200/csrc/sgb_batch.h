@@ -36,5 +36,9 @@ cudaError_t launch_batch_transform(const BatchParams& B, uint32_t n_tiles, float
 cudaError_t launch_batch_factor(const BatchParams& B, int factor, int robust, uint32_t n_tiles, bool voxel, bool err, const uint32_t* vcorr, cudaStream_t st);
 /// out: [members][44] (linearize) or [members] (error)
 cudaError_t launch_batch_segment(const BatchParams& B, uint32_t n_members, bool linearize, double* out, cudaStream_t st);
+/// batched align(): every member whose phase matches the round (linearize: kPhaseLinearize, else kPhaseTrial) takes its optimiser step
+/// from `out` (what launch_batch_segment wrote); then every member's next pose (row-major R | t) goes to poses and its phase to phase
+cudaError_t launch_batch_step(const AlignOptions& o, uint32_t n_members, bool linearize, const double* out, MemberState* state, double* poses,
+                              uint8_t* phase, cudaStream_t st);
 
 }  // namespace sgb

@@ -32,15 +32,16 @@ int batch_check(sgb_ctx* ctx, const char* who, const double* T) {
 }
 
 // The tables of one call: every active non-empty member's points cut into tiles of kLinBlock (the virtual source concatenates the
-// active members in member order), each member's pose (row-major R | t).  Uploaded on the context's stream.
+// active members in member order), each member's pose (row-major R | t; T = nullptr: b_poses already holds them).  Uploaded on the
+// context's stream.
 int batch_tables(sgb_ctx* ctx, const double* T, const uint8_t* active, bool seeds, uint32_t* n_tiles, uint32_t* n_virtual) {
   const size_t B = batch_members(ctx);
-  std::vector<double> poses(12 * B);
+  std::vector<double> poses(T ? 12 * B : 0);
   std::vector<BatchTile> tiles;
   std::vector<uint4> members(B);
   uint32_t v = 0;
   for (size_t m = 0; m < B; m++) {
-    pose_from_colmajor(T + 16 * m, poses.data() + 12 * m);
+    if (T) pose_from_colmajor(T + 16 * m, poses.data() + 12 * m);
     const bool act = !active || active[m];
     const uint32_t first = static_cast<uint32_t>(ctx->b_offsets[m]), n = static_cast<uint32_t>(ctx->b_offsets[m + 1] - ctx->b_offsets[m]);
     const uint32_t t0 = static_cast<uint32_t>(tiles.size());
@@ -51,7 +52,7 @@ int batch_tables(sgb_ctx* ctx, const double* T, const uint8_t* active, bool seed
     members[m] = make_uint4(t0, static_cast<uint32_t>(tiles.size()) - t0, (act ? kMemberActive : 0u) | (seeds && ctx->b_seeded[m] ? kMemberSeeded : 0u), 0u);
   }
   // pageable host memory: the copies are staged before cudaMemcpyAsync returns
-  CU(cudaMemcpyAsync(ctx->b_poses.p, poses.data(), poses.size() * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
+  if (T) CU(cudaMemcpyAsync(ctx->b_poses.p, poses.data(), poses.size() * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
   CU(cudaMemcpyAsync(ctx->b_members.p, members.data(), members.size() * sizeof(uint4), cudaMemcpyHostToDevice, ctx->stream));
   if (!tiles.empty()) CU(cudaMemcpyAsync(ctx->b_tiles.p, tiles.data(), tiles.size() * sizeof(BatchTile), cudaMemcpyHostToDevice, ctx->stream));
   *n_tiles = static_cast<uint32_t>(tiles.size());
@@ -78,6 +79,88 @@ BatchParams batch_params(sgb_ctx* ctx, const LinParams& P) {
 int copy_out(sgb_ctx* ctx, double* out, size_t doubles) {
   CU(cudaMemcpyAsync(out, ctx->b_out.p, doubles * sizeof(double), cudaMemcpyDefault, ctx->stream));
   CU(cudaStreamSynchronize(ctx->stream));
+  return 0;
+}
+
+// One linearize of the active members (arguments checked by the caller) into b_out, asynchronous.  T = nullptr: poses already in b_poses.
+int linearize_round(sgb_ctx* ctx, int factor, int robust, double robust_c, int rejector, double max_dist_sq, const double* T, const uint8_t* active) {
+  const size_t B = batch_members(ctx);
+  CU(cudaSetDevice(ctx->device));
+  const bool voxel = ctx->tgt_state == TargetState::VoxelMap;
+  // a new target (or none linearised yet) invalidates every member's cached state; sgb_drop_seeds only the seeds
+  if (!ctx->have_lin) std::fill(ctx->b_lin.begin(), ctx->b_lin.end(), 0);
+  if (!ctx->corr_seeds) std::fill(ctx->b_seeded.begin(), ctx->b_seeded.end(), 0);
+  uint32_t n_tiles = 0, n_virtual = 0;
+  if (int rc = batch_tables(ctx, T, active, !voxel, &n_tiles, &n_virtual)) return rc;
+  LinParams P;
+  fill_params(ctx, P, kIdentity);
+  BatchParams Bp = batch_params(ctx, P);
+  Bp.max_dist_sq_d = rejector == SGB_REJECT_DISTANCE ? max_dist_sq : DBL_MAX;
+  Bp.robust_c = robust_c;
+  if (ctx->n_tgt == 0) {  // nothing to match: every active member's points are unmatched, its sums zero
+    n_tiles = 0;
+    for (size_t m = 0; m < B; m++) {
+      const size_t nm = ctx->b_offsets[m + 1] - ctx->b_offsets[m];
+      if ((!active || active[m]) && nm) CU(cudaMemsetAsync(ctx->b_corr.as<uint32_t>() + ctx->b_offsets[m], 0xFF, nm * sizeof(uint32_t), ctx->stream));
+    }
+    std::vector<uint4> none(B, make_uint4(0, 0, 0, 0));
+    for (size_t m = 0; m < B; m++) none[m].z = (!active || active[m]) ? kMemberActive : 0u;
+    CU(cudaMemcpyAsync(ctx->b_members.p, none.data(), B * sizeof(uint4), cudaMemcpyHostToDevice, ctx->stream));
+  }
+  if (n_tiles && !voxel) {
+    // the search runs over the virtual source: the active members' queries, already transformed into the target's frame
+    CU(launch_batch_transform(Bp, n_tiles, ctx->b_vq.as<float4>(), ctx->b_vcorr.as<uint32_t>(), ctx->stream));
+    ctx->launches += 1;
+    P.src.pts = ctx->b_vq.as<float4>();
+    P.src.covA = P.src.covB = nullptr;
+    P.src.centre = ctx->tgt_centre.as<double>();  // identity pose, source centre = target centre: the search takes the stored query as is
+    P.src.n = n_virtual;
+    P.src.run = 1;
+    P.corr = ctx->b_vcorr.as<uint32_t>();
+    P.use_prev = 1;  // per member: its previous correspondences, or kNone
+    P.max_dist_sq = search_bound(rejector, max_dist_sq);
+    if (int rc = launch_point_search(ctx, P, ctx->tree_depth > 0 ? ctx->tree_depth : 1)) return rc;
+    ctx->launches += 1;
+  }
+  if (n_tiles) {
+    CU(launch_batch_factor(Bp, factor, robust, n_tiles, voxel, false, ctx->b_vcorr.as<uint32_t>(), ctx->stream));
+    ctx->launches += 1;
+  }
+  CU(launch_batch_segment(Bp, static_cast<uint32_t>(B), true, ctx->b_out.as<double>(), ctx->stream));
+  ctx->launches += 1;
+  for (size_t m = 0; m < B; m++) {
+    if (active && !active[m]) continue;
+    ctx->b_lin[m] = 1;
+    ctx->b_seeded[m] = 1;
+  }
+  ctx->have_lin = true;
+  ctx->corr_seeds = true;
+  ctx->lin_factor = factor;
+  ctx->lin_robust = robust;
+  ctx->lin_c = robust_c;
+  return 0;
+}
+
+// One error() of the active members (every one linearised against the current target) into b_out[0, B), asynchronous.  T as above.
+int error_round(sgb_ctx* ctx, const double* T, const uint8_t* active) {
+  const size_t B = batch_members(ctx);
+  CU(cudaSetDevice(ctx->device));
+  uint32_t n_tiles = 0, n_virtual = 0;
+  if (int rc = batch_tables(ctx, T, active, false, &n_tiles, &n_virtual)) return rc;
+  LinParams P;
+  fill_params(ctx, P, kIdentity);
+  BatchParams Bp = batch_params(ctx, P);
+  Bp.robust_c = ctx->lin_c;
+  if (n_tiles && ctx->n_tgt) {
+    CU(launch_batch_factor(Bp, ctx->lin_factor, ctx->lin_robust, n_tiles, ctx->tgt_state == TargetState::VoxelMap, true, nullptr, ctx->stream));
+    ctx->launches += 1;
+  } else {
+    n_tiles = 0;
+    std::vector<uint4> none(B, make_uint4(0, 0, 0, 0));
+    CU(cudaMemcpyAsync(ctx->b_members.p, none.data(), B * sizeof(uint4), cudaMemcpyHostToDevice, ctx->stream));
+  }
+  CU(launch_batch_segment(Bp, static_cast<uint32_t>(B), false, ctx->b_out.as<double>(), ctx->stream));
+  ctx->launches += 1;
   return 0;
 }
 
@@ -160,59 +243,7 @@ int sgb_linearize_batch(sgb_ctx* ctx, int factor, int robust, double robust_c, i
   if (batch_points(ctx) && ctx->n_tgt) {
     if (int rc = check_target(ctx, "sgb_linearize_batch", factor)) return rc;
   }
-  CU(cudaSetDevice(ctx->device));
-  const bool voxel = ctx->tgt_state == TargetState::VoxelMap;
-  // a new target (or none linearised yet) invalidates every member's cached state; sgb_drop_seeds only the seeds
-  if (!ctx->have_lin) std::fill(ctx->b_lin.begin(), ctx->b_lin.end(), 0);
-  if (!ctx->corr_seeds) std::fill(ctx->b_seeded.begin(), ctx->b_seeded.end(), 0);
-  uint32_t n_tiles = 0, n_virtual = 0;
-  if (int rc = batch_tables(ctx, T, active, !voxel, &n_tiles, &n_virtual)) return rc;
-  LinParams P;
-  fill_params(ctx, P, kIdentity);
-  BatchParams Bp = batch_params(ctx, P);
-  Bp.max_dist_sq_d = rejector == SGB_REJECT_DISTANCE ? max_dist_sq : DBL_MAX;
-  Bp.robust_c = robust_c;
-  if (ctx->n_tgt == 0) {  // nothing to match: every active member's points are unmatched, its sums zero
-    n_tiles = 0;
-    for (size_t m = 0; m < B; m++) {
-      const size_t nm = ctx->b_offsets[m + 1] - ctx->b_offsets[m];
-      if ((!active || active[m]) && nm) CU(cudaMemsetAsync(ctx->b_corr.as<uint32_t>() + ctx->b_offsets[m], 0xFF, nm * sizeof(uint32_t), ctx->stream));
-    }
-    std::vector<uint4> none(B, make_uint4(0, 0, 0, 0));
-    for (size_t m = 0; m < B; m++) none[m].z = (!active || active[m]) ? kMemberActive : 0u;
-    CU(cudaMemcpyAsync(ctx->b_members.p, none.data(), B * sizeof(uint4), cudaMemcpyHostToDevice, ctx->stream));
-  }
-  if (n_tiles && !voxel) {
-    // the search runs over the virtual source: the active members' queries, already transformed into the target's frame
-    CU(launch_batch_transform(Bp, n_tiles, ctx->b_vq.as<float4>(), ctx->b_vcorr.as<uint32_t>(), ctx->stream));
-    ctx->launches += 1;
-    P.src.pts = ctx->b_vq.as<float4>();
-    P.src.covA = P.src.covB = nullptr;
-    P.src.centre = ctx->tgt_centre.as<double>();  // identity pose, source centre = target centre: the search takes the stored query as is
-    P.src.n = n_virtual;
-    P.src.run = 1;
-    P.corr = ctx->b_vcorr.as<uint32_t>();
-    P.use_prev = 1;  // per member: its previous correspondences, or kNone
-    P.max_dist_sq = search_bound(rejector, max_dist_sq);
-    if (int rc = launch_point_search(ctx, P, ctx->tree_depth > 0 ? ctx->tree_depth : 1)) return rc;
-    ctx->launches += 1;
-  }
-  if (n_tiles) {
-    CU(launch_batch_factor(Bp, factor, robust, n_tiles, voxel, false, ctx->b_vcorr.as<uint32_t>(), ctx->stream));
-    ctx->launches += 1;
-  }
-  CU(launch_batch_segment(Bp, static_cast<uint32_t>(B), true, ctx->b_out.as<double>(), ctx->stream));
-  ctx->launches += 1;
-  for (size_t m = 0; m < B; m++) {
-    if (active && !active[m]) continue;
-    ctx->b_lin[m] = 1;
-    ctx->b_seeded[m] = 1;
-  }
-  ctx->have_lin = true;
-  ctx->corr_seeds = true;
-  ctx->lin_factor = factor;
-  ctx->lin_robust = robust;
-  ctx->lin_c = robust_c;
+  if (int rc = linearize_round(ctx, factor, robust, robust_c, rejector, max_dist_sq, T, active)) return rc;
   return copy_out(ctx, out44, 44 * B);
 }
 
@@ -226,24 +257,86 @@ int sgb_error_batch(sgb_ctx* ctx, const double* T, const uint8_t* active, double
   for (size_t m = 0; m < B; m++)
     if ((!active || active[m]) && !ctx->b_lin[m])
       return fail(ctx, 1, "sgb_error_batch: member " + std::to_string(m) + " is active but has not been linearised against the current target");
-  CU(cudaSetDevice(ctx->device));
-  uint32_t n_tiles = 0, n_virtual = 0;
-  if (int rc = batch_tables(ctx, T, active, false, &n_tiles, &n_virtual)) return rc;
-  LinParams P;
-  fill_params(ctx, P, kIdentity);
-  BatchParams Bp = batch_params(ctx, P);
-  Bp.robust_c = ctx->lin_c;
-  if (n_tiles && ctx->n_tgt) {
-    CU(launch_batch_factor(Bp, ctx->lin_factor, ctx->lin_robust, n_tiles, ctx->tgt_state == TargetState::VoxelMap, true, nullptr, ctx->stream));
-    ctx->launches += 1;
-  } else {
-    n_tiles = 0;
-    std::vector<uint4> none(B, make_uint4(0, 0, 0, 0));
-    CU(cudaMemcpyAsync(ctx->b_members.p, none.data(), B * sizeof(uint4), cudaMemcpyHostToDevice, ctx->stream));
-  }
-  CU(launch_batch_segment(Bp, static_cast<uint32_t>(B), false, ctx->b_out.as<double>(), ctx->stream));
-  ctx->launches += 1;
+  if (int rc = error_round(ctx, T, active)) return rc;
   return copy_out(ctx, out_e, B);
+}
+
+int sgb_align_batch(sgb_ctx* ctx, const sgb_align_options* o, const double* init_T, double* out_T, double* out_info, double* out_Hb) {
+  if (!ctx) return 1;
+  if (int rc = batch_check(ctx, "sgb_align_batch", init_T)) return rc;
+  if (!o) return fail(ctx, 1, "sgb_align_batch: null options");
+  if (!out_T || !out_info) return fail(ctx, 1, "sgb_align_batch: null output");
+  if (o->factor_kind < 0 || o->factor_kind > 2 || o->robust_kind < 0 || o->robust_kind > 2 || o->rejector_kind < 0 || o->rejector_kind > 1 ||
+      o->optimizer_kind < 0 || o->optimizer_kind > 1)
+    return fail(ctx, 1, "sgb_align_batch: invalid factor/robust/rejector/optimizer kind");
+  const size_t B = batch_members(ctx);
+  if (B == 0) return 0;
+  if (batch_points(ctx) && ctx->n_tgt) {
+    if (int rc = check_target(ctx, "sgb_align_batch", o->factor_kind)) return rc;
+  }
+  CU(cudaSetDevice(ctx->device));
+  AlignOptions ao;
+  ao.lm = o->optimizer_kind == SGB_OPT_LEVENBERG_MARQUARDT;
+  ao.max_iterations = o->max_iterations;
+  ao.max_inner_iterations = o->max_inner_iterations;
+  ao.gn_lambda = o->gn_lambda;
+  ao.init_lambda = o->init_lambda;
+  ao.lambda_factor = o->lambda_factor;
+  ao.rotation_eps = o->rotation_eps;
+  ao.translation_eps = o->translation_eps;
+  for (int i = 0; i < 6; i++) ao.dof_mask[i] = o->dof_mask[i];
+  // the initial state and poses: the only upload of poses in the whole align
+  std::vector<MemberState> state(B);
+  std::vector<double> poses(12 * B);
+  std::vector<uint8_t> phase(B);
+  for (size_t m = 0; m < B; m++) {
+    align_init(ao, init_T + 16 * m, state[m]);
+    pose_from_colmajor(init_T + 16 * m, poses.data() + 12 * m);
+    phase[m] = static_cast<uint8_t>(state[m].phase);
+  }
+  CU(ctx->b_state.reserve(B * sizeof(MemberState)));
+  CU(ctx->b_phase.reserve(B));
+  CU(cudaMemcpyAsync(ctx->b_state.p, state.data(), B * sizeof(MemberState), cudaMemcpyHostToDevice, ctx->stream));
+  CU(cudaMemcpyAsync(ctx->b_poses.p, poses.data(), poses.size() * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
+  // Rounds in lockstep: error() for every member with a pending trial until none has one, else a linearize of every member still
+  // iterating; each round ends with one step launch.  The host only reads the phases to build the next round's tile tables.
+  std::vector<uint8_t> active(B);
+  for (;;) {
+    bool any_trial = false, any_lin = false;
+    for (size_t m = 0; m < B; m++) {
+      any_trial |= phase[m] == kPhaseTrial;
+      any_lin |= phase[m] == kPhaseLinearize;
+    }
+    if (!any_trial && !any_lin) break;
+    const bool lin = !any_trial;
+    for (size_t m = 0; m < B; m++) active[m] = phase[m] == (lin ? kPhaseLinearize : kPhaseTrial);
+    if (lin) {
+      if (int rc = linearize_round(ctx, o->factor_kind, o->robust_kind, o->robust_c, o->rejector_kind, o->max_dist_sq, nullptr, active.data())) return rc;
+    } else {
+      if (int rc = error_round(ctx, nullptr, active.data())) return rc;
+    }
+    CU(launch_batch_step(ao, static_cast<uint32_t>(B), lin, ctx->b_out.as<double>(), ctx->b_state.as<MemberState>(), ctx->b_poses.as<double>(),
+                         ctx->b_phase.as<uint8_t>(), ctx->stream));
+    ctx->launches += 1;
+    CU(cudaMemcpyAsync(phase.data(), ctx->b_phase.p, B, cudaMemcpyDeviceToHost, ctx->stream));
+    CU(cudaStreamSynchronize(ctx->stream));
+  }
+  CU(cudaMemcpyAsync(state.data(), ctx->b_state.p, B * sizeof(MemberState), cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));
+  for (size_t m = 0; m < B; m++) {
+    const MemberState& s = state[m];
+    std::memcpy(out_T + 16 * m, s.T, 16 * sizeof(double));
+    double* info = out_info + 4 * m;
+    info[0] = s.converged ? 1.0 : 0.0;
+    info[1] = s.iterations;
+    info[2] = s.inliers;
+    info[3] = s.e;
+    if (out_Hb) {
+      std::memcpy(out_Hb + 42 * m, s.H, 36 * sizeof(double));
+      std::memcpy(out_Hb + 42 * m + 36, s.b, 6 * sizeof(double));
+    }
+  }
+  return 0;
 }
 
 int sgb_correspondences_batch(sgb_ctx* ctx, uint64_t* out) {

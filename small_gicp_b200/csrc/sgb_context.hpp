@@ -170,6 +170,7 @@ struct sgb_ctx {
   sgb::DevBuf b_corr;                      // per stored point: cached correspondence
   sgb::DevBuf b_vq, b_vcorr;               // virtual source of the search: transformed queries of the active members and what the search found
   sgb::DevBuf b_partials, b_out;           // per-tile partial sums, per-member results
+  sgb::DevBuf b_state, b_phase;            // sgb_align_batch: per member MemberState / next round (kPhase*, one byte)
 };
 
 namespace sgb {

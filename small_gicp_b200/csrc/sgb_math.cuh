@@ -10,9 +10,11 @@
 
 #if defined(__CUDACC__)
 #define SGB_HD __device__ __forceinline__
+#define SGB_HHD __host__ __device__ inline  // also called by the host code of the library (sgb_capi_batch.cu)
 #else
 #include <cmath>
 #define SGB_HD inline
+#define SGB_HHD inline
 #endif
 
 namespace sgb {
@@ -412,6 +414,242 @@ SGB_HD int expand_positions(int k, int& p0, int& p1) {
   }
   p0 = k == 27 ? 42 : 43;  // e, inlier count
   return 1;
+}
+
+// ---------------------------------------------------------------------------------------------------------------------------------
+// The optimiser of batched align() (batch_step_kernel, sgb_batch.cu): GaussNewtonOptimizer / LevenbergMarquardtOptimizer of
+// small_gicp_b200/host/include/small_gicp_b200/registration.hpp as a per-member state machine, one call per round.  The solve, the
+// exponential and the pose product are written operation for operation like solve_ldlt / so3_exp / se3_exp / Isometry3d::operator* of
+// core.hpp: compiled for the host without FMA contraction (tests/host_step) they give the same bits.  The installed host mirror must not
+// depend on csrc/, so core.hpp keeps its own definitions; a change to either copy must be made to both.
+// Matrices are column-major like core.hpp's Mat: A(r, c) = A[c * rows + r].  Poses are 4x4 (Isometry3d::data()).
+// ---------------------------------------------------------------------------------------------------------------------------------
+
+/// x = A^-1 rhs for a symmetric 6x6 A (destroyed) by LDL^T with diagonal pivoting; zero pivots give zero components (core.hpp solve_ldlt).
+SGB_HD void solve_ldlt6(double* A, const double* rhs, double* x) {
+  constexpr int n = 6;
+  int perm[n];
+  for (int i = 0; i < n; i++) perm[i] = i;
+  for (int k = 0; k < n; k++) {
+    int piv = k;
+    for (int i = k + 1; i < n; i++)
+      if (fabs(A[i * n + i]) > fabs(A[piv * n + piv])) piv = i;
+    if (piv != k) {
+      for (int j = 0; j < n; j++) {
+        const double t = A[j * n + k];
+        A[j * n + k] = A[j * n + piv];
+        A[j * n + piv] = t;
+      }
+      for (int i = 0; i < n; i++) {
+        const double t = A[k * n + i];
+        A[k * n + i] = A[piv * n + i];
+        A[piv * n + i] = t;
+      }
+      const int t = perm[k];
+      perm[k] = perm[piv];
+      perm[piv] = t;
+    }
+    for (int j = 0; j < k; j++) A[k * n + k] -= A[j * n + k] * A[j * n + k] * A[j * n + j];
+    for (int i = k + 1; i < n; i++) {
+      double s = A[k * n + i];
+      for (int j = 0; j < k; j++) s -= A[j * n + i] * A[j * n + k] * A[j * n + j];
+      A[k * n + i] = A[k * n + k] != 0.0 ? s / A[k * n + k] : 0.0;
+    }
+  }
+  double y[n];
+  for (int i = 0; i < n; i++) y[i] = rhs[perm[i]];
+  for (int i = 0; i < n; i++)
+    for (int j = 0; j < i; j++) y[i] -= A[j * n + i] * y[j];
+  for (int i = 0; i < n; i++) y[i] = fabs(A[i * n + i]) > 0.0 ? y[i] / A[i * n + i] : 0.0;
+  for (int i = n - 1; i >= 0; i--)
+    for (int j = i + 1; j < n; j++) y[i] -= A[i * n + j] * y[j];
+  for (int i = 0; i < n; i++) x[perm[i]] = y[i];
+}
+
+/// (H + lambda I) delta = -b  (detail::damped_step of registration.hpp)
+SGB_HD void damped_step6(const double* H, const double* b, double lambda, double* delta) {
+  double A[36], rhs[6];
+  for (int i = 0; i < 36; i++) A[i] = H[i];
+  for (int i = 0; i < 6; i++) A[i * 6 + i] += lambda;
+  for (int i = 0; i < 6; i++) rhs[i] = -b[i];
+  solve_ldlt6(A, rhs, delta);
+}
+
+/// out = A v for a 3x3 A (Mat's product: each entry summed from 0 in k order)
+SGB_HD void mat3_vec(const double* A, const double* v, double* out) {
+  for (int r = 0; r < 3; r++) out[r] = 0.0;
+  for (int k = 0; k < 3; k++)
+    for (int r = 0; r < 3; r++) out[r] += A[k * 3 + r] * v[k];
+}
+
+/// rotation matrix of a rotation vector through the unit quaternion (core.hpp so3_exp)
+SGB_HD void so3_exp3(const double* omega, double* R) {
+  double th2 = 0.0;
+  for (int i = 0; i < 3; i++) th2 += omega[i] * omega[i];
+  double im, re;
+  if (th2 < 1e-10) {
+    const double th4 = th2 * th2;
+    im = 0.5 - th2 / 48.0 + th4 / 3840.0;
+    re = 1.0 - th2 / 8.0 + th4 / 384.0;
+  } else {
+    const double th = sqrt(th2);
+    im = sin(0.5 * th) / th;
+    re = cos(0.5 * th);
+  }
+  const double w = re, x = im * omega[0], y = im * omega[1], z = im * omega[2];
+  R[0] = 1.0 - 2.0 * (y * y + z * z);
+  R[3] = 2.0 * (x * y - z * w);
+  R[6] = 2.0 * (x * z + y * w);
+  R[1] = 2.0 * (x * y + z * w);
+  R[4] = 1.0 - 2.0 * (x * x + z * z);
+  R[7] = 2.0 * (y * z - x * w);
+  R[2] = 2.0 * (x * z - y * w);
+  R[5] = 2.0 * (y * z + x * w);
+  R[8] = 1.0 - 2.0 * (x * x + y * y);
+}
+
+/// 4x4 pose of a twist [rx ry rz tx ty tz] (core.hpp se3_exp)
+SGB_HD void se3_exp6(const double* a, double* T) {
+  const double* omega = a;
+  const double* v = a + 3;
+  double th2 = 0.0;
+  for (int i = 0; i < 3; i++) th2 += omega[i] * omega[i];
+  const double th = sqrt(th2);
+  double R[9], t[3];
+  so3_exp3(omega, R);
+  if (th < 1e-10) {
+    mat3_vec(R, v, t);
+  } else {
+    double W[9] = {0.0, omega[2], -omega[1], -omega[2], 0.0, omega[0], omega[1], -omega[0], 0.0};  // skew(omega)
+    double WW[9];
+    for (int i = 0; i < 9; i++) WW[i] = 0.0;
+    for (int c = 0; c < 3; c++)
+      for (int k = 0; k < 3; k++)
+        for (int r = 0; r < 3; r++) WW[c * 3 + r] += W[k * 3 + r] * W[c * 3 + k];
+    const double s1 = (1.0 - cos(th)) / th2, s2 = (th - sin(th)) / (th2 * th);
+    double V[9];
+    for (int i = 0; i < 9; i++) V[i] = ((i % 4 == 0) ? 1.0 : 0.0) + W[i] * s1;  // Identity() + W * s1
+    for (int i = 0; i < 9; i++) V[i] = V[i] + WW[i] * s2;
+    mat3_vec(V, v, t);
+  }
+  for (int c = 0; c < 3; c++) {
+    for (int r = 0; r < 3; r++) T[c * 4 + r] = R[c * 3 + r];
+    T[c * 4 + 3] = 0.0;
+  }
+  for (int r = 0; r < 3; r++) T[12 + r] = t[r];
+  T[15] = 1.0;
+}
+
+/// out = A B for 4x4 poses (core.hpp Isometry3d::operator*: the full product, then the last row reset)
+SGB_HD void pose_mul(const double* A, const double* B, double* out) {
+  for (int i = 0; i < 16; i++) out[i] = 0.0;
+  for (int c = 0; c < 4; c++)
+    for (int k = 0; k < 4; k++) {
+      const double b = B[c * 4 + k];
+      for (int r = 0; r < 4; r++) out[c * 4 + r] += A[k * 4 + r] * b;
+    }
+  out[3] = out[7] = out[11] = 0.0;
+  out[15] = 1.0;
+}
+
+/// TerminationCriteria::converged: |delta_rot| <= rotation_eps && |delta_trans| <= translation_eps
+SGB_HD bool step_converged(const double* d, double rotation_eps, double translation_eps) {
+  double r = 0.0, t = 0.0;
+  for (int i = 0; i < 3; i++) r += d[i] * d[i];
+  for (int i = 3; i < 6; i++) t += d[i] * d[i];
+  return sqrt(r) <= rotation_eps && sqrt(t) <= translation_eps;
+}
+
+/// What the optimiser of one batched align() needs besides the reduction (sgb_align_options of include/sgicp_b200.h).
+struct AlignOptions {
+  int lm;  // 0: Gauss-Newton, 1: Levenberg-Marquardt
+  int max_iterations, max_inner_iterations;
+  double gn_lambda, init_lambda, lambda_factor;
+  double rotation_eps, translation_eps;
+  double dof_mask[6];  // RestrictDoFFactor: H(i,i) += 1e9 |mask_i - 1| (all ones: + 0, i.e. NullFactor)
+};
+
+/// next round of a member: linearize at T, error() at the candidate (LM), or nothing
+enum : int { kPhaseLinearize = 0, kPhaseTrial = 1, kPhaseDone = 2 };
+
+/// One member's optimiser between rounds.  T, converged, iterations, H, b, e and inliers are its RegistrationResult so far.
+struct MemberState {
+  double T[16];     // current pose
+  double cand[16];  // LM: candidate pose of the pending trial
+  double delta[6];  // LM: increment of the pending trial
+  double H[36], b[6], e, inliers;  // last linearize (H with the RestrictDoFFactor term); e = LM's e / the result's error
+  double lambda;
+  int phase, it, trial, converged, iterations;
+};
+
+SGB_HHD void align_init(const AlignOptions& o, const double* T0, MemberState& s) {
+  for (int i = 0; i < 16; i++) s.T[i] = s.cand[i] = T0[i];
+  for (int i = 0; i < 6; i++) s.delta[i] = s.b[i] = 0.0;
+  for (int i = 0; i < 36; i++) s.H[i] = 0.0;
+  s.e = s.inliers = 0.0;
+  s.lambda = o.init_lambda;
+  s.phase = o.max_iterations > 0 ? kPhaseLinearize : kPhaseDone;
+  s.it = s.trial = s.converged = s.iterations = 0;
+}
+
+SGB_HD void lm_propose(MemberState& s) {
+  damped_step6(s.H, s.b, s.lambda, s.delta);
+  double E[16];
+  se3_exp6(s.delta, E);
+  pose_mul(s.T, E, s.cand);
+}
+
+/// the outer iteration s.it is over: the next one, unless converged or out of iterations
+SGB_HD void end_iteration(const AlignOptions& o, MemberState& s) {
+  s.iterations = s.it;
+  s.it++;
+  s.phase = (s.it < o.max_iterations && !s.converged) ? kPhaseLinearize : kPhaseDone;
+}
+
+/// out44 = H | b | e | inliers of the linearize at s.T
+SGB_HD void align_after_linearize(const AlignOptions& o, MemberState& s, const double* out44) {
+  for (int i = 0; i < 36; i++) s.H[i] = out44[i];  // symmetric: row- and column-major agree
+  for (int i = 0; i < 6; i++) s.H[i * 6 + i] += 1e9 * fabs(o.dof_mask[i] - 1.0);
+  for (int i = 0; i < 6; i++) s.b[i] = out44[36 + i];
+  s.e = out44[42];
+  s.inliers = out44[43];
+  if (!o.lm) {
+    double d[6], E[16], T[16];
+    damped_step6(s.H, s.b, o.gn_lambda, d);
+    s.converged = step_converged(d, o.rotation_eps, o.translation_eps);
+    se3_exp6(d, E);
+    pose_mul(s.T, E, T);
+    for (int i = 0; i < 16; i++) s.T[i] = T[i];
+    end_iteration(o, s);
+    return;
+  }
+  s.trial = 0;
+  if (o.max_inner_iterations <= 0) {  // no trial: nothing accepted
+    s.iterations = s.it;
+    s.phase = kPhaseDone;
+    return;
+  }
+  lm_propose(s);
+  s.phase = kPhaseTrial;
+}
+
+/// candidate_e = error() at s.cand with the correspondences of the last linearize (LM)
+SGB_HD void align_after_error(const AlignOptions& o, MemberState& s, double candidate_e) {
+  if (candidate_e <= s.e) {
+    s.converged = step_converged(s.delta, o.rotation_eps, o.translation_eps);
+    for (int i = 0; i < 16; i++) s.T[i] = s.cand[i];
+    s.lambda /= o.lambda_factor;
+    s.e = candidate_e;
+    end_iteration(o, s);
+    return;
+  }
+  s.lambda *= o.lambda_factor;
+  if (++s.trial < o.max_inner_iterations) {
+    lm_propose(s);
+    return;
+  }
+  s.iterations = s.it;  // every trial rejected: the reference breaks out of the outer loop
+  s.phase = kPhaseDone;
 }
 
 }  // namespace sgb

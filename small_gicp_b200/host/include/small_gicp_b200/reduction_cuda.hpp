@@ -162,6 +162,16 @@ struct ParallelReductionCUDA {
     mirror->owned = false;
   }
 
+  /// BatchRegistration: mirror the target and its search structure as the first linearize() of an align() does, and return the context.
+  /// The caller replaces the source with a batch, so the source mirror is dropped.
+  template <typename Target, typename Tree>
+  sgb_ctx* batch_context(const Target& target, const Tree& target_tree) const {
+    sgb_ctx* ctx = context();
+    mirror_target(ctx, target, target_tree, true);
+    mirror->source_valid = false;
+    return ctx;
+  }
+
   sgb_ctx* context() const {
     if (!mirror) mirror = std::make_shared<detail::DeviceMirror>();
     if (!mirror->ctx) {

@@ -12,6 +12,7 @@
 #include <small_gicp_b200/kdtree.hpp>
 #include <small_gicp_b200/reduction_cuda.hpp>
 #include <small_gicp_b200/registration.hpp>
+#include <small_gicp_b200/registration_batch.hpp>
 #include <small_gicp_b200/registration_helper.hpp>
 #include <small_gicp_b200/voxelmap.hpp>
 
@@ -85,26 +86,114 @@ RegistrationResult run(const Options& o, const std::shared_ptr<PointCloud>& targ
   return reg.align(*target, *source, tree, init);
 }
 
-template <typename Factor, bool kRobust>
-RegistrationResult dispatch_rest(const Options& o, const std::shared_ptr<PointCloud>& t, const std::shared_ptr<PointCloud>& s, const Isometry3d& init) {
+/// BatchRegistration<...>::align of every source from its initial pose, configured like run()
+template <typename Factor, typename General, typename Rejector, typename Optimizer, bool kRobust>
+std::vector<RegistrationResult> run_batch(const Options& o, const std::shared_ptr<PointCloud>& target, const std::vector<PointCloud>& sources,
+                                          const std::vector<Isometry3d>& init) {
+  BatchRegistration<Factor, General, Rejector, Optimizer> reg;
+  configure(reg, o);
+  set_rejector(reg, o, std::is_same<Rejector, DistanceRejector>());
+  set_general(reg, o, std::is_same<General, RestrictDoFFactor>());
+  set_robust(reg.point_factor, o, std::integral_constant<bool, kRobust>());
+  if (o.tree == 2) {
+    GaussianVoxelMap map(o.voxel_resolution);
+    map.set_search_offsets(o.voxel_search_offsets);
+    map.insert(*target);
+    return reg.align(map, map, sources, init);
+  }
+  if (o.tree == 1) {
+    DeviceKdTree<PointCloud> tree(target);
+    return reg.align(*target, tree, sources, init);
+  }
+  KdTree<PointCloud> tree(target);
+  return reg.align(*target, tree, sources, init);
+}
+
+/// The registration types chosen by the options: job.call<Factor, GeneralFactor, Rejector, Optimizer, kRobust>().
+struct SingleJob {
+  const Options& o;
+  const std::shared_ptr<PointCloud>& target;
+  const std::shared_ptr<PointCloud>& source;
+  const Isometry3d& init;
+  RegistrationResult result;
+  template <typename Factor, typename General, typename Rejector, typename Optimizer, bool kRobust>
+  void call() {
+    result = run<Factor, General, Rejector, Optimizer, kRobust>(o, target, source, init);
+  }
+};
+struct BatchJob {
+  const Options& o;
+  const std::shared_ptr<PointCloud>& target;
+  const std::vector<PointCloud>& sources;
+  const std::vector<Isometry3d>& init;
+  std::vector<RegistrationResult> results;
+  template <typename Factor, typename General, typename Rejector, typename Optimizer, bool kRobust>
+  void call() {
+    results = run_batch<Factor, General, Rejector, Optimizer, kRobust>(o, target, sources, init);
+  }
+};
+
+template <typename Factor, bool kRobust, typename Job>
+void dispatch_rest(const Options& o, Job& job) {
   const int key = (o.restrict_dof ? 4 : 0) | (o.rejector == SGB_REJECT_DISTANCE ? 2 : 0) | (o.optimizer ? 1 : 0);
   switch (key) {
-    case 0: return run<Factor, NullFactor, NullRejector, GaussNewtonOptimizer, kRobust>(o, t, s, init);
-    case 1: return run<Factor, NullFactor, NullRejector, LevenbergMarquardtOptimizer, kRobust>(o, t, s, init);
-    case 2: return run<Factor, NullFactor, DistanceRejector, GaussNewtonOptimizer, kRobust>(o, t, s, init);
-    case 3: return run<Factor, NullFactor, DistanceRejector, LevenbergMarquardtOptimizer, kRobust>(o, t, s, init);
-    case 4: return run<Factor, RestrictDoFFactor, NullRejector, GaussNewtonOptimizer, kRobust>(o, t, s, init);
-    case 5: return run<Factor, RestrictDoFFactor, NullRejector, LevenbergMarquardtOptimizer, kRobust>(o, t, s, init);
-    case 6: return run<Factor, RestrictDoFFactor, DistanceRejector, GaussNewtonOptimizer, kRobust>(o, t, s, init);
-    default: return run<Factor, RestrictDoFFactor, DistanceRejector, LevenbergMarquardtOptimizer, kRobust>(o, t, s, init);
+    case 0: return job.template call<Factor, NullFactor, NullRejector, GaussNewtonOptimizer, kRobust>();
+    case 1: return job.template call<Factor, NullFactor, NullRejector, LevenbergMarquardtOptimizer, kRobust>();
+    case 2: return job.template call<Factor, NullFactor, DistanceRejector, GaussNewtonOptimizer, kRobust>();
+    case 3: return job.template call<Factor, NullFactor, DistanceRejector, LevenbergMarquardtOptimizer, kRobust>();
+    case 4: return job.template call<Factor, RestrictDoFFactor, NullRejector, GaussNewtonOptimizer, kRobust>();
+    case 5: return job.template call<Factor, RestrictDoFFactor, NullRejector, LevenbergMarquardtOptimizer, kRobust>();
+    case 6: return job.template call<Factor, RestrictDoFFactor, DistanceRejector, GaussNewtonOptimizer, kRobust>();
+    default: return job.template call<Factor, RestrictDoFFactor, DistanceRejector, LevenbergMarquardtOptimizer, kRobust>();
   }
 }
 
-template <typename Base>
-RegistrationResult dispatch_robust(const Options& o, const std::shared_ptr<PointCloud>& t, const std::shared_ptr<PointCloud>& s, const Isometry3d& init) {
-  if (o.robust == SGB_ROBUST_HUBER) return dispatch_rest<RobustFactor<Huber, Base>, true>(o, t, s, init);
-  if (o.robust == SGB_ROBUST_CAUCHY) return dispatch_rest<RobustFactor<Cauchy, Base>, true>(o, t, s, init);
-  return dispatch_rest<Base, false>(o, t, s, init);
+template <typename Base, typename Job>
+void dispatch_robust(const Options& o, Job& job) {
+  if (o.robust == SGB_ROBUST_HUBER) return dispatch_rest<RobustFactor<Huber, Base>, true>(o, job);
+  if (o.robust == SGB_ROBUST_CAUCHY) return dispatch_rest<RobustFactor<Cauchy, Base>, true>(o, job);
+  return dispatch_rest<Base, false>(o, job);
+}
+
+/// false: invalid factor kind
+template <typename Job>
+bool dispatch(const Options& o, Job& job) {
+  switch (o.factor) {
+    case SGB_FACTOR_ICP: dispatch_robust<ICPFactor>(o, job); return true;
+    case SGB_FACTOR_PLANE_ICP: dispatch_robust<PointToPlaneICPFactor>(o, job); return true;
+    case SGB_FACTOR_GICP: dispatch_robust<GICPFactor>(o, job); return true;
+    default: return false;
+  }
+}
+
+Options parse_options(const double* q) {
+  Options o;
+  o.factor = static_cast<int>(q[0]);
+  o.robust = static_cast<int>(q[1]);
+  o.robust_c = q[2];
+  o.rejector = static_cast<int>(q[3]);
+  o.max_dist_sq = q[4];
+  o.optimizer = static_cast<int>(q[5]);
+  o.max_iterations = static_cast<int>(q[6]);
+  o.rotation_eps = q[7];
+  o.translation_eps = q[8];
+  o.tree = static_cast<int>(q[9]);
+  o.voxel_resolution = q[10];
+  o.voxel_search_offsets = static_cast<int>(q[11]);
+  o.restrict_dof = static_cast<int>(q[12]);
+  for (int i = 0; i < 6; i++) o.dof_mask[i] = q[13 + i];
+  o.device = static_cast<int>(q[19]);
+  return o;
+}
+
+void write_result(const RegistrationResult& r, double* T_out16, double* scalars_out4, double* H_out36, double* b_out6) {
+  std::memcpy(T_out16, r.T_target_source.matrix().data(), sizeof(double) * 16);
+  scalars_out4[0] = r.converged ? 1.0 : 0.0;
+  scalars_out4[1] = static_cast<double>(r.iterations);
+  scalars_out4[2] = static_cast<double>(r.num_inliers);
+  scalars_out4[3] = r.error;
+  if (H_out36) std::memcpy(H_out36, r.H.data(), sizeof(double) * 36);
+  if (b_out6) std::memcpy(b_out6, r.b.data(), sizeof(double) * 6);
 }
 
 std::shared_ptr<PointCloud> make_cloud(size_t n, const double* pts4, const double* normals4, const double* covs16) {
@@ -131,41 +220,46 @@ int sgbh_align(size_t n_target, const double* target_pts4, const double* target_
                const double* source_pts4, const double* source_covs16, const double* options21, const double* init_T16, double* T_out16, double* scalars_out4,
                double* H_out36, double* b_out6) {
   try {
-    Options o;
-    const double* q = options21;
-    o.factor = static_cast<int>(q[0]);
-    o.robust = static_cast<int>(q[1]);
-    o.robust_c = q[2];
-    o.rejector = static_cast<int>(q[3]);
-    o.max_dist_sq = q[4];
-    o.optimizer = static_cast<int>(q[5]);
-    o.max_iterations = static_cast<int>(q[6]);
-    o.rotation_eps = q[7];
-    o.translation_eps = q[8];
-    o.tree = static_cast<int>(q[9]);
-    o.voxel_resolution = q[10];
-    o.voxel_search_offsets = static_cast<int>(q[11]);
-    o.restrict_dof = static_cast<int>(q[12]);
-    for (int i = 0; i < 6; i++) o.dof_mask[i] = q[13 + i];
-    o.device = static_cast<int>(q[19]);
+    const Options o = parse_options(options21);
     auto target = make_cloud(n_target, target_pts4, target_normals4, target_covs16);
     auto source = make_cloud(n_source, source_pts4, nullptr, source_covs16);
     Isometry3d init;
     std::memcpy(init.matrix().data(), init_T16, sizeof(double) * 16);
-    RegistrationResult r;
-    switch (o.factor) {
-      case SGB_FACTOR_ICP: r = dispatch_robust<ICPFactor>(o, target, source, init); break;
-      case SGB_FACTOR_PLANE_ICP: r = dispatch_robust<PointToPlaneICPFactor>(o, target, source, init); break;
-      case SGB_FACTOR_GICP: r = dispatch_robust<GICPFactor>(o, target, source, init); break;
-      default: g_error = "sgbh_align: invalid factor kind"; return 1;
+    SingleJob job{o, target, source, init, RegistrationResult()};
+    if (!dispatch(o, job)) {
+      g_error = "sgbh_align: invalid factor kind";
+      return 1;
     }
-    std::memcpy(T_out16, r.T_target_source.matrix().data(), sizeof(double) * 16);
-    scalars_out4[0] = r.converged ? 1.0 : 0.0;
-    scalars_out4[1] = static_cast<double>(r.iterations);
-    scalars_out4[2] = static_cast<double>(r.num_inliers);
-    scalars_out4[3] = r.error;
-    if (H_out36) std::memcpy(H_out36, r.H.data(), sizeof(double) * 36);
-    if (b_out6) std::memcpy(b_out6, r.b.data(), sizeof(double) * 6);
+    write_result(job.result, T_out16, scalars_out4, H_out36, b_out6);
+    return 0;
+  } catch (const std::exception& e) {
+    g_error = e.what();
+    return 2;
+  }
+}
+
+/// BatchRegistration<...>::align: the options of sgbh_align; n_members sources concatenated (member m = rows offsets[m] .. offsets[m+1]),
+/// one initial pose per member.  Outputs as sgbh_align's, member after member (16 / 4 / 36 / 6 doubles each).
+int sgbh_align_batch(size_t n_target, const double* target_pts4, const double* target_normals4, const double* target_covs16, size_t n_members,
+                     const size_t* offsets, const double* source_pts4, const double* source_covs16, const double* options21, const double* init_T16xB,
+                     double* T_out16xB, double* scalars_out4xB, double* H_out36xB, double* b_out6xB) {
+  try {
+    const Options o = parse_options(options21);
+    auto target = make_cloud(n_target, target_pts4, target_normals4, target_covs16);
+    std::vector<PointCloud> sources(n_members);
+    std::vector<Isometry3d> init(n_members);
+    for (size_t m = 0; m < n_members; m++) {
+      const size_t off = offsets[m], n = offsets[m + 1] - off;
+      sources[m] = *make_cloud(n, source_pts4 + 4 * off, nullptr, source_covs16 ? source_covs16 + 16 * off : nullptr);
+      std::memcpy(init[m].matrix().data(), init_T16xB + 16 * m, sizeof(double) * 16);
+    }
+    BatchJob job{o, target, sources, init, {}};
+    if (!dispatch(o, job)) {
+      g_error = "sgbh_align_batch: invalid factor kind";
+      return 1;
+    }
+    for (size_t m = 0; m < n_members; m++)
+      write_result(job.results[m], T_out16xB + 16 * m, scalars_out4xB + 4 * m, H_out36xB ? H_out36xB + 36 * m : nullptr, b_out6xB ? b_out6xB + 6 * m : nullptr);
     return 0;
   } catch (const std::exception& e) {
     g_error = e.what();

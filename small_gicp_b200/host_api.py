@@ -98,6 +98,58 @@ def align(
     return r
 
 
+def align_batch(
+    target_points,
+    sources,
+    target_normals=None,
+    target_covs=None,
+    source_covs=None,
+    init_Ts=None,
+    factor=capi.FACTOR_GICP,
+    robust=capi.ROBUST_NONE,
+    robust_c=1.0,
+    rejector=capi.REJECT_DISTANCE,
+    max_dist_sq=1.0,
+    optimizer=OPT_LM,
+    max_iterations=20,
+    rotation_eps=0.1 * np.pi / 180.0,
+    translation_eps=1e-3,
+    tree=TREE_HOST_KDTREE,
+    voxel_resolution=1.0,
+    voxel_search_offsets=1,
+    dof_mask=None,
+    device=0,
+):
+    """BatchRegistration<Factor, GeneralFactor, Rejector, Optimizer>::align (C++ host mirror): every source (a list of (N_m, 3|4) arrays)
+    from its initial pose (init_Ts: (B, 4, 4), default identity); source_covs: None or a list of (N_m, 4, 4).  Keyword arguments as align().
+    Returns capi.BatchAlignResult (per-member arrays)."""
+    L = _lib()
+    if not hasattr(L.sgbh_align_batch, "_typed"):
+        L.sgbh_align_batch.restype = C.c_int
+        L.sgbh_align_batch.argtypes = [C.c_size_t, _dp, _dp, _dp, C.c_size_t, C.POINTER(C.c_size_t), _dp, _dp, _dp, _dp, _dp, _dp, _dp, _dp]
+        L.sgbh_align_batch._typed = True
+    tp = capi._points4(target_points)
+    tn, tc = _f64(target_normals), _f64(target_covs)
+    members = [capi._points4(s) for s in sources]
+    B = len(members)
+    offsets = np.zeros(B + 1, dtype=np.uintp)
+    offsets[1:] = np.cumsum([m.shape[0] for m in members])
+    sp = np.ascontiguousarray(np.concatenate(members) if B else np.zeros((0, 4)))
+    sc = None if source_covs is None else np.ascontiguousarray(np.concatenate([_f64(c) for c in source_covs]) if B else np.zeros((0, 4, 4)))
+    opts = np.zeros(21)
+    opts[:13] = [factor, robust, robust_c, rejector, max_dist_sq, optimizer, max_iterations, rotation_eps, translation_eps, tree, voxel_resolution, voxel_search_offsets, 0 if dof_mask is None else 1]
+    opts[13:19] = 1.0 if dof_mask is None else np.asarray(dof_mask, dtype=float)
+    opts[19] = device
+    Ts = np.tile(np.eye(4), (B, 1, 1)) if init_Ts is None else np.asarray(init_Ts, dtype=float).reshape(B, 4, 4)
+    T0 = np.ascontiguousarray(Ts.transpose(0, 2, 1))
+    T, sc4, H, b = np.zeros((max(B, 1), 16)), np.zeros((max(B, 1), 4)), np.zeros((max(B, 1), 36)), np.zeros((max(B, 1), 6))
+    rc = L.sgbh_align_batch(tp.shape[0], _d(tp), _d(tn), _d(tc), B, offsets.ctypes.data_as(C.POINTER(C.c_size_t)), _d(sp), _d(sc), _d(opts), _d(T0), _d(T), _d(sc4),
+                            _d(H), _d(b))
+    if rc != 0:
+        raise capi.SgbError(L.sgbh_last_error().decode())
+    return capi.BatchAlignResult(T[:B], sc4[:B], np.concatenate([H, b], axis=1)[:B])
+
+
 ICP, PLANE_ICP, GICP, VGICP = 0, 1, 2, 3  # RegistrationSetting::RegistrationType
 
 
