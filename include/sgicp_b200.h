@@ -130,6 +130,14 @@ int sgb_target_build_voxelmap(sgb_ctx* ctx, size_t n, const double* points_xyz1,
  * most 2^29 voxels in all (the table regions are addressed with 32-bit slot numbers), else the call fails with a message. */
 int sgb_target_build_voxelmaps(sgb_ctx* ctx, size_t n_maps, const size_t* offsets, const double* points_xyz1, const double* covs_4x4 /*or NULL*/,
                                double leaf_size, int search_offsets);
+/* n_maps point clouds, each with its own kd-tree, as ONE target for the batched calls only (member m is aligned against map m; see the
+ * batch section).  offsets, points, normals and covariances as for sgb_target_build_voxelmaps (host, page-locked or device memory; empty
+ * maps allowed).  Map m is stored as sgb_target_set_points + sgb_target_build_kdtree would store it alone: FP32 about the box centre of
+ * its own points, leaves of at most 32 points cut by median splits along the widest axis; a member can only ever match its own map's
+ * points.  The launch count depends on the size of the largest map only, never on n_maps, and there is no host synchronisation.
+ * n_maps <= SGB_BATCH_MAX_MEMBERS and fewer than 2^30 points in all, else the call fails with a message. */
+int sgb_target_build_kdtrees(sgb_ctx* ctx, size_t n_maps, const size_t* offsets, const double* points_xyz1, const double* normals_xyz0 /*or NULL*/,
+                             const double* covs_4x4 /*or NULL*/);
 /* k nearest neighbours (1 <= k <= 32) of arbitrary query points in the target's kd-tree: replaces KdTree::knn_search /
  * nearest_neighbor_search (ann/kdtree.hpp:165-189,254-274) and the batch_knn_search / batch_nearest_neighbor_search of the
  * Python binding (src/python/kdtree.cpp).  out_indices / out_sq_dists: n_queries x k, original target indices.  The distance reported
@@ -191,7 +199,16 @@ int sgb_num_inliers(sgb_ctx* ctx, size_t* n);
  * member as a batch of one; its correspondences are voxel ids within its own map (id << 32).  On such a target the single-source calls
  * (sgb_linearize, sgb_error, their _device variants, sgb_correspondences, sgb_num_inliers) and sgb_target_batch_knn,
  * sgb_target_estimate_features, sgb_target_set_kdtree / _build_kdtree fail with a message.  Pair one source with many maps (or many
- * sources with one map) by repeating the cloud. */
+ * sources with one map) by repeating the cloud.
+ * Many kd-trees: after sgb_target_build_kdtrees, member m is paired with map m in the same way, for ICP, point-to-plane (the maps need
+ * normals) and GICP (covariances).  A linearize round is 3 launches (search, factor, per-member sums) and an error round 2, whatever the
+ * member count.  The calls fail with a message while the member count differs from the map count.  Each member's results are
+ * bit-identical to a context holding its map alone (sgb_target_set_points + sgb_target_build_kdtree) and that member as a batch of one,
+ * except at exact FP32 distance ties; and they are bit-identical whatever else is in the batch INCLUDING at exact ties, since a member is
+ * searched by warps of its own points only.  Its correspondences are original indices within its own map.  sgb_target_size returns
+ * the total point count.  On such a target the single-source calls (sgb_linearize, sgb_error, their _device variants,
+ * sgb_correspondences, sgb_num_inliers), sgb_target_batch_knn, sgb_target_estimate_features, sgb_target_set_kdtree / _build_kdtree
+ * and sgb_target_adopt_source fail with a message. */
 #define SGB_BATCH_MAX_MEMBERS 65536
 /* offsets: n_members + 1 ascending entries, offsets[0] = 0; member m = points offsets[m] .. offsets[m+1] (empty members allowed).
  * points / covariances: all members concatenated, in the layouts above (host, page-locked or device memory). */

@@ -1,20 +1,23 @@
-"""Batched VGICP over many target maps (sgb_target_build_voxelmaps) against one pair after another, on one GPU.
+"""Batched VGICP over many target maps (sgb_target_build_voxelmaps), or batched GICP over many kd-trees (sgb_target_build_kdtrees,
+--target kdtree), against one pair after another, on one GPU.
 
 Workload: consecutive frames of the synthetic LiDAR stream (synthetic.lidar_frame_torch in the 16M-point world, 1 m forward + 1 deg
 yaw per frame), each voxel-grid sampled at 0.25 m with k = 20 covariances estimated on the device, all outside the timed window, and kept
 on the device (all frames concatenated in one tensor; both paths pass device pointers, so no host copy is timed).  Pair i:
 frame i is the target map, frame i + 1 the source, from the ground-truth relative pose perturbed by 0.5 deg / 0.1 m.  VGICP at leaf 1.0,
-search_offsets 1, Levenberg-Marquardt and Gauss-Newton, B in {1, 8, 64, 512} pairs.
+search_offsets 1 (--target kdtree: GICP against a kd-tree of the target frame), Levenberg-Marquardt and Gauss-Newton, B in
+{1, 8, 64, 512} pairs.
 
 Compared in one process, repetitions alternated, median of --reps:
-  (a) build_target_voxelmaps + set_source_batch + align_batch over all B pairs;
-  (b) one pair after another on one context: build_target_voxelmap + set_source_batch of one member + align_batch;
+  (a) build_target_voxelmaps (kdtree: build_target_kdtrees) + set_source_batch + align_batch over all B pairs;
+  (b) one pair after another on one context: build_target_voxelmap (kdtree: set_target + build_target_kdtree) + set_source_batch of
+      one member + align_batch;
   (c) (a) and (b) with the map building left out of both: the maps of (a) are built once beforehand, those of (b) before each pair's
       timed part.
 (a) and (b) are checked to reach bit-identical poses before anything is timed.  Also reported: rounds, kernel launches per call and the
 build on its own.  The card's name, power limit and maximum SM clock are read with nvidia-smi (read-only) and written next to the numbers.
 
-    python scripts/bench_align_pairs.py [--sizes 1,8,64,512] [--reps 10] [--out FILE]
+    python scripts/bench_align_pairs.py [--target voxelmap|kdtree] [--sizes 1,8,64,512] [--reps 10] [--out FILE]
 """
 import argparse
 import json
@@ -35,6 +38,7 @@ LEAF, OFFSETS = 1.0, 1
 
 def main():
     ap = argparse.ArgumentParser()
+    ap.add_argument("--target", choices=("voxelmap", "kdtree"), default="voxelmap")
     ap.add_argument("--sizes", default="1,8,64,512")
     ap.add_argument("--reps", type=int, default=10)
     ap.add_argument("--out", default="")
@@ -83,7 +87,10 @@ def main():
 
             def build_a():
                 t0 = time.perf_counter()
-                ctx_a.build_target_voxelmaps(*tgt, LEAF, OFFSETS)
+                if args.target == "kdtree":
+                    ctx_a.build_target_kdtrees(tgt[0], None, tgt[1])
+                else:
+                    ctx_a.build_target_voxelmaps(*tgt, LEAF, OFFSETS)
                 ctx_a.synchronize()
                 return time.perf_counter() - t0
 
@@ -99,7 +106,11 @@ def main():
                 T, it = np.empty((B, 4, 4)), np.empty(B, np.int64)
                 for i in range(B):
                     t0 = time.perf_counter()
-                    ctx_b.build_target_voxelmap(one_p[i], one_c[i], LEAF, OFFSETS)
+                    if args.target == "kdtree":
+                        ctx_b.set_target(one_p[i], None, one_c[i])
+                        ctx_b.build_target_kdtree()
+                    else:
+                        ctx_b.build_target_voxelmap(one_p[i], one_c[i], LEAF, OFFSETS)
                     ctx_b.synchronize()
                     t1 = time.perf_counter()
                     ctx_b.set_source_batch((one_p[i + 1], [0, len(one_p[i + 1])]), one_c[i + 1])
@@ -137,6 +148,7 @@ def main():
             med = lambda x: 1e3 * float(np.median(x))
             rec = {
                 "B": B,
+                "target": args.target,
                 "optimizer": name,
                 "iterations_max": int(ra.iterations.max()),
                 "converged": int(ra.converged.sum()),
@@ -164,7 +176,7 @@ def main():
     if args.out:
         os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
         with open(args.out, "w") as f:
-            json.dump({"setup": info, "results": results}, f, indent=1)
+            json.dump({"setup": info, "target": args.target, "results": results}, f, indent=1)
 
 
 if __name__ == "__main__":

@@ -63,6 +63,7 @@ _SIGNATURES = {
     "sgb_target_set_voxelmap": (C.c_int, [_vp, C.c_double, C.c_size_t, _i32p, _dp, _dp, C.c_int]),
     "sgb_target_build_voxelmap": (C.c_int, [_vp, C.c_size_t, _dp, _dp, C.c_double, C.c_int]),
     "sgb_target_build_voxelmaps": (C.c_int, [_vp, C.c_size_t, C.POINTER(C.c_size_t), _dp, _dp, C.c_double, C.c_int]),
+    "sgb_target_build_kdtrees": (C.c_int, [_vp, C.c_size_t, C.POINTER(C.c_size_t), _dp, _dp, _dp]),
     "sgb_target_batch_knn": (C.c_int, [_vp, C.c_size_t, _dp, C.c_int, _u64p, _dp]),
     "sgb_target_size": (C.c_size_t, [_vp]),
     "sgb_source_set_points": (C.c_int, [_vp, C.c_size_t, _dp, _dp]),
@@ -270,6 +271,34 @@ class Context:
             assert tuple(c.shape) == (p.shape[0], 4, 4)
         self._check(self._L.sgb_target_build_voxelmaps(self._h, offsets.size - 1, offsets.ctypes.data_as(C.POINTER(C.c_size_t)), _d(p), _d(c),
                                                        float(leaf_size), int(search_offsets)))
+
+    def build_target_kdtrees(self, points_list, normals_list=None, covs_list=None):
+        """one kd-tree per cloud, as ONE target of the batched calls: member m of the batch is aligned against map m (ICP, point-to-plane
+        with normals, GICP with covariances).  points_list: a list of (N_m, 3|4) arrays, or (points (N, 3|4), offsets (B + 1,)) with the
+        clouds concatenated (numpy or torch).  normals_list / covs_list: None, a list of (N_m, 4) / (N_m, 4, 4) arrays, or one
+        (N, 4) / (N, 4, 4) array."""
+        if isinstance(points_list, tuple):
+            points, offsets = points_list
+            p = _points4(points)
+            offsets = np.ascontiguousarray(offsets, dtype=np.uintp)
+            if offsets.ndim != 1 or offsets.size < 1 or int(offsets[-1]) != p.shape[0]:
+                raise SgbError(f"build_target_kdtrees: offsets must have B + 1 entries ending at the point count {p.shape[0]}")
+        else:
+            members = [_points4(x) for x in points_list]
+            offsets = np.zeros(len(members) + 1, dtype=np.uintp)
+            offsets[1:] = np.cumsum([m.shape[0] for m in members])
+            p = np.concatenate(members) if members else np.zeros((0, 4))
+
+        def _joined(xs, shape):
+            if xs is None:
+                return None
+            a = _f64(xs) if not isinstance(xs, (list, tuple)) else (np.concatenate([_f64(x) for x in xs]) if len(xs) else np.zeros((0,) + shape))
+            assert tuple(a.shape) == (p.shape[0],) + shape
+            return a
+
+        n = _joined(normals_list, (4,))
+        c = _joined(covs_list, (4, 4))
+        self._check(self._L.sgb_target_build_kdtrees(self._h, offsets.size - 1, offsets.ctypes.data_as(C.POINTER(C.c_size_t)), _d(p), _d(n), _d(c)))
 
     def target_batch_knn(self, queries, k=1):
         """KdTree.batch_knn_search(queries, k) on the device -> (indices (N,k) uint64, squared distances (N,k))"""

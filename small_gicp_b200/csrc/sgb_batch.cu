@@ -6,6 +6,7 @@
 //   batch_factor_kernel     one CTA per 128-point tile of ONE member: FP64 rejector + factor (or error()) at that member's pose,
 //                           voxel-map probe for VGICP (vox_nearest, as in linearize_vox_kernel), CTA sum -> one partial per tile
 //   batch_maps_factor_kernel  the same for a multi-map voxel target: member m's tiles use map m's centre and table region
+//   batch_trees_factor_kernel the same for many kd-trees: member m's tiles use map m's centre and what the forest search found
 //   batch_segment_kernel    one CTA per member: its tiles' partials in tile order -> H|b|e|inliers (or e) of that member
 //   batch_step_kernel       batched align(): one thread per member, its Gauss-Newton / Levenberg-Marquardt step (sgb_math.cuh) after a
 //                           round, its next pose and phase
@@ -163,6 +164,13 @@ __global__ void __launch_bounds__(kLinBlock, 4) batch_maps_factor_kernel(const _
   batch_factor_tile<FACTOR, ROBUST, true, ERR, true>(B, nullptr, map_centres, map_regions);
 }
 
+// Many kd-trees (sgb_target_build_kdtrees): member m centred on map m's centre, vcorr = what forest_search_kernel found in map m.
+template <int FACTOR, int ROBUST, bool ERR>
+__global__ void __launch_bounds__(kLinBlock, 4) batch_trees_factor_kernel(const __grid_constant__ BatchParams B, const uint32_t* __restrict__ vcorr,
+                                                                         const double* __restrict__ map_centres) {
+  batch_factor_tile<FACTOR, ROBUST, false, ERR, true>(B, vcorr, map_centres, nullptr);
+}
+
 // One CTA per member: warp w adds tiles w, w + 8, ... of the member in order, then the 8 warp sums are added in warp order.  The order
 // depends on the member's tile count only.  Members without tiles (inactive or empty) get zeros.  LIN: the member's pose becomes its
 // linearisation pose (read by later error() calls).
@@ -250,6 +258,17 @@ cudaError_t launch_batch_maps_factor(const BatchParams& B, int factor, int robus
       batch_maps_factor_kernel<(f == 1 ? 0 : f), r, true><<<n_tiles, kLinBlock, 0, st>>>(B, map_centres, map_regions);
     else
       batch_maps_factor_kernel<(f == 1 ? 0 : f), r, false><<<n_tiles, kLinBlock, 0, st>>>(B, map_centres, map_regions);
+    return cudaGetLastError();
+  });
+}
+
+cudaError_t launch_batch_trees_factor(const BatchParams& B, int factor, int robust, uint32_t n_tiles, bool err, const uint32_t* vcorr, const double* map_centres,
+                                      cudaStream_t st) {
+  return dispatch_factor_robust(factor, robust, cudaErrorInvalidValue, [&](auto f, auto r) {
+    if (err)
+      batch_trees_factor_kernel<f, r, true><<<n_tiles, kLinBlock, 0, st>>>(B, vcorr, map_centres);
+    else
+      batch_trees_factor_kernel<f, r, false><<<n_tiles, kLinBlock, 0, st>>>(B, vcorr, map_centres);
     return cudaGetLastError();
   });
 }

@@ -38,6 +38,10 @@ cudaError_t launch_batch_factor(const BatchParams& B, int factor, int robust, ui
 /// mask, first voxel, voxel count) of each map (sgb_target_build_voxelmaps).  VGICP probe (err = false) or error() (err = true).
 cudaError_t launch_batch_maps_factor(const BatchParams& B, int factor, int robust, uint32_t n_tiles, bool err, const double* map_centres,
                                      const uint4* map_regions, cudaStream_t st);
+/// The same over many kd-trees (member m against map m, sgb_target_build_kdtrees): map_centres [maps][4]; vcorr = the forest search's
+/// result over the call's virtual source (err = false) or unused (err = true).  ICP, point-to-plane or GICP.
+cudaError_t launch_batch_trees_factor(const BatchParams& B, int factor, int robust, uint32_t n_tiles, bool err, const uint32_t* vcorr, const double* map_centres,
+                                      cudaStream_t st);
 /// out: [members][44] (linearize) or [members] (error)
 cudaError_t launch_batch_segment(const BatchParams& B, uint32_t n_members, bool linearize, double* out, cudaStream_t st);
 /// batched align(): every member whose phase matches the round (linearize: kPhaseLinearize, else kPhaseTrial) takes its optimiser step

@@ -73,6 +73,9 @@ int zero_result(sgb_ctx* ctx, const double* T, double* d_out, bool linearize) {
 
 // the single-source calls need one target: a multi-map voxel target serves the batched calls only
 int single_target_check(sgb_ctx* ctx, const char* who) {
+  if (ctx->tgt_state == TargetState::KdTrees)
+    return fail(ctx, 1, std::string(who) + ": the target holds " + std::to_string(ctx->kt_maps) +
+                            " kd-trees (sgb_target_build_kdtrees), which only the batched calls use; set a single target first");
   if (ctx->tgt_state != TargetState::VoxelMaps) return 0;
   return fail(ctx, 1, std::string(who) + ": the target holds " + std::to_string(ctx->vm_maps) +
                           " voxel maps (sgb_target_build_voxelmaps), which only the batched calls use; set a single target first");
@@ -152,6 +155,27 @@ int sgb::begin_voxel_target(sgb_ctx* ctx, size_t n, bool covs, double leaf_size,
   ctx->vox_inv_leaf = 1.0 / leaf_size;
   CU(ctx->tgt_centre.reserve(4 * sizeof(double)));
   CU(ctx->tgt_bounds.reserve(6 * sizeof(double)));
+  return 0;
+}
+
+int sgb::begin_forest_target(sgb_ctx* ctx, size_t n, bool normals, bool covs, size_t n_maps) {
+  ctx->tgt_state = TargetState::KdTrees;
+  ctx->kt_maps = n_maps;
+  ctx->vm_maps = 0;
+  ctx->n_tgt = n;
+  ctx->tgt_has_normals = normals;
+  ctx->tgt_has_covs = covs;
+  ctx->tgt_has_lo = false;
+  ctx->grid_ready = false;
+  forget_linearisation(ctx);
+  CU(ctx->tgt_centre.reserve(4 * sizeof(double)));
+  CU(ctx->tgt_bounds.reserve(6 * sizeof(double)));
+  return 0;
+}
+
+size_t sgb::target_maps(const sgb_ctx* ctx) {
+  if (ctx->tgt_state == TargetState::VoxelMaps) return ctx->vm_maps;
+  if (ctx->tgt_state == TargetState::KdTrees) return ctx->kt_maps;
   return 0;
 }
 
@@ -253,7 +277,8 @@ int sgb::store_source(sgb_ctx* ctx, size_t off, size_t n, double* centre, double
 }
 
 int sgb::check_target(sgb_ctx* ctx, const char* who, int factor) {
-  if (ctx->tgt_state != TargetState::Tree && ctx->tgt_state != TargetState::VoxelMap && ctx->tgt_state != TargetState::VoxelMaps)
+  if (ctx->tgt_state != TargetState::Tree && ctx->tgt_state != TargetState::VoxelMap && ctx->tgt_state != TargetState::VoxelMaps &&
+      ctx->tgt_state != TargetState::KdTrees)
     return fail(ctx, 1, std::string(who) + ": target has no search structure (call sgb_target_set_kdtree / _build_kdtree / _set_voxelmap)");
   if (factor == SGB_FACTOR_PLANE_ICP && (!ctx->tgt_has_normals || ctx->tgt_state == TargetState::VoxelMap || ctx->tgt_state == TargetState::VoxelMaps))
     return fail(ctx, 1, std::string(who) + ": point-to-plane needs target normals");
@@ -790,6 +815,8 @@ int sgb_target_set_kdtree(sgb_ctx* ctx, const void* nodes24, size_t n_nodes, uin
   if (!ctx) return 1;
   if (ctx->tgt_state == TargetState::VoxelMap || ctx->tgt_state == TargetState::VoxelMaps)
     return fail(ctx, 1, "sgb_target_set_kdtree: the target is a voxel map; call sgb_target_set_points first");
+  if (ctx->tgt_state == TargetState::KdTrees)
+    return fail(ctx, 1, "sgb_target_set_kdtree: the target holds many kd-trees (sgb_target_build_kdtrees); call sgb_target_set_points first");
   if (ctx->n_tgt == 0) {
     ctx->tgt_state = TargetState::Tree;  // nothing to search
     return 0;
@@ -812,6 +839,8 @@ int sgb_target_build_kdtree(sgb_ctx* ctx, int max_leaf_size) {
   if (!ctx) return 1;
   if (ctx->tgt_state == TargetState::VoxelMap || ctx->tgt_state == TargetState::VoxelMaps)
     return fail(ctx, 1, "sgb_target_build_kdtree: the target is a voxel map; call sgb_target_set_points first");
+  if (ctx->tgt_state == TargetState::KdTrees)
+    return fail(ctx, 1, "sgb_target_build_kdtree: the target holds many kd-trees (sgb_target_build_kdtrees); call sgb_target_set_points first");
   if (ctx->n_tgt == 0) {
     ctx->tgt_state = TargetState::Tree;  // nothing to search
     return 0;

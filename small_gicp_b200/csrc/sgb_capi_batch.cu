@@ -12,6 +12,7 @@
 #include "../../include/sgicp_b200.h"
 #include "sgb_batch.h"
 #include "sgb_context.hpp"
+#include "sgb_forest.h"
 #include "sgb_kernels.h"
 
 using namespace sgb;
@@ -31,15 +32,19 @@ int batch_check(sgb_ctx* ctx, const char* who, const double* T) {
   if (ctx->tgt_state == TargetState::VoxelMaps && batch_members(ctx) != ctx->vm_maps)
     return fail(ctx, 1, std::string(who) + ": the batch has " + std::to_string(batch_members(ctx)) + " members but the target holds " +
                             std::to_string(ctx->vm_maps) + " voxel maps (member m is aligned against map m)");
+  if (ctx->tgt_state == TargetState::KdTrees && batch_members(ctx) != ctx->kt_maps)
+    return fail(ctx, 1, std::string(who) + ": the batch has " + std::to_string(batch_members(ctx)) + " members but the target holds " +
+                            std::to_string(ctx->kt_maps) + " kd-trees (member m is aligned against map m)");
   return 0;
 }
 
 bool voxel_target(const sgb_ctx* ctx) { return ctx->tgt_state == TargetState::VoxelMap || ctx->tgt_state == TargetState::VoxelMaps; }
 
-// the factor kernel of one round over the target's kind: one voxel map or a point target (launch_batch_factor), or many maps
+// the factor kernel of one round over the target's kind: one voxel map or a point target (launch_batch_factor), or many maps / trees
 cudaError_t launch_factor(sgb_ctx* ctx, const BatchParams& Bp, int factor, int robust, uint32_t n_tiles, bool err, const uint32_t* vcorr) {
   if (ctx->tgt_state == TargetState::VoxelMaps)
     return launch_batch_maps_factor(Bp, factor, robust, n_tiles, err, ctx->vm_centres.as<double>(), ctx->vm_regions.as<uint4>(), ctx->stream);
+  if (ctx->tgt_state == TargetState::KdTrees) return launch_batch_trees_factor(Bp, factor, robust, n_tiles, err, vcorr, ctx->kt_centres.as<double>(), ctx->stream);
   return launch_batch_factor(Bp, factor, robust, n_tiles, voxel_target(ctx), err, vcorr, ctx->stream);
 }
 
@@ -119,7 +124,14 @@ int linearize_round(sgb_ctx* ctx, int factor, int robust, double robust_c, int r
     for (size_t m = 0; m < B; m++) none[m].z = (!active || active[m]) ? kMemberActive : 0u;
     CU(cudaMemcpyAsync(ctx->b_members.p, none.data(), B * sizeof(uint4), cudaMemcpyHostToDevice, ctx->stream));
   }
-  if (n_tiles && !voxel) {
+  if (n_tiles && ctx->tgt_state == TargetState::KdTrees) {
+    // many trees: every tile searched in its member's own tree, straight from the stored points at the member's pose (sgb_forest.cu)
+    const uint32_t* tab = ctx->kt_tables.as<uint32_t>();
+    const size_t M = ctx->kt_maps;
+    const ForestView F{ctx->tgt_pnodes.as<float4>(), ctx->kt_centres.as<double>(), tab, tab + 3 * (M + 1)};
+    CU(launch_forest_search(Bp, F, n_tiles, ctx->kt_depth, search_bound(rejector, max_dist_sq), ctx->b_vcorr.as<uint32_t>(), ctx->stream));
+    ctx->launches += 1;
+  } else if (n_tiles && !voxel) {
     // the search runs over the virtual source: the active members' queries, already transformed into the target's frame
     CU(launch_batch_transform(Bp, n_tiles, ctx->b_vq.as<float4>(), ctx->b_vcorr.as<uint32_t>(), ctx->stream));
     ctx->launches += 1;

@@ -10,6 +10,7 @@
 
 #include "../../include/sgicp_b200.h"
 #include "sgb_context.hpp"
+#include "sgb_forest.h"
 #include "sgb_kdtree_host.hpp"
 #include "sgb_kernels.h"
 
@@ -309,6 +310,8 @@ int sgb_voxelgrid_sampling(sgb_ctx* ctx, size_t n, const double* points, double 
 // the source of this align() is the target of the next one.  Everything that already exists on the device is taken over, not rebuilt.
 int sgb_target_adopt_source(sgb_ctx* ctx) {
   if (!ctx) return 1;
+  if (ctx->tgt_state == TargetState::KdTrees)
+    return fail(ctx, 1, "sgb_target_adopt_source: the target holds many kd-trees (sgb_target_build_kdtrees); set a single target first");
   if (ctx->src_state != SourceState::Single || ctx->n_src == 0) return fail(ctx, 1, "sgb_target_adopt_source: no source points (call sgb_source_set_points first)");
   CU(cudaSetDevice(ctx->device));
   const size_t n = ctx->n_src;
@@ -498,6 +501,139 @@ int sgb_target_build_voxelmaps(sgb_ctx* ctx, size_t n_maps, const size_t* offset
                             ctx->tgt_covB.as<float4>(), ctx->vox_table.as<int4>(), table_slots, ctx->stream));
   ctx->launches += 4;
   ctx->n_tgt = n_vox;
+  return 0;
+}
+
+// Many point clouds with their kd-trees as one target of the batched calls (sgb_forest.cu).  Every size follows from the host offsets,
+// so the build is launched without a host synchronisation, in a number of launches set by the largest map alone.  Map m is stored as
+// sgb_target_set_points + sgb_target_build_kdtree store it alone: centred FP32 on its own box centre, w = index within the map, leaves
+// of at most kLbvhLeafPoints points cut by median splits along the widest axis of every node.
+int sgb_target_build_kdtrees(sgb_ctx* ctx, size_t n_maps, const size_t* offsets, const double* points, const double* normals, const double* covs) {
+  if (!ctx) return 1;
+  const std::string who = "sgb_target_build_kdtrees: ";
+  if (n_maps > SGB_BATCH_MAX_MEMBERS) return fail(ctx, 1, who + std::to_string(n_maps) + " maps, at most " + std::to_string(SGB_BATCH_MAX_MEMBERS));
+  if (!offsets) return fail(ctx, 1, who + "null offsets");
+  if (offsets[0] != 0) return fail(ctx, 1, who + "offsets[0] must be 0");
+  for (size_t m = 0; m < n_maps; m++)
+    if (offsets[m + 1] < offsets[m]) return fail(ctx, 1, who + "offsets must be ascending (map " + std::to_string(m) + ")");
+  const size_t n = offsets[n_maps];
+  if (n >= (1ull << 30)) return fail(ctx, 1, who + "too many points (fewer than 2^30 in all)");
+  if (n && !points) return fail(ctx, 1, who + "null points");
+  CU(cudaSetDevice(ctx->device));
+  if (int rc = begin_forest_target(ctx, n, normals != nullptr, covs != nullptr, n_maps)) return rc;
+  const size_t M = std::max<size_t>(n_maps, 1);
+  CU(ctx->kt_centres.reserve(M * 4 * sizeof(double)));
+  ctx->kt_depth = 1;
+  if (n == 0) return 0;
+  // per map, as build_lbvh sizes one tree: P = 2^depth leaf slots of at most kLbvhLeafPoints points, P - 1 packet records, and the
+  // first level whose nodes fit a shared-memory segment
+  const size_t T = 3 * (n_maps + 1) + 3 * n_maps;
+  std::vector<uint32_t> tab(T, 0);
+  uint32_t* pt_off = tab.data();
+  uint32_t* slot_off = pt_off + (n_maps + 1);
+  uint32_t* seg_off = slot_off + (n_maps + 1);
+  uint32_t* node_base = seg_off + (n_maps + 1);
+  uint32_t* depth = node_base + n_maps;
+  uint32_t* level0 = depth + n_maps;
+  uint32_t max_depth = 0, radix_levels = 0;
+  size_t nodes = 0;
+  for (size_t m = 0; m < n_maps; m++) {
+    const uint32_t nm = static_cast<uint32_t>(offsets[m + 1] - offsets[m]);
+    pt_off[m] = static_cast<uint32_t>(offsets[m]);
+    node_base[m] = static_cast<uint32_t>(nodes);
+    uint32_t P = 0, d = 0, l0 = 0, segs = 0;
+    if (nm) {
+      P = 2;
+      d = 1;
+      while (static_cast<uint64_t>(P) * kLbvhLeafPoints < nm) {
+        P <<= 1;
+        d++;
+      }
+      l0 = kd_smem_first_level(nm, d);
+      segs = 1u << l0;
+      nodes += P - 1;
+    }
+    depth[m] = d;
+    level0[m] = l0;
+    slot_off[m + 1] = slot_off[m] + P;
+    seg_off[m + 1] = seg_off[m] + segs;
+    max_depth = std::max(max_depth, d);
+    radix_levels = std::max(radix_levels, l0);
+  }
+  pt_off[n_maps] = static_cast<uint32_t>(n);
+  if (max_depth + 1 > 40) return fail(ctx, 1, who + "tree too deep");
+  const uint32_t n_segments = seg_off[n_maps], n_slots = slot_off[n_maps];
+  int key_bits = 32;
+  while ((1ull << (key_bits - 32)) < n_segments) key_bits++;
+  CU(ctx->kt_tables.reserve(T * sizeof(uint32_t)));
+  // pageable host memory: staged before cudaMemcpyAsync returns
+  CU(cudaMemcpyAsync(ctx->kt_tables.p, tab.data(), T * sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
+  CU(ctx->stage_pts.reserve(n * 4 * sizeof(double)));
+  CU(cudaMemcpyAsync(ctx->stage_pts.p, points, n * 4 * sizeof(double), cudaMemcpyDefault, ctx->stream));
+  if (normals) {
+    CU(ctx->stage_normals.reserve(n * 4 * sizeof(double)));
+    CU(cudaMemcpyAsync(ctx->stage_normals.p, normals, n * 4 * sizeof(double), cudaMemcpyDefault, ctx->stream));
+    CU(ctx->tgt_orig_normals.reserve(n * sizeof(float4)));
+    CU(ctx->tgt_normals.reserve(n * sizeof(float4)));
+  }
+  if (covs) {
+    CU(ctx->stage_covs.reserve(n * 16 * sizeof(double)));
+    CU(cudaMemcpyAsync(ctx->stage_covs.p, covs, n * 16 * sizeof(double), cudaMemcpyDefault, ctx->stream));
+    CU(ctx->tgt_orig_covA.reserve(n * sizeof(float4)));
+    CU(ctx->tgt_orig_covB.reserve(n * sizeof(float4)));
+    CU(ctx->tgt_covA.reserve(n * sizeof(float4)));
+    CU(ctx->tgt_covB.reserve(n * sizeof(float4)));
+  }
+  CU(ctx->tgt_orig_pts.reserve(n * sizeof(float4)));
+  CU(ctx->tgt_pts.reserve(n * sizeof(float4)));
+  CU(ctx->tgt_perm.reserve(n * sizeof(uint32_t)));
+  CU(ctx->tgt_pnodes.reserve(std::max<size_t>(nodes, 1) * 64));
+  CU(ctx->pre_boxes.reserve(static_cast<size_t>(n_segments) * 6 * sizeof(uint32_t)));
+  CU(ctx->keys_in.reserve(n * sizeof(uint64_t)));
+  CU(ctx->keys_out.reserve(n * sizeof(uint64_t)));
+  CU(ctx->vals_in.reserve(n * sizeof(uint32_t)));
+  size_t sort_bytes = 0;
+  if (radix_levels) {
+    CU(sort_pairs_u64_u32_bits(nullptr, sort_bytes, ctx->keys_in.as<uint64_t>(), ctx->keys_out.as<uint64_t>(), ctx->vals_in.as<uint32_t>(),
+                               ctx->tgt_perm.as<uint32_t>(), n, key_bits, ctx->stream));
+    CU(ctx->sort_temp.reserve(sort_bytes));
+  }
+  const uint32_t* tp = ctx->kt_tables.as<uint32_t>();
+  ForestBuild b = {};
+  b.tables = ForestTables{tp, tp + (n_maps + 1), tp + 2 * (n_maps + 1), tp + 3 * (n_maps + 1), tp + 3 * (n_maps + 1) + n_maps,
+                          tp + 3 * (n_maps + 1) + 2 * n_maps, static_cast<uint32_t>(n_maps)};
+  b.n = static_cast<uint32_t>(n);
+  b.n_segments = n_segments;
+  b.n_slots = n_slots;
+  b.radix_levels = radix_levels;
+  b.max_depth = max_depth;
+  b.key_bits = key_bits;
+  b.sm_count = ctx->sm_count;
+  b.points = ctx->stage_pts.as<double>();
+  b.normals = normals ? ctx->stage_normals.as<double>() : nullptr;
+  b.covs = covs ? ctx->stage_covs.as<double>() : nullptr;
+  b.centres = ctx->kt_centres.as<double>();
+  b.orig_pts = ctx->tgt_orig_pts.as<float4>();
+  b.orig_normals = normals ? ctx->tgt_orig_normals.as<float4>() : nullptr;
+  b.orig_covA = covs ? ctx->tgt_orig_covA.as<float4>() : nullptr;
+  b.orig_covB = covs ? ctx->tgt_orig_covB.as<float4>() : nullptr;
+  b.leaf_pts = ctx->tgt_pts.as<float4>();
+  b.leaf_normals = ctx->tgt_normals.as<float4>();
+  b.leaf_covA = ctx->tgt_covA.as<float4>();
+  b.leaf_covB = ctx->tgt_covB.as<float4>();
+  b.perm = ctx->tgt_perm.as<uint32_t>();
+  b.pnodes = ctx->tgt_pnodes.as<float4>();
+  b.boxes = ctx->pre_boxes.as<uint32_t>();
+  b.keys_in = ctx->keys_in.as<uint64_t>();
+  b.keys_out = ctx->keys_out.as<uint64_t>();
+  b.vals_in = ctx->vals_in.as<uint32_t>();
+  b.sort_temp = ctx->sort_temp.p;
+  b.sort_temp_bytes = sort_bytes;
+  int launches = 0;
+  CU(launch_forest_build(b, ctx->stream, &launches));
+  ctx->launches += launches;
+  ctx->kt_depth = static_cast<int>(max_depth) + 1;
+  ctx->n_pnodes = nodes;
   return 0;
 }
 

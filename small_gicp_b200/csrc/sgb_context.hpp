@@ -51,7 +51,9 @@ struct DevBuf {
 /// resident, and tgt_perm / tgt_pts / tgt_pnodes (+ the grid front end when grid_ready) are their search structure.  VoxelMap: tgt_pts /
 /// tgt_cov* hold n_tgt voxels and vox_table indexes them; tgt_orig_* belong to no one.  VoxelMaps: vm_maps voxel maps for batched calls
 /// only (member m against map m): their voxels concatenated in map order in tgt_pts / tgt_cov*, one region of vox_table per map.
-enum class TargetState { None, Points, Tree, VoxelMap, VoxelMaps };
+/// KdTrees: kt_maps point clouds with their kd-trees, for batched calls only (member m against map m): points and features concatenated
+/// in map order in leaf order in tgt_pts / tgt_normals / tgt_cov*, each map's packet records at its own base in tgt_pnodes.
+enum class TargetState { None, Points, Tree, VoxelMap, VoxelMaps, KdTrees };
 /// What the source is.  Single: one cloud of n_src points.  Batch: b_offsets.size() - 1 members concatenated (n_src = 0).
 enum class SourceState { None, Single, Batch };
 
@@ -122,6 +124,11 @@ struct sgb_ctx {
   size_t vm_maps = 0;
   sgb::DevBuf vm_centres, vm_regions;
   sgb::DevBuf vm_offsets, vm_caps, vm_keys, vm_vals;  // build scratch: point offsets, table capacities / their scan, the second sort
+  // many kd-trees (KdTrees, sgb_target_build_kdtrees, sgb_forest.h): per map its centre [4] and the uint32 tables of ForestTables
+  // (pt_off, slot_off, seg_off: n_maps + 1 each; node_base, depth, level0: n_maps each); kt_depth = stack entries of the search
+  size_t kt_maps = 0;
+  int kt_depth = 1;
+  sgb::DevBuf kt_centres, kt_tables;
 
   // ---- source ----
   sgb::SourceState src_state = sgb::SourceState::None;
@@ -197,6 +204,11 @@ int begin_point_target(sgb_ctx* ctx, size_t n, bool normals, bool covs, bool lo)
 /// a voxel map of n voxels (maps: n_maps voxel maps, VoxelMaps) replaces the target (the caller fills tgt_pts / tgt_cov*, vox_table and
 /// for maps vm_centres / vm_regions)
 int begin_voxel_target(sgb_ctx* ctx, size_t n, bool covs, double leaf_size, int search_offsets, bool maps = false, size_t n_maps = 0);
+/// n_maps point clouds of n points in all (with normals / covariances as flagged) replace the target as many kd-trees (KdTrees); the
+/// caller fills tgt_pts / tgt_normals / tgt_cov* / tgt_pnodes and kt_*
+int begin_forest_target(sgb_ctx* ctx, size_t n, bool normals, bool covs, size_t n_maps);
+/// the map count of a multi-map target (VoxelMaps or KdTrees), else 0
+size_t target_maps(const sgb_ctx* ctx);
 /// the point target's tree in tgt_perm / tgt_pts / tgt_pnodes (depth, n_pnodes packet records) becomes its search structure; builds the grid
 int install_tree(sgb_ctx* ctx, int depth, size_t n_pnodes);
 /// a single cloud of n points, a batch (n = 0) or nothing replaces the source

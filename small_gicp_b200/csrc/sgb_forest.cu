@@ -1,0 +1,541 @@
+// SPDX-License-Identifier: MIT
+// Many kd-trees as ONE target of the batched calls (sgb_target_build_kdtrees; DESIGN.md §11 "Many trees"): member m is searched in map
+// m's tree only.  Map m is stored as sgb_target_set_points + sgb_target_build_kdtree store it alone -- centred FP32 on its own box centre,
+// w = index within the map, leaves of at most kLbvhLeafPoints points cut by median splits along the widest axis, 64-byte packet records
+// -- and the maps are concatenated in map order: points and features in tgt_*, the record blocks in tgt_pnodes at per-map bases.
+// Leaf records hold GLOBAL positions, so a correspondence is one position in tgt_pts as for a single tree.
+//
+// Build (launches depend on the size of the largest map only, never on the map count; no host synchronisation):
+//   forest_centres_kernel       one CTA per map: box of its points -> centre, as launch_bounds_centre computes it for one cloud
+//   forest_convert_kernel       centred FP32 points and packed features in original order (+ the first working copy of the points)
+//   forest_boxes_kernel / forest_keys_kernel   one radix level of every map whose nodes at that level still exceed kKdSegMax points;
+//                               the caller sorts by (global node, coordinate along the node's widest axis) and re-gathers
+//   forest_refine_smem_kernel   every (map, subtree of <= kKdSegMax points) segment refined in shared memory, one CTA each
+//   forest_leaf_kernel / forest_level_kernel   the packet records of every map, one launch per tree level
+// Search:
+//   forest_search_kernel        one CTA per BatchTile (128 consecutive stored points of ONE member): warp-cooperative exact nearest-
+//                               neighbour walk over that member's map, as packet_search_kernel walks one tree
+#include <algorithm>
+#include <cfloat>
+
+#include "sgb_batch.h"
+#include "sgb_device.cuh"
+#include "sgb_forest.h"
+#include "sgb_kernels.h"
+
+namespace sgb {
+
+namespace {
+
+/// the map that owns x: the largest m < n_maps with prefix[m] <= x (prefix ascending, prefix[0] <= x < prefix[n_maps]); among maps
+/// that own nothing (equal prefix entries) it is the next one that does
+__device__ __forceinline__ uint32_t forest_map_of(const uint32_t* __restrict__ prefix, uint32_t n_maps, uint32_t x) {
+  uint32_t lo = 0, hi = n_maps;
+  while (hi - lo > 1u) {
+    const uint32_t mid = (lo + hi) >> 1;
+    if (__ldg(&prefix[mid]) <= x) lo = mid;
+    else hi = mid;
+  }
+  return lo;
+}
+
+// The helpers below are copies of tree_bound / tree_node_of / float_flip / float_unflip / lbvh_store_child in sgb_kernels.cu: sharing
+// them would change the code of the single-tree build kernels there.
+__device__ __forceinline__ uint32_t forest_bound(uint32_t j, uint32_t count, uint32_t n) {
+  return static_cast<uint32_t>((static_cast<uint64_t>(j) * n) / count);
+}
+__device__ __forceinline__ uint32_t forest_node_of(uint32_t i, uint32_t count, uint32_t n) {
+  return static_cast<uint32_t>(((static_cast<uint64_t>(i) + 1u) * count + n - 1u) / n) - 1u;
+}
+__device__ __forceinline__ uint32_t forest_flip(float f) {
+  const uint32_t u = __float_as_uint(f);
+  return u ^ ((u >> 31) ? 0xFFFFFFFFu : 0x80000000u);
+}
+__device__ __forceinline__ float forest_unflip(uint32_t u) { return __uint_as_float(u ^ ((u >> 31) ? 0x80000000u : 0xFFFFFFFFu)); }
+__device__ __forceinline__ void forest_store_child(float4* pnodes, uint32_t child_heap, const float lo[3], const float hi[3], uint32_t a, uint32_t b) {
+  const uint32_t parent = (child_heap - 1u) >> 1, side = (child_heap & 1u) ? 0u : 1u;  // odd heap index = left child
+  pnodes[parent * 4 + side * 2 + 0] = make_float4(lo[0], lo[1], lo[2], __uint_as_float(a));
+  pnodes[parent * 4 + side * 2 + 1] = make_float4(hi[0], hi[1], hi[2], __uint_as_float(b));
+}
+
+/// the node of map-local position `local` at radix level `level` as a global box / key id: the first shared-memory segment it covers
+/// (segments are map m's nodes at its level level0, numbered from seg_off[m]); ~0: the map is past its radix levels
+__device__ __forceinline__ uint32_t forest_level_node(const ForestTables& F, uint32_t m, uint32_t local, uint32_t n, uint32_t level) {
+  const uint32_t l0 = __ldg(&F.level0[m]);
+  if (level >= l0) return ~0u;
+  return __ldg(&F.seg_off[m]) + (forest_node_of(local, 1u << level, n) << (l0 - level));
+}
+
+__global__ void __launch_bounds__(256) forest_centres_kernel(const double4* __restrict__ pts, const ForestTables F, double* centres) {
+  __shared__ double s_red[8][6];
+  const uint32_t m = blockIdx.x, first = F.pt_off[m], last = F.pt_off[m + 1];
+  double lo[3] = {DBL_MAX, DBL_MAX, DBL_MAX}, hi[3] = {-DBL_MAX, -DBL_MAX, -DBL_MAX};
+  for (uint32_t i = first + threadIdx.x; i < last; i += blockDim.x) {
+    const double4 p = pts[i];
+    lo[0] = fmin(lo[0], p.x); lo[1] = fmin(lo[1], p.y); lo[2] = fmin(lo[2], p.z);
+    hi[0] = fmax(hi[0], p.x); hi[1] = fmax(hi[1], p.y); hi[2] = fmax(hi[2], p.z);
+  }
+#pragma unroll
+  for (int d = 0; d < 3; d++) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      lo[d] = fmin(lo[d], __shfl_down_sync(0xffffffffu, lo[d], o));
+      hi[d] = fmax(hi[d], __shfl_down_sync(0xffffffffu, hi[d], o));
+    }
+  }
+  const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
+  if (lane == 0) {
+#pragma unroll
+    for (int d = 0; d < 3; d++) {
+      s_red[warp][d] = lo[d];
+      s_red[warp][3 + d] = hi[d];
+    }
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    for (int w = 1; w < 8; w++) {
+#pragma unroll
+      for (int d = 0; d < 3; d++) {
+        lo[d] = fmin(lo[d], s_red[w][d]);
+        hi[d] = fmax(hi[d], s_red[w][3 + d]);
+      }
+    }
+    // min / max are exact: the same centre as centre_kernel computes from the atomics of a single build
+    double* c = centres + 4 * static_cast<size_t>(m);
+    double ext = 0.0;
+    for (int d = 0; d < 3; d++) {
+      c[d] = (lo[d] <= hi[d]) ? 0.5 * (lo[d] + hi[d]) : 0.0;
+      ext = fmax(ext, hi[d] - lo[d]);
+    }
+    c[3] = ext > 0.0 ? ext : 1.0;
+  }
+}
+
+// raw (double AoS) -> centred float4 in original order (w = index within the map) and its working copy, features packed, perm = identity
+__global__ void forest_convert_kernel(const double4* __restrict__ pts, const double4* __restrict__ normals, const double* __restrict__ covs, uint32_t n,
+                                      const ForestTables F, const double* __restrict__ centres, float4* out_pts, float4* work_pts, float4* out_normals,
+                                      float4* out_covA, float4* out_covB, uint32_t* perm) {
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    const uint32_t m = forest_map_of(F.pt_off, F.n_maps, i);
+    const double* c = centres + 4 * static_cast<size_t>(m);
+    const double4 p = pts[i];
+    const double x = p.x - c[0], y = p.y - c[1], z = p.z - c[2];
+    const float4 f = make_float4((float)x, (float)y, (float)z, __int_as_float(static_cast<int>(i - F.pt_off[m])));
+    out_pts[i] = f;
+    work_pts[i] = f;
+    perm[i] = i;
+    if (normals) {
+      const double4 nn = normals[i];
+      out_normals[i] = make_float4((float)nn.x, (float)nn.y, (float)nn.z, 0.f);
+    }
+    if (covs) {
+      const double* cv = covs + static_cast<size_t>(i) * 16;
+      out_covA[i] = pack_covA(cv);
+      out_covB[i] = pack_covB(cv);
+    }
+  }
+}
+
+__global__ void forest_boxes_init_kernel(uint32_t* boxes, uint32_t count) {
+  const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t < count * 6u) boxes[t] = (t % 6u) < 3u ? 0xFFFFFFFFu : 0u;
+}
+
+// node boxes of one radix level (the warp pre-reduction of kd_boxes_kernel in sgb_kernels.cu; a CTA here may span maps)
+__global__ void forest_boxes_kernel(const float4* __restrict__ pts, uint32_t n, const ForestTables F, uint32_t level, uint32_t* boxes) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  const bool valid = i < n;
+  const uint32_t idx = valid ? i : n - 1u;
+  const uint32_t m = forest_map_of(F.pt_off, F.n_maps, idx), first = F.pt_off[m];
+  const uint32_t node = forest_level_node(F, m, idx - first, F.pt_off[m + 1] - first, level);
+  const float4 p = pts[idx];
+  uint32_t v[6] = {forest_flip(p.x), forest_flip(p.y), forest_flip(p.z), forest_flip(p.x), forest_flip(p.y), forest_flip(p.z)};
+  const uint32_t node0 = __shfl_sync(0xffffffffu, node, 0);
+  if (__all_sync(0xffffffffu, node == node0)) {
+    if (node0 == ~0u) return;
+#pragma unroll
+    for (int a = 0; a < 3; a++) {
+      v[a] = __reduce_min_sync(0xffffffffu, v[a]);
+      v[3 + a] = __reduce_max_sync(0xffffffffu, v[3 + a]);
+    }
+    if ((threadIdx.x & 31u) == 0) {
+#pragma unroll
+      for (int a = 0; a < 3; a++) {
+        atomicMin(&boxes[node0 * 6 + a], v[a]);
+        atomicMax(&boxes[node0 * 6 + 3 + a], v[3 + a]);
+      }
+    }
+  } else if (valid && node != ~0u) {
+#pragma unroll
+    for (int a = 0; a < 3; a++) {
+      atomicMin(&boxes[node * 6 + a], v[a]);
+      atomicMax(&boxes[node * 6 + 3 + a], v[3 + a]);
+    }
+  }
+}
+
+// key = (global node << 32) | coordinate along the node's widest axis (as kd_keys_kernel in sgb_kernels.cu); a map past its radix levels
+// keys all its points (its first segment << 32): the stable sort keeps their order and the maps stay in map order
+__global__ void forest_keys_kernel(const float4* __restrict__ pts, uint32_t n, const ForestTables F, uint32_t level, const uint32_t* __restrict__ boxes,
+                                   uint64_t* keys) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const uint32_t m = forest_map_of(F.pt_off, F.n_maps, i), first = F.pt_off[m];
+  const uint32_t node = forest_level_node(F, m, i - first, F.pt_off[m + 1] - first, level);
+  if (node == ~0u) {
+    keys[i] = static_cast<uint64_t>(F.seg_off[m]) << 32;
+    return;
+  }
+  const float ex = forest_unflip(boxes[node * 6 + 3]) - forest_unflip(boxes[node * 6 + 0]);
+  const float ey = forest_unflip(boxes[node * 6 + 4]) - forest_unflip(boxes[node * 6 + 1]);
+  const float ez = forest_unflip(boxes[node * 6 + 5]) - forest_unflip(boxes[node * 6 + 2]);
+  const float4 p = pts[i];
+  const float c = ex >= ey ? (ex >= ez ? p.x : p.z) : (ey >= ez ? p.y : p.z);
+  keys[i] = (static_cast<uint64_t>(node) << 32) | forest_flip(c);
+}
+
+// A copy of kd_refine_smem_kernel (sgb_kernels.cu) over every map's segments: CTA b owns segment b - seg_off[m] of map m (a node of
+// its level level0 with at most kKdSegMax points) and runs its remaining levels down to the leaves in shared memory.  perm receives
+// global original positions (the map's first position + w).
+__global__ void __launch_bounds__(1024) forest_refine_smem_kernel(float4* __restrict__ leaf_pts, uint32_t* __restrict__ perm, const ForestTables F) {
+  extern __shared__ __align__(16) unsigned char s_raw[];
+  float4* s_pts = reinterpret_cast<float4*>(s_raw);                                                        // [2][kForestSegMax]
+  unsigned long long* s_key = reinterpret_cast<unsigned long long*>(s_raw + 2 * kForestSegMax * sizeof(float4));  // [kForestSegMax]
+  uint32_t* s_idx = reinterpret_cast<uint32_t*>(s_key + kForestSegMax);                                   // [kForestSegMax]
+  uint32_t* s_box = s_idx + kForestSegMax;                                                                // [kForestSegNodes][6]
+  const uint32_t tid = threadIdx.x;
+  const uint32_t map = forest_map_of(F.seg_off, F.n_maps, blockIdx.x);
+  const uint32_t b = blockIdx.x - F.seg_off[map], base = F.pt_off[map], n = F.pt_off[map + 1] - base;
+  const uint32_t level0 = F.level0[map], levels = F.depth[map];
+  const uint32_t first = forest_bound(b, 1u << level0, n), last = forest_bound(b + 1u, 1u << level0, n), m = last - first;
+  float4* pts = leaf_pts + base;
+  for (uint32_t t = tid; t < m; t += blockDim.x) s_pts[t] = pts[first + t];
+  uint32_t cur = 0;
+  __syncthreads();
+  for (uint32_t level = level0; level < levels; level++) {
+    const uint32_t count = 1u << level, node_first = b << (level - level0), n_nodes = 1u << (level - level0);
+    for (uint32_t t = tid; t < n_nodes * 6u; t += blockDim.x) s_box[t] = (t % 6u) < 3u ? 0xFFFFFFFFu : 0u;
+    __syncthreads();
+    const float4* P0 = s_pts + cur * kForestSegMax;
+    for (uint32_t t = tid; t < m; t += blockDim.x) {
+      const float4 p = P0[t];
+      uint32_t* bx = s_box + (forest_node_of(first + t, count, n) - node_first) * 6u;
+      atomicMin(&bx[0], forest_flip(p.x));
+      atomicMin(&bx[1], forest_flip(p.y));
+      atomicMin(&bx[2], forest_flip(p.z));
+      atomicMax(&bx[3], forest_flip(p.x));
+      atomicMax(&bx[4], forest_flip(p.y));
+      atomicMax(&bx[5], forest_flip(p.z));
+    }
+    __syncthreads();
+    for (uint32_t t = tid; t < kForestSegMax; t += blockDim.x) {
+      unsigned long long key = ~0ull;  // padding sorts to the end
+      if (t < m) {
+        const uint32_t node = forest_node_of(first + t, count, n) - node_first;
+        const uint32_t* bx = s_box + node * 6u;
+        const float ex = forest_unflip(bx[3]) - forest_unflip(bx[0]), ey = forest_unflip(bx[4]) - forest_unflip(bx[1]), ez = forest_unflip(bx[5]) - forest_unflip(bx[2]);
+        const float4 p = P0[t];
+        const float c = ex >= ey ? (ex >= ez ? p.x : p.z) : (ey >= ez ? p.y : p.z);
+        key = (static_cast<unsigned long long>(node) << 32) | forest_flip(c);
+      }
+      s_key[t] = key;
+      s_idx[t] = t;
+    }
+    __syncthreads();
+    for (uint32_t k = 2; k <= kForestSegMax; k <<= 1) {
+      for (uint32_t j = k >> 1; j > 0; j >>= 1) {
+        for (uint32_t t = tid; t < kForestSegMax / 2u; t += blockDim.x) {
+          const uint32_t lo = ((t & ~(j - 1u)) << 1) | (t & (j - 1u)), hi = lo | j;
+          const bool up = (lo & k) == 0u;
+          const unsigned long long a = s_key[lo], c = s_key[hi];
+          if ((a > c) == up) {
+            s_key[lo] = c;
+            s_key[hi] = a;
+            const uint32_t ia = s_idx[lo];
+            s_idx[lo] = s_idx[hi];
+            s_idx[hi] = ia;
+          }
+        }
+        __syncthreads();
+      }
+    }
+    float4* P1 = s_pts + (cur ^ 1u) * kForestSegMax;
+    for (uint32_t t = tid; t < m; t += blockDim.x) P1[t] = P0[s_idx[t]];
+    cur ^= 1u;
+    __syncthreads();
+  }
+  const float4* Pf = s_pts + cur * kForestSegMax;
+  for (uint32_t t = tid; t < m; t += blockDim.x) {
+    const float4 p = Pf[t];
+    pts[first + t] = p;
+    perm[base + first + t] = base + static_cast<uint32_t>(__float_as_int(p.w));
+  }
+}
+
+// one warp per leaf slot of any map (lbvh_leaf_kernel in sgb_kernels.cu): bounding box of its points -> the parent's child record in the
+// map's record block; a = the leaf's first GLOBAL position
+__global__ void forest_leaf_kernel(const float4* __restrict__ leaf_pts, const ForestTables F, uint32_t n_slots, float4* pnodes) {
+  const uint32_t slot = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31u;
+  if (slot >= n_slots) return;
+  const uint32_t m = forest_map_of(F.slot_off, F.n_maps, slot);
+  const uint32_t j = slot - F.slot_off[m], P = F.slot_off[m + 1] - F.slot_off[m];
+  const uint32_t base = F.pt_off[m], n = F.pt_off[m + 1] - base;
+  const uint32_t first = forest_bound(j, P, n), last = forest_bound(j + 1u, P, n), idx = first + lane;
+  float lo[3] = {INFINITY, INFINITY, INFINITY}, hi[3] = {-INFINITY, -INFINITY, -INFINITY};
+  if (idx < last) {
+    const float4 p = leaf_pts[base + idx];
+    lo[0] = hi[0] = p.x;
+    lo[1] = hi[1] = p.y;
+    lo[2] = hi[2] = p.z;
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+#pragma unroll
+    for (int a = 0; a < 3; a++) {
+      lo[a] = fminf(lo[a], __shfl_xor_sync(0xffffffffu, lo[a], o));
+      hi[a] = fmaxf(hi[a], __shfl_xor_sync(0xffffffffu, hi[a], o));
+    }
+  }
+  if (lane == 0) {
+    const uint32_t cnt = last - first;
+    forest_store_child(pnodes + 4 * static_cast<size_t>(F.node_base[m]), (P - 1u) + j, lo, hi, cnt ? base + first : 0u, cnt);
+  }
+}
+
+// the inner nodes at `level` of every map that has that level (lbvh_level_kernel in sgb_kernels.cu): union box -> the parent's record
+__global__ void forest_level_kernel(const ForestTables F, uint32_t level, float4* pnodes) {
+  const uint64_t total = static_cast<uint64_t>(F.n_maps) << level;
+  for (uint64_t t = blockIdx.x * static_cast<uint64_t>(blockDim.x) + threadIdx.x; t < total; t += static_cast<uint64_t>(gridDim.x) * blockDim.x) {
+    const uint32_t m = static_cast<uint32_t>(t >> level);
+    if (F.depth[m] <= level) continue;  // the map's inner levels are 0 .. depth - 1
+    const uint32_t node = ((1u << level) - 1u) + static_cast<uint32_t>(t & ((1ull << level) - 1ull));
+    float4* nodes = pnodes + 4 * static_cast<size_t>(F.node_base[m]);
+    const float4 l0 = nodes[node * 4 + 0], l1 = nodes[node * 4 + 1], r0 = nodes[node * 4 + 2], r1 = nodes[node * 4 + 3];
+    const float lo[3] = {fminf(l0.x, r0.x), fminf(l0.y, r0.y), fminf(l0.z, r0.z)};
+    const float hi[3] = {fmaxf(l1.x, r1.x), fmaxf(l1.y, r1.y), fmaxf(l1.z, r1.z)};
+    forest_store_child(nodes, node, lo, hi, node, 0u);
+  }
+}
+
+// ---- search ----------------------------------------------------------------------------------------------------------------------
+constexpr int kForestWarps = kLinBlock / 32;
+constexpr int kForestDenseLanes = 18;  // as kPacketDenseLanes (sgb_kernels_packet.cu)
+constexpr int kForestStack = 40;
+
+// One CTA per BatchTile: warp w takes the tile's points 32 w .. 32 w + 31, all of ONE member m, and walks map m's tree once for all of
+// them -- the walk of packet_search_kernel (sgb_kernels_packet.cu): one shared stack, warp votes, warp-uniform node and leaf loads, the
+// dense scan (every lane tests every point) or the sparse one (the whole warp serves one interested lane at a time).  Nothing of any
+// other member enters a warp, so a member's correspondences depend on its own points, pose and seeds only.
+__global__ void __launch_bounds__(kLinBlock, 8) forest_search_kernel(const __grid_constant__ BatchParams B, const __grid_constant__ ForestView F,
+                                                                     float bound, uint32_t* __restrict__ vcorr) {
+  extern __shared__ float s_dist[];  // [max_depth][kLinBlock] per-lane box distance of each pending subtree
+  __shared__ uint2 s_child[kForestWarps][kForestStack];
+  const BatchTile t = B.tiles[blockIdx.x];
+  const uint32_t lane = threadIdx.x & 31u, wib = threadIdx.x >> 5;
+  if (wib * 32u >= t.count) return;  // warp-uniform; no CTA barrier below
+  const uint32_t m = t.member;
+  const bool valid = threadIdx.x < t.count;
+  const uint32_t i = t.first + threadIdx.x, v = t.vfirst + threadIdx.x;
+  const uint32_t n_map = F.pt_off[m + 1] - F.pt_off[m];
+  if (n_map == 0) {
+    if (valid) vcorr[v] = kNone;
+    return;
+  }
+  const float4* __restrict__ pnodes = F.pnodes + 4 * static_cast<size_t>(F.node_base[m]);
+  const float4* __restrict__ pts = B.tgt.pts;
+  float* my_dist = s_dist + threadIdx.x;
+  uint2* my_child = s_child[wib];
+
+  float fx = 0.f, fy = 0.f, fz = 0.f;
+  float best_d = -1.0f;  // an idle lane is never interested in anything
+  uint32_t best = kNone;
+  if (valid) {
+    const double* R = B.poses + 12 * static_cast<size_t>(m);
+    const double* cs = B.centres + 4 * static_cast<size_t>(m);
+    const double3 tp = centred_translation(R, cs[0], cs[1], cs[2], F.centres + 4 * static_cast<size_t>(m));
+    const float3 f = centred_query_f32(R, tp, __ldg(&B.pts[i]));
+    fx = f.x;
+    fy = f.y;
+    fz = f.z;
+    best_d = bound;
+    // the member's previous correspondence: an upper bound only prunes
+    const uint32_t prev = (B.members[m].z & kMemberSeeded) ? B.corr[i] : kNone;
+    if (prev != kNone) {
+      const float4 q = __ldg(&pts[prev]);
+      const float dx = q.x - fx, dy = q.y - fy, dz = q.z - fz;
+      const float d = dx * dx + dy * dy + dz * dz;
+      if (d < best_d) {
+        best_d = d;
+        best = prev;
+      }
+    }
+  }
+
+  int sp = 0;
+  uint32_t cur = 0;    // inner node being expanded (index within the map's record block)
+  bool expand = true;  // false: nothing to expand, take the next pending subtree
+  uint32_t leaf_first = 0, leaf_cnt = 0;
+  float leaf_d = 0.f;
+  for (;;) {
+    if (expand) {
+      const float4 n0 = __ldg(&pnodes[cur * 4 + 0]), n1 = __ldg(&pnodes[cur * 4 + 1]);
+      const float4 n2 = __ldg(&pnodes[cur * 4 + 2]), n3 = __ldg(&pnodes[cur * 4 + 3]);
+      const float dl = box_dist2(fx, fy, fz, n0, n1), dr = box_dist2(fx, fy, fz, n2, n3);
+      const bool wl = dl < best_d, wr = dr < best_d;
+      const unsigned ml = __ballot_sync(0xffffffffu, wl), mr = __ballot_sync(0xffffffffu, wr);
+      uint32_t ca, cb;
+      if (ml && mr) {
+        const unsigned closer_l = __ballot_sync(0xffffffffu, (wl || wr) && dl <= dr);
+        const bool left_first = 2 * __popc(closer_l) >= __popc(ml | mr);
+        my_dist[sp * kLinBlock] = left_first ? dr : dl;
+        if (lane == 0) my_child[sp] = left_first ? make_uint2(__float_as_uint(n2.w), __float_as_uint(n3.w)) : make_uint2(__float_as_uint(n0.w), __float_as_uint(n1.w));
+        sp++;
+        ca = left_first ? __float_as_uint(n0.w) : __float_as_uint(n2.w);
+        cb = left_first ? __float_as_uint(n1.w) : __float_as_uint(n3.w);
+        leaf_d = left_first ? dl : dr;
+      } else if (ml) {
+        ca = __float_as_uint(n0.w);
+        cb = __float_as_uint(n1.w);
+        leaf_d = dl;
+      } else if (mr) {
+        ca = __float_as_uint(n2.w);
+        cb = __float_as_uint(n3.w);
+        leaf_d = dr;
+      } else {
+        expand = false;
+        continue;
+      }
+      if (cb == 0u) {  // inner child
+        cur = ca;
+        continue;
+      }
+      leaf_first = ca;
+      leaf_cnt = cb;
+    } else {
+      bool got = false;
+      uint2 c = make_uint2(0u, 0u);
+      while (sp > 0) {
+        sp--;
+        const float d = my_dist[sp * kLinBlock];
+        if (__any_sync(0xffffffffu, d < best_d)) {
+          __syncwarp();  // lane 0's push of this entry is visible
+          c = my_child[sp];
+          __syncwarp();  // ... and every lane has read it before lane 0 may push over it
+          leaf_d = d;
+          got = true;
+          break;
+        }
+      }
+      if (!got) break;
+      if (c.y == 0u) {
+        cur = c.x;
+        expand = true;
+        continue;
+      }
+      leaf_first = c.x;
+      leaf_cnt = c.y;
+    }
+    // ---- leaf (global positions) ----
+    const unsigned want = __ballot_sync(0xffffffffu, leaf_d < best_d);
+    if (__popc(want) > kForestDenseLanes) {
+      const float4* lp = pts + leaf_first;
+#pragma unroll 4
+      for (uint32_t j = 0; j < leaf_cnt; j++) {
+        const float4 q = __ldg(&lp[j]);
+        const float dx = q.x - fx, dy = q.y - fy, dz = q.z - fz;
+        const float d = dx * dx + dy * dy + dz * dz;
+        if (d < best_d) {
+          best_d = d;
+          best = leaf_first + j;
+        }
+      }
+    } else {
+      for (uint32_t base = 0; base < leaf_cnt; base += 32u) {
+        const uint32_t j = base + lane;
+        float4 q = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (j < leaf_cnt) q = __ldg(&pts[leaf_first + j]);
+        unsigned todo = want;
+        while (todo) {
+          const int src = __ffs(todo) - 1;
+          todo &= todo - 1;
+          const float qx = __shfl_sync(0xffffffffu, fx, src), qy = __shfl_sync(0xffffffffu, fy, src), qz = __shfl_sync(0xffffffffu, fz, src);
+          const float dx = q.x - qx, dy = q.y - qy, dz = q.z - qz;
+          const uint32_t dbits = j < leaf_cnt ? __float_as_uint(dx * dx + dy * dy + dz * dz) : 0x7f800000u;
+          const uint32_t dmin = __reduce_min_sync(0xffffffffu, dbits);
+          const unsigned who = __ballot_sync(0xffffffffu, dbits == dmin);  // lowest lane = first point in scan order
+          if (static_cast<int>(lane) == src) {
+            const float d = __uint_as_float(dmin);
+            if (d < best_d) {
+              best_d = d;
+              best = leaf_first + base + (__ffs(who) - 1);
+            }
+          }
+        }
+      }
+    }
+    expand = false;
+  }
+  __syncwarp();
+  if (valid) vcorr[v] = best;
+}
+
+}  // namespace
+
+cudaError_t launch_forest_build(const ForestBuild& b, cudaStream_t st, int* launches) {
+  const ForestTables& F = b.tables;
+  int count = 0;
+  const uint32_t n = b.n;
+  forest_centres_kernel<<<F.n_maps, 256, 0, st>>>(reinterpret_cast<const double4*>(b.points), F, b.centres);
+  const uint32_t cgrid = std::min<uint32_t>((n + 255u) / 256u, static_cast<uint32_t>(b.sm_count) * 8u);
+  forest_convert_kernel<<<cgrid, 256, 0, st>>>(reinterpret_cast<const double4*>(b.points), reinterpret_cast<const double4*>(b.normals), b.covs, n, F, b.centres,
+                                               b.orig_pts, b.leaf_pts, b.orig_normals, b.orig_covA, b.orig_covB, b.perm);
+  count += 2;
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return e;
+  // radix levels: every map whose nodes at this level still hold more than kForestSegMax points
+  for (uint32_t level = 0; level < b.radix_levels; level++) {
+    forest_boxes_init_kernel<<<(b.n_segments * 6u + 255u) / 256u, 256, 0, st>>>(b.boxes, b.n_segments);
+    forest_boxes_kernel<<<(n + 255u) / 256u, 256, 0, st>>>(b.leaf_pts, n, F, level, b.boxes);
+    forest_keys_kernel<<<(n + 255u) / 256u, 256, 0, st>>>(b.leaf_pts, n, F, level, b.boxes, b.keys_in);
+    if ((e = cudaMemcpyAsync(b.vals_in, b.perm, n * sizeof(uint32_t), cudaMemcpyDeviceToDevice, st)) != cudaSuccess) return e;
+    size_t tb = b.sort_temp_bytes;
+    if ((e = sort_pairs_u64_u32_bits(b.sort_temp, tb, b.keys_in, b.keys_out, b.vals_in, b.perm, n, b.key_bits, st)) != cudaSuccess) return e;
+    if ((e = launch_gather(b.perm, n, b.orig_pts, b.leaf_pts, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, b.sm_count, st)) != cudaSuccess) return e;
+    count += 6;
+  }
+  // every (map, segment) below: one CTA each
+  const size_t smem = 2 * kForestSegMax * sizeof(float4) + kForestSegMax * (sizeof(unsigned long long) + sizeof(uint32_t)) + kForestSegNodes * 6 * sizeof(uint32_t);
+  static bool configured = false;
+  if (!configured) {
+    if ((e = cudaFuncSetAttribute(forest_refine_smem_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem))) != cudaSuccess) return e;
+    configured = true;
+  }
+  forest_refine_smem_kernel<<<b.n_segments, 1024, smem, st>>>(b.leaf_pts, b.perm, F);
+  count += 1;
+  if (b.orig_normals || b.orig_covA) {
+    if ((e = launch_gather(b.perm, n, nullptr, nullptr, b.orig_normals, b.leaf_normals, b.orig_covA, b.leaf_covA, b.orig_covB, b.leaf_covB, b.sm_count, st)) !=
+        cudaSuccess)
+      return e;
+    count += 1;
+  }
+  // records: the leaves, then one launch per inner level, deepest first (a map joins once the level is within its depth)
+  forest_leaf_kernel<<<(b.n_slots + 7u) / 8u, 256, 0, st>>>(b.leaf_pts, F, b.n_slots, b.pnodes);
+  count += 1;
+  for (uint32_t level = b.max_depth - 1u; level >= 1u && level < b.max_depth; level--) {
+    const uint64_t threads = static_cast<uint64_t>(F.n_maps) << level;
+    const uint64_t g = std::min<uint64_t>((threads + 255u) / 256u, static_cast<uint64_t>(b.sm_count) * 16u);
+    forest_level_kernel<<<static_cast<unsigned>(g), 256, 0, st>>>(F, level, b.pnodes);
+    count += 1;
+  }
+  if (launches) *launches = count;
+  return cudaGetLastError();
+}
+
+cudaError_t launch_forest_search(const BatchParams& B, const ForestView& F, uint32_t n_tiles, int max_depth, float bound, uint32_t* vcorr, cudaStream_t st) {
+  if (max_depth < 1 || max_depth > kForestStack) return cudaErrorInvalidValue;
+  const size_t smem = static_cast<size_t>(max_depth) * kLinBlock * sizeof(float);
+  forest_search_kernel<<<n_tiles, kLinBlock, smem, st>>>(B, F, bound, vcorr);
+  return cudaGetLastError();
+}
+
+}  // namespace sgb

@@ -1,0 +1,61 @@
+// SPDX-License-Identifier: MIT
+// Many kd-trees as one target of the batched calls: device tables, build and search launchers (sgb_forest.cu; C-ABI
+// sgb_target_build_kdtrees in sgb_capi_preprocess.cu, batched rounds in sgb_capi_batch.cu).
+#pragma once
+#include <cuda_runtime.h>
+#include <stdint.h>
+
+#include "sgb_batch.h"
+
+namespace sgb {
+
+/// shared-memory segment of the refinement (points) and its most nodes at one level: kKdSegMax / kKdSegNodes of sgb_kernels.cu
+constexpr uint32_t kForestSegMax = 2048;
+constexpr uint32_t kForestSegNodes = 128;
+
+/// Per-map tables on the device, all derived on the host from the map offsets.  Prefix arrays have n_maps + 1 entries.
+struct ForestTables {
+  const uint32_t* pt_off;     // first point of map m (points concatenated in map order)
+  const uint32_t* slot_off;   // first leaf slot of map m (P_m = 2^depth slots, 0 for an empty map)
+  const uint32_t* seg_off;    // first shared-memory segment of map m (2^level0 segments, 0 for an empty map)
+  const uint32_t* node_base;  // [n_maps] first packet record of map m in the record array (P_m - 1 records)
+  const uint32_t* depth;      // [n_maps] inner levels of map m's tree (0: empty map)
+  const uint32_t* level0;     // [n_maps] first level whose nodes hold at most kForestSegMax points
+  uint32_t n_maps;
+};
+
+/// What the search reads: the record blocks, each map's centre [4] and the tables above.
+struct ForestView {
+  const float4* pnodes;
+  const double* centres;
+  const uint32_t* pt_off;
+  const uint32_t* node_base;
+};
+
+/// One build (device pointers; orig_* in original order, leaf_* in leaf order).
+struct ForestBuild {
+  ForestTables tables;
+  uint32_t n, n_segments, n_slots, radix_levels, max_depth;
+  int key_bits, sm_count;
+  const double* points;   // n x 4
+  const double* normals;  // n x 4 or null
+  const double* covs;     // n x 16 or null
+  double* centres;        // [n_maps][4]
+  float4 *orig_pts, *orig_normals, *orig_covA, *orig_covB;
+  float4 *leaf_pts, *leaf_normals, *leaf_covA, *leaf_covB;
+  uint32_t* perm;         // leaf position -> global original position
+  float4* pnodes;
+  uint32_t* boxes;        // n_segments x 6
+  uint64_t *keys_in, *keys_out;
+  uint32_t* vals_in;
+  void* sort_temp;
+  size_t sort_temp_bytes;
+};
+
+/// Launches the whole build on st (no host synchronisation); *launches = launches made (memory copies and radix sorts count one each).
+cudaError_t launch_forest_build(const ForestBuild& b, cudaStream_t st, int* launches);
+/// Exact nearest neighbour of every point of the call's tiles in its member's map; vcorr[vfirst + k] = global leaf position or kNone.
+/// max_depth: stack entries per lane (inner levels of the deepest tree + 1, at most 40); bound: the FP32 search bound (search_bound).
+cudaError_t launch_forest_search(const BatchParams& B, const ForestView& F, uint32_t n_tiles, int max_depth, float bound, uint32_t* vcorr, cudaStream_t st);
+
+}  // namespace sgb

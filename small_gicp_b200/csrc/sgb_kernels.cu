@@ -420,6 +420,8 @@ __global__ void curve_keys_kernel(const float4* __restrict__ pts, size_t n, cons
 // consecutive points, hierarchy = the implicit perfect binary tree over P = 2^ceil(log2(#leaves)) leaf slots (node i has
 // children 2i+1, 2i+2; missing leaves are empty boxes that no query ever enters).  Every step is a data-parallel kernel;
 // the output is the same 64-byte packet record array the search kernel consumes.
+// sgb_forest.cu keeps copies of the helpers and kernels below (tree_bound ... lbvh_level_kernel) for many trees at once (forest_*): a
+// change to one side belongs in the other.
 // ---------------------------------------------------------------------------------------------
 __device__ __forceinline__ void lbvh_store_child(float4* pnodes, uint32_t child_heap, const float lo[3], const float hi[3], uint32_t a, uint32_t b) {
   const uint32_t parent = (child_heap - 1u) >> 1, side = (child_heap & 1u) ? 0u : 1u;  // odd heap index = left child
@@ -513,7 +515,8 @@ __global__ void kd_keys_kernel(const float4* __restrict__ pts, uint32_t n, uint3
 // (shared-memory atomics on order-preserving integer images of the floats), key = (node, coordinate along the node's widest axis),
 // bitonic sort of (key, slot), permutation of the points.  Above level0 a level is ~12 launches (boxes, keys, radix sort, gather); for a
 // 16k-point frame that was 9 levels = ~110 launches of pure launch latency, now 3 levels + this kernel.  Same keys, same balanced
-// position boundaries as the per-level path (ties may land differently -- any order is a valid tree).
+// position boundaries as the per-level path (ties may land differently -- any order is a valid tree).  forest_refine_smem_kernel
+// (sgb_forest.cu) is its copy over many maps' segments.
 constexpr uint32_t kKdSegMax = 2048;
 constexpr uint32_t kKdSegNodes = 128;
 __global__ void __launch_bounds__(1024) kd_refine_smem_kernel(float4* __restrict__ leaf_pts, uint32_t* __restrict__ perm, uint32_t n, uint32_t level0, uint32_t levels) {

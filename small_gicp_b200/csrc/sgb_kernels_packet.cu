@@ -12,6 +12,7 @@
 // The tree is the kd-tree (same leaves, same permutation) with each inner node carrying the tight bounding boxes of its two
 // children (64 B, "BVH2" layout):  float4[4] = {L.lo|L.a, L.hi|L.b, R.lo|R.a, R.hi|R.b} where a child is a leaf
 // (a = first point, b = count > 0) or an inner node (a = node index, b = 0).
+// forest_search_kernel (sgb_forest.cu) copies this walk for a batch over many trees, one member per warp.
 #include <algorithm>
 #include <cfloat>
 #include <cstdlib>

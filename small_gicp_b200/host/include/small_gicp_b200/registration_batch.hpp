@@ -82,6 +82,22 @@ struct BatchRegistration {
     return run(ctx, init_Ts);
   }
 
+  /// One RegistrationResult per (target, source) pair, in order: source m from init_Ts[m] against targets[m] through its own kd-tree
+  /// (Registration<>::align with a KdTree of the target), all pairs in one sgb_align_batch call.  The trees are built on the device in one
+  /// sgb_target_build_kdtrees call; the targets need normals for point-to-plane and covariances for GICP.  The context's target is
+  /// replaced, so the reduction's target mirror is dropped.
+  template <typename Target, typename Source>
+  std::vector<RegistrationResult> align(const std::vector<Target>& targets, const std::vector<Source>& sources, const std::vector<Isometry3d>& init_Ts) const {
+    if (sources.size() != init_Ts.size()) throw std::runtime_error("BatchRegistration: one initial pose per source");
+    if (targets.size() != sources.size()) throw std::runtime_error("BatchRegistration: one target per source");
+    sgb_ctx* ctx = reduction.context();
+    reduction.invalidate();
+    const Concatenated tgt(targets, true), src(sources);
+    check(ctx, sgb_target_build_kdtrees(ctx, targets.size(), tgt.offsets.data(), tgt.points.data(), tgt.normals_or_null(), tgt.covs_or_null()));
+    check(ctx, sgb_source_set_batch(ctx, sources.size(), src.offsets.data(), src.points.data(), src.covs_or_null()));
+    return run(ctx, init_Ts);
+  }
+
   TerminationCriteria criteria;
   CorrespondenceRejector rejector;
   PointFactorSetting point_factor;
@@ -90,29 +106,33 @@ struct BatchRegistration {
   Optimizer optimizer;
 
 private:
-  /// clouds concatenated in the C-ABI's batch layout; covariances only if every non-empty cloud has them
+  /// clouds concatenated in the C-ABI's batch layout; covariances (and with want_normals normals) only if every non-empty cloud has them
   struct Concatenated {
     std::vector<size_t> offsets;
-    std::vector<double> points, covs;
-    bool has_covs = true;
+    std::vector<double> points, normals, covs;
+    bool has_normals = true, has_covs = true;
     template <typename Cloud>
-    explicit Concatenated(const std::vector<Cloud>& clouds) : offsets(clouds.size() + 1, 0) {
+    explicit Concatenated(const std::vector<Cloud>& clouds, bool want_normals = false) : offsets(clouds.size() + 1, 0), has_normals(want_normals) {
       const size_t B = clouds.size();
       std::vector<detail::CloudArrays<Cloud>> arrays;
       arrays.reserve(B);
       for (size_t m = 0; m < B; m++) {
-        arrays.emplace_back(clouds[m], false);
+        arrays.emplace_back(clouds[m], want_normals);
         offsets[m + 1] = offsets[m] + arrays[m].n;
+        has_normals = has_normals && (arrays[m].n == 0 || arrays[m].normals);
         has_covs = has_covs && (arrays[m].n == 0 || arrays[m].covs);
       }
       points.resize(4 * offsets[B]);
+      normals.resize(has_normals ? 4 * offsets[B] : 0);
       covs.resize(has_covs ? 16 * offsets[B] : 0);
       for (size_t m = 0; m < B; m++) {
         if (arrays[m].n == 0) continue;
         std::memcpy(points.data() + 4 * offsets[m], arrays[m].points, arrays[m].n * 4 * sizeof(double));
+        if (has_normals) std::memcpy(normals.data() + 4 * offsets[m], arrays[m].normals, arrays[m].n * 4 * sizeof(double));
         if (has_covs) std::memcpy(covs.data() + 16 * offsets[m], arrays[m].covs, arrays[m].n * 16 * sizeof(double));
       }
     }
+    const double* normals_or_null() const { return has_normals ? normals.data() : nullptr; }
     const double* covs_or_null() const { return has_covs ? covs.data() : nullptr; }
   };
 

@@ -118,6 +118,7 @@ std::vector<RegistrationResult> run_pairs(const Options& o, const std::vector<Po
   set_rejector(reg, o, std::is_same<Rejector, DistanceRejector>());
   set_general(reg, o, std::is_same<General, RestrictDoFFactor>());
   set_robust(reg.point_factor, o, std::integral_constant<bool, kRobust>());
+  if (o.tree == 1) return reg.align(targets, sources, init);  // TREE_DEVICE_KDTREE: a kd-tree per target
   return reg.align(targets, sources, init, o.voxel_resolution, o.voxel_search_offsets);
 }
 
@@ -153,11 +154,10 @@ struct PairsJob {
   std::vector<RegistrationResult> results;
   template <typename Factor, typename General, typename Rejector, typename Optimizer, bool kRobust>
   void call() {
-    if constexpr (std::is_same_v<Factor, PointToPlaneICPFactor> || std::is_same_v<Factor, RobustFactor<Huber, PointToPlaneICPFactor>> ||
-                  std::is_same_v<Factor, RobustFactor<Cauchy, PointToPlaneICPFactor>>)
-      throw std::runtime_error("sgbh_align_batch_pairs: a voxel map has no normals (point-to-plane)");
-    else
-      results = run_pairs<Factor, General, Rejector, Optimizer, kRobust>(o, targets, sources, init);
+    constexpr bool plane = std::is_same_v<Factor, PointToPlaneICPFactor> || std::is_same_v<Factor, RobustFactor<Huber, PointToPlaneICPFactor>> ||
+                           std::is_same_v<Factor, RobustFactor<Cauchy, PointToPlaneICPFactor>>;
+    if (plane && o.tree != 1) throw std::runtime_error("sgbh_align_batch_pairs: a voxel map has no normals (point-to-plane)");
+    results = run_pairs<Factor, General, Rejector, Optimizer, kRobust>(o, targets, sources, init);
   }
 };
 
@@ -295,10 +295,11 @@ int sgbh_align_batch(size_t n_target, const double* target_pts4, const double* t
   }
 }
 
-/// BatchRegistration<...>::align over (target, source) pairs: the options of sgbh_align (voxel_resolution and search offsets of the maps
-/// among them); target m = rows target_offsets[m] .. target_offsets[m+1] (with covariances or none), source m likewise.  Outputs as
-/// sgbh_align_batch's.
-int sgbh_align_batch_pairs(size_t n_pairs, const size_t* target_offsets, const double* target_pts4, const double* target_covs16, const size_t* source_offsets,
+/// BatchRegistration<...>::align over (target, source) pairs: the options of sgbh_align (tree 1 = TREE_DEVICE_KDTREE: a kd-tree per
+/// target; otherwise a Gaussian voxel map per target with voxel_resolution and search offsets); target m = rows target_offsets[m] ..
+/// target_offsets[m+1] (with normals / covariances or none), source m likewise.  Outputs as sgbh_align_batch's.
+int sgbh_align_batch_pairs(size_t n_pairs, const size_t* target_offsets, const double* target_pts4, const double* target_normals4, const double* target_covs16,
+                           const size_t* source_offsets,
                            const double* source_pts4, const double* source_covs16, const double* options21, const double* init_T16xB, double* T_out16xB,
                            double* scalars_out4xB, double* H_out36xB, double* b_out6xB) {
   try {
@@ -308,7 +309,7 @@ int sgbh_align_batch_pairs(size_t n_pairs, const size_t* target_offsets, const d
     for (size_t m = 0; m < n_pairs; m++) {
       const size_t to = target_offsets[m], tn = target_offsets[m + 1] - to;
       const size_t so = source_offsets[m], sn = source_offsets[m + 1] - so;
-      targets[m] = *make_cloud(tn, target_pts4 + 4 * to, nullptr, target_covs16 ? target_covs16 + 16 * to : nullptr);
+      targets[m] = *make_cloud(tn, target_pts4 + 4 * to, target_normals4 ? target_normals4 + 4 * to : nullptr, target_covs16 ? target_covs16 + 16 * to : nullptr);
       sources[m] = *make_cloud(sn, source_pts4 + 4 * so, nullptr, source_covs16 ? source_covs16 + 16 * so : nullptr);
       std::memcpy(init[m].matrix().data(), init_T16xB + 16 * m, sizeof(double) * 16);
     }

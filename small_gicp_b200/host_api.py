@@ -169,14 +169,20 @@ def align_batch_pairs(
     voxel_search_offsets=1,
     dof_mask=None,
     device=0,
+    tree=TREE_VOXELMAP,
+    target_normals=None,
 ):
     """BatchRegistration<...>::align(targets, sources, init_Ts, voxel_resolution, search_offsets) (C++ host mirror): source m against a
-    Gaussian voxel map of targets[m], every pair in one batched call.  targets / sources: lists of (N_m, 3|4) arrays; target_covs /
-    source_covs: None or lists of (N_m, 4, 4).  Keyword arguments as align_batch().  Returns capi.BatchAlignResult."""
+    Gaussian voxel map of targets[m], every pair in one batched call; with tree=TREE_DEVICE_KDTREE BatchRegistration<...>::align(targets,
+    sources, init_Ts): source m against a kd-tree of targets[m].  targets / sources: lists of (N_m, 3|4) arrays; target_covs / source_covs:
+    None or lists of (N_m, 4, 4); target_normals: None or a list of (N_m, 4) (point-to-plane, kd-trees only).  Keyword arguments as
+    align_batch().  Returns capi.BatchAlignResult."""
     L = _lib()
+    if tree not in (TREE_VOXELMAP, TREE_DEVICE_KDTREE):
+        raise capi.SgbError("align_batch_pairs: tree must be TREE_VOXELMAP or TREE_DEVICE_KDTREE")
     if not hasattr(L.sgbh_align_batch_pairs, "_typed"):
         L.sgbh_align_batch_pairs.restype = C.c_int
-        L.sgbh_align_batch_pairs.argtypes = [C.c_size_t, C.POINTER(C.c_size_t), _dp, _dp, C.POINTER(C.c_size_t), _dp, _dp, _dp, _dp, _dp, _dp, _dp, _dp]
+        L.sgbh_align_batch_pairs.argtypes = [C.c_size_t, C.POINTER(C.c_size_t), _dp, _dp, _dp, C.POINTER(C.c_size_t), _dp, _dp, _dp, _dp, _dp, _dp, _dp, _dp]
         L.sgbh_align_batch_pairs._typed = True
     assert len(targets) == len(sources), "one target per source"
     B = len(sources)
@@ -191,15 +197,18 @@ def align_batch_pairs(
 
     to, tp, tc = concat(targets, target_covs)
     so, sp, sc = concat(sources, source_covs)
+    tn = None if target_normals is None else np.ascontiguousarray(np.concatenate([_f64(x) for x in target_normals]) if B else np.zeros((0, 4)))
+    if tn is not None:
+        assert tn.shape == (tp.shape[0], 4)
     opts = np.zeros(21)
-    opts[:13] = [factor, robust, robust_c, rejector, max_dist_sq, optimizer, max_iterations, rotation_eps, translation_eps, TREE_VOXELMAP, voxel_resolution,
+    opts[:13] = [factor, robust, robust_c, rejector, max_dist_sq, optimizer, max_iterations, rotation_eps, translation_eps, tree, voxel_resolution,
                  voxel_search_offsets, 0 if dof_mask is None else 1]
     opts[13:19] = 1.0 if dof_mask is None else np.asarray(dof_mask, dtype=float)
     opts[19] = device
     Ts = np.tile(np.eye(4), (B, 1, 1)) if init_Ts is None else np.asarray(init_Ts, dtype=float).reshape(B, 4, 4)
     T0 = np.ascontiguousarray(Ts.transpose(0, 2, 1))
     T, sc4, H, b = np.zeros((max(B, 1), 16)), np.zeros((max(B, 1), 4)), np.zeros((max(B, 1), 36)), np.zeros((max(B, 1), 6))
-    rc = L.sgbh_align_batch_pairs(B, to.ctypes.data_as(C.POINTER(C.c_size_t)), _d(tp), _d(tc), so.ctypes.data_as(C.POINTER(C.c_size_t)), _d(sp), _d(sc),
+    rc = L.sgbh_align_batch_pairs(B, to.ctypes.data_as(C.POINTER(C.c_size_t)), _d(tp), _d(tn), _d(tc), so.ctypes.data_as(C.POINTER(C.c_size_t)), _d(sp), _d(sc),
                                   _d(opts), _d(T0), _d(T), _d(sc4), _d(H), _d(b))
     if rc != 0:
         raise capi.SgbError(L.sgbh_last_error().decode())
