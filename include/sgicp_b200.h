@@ -274,6 +274,23 @@ int sgb_target_adopt_source(sgb_ctx* ctx);
  * voxel = mean of its points, voxels ordered by the reference's 63-bit key (x | y<<21 | z<<42 of floor(p/leaf)+2^20);
  * points whose voxel coordinate leaves the 21-bit range are dropped.  out_points_xyz1 must hold n points. */
 int sgb_voxelgrid_sampling(sgb_ctx* ctx, size_t n, const double* points_xyz1, double leaf_size, double* out_points_xyz1, size_t* n_out);
+/* Many clouds at once, for preparing a sequence of frames: the outputs feed sgb_target_build_kdtrees / sgb_target_build_voxelmaps /
+ * sgb_source_set_batch.  offsets: n_clouds + 1 ascending entries, offsets[0] = 0; cloud c = points offsets[c] .. offsets[c+1] (empty clouds
+ * allowed); host, page-locked or device memory.  Neither call changes the context's target, source, batch, seeds or linearisation cache.
+ * sgb_voxelgrid_sampling_batch: cloud c's output is sgb_voxelgrid_sampling of cloud c alone, bit for bit, at out_points_xyz1[out_offsets[c]
+ * .. out_offsets[c+1]) (out_points_xyz1 must hold offsets[n_clouds] points; out_offsets: host memory, n_clouds + 1 entries).  A launch
+ * count independent of n_clouds and one host synchronisation (a host out_points_xyz1 adds the copy of the means).  n_clouds <=
+ * SGB_BATCH_MAX_MEMBERS, fewer than 2^31 points in all, leaf_size > 0, else the call fails with a message. */
+int sgb_voxelgrid_sampling_batch(sgb_ctx* ctx, size_t n_clouds, const size_t* offsets, const double* points_xyz1, double leaf_size,
+                                 double* out_points_xyz1, size_t* out_offsets);
+/* sgb_estimate_features_batch: cloud c's normals / covariances are those of sgb_estimate_features of cloud c alone, in the caller's
+ * concatenated order, EXCEPT where exact FP32 distance ties among a point's k + 4 nearest candidates are ranked differently (cloud c's
+ * kd-tree is built as sgb_target_build_kdtrees builds map c, without the single call's curve pre-sort, so equal coordinates may sit in
+ * another order); a cloud's results are bit-identical whatever else is in the batch, ties included.  Either output may be NULL.
+ * num_neighbors in 1..32, n_clouds <= SGB_BATCH_MAX_MEMBERS, fewer than 2^30 points in all, else the call fails with a message.  The
+ * launch count depends on the size of the largest cloud only; one host synchronisation at the end, as sgb_estimate_features. */
+int sgb_estimate_features_batch(sgb_ctx* ctx, size_t n_clouds, const size_t* offsets, const double* points_xyz1, int num_neighbors,
+                                double* out_normals_xyz0 /*or NULL*/, double* out_covs_4x4 /*or NULL*/);
 
 #ifdef __cplusplus
 }

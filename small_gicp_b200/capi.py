@@ -84,6 +84,8 @@ _SIGNATURES = {
     "sgb_source_estimate_features": (C.c_int, [_vp, C.c_int]),
     "sgb_target_adopt_source": (C.c_int, [_vp]),
     "sgb_voxelgrid_sampling": (C.c_int, [_vp, C.c_size_t, _dp, C.c_double, _dp, C.POINTER(C.c_size_t)]),
+    "sgb_voxelgrid_sampling_batch": (C.c_int, [_vp, C.c_size_t, C.POINTER(C.c_size_t), _dp, C.c_double, _dp, C.POINTER(C.c_size_t)]),
+    "sgb_estimate_features_batch": (C.c_int, [_vp, C.c_size_t, C.POINTER(C.c_size_t), _dp, C.c_int, _dp, _dp]),
 }
 
 
@@ -505,3 +507,53 @@ class Context:
         m = C.c_size_t(0)
         self._check(self._L.sgb_voxelgrid_sampling(self._h, p.shape[0], _d(p), float(leaf_size), _d(out), C.byref(m)))
         return out[: int(m.value)].copy()
+
+    # ---- many clouds at once (frames of a sequence): plain concatenated arrays in the caller's order ----
+    @staticmethod
+    def _clouds(points_list, who):
+        """a list of (N_m, 3|4) clouds, or (points (N, 3|4), offsets (B + 1,)) -> (points (N, 4), offsets as size_t); CUDA tensors stay
+        on the device"""
+        if isinstance(points_list, tuple):
+            points, offsets = points_list
+            p = _points4(points)
+            offsets = np.ascontiguousarray(offsets.cpu().numpy() if _is_dev(offsets) else offsets, dtype=np.uintp)
+            if offsets.ndim != 1 or offsets.size < 1 or int(offsets[-1]) != p.shape[0]:
+                raise SgbError(f"{who}: offsets must have B + 1 entries ending at the point count {p.shape[0]}")
+            return p, offsets
+        members = [_points4(x) for x in points_list]
+        offsets = np.zeros(len(members) + 1, dtype=np.uintp)
+        offsets[1:] = np.cumsum([m.shape[0] for m in members])
+        if members and all(_is_dev(m) for m in members):
+            import torch
+
+            return torch.cat(members).contiguous(), offsets
+        p = np.concatenate([m.cpu().numpy() if _is_dev(m) else m for m in members]) if members else np.zeros((0, 4))
+        return np.ascontiguousarray(p), offsets
+
+    def voxelgrid_sampling_batch(self, points_list, leaf_size):
+        """voxelgrid_sampling of every cloud in one call: points_list as for build_target_voxelmaps.  Returns (points (M, 4), offsets
+        (B + 1,) int64): cloud c's voxels are points[offsets[c]:offsets[c+1]], bit-identical to voxelgrid_sampling of that cloud alone.
+        CUDA tensors in give a CUDA tensor out."""
+        p, offsets = self._clouds(points_list, "voxelgrid_sampling_batch")
+        out = p.new_empty(p.shape) if _is_dev(p) else np.empty_like(p)
+        out_off = np.zeros(offsets.size, dtype=np.uintp)
+        self._check(self._L.sgb_voxelgrid_sampling_batch(self._h, offsets.size - 1, offsets.ctypes.data_as(C.POINTER(C.c_size_t)), _d(p), float(leaf_size),
+                                                         _d(out), out_off.ctypes.data_as(C.POINTER(C.c_size_t))))
+        m = int(out_off[-1])
+        return (out[:m].clone() if _is_dev(out) else out[:m].copy()), out_off.astype(np.int64)
+
+    def estimate_features_batch(self, points_list, num_neighbors=20, normals=True, covs=True):
+        """estimate_features of every cloud in one call: points_list as for build_target_voxelmaps.  Returns (normals (N, 4) | None,
+        covs (N, 4, 4) | None) in the concatenated order; CUDA tensors in give CUDA tensors out."""
+        p, offsets = self._clouds(points_list, "estimate_features_batch")
+        if _is_dev(p) and p.is_cuda:
+            import torch
+
+            n_out = torch.empty((p.shape[0], 4), dtype=torch.float64, device=p.device) if normals else None
+            c_out = torch.empty((p.shape[0], 4, 4), dtype=torch.float64, device=p.device) if covs else None
+        else:
+            n_out = np.empty((p.shape[0], 4)) if normals else None
+            c_out = np.empty((p.shape[0], 4, 4)) if covs else None
+        self._check(self._L.sgb_estimate_features_batch(self._h, offsets.size - 1, offsets.ctypes.data_as(C.POINTER(C.c_size_t)), _d(p), int(num_neighbors),
+                                                        _d(n_out), _d(c_out)))
+        return n_out, c_out

@@ -189,6 +189,123 @@ int sort_into_voxels(sgb_ctx* ctx, size_t n, double inv_leaf) {
   return 0;
 }
 
+// n_maps clouds (host offsets, checked; offsets[n_maps] = n > 0) at stage_pts sorted into per-cloud voxels of edge 1 / inv_leaf
+// (sgb_preprocess.cu: voxelmaps_*): keys_in / vals_in = voxel keys (bit 63 = the parity of the cloud's rank among the clouds with points)
+// / original indices in (cloud, valid, key) order, pre_heads[0, n] = voxel heads, pre_slots = their exclusive scan (pre_slots[n] = voxel
+// count), regions[m].z / .w = cloud m's first voxel / voxel count, vm_caps[0, n_maps] = the table capacity of each cloud's voxel map.
+// sort_temp holds cap_scan_bytes, enough for the scan of those capacities.  7 launches, none of them per cloud.
+int sort_into_voxelmaps(sgb_ctx* ctx, size_t n_maps, const size_t* offsets, double inv_leaf, uint4* regions, size_t& cap_scan_bytes) {
+  const size_t n = offsets[n_maps];
+  const uint32_t maps = static_cast<uint32_t>(n_maps);
+  // the point offsets, then per map the parity of its rank among the maps with points (bit 63 of its stored keys, sgb_preprocess.cu)
+  std::vector<uint32_t> off32(offsets, offsets + n_maps + 1);
+  off32.resize(2 * n_maps + 1);
+  uint32_t rank = 0;
+  for (size_t m = 0; m < n_maps; m++) {
+    off32[n_maps + 1 + m] = rank & 1u;
+    if (offsets[m + 1] > offsets[m]) rank++;
+  }
+  CU(ctx->vm_offsets.reserve(off32.size() * sizeof(uint32_t)));
+  CU(ctx->vm_caps.reserve(2 * (n_maps + 1) * sizeof(uint32_t)));
+  CU(ctx->vm_keys.reserve(n * sizeof(uint64_t)));
+  CU(ctx->vm_vals.reserve(n * sizeof(uint32_t)));
+  CU(cudaMemcpyAsync(ctx->vm_offsets.p, off32.data(), off32.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
+  CU(ctx->keys_in.reserve(n * sizeof(uint64_t)));
+  CU(ctx->keys_out.reserve(n * sizeof(uint64_t)));
+  CU(ctx->vals_in.reserve(n * sizeof(uint32_t)));
+  CU(ctx->pre_vals_out.reserve(n * sizeof(uint32_t)));
+  CU(ctx->pre_heads.reserve((n + 1) * sizeof(uint32_t)));
+  CU(ctx->pre_slots.reserve((n + 1) * sizeof(uint32_t)));
+  int map_bits = 1;  // (map << 1 | valid) < 2 n_maps
+  while ((1ull << map_bits) < 2ull * n_maps) map_bits++;
+  uint64_t* keys = ctx->keys_in.as<uint64_t>();
+  uint32_t* vals = ctx->vals_in.as<uint32_t>();
+  uint32_t* caps = ctx->vm_caps.as<uint32_t>();
+  size_t sort_bytes = 0, map_sort_bytes = 0, scan_bytes = 0;
+  cap_scan_bytes = 0;
+  CU(sort_pairs_u64_u32_bits(nullptr, sort_bytes, keys, ctx->keys_out.as<uint64_t>(), vals, ctx->pre_vals_out.as<uint32_t>(), n, 63, ctx->stream));
+  CU(sort_pairs_u64_u32_bits(nullptr, map_sort_bytes, keys, ctx->vm_keys.as<uint64_t>(), vals, ctx->vm_vals.as<uint32_t>(), n, map_bits, ctx->stream));
+  CU(exclusive_sum_u32(nullptr, scan_bytes, ctx->pre_heads.as<uint32_t>(), ctx->pre_slots.as<uint32_t>(), n + 1, ctx->stream));
+  CU(exclusive_sum_u32(nullptr, cap_scan_bytes, caps, caps + n_maps + 1, n_maps + 1, ctx->stream));
+  CU(ctx->sort_temp.reserve(std::max(std::max(sort_bytes, map_sort_bytes), std::max(scan_bytes, cap_scan_bytes))));
+  // (map, valid, key) order: the key sort, then a stable sort by (map, valid); keys_in / vals_in end up holding the ordered keys / indices
+  CU(launch_voxel_keys(ctx->stage_pts.as<double>(), n, inv_leaf, keys, vals, ctx->sm_count, ctx->stream));
+  CU(sort_pairs_u64_u32_bits(ctx->sort_temp.p, sort_bytes, keys, ctx->keys_out.as<uint64_t>(), vals, ctx->pre_vals_out.as<uint32_t>(), n, 63, ctx->stream));
+  CU(launch_voxelmaps_sort_keys(ctx->keys_out.as<uint64_t>(), ctx->pre_vals_out.as<uint32_t>(), n, ctx->vm_offsets.as<uint32_t>(), maps, keys, vals, ctx->sm_count,
+                                ctx->stream));
+  CU(sort_pairs_u64_u32_bits(ctx->sort_temp.p, map_sort_bytes, keys, ctx->vm_keys.as<uint64_t>(), vals, ctx->vm_vals.as<uint32_t>(), n, map_bits, ctx->stream));
+  CU(launch_voxelmaps_order(ctx->vm_keys.as<uint64_t>(), ctx->vm_vals.as<uint32_t>(), ctx->keys_out.as<uint64_t>(), ctx->pre_vals_out.as<uint32_t>(), n,
+                            ctx->vm_offsets.as<uint32_t>() + n_maps + 1, keys,
+                            vals, ctx->pre_heads.as<uint32_t>(), ctx->sm_count, ctx->stream));
+  CU(exclusive_sum_u32(ctx->sort_temp.p, scan_bytes, ctx->pre_heads.as<uint32_t>(), ctx->pre_slots.as<uint32_t>(), n + 1, ctx->stream));
+  // per map: voxels and table capacity
+  CU(launch_voxelmaps_count(ctx->vm_offsets.as<uint32_t>(), maps, ctx->pre_slots.as<uint32_t>(), regions, caps, ctx->stream));
+  ctx->launches += 7;
+  return 0;
+}
+
+// The layout of a forest over n_maps clouds (host offsets, checked), as build_lbvh sizes one tree per map: P = 2^depth leaf slots of at
+// most kLbvhLeafPoints points, P - 1 packet records, and the first level whose nodes fit a shared-memory segment.  tab: the uint32
+// ForestTables (pt_off, slot_off, seg_off: n_maps + 1 each; node_base, depth, level0: n_maps each).
+struct ForestPlan {
+  std::vector<uint32_t> tab;
+  uint32_t max_depth = 0, radix_levels = 0, n_segments = 0, n_slots = 0;
+  size_t nodes = 0;
+  int key_bits = 32;
+};
+void plan_forest(size_t n_maps, const size_t* offsets, ForestPlan& p) {
+  p.tab.assign(3 * (n_maps + 1) + 3 * n_maps, 0);
+  uint32_t* pt_off = p.tab.data();
+  uint32_t* slot_off = pt_off + (n_maps + 1);
+  uint32_t* seg_off = slot_off + (n_maps + 1);
+  uint32_t* node_base = seg_off + (n_maps + 1);
+  uint32_t* depth = node_base + n_maps;
+  uint32_t* level0 = depth + n_maps;
+  for (size_t m = 0; m < n_maps; m++) {
+    const uint32_t nm = static_cast<uint32_t>(offsets[m + 1] - offsets[m]);
+    pt_off[m] = static_cast<uint32_t>(offsets[m]);
+    node_base[m] = static_cast<uint32_t>(p.nodes);
+    uint32_t P = 0, d = 0, l0 = 0, segs = 0;
+    if (nm) {
+      P = 2;
+      d = 1;
+      while (static_cast<uint64_t>(P) * kLbvhLeafPoints < nm) {
+        P <<= 1;
+        d++;
+      }
+      l0 = kd_smem_first_level(nm, d);
+      segs = 1u << l0;
+      p.nodes += P - 1;
+    }
+    depth[m] = d;
+    level0[m] = l0;
+    slot_off[m + 1] = slot_off[m] + P;
+    seg_off[m + 1] = seg_off[m] + segs;
+    p.max_depth = std::max(p.max_depth, d);
+    p.radix_levels = std::max(p.radix_levels, l0);
+  }
+  pt_off[n_maps] = static_cast<uint32_t>(offsets[n_maps]);
+  p.n_segments = seg_off[n_maps];
+  p.n_slots = slot_off[n_maps];
+  p.key_bits = 32;
+  while ((1ull << (p.key_bits - 32)) < p.n_segments) p.key_bits++;
+}
+// the device tables of a plan uploaded to tp
+ForestTables forest_tables(const uint32_t* tp, size_t n_maps) {
+  return ForestTables{tp, tp + (n_maps + 1), tp + 2 * (n_maps + 1), tp + 3 * (n_maps + 1), tp + 3 * (n_maps + 1) + n_maps,
+                      tp + 3 * (n_maps + 1) + 2 * n_maps, static_cast<uint32_t>(n_maps)};
+}
+
+// offsets of n_clouds clouds (what: "map" or "cloud") as the many-cloud calls take them: n_clouds + 1 ascending entries from 0
+int check_offsets(sgb_ctx* ctx, const std::string& who, size_t n_clouds, const size_t* offsets, const std::string& what) {
+  if (n_clouds > SGB_BATCH_MAX_MEMBERS) return fail(ctx, 1, who + std::to_string(n_clouds) + " " + what + "s, at most " + std::to_string(SGB_BATCH_MAX_MEMBERS));
+  if (!offsets) return fail(ctx, 1, who + "null offsets");
+  if (offsets[0] != 0) return fail(ctx, 1, who + "offsets[0] must be 0");
+  for (size_t m = 0; m < n_clouds; m++)
+    if (offsets[m + 1] < offsets[m]) return fail(ctx, 1, who + "offsets must be ascending (" + what + " " + std::to_string(m) + ")");
+  return 0;
+}
+
 }  // namespace
 
 extern "C" {
@@ -306,6 +423,129 @@ int sgb_voxelgrid_sampling(sgb_ctx* ctx, size_t n, const double* points, double 
   return 0;
 }
 
+// Many clouds down-sampled in one pass: the (cloud, valid, key) order of sgb_target_build_voxelmaps (sort_into_voxelmaps), whose bit 63
+// stops voxel_means_kernel's run over equal keys at every cloud boundary, so that cloud c's voxels are those of sgb_voxelgrid_sampling
+// of cloud c alone, in the same ascending key order, with their sums in the same ascending original index order.
+int sgb_voxelgrid_sampling_batch(sgb_ctx* ctx, size_t n_clouds, const size_t* offsets, const double* points, double leaf_size, double* out_points,
+                                 size_t* out_offsets) {
+  if (!ctx) return 1;
+  const std::string who = "sgb_voxelgrid_sampling_batch: ";
+  if (!out_offsets) return fail(ctx, 1, who + "null out_offsets");
+  if (int rc = check_offsets(ctx, who, n_clouds, offsets, "cloud")) return rc;
+  const size_t n = offsets[n_clouds];
+  if (n >= (1ull << 31)) return fail(ctx, 1, who + "too many points (fewer than 2^31 in all)");
+  if (n && (!points || !out_points)) return fail(ctx, 1, who + "null buffer");
+  if (!(leaf_size > 0.0)) return fail(ctx, 1, who + "leaf_size must be positive");
+  std::fill(out_offsets, out_offsets + n_clouds + 1, size_t{0});
+  if (n == 0) return 0;
+  CU(cudaSetDevice(ctx->device));
+  CU(ctx->stage_pts.reserve(n * 4 * sizeof(double)));
+  CU(cudaMemcpyAsync(ctx->stage_pts.p, points, n * 4 * sizeof(double), cudaMemcpyDefault, ctx->stream));
+  CU(ctx->pre_regions.reserve(n_clouds * sizeof(uint4)));
+  size_t cap_scan_bytes = 0;
+  if (int rc = sort_into_voxelmaps(ctx, n_clouds, offsets, 1.0 / leaf_size, ctx->pre_regions.as<uint4>(), cap_scan_bytes)) return rc;
+  // the means straight into a device-resident output (voxel ids are global, cloud after cloud); a host output goes through staging
+  cudaPointerAttributes attr = {};
+  CU(cudaPointerGetAttributes(&attr, out_points));
+  const bool direct = attr.type == cudaMemoryTypeManaged || (attr.type == cudaMemoryTypeDevice && attr.device == ctx->device);
+  if (!direct) CU(ctx->stage_covs.reserve(n * 4 * sizeof(double)));
+  double* means = direct ? out_points : ctx->stage_covs.as<double>();
+  CU(launch_voxel_means(ctx->keys_in.as<uint64_t>(), ctx->vals_in.as<uint32_t>(), ctx->pre_heads.as<uint32_t>(), ctx->pre_slots.as<uint32_t>(), n,
+                        ctx->stage_pts.as<double>(), means, ctx->sm_count, ctx->stream));
+  ctx->launches += 1;
+  // the one synchronisation: every cloud's first voxel, and the voxel count
+  std::vector<uint4> regions(n_clouds);
+  uint32_t* h = reinterpret_cast<uint32_t*>(ctx->h_out + 56);
+  CU(cudaMemcpyAsync(regions.data(), ctx->pre_regions.p, n_clouds * sizeof(uint4), cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaMemcpyAsync(h, ctx->pre_slots.as<uint32_t>() + n, sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));
+  const uint32_t count = h[0];
+  for (size_t c = 0; c < n_clouds; c++) out_offsets[c] = regions[c].z;
+  out_offsets[n_clouds] = count;
+  if (!direct && count) {
+    CU(cudaMemcpyAsync(out_points, ctx->stage_covs.p, static_cast<size_t>(count) * 4 * sizeof(double), cudaMemcpyDefault, ctx->stream));
+    CU(cudaStreamSynchronize(ctx->stream));
+  }
+  return 0;
+}
+
+// Features of many clouds: a forest over them (launch_forest_build, as sgb_target_build_kdtrees builds it, here in the preprocessing
+// scratch) and the single cloud's features body run on each point's own map (launch_forest_features).  Map m's tree is built from its own
+// points alone, so a cloud's results do not depend on the rest of the batch.
+int sgb_estimate_features_batch(sgb_ctx* ctx, size_t n_clouds, const size_t* offsets, const double* points, int num_neighbors, double* out_normals,
+                                double* out_covs) {
+  if (!ctx) return 1;
+  const std::string who = "sgb_estimate_features_batch: ";
+  if (int rc = check_offsets(ctx, who, n_clouds, offsets, "cloud")) return rc;
+  const size_t n = offsets[n_clouds];
+  if (num_neighbors < 1 || num_neighbors > 32) return fail(ctx, 1, who + "num_neighbors must be in 1..32");
+  if (n >= (1ull << 30)) return fail(ctx, 1, who + "too many points (fewer than 2^30 in all)");
+  if (n && !points) return fail(ctx, 1, who + "null points");
+  if (n == 0 || (!out_normals && !out_covs)) return 0;
+  CU(cudaSetDevice(ctx->device));
+  ForestPlan plan;
+  plan_forest(n_clouds, offsets, plan);
+  const size_t T = plan.tab.size();
+  CU(ctx->pre_tables.reserve(T * sizeof(uint32_t)));
+  // pageable host memory: staged before cudaMemcpyAsync returns
+  CU(cudaMemcpyAsync(ctx->pre_tables.p, plan.tab.data(), T * sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
+  CU(ctx->stage_pts.reserve(n * 4 * sizeof(double)));
+  CU(cudaMemcpyAsync(ctx->stage_pts.p, points, n * 4 * sizeof(double), cudaMemcpyDefault, ctx->stream));
+  CU(ctx->pre_centres.reserve(n_clouds * 4 * sizeof(double)));
+  CU(ctx->pre_pts.reserve(n * sizeof(float4)));
+  CU(ctx->pre_lo.reserve(n * sizeof(float4)));
+  CU(ctx->pre_leaf_pts.reserve(n * sizeof(float4)));
+  CU(ctx->pre_perm.reserve(n * sizeof(uint32_t)));
+  CU(ctx->pre_nodes.reserve(std::max<size_t>(plan.nodes, 1) * 64));
+  CU(ctx->pre_boxes.reserve(static_cast<size_t>(plan.n_segments) * 6 * sizeof(uint32_t)));
+  CU(ctx->keys_in.reserve(n * sizeof(uint64_t)));
+  CU(ctx->keys_out.reserve(n * sizeof(uint64_t)));
+  CU(ctx->vals_in.reserve(n * sizeof(uint32_t)));
+  size_t sort_bytes = 0;
+  if (plan.radix_levels) {
+    CU(sort_pairs_u64_u32_bits(nullptr, sort_bytes, ctx->keys_in.as<uint64_t>(), ctx->keys_out.as<uint64_t>(), ctx->vals_in.as<uint32_t>(),
+                               ctx->pre_perm.as<uint32_t>(), n, plan.key_bits, ctx->stream));
+    CU(ctx->sort_temp.reserve(sort_bytes));
+  }
+  ctx->src_tree_valid = false;  // the scratch tree buffers are about to hold this forest
+  ForestBuild b = {};
+  b.tables = forest_tables(ctx->pre_tables.as<uint32_t>(), n_clouds);
+  b.n = static_cast<uint32_t>(n);
+  b.n_segments = plan.n_segments;
+  b.n_slots = plan.n_slots;
+  b.radix_levels = plan.radix_levels;
+  b.max_depth = plan.max_depth;
+  b.key_bits = plan.key_bits;
+  b.sm_count = ctx->sm_count;
+  b.points = ctx->stage_pts.as<double>();
+  b.centres = ctx->pre_centres.as<double>();
+  b.orig_pts = ctx->pre_pts.as<float4>();
+  b.orig_lo = ctx->pre_lo.as<float4>();
+  b.leaf_pts = ctx->pre_leaf_pts.as<float4>();
+  b.perm = ctx->pre_perm.as<uint32_t>();
+  b.pnodes = ctx->pre_nodes.as<float4>();
+  b.boxes = ctx->pre_boxes.as<uint32_t>();
+  b.keys_in = ctx->keys_in.as<uint64_t>();
+  b.keys_out = ctx->keys_out.as<uint64_t>();
+  b.vals_in = ctx->vals_in.as<uint32_t>();
+  b.sort_temp = ctx->sort_temp.p;
+  b.sort_temp_bytes = sort_bytes;
+  int launches = 0;
+  CU(launch_forest_build(b, ctx->stream, &launches));
+  ctx->launches += launches;
+  if (out_normals) CU(ctx->pre_out_normals.reserve(n * 4 * sizeof(double)));
+  if (out_covs) CU(ctx->pre_out_covs.reserve(n * 16 * sizeof(double)));
+  const int mode = (out_normals ? 1 : 0) | (out_covs ? 2 : 0);
+  CU(launch_forest_features(ctx->pre_nodes.as<float4>(), ctx->pre_leaf_pts.as<float4>(), static_cast<uint32_t>(n), num_neighbors, b.tables,
+                            ctx->pre_centres.as<double>(), mode, out_normals ? ctx->pre_out_normals.as<double>() : nullptr,
+                            out_covs ? ctx->pre_out_covs.as<double>() : nullptr, static_cast<int>(plan.max_depth) + 1, ctx->pre_lo.as<float4>(), ctx->stream));
+  ctx->launches += 1;
+  if (out_normals) CU(cudaMemcpyAsync(out_normals, ctx->pre_out_normals.p, n * 4 * sizeof(double), cudaMemcpyDefault, ctx->stream));
+  if (out_covs) CU(cudaMemcpyAsync(out_covs, ctx->pre_out_covs.p, n * 16 * sizeof(double), cudaMemcpyDefault, ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));
+  return 0;
+}
+
 // The frame-stream hand-over (odometry_benchmark_small_gicp_tbb.cpp:41-43: `target_points = points; target_tree = tree;`): the cloud that was
 // the source of this align() is the target of the next one.  Everything that already exists on the device is taken over, not rebuilt.
 int sgb_target_adopt_source(sgb_ctx* ctx) {
@@ -406,11 +646,7 @@ int sgb_target_build_voxelmaps(sgb_ctx* ctx, size_t n_maps, const size_t* offset
                                int search_offsets) {
   if (!ctx) return 1;
   const std::string who = "sgb_target_build_voxelmaps: ";
-  if (n_maps > SGB_BATCH_MAX_MEMBERS) return fail(ctx, 1, who + std::to_string(n_maps) + " maps, at most " + std::to_string(SGB_BATCH_MAX_MEMBERS));
-  if (!offsets) return fail(ctx, 1, who + "null offsets");
-  if (offsets[0] != 0) return fail(ctx, 1, who + "offsets[0] must be 0");
-  for (size_t m = 0; m < n_maps; m++)
-    if (offsets[m + 1] < offsets[m]) return fail(ctx, 1, who + "offsets must be ascending (map " + std::to_string(m) + ")");
+  if (int rc = check_offsets(ctx, who, n_maps, offsets, "map")) return rc;
   const size_t n = offsets[n_maps];
   if (n >= (1ull << 31)) return fail(ctx, 1, who + "too many points");
   if (n && !points) return fail(ctx, 1, who + "null points");
@@ -423,57 +659,21 @@ int sgb_target_build_voxelmaps(sgb_ctx* ctx, size_t n_maps, const size_t* offset
   CU(ctx->vm_regions.reserve(M * sizeof(uint4)));
   if (n == 0) return 0;
   const uint32_t maps = static_cast<uint32_t>(n_maps);
-  // the point offsets, then per map the parity of its rank among the maps with points (bit 63 of its stored keys, sgb_preprocess.cu)
-  std::vector<uint32_t> off32(offsets, offsets + n_maps + 1);
-  off32.resize(2 * n_maps + 1);
-  uint32_t rank = 0;
-  for (size_t m = 0; m < n_maps; m++) {
-    off32[n_maps + 1 + m] = rank & 1u;
-    if (offsets[m + 1] > offsets[m]) rank++;
-  }
-  CU(ctx->vm_offsets.reserve(off32.size() * sizeof(uint32_t)));
-  CU(ctx->vm_caps.reserve(2 * (n_maps + 1) * sizeof(uint32_t)));
-  CU(ctx->vm_keys.reserve(n * sizeof(uint64_t)));
-  CU(ctx->vm_vals.reserve(n * sizeof(uint32_t)));
   CU(ctx->stage_pts.reserve(n * 4 * sizeof(double)));
   CU(cudaMemcpyAsync(ctx->stage_pts.p, points, n * 4 * sizeof(double), cudaMemcpyDefault, ctx->stream));
   if (covs) {
     CU(ctx->stage_covs.reserve(n * 16 * sizeof(double)));
     CU(cudaMemcpyAsync(ctx->stage_covs.p, covs, n * 16 * sizeof(double), cudaMemcpyDefault, ctx->stream));
   }
-  CU(cudaMemcpyAsync(ctx->vm_offsets.p, off32.data(), off32.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
-  CU(ctx->keys_in.reserve(n * sizeof(uint64_t)));
-  CU(ctx->keys_out.reserve(n * sizeof(uint64_t)));
-  CU(ctx->vals_in.reserve(n * sizeof(uint32_t)));
-  CU(ctx->pre_vals_out.reserve(n * sizeof(uint32_t)));
-  CU(ctx->pre_heads.reserve((n + 1) * sizeof(uint32_t)));
-  CU(ctx->pre_slots.reserve((n + 1) * sizeof(uint32_t)));
-  int map_bits = 1;  // (map << 1 | valid) < 2 n_maps
-  while ((1ull << map_bits) < 2ull * n_maps) map_bits++;
+  size_t cap_scan_bytes = 0;
+  if (int rc = sort_into_voxelmaps(ctx, n_maps, offsets, 1.0 / leaf_size, ctx->vm_regions.as<uint4>(), cap_scan_bytes)) return rc;
   uint64_t* keys = ctx->keys_in.as<uint64_t>();
   uint32_t* vals = ctx->vals_in.as<uint32_t>();
   uint32_t* caps = ctx->vm_caps.as<uint32_t>();
   uint32_t* cap_scan = caps + n_maps + 1;
-  size_t sort_bytes = 0, map_sort_bytes = 0, scan_bytes = 0, cap_scan_bytes = 0;
-  CU(sort_pairs_u64_u32_bits(nullptr, sort_bytes, keys, ctx->keys_out.as<uint64_t>(), vals, ctx->pre_vals_out.as<uint32_t>(), n, 63, ctx->stream));
-  CU(sort_pairs_u64_u32_bits(nullptr, map_sort_bytes, keys, ctx->vm_keys.as<uint64_t>(), vals, ctx->vm_vals.as<uint32_t>(), n, map_bits, ctx->stream));
-  CU(exclusive_sum_u32(nullptr, scan_bytes, ctx->pre_heads.as<uint32_t>(), ctx->pre_slots.as<uint32_t>(), n + 1, ctx->stream));
-  CU(exclusive_sum_u32(nullptr, cap_scan_bytes, caps, cap_scan, n_maps + 1, ctx->stream));
-  CU(ctx->sort_temp.reserve(std::max(std::max(sort_bytes, map_sort_bytes), std::max(scan_bytes, cap_scan_bytes))));
-  // (map, valid, key) order: the key sort, then a stable sort by (map, valid); keys_in / vals_in end up holding the ordered keys / indices
-  CU(launch_voxel_keys(ctx->stage_pts.as<double>(), n, 1.0 / leaf_size, keys, vals, ctx->sm_count, ctx->stream));
-  CU(sort_pairs_u64_u32_bits(ctx->sort_temp.p, sort_bytes, keys, ctx->keys_out.as<uint64_t>(), vals, ctx->pre_vals_out.as<uint32_t>(), n, 63, ctx->stream));
-  CU(launch_voxelmaps_sort_keys(ctx->keys_out.as<uint64_t>(), ctx->pre_vals_out.as<uint32_t>(), n, ctx->vm_offsets.as<uint32_t>(), maps, keys, vals, ctx->sm_count,
-                                ctx->stream));
-  CU(sort_pairs_u64_u32_bits(ctx->sort_temp.p, map_sort_bytes, keys, ctx->vm_keys.as<uint64_t>(), vals, ctx->vm_vals.as<uint32_t>(), n, map_bits, ctx->stream));
-  CU(launch_voxelmaps_order(ctx->vm_keys.as<uint64_t>(), ctx->vm_vals.as<uint32_t>(), ctx->keys_out.as<uint64_t>(), ctx->pre_vals_out.as<uint32_t>(), n,
-                            ctx->vm_offsets.as<uint32_t>() + n_maps + 1, keys,
-                            vals, ctx->pre_heads.as<uint32_t>(), ctx->sm_count, ctx->stream));
-  CU(exclusive_sum_u32(ctx->sort_temp.p, scan_bytes, ctx->pre_heads.as<uint32_t>(), ctx->pre_slots.as<uint32_t>(), n + 1, ctx->stream));
-  // per map: voxels and table capacity, then the table's layout
-  CU(launch_voxelmaps_count(ctx->vm_offsets.as<uint32_t>(), maps, ctx->pre_slots.as<uint32_t>(), ctx->vm_regions.as<uint4>(), caps, ctx->stream));
+  // the table's layout
   CU(exclusive_sum_u32(ctx->sort_temp.p, cap_scan_bytes, caps, cap_scan, n_maps + 1, ctx->stream));
-  ctx->launches += 8;
+  ctx->launches += 1;
   // the one synchronisation: voxel count and table size (into the page-locked result slot)
   uint32_t* h = reinterpret_cast<uint32_t*>(ctx->h_out + 56);
   CU(cudaMemcpyAsync(h, ctx->pre_slots.as<uint32_t>() + n, sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
@@ -511,11 +711,7 @@ int sgb_target_build_voxelmaps(sgb_ctx* ctx, size_t n_maps, const size_t* offset
 int sgb_target_build_kdtrees(sgb_ctx* ctx, size_t n_maps, const size_t* offsets, const double* points, const double* normals, const double* covs) {
   if (!ctx) return 1;
   const std::string who = "sgb_target_build_kdtrees: ";
-  if (n_maps > SGB_BATCH_MAX_MEMBERS) return fail(ctx, 1, who + std::to_string(n_maps) + " maps, at most " + std::to_string(SGB_BATCH_MAX_MEMBERS));
-  if (!offsets) return fail(ctx, 1, who + "null offsets");
-  if (offsets[0] != 0) return fail(ctx, 1, who + "offsets[0] must be 0");
-  for (size_t m = 0; m < n_maps; m++)
-    if (offsets[m + 1] < offsets[m]) return fail(ctx, 1, who + "offsets must be ascending (map " + std::to_string(m) + ")");
+  if (int rc = check_offsets(ctx, who, n_maps, offsets, "map")) return rc;
   const size_t n = offsets[n_maps];
   if (n >= (1ull << 30)) return fail(ctx, 1, who + "too many points (fewer than 2^30 in all)");
   if (n && !points) return fail(ctx, 1, who + "null points");
@@ -525,49 +721,16 @@ int sgb_target_build_kdtrees(sgb_ctx* ctx, size_t n_maps, const size_t* offsets,
   CU(ctx->kt_centres.reserve(M * 4 * sizeof(double)));
   ctx->kt_depth = 1;
   if (n == 0) return 0;
-  // per map, as build_lbvh sizes one tree: P = 2^depth leaf slots of at most kLbvhLeafPoints points, P - 1 packet records, and the
-  // first level whose nodes fit a shared-memory segment
-  const size_t T = 3 * (n_maps + 1) + 3 * n_maps;
-  std::vector<uint32_t> tab(T, 0);
-  uint32_t* pt_off = tab.data();
-  uint32_t* slot_off = pt_off + (n_maps + 1);
-  uint32_t* seg_off = slot_off + (n_maps + 1);
-  uint32_t* node_base = seg_off + (n_maps + 1);
-  uint32_t* depth = node_base + n_maps;
-  uint32_t* level0 = depth + n_maps;
-  uint32_t max_depth = 0, radix_levels = 0;
-  size_t nodes = 0;
-  for (size_t m = 0; m < n_maps; m++) {
-    const uint32_t nm = static_cast<uint32_t>(offsets[m + 1] - offsets[m]);
-    pt_off[m] = static_cast<uint32_t>(offsets[m]);
-    node_base[m] = static_cast<uint32_t>(nodes);
-    uint32_t P = 0, d = 0, l0 = 0, segs = 0;
-    if (nm) {
-      P = 2;
-      d = 1;
-      while (static_cast<uint64_t>(P) * kLbvhLeafPoints < nm) {
-        P <<= 1;
-        d++;
-      }
-      l0 = kd_smem_first_level(nm, d);
-      segs = 1u << l0;
-      nodes += P - 1;
-    }
-    depth[m] = d;
-    level0[m] = l0;
-    slot_off[m + 1] = slot_off[m] + P;
-    seg_off[m + 1] = seg_off[m] + segs;
-    max_depth = std::max(max_depth, d);
-    radix_levels = std::max(radix_levels, l0);
-  }
-  pt_off[n_maps] = static_cast<uint32_t>(n);
+  ForestPlan plan;
+  plan_forest(n_maps, offsets, plan);
+  const uint32_t max_depth = plan.max_depth, radix_levels = plan.radix_levels, n_segments = plan.n_segments, n_slots = plan.n_slots;
+  const size_t nodes = plan.nodes;
+  const int key_bits = plan.key_bits;
   if (max_depth + 1 > 40) return fail(ctx, 1, who + "tree too deep");
-  const uint32_t n_segments = seg_off[n_maps], n_slots = slot_off[n_maps];
-  int key_bits = 32;
-  while ((1ull << (key_bits - 32)) < n_segments) key_bits++;
+  const size_t T = plan.tab.size();
   CU(ctx->kt_tables.reserve(T * sizeof(uint32_t)));
   // pageable host memory: staged before cudaMemcpyAsync returns
-  CU(cudaMemcpyAsync(ctx->kt_tables.p, tab.data(), T * sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
+  CU(cudaMemcpyAsync(ctx->kt_tables.p, plan.tab.data(), T * sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
   CU(ctx->stage_pts.reserve(n * 4 * sizeof(double)));
   CU(cudaMemcpyAsync(ctx->stage_pts.p, points, n * 4 * sizeof(double), cudaMemcpyDefault, ctx->stream));
   if (normals) {
@@ -598,10 +761,8 @@ int sgb_target_build_kdtrees(sgb_ctx* ctx, size_t n_maps, const size_t* offsets,
                                ctx->tgt_perm.as<uint32_t>(), n, key_bits, ctx->stream));
     CU(ctx->sort_temp.reserve(sort_bytes));
   }
-  const uint32_t* tp = ctx->kt_tables.as<uint32_t>();
   ForestBuild b = {};
-  b.tables = ForestTables{tp, tp + (n_maps + 1), tp + 2 * (n_maps + 1), tp + 3 * (n_maps + 1), tp + 3 * (n_maps + 1) + n_maps,
-                          tp + 3 * (n_maps + 1) + 2 * n_maps, static_cast<uint32_t>(n_maps)};
+  b.tables = forest_tables(ctx->kt_tables.as<uint32_t>(), n_maps);
   b.n = static_cast<uint32_t>(n);
   b.n_segments = n_segments;
   b.n_slots = n_slots;

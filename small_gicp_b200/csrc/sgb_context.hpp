@@ -155,6 +155,9 @@ struct sgb_ctx {
   // ---- preprocessing scratch (sgb_capi_preprocess.cu) ----
   sgb::DevBuf pre_pts, pre_leaf_pts, pre_nodes, pre_perm, pre_centre, pre_bounds, pre_out_normals, pre_out_covs, pre_heads, pre_slots, pre_vals_out;
   sgb::DevBuf pre_vox_coords;  // integer voxel coordinates of sgb_target_build_voxelmap
+  // many clouds (sgb_voxelgrid_sampling_batch / sgb_estimate_features_batch): per cloud its voxel region, and its centre [4] + the
+  // ForestTables of the scratch forest (pre_pts / pre_leaf_pts / pre_perm / pre_nodes hold its points and records)
+  sgb::DevBuf pre_regions, pre_centres, pre_tables;
 
   // ---- multi-GPU exchange fused into the reduction's finishing CTA (sgb_comm_*, CommParams in sgb_device.cuh) ----
   sgb::DevBuf comm_mail;                  // this rank's mailbox (zeroed at allocation)

@@ -7,7 +7,8 @@
 //
 // Build (launches depend on the size of the largest map only, never on the map count; no host synchronisation):
 //   forest_centres_kernel       one CTA per map: box of its points -> centre, as launch_bounds_centre computes it for one cloud
-//   forest_convert_kernel       centred FP32 points and packed features in original order (+ the first working copy of the points)
+//   forest_convert_kernel       centred FP32 points and packed features in original order (+ the first working copy of the points, and
+//                               for feature estimation the FP32 rounding residuals)
 //   forest_boxes_kernel / forest_keys_kernel   one radix level of every map whose nodes at that level still exceed kKdSegMax points;
 //                               the caller sorts by (global node, coordinate along the node's widest axis) and re-gathers
 //   forest_refine_smem_kernel   every (map, subtree of <= kKdSegMax points) segment refined in shared memory, one CTA each
@@ -15,6 +16,7 @@
 // Search:
 //   forest_search_kernel        one CTA per BatchTile (128 consecutive stored points of ONE member): warp-cooperative exact nearest-
 //                               neighbour walk over that member's map, as packet_search_kernel walks one tree
+// The same build over the preprocessing scratch serves sgb_estimate_features_batch (forest_features_kernel, sgb_preprocess.cu).
 #include <algorithm>
 #include <cfloat>
 
@@ -26,18 +28,6 @@
 namespace sgb {
 
 namespace {
-
-/// the map that owns x: the largest m < n_maps with prefix[m] <= x (prefix ascending, prefix[0] <= x < prefix[n_maps]); among maps
-/// that own nothing (equal prefix entries) it is the next one that does
-__device__ __forceinline__ uint32_t forest_map_of(const uint32_t* __restrict__ prefix, uint32_t n_maps, uint32_t x) {
-  uint32_t lo = 0, hi = n_maps;
-  while (hi - lo > 1u) {
-    const uint32_t mid = (lo + hi) >> 1;
-    if (__ldg(&prefix[mid]) <= x) lo = mid;
-    else hi = mid;
-  }
-  return lo;
-}
 
 // The helpers below are copies of tree_bound / tree_node_of / float_flip / float_unflip / lbvh_store_child in sgb_kernels.cu: sharing
 // them would change the code of the single-tree build kernels there.
@@ -111,10 +101,11 @@ __global__ void __launch_bounds__(256) forest_centres_kernel(const double4* __re
   }
 }
 
-// raw (double AoS) -> centred float4 in original order (w = index within the map) and its working copy, features packed, perm = identity
+// raw (double AoS) -> centred float4 in original order (w = index within the map) and its working copy, features packed, perm = identity;
+// out_lo (or null): what the rounding to FP32 dropped, convert_kernel's formula (sgb_kernels.cu)
 __global__ void forest_convert_kernel(const double4* __restrict__ pts, const double4* __restrict__ normals, const double* __restrict__ covs, uint32_t n,
                                       const ForestTables F, const double* __restrict__ centres, float4* out_pts, float4* work_pts, float4* out_normals,
-                                      float4* out_covA, float4* out_covB, uint32_t* perm) {
+                                      float4* out_covA, float4* out_covB, uint32_t* perm, float4* out_lo) {
   for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
     const uint32_t m = forest_map_of(F.pt_off, F.n_maps, i);
     const double* c = centres + 4 * static_cast<size_t>(m);
@@ -124,6 +115,7 @@ __global__ void forest_convert_kernel(const double4* __restrict__ pts, const dou
     out_pts[i] = f;
     work_pts[i] = f;
     perm[i] = i;
+    if (out_lo) out_lo[i] = make_float4((float)(x - (double)(float)x), (float)(y - (double)(float)y), (float)(z - (double)(float)z), 0.f);
     if (normals) {
       const double4 nn = normals[i];
       out_normals[i] = make_float4((float)nn.x, (float)nn.y, (float)nn.z, 0.f);
@@ -488,7 +480,7 @@ cudaError_t launch_forest_build(const ForestBuild& b, cudaStream_t st, int* laun
   forest_centres_kernel<<<F.n_maps, 256, 0, st>>>(reinterpret_cast<const double4*>(b.points), F, b.centres);
   const uint32_t cgrid = std::min<uint32_t>((n + 255u) / 256u, static_cast<uint32_t>(b.sm_count) * 8u);
   forest_convert_kernel<<<cgrid, 256, 0, st>>>(reinterpret_cast<const double4*>(b.points), reinterpret_cast<const double4*>(b.normals), b.covs, n, F, b.centres,
-                                               b.orig_pts, b.leaf_pts, b.orig_normals, b.orig_covA, b.orig_covB, b.perm);
+                                               b.orig_pts, b.leaf_pts, b.orig_normals, b.orig_covA, b.orig_covB, b.perm, b.orig_lo);
   count += 2;
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return e;

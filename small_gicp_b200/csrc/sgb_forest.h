@@ -24,6 +24,20 @@ struct ForestTables {
   uint32_t n_maps;
 };
 
+#ifdef __CUDACC__
+/// the map that owns x: the largest m < n_maps with prefix[m] <= x (prefix ascending, prefix[0] <= x < prefix[n_maps]); among maps
+/// that own nothing (equal prefix entries) it is the next one that does
+__device__ __forceinline__ uint32_t forest_map_of(const uint32_t* __restrict__ prefix, uint32_t n_maps, uint32_t x) {
+  uint32_t lo = 0, hi = n_maps;
+  while (hi - lo > 1u) {
+    const uint32_t mid = (lo + hi) >> 1;
+    if (__ldg(&prefix[mid]) <= x) lo = mid;
+    else hi = mid;
+  }
+  return lo;
+}
+#endif
+
 /// What the search reads: the record blocks, each map's centre [4] and the tables above.
 struct ForestView {
   const float4* pnodes;
@@ -43,6 +57,7 @@ struct ForestBuild {
   double* centres;        // [n_maps][4]
   float4 *orig_pts, *orig_normals, *orig_covA, *orig_covB;
   float4 *leaf_pts, *leaf_normals, *leaf_covA, *leaf_covB;
+  float4* orig_lo;        // null, or what the FP32 rounding of orig_pts dropped (convert_kernel's out_lo): feature estimation only
   uint32_t* perm;         // leaf position -> global original position
   float4* pnodes;
   uint32_t* boxes;        // n_segments x 6
@@ -57,5 +72,10 @@ cudaError_t launch_forest_build(const ForestBuild& b, cudaStream_t st, int* laun
 /// Exact nearest neighbour of every point of the call's tiles in its member's map; vcorr[vfirst + k] = global leaf position or kNone.
 /// max_depth: stack entries per lane (inner levels of the deepest tree + 1, at most 40); bound: the FP32 search bound (search_bound).
 cudaError_t launch_forest_search(const BatchParams& B, const ForestView& F, uint32_t n_tiles, int max_depth, float bound, uint32_t* vcorr, cudaStream_t st);
+/// Normals (mode bit 0) / covariances (bit 1) of every point of a built forest from its k nearest neighbours in its own map, as
+/// launch_features computes them for one cloud (sgb_preprocess.cu): one thread per leaf-ordered point, outputs in the double layout at
+/// the point's global original position.  lo: the build's orig_lo, or null.  depth: stack entries (inner levels of the deepest tree + 1).
+cudaError_t launch_forest_features(const float4* pnodes, const float4* leaf_pts, uint32_t n, int k, const ForestTables& F, const double* centres, int mode,
+                                   double* out_normals_d, double* out_covs_d, int depth, const float4* lo, cudaStream_t st);
 
 }  // namespace sgb

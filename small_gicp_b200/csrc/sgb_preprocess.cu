@@ -6,11 +6,14 @@
 //       (/root/reference/include/small_gicp/util/normal_estimation.hpp:12-140, normal_estimation_omp.hpp:9-60)
 //   * voxel-grid down-sampling: 3 x 21-bit voxel key, radix sort, segmented mean
 //       replaces voxelgrid_sampling{,_omp,_tbb} (.../util/downsampling.hpp:22-78)
+//   * many clouds at once: the features body over a forest of kd-trees (forest_features_kernel), and the voxel means over the
+//     (cloud, valid, key) order of the many-maps sort (sgb_capi_preprocess.cu)
 #include <cfloat>
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
 
 #include "sgb_device.cuh"
+#include "sgb_forest.h"
 #include "sgb_kernels.h"
 
 namespace sgb {
@@ -114,9 +117,9 @@ __device__ __forceinline__ void bvh_knn(const float4* __restrict__ pnodes, const
   }
 }
 
-/// One thread per point of the cloud in LEAF order (neighbouring threads query neighbouring points).
-/// mode bit 0: normals, bit 1: covariances.  Outputs are written in the cloud's ORIGINAL order
-/// (index carried in pts[].w): device layout (float4 streams) and / or the reference's double layout.
+/// The features of the point at leaf position i (features_kernel, forest_features_kernel).  mode bit 0: normals, bit 1: covariances.
+/// The cloud's points and its lo residuals are indexed by base + w (w = pts[].w, the index within the cloud); outputs are written at
+/// base + w (or at i with leaf_order_out): device layout (float4 streams) and / or the reference's double layout.
 ///
 /// Neighbour sets.  The search runs on the centred FP32 coordinates (rounded by up to ~2 um at 50 m), the reference on doubles: at the
 /// k-th neighbour a near-tie could swap one point of the set -- rare (0.5 % of the points), but a different covariance where it happens.
@@ -125,20 +128,17 @@ __device__ __forceinline__ void bvh_knn(const float4* __restrict__ pnodes, const
 /// equidistant to ~1e-12 m^2, and the covariance sums use the exact coordinates as well.  lo == nullptr: FP32 coordinates throughout.
 constexpr int kFeatExtra = 4;
 template <int KMAX>
-__global__ void __launch_bounds__(kLinBlock) features_kernel(const float4* __restrict__ pnodes, const float4* __restrict__ pts, uint32_t n, int k,
-                                                             const double* __restrict__ centre, int mode, float4* out_normals, float4* out_covA,
-                                                             float4* out_covB, double* out_normals_d, double* out_covs_d, int leaf_order_out, int depth,
-                                                             const float4* __restrict__ lo) {
-  extern __shared__ uint2 s_stack[];  // [depth][kLinBlock] descriptors, then [depth][kLinBlock] distances
+__device__ __forceinline__ void features_point(const float4* __restrict__ pnodes, const float4* __restrict__ pts, uint32_t i, uint32_t base, int k,
+                                               const double* __restrict__ centre, int mode, float4* out_normals, float4* out_covA, float4* out_covB,
+                                               double* out_normals_d, double* out_covs_d, int leaf_order_out, int depth, const float4* __restrict__ lo,
+                                               uint2* s_stack) {
   constexpr int KC = KMAX + kFeatExtra;
-  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
   const float4 q = __ldg(&pts[i]);
   KnnList<KC> L;
   const int kc = lo ? k + kFeatExtra : k;
   L.init(kc);
   bvh_knn<KC>(pnodes, pts, q.x, q.y, q.z, L, s_stack, reinterpret_cast<float*>(s_stack + static_cast<size_t>(depth) * kLinBlock));
-  const uint32_t qo = static_cast<uint32_t>(__float_as_int(q.w));
+  const uint32_t qo = base + static_cast<uint32_t>(__float_as_int(q.w));
   double qx = q.x, qy = q.y, qz = q.z;
   if (lo) {
     const float4 l = __ldg(&lo[qo]);
@@ -149,7 +149,7 @@ __global__ void __launch_bounds__(kLinBlock) features_kernel(const float4* __res
     const float4 t = __ldg(&pts[L.i[j]]);
     double tx = t.x, ty = t.y, tz = t.z;
     if (lo) {
-      const float4 l = __ldg(&lo[static_cast<uint32_t>(__float_as_int(t.w))]);
+      const float4 l = __ldg(&lo[base + static_cast<uint32_t>(__float_as_int(t.w))]);
       tx += l.x; ty += l.y; tz += l.z;
     }
     x = tx - qx; y = ty - qy; z = tz - qz;
@@ -234,6 +234,58 @@ __global__ void __launch_bounds__(kLinBlock) features_kernel(const float4* __res
       o[12] = 0.0; o[13] = 0.0; o[14] = 0.0; o[15] = 0.0;
     }
   }
+}
+
+/// One thread per point of the cloud in LEAF order (neighbouring threads query neighbouring points); outputs in ORIGINAL order
+/// (w = index) unless leaf_order_out.
+template <int KMAX>
+__global__ void __launch_bounds__(kLinBlock) features_kernel(const float4* __restrict__ pnodes, const float4* __restrict__ pts, uint32_t n, int k,
+                                                             const double* __restrict__ centre, int mode, float4* out_normals, float4* out_covA,
+                                                             float4* out_covB, double* out_normals_d, double* out_covs_d, int leaf_order_out, int depth,
+                                                             const float4* __restrict__ lo) {
+  extern __shared__ uint2 s_stack[];  // [depth][kLinBlock] descriptors, then [depth][kLinBlock] distances
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  features_point<KMAX>(pnodes, pts, i, 0u, k, centre, mode, out_normals, out_covA, out_covB, out_normals_d, out_covs_d, leaf_order_out, depth, lo, s_stack);
+}
+
+/// The forest of many clouds (launch_forest_features): one thread per leaf-ordered point of any map.  Map m's points occupy leaf and
+/// original positions pt_off[m] .. pt_off[m+1] with w = the index within the map, its records start at node_base[m] and hold global
+/// leaf positions, so the single cloud's body runs unchanged on map m's records, centre and base pt_off[m].
+template <int KMAX>
+__global__ void __launch_bounds__(kLinBlock) forest_features_kernel(const float4* __restrict__ pnodes, const float4* __restrict__ pts, uint32_t n, int k,
+                                                                    const uint32_t* __restrict__ pt_off, const uint32_t* __restrict__ node_base,
+                                                                    uint32_t n_maps, const double* __restrict__ centres, int mode, double* out_normals_d,
+                                                                    double* out_covs_d, int depth, const float4* __restrict__ lo) {
+  extern __shared__ uint2 s_stack[];  // [depth][kLinBlock] descriptors, then [depth][kLinBlock] distances
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const uint32_t m = forest_map_of(pt_off, n_maps, i);
+  features_point<KMAX>(pnodes + 4 * static_cast<size_t>(__ldg(&node_base[m])), pts, i, __ldg(&pt_off[m]), k, centres + 4 * static_cast<size_t>(m), mode,
+                       nullptr, nullptr, nullptr, out_normals_d, out_covs_d, 0, depth, lo, s_stack);
+}
+
+template <int KMAX>
+static cudaError_t launch_forest_features_t(const float4* pnodes, const float4* pts, uint32_t n, int k, const ForestTables& F, const double* centres, int mode,
+                                            double* ond, double* ocd, int depth, const float4* lo, cudaStream_t st) {
+  if (depth < 1) depth = 1;
+  const size_t smem = static_cast<size_t>(depth) * kLinBlock * (sizeof(uint2) + sizeof(float));
+  if (smem > 48 * 1024) {
+    cudaError_t e = cudaFuncSetAttribute(forest_features_kernel<KMAX>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
+    if (e != cudaSuccess) return e;
+  }
+  const int grid = static_cast<int>((n + kLinBlock - 1) / kLinBlock);
+  forest_features_kernel<KMAX><<<grid, kLinBlock, smem, st>>>(pnodes, pts, n, k, F.pt_off, F.node_base, F.n_maps, centres, mode, ond, ocd, depth, lo);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_forest_features(const float4* pnodes, const float4* leaf_pts, uint32_t n, int k, const ForestTables& F, const double* centres, int mode,
+                                   double* out_normals_d, double* out_covs_d, int depth, const float4* lo, cudaStream_t st) {
+  if (n == 0) return cudaSuccess;
+  if (k <= 10) return launch_forest_features_t<10>(pnodes, leaf_pts, n, k, F, centres, mode, out_normals_d, out_covs_d, depth, lo, st);
+  if (k <= 20) return launch_forest_features_t<20>(pnodes, leaf_pts, n, k, F, centres, mode, out_normals_d, out_covs_d, depth, lo, st);
+  if (k <= 32) return launch_forest_features_t<32>(pnodes, leaf_pts, n, k, F, centres, mode, out_normals_d, out_covs_d, depth, lo, st);
+  return cudaErrorInvalidValue;
 }
 
 template <int KMAX>

@@ -1,6 +1,6 @@
 // SPDX-License-Identifier: MIT
 // Convenience API with the reference's names and defaults:
-//   RegistrationSetting, preprocess_points(), create_gaussian_voxelmap(), align() x3
+//   RegistrationSetting, preprocess_points(), create_gaussian_voxelmap(), align() x3; preprocess_points_batch() for many clouds (extension)
 //   (/root/reference/include/small_gicp/registration/registration_helper.hpp:18-90,
 //    /root/reference/src/small_gicp/registration/registration_helper.cpp:22-137)
 // Differences by construction: down-sampling and normal/covariance estimation run on the device through the C-ABI
@@ -100,6 +100,41 @@ inline std::pair<PointCloud::Ptr, std::shared_ptr<KdTree<PointCloud>>> preproces
   auto kdtree = std::make_shared<KdTree<PointCloud>>(downsampled);
   estimate_normals_covariances(*downsampled, num_neighbors, device);
   return {downsampled, kdtree};
+}
+
+/// Many clouds prepared at once (a sequence of frames): device voxel grid of every cloud in one call (sgb_voxelgrid_sampling_batch), then
+/// k-NN normals + covariances of every down-sampled cloud in one call (sgb_estimate_features_batch).  Returns one down-sampled cloud per
+/// input; each equals preprocess_points(cloud, downsampling_resolution, num_neighbors).first, up to the exact-FP32-tie clause of
+/// sgb_estimate_features_batch.  No host trees are built: sgb_target_build_kdtrees / BatchRegistration build theirs on the device.
+inline std::vector<PointCloud::Ptr> preprocess_points_batch(const std::vector<PointCloud>& clouds, double downsampling_resolution, int num_neighbors = 10,
+                                                            int device = 0) {
+  const size_t B = clouds.size();
+  std::vector<PointCloud::Ptr> out(B);
+  std::vector<size_t> offsets(B + 1, 0), down_offsets(B + 1, 0);
+  for (size_t c = 0; c < B; c++) {
+    out[c] = std::make_shared<PointCloud>();
+    offsets[c + 1] = offsets[c] + clouds[c].size();
+  }
+  const size_t n = offsets[B];
+  if (n == 0) return out;
+  std::vector<Vector4d> pts(n), down(n);
+  for (size_t c = 0; c < B; c++) std::copy(clouds[c].points.begin(), clouds[c].points.end(), pts.begin() + offsets[c]);
+  sgb_ctx* ctx = detail::helper_context(device);
+  detail::helper_check(ctx, sgb_voxelgrid_sampling_batch(ctx, B, offsets.data(), pts[0].data(), downsampling_resolution, down[0].data(), down_offsets.data()));
+  const size_t m = down_offsets[B];
+  if (m == 0) return out;
+  std::vector<Vector4d> normals(m);
+  std::vector<Matrix4d> covs(m);
+  detail::helper_check(ctx, sgb_estimate_features_batch(ctx, B, down_offsets.data(), down[0].data(), num_neighbors, normals[0].data(), covs[0].data()));
+  for (size_t c = 0; c < B; c++) {
+    const size_t first = down_offsets[c], count = down_offsets[c + 1] - first;
+    PointCloud& o = *out[c];
+    o.resize(count);
+    std::copy(down.begin() + first, down.begin() + first + count, o.points.begin());
+    std::copy(normals.begin() + first, normals.begin() + first + count, o.normals.begin());
+    std::copy(covs.begin() + first, covs.begin() + first + count, o.covs.begin());
+  }
+  return out;
 }
 
 inline GaussianVoxelMap::Ptr create_gaussian_voxelmap(const PointCloud& points, double voxel_resolution) {

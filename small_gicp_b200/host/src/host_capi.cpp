@@ -371,6 +371,38 @@ int sgbh_helper_align(size_t n_target, const double* target_pts4, size_t n_sourc
   }
 }
 
+/// preprocess_points(cloud, resolution, num_neighbors).first of every cloud (batch = 0), or preprocess_points_batch(clouds, ...)
+/// (batch = 1): cloud c = rows offsets[c] .. offsets[c+1].  Outputs concatenated (each buffer holds offsets[n_clouds] rows); out_offsets:
+/// n_clouds + 1 entries.
+int sgbh_preprocess_points(size_t n_clouds, const size_t* offsets, const double* pts4, double downsampling_resolution, int num_neighbors, int device, int batch,
+                           double* out_pts4, double* out_normals4, double* out_covs16, size_t* out_offsets) {
+  try {
+    std::vector<PointCloud> clouds(n_clouds);
+    for (size_t c = 0; c < n_clouds; c++) clouds[c] = *make_cloud(offsets[c + 1] - offsets[c], pts4 + 4 * offsets[c], nullptr, nullptr);
+    std::vector<PointCloud::Ptr> out;
+    if (batch) {
+      out = preprocess_points_batch(clouds, downsampling_resolution, num_neighbors, device);
+    } else {
+      for (const auto& c : clouds) out.push_back(preprocess_points(c, downsampling_resolution, num_neighbors, 4, device).first);
+    }
+    out_offsets[0] = 0;
+    for (size_t c = 0; c < n_clouds; c++) {
+      const PointCloud& o = *out[c];
+      const size_t first = out_offsets[c], m = o.size();
+      if (m) {
+        std::memcpy(out_pts4 + 4 * first, o.points[0].data(), m * sizeof(Vector4d));
+        std::memcpy(out_normals4 + 4 * first, o.normals[0].data(), m * sizeof(Vector4d));
+        std::memcpy(out_covs16 + 16 * first, o.covs[0].data(), m * sizeof(Matrix4d));
+      }
+      out_offsets[c + 1] = first + m;
+    }
+    return 0;
+  } catch (const std::exception& e) {
+    g_error = e.what();
+    return 2;
+  }
+}
+
 /// Host KdTree<PointCloud>::knn_search over a batch of queries (API-surface check of the mirror, CPU-only).
 int sgbh_kdtree_knn(size_t n, const double* pts4, size_t nq, const double* queries4, int k, uint64_t* idx_out, double* d2_out) {
   try {

@@ -241,6 +241,30 @@ def helper_align(target_points, source_points, init_T=None, type=GICP, voxel_res
     return r
 
 
+def preprocess_points(clouds, downsampling_resolution=0.25, num_neighbors=10, batch=False, device=0):
+    """preprocess_points(cloud, ...).first of every cloud (C++ host mirror), or with batch=True preprocess_points_batch(clouds, ...):
+    clouds is a list of (N_m, 3|4) arrays.  Returns a list of (points (M_m, 4), normals (M_m, 4), covs (M_m, 4, 4))."""
+    L = _lib()
+    if not hasattr(L.sgbh_preprocess_points, "_typed"):
+        L.sgbh_preprocess_points.restype = C.c_int
+        L.sgbh_preprocess_points.argtypes = [C.c_size_t, C.POINTER(C.c_size_t), _dp, C.c_double, C.c_int, C.c_int, C.c_int, _dp, _dp, _dp,
+                                             C.POINTER(C.c_size_t)]
+        L.sgbh_preprocess_points._typed = True
+    members = [capi._points4(c) for c in clouds]
+    B = len(members)
+    offsets = np.zeros(B + 1, dtype=np.uintp)
+    offsets[1:] = np.cumsum([m.shape[0] for m in members])
+    p = np.ascontiguousarray(np.concatenate(members) if B else np.zeros((0, 4)))
+    n = max(p.shape[0], 1)
+    pts, nrm, cov = np.zeros((n, 4)), np.zeros((n, 4)), np.zeros((n, 4, 4))
+    out_off = np.zeros(B + 1, dtype=np.uintp)
+    rc = L.sgbh_preprocess_points(B, offsets.ctypes.data_as(C.POINTER(C.c_size_t)), _d(p), float(downsampling_resolution), int(num_neighbors), int(device),
+                                  int(bool(batch)), _d(pts), _d(nrm), _d(cov), out_off.ctypes.data_as(C.POINTER(C.c_size_t)))
+    if rc != 0:
+        raise capi.SgbError(L.sgbh_last_error().decode())
+    return [(pts[a:b].copy(), nrm[a:b].copy(), cov[a:b].copy()) for a, b in zip(out_off[:-1].astype(np.int64), out_off[1:].astype(np.int64))]
+
+
 def kdtree_knn(points, queries, k):
     """KdTree<PointCloud>(points).knn_search for each query (host mirror, CPU)."""
     L = _lib()
