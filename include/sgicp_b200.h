@@ -191,15 +191,16 @@ int sgb_num_inliers(sgb_ctx* ctx, size_t* n);
  * target points: the search returns an exact nearest neighbour, but which of two equidistant ones it returns depends on the
  * traversal, and that may depend on the other queries of a 32-query chunk (members are not padded to chunks) and on the batch's
  * total pending count.  sgb_drop_seeds applies to every member.
- * The upload is not batched: sgb_source_set_batch runs the single-source conversion and sort per non-empty member (5 launches, 7
- * with covariances), so its cost grows with the member count.
+ * The upload is batched: sgb_source_set_batch stores all clouds in 6 launches whatever their count (with or without covariances),
+ * each bit-identical to sgb_source_set_points of that cloud alone.
  * Many targets: after sgb_target_build_voxelmaps, member m is paired with map m -- sgb_linearize_batch, sgb_error_batch,
  * sgb_align_batch and sgb_correspondences_batch work as against one voxel map (same launches per round), and fail with a message while
  * the member count differs from the map count.  Each member's results are bit-identical to a context holding its map alone and that
  * member as a batch of one; its correspondences are voxel ids within its own map (id << 32).  On such a target the single-source calls
  * (sgb_linearize, sgb_error, their _device variants, sgb_correspondences, sgb_num_inliers) and sgb_target_batch_knn,
- * sgb_target_estimate_features, sgb_target_set_kdtree / _build_kdtree fail with a message.  Pair one source with many maps (or many
- * sources with one map) by repeating the cloud.
+ * sgb_target_estimate_features, sgb_target_set_kdtree / _build_kdtree fail with a message.  Pair one source with many maps, many
+ * sources with one map, or a cloud with several initial poses through sgb_source_set_pairs below: each cloud is stored once and
+ * each map built once.
  * Many kd-trees: after sgb_target_build_kdtrees, member m is paired with map m in the same way, for ICP, point-to-plane (the maps need
  * normals) and GICP (covariances).  A linearize round is 3 launches (search, factor, per-member sums) and an error round 2, whatever the
  * member count.  The calls fail with a message while the member count differs from the map count.  Each member's results are
@@ -213,6 +214,19 @@ int sgb_num_inliers(sgb_ctx* ctx, size_t* n);
 /* offsets: n_members + 1 ascending entries, offsets[0] = 0; member m = points offsets[m] .. offsets[m+1] (empty members allowed).
  * points / covariances: all members concatenated, in the layouts above (host, page-locked or device memory). */
 int sgb_source_set_batch(sgb_ctx* ctx, size_t n_members, const size_t* offsets, const double* points_xyz1, const double* covs_4x4 /*or NULL*/);
+/* The batch's members become n_members (cloud, map) pairs drawn from the clouds of the last sgb_source_set_batch: member p is a copy of
+ * cloud clouds[p] as stored (or cloud p when clouds == NULL, which needs n_members == the cloud count), aligned against map maps[p] of a
+ * many-maps / many-kd-trees target (maps == NULL: against map p, or the one target; S copies of a cloud against one target are S
+ * starts).  Index arrays in host memory.  No upload, no re-sort: 1 launch whatever n_members is, plus 1 at the first batched call after
+ * the pairing or the target changed (the maps seen through the pairing).  Afterwards sgb_linearize_batch, sgb_error_batch,
+ * sgb_align_batch, sgb_correspondences_batch and sgb_drop_seeds work on the pair members (poses, outputs and correspondences per member,
+ * in pair order; correspondences in its cloud's original order), each bit-identical to that cloud uploaded again as a member paired
+ * with that map; the per-member state starts afresh as after sgb_source_set_batch.  Calling it again re-pairs the same clouds;
+ * sgb_source_set_batch or sgb_source_set_points forgets the pairing.  Every batched call checks maps against the current target: a
+ * maps[p] beyond its map count, or a maps table with a target that is not many maps or many kd-trees, fails with a message (without a
+ * maps table the member count must equal the map count, as without pairs).  n_members <= SGB_BATCH_MAX_MEMBERS, fewer than 2^31 member
+ * points in all, every clouds[p] below the cloud count, a batch set, else the call fails with a message; n_members = 0: an empty batch. */
+int sgb_source_set_pairs(sgb_ctx* ctx, size_t n_members, const uint32_t* clouds /*or NULL*/, const uint32_t* maps /*or NULL*/);
 /* One linearize per member at its pose T_colmajor16xB[16 m ..]: out44xB[44 m ..] = H(36) | b(6) | e | num_inliers.  active (or NULL =
  * all): an inactive member costs no search or factor work, gets zeros and keeps its cached correspondences and linearisation pose.
  * out44xB may be host or device memory; the call returns when the results are there. */

@@ -75,6 +75,7 @@ _SIGNATURES = {
     "sgb_correspondences": (C.c_int, [_vp, _u64p]),
     "sgb_num_inliers": (C.c_int, [_vp, C.POINTER(C.c_size_t)]),
     "sgb_source_set_batch": (C.c_int, [_vp, C.c_size_t, C.POINTER(C.c_size_t), _dp, _dp]),
+    "sgb_source_set_pairs": (C.c_int, [_vp, C.c_size_t, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32)]),
     "sgb_linearize_batch": (C.c_int, [_vp, C.c_int, C.c_int, C.c_double, C.c_int, C.c_double, _dp, C.POINTER(C.c_uint8), _dp]),
     "sgb_error_batch": (C.c_int, [_vp, _dp, C.POINTER(C.c_uint8), _dp]),
     "sgb_correspondences_batch": (C.c_int, [_vp, _u64p]),
@@ -376,6 +377,22 @@ class Context:
         offsets = offsets.astype(np.uintp)
         self._check(self._L.sgb_source_set_batch(self._h, offsets.size - 1, offsets.ctypes.data_as(C.POINTER(C.c_size_t)), _d(p), _d(c)))
         self._batch_offsets = offsets.astype(np.int64)
+        self._cloud_offsets = self._batch_offsets
+
+    def set_source_pairs(self, clouds=None, maps=None):
+        """the batch's members become (cloud, map) pairs of the clouds of the last set_source_batch, without a new upload: member p is
+        cloud clouds[p] (None: cloud p, one member per cloud) aligned against map maps[p] of a many-maps / many-kd-trees target (None:
+        map p, or the one target).  The batched calls then take and return one pose / result per member."""
+        cl = None if clouds is None else np.ascontiguousarray(clouds, dtype=np.uint32).reshape(-1)
+        mp = None if maps is None else np.ascontiguousarray(maps, dtype=np.uint32).reshape(-1)
+        n_clouds = self._cloud_offsets.size - 1 if hasattr(self, "_cloud_offsets") else 0
+        P = cl.size if cl is not None else (mp.size if mp is not None else n_clouds)
+        if cl is not None and mp is not None and mp.size != P:
+            raise SgbError(f"set_source_pairs: {cl.size} clouds but {mp.size} maps")
+        u32p = C.POINTER(C.c_uint32)
+        self._check(self._L.sgb_source_set_pairs(self._h, P, None if cl is None else cl.ctypes.data_as(u32p), None if mp is None else mp.ctypes.data_as(u32p)))
+        sizes = np.diff(self._cloud_offsets)
+        self._batch_offsets = np.concatenate([[0], np.cumsum(sizes[cl] if cl is not None else sizes)]).astype(np.int64)
 
     def _batch_args(self, Ts, active):
         Ts = np.asarray(Ts, dtype=np.float64)

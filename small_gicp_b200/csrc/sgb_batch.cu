@@ -10,8 +10,11 @@
 //   batch_segment_kernel    one CTA per member: its tiles' partials in tile order -> H|b|e|inliers (or e) of that member
 //   batch_step_kernel       batched align(): one thread per member, its Gauss-Newton / Levenberg-Marquardt step (sgb_math.cuh) after a
 //                           round, its next pose and phase
+//   pair_gather_kernel      sgb_source_set_pairs: every member's replica of its stored cloud, in one launch over all member points
+//   pair_view_kernel        the many-maps tables above seen through the pairing (member p -> map maps[p]), one CTA
 // A member's sums depend on its own points, pose and correspondences only, added in an order fixed by its size: bit-identical whatever
 // else is in the batch.
+#include <algorithm>
 #include <cfloat>
 
 #include "sgb_batch.h"
@@ -228,6 +231,103 @@ __global__ void __launch_bounds__(kStepBlock) batch_step_kernel(const __grid_con
 cudaError_t launch_batch_step(const AlignOptions& o, uint32_t n_members, bool linearize, const double* out, MemberState* state, double* poses,
                               uint8_t* phase, cudaStream_t st) {
   batch_step_kernel<<<(n_members + kStepBlock - 1) / kStepBlock, kStepBlock, 0, st>>>(o, n_members, linearize, out, state, poses, phase);
+  return cudaGetLastError();
+}
+
+// the member (or cloud) that owns position i of a prefix table with n entries + 1 (empty ones own nothing)
+__device__ __forceinline__ uint32_t owner_of(const uint32_t* __restrict__ prefix, uint32_t n, uint32_t i) {
+  uint32_t lo = 0, hi = n;
+  while (hi - lo > 1u) {
+    const uint32_t mid = (lo + hi) >> 1;
+    if (__ldg(&prefix[mid]) <= i) lo = mid;
+    else hi = mid;
+  }
+  return lo;
+}
+
+// Pair members: member p is a replica of stored cloud clouds[p].  Positions 0 .. n - 1 copy the member points (FP32 point, packed
+// covariance, search order -> original index), the next 10 P the member's centre [4] and bounds [6].
+__global__ void pair_gather_kernel(const PairGather g) {
+  const uint32_t total = g.n + 10u * g.n_members;
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
+    if (i < g.n) {
+      const uint32_t p = owner_of(g.member_off, g.n_members, i);
+      const uint32_t s = g.cloud_off[g.clouds[p]] + (i - g.member_off[p]);
+      g.out_pts[i] = g.pts[s];
+      g.out_perm[i] = g.perm[s];
+      if (g.covA) {
+        g.out_covA[i] = g.covA[s];
+        g.out_covB[i] = g.covB[s];
+      }
+    } else {
+      const uint32_t k = i - g.n, p = k / 10u, j = k % 10u, c = g.clouds[p];
+      if (j < 4u) g.out_centres[4 * static_cast<size_t>(p) + j] = g.centres[4 * static_cast<size_t>(c) + j];
+      else g.out_bounds[6 * static_cast<size_t>(p) + j - 4u] = g.bounds[6 * static_cast<size_t>(c) + j - 4u];
+    }
+  }
+}
+
+// The per-member view of a many-maps target, one CTA: member p reads map maps[p].  Many kd-trees: pt_off = the prefix sum of the members'
+// map sizes (the search reads only pt_off[p + 1] - pt_off[p], so the sum may wrap around 2^32: every map is below 2^30 points),
+// node_base[p], centres[p].  Voxel maps: centres[p], regions[p].
+constexpr int kViewBlock = 1024;
+__global__ void __launch_bounds__(kViewBlock) pair_view_kernel(const PairView v) {
+  __shared__ uint32_t s_warp[kViewBlock / 32];
+  const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
+  uint32_t carry = 0;
+  for (uint32_t base = 0; base < v.n_members; base += kViewBlock) {
+    const uint32_t p = base + threadIdx.x;
+    uint32_t size = 0;
+    if (p < v.n_members) {
+      const uint32_t q = v.maps[p];
+      for (int d = 0; d < 4; d++) v.centres[4 * static_cast<size_t>(p) + d] = v.map_centres[4 * static_cast<size_t>(q) + d];
+      if (v.map_pt_off) {
+        size = v.map_pt_off[q + 1] - v.map_pt_off[q];
+        v.node_base[p] = v.map_node_base[q];
+      }
+      if (v.map_regions) v.regions[p] = v.map_regions[q];
+    }
+    if (!v.map_pt_off) continue;
+    // CTA exclusive scan of the sizes: within each warp, then over the warp totals
+    uint32_t incl = size;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const uint32_t y = __shfl_up_sync(0xffffffffu, incl, o);
+      if (lane >= static_cast<uint32_t>(o)) incl += y;
+    }
+    if (lane == 31u) s_warp[warp] = incl;
+    __syncthreads();
+    if (warp == 0) {
+      uint32_t w = s_warp[lane], wi = w;
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1) {
+        const uint32_t y = __shfl_up_sync(0xffffffffu, wi, o);
+        if (lane >= static_cast<uint32_t>(o)) wi += y;
+      }
+      s_warp[lane] = wi - w;  // exclusive prefix of the warp totals
+    }
+    __syncthreads();
+    if (p < v.n_members) v.pt_off[p] = carry + s_warp[warp] + incl - size;
+    const uint32_t chunk = __shfl_sync(0xffffffffu, incl, 31) + s_warp[warp];  // the last warp's view of the chunk total
+    __syncthreads();  // s_warp is reused by the next chunk
+    if (warp == kViewBlock / 32 - 1) s_warp[0] = chunk;
+    __syncthreads();
+    carry += s_warp[0];
+    __syncthreads();
+  }
+  if (v.map_pt_off && threadIdx.x == 0) v.pt_off[v.n_members] = carry;
+}
+
+cudaError_t launch_pair_gather(const PairGather& g, int sm_count, cudaStream_t st) {
+  const uint64_t total = g.n + 10ull * g.n_members;
+  if (total == 0) return cudaSuccess;
+  const uint64_t grid = std::min<uint64_t>((total + 255u) / 256u, static_cast<uint64_t>(sm_count) * 8u);
+  pair_gather_kernel<<<static_cast<unsigned>(grid), 256, 0, st>>>(g);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_pair_view(const PairView& v, cudaStream_t st) {
+  pair_view_kernel<<<1, kViewBlock, 0, st>>>(v);
   return cudaGetLastError();
 }
 

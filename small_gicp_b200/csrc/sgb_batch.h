@@ -42,6 +42,32 @@ cudaError_t launch_batch_maps_factor(const BatchParams& B, int factor, int robus
 /// result over the call's virtual source (err = false) or unused (err = true).  ICP, point-to-plane or GICP.
 cudaError_t launch_batch_trees_factor(const BatchParams& B, int factor, int robust, uint32_t n_tiles, bool err, const uint32_t* vcorr, const double* map_centres,
                                       cudaStream_t st);
+/// Members as (cloud, map) pairs (sgb_source_set_pairs): member p = a replica of stored cloud clouds[p], at member_off[p] .. member_off[p+1]
+/// of the member buffers; its centre and bounds too.  covA = null: no covariances.
+struct PairGather {
+  uint32_t n, n_members;  // member points, members
+  const uint32_t *member_off, *clouds, *cloud_off;
+  const float4 *pts, *covA, *covB;
+  const uint32_t* perm;
+  const double *centres, *bounds;
+  float4 *out_pts, *out_covA, *out_covB;
+  uint32_t* out_perm;
+  double *out_centres, *out_bounds;
+};
+cudaError_t launch_pair_gather(const PairGather& g, int sm_count, cudaStream_t st);
+/// What the round kernels read per map, indexed by member instead (member p -> map maps[p]): centres [members][4]; many kd-trees
+/// (map_pt_off non-null): pt_off [members + 1] and node_base [members] of a ForestView; voxel maps (map_regions non-null): regions.
+struct PairView {
+  uint32_t n_members;
+  const uint32_t* maps;
+  const double* map_centres;
+  const uint32_t *map_pt_off, *map_node_base;
+  const uint4* map_regions;
+  double* centres;
+  uint32_t *pt_off, *node_base;
+  uint4* regions;
+};
+cudaError_t launch_pair_view(const PairView& v, cudaStream_t st);
 /// out: [members][44] (linearize) or [members] (error)
 cudaError_t launch_batch_segment(const BatchParams& B, uint32_t n_members, bool linearize, double* out, cudaStream_t st);
 /// batched align(): every member whose phase matches the round (linearize: kPhaseLinearize, else kPhaseTrial) takes its optimiser step

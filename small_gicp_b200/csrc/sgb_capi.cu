@@ -84,6 +84,7 @@ int single_target_check(sgb_ctx* ctx, const char* who) {
 void forget_linearisation(sgb_ctx* ctx) {
   ctx->have_lin = false;
   ctx->corr_seeds = false;
+  ctx->b_view_ok = false;  // the target (or the pairing) it was built from may have changed
 }
 
 }  // namespace
@@ -192,6 +193,15 @@ void sgb::begin_source(sgb_ctx* ctx, SourceState state, size_t n, bool covs) {
   ctx->n_src = n;
   ctx->src_has_covs = covs;
   ctx->src_has_lo = ctx->src_tree_valid = ctx->src_cov_orig_valid = false;
+  ctx->b_paired = ctx->b_pair_has_maps = false;
+  ctx->b_pair_maps.clear();
+  forget_linearisation(ctx);
+}
+
+void sgb::begin_pairs(sgb_ctx* ctx) {
+  ctx->b_paired = true;
+  ctx->b_pair_has_maps = false;
+  ctx->b_pair_maps.clear();
   forget_linearisation(ctx);
 }
 

@@ -1,5 +1,6 @@
 // SPDX-License-Identifier: MIT
-// C-ABI of batched registration (include/sgicp_b200.h: sgb_source_set_batch, sgb_{linearize,error,correspondences}_batch).
+// C-ABI of batched registration (include/sgicp_b200.h: sgb_source_set_batch, sgb_source_set_pairs,
+// sgb_{linearize,error,align,correspondences}_batch).
 // Kernels in sgb_batch.cu; DESIGN.md §11.
 #include <cuda_runtime.h>
 
@@ -25,10 +26,27 @@ size_t batch_points(const sgb_ctx* ctx) { return ctx->b_offsets.empty() ? 0 : ct
 size_t batch_members(const sgb_ctx* ctx) { return ctx->b_offsets.empty() ? 0 : ctx->b_offsets.size() - 1; }
 size_t max_tiles(const sgb_ctx* ctx) { return batch_points(ctx) / kLinBlock + batch_members(ctx) + 1; }
 
+bool many_maps(const sgb_ctx* ctx) { return ctx->tgt_state == TargetState::VoxelMaps || ctx->tgt_state == TargetState::KdTrees; }
+// the members read the per-map tables through the pairing's view (PairView)
+bool paired_maps(const sgb_ctx* ctx) { return ctx->b_pair_has_maps && many_maps(ctx); }
+
 int batch_check(sgb_ctx* ctx, const char* who, const double* T) {
   if (ctx->src_state != SourceState::Batch) return fail(ctx, 1, std::string(who) + ": the context holds no batch of sources (call sgb_source_set_batch)");
   if (ctx->comm_world > 1) return fail(ctx, 1, std::string(who) + ": batched calls are single-GPU only (call sgb_comm_disconnect first)");
   if (!T) return fail(ctx, 1, std::string(who) + ": null poses");
+  if (ctx->b_pair_has_maps) {
+    // the target may have been replaced since the pairing: its maps are checked at every call
+    if (!many_maps(ctx))
+      return fail(ctx, 1, std::string(who) + ": the pairing names a map per member (sgb_source_set_pairs) but the target is not a many-maps or many-kd-trees target");
+    const size_t maps = target_maps(ctx);
+    if (ctx->b_pair_max_map >= maps) {
+      for (size_t p = 0; p < ctx->b_pair_maps.size(); p++)
+        if (ctx->b_pair_maps[p] >= maps)
+          return fail(ctx, 1, std::string(who) + ": member " + std::to_string(p) + " is paired with map " + std::to_string(ctx->b_pair_maps[p]) +
+                                  " but the target holds " + std::to_string(maps) + " maps");
+    }
+    return 0;
+  }
   if (ctx->tgt_state == TargetState::VoxelMaps && batch_members(ctx) != ctx->vm_maps)
     return fail(ctx, 1, std::string(who) + ": the batch has " + std::to_string(batch_members(ctx)) + " members but the target holds " +
                             std::to_string(ctx->vm_maps) + " voxel maps (member m is aligned against map m)");
@@ -41,11 +59,43 @@ int batch_check(sgb_ctx* ctx, const char* who, const double* T) {
 bool voxel_target(const sgb_ctx* ctx) { return ctx->tgt_state == TargetState::VoxelMap || ctx->tgt_state == TargetState::VoxelMaps; }
 
 // the factor kernel of one round over the target's kind: one voxel map or a point target (launch_batch_factor), or many maps / trees
+// (with a pairing's map table: the member-indexed view of the maps instead of the map-indexed tables)
 cudaError_t launch_factor(sgb_ctx* ctx, const BatchParams& Bp, int factor, int robust, uint32_t n_tiles, bool err, const uint32_t* vcorr) {
+  const bool view = paired_maps(ctx);
   if (ctx->tgt_state == TargetState::VoxelMaps)
-    return launch_batch_maps_factor(Bp, factor, robust, n_tiles, err, ctx->vm_centres.as<double>(), ctx->vm_regions.as<uint4>(), ctx->stream);
-  if (ctx->tgt_state == TargetState::KdTrees) return launch_batch_trees_factor(Bp, factor, robust, n_tiles, err, vcorr, ctx->kt_centres.as<double>(), ctx->stream);
+    return launch_batch_maps_factor(Bp, factor, robust, n_tiles, err, (view ? ctx->v_centres : ctx->vm_centres).as<double>(),
+                                    (view ? ctx->v_regions : ctx->vm_regions).as<uint4>(), ctx->stream);
+  if (ctx->tgt_state == TargetState::KdTrees)
+    return launch_batch_trees_factor(Bp, factor, robust, n_tiles, err, vcorr, (view ? ctx->v_centres : ctx->kt_centres).as<double>(), ctx->stream);
   return launch_batch_factor(Bp, factor, robust, n_tiles, voxel_target(ctx), err, vcorr, ctx->stream);
+}
+
+// Builds the pairing's view of the current target (one launch) unless it is up to date: forget_linearisation, which every target
+// transition and every pairing goes through, marks it stale.
+int pair_view(sgb_ctx* ctx) {
+  if (!paired_maps(ctx) || ctx->b_view_ok) return 0;
+  CU(cudaSetDevice(ctx->device));
+  const size_t P = batch_members(ctx);
+  PairView v = {};
+  v.n_members = static_cast<uint32_t>(P);
+  v.maps = ctx->p_tables.as<uint32_t>() + 2 * P + 1;
+  v.centres = ctx->v_centres.as<double>();
+  if (ctx->tgt_state == TargetState::KdTrees) {
+    const uint32_t* tab = ctx->kt_tables.as<uint32_t>();
+    v.map_centres = ctx->kt_centres.as<double>();
+    v.map_pt_off = tab;
+    v.map_node_base = tab + 3 * (ctx->kt_maps + 1);
+    v.pt_off = ctx->v_tables.as<uint32_t>();
+    v.node_base = v.pt_off + P + 1;
+  } else {
+    v.map_centres = ctx->vm_centres.as<double>();
+    v.map_regions = ctx->vm_regions.as<uint4>();
+    v.regions = ctx->v_regions.as<uint4>();
+  }
+  CU(launch_pair_view(v, ctx->stream));
+  ctx->launches += 1;
+  ctx->b_view_ok = true;
+  return 0;
 }
 
 // The tables of one call: every active non-empty member's points cut into tiles of kLinBlock (the virtual source concatenates the
@@ -80,10 +130,11 @@ int batch_tables(sgb_ctx* ctx, const double* T, const uint8_t* active, bool seed
 BatchParams batch_params(sgb_ctx* ctx, const LinParams& P) {
   BatchParams B = {};
   B.tgt = P.tgt;
-  B.pts = ctx->src_pts.as<float4>();
-  B.covA = ctx->src_covA.as<float4>();
-  B.covB = ctx->src_covB.as<float4>();
-  B.centres = ctx->b_centres.as<double>();
+  const bool pairs = ctx->b_paired;  // the members' replicas, else the stored clouds themselves
+  B.pts = (pairs ? ctx->p_pts : ctx->src_pts).as<float4>();
+  B.covA = (pairs ? ctx->p_covA : ctx->src_covA).as<float4>();
+  B.covB = (pairs ? ctx->p_covB : ctx->src_covB).as<float4>();
+  B.centres = (pairs ? ctx->p_centres : ctx->b_centres).as<double>();
   B.poses = ctx->b_poses.as<double>();
   B.lin_poses = ctx->b_lin_poses.as<double>();
   B.tiles = ctx->b_tiles.as<BatchTile>();
@@ -126,9 +177,10 @@ int linearize_round(sgb_ctx* ctx, int factor, int robust, double robust_c, int r
   }
   if (n_tiles && ctx->tgt_state == TargetState::KdTrees) {
     // many trees: every tile searched in its member's own tree, straight from the stored points at the member's pose (sgb_forest.cu)
-    const uint32_t* tab = ctx->kt_tables.as<uint32_t>();
-    const size_t M = ctx->kt_maps;
-    const ForestView F{ctx->tgt_pnodes.as<float4>(), ctx->kt_centres.as<double>(), tab, tab + 3 * (M + 1)};
+    const bool view = paired_maps(ctx);
+    const uint32_t* tab = (view ? ctx->v_tables : ctx->kt_tables).as<uint32_t>();
+    const size_t M = view ? B : ctx->kt_maps;
+    const ForestView F{ctx->tgt_pnodes.as<float4>(), (view ? ctx->v_centres : ctx->kt_centres).as<double>(), tab, tab + (view ? M + 1 : 3 * (M + 1))};
     CU(launch_forest_search(Bp, F, n_tiles, ctx->kt_depth, search_bound(rejector, max_dist_sq), ctx->b_vcorr.as<uint32_t>(), ctx->stream));
     ctx->launches += 1;
   } else if (n_tiles && !voxel) {
@@ -188,32 +240,12 @@ int error_round(sgb_ctx* ctx, const double* T, const uint8_t* active) {
   return 0;
 }
 
-}  // namespace
-
-extern "C" {
-
-int sgb_source_set_batch(sgb_ctx* ctx, size_t n_members, const size_t* offsets, const double* points, const double* covs) {
-  if (!ctx) return 1;
-  if (n_members > SGB_BATCH_MAX_MEMBERS)
-    return fail(ctx, 1, "sgb_source_set_batch: " + std::to_string(n_members) + " members, at most " + std::to_string(SGB_BATCH_MAX_MEMBERS));
-  if (!offsets) return fail(ctx, 1, "sgb_source_set_batch: null offsets");
-  if (offsets[0] != 0) return fail(ctx, 1, "sgb_source_set_batch: offsets[0] must be 0");
-  size_t largest = 0;
-  for (size_t m = 0; m < n_members; m++) {
-    if (offsets[m + 1] < offsets[m]) return fail(ctx, 1, "sgb_source_set_batch: offsets must be ascending (member " + std::to_string(m) + ")");
-    largest = std::max(largest, offsets[m + 1] - offsets[m]);
-  }
-  const size_t n = offsets[n_members];
-  if (n >= (1ull << 31)) return fail(ctx, 1, "sgb_source_set_batch: too many points");
-  if (n && !points) return fail(ctx, 1, "sgb_source_set_batch: null points");
-  CU(cudaSetDevice(ctx->device));
-  begin_source(ctx, SourceState::Batch, 0, covs != nullptr);
-  ctx->b_offsets.assign(offsets, offsets + n_members + 1);
+// Sizes everything a call on the members of b_offsets touches (so that no round allocates), clears their per-member state and
+// correspondences: a new batch and a new pairing start alike.
+int reserve_members(sgb_ctx* ctx) {
+  const size_t n_members = batch_members(ctx), B = std::max<size_t>(n_members, 1), nn = std::max<size_t>(batch_points(ctx), 1);
   ctx->b_lin.assign(n_members, 0);
   ctx->b_seeded.assign(n_members, 0);
-  const size_t B = std::max<size_t>(n_members, 1), nn = std::max<size_t>(n, 1);
-  CU(ctx->b_centres.reserve(B * 4 * sizeof(double)));
-  CU(ctx->b_bounds.reserve(B * 6 * sizeof(double)));
   CU(ctx->b_poses.reserve(B * 12 * sizeof(double)));
   CU(ctx->b_lin_poses.reserve(B * 12 * sizeof(double)));
   CU(ctx->b_members.reserve(B * sizeof(uint4)));
@@ -224,7 +256,35 @@ int sgb_source_set_batch(sgb_ctx* ctx, size_t n_members, const size_t* offsets, 
   CU(ctx->b_vq.reserve(nn * sizeof(float4)));
   CU(ctx->b_vcorr.reserve(nn * sizeof(uint32_t)));
   CU(cudaMemsetAsync(ctx->b_corr.p, 0xFF, nn * sizeof(uint32_t), ctx->stream));  // no correspondences before the first linearize
-  if (int rc = reserve_query_scratch(ctx, nn)) return rc;
+  return reserve_query_scratch(ctx, nn);
+}
+
+}  // namespace
+
+extern "C" {
+
+int sgb_source_set_batch(sgb_ctx* ctx, size_t n_members, const size_t* offsets, const double* points, const double* covs) {
+  if (!ctx) return 1;
+  if (n_members > SGB_BATCH_MAX_MEMBERS)
+    return fail(ctx, 1, "sgb_source_set_batch: " + std::to_string(n_members) + " members, at most " + std::to_string(SGB_BATCH_MAX_MEMBERS));
+  if (!offsets) return fail(ctx, 1, "sgb_source_set_batch: null offsets");
+  if (offsets[0] != 0) return fail(ctx, 1, "sgb_source_set_batch: offsets[0] must be 0");
+  for (size_t m = 0; m < n_members; m++)
+    if (offsets[m + 1] < offsets[m]) return fail(ctx, 1, "sgb_source_set_batch: offsets must be ascending (member " + std::to_string(m) + ")");
+  const size_t n = offsets[n_members];
+  if (n >= (1ull << 31)) return fail(ctx, 1, "sgb_source_set_batch: too many points");
+  if (n && !points) return fail(ctx, 1, "sgb_source_set_batch: null points");
+  CU(cudaSetDevice(ctx->device));
+  begin_source(ctx, SourceState::Batch, 0, covs != nullptr);
+  ctx->b_cloud_offsets.assign(offsets, offsets + n_members + 1);
+  ctx->b_offsets = ctx->b_cloud_offsets;  // no pairing: the members are the clouds
+  const size_t B = std::max<size_t>(n_members, 1), nn = std::max<size_t>(n, 1);
+  CU(ctx->b_centres.reserve(B * 4 * sizeof(double)));
+  CU(ctx->b_bounds.reserve(B * 6 * sizeof(double)));
+  if (int rc = reserve_members(ctx)) return rc;
+  const std::vector<uint32_t> off32(offsets, offsets + n_members + 1);
+  CU(ctx->b_cloud_off.reserve(off32.size() * sizeof(uint32_t)));
+  CU(cudaMemcpyAsync(ctx->b_cloud_off.p, off32.data(), off32.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
   if (n == 0) return 0;
   CU(ctx->stage_pts.reserve(n * 4 * sizeof(double)));
   CU(ctx->tmp_pts.reserve(n * sizeof(float4)));
@@ -241,18 +301,113 @@ int sgb_source_set_batch(sgb_ctx* ctx, size_t n_members, const size_t* offsets, 
     CU(ctx->src_covB.reserve(n * sizeof(float4)));
     CU(cudaMemcpyAsync(ctx->stage_covs.p, covs, n * 16 * sizeof(double), cudaMemcpyDefault, ctx->stream));
   }
-  size_t temp_bytes = 0;
-  CU(sort_pairs_u64_u32_bits(nullptr, temp_bytes, ctx->keys_in.as<uint64_t>(), ctx->keys_out.as<uint64_t>(), ctx->vals_in.as<uint32_t>(),
-                             ctx->src_perm.as<uint32_t>(), largest, 63, ctx->stream));
-  CU(ctx->sort_temp.reserve(temp_bytes));
-  // Every member is stored exactly as sgb_source_set_points stores one cloud: centred on its own box, rounded to FP32, sorted along the
+  // Every cloud is stored exactly as sgb_source_set_points stores one cloud: centred on its own box, rounded to FP32, sorted along the
   // curve within itself, covariances packed into its search order.  Its slice of the storage is contiguous.
-  for (size_t m = 0; m < n_members; m++) {
-    const size_t off = offsets[m], nm = offsets[m + 1] - offsets[m];
-    if (nm == 0) continue;
-    if (int rc = store_source(ctx, off, nm, ctx->b_centres.as<double>() + 4 * m, ctx->b_bounds.as<double>() + 6 * m, nullptr, temp_bytes, 1, covs ? 1 : 0, nullptr))
-      return rc;
+  StoreClouds sc = {};
+  sc.n = static_cast<uint32_t>(n);
+  sc.n_clouds = static_cast<uint32_t>(n_members);
+  sc.cloud_bits = 1;
+  while ((1ull << sc.cloud_bits) < n_members) sc.cloud_bits++;
+  sc.sm_count = ctx->sm_count;
+  sc.points = ctx->stage_pts.as<double>();
+  sc.covs = covs ? ctx->stage_covs.as<double>() : nullptr;
+  sc.offsets = ctx->b_cloud_off.as<uint32_t>();
+  sc.bounds = ctx->b_bounds.as<double>();
+  sc.centres = ctx->b_centres.as<double>();
+  sc.orig_pts = ctx->tmp_pts.as<float4>();
+  sc.keys_a = ctx->keys_in.as<uint64_t>();
+  sc.keys_b = ctx->keys_out.as<uint64_t>();
+  sc.vals_a = ctx->vals_in.as<uint32_t>();
+  sc.vals_b = ctx->src_rank.as<uint32_t>();
+  sc.pts = ctx->src_pts.as<float4>();
+  sc.covA = ctx->src_covA.as<float4>();
+  sc.covB = ctx->src_covB.as<float4>();
+  sc.perm = ctx->src_perm.as<uint32_t>();
+  size_t key_bytes = 0, cloud_bytes = 0;
+  CU(sort_pairs_u64_u32_bits(nullptr, key_bytes, sc.keys_a, sc.keys_b, sc.vals_a, sc.vals_b, n, 63, ctx->stream));
+  CU(sort_pairs_u64_u32_bits(nullptr, cloud_bytes, sc.keys_a, sc.keys_b, sc.vals_b, sc.vals_a, n, sc.cloud_bits, ctx->stream));
+  sc.sort_temp_bytes = std::max(key_bytes, cloud_bytes);
+  CU(ctx->sort_temp.reserve(sc.sort_temp_bytes));
+  sc.sort_temp = ctx->sort_temp.p;
+  CU(launch_store_clouds(sc, ctx->stream));
+  ctx->launches += 6;
+  return 0;
+}
+
+int sgb_source_set_pairs(sgb_ctx* ctx, size_t n_members, const uint32_t* clouds, const uint32_t* maps) {
+  if (!ctx) return 1;
+  if (ctx->src_state != SourceState::Batch) return fail(ctx, 1, "sgb_source_set_pairs: the context holds no batch of sources (call sgb_source_set_batch)");
+  if (n_members > SGB_BATCH_MAX_MEMBERS)
+    return fail(ctx, 1, "sgb_source_set_pairs: " + std::to_string(n_members) + " members, at most " + std::to_string(SGB_BATCH_MAX_MEMBERS));
+  const std::vector<size_t>& coff = ctx->b_cloud_offsets;
+  const size_t N = coff.size() - 1, P = n_members;
+  if (!clouds && P != N)
+    return fail(ctx, 1, "sgb_source_set_pairs: without a cloud table member p is cloud p, so the member count (" + std::to_string(P) +
+                            ") must equal the cloud count (" + std::to_string(N) + ")");
+  // the device table: member offsets [P + 1] | cloud of each member [P] | map of each member [P] (only with maps)
+  std::vector<uint32_t> tab(2 * P + 1 + (maps ? P : 0));
+  std::vector<size_t> member_off(P + 1, 0);
+  uint32_t max_map = 0;
+  for (size_t p = 0; p < P; p++) {
+    const size_t c = clouds ? clouds[p] : p;
+    if (c >= N)
+      return fail(ctx, 1, "sgb_source_set_pairs: member " + std::to_string(p) + " names cloud " + std::to_string(c) + " but the batch holds " +
+                              std::to_string(N) + " clouds");
+    member_off[p + 1] = member_off[p] + (coff[c + 1] - coff[c]);
+    if (member_off[p + 1] >= (1ull << 31)) return fail(ctx, 1, "sgb_source_set_pairs: too many member points (at most 2^31 - 1 in all)");
+    tab[P + 1 + p] = static_cast<uint32_t>(c);
+    if (maps) {
+      tab[2 * P + 1 + p] = maps[p];
+      max_map = std::max(max_map, maps[p]);
+    }
   }
+  for (size_t p = 0; p <= P; p++) tab[p] = static_cast<uint32_t>(member_off[p]);
+  const size_t n = member_off[P];
+  CU(cudaSetDevice(ctx->device));
+  begin_pairs(ctx);
+  ctx->b_offsets = member_off;
+  ctx->b_pair_has_maps = maps != nullptr;
+  if (maps) ctx->b_pair_maps.assign(maps, maps + P);
+  ctx->b_pair_max_map = max_map;
+  const size_t B = std::max<size_t>(P, 1), nn = std::max<size_t>(n, 1);
+  if (int rc = reserve_members(ctx)) return rc;
+  CU(ctx->p_tables.reserve(tab.size() * sizeof(uint32_t)));
+  CU(ctx->p_pts.reserve(nn * sizeof(float4)));
+  CU(ctx->p_perm.reserve(nn * sizeof(uint32_t)));
+  CU(ctx->p_centres.reserve(B * 4 * sizeof(double)));
+  CU(ctx->p_bounds.reserve(B * 6 * sizeof(double)));
+  if (ctx->src_has_covs) {
+    CU(ctx->p_covA.reserve(nn * sizeof(float4)));
+    CU(ctx->p_covB.reserve(nn * sizeof(float4)));
+  }
+  if (maps) {  // the view of whatever many-maps target the calls meet (pair_view)
+    CU(ctx->v_centres.reserve(B * 4 * sizeof(double)));
+    CU(ctx->v_tables.reserve((2 * B + 1) * sizeof(uint32_t)));
+    CU(ctx->v_regions.reserve(B * sizeof(uint4)));
+  }
+  if (P == 0) return 0;
+  // pageable host memory: the copy is staged before cudaMemcpyAsync returns
+  CU(cudaMemcpyAsync(ctx->p_tables.p, tab.data(), tab.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
+  PairGather g = {};
+  g.n = static_cast<uint32_t>(n);
+  g.n_members = static_cast<uint32_t>(P);
+  g.member_off = ctx->p_tables.as<uint32_t>();
+  g.clouds = g.member_off + P + 1;
+  g.cloud_off = ctx->b_cloud_off.as<uint32_t>();
+  g.pts = ctx->src_pts.as<float4>();
+  g.covA = ctx->src_has_covs ? ctx->src_covA.as<float4>() : nullptr;
+  g.covB = ctx->src_covB.as<float4>();
+  g.perm = ctx->src_perm.as<uint32_t>();
+  g.centres = ctx->b_centres.as<double>();
+  g.bounds = ctx->b_bounds.as<double>();
+  g.out_pts = ctx->p_pts.as<float4>();
+  g.out_covA = ctx->p_covA.as<float4>();
+  g.out_covB = ctx->p_covB.as<float4>();
+  g.out_perm = ctx->p_perm.as<uint32_t>();
+  g.out_centres = ctx->p_centres.as<double>();
+  g.out_bounds = ctx->p_bounds.as<double>();
+  CU(launch_pair_gather(g, ctx->sm_count, ctx->stream));
+  ctx->launches += 1;
   return 0;
 }
 
@@ -267,6 +422,7 @@ int sgb_linearize_batch(sgb_ctx* ctx, int factor, int robust, double robust_c, i
   if (batch_points(ctx) && ctx->n_tgt) {
     if (int rc = check_target(ctx, "sgb_linearize_batch", factor)) return rc;
   }
+  if (int rc = pair_view(ctx)) return rc;
   if (int rc = linearize_round(ctx, factor, robust, robust_c, rejector, max_dist_sq, T, active)) return rc;
   return copy_out(ctx, out44, 44 * B);
 }
@@ -281,6 +437,7 @@ int sgb_error_batch(sgb_ctx* ctx, const double* T, const uint8_t* active, double
   for (size_t m = 0; m < B; m++)
     if ((!active || active[m]) && !ctx->b_lin[m])
       return fail(ctx, 1, "sgb_error_batch: member " + std::to_string(m) + " is active but has not been linearised against the current target");
+  if (int rc = pair_view(ctx)) return rc;
   if (int rc = error_round(ctx, T, active)) return rc;
   return copy_out(ctx, out_e, B);
 }
@@ -299,6 +456,7 @@ int sgb_align_batch(sgb_ctx* ctx, const sgb_align_options* o, const double* init
     if (int rc = check_target(ctx, "sgb_align_batch", o->factor_kind)) return rc;
   }
   CU(cudaSetDevice(ctx->device));
+  if (int rc = pair_view(ctx)) return rc;
   AlignOptions ao;
   ao.lm = o->optimizer_kind == SGB_OPT_LEVENBERG_MARQUARDT;
   ao.max_iterations = o->max_iterations;
@@ -371,6 +529,7 @@ int sgb_correspondences_batch(sgb_ctx* ctx, uint64_t* out) {
   if (!out) return fail(ctx, 1, "sgb_correspondences_batch: null output");
   CU(cudaSetDevice(ctx->device));
   CU(ctx->corr64.reserve(n * sizeof(uint64_t)));
+  const uint32_t* perm = (ctx->b_paired ? ctx->p_perm : ctx->src_perm).as<uint32_t>();
   for (size_t m = 0; m + 1 < ctx->b_offsets.size(); m++) {
     const size_t off = ctx->b_offsets[m], nm = ctx->b_offsets[m + 1] - off;
     if (nm == 0) continue;
@@ -381,11 +540,9 @@ int sgb_correspondences_batch(sgb_ctx* ctx, uint64_t* out) {
     }
     // a multi-map target: the id within the member's own map (tgt_pts[k].w), as a context holding that map alone reports it
     if (ctx->tgt_state == TargetState::VoxelMaps)
-      CU(launch_voxelmaps_correspondences(ctx->b_corr.as<uint32_t>() + off, ctx->src_perm.as<uint32_t>() + off, nm, ctx->tgt_pts.as<float4>(),
-                                          ctx->corr64.as<uint64_t>() + off, ctx->sm_count, ctx->stream));
+      CU(launch_voxelmaps_correspondences(ctx->b_corr.as<uint32_t>() + off, perm + off, nm, ctx->tgt_pts.as<float4>(), ctx->corr64.as<uint64_t>() + off, ctx->sm_count, ctx->stream));
     else
-      CU(launch_correspondences(ctx->b_corr.as<uint32_t>() + off, ctx->src_perm.as<uint32_t>() + off, nm, ctx->tgt_pts.as<float4>(),
-                                voxel_target(ctx) ? 1 : 0, ctx->corr64.as<uint64_t>() + off, ctx->sm_count, ctx->stream));
+      CU(launch_correspondences(ctx->b_corr.as<uint32_t>() + off, perm + off, nm, ctx->tgt_pts.as<float4>(), voxel_target(ctx) ? 1 : 0, ctx->corr64.as<uint64_t>() + off, ctx->sm_count, ctx->stream));
     ctx->launches += 1;
   }
   CU(cudaMemcpyAsync(out, ctx->corr64.p, n * sizeof(uint64_t), cudaMemcpyDefault, ctx->stream));

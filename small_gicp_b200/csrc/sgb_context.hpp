@@ -187,6 +187,20 @@ struct sgb_ctx {
   sgb::DevBuf b_vq, b_vcorr;               // virtual source of the search: transformed queries of the active members and what the search found
   sgb::DevBuf b_partials, b_out;           // per-tile partial sums, per-member results
   sgb::DevBuf b_state, b_phase;            // sgb_align_batch: per member MemberState / next round (kPhase*, one byte)
+  // The clouds of sgb_source_set_batch are stored once (src_* and b_centres / b_bounds, cloud after cloud).  Without a pairing the
+  // members are those clouds.  After sgb_source_set_pairs (b_paired) member p is a replica of one stored cloud in p_*, b_offsets are
+  // the members' offsets, and b_pair_maps (empty: member m against map m) names each member's map.
+  std::vector<size_t> b_cloud_offsets;     // clouds + 1
+  sgb::DevBuf b_cloud_off;                 // the same as uint32, on the device
+  bool b_paired = false;
+  bool b_pair_has_maps = false;  // the pairing has a maps table (possibly of 0 members)
+  std::vector<uint32_t> b_pair_maps;
+  uint32_t b_pair_max_map = 0;
+  sgb::DevBuf p_tables;                    // uint32: member offsets [members + 1] | cloud of each member | map of each member
+  sgb::DevBuf p_pts, p_covA, p_covB, p_perm, p_centres, p_bounds;
+  // the many-maps target seen through b_pair_maps (PairView): rebuilt by the first batched call after the pairing or the target changed
+  bool b_view_ok = false;
+  sgb::DevBuf v_centres, v_tables, v_regions;  // [members][4] / pt_off [members + 1] | node_base [members] / [members]
 };
 
 namespace sgb {
@@ -214,8 +228,10 @@ int begin_forest_target(sgb_ctx* ctx, size_t n, bool normals, bool covs, size_t 
 size_t target_maps(const sgb_ctx* ctx);
 /// the point target's tree in tgt_perm / tgt_pts / tgt_pnodes (depth, n_pnodes packet records) becomes its search structure; builds the grid
 int install_tree(sgb_ctx* ctx, int depth, size_t n_pnodes);
-/// a single cloud of n points, a batch (n = 0) or nothing replaces the source
+/// a single cloud of n points, a batch (n = 0) or nothing replaces the source (and forgets any pairing of a batch)
 void begin_source(sgb_ctx* ctx, SourceState state, size_t n, bool covs);
+/// the batch's members become pairs of its stored clouds (the caller fills b_offsets, b_pair_maps and the replicas)
+void begin_pairs(sgb_ctx* ctx);
 /// normals and covariances (target) or covariances (source) were estimated on the device
 void features_changed(sgb_ctx* ctx, bool target);
 

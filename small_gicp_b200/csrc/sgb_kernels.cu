@@ -403,6 +403,107 @@ __global__ void convert_cov_scatter_kernel(const double* __restrict__ covs, size
   }
 }
 
+// ---- many source clouds stored in one pass (sgb_source_set_batch): cloud c = points off[c] .. off[c+1], each stored exactly as
+// store_source stores it alone.  Here because the curve (curve_key, d_use_hilbert) must have one definition per library.
+// One CTA per cloud: its exact box -> bounds [6] and centre [4], centre_kernel's formula (min / max are exact, so the atomics of
+// launch_bounds_centre give the same values)
+__global__ void __launch_bounds__(256) clouds_box_kernel(const double4* __restrict__ pts, const uint32_t* __restrict__ off, double* bounds, double* centres) {
+  __shared__ double s_red[8][6];
+  const uint32_t c = blockIdx.x, first = off[c], last = off[c + 1];
+  double lo[3] = {DBL_MAX, DBL_MAX, DBL_MAX}, hi[3] = {-DBL_MAX, -DBL_MAX, -DBL_MAX};
+  for (uint32_t i = first + threadIdx.x; i < last; i += blockDim.x) {
+    const double4 p = pts[i];
+    lo[0] = fmin(lo[0], p.x); lo[1] = fmin(lo[1], p.y); lo[2] = fmin(lo[2], p.z);
+    hi[0] = fmax(hi[0], p.x); hi[1] = fmax(hi[1], p.y); hi[2] = fmax(hi[2], p.z);
+  }
+#pragma unroll
+  for (int d = 0; d < 3; d++) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      lo[d] = fmin(lo[d], __shfl_down_sync(0xffffffffu, lo[d], o));
+      hi[d] = fmax(hi[d], __shfl_down_sync(0xffffffffu, hi[d], o));
+    }
+  }
+  const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
+  if (lane == 0) {
+#pragma unroll
+    for (int d = 0; d < 3; d++) {
+      s_red[warp][d] = lo[d];
+      s_red[warp][3 + d] = hi[d];
+    }
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    for (int w = 1; w < 8; w++) {
+#pragma unroll
+      for (int d = 0; d < 3; d++) {
+        lo[d] = fmin(lo[d], s_red[w][d]);
+        hi[d] = fmax(hi[d], s_red[w][3 + d]);
+      }
+    }
+    double* b = bounds + 6 * static_cast<size_t>(c);
+    double* ce = centres + 4 * static_cast<size_t>(c);
+    double ext = 0.0;
+    for (int d = 0; d < 3; d++) {
+      b[d] = lo[d];
+      b[3 + d] = hi[d];
+      ce[d] = (lo[d] <= hi[d]) ? 0.5 * (lo[d] + hi[d]) : 0.0;
+      ext = fmax(ext, hi[d] - lo[d]);
+    }
+    ce[3] = ext > 0.0 ? ext : 1.0;
+  }
+}
+
+// the cloud that owns global position i (forest_map_of: empty clouds own nothing)
+__device__ __forceinline__ uint32_t cloud_of(const uint32_t* __restrict__ off, uint32_t n_clouds, uint32_t i) {
+  uint32_t lo = 0, hi = n_clouds;
+  while (hi - lo > 1u) {
+    const uint32_t mid = (lo + hi) >> 1;
+    if (__ldg(&off[mid]) <= i) lo = mid;
+    else hi = mid;
+  }
+  return lo;
+}
+
+// convert_kernel's arithmetic about each point's own cloud centre: centred FP32 point in original order (w = index within the cloud),
+// curve key, vals = global position
+__global__ void clouds_convert_kernel(const double4* __restrict__ pts, uint32_t n, const uint32_t* __restrict__ off, uint32_t n_clouds,
+                                      const double* __restrict__ centres, float4* out_pts, uint64_t* keys, uint32_t* vals) {
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    const uint32_t c = cloud_of(off, n_clouds, i);
+    const double* centre = centres + 4 * static_cast<size_t>(c);
+    const double cx = centre[0], cy = centre[1], cz = centre[2];
+    const double inv_ext = 2097151.0 / centre[3];
+    const double4 p = pts[i];
+    const double x = p.x - cx, y = p.y - cy, z = p.z - cz;
+    out_pts[i] = make_float4((float)x, (float)y, (float)z, __int_as_float(static_cast<int>(i - off[c])));
+    keys[i] = curve_key(x, y, z, 0.5 * centre[3], inv_ext);
+    vals[i] = i;
+  }
+}
+
+// after the stable key sort (vals = global positions in key order): the cloud of each, the key of the stable sort by cloud
+__global__ void clouds_ids_kernel(const uint32_t* __restrict__ vals, uint32_t n, const uint32_t* __restrict__ off, uint32_t n_clouds, uint64_t* keys) {
+  for (uint32_t j = blockIdx.x * blockDim.x + threadIdx.x; j < n; j += gridDim.x * blockDim.x) keys[j] = cloud_of(off, n_clouds, vals[j]);
+}
+
+// order = global positions in (cloud, key, index) order, the per-cloud sort's order: every cloud's search-order points, the
+// search order -> index within the cloud (the converted point's w), covariances packed into that order
+__global__ void clouds_store_kernel(const uint32_t* __restrict__ order, uint32_t n, const float4* __restrict__ orig, const double* __restrict__ covs, float4* pts,
+                                    uint32_t* perm, float4* covA, float4* covB) {
+  for (uint32_t j = blockIdx.x * blockDim.x + threadIdx.x; j < n; j += gridDim.x * blockDim.x) {
+    const uint32_t g = order[j];
+    const float4 f = orig[g];
+    pts[j] = f;
+    perm[j] = static_cast<uint32_t>(__float_as_int(f.w));
+    if (covs) {
+      const double* c = covs + static_cast<size_t>(g) * 16;
+      covA[j] = pack_covA(c);
+      covB[j] = pack_covB(c);
+    }
+  }
+}
+
 // curve keys of points that are already on the device in centred FP32 form (target: device-side tree construction)
 __global__ void curve_keys_kernel(const float4* __restrict__ pts, size_t n, const double* __restrict__ centre, uint64_t* keys, uint32_t* vals) {
   const double inv_ext = 2097151.0 / centre[3], h = 0.5 * centre[3];
@@ -797,6 +898,21 @@ cudaError_t launch_voxelmaps_correspondences(const uint32_t* corr, const uint32_
                                              cudaStream_t st) {
   if (!n) return cudaSuccess;
   voxelmaps_correspondences_kernel<<<grid_for(n, 256, sm_count * 8), 256, 0, st>>>(corr, perm, n, tgt_pts, out);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_store_clouds(const StoreClouds& s, cudaStream_t st) {
+  const uint32_t n = s.n;
+  clouds_box_kernel<<<s.n_clouds, 256, 0, st>>>(reinterpret_cast<const double4*>(s.points), s.offsets, s.bounds, s.centres);
+  const int g = grid_for(n, 256, s.sm_count * 8);
+  clouds_convert_kernel<<<g, 256, 0, st>>>(reinterpret_cast<const double4*>(s.points), n, s.offsets, s.n_clouds, s.centres, s.orig_pts, s.keys_a, s.vals_a);
+  size_t tb = s.sort_temp_bytes;
+  cudaError_t e = sort_pairs_u64_u32_bits(s.sort_temp, tb, s.keys_a, s.keys_b, s.vals_a, s.vals_b, n, 63, st);
+  if (e != cudaSuccess) return e;
+  clouds_ids_kernel<<<g, 256, 0, st>>>(s.vals_b, n, s.offsets, s.n_clouds, s.keys_a);
+  tb = s.sort_temp_bytes;
+  if ((e = sort_pairs_u64_u32_bits(s.sort_temp, tb, s.keys_a, s.keys_b, s.vals_b, s.vals_a, n, s.cloud_bits, st)) != cudaSuccess) return e;
+  clouds_store_kernel<<<g, 256, 0, st>>>(s.vals_a, n, s.orig_pts, s.covs, s.pts, s.perm, s.covA, s.covB);
   return cudaGetLastError();
 }
 

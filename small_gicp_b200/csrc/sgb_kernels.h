@@ -89,6 +89,26 @@ cudaError_t launch_bounds_centre(const double* d_pts4, size_t n, double* d_bound
 cudaError_t launch_convert(const double* d_pts4, const double* d_normals4, const double* d_covs16, size_t n, const double* d_centre4, float4* out_pts,
                            float4* out_normals, float4* out_covA, float4* out_covB, uint64_t* keys, uint32_t* vals, int sm_count, cudaStream_t st,
                            float4* out_lo = nullptr);
+/// Many source clouds stored in one pass, each bit-identical to store_source of it alone (sgb_source_set_batch): cloud c = points
+/// offsets[c] .. offsets[c+1] (device, uint32).  Per-cloud box and centre, FP32 conversion and curve keys, a stable key sort, a stable
+/// sort by cloud (cloud_bits bits), then the points, search order -> index within the cloud, and covariances (covs or null) in
+/// (cloud, key, index) order: the order of the per-cloud sorts.  6 launches (the two sorts count one each), whatever n_clouds is.
+struct StoreClouds {
+  uint32_t n, n_clouds;
+  int cloud_bits, sm_count;
+  const double* points;  // n x 4
+  const double* covs;    // n x 16 or null
+  const uint32_t* offsets;
+  double *bounds, *centres;  // [n_clouds][6] / [n_clouds][4]
+  float4* orig_pts;          // scratch: centred FP32 points in original order, w = index within the cloud
+  uint64_t *keys_a, *keys_b;
+  uint32_t *vals_a, *vals_b;
+  void* sort_temp;
+  size_t sort_temp_bytes;  // enough for both sorts of n pairs
+  float4 *pts, *covA, *covB;
+  uint32_t* perm;
+};
+cudaError_t launch_store_clouds(const StoreClouds& s, cudaStream_t st);
 cudaError_t launch_inverse_perm(const uint32_t* perm, size_t n, uint32_t* rank, int sm_count, cudaStream_t st);
 cudaError_t launch_convert_cov_scatter(const double* d_covs16, size_t first, size_t n, const uint32_t* rank, float4* outA, float4* outB, float4* origA,
                                        float4* origB, int sm_count, cudaStream_t st);

@@ -6,8 +6,10 @@
 #pragma once
 #include <cstring>
 #include <stdexcept>
+#include <tuple>
 #include <string>
 #include <type_traits>
+#include <utility>
 #include <vector>
 
 #include "../../../../include/sgicp_b200.h"
@@ -67,8 +69,8 @@ struct BatchRegistration {
 
   /// One RegistrationResult per (target, source) pair, in order: source m from init_Ts[m] against a Gaussian voxel map of targets[m]
   /// (GaussianVoxelMap(voxel_resolution) with search_offsets 1 / 7 / 27, inserted once), all pairs in one sgb_align_batch call.  The maps are
-  /// built on the device in one sgb_target_build_voxelmaps call; the targets need covariances for GICP.  Repeat a cloud to pair it
-  /// with several others.  The context's target is replaced, so the reduction's target mirror is dropped.
+  /// built on the device in one sgb_target_build_voxelmaps call; the targets need covariances for GICP.  To pair a cloud with
+  /// several others, use the overload with a pair list.  The context's target is replaced, so the reduction's target mirror is dropped.
   template <typename Target, typename Source>
   std::vector<RegistrationResult> align(const std::vector<Target>& targets, const std::vector<Source>& sources, const std::vector<Isometry3d>& init_Ts,
                                         double voxel_resolution, int search_offsets) const {
@@ -95,6 +97,44 @@ struct BatchRegistration {
     const Concatenated tgt(targets, true), src(sources);
     check(ctx, sgb_target_build_kdtrees(ctx, targets.size(), tgt.offsets.data(), tgt.points.data(), tgt.normals_or_null(), tgt.covs_or_null()));
     check(ctx, sgb_source_set_batch(ctx, sources.size(), src.offsets.data(), src.points.data(), src.covs_or_null()));
+    return run(ctx, init_Ts);
+  }
+
+  /// One RegistrationResult per (source index, target index) pair, in order: sources[pairs[p].first] from init_Ts[p] against the kd-tree
+  /// of targets[pairs[p].second].  Each target's tree is built once and each source uploaded once, however many pairs use it
+  /// (sgb_source_set_pairs); all pairs in one sgb_align_batch call.  Normals / covariances as for the one-to-one overload.
+  template <typename Target, typename Source>
+  std::vector<RegistrationResult> align(const std::vector<Target>& targets, const std::vector<Source>& sources, const std::vector<std::pair<size_t, size_t>>& pairs,
+                                        const std::vector<Isometry3d>& init_Ts) const {
+    sgb_ctx* ctx = reduction.context();
+    reduction.invalidate();
+    const Concatenated tgt(targets, true);
+    check(ctx, sgb_target_build_kdtrees(ctx, targets.size(), tgt.offsets.data(), tgt.points.data(), tgt.normals_or_null(), tgt.covs_or_null()));
+    return run_pairs(ctx, sources, targets.size(), pairs, init_Ts);
+  }
+
+  /// The same against a Gaussian voxel map of each target (the voxel-map overload's settings), each map built once.
+  template <typename Target, typename Source>
+  std::vector<RegistrationResult> align(const std::vector<Target>& targets, const std::vector<Source>& sources, const std::vector<std::pair<size_t, size_t>>& pairs,
+                                        const std::vector<Isometry3d>& init_Ts, double voxel_resolution, int search_offsets) const {
+    sgb_ctx* ctx = reduction.context();
+    reduction.invalidate();
+    const Concatenated tgt(targets);
+    check(ctx, sgb_target_build_voxelmaps(ctx, targets.size(), tgt.offsets.data(), tgt.points.data(), tgt.covs_or_null(), voxel_resolution, search_offsets));
+    return run_pairs(ctx, sources, targets.size(), pairs, init_Ts);
+  }
+
+  /// Multi-start: one RegistrationResult per member, in order: sources[cloud_of_member[p]] from init_Ts[p] against the one target, each
+  /// source uploaded once however many starts it has.
+  template <typename Target, typename Tree, typename Source>
+  std::vector<RegistrationResult> align(const Target& target, const Tree& target_tree, const std::vector<Source>& sources, const std::vector<size_t>& cloud_of_member,
+                                        const std::vector<Isometry3d>& init_Ts) const {
+    if (cloud_of_member.size() != init_Ts.size()) throw std::runtime_error("BatchRegistration: one initial pose per member");
+    sgb_ctx* ctx = reduction.batch_context(target, target_tree);
+    const Concatenated src(sources);
+    check(ctx, sgb_source_set_batch(ctx, sources.size(), src.offsets.data(), src.points.data(), src.covs_or_null()));
+    const std::vector<uint32_t> clouds = indices(cloud_of_member, sources.size(), "source");
+    check(ctx, sgb_source_set_pairs(ctx, clouds.size(), clouds.data(), nullptr));
     return run(ctx, init_Ts);
   }
 
@@ -135,6 +175,29 @@ private:
     const double* normals_or_null() const { return has_normals ? normals.data() : nullptr; }
     const double* covs_or_null() const { return has_covs ? covs.data() : nullptr; }
   };
+
+  static std::vector<uint32_t> indices(const std::vector<size_t>& idx, size_t count, const char* what) {
+    std::vector<uint32_t> out(idx.size());
+    for (size_t p = 0; p < idx.size(); p++) {
+      if (idx[p] >= count) throw std::runtime_error(std::string("BatchRegistration: member ") + std::to_string(p) + " names " + what + " " + std::to_string(idx[p]) + " of " + std::to_string(count));
+      out[p] = static_cast<uint32_t>(idx[p]);
+    }
+    return out;
+  }
+
+  /// the sources uploaded once, paired as the list says with the maps of the context's many-maps target, then aligned
+  template <typename Source>
+  std::vector<RegistrationResult> run_pairs(sgb_ctx* ctx, const std::vector<Source>& sources, size_t n_maps, const std::vector<std::pair<size_t, size_t>>& pairs,
+                                            const std::vector<Isometry3d>& init_Ts) const {
+    if (pairs.size() != init_Ts.size()) throw std::runtime_error("BatchRegistration: one initial pose per pair");
+    std::vector<size_t> c(pairs.size()), t(pairs.size());
+    for (size_t p = 0; p < pairs.size(); p++) std::tie(c[p], t[p]) = pairs[p];
+    const Concatenated src(sources);
+    check(ctx, sgb_source_set_batch(ctx, sources.size(), src.offsets.data(), src.points.data(), src.covs_or_null()));
+    const std::vector<uint32_t> clouds = indices(c, sources.size(), "source"), maps = indices(t, n_maps, "target");
+    check(ctx, sgb_source_set_pairs(ctx, clouds.size(), clouds.data(), maps.data()));
+    return run(ctx, init_Ts);
+  }
 
   /// sgb_align_batch of the context's batch from init_Ts with this registration's settings
   std::vector<RegistrationResult> run(sgb_ctx* ctx, const std::vector<Isometry3d>& init_Ts) const {

@@ -89,7 +89,7 @@ RegistrationResult run(const Options& o, const std::shared_ptr<PointCloud>& targ
 /// BatchRegistration<...>::align of every source from its initial pose, configured like run()
 template <typename Factor, typename General, typename Rejector, typename Optimizer, bool kRobust>
 std::vector<RegistrationResult> run_batch(const Options& o, const std::shared_ptr<PointCloud>& target, const std::vector<PointCloud>& sources,
-                                          const std::vector<Isometry3d>& init) {
+                                          const std::vector<Isometry3d>& init, const std::vector<size_t>* cloud_of_member) {
   BatchRegistration<Factor, General, Rejector, Optimizer> reg;
   configure(reg, o);
   set_rejector(reg, o, std::is_same<Rejector, DistanceRejector>());
@@ -99,27 +99,28 @@ std::vector<RegistrationResult> run_batch(const Options& o, const std::shared_pt
     GaussianVoxelMap map(o.voxel_resolution);
     map.set_search_offsets(o.voxel_search_offsets);
     map.insert(*target);
-    return reg.align(map, map, sources, init);
+    return cloud_of_member ? reg.align(map, map, sources, *cloud_of_member, init) : reg.align(map, map, sources, init);
   }
   if (o.tree == 1) {
     DeviceKdTree<PointCloud> tree(target);
-    return reg.align(*target, tree, sources, init);
+    return cloud_of_member ? reg.align(*target, tree, sources, *cloud_of_member, init) : reg.align(*target, tree, sources, init);
   }
   KdTree<PointCloud> tree(target);
-  return reg.align(*target, tree, sources, init);
+  return cloud_of_member ? reg.align(*target, tree, sources, *cloud_of_member, init) : reg.align(*target, tree, sources, init);
 }
 
 /// BatchRegistration<...>::align of every (target, source) pair: source m against a Gaussian voxel map of targets[m], configured like run()
 template <typename Factor, typename General, typename Rejector, typename Optimizer, bool kRobust>
 std::vector<RegistrationResult> run_pairs(const Options& o, const std::vector<PointCloud>& targets, const std::vector<PointCloud>& sources,
-                                          const std::vector<Isometry3d>& init) {
+                                          const std::vector<Isometry3d>& init, const std::vector<std::pair<size_t, size_t>>* pairs) {
   BatchRegistration<Factor, General, Rejector, Optimizer> reg;
   configure(reg, o);
   set_rejector(reg, o, std::is_same<Rejector, DistanceRejector>());
   set_general(reg, o, std::is_same<General, RestrictDoFFactor>());
   set_robust(reg.point_factor, o, std::integral_constant<bool, kRobust>());
-  if (o.tree == 1) return reg.align(targets, sources, init);  // TREE_DEVICE_KDTREE: a kd-tree per target
-  return reg.align(targets, sources, init, o.voxel_resolution, o.voxel_search_offsets);
+  if (o.tree == 1) return pairs ? reg.align(targets, sources, *pairs, init) : reg.align(targets, sources, init);  // TREE_DEVICE_KDTREE: a kd-tree per target
+  return pairs ? reg.align(targets, sources, *pairs, init, o.voxel_resolution, o.voxel_search_offsets)
+               : reg.align(targets, sources, init, o.voxel_resolution, o.voxel_search_offsets);
 }
 
 /// The registration types chosen by the options: job.call<Factor, GeneralFactor, Rejector, Optimizer, kRobust>().
@@ -139,10 +140,11 @@ struct BatchJob {
   const std::shared_ptr<PointCloud>& target;
   const std::vector<PointCloud>& sources;
   const std::vector<Isometry3d>& init;
+  const std::vector<size_t>* cloud_of_member;  // or null: one member per source
   std::vector<RegistrationResult> results;
   template <typename Factor, typename General, typename Rejector, typename Optimizer, bool kRobust>
   void call() {
-    results = run_batch<Factor, General, Rejector, Optimizer, kRobust>(o, target, sources, init);
+    results = run_batch<Factor, General, Rejector, Optimizer, kRobust>(o, target, sources, init, cloud_of_member);
   }
 };
 
@@ -151,13 +153,14 @@ struct PairsJob {
   const std::vector<PointCloud>& targets;
   const std::vector<PointCloud>& sources;
   const std::vector<Isometry3d>& init;
+  const std::vector<std::pair<size_t, size_t>>* pairs;  // or null: source m against target m
   std::vector<RegistrationResult> results;
   template <typename Factor, typename General, typename Rejector, typename Optimizer, bool kRobust>
   void call() {
     constexpr bool plane = std::is_same_v<Factor, PointToPlaneICPFactor> || std::is_same_v<Factor, RobustFactor<Huber, PointToPlaneICPFactor>> ||
                            std::is_same_v<Factor, RobustFactor<Cauchy, PointToPlaneICPFactor>>;
     if (plane && o.tree != 1) throw std::runtime_error("sgbh_align_batch_pairs: a voxel map has no normals (point-to-plane)");
-    results = run_pairs<Factor, General, Rejector, Optimizer, kRobust>(o, targets, sources, init);
+    results = run_pairs<Factor, General, Rejector, Optimizer, kRobust>(o, targets, sources, init, pairs);
   }
 };
 
@@ -266,22 +269,25 @@ int sgbh_align(size_t n_target, const double* target_pts4, const double* target_
   }
 }
 
-/// BatchRegistration<...>::align: the options of sgbh_align; n_members sources concatenated (member m = rows offsets[m] .. offsets[m+1]),
-/// one initial pose per member.  Outputs as sgbh_align's, member after member (16 / 4 / 36 / 6 doubles each).
-int sgbh_align_batch(size_t n_target, const double* target_pts4, const double* target_normals4, const double* target_covs16, size_t n_members,
+/// BatchRegistration<...>::align: the options of sgbh_align; n_sources sources concatenated (source m = rows offsets[m] .. offsets[m+1]).
+/// cloud_of_member NULL: one member per source (n_members = n_sources); else member p is source cloud_of_member[p] (the multi-start
+/// overload).  One initial pose per member.  Outputs as sgbh_align's, member after member (16 / 4 / 36 / 6 doubles each).
+int sgbh_align_batch(size_t n_target, const double* target_pts4, const double* target_normals4, const double* target_covs16, size_t n_sources,
                      const size_t* offsets, const double* source_pts4, const double* source_covs16, const double* options21, const double* init_T16xB,
-                     double* T_out16xB, double* scalars_out4xB, double* H_out36xB, double* b_out6xB) {
+                     double* T_out16xB, double* scalars_out4xB, double* H_out36xB, double* b_out6xB, size_t n_members, const size_t* cloud_of_member) {
   try {
     const Options o = parse_options(options21);
     auto target = make_cloud(n_target, target_pts4, target_normals4, target_covs16);
-    std::vector<PointCloud> sources(n_members);
-    std::vector<Isometry3d> init(n_members);
-    for (size_t m = 0; m < n_members; m++) {
+    std::vector<PointCloud> sources(n_sources);
+    for (size_t m = 0; m < n_sources; m++) {
       const size_t off = offsets[m], n = offsets[m + 1] - off;
       sources[m] = *make_cloud(n, source_pts4 + 4 * off, nullptr, source_covs16 ? source_covs16 + 16 * off : nullptr);
-      std::memcpy(init[m].matrix().data(), init_T16xB + 16 * m, sizeof(double) * 16);
     }
-    BatchJob job{o, target, sources, init, {}};
+    if (!cloud_of_member) n_members = n_sources;
+    const std::vector<size_t> members(cloud_of_member, cloud_of_member + (cloud_of_member ? n_members : 0));
+    std::vector<Isometry3d> init(n_members);
+    for (size_t m = 0; m < n_members; m++) std::memcpy(init[m].matrix().data(), init_T16xB + 16 * m, sizeof(double) * 16);
+    BatchJob job{o, target, sources, init, cloud_of_member ? &members : nullptr, {}};
     if (!dispatch(o, job)) {
       g_error = "sgbh_align_batch: invalid factor kind";
       return 1;
@@ -296,24 +302,33 @@ int sgbh_align_batch(size_t n_target, const double* target_pts4, const double* t
 }
 
 /// BatchRegistration<...>::align over (target, source) pairs: the options of sgbh_align (tree 1 = TREE_DEVICE_KDTREE: a kd-tree per
-/// target; otherwise a Gaussian voxel map per target with voxel_resolution and search offsets); target m = rows target_offsets[m] ..
-/// target_offsets[m+1] (with normals / covariances or none), source m likewise.  Outputs as sgbh_align_batch's.
+/// target; otherwise a Gaussian voxel map per target with voxel_resolution and search offsets); target t = rows target_offsets[t] ..
+/// target_offsets[t+1] (with normals / covariances or none), source s likewise.  pairs2 NULL: n_targets = n_sources = n_pairs, source m
+/// against target m; else pair p = (source pairs2[2p], target pairs2[2p+1]) (the pair-list overloads).  One initial pose per pair;
+/// outputs as sgbh_align_batch's.
 int sgbh_align_batch_pairs(size_t n_pairs, const size_t* target_offsets, const double* target_pts4, const double* target_normals4, const double* target_covs16,
                            const size_t* source_offsets,
                            const double* source_pts4, const double* source_covs16, const double* options21, const double* init_T16xB, double* T_out16xB,
-                           double* scalars_out4xB, double* H_out36xB, double* b_out6xB) {
+                           double* scalars_out4xB, double* H_out36xB, double* b_out6xB, size_t n_targets, size_t n_sources, const size_t* pairs2) {
   try {
     const Options o = parse_options(options21);
-    std::vector<PointCloud> targets(n_pairs), sources(n_pairs);
-    std::vector<Isometry3d> init(n_pairs);
-    for (size_t m = 0; m < n_pairs; m++) {
-      const size_t to = target_offsets[m], tn = target_offsets[m + 1] - to;
-      const size_t so = source_offsets[m], sn = source_offsets[m + 1] - so;
-      targets[m] = *make_cloud(tn, target_pts4 + 4 * to, target_normals4 ? target_normals4 + 4 * to : nullptr, target_covs16 ? target_covs16 + 16 * to : nullptr);
-      sources[m] = *make_cloud(sn, source_pts4 + 4 * so, nullptr, source_covs16 ? source_covs16 + 16 * so : nullptr);
-      std::memcpy(init[m].matrix().data(), init_T16xB + 16 * m, sizeof(double) * 16);
+    if (!pairs2) n_targets = n_sources = n_pairs;
+    std::vector<PointCloud> targets(n_targets), sources(n_sources);
+    for (size_t t = 0; t < n_targets; t++) {
+      const size_t to = target_offsets[t], tn = target_offsets[t + 1] - to;
+      targets[t] = *make_cloud(tn, target_pts4 + 4 * to, target_normals4 ? target_normals4 + 4 * to : nullptr, target_covs16 ? target_covs16 + 16 * to : nullptr);
     }
-    PairsJob job{o, targets, sources, init, {}};
+    for (size_t m = 0; m < n_sources; m++) {
+      const size_t so = source_offsets[m], sn = source_offsets[m + 1] - so;
+      sources[m] = *make_cloud(sn, source_pts4 + 4 * so, nullptr, source_covs16 ? source_covs16 + 16 * so : nullptr);
+    }
+    std::vector<Isometry3d> init(n_pairs);
+    std::vector<std::pair<size_t, size_t>> pairs(pairs2 ? n_pairs : 0);
+    for (size_t p = 0; p < n_pairs; p++) {
+      std::memcpy(init[p].matrix().data(), init_T16xB + 16 * p, sizeof(double) * 16);
+      if (pairs2) pairs[p] = {pairs2[2 * p], pairs2[2 * p + 1]};
+    }
+    PairsJob job{o, targets, sources, init, pairs2 ? &pairs : nullptr, {}};
     if (!dispatch(o, job)) {
       g_error = "sgbh_align_batch_pairs: invalid factor kind";
       return 1;

@@ -119,14 +119,17 @@ def align_batch(
     voxel_search_offsets=1,
     dof_mask=None,
     device=0,
+    cloud_of_member=None,
 ):
     """BatchRegistration<Factor, GeneralFactor, Rejector, Optimizer>::align (C++ host mirror): every source (a list of (N_m, 3|4) arrays)
     from its initial pose (init_Ts: (B, 4, 4), default identity); source_covs: None or a list of (N_m, 4, 4).  Keyword arguments as align().
-    Returns capi.BatchAlignResult (per-member arrays)."""
+    cloud_of_member (or None: one member per source): member p is source cloud_of_member[p], each source uploaded once (multi-start;
+    one initial pose per member).  Returns capi.BatchAlignResult (per-member arrays)."""
     L = _lib()
     if not hasattr(L.sgbh_align_batch, "_typed"):
         L.sgbh_align_batch.restype = C.c_int
-        L.sgbh_align_batch.argtypes = [C.c_size_t, _dp, _dp, _dp, C.c_size_t, C.POINTER(C.c_size_t), _dp, _dp, _dp, _dp, _dp, _dp, _dp, _dp]
+        L.sgbh_align_batch.argtypes = [C.c_size_t, _dp, _dp, _dp, C.c_size_t, C.POINTER(C.c_size_t), _dp, _dp, _dp, _dp, _dp, _dp, _dp, _dp, C.c_size_t,
+                                       C.POINTER(C.c_size_t)]
         L.sgbh_align_batch._typed = True
     tp = capi._points4(target_points)
     tn, tc = _f64(target_normals), _f64(target_covs)
@@ -140,11 +143,15 @@ def align_batch(
     opts[:13] = [factor, robust, robust_c, rejector, max_dist_sq, optimizer, max_iterations, rotation_eps, translation_eps, tree, voxel_resolution, voxel_search_offsets, 0 if dof_mask is None else 1]
     opts[13:19] = 1.0 if dof_mask is None else np.asarray(dof_mask, dtype=float)
     opts[19] = device
+    n_sources = B
+    com = None if cloud_of_member is None else np.ascontiguousarray(cloud_of_member, dtype=np.uintp).reshape(-1)
+    if com is not None:
+        B = com.size
     Ts = np.tile(np.eye(4), (B, 1, 1)) if init_Ts is None else np.asarray(init_Ts, dtype=float).reshape(B, 4, 4)
     T0 = np.ascontiguousarray(Ts.transpose(0, 2, 1))
     T, sc4, H, b = np.zeros((max(B, 1), 16)), np.zeros((max(B, 1), 4)), np.zeros((max(B, 1), 36)), np.zeros((max(B, 1), 6))
-    rc = L.sgbh_align_batch(tp.shape[0], _d(tp), _d(tn), _d(tc), B, offsets.ctypes.data_as(C.POINTER(C.c_size_t)), _d(sp), _d(sc), _d(opts), _d(T0), _d(T), _d(sc4),
-                            _d(H), _d(b))
+    rc = L.sgbh_align_batch(tp.shape[0], _d(tp), _d(tn), _d(tc), n_sources, offsets.ctypes.data_as(C.POINTER(C.c_size_t)), _d(sp), _d(sc), _d(opts), _d(T0), _d(T),
+                            _d(sc4), _d(H), _d(b), B, None if com is None else com.ctypes.data_as(C.POINTER(C.c_size_t)))
     if rc != 0:
         raise capi.SgbError(L.sgbh_last_error().decode())
     return capi.BatchAlignResult(T[:B], sc4[:B], np.concatenate([H, b], axis=1)[:B])
@@ -171,33 +178,38 @@ def align_batch_pairs(
     device=0,
     tree=TREE_VOXELMAP,
     target_normals=None,
+    pairs=None,
 ):
     """BatchRegistration<...>::align(targets, sources, init_Ts, voxel_resolution, search_offsets) (C++ host mirror): source m against a
     Gaussian voxel map of targets[m], every pair in one batched call; with tree=TREE_DEVICE_KDTREE BatchRegistration<...>::align(targets,
     sources, init_Ts): source m against a kd-tree of targets[m].  targets / sources: lists of (N_m, 3|4) arrays; target_covs / source_covs:
-    None or lists of (N_m, 4, 4); target_normals: None or a list of (N_m, 4) (point-to-plane, kd-trees only).  Keyword arguments as
-    align_batch().  Returns capi.BatchAlignResult."""
+    None or lists of (N_m, 4, 4); target_normals: None or a list of (N_m, 4) (point-to-plane, kd-trees only).  pairs (or None: source m
+    against target m): a (P, 2) list of (source index, target index), the pair-list overloads -- each target built once, each source
+    uploaded once, one initial pose per pair.  Keyword arguments as align_batch().  Returns capi.BatchAlignResult."""
     L = _lib()
     if tree not in (TREE_VOXELMAP, TREE_DEVICE_KDTREE):
         raise capi.SgbError("align_batch_pairs: tree must be TREE_VOXELMAP or TREE_DEVICE_KDTREE")
     if not hasattr(L.sgbh_align_batch_pairs, "_typed"):
         L.sgbh_align_batch_pairs.restype = C.c_int
-        L.sgbh_align_batch_pairs.argtypes = [C.c_size_t, C.POINTER(C.c_size_t), _dp, _dp, _dp, C.POINTER(C.c_size_t), _dp, _dp, _dp, _dp, _dp, _dp, _dp, _dp]
+        L.sgbh_align_batch_pairs.argtypes = [C.c_size_t, C.POINTER(C.c_size_t), _dp, _dp, _dp, C.POINTER(C.c_size_t), _dp, _dp, _dp, _dp, _dp, _dp, _dp, _dp,
+                                             C.c_size_t, C.c_size_t, C.POINTER(C.c_size_t)]
         L.sgbh_align_batch_pairs._typed = True
-    assert len(targets) == len(sources), "one target per source"
-    B = len(sources)
+    pl = None if pairs is None else np.ascontiguousarray(pairs, dtype=np.uintp).reshape(-1, 2)
+    if pl is None:
+        assert len(targets) == len(sources), "one target per source"
+    B = len(sources) if pl is None else pl.shape[0]
 
     def concat(clouds, covs):
         members = [capi._points4(c) for c in clouds]
-        offsets = np.zeros(B + 1, dtype=np.uintp)
+        offsets = np.zeros(len(members) + 1, dtype=np.uintp)
         offsets[1:] = np.cumsum([m.shape[0] for m in members])
-        p = np.ascontiguousarray(np.concatenate(members) if B else np.zeros((0, 4)))
-        c = None if covs is None else np.ascontiguousarray(np.concatenate([_f64(x) for x in covs]) if B else np.zeros((0, 4, 4)))
+        p = np.ascontiguousarray(np.concatenate(members) if members else np.zeros((0, 4)))
+        c = None if covs is None else np.ascontiguousarray(np.concatenate([_f64(x) for x in covs]) if members else np.zeros((0, 4, 4)))
         return offsets, p, c
 
     to, tp, tc = concat(targets, target_covs)
     so, sp, sc = concat(sources, source_covs)
-    tn = None if target_normals is None else np.ascontiguousarray(np.concatenate([_f64(x) for x in target_normals]) if B else np.zeros((0, 4)))
+    tn = None if target_normals is None else np.ascontiguousarray(np.concatenate([_f64(x) for x in target_normals]) if len(targets) else np.zeros((0, 4)))
     if tn is not None:
         assert tn.shape == (tp.shape[0], 4)
     opts = np.zeros(21)
@@ -209,7 +221,8 @@ def align_batch_pairs(
     T0 = np.ascontiguousarray(Ts.transpose(0, 2, 1))
     T, sc4, H, b = np.zeros((max(B, 1), 16)), np.zeros((max(B, 1), 4)), np.zeros((max(B, 1), 36)), np.zeros((max(B, 1), 6))
     rc = L.sgbh_align_batch_pairs(B, to.ctypes.data_as(C.POINTER(C.c_size_t)), _d(tp), _d(tn), _d(tc), so.ctypes.data_as(C.POINTER(C.c_size_t)), _d(sp), _d(sc),
-                                  _d(opts), _d(T0), _d(T), _d(sc4), _d(H), _d(b))
+                                  _d(opts), _d(T0), _d(T), _d(sc4), _d(H), _d(b), len(targets), len(sources),
+                                  None if pl is None else pl.ctypes.data_as(C.POINTER(C.c_size_t)))
     if rc != 0:
         raise capi.SgbError(L.sgbh_last_error().decode())
     return capi.BatchAlignResult(T[:B], sc4[:B], np.concatenate([H, b], axis=1)[:B])
