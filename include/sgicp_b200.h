@@ -200,7 +200,7 @@ int sgb_num_inliers(sgb_ctx* ctx, size_t* n);
  * (sgb_linearize, sgb_error, their _device variants, sgb_correspondences, sgb_num_inliers) and sgb_target_batch_knn,
  * sgb_target_estimate_features, sgb_target_set_kdtree / _build_kdtree fail with a message.  Pair one source with many maps, many
  * sources with one map, or a cloud with several initial poses through sgb_source_set_pairs below: each cloud is stored once and
- * each map built once.
+ * each map built once.  A source against the union of several posed kd-tree maps: sgb_source_set_submaps.
  * Many kd-trees: after sgb_target_build_kdtrees, member m is paired with map m in the same way, for ICP, point-to-plane (the maps need
  * normals) and GICP (covariances).  A linearize round is 3 launches (search, factor, per-member sums) and an error round 2, whatever the
  * member count.  The calls fail with a message while the member count differs from the map count.  Each member's results are
@@ -227,6 +227,30 @@ int sgb_source_set_batch(sgb_ctx* ctx, size_t n_members, const size_t* offsets, 
  * maps table the member count must equal the map count, as without pairs).  n_members <= SGB_BATCH_MAX_MEMBERS, fewer than 2^31 member
  * points in all, every clouds[p] below the cloud count, a batch set, else the call fails with a message; n_members = 0: an empty batch. */
 int sgb_source_set_pairs(sgb_ctx* ctx, size_t n_members, const uint32_t* clouds /*or NULL*/, const uint32_t* maps /*or NULL*/);
+/* Submaps: the batch's members become n_members (cloud, submap) pairs.  Member p = stored cloud clouds[p] (NULL: cloud p) against the UNION
+ * of its entries j = list_off[p] .. list_off[p+1] - 1 (list_off: n_members + 1 ascending, list_off[0] = 0): entry j = map entry_maps[j] of a
+ * many-kd-trees target (sgb_target_build_kdtrees), placed by the rigid pose entry_poses16[16 j ..] (map -> common frame, column-major
+ * 4x4; NULL = all identity).  A scan against a local map of several keyframes each at its own pose, or against the few tiles of a tiled
+ * map around it, without building or storing a tree of the union: every map is built once, whatever lists name it and however often the
+ * poses change.  Nothing of a map is transformed.  Rigid motions preserve distances, so the nearest neighbour in the placed union is the
+ * nearest over the entries of the nearest in each map's own frame at the member's pose carried into that frame (P_j^-1 T), and the ICP and
+ * GICP terms r^T (C_t + R C_s R^T)^-1 r with their derivatives by the right perturbation of T are the same in either frame: each point
+ * is linearised against its correspondence's map as stored.  Point-to-plane is not (the reference's residual is the element-wise n o r):
+ * SGB_FACTOR_PLANE_ICP fails with a message.  The poses, init_T16xB and out_T16xB of the batched calls are source -> common frame.
+ * It is a pairing like sgb_source_set_pairs: index arrays and poses in host memory, one copy of the lists and 1 launch whatever the
+ * counts, plus 1 at the first batched call after it or after the target changed; the per-member state starts afresh; calling it again
+ * re-pairs or changes the poses: no map is rebuilt and no cloud uploaded, but the call is a full pairing even if only poses changed
+ * (the replicas are gathered again, 1 launch over all member points, and every member's cached correspondences and seeds are dropped);
+ * sgb_source_set_batch, sgb_source_set_pairs or sgb_source_set_points forgets it.
+ * A linearize round stays 3 launches and an error round 2.  The same map may appear in many lists and, at different poses, several times
+ * in one; an empty list gives the member no correspondences and zero sums.  At an exact FP32 distance tie between two entries the earlier
+ * entry wins (a search seed aside, as in one tree); a member's results depend on its own points, pose, list and seeds only.
+ * sgb_correspondences_batch reports (entry index within the member's list) << 32 | original index within that entry's map.  Every batched
+ * call checks the lists against the current target: a target that is not many kd-trees (voxel maps included), or an entry_maps[j] beyond
+ * its map count, fails with a message.  Limits of sgb_source_set_pairs, fewer than 2^31 entries in all, and every pose rigid (rotation
+ * block orthonormal to 1e-6, determinant > 0, last row 0 0 0 1), else the call fails with a message. */
+int sgb_source_set_submaps(sgb_ctx* ctx, size_t n_members, const uint32_t* clouds /*or NULL*/, const size_t* list_off, const uint32_t* entry_maps,
+                           const double* entry_poses16 /*or NULL*/);
 /* One linearize per member at its pose T_colmajor16xB[16 m ..]: out44xB[44 m ..] = H(36) | b(6) | e | num_inliers.  active (or NULL =
  * all): an inactive member costs no search or factor work, gets zeros and keeps its cached correspondences and linearisation pose.
  * out44xB may be host or device memory; the call returns when the results are there. */

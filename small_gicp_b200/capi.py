@@ -76,6 +76,7 @@ _SIGNATURES = {
     "sgb_num_inliers": (C.c_int, [_vp, C.POINTER(C.c_size_t)]),
     "sgb_source_set_batch": (C.c_int, [_vp, C.c_size_t, C.POINTER(C.c_size_t), _dp, _dp]),
     "sgb_source_set_pairs": (C.c_int, [_vp, C.c_size_t, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32)]),
+    "sgb_source_set_submaps": (C.c_int, [_vp, C.c_size_t, C.POINTER(C.c_uint32), C.POINTER(C.c_size_t), C.POINTER(C.c_uint32), _dp]),
     "sgb_linearize_batch": (C.c_int, [_vp, C.c_int, C.c_int, C.c_double, C.c_int, C.c_double, _dp, C.POINTER(C.c_uint8), _dp]),
     "sgb_error_batch": (C.c_int, [_vp, _dp, C.POINTER(C.c_uint8), _dp]),
     "sgb_correspondences_batch": (C.c_int, [_vp, _u64p]),
@@ -391,6 +392,31 @@ class Context:
             raise SgbError(f"set_source_pairs: {cl.size} clouds but {mp.size} maps")
         u32p = C.POINTER(C.c_uint32)
         self._check(self._L.sgb_source_set_pairs(self._h, P, None if cl is None else cl.ctypes.data_as(u32p), None if mp is None else mp.ctypes.data_as(u32p)))
+        sizes = np.diff(self._cloud_offsets)
+        self._batch_offsets = np.concatenate([[0], np.cumsum(sizes[cl] if cl is not None else sizes)]).astype(np.int64)
+
+    def set_source_submaps(self, lists, poses=None, clouds=None):
+        """the batch's members become (cloud, submap) pairs: member p is cloud clouds[p] (None: cloud p) aligned against the union of the
+        maps lists[p] (map indices of a many-kd-trees target), map lists[p][j] placed by the rigid 4x4 pose poses[p][j] (map -> common
+        frame; poses None: all identity).  Each map stays as built; ICP and GICP.  The batched calls then take and return one pose per
+        member, source -> common frame, and correspondences_batch reports (entry within the list) << 32 | index within that map."""
+        lists = [np.asarray(l, dtype=np.uint32).reshape(-1) for l in lists]
+        P = len(lists)
+        off = np.zeros(P + 1, dtype=np.uintp)
+        off[1:] = np.cumsum([l.size for l in lists])
+        maps = np.ascontiguousarray(np.concatenate(lists) if P else np.zeros(0), dtype=np.uint32)
+        pc = None
+        if poses is not None:
+            if len(poses) != P or any(len(poses[p]) != lists[p].size for p in range(P)):
+                raise SgbError("set_source_submaps: one pose per list entry")
+            flat = [np.asarray(T, dtype=np.float64).reshape(4, 4).T for p in range(P) for T in poses[p]]  # column-major
+            pc = np.ascontiguousarray(np.array(flat).reshape(-1, 16)) if flat else np.zeros((1, 16))
+        cl = None if clouds is None else np.ascontiguousarray(clouds, dtype=np.uint32).reshape(-1)
+        if cl is not None and cl.size != P:
+            raise SgbError(f"set_source_submaps: {cl.size} clouds but {P} lists")
+        u32p = C.POINTER(C.c_uint32)
+        self._check(self._L.sgb_source_set_submaps(self._h, P, None if cl is None else cl.ctypes.data_as(u32p), off.ctypes.data_as(C.POINTER(C.c_size_t)),
+                                                   maps.ctypes.data_as(u32p), _d(pc)))
         sizes = np.diff(self._cloud_offsets)
         self._batch_offsets = np.concatenate([[0], np.cumsum(sizes[cl] if cl is not None else sizes)]).astype(np.int64)
 

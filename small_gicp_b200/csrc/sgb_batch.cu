@@ -12,6 +12,9 @@
 //                           round, its next pose and phase
 //   pair_gather_kernel      sgb_source_set_pairs: every member's replica of its stored cloud, in one launch over all member points
 //   pair_view_kernel        the many-maps tables above seen through the pairing (member p -> map maps[p]), one CTA
+//   batch_submap_factor_kernel  batch_trees_factor_kernel for submap members (sgb_source_set_submaps): each point at the member's pose
+//                           relative to the placement of the entry its correspondence lies in, against that entry's map as stored
+//   submap_view_kernel      the per-entry tables of the submap lists from the target's per-map tables, one thread per entry
 // A member's sums depend on its own points, pose and correspondences only, added in an order fixed by its size: bit-identical whatever
 // else is in the batch.
 #include <algorithm>
@@ -81,9 +84,12 @@ __global__ void __launch_bounds__(kLinBlock) batch_transform_kernel(const __grid
 // One tile of batch_factor_kernel.  ERR = false: linearize (VOX: voxel-map probe here; else vcorr = what the search found); ERR = true:
 // error() with the cached corr[].  MAPS: a multi-map voxel target -- member m is centred on map m's centre (map_centres[4 m ..]) and
 // probes map m's region of the table (map_regions[m]: first slot, mask); otherwise the target's one centre and table.
-template <int FACTOR, int ROBUST, bool VOX, bool ERR, bool MAPS>
+// SUB: submap members (S, sgb_source_set_submaps) -- the correspondence lies in entry S->centry[i] of the member's list, and the point is
+// linearised at the member's pose relative to that entry's placement against the entry's map as stored.  r^T M r and its derivatives by
+// the right perturbation of the pose are invariant under the placement, so this IS the point's share of the sums against the union.
+template <int FACTOR, int ROBUST, bool VOX, bool ERR, bool MAPS, bool SUB = false>
 __device__ __forceinline__ void batch_factor_tile(const BatchParams& B, const uint32_t* __restrict__ vcorr, const double* __restrict__ map_centres,
-                                                  const uint4* __restrict__ map_regions) {
+                                                  const uint4* __restrict__ map_regions, const SubmapView* S = nullptr) {
   constexpr int NACC = ERR ? 1 : kAcc + 1;
   double acc[NACC];
 #pragma unroll
@@ -101,7 +107,26 @@ __device__ __forceinline__ void batch_factor_tile(const BatchParams& B, const ui
     const float4 sp = __ldg(&B.pts[i]);
     const float4 z = make_float4(0.f, 0.f, 0.f, 0.f);
     const float4 sA = FACTOR == 2 ? __ldg(&B.covA[i]) : z, sB = FACTOR == 2 ? __ldg(&B.covB[i]) : z;
-    if (ERR) {
+    if (SUB) {
+      uint32_t k = ERR ? B.corr[i] : vcorr[t.vfirst + tid];
+      if (k != kNone) {
+        const size_t e = __ldg(&S->entry_off[t.member]) + S->centry[i];
+        const double* Pinv = S->inv_poses + 12 * e;
+        double Rk[12];
+        relative_pose(Pinv, R, Rk);
+        const double3 tk = centred_translation(Rk, csx, csy, csz, S->centres + 4 * e);
+        const float4 tq = __ldg(&B.tgt.pts[k]);
+        const float4 t1 = FACTOR == 2 ? __ldg(&B.tgt.covA[k]) : z, t2 = FACTOR == 2 ? __ldg(&B.tgt.covB[k]) : z;
+        if (ERR) {
+          double Rlin[12];  // the member's linearisation pose through the same placement
+          relative_pose(Pinv, B.lin_poses + 12 * static_cast<size_t>(t.member), Rlin);
+          acc[0] += point_error<FACTOR, ROBUST>(Rk, tk.x, tk.y, tk.z, Rlin, B.robust_c, sp, sA, sB, tq, t1, t2);
+        } else if (!point_linearize_source<FACTOR, ROBUST>(Rk, tk.x, tk.y, tk.z, csx, csy, csz, B.max_dist_sq_d, B.robust_c, sp, &sA, &sB, tq, &t1, &t2, acc)) {
+          k = kNone;  // rejected: error() and the correspondences must not see it
+        }
+      }
+      if (!ERR) B.corr[i] = k;
+    } else if (ERR) {
       const uint32_t k = B.corr[i];
       if (k != kNone) {
         const float4 tq = __ldg(&B.tgt.pts[k]);
@@ -172,6 +197,13 @@ template <int FACTOR, int ROBUST, bool ERR>
 __global__ void __launch_bounds__(kLinBlock, 4) batch_trees_factor_kernel(const __grid_constant__ BatchParams B, const uint32_t* __restrict__ vcorr,
                                                                          const double* __restrict__ map_centres) {
   batch_factor_tile<FACTOR, ROBUST, false, ERR, true>(B, vcorr, map_centres, nullptr);
+}
+
+// Submap members (sgb_source_set_submaps) on many kd-trees: vcorr and S.centry = what submap_search_kernel found over the member's entries.
+template <int FACTOR, int ROBUST, bool ERR>
+__global__ void __launch_bounds__(kLinBlock, 4) batch_submap_factor_kernel(const __grid_constant__ BatchParams B, const uint32_t* __restrict__ vcorr,
+                                                                          const __grid_constant__ SubmapView S) {
+  batch_factor_tile<FACTOR, ROBUST, false, ERR, false, true>(B, vcorr, nullptr, nullptr, &S);  // MAPS = false: no per-member centre table is read
 }
 
 // One CTA per member: warp w adds tiles w, w + 8, ... of the member in order, then the 8 warp sums are added in warp order.  The order
@@ -307,6 +339,24 @@ __global__ void __launch_bounds__(kViewBlock) pair_view_kernel(const PairView v)
   if (v.map_pt_off && threadIdx.x == 0) v.pt_off[v.n_members] = carry;
 }
 
+// Submap entries seen through the target's per-map tables: entry j -> map entry_maps[j], one thread per entry.
+__global__ void submap_view_kernel(const SubmapViewBuild v) {
+  for (uint32_t j = blockIdx.x * blockDim.x + threadIdx.x; j < v.n_entries; j += gridDim.x * blockDim.x) {
+    const uint32_t q = v.entry_maps[j], first = v.map_pt_off[q];
+    v.entries[j] = make_uint4(first, v.map_pt_off[q + 1] - first, v.map_node_base[q], q);
+    for (int d = 0; d < 4; d++) v.centres[4 * static_cast<size_t>(j) + d] = v.map_centres[4 * static_cast<size_t>(q) + d];
+  }
+}
+
+// correspondences of a submap member in the caller's order: out[perm[i]] = (entry << 32) | original index within the entry's map
+__global__ void submap_correspondences_kernel(const uint32_t* __restrict__ corr, const uint32_t* __restrict__ centry, const uint32_t* __restrict__ perm, size_t n,
+                                              const float4* __restrict__ tgt_pts, uint64_t* out) {
+  for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < n; i += static_cast<size_t>(gridDim.x) * blockDim.x) {
+    const uint32_t k = corr[i];
+    out[perm[i]] = k == kNone ? ~0ull : (static_cast<uint64_t>(centry[i]) << 32) | static_cast<uint32_t>(__float_as_int(tgt_pts[k].w));
+  }
+}
+
 cudaError_t launch_pair_gather(const PairGather& g, int sm_count, cudaStream_t st) {
   const uint64_t total = g.n + 10ull * g.n_members;
   if (total == 0) return cudaSuccess;
@@ -360,6 +410,33 @@ cudaError_t launch_batch_trees_factor(const BatchParams& B, int factor, int robu
       batch_trees_factor_kernel<f, r, false><<<n_tiles, kLinBlock, 0, st>>>(B, vcorr, map_centres);
     return cudaGetLastError();
   });
+}
+
+cudaError_t launch_batch_submap_factor(const BatchParams& B, int factor, int robust, uint32_t n_tiles, bool err, const uint32_t* vcorr, const SubmapView& S,
+                                       cudaStream_t st) {
+  if (factor == 1) return cudaErrorInvalidValue;  // n o r is not invariant under a placement: no point-to-plane against a union
+  return dispatch_factor_robust(factor, robust, cudaErrorInvalidValue, [&](auto f, auto r) {
+    if (err)
+      batch_submap_factor_kernel<(f == 1 ? 0 : f), r, true><<<n_tiles, kLinBlock, 0, st>>>(B, vcorr, S);
+    else
+      batch_submap_factor_kernel<(f == 1 ? 0 : f), r, false><<<n_tiles, kLinBlock, 0, st>>>(B, vcorr, S);
+    return cudaGetLastError();
+  });
+}
+
+cudaError_t launch_submap_view(const SubmapViewBuild& v, int sm_count, cudaStream_t st) {
+  if (v.n_entries == 0) return cudaSuccess;
+  const uint32_t grid = std::min<uint32_t>((v.n_entries + 255u) / 256u, static_cast<uint32_t>(sm_count) * 8u);
+  submap_view_kernel<<<grid, 256, 0, st>>>(v);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_submap_correspondences(const uint32_t* corr, const uint32_t* centry, const uint32_t* perm, size_t n, const float4* tgt_pts, uint64_t* out,
+                                          int sm_count, cudaStream_t st) {
+  if (!n) return cudaSuccess;
+  const size_t grid = std::min<size_t>((n + 255u) / 256u, static_cast<size_t>(sm_count) * 8u);
+  submap_correspondences_kernel<<<static_cast<unsigned>(grid), 256, 0, st>>>(corr, centry, perm, n, tgt_pts, out);
+  return cudaGetLastError();
 }
 
 cudaError_t launch_batch_segment(const BatchParams& B, uint32_t n_members, bool linearize, double* out, cudaStream_t st) {

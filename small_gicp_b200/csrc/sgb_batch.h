@@ -68,6 +68,33 @@ struct PairView {
   uint4* regions;
 };
 cudaError_t launch_pair_view(const PairView& v, cudaStream_t st);
+/// Submap members (sgb_source_set_submaps): member p is aligned against the union of its entries entry_off[p] .. entry_off[p + 1] - 1,
+/// entry j = one map of a many-kd-trees target placed by a rigid pose.  Nothing of a map is transformed: the member's pose is carried
+/// into each map's stored frame (relative_pose) instead.
+struct SubmapView {
+  const uint32_t* entry_off;  // [members + 1]
+  const uint4* entries;       // per entry: first point of its map in tgt_pts, point count, first packet record, map
+  const double* centres;      // [entries][4] the map's centre
+  const double* inv_poses;    // [entries][12] inverse of the entry's placement, row-major R^T | -R^T t
+  uint32_t* centry;           // per stored member point, beside BatchParams::corr: the entry (within the member's list) its correspondence lies in
+};
+/// The per-entry tables above from the target's per-map tables, one launch: entry j -> map entry_maps[j].
+struct SubmapViewBuild {
+  uint32_t n_entries;
+  const uint32_t* entry_maps;
+  const uint32_t *map_pt_off, *map_node_base;
+  const double* map_centres;
+  uint4* entries;
+  double* centres;
+};
+cudaError_t launch_submap_view(const SubmapViewBuild& v, int sm_count, cudaStream_t st);
+/// launch_batch_trees_factor for submap members: each point's correspondence is linearised (err = false; vcorr = what the submap search
+/// found) or re-evaluated (err = true) at the member's pose relative to the entry S.centry names.  ICP or GICP.
+cudaError_t launch_batch_submap_factor(const BatchParams& B, int factor, int robust, uint32_t n_tiles, bool err, const uint32_t* vcorr, const SubmapView& S,
+                                       cudaStream_t st);
+/// launch_correspondences for one submap member: out[perm[i]] = (entry << 32) | original index within the entry's map
+cudaError_t launch_submap_correspondences(const uint32_t* corr, const uint32_t* centry, const uint32_t* perm, size_t n, const float4* tgt_pts, uint64_t* out,
+                                          int sm_count, cudaStream_t st);
 /// out: [members][44] (linearize) or [members] (error)
 cudaError_t launch_batch_segment(const BatchParams& B, uint32_t n_members, bool linearize, double* out, cudaStream_t st);
 /// batched align(): every member whose phase matches the round (linearize: kPhaseLinearize, else kPhaseTrial) takes its optimiser step

@@ -193,14 +193,14 @@ void sgb::begin_source(sgb_ctx* ctx, SourceState state, size_t n, bool covs) {
   ctx->n_src = n;
   ctx->src_has_covs = covs;
   ctx->src_has_lo = ctx->src_tree_valid = ctx->src_cov_orig_valid = false;
-  ctx->b_paired = ctx->b_pair_has_maps = false;
+  ctx->b_paired = ctx->b_pair_has_maps = ctx->b_submaps = false;
   ctx->b_pair_maps.clear();
   forget_linearisation(ctx);
 }
 
 void sgb::begin_pairs(sgb_ctx* ctx) {
   ctx->b_paired = true;
-  ctx->b_pair_has_maps = false;
+  ctx->b_pair_has_maps = ctx->b_submaps = false;
   ctx->b_pair_maps.clear();
   forget_linearisation(ctx);
 }

@@ -1,11 +1,12 @@
 // SPDX-License-Identifier: MIT
-// C-ABI of batched registration (include/sgicp_b200.h: sgb_source_set_batch, sgb_source_set_pairs,
+// C-ABI of batched registration (include/sgicp_b200.h: sgb_source_set_batch, sgb_source_set_pairs, sgb_source_set_submaps,
 // sgb_{linearize,error,align,correspondences}_batch).
-// Kernels in sgb_batch.cu; DESIGN.md §11.
+// Kernels in sgb_batch.cu (many kd-trees and submaps: the searches in sgb_forest.cu); DESIGN.md §11.
 #include <cuda_runtime.h>
 
 #include <algorithm>
 #include <cfloat>
+#include <cmath>
 #include <cstring>
 #include <string>
 #include <vector>
@@ -34,6 +35,20 @@ int batch_check(sgb_ctx* ctx, const char* who, const double* T) {
   if (ctx->src_state != SourceState::Batch) return fail(ctx, 1, std::string(who) + ": the context holds no batch of sources (call sgb_source_set_batch)");
   if (ctx->comm_world > 1) return fail(ctx, 1, std::string(who) + ": batched calls are single-GPU only (call sgb_comm_disconnect first)");
   if (!T) return fail(ctx, 1, std::string(who) + ": null poses");
+  if (ctx->b_submaps) {
+    // as for a pairing's maps: the target may have been replaced since, so the lists are checked at every call
+    if (ctx->tgt_state != TargetState::KdTrees)
+      return fail(ctx, 1, std::string(who) + ": the members are aligned against submaps (sgb_source_set_submaps), which are lists of maps of a many-kd-trees target "
+                              "(sgb_target_build_kdtrees); the current target is not one (submaps over voxel maps are not supported)");
+    if (ctx->b_pair_max_map >= ctx->kt_maps) {
+      for (size_t p = 0; p + 1 < ctx->b_sub_off.size(); p++)
+        for (uint32_t j = ctx->b_sub_off[p]; j < ctx->b_sub_off[p + 1]; j++)
+          if (ctx->b_sub_maps[j] >= ctx->kt_maps)
+            return fail(ctx, 1, std::string(who) + ": entry " + std::to_string(j - ctx->b_sub_off[p]) + " of member " + std::to_string(p) + " names map " +
+                                    std::to_string(ctx->b_sub_maps[j]) + " but the target holds " + std::to_string(ctx->kt_maps) + " maps");
+    }
+    return 0;
+  }
   if (ctx->b_pair_has_maps) {
     // the target may have been replaced since the pairing: its maps are checked at every call
     if (!many_maps(ctx))
@@ -56,12 +71,37 @@ int batch_check(sgb_ctx* ctx, const char* who, const double* T) {
   return 0;
 }
 
+// n o r, the reference's point-to-plane residual, changes with the frame it is evaluated in, so it has no meaning against maps that
+// each sit in a frame of their own
+int submap_factor_check(sgb_ctx* ctx, const char* who, int factor) {
+  if (!ctx->b_submaps || factor != SGB_FACTOR_PLANE_ICP) return 0;
+  return fail(ctx, 1, std::string(who) + ": SGB_FACTOR_PLANE_ICP is not available against submaps (sgb_source_set_submaps): its residual is the element-wise "
+                          "product of the normal and the point difference, which is not invariant under the poses that place the maps; use ICP or GICP");
+}
+
+// the layout of s_tables, the one upload of sgb_source_set_submaps: inverse entry poses [entries][12] | entry_off [members + 1] | entry_maps [entries]
+struct SubmapTables {
+  const double* inv_poses;
+  const uint32_t *entry_off, *entry_maps;
+};
+SubmapTables submap_tables(const sgb_ctx* ctx) {
+  const size_t E = ctx->b_sub_maps.size();
+  const double* poses = ctx->s_tables.as<double>();
+  const uint32_t* off = reinterpret_cast<const uint32_t*>(poses + 12 * E);
+  return SubmapTables{poses, off, off + ctx->b_sub_off.size()};
+}
+SubmapView submap_view(const sgb_ctx* ctx) {
+  const SubmapTables t = submap_tables(ctx);
+  return SubmapView{t.entry_off, ctx->s_entries.as<uint4>(), ctx->s_centres.as<double>(), t.inv_poses, ctx->b_centry.as<uint32_t>()};
+}
+
 bool voxel_target(const sgb_ctx* ctx) { return ctx->tgt_state == TargetState::VoxelMap || ctx->tgt_state == TargetState::VoxelMaps; }
 
 // the factor kernel of one round over the target's kind: one voxel map or a point target (launch_batch_factor), or many maps / trees
 // (with a pairing's map table: the member-indexed view of the maps instead of the map-indexed tables)
 cudaError_t launch_factor(sgb_ctx* ctx, const BatchParams& Bp, int factor, int robust, uint32_t n_tiles, bool err, const uint32_t* vcorr) {
   const bool view = paired_maps(ctx);
+  if (ctx->b_submaps) return launch_batch_submap_factor(Bp, factor, robust, n_tiles, err, vcorr, submap_view(ctx), ctx->stream);
   if (ctx->tgt_state == TargetState::VoxelMaps)
     return launch_batch_maps_factor(Bp, factor, robust, n_tiles, err, (view ? ctx->v_centres : ctx->vm_centres).as<double>(),
                                     (view ? ctx->v_regions : ctx->vm_regions).as<uint4>(), ctx->stream);
@@ -73,6 +113,22 @@ cudaError_t launch_factor(sgb_ctx* ctx, const BatchParams& Bp, int factor, int r
 // Builds the pairing's view of the current target (one launch) unless it is up to date: forget_linearisation, which every target
 // transition and every pairing goes through, marks it stale.
 int pair_view(sgb_ctx* ctx) {
+  if (ctx->b_submaps && !ctx->b_view_ok) {  // batch_check has passed: the target is many kd-trees and holds every listed map
+    CU(cudaSetDevice(ctx->device));
+    const uint32_t* tab = ctx->kt_tables.as<uint32_t>();
+    SubmapViewBuild v = {};
+    v.n_entries = static_cast<uint32_t>(ctx->b_sub_maps.size());
+    v.entry_maps = submap_tables(ctx).entry_maps;
+    v.map_pt_off = tab;
+    v.map_node_base = tab + 3 * (ctx->kt_maps + 1);
+    v.map_centres = ctx->kt_centres.as<double>();
+    v.entries = ctx->s_entries.as<uint4>();
+    v.centres = ctx->s_centres.as<double>();
+    CU(launch_submap_view(v, ctx->sm_count, ctx->stream));
+    ctx->launches += v.n_entries ? 1 : 0;
+    ctx->b_view_ok = true;
+    return 0;
+  }
   if (!paired_maps(ctx) || ctx->b_view_ok) return 0;
   CU(cudaSetDevice(ctx->device));
   const size_t P = batch_members(ctx);
@@ -175,7 +231,12 @@ int linearize_round(sgb_ctx* ctx, int factor, int robust, double robust_c, int r
     for (size_t m = 0; m < B; m++) none[m].z = (!active || active[m]) ? kMemberActive : 0u;
     CU(cudaMemcpyAsync(ctx->b_members.p, none.data(), B * sizeof(uint4), cudaMemcpyHostToDevice, ctx->stream));
   }
-  if (n_tiles && ctx->tgt_state == TargetState::KdTrees) {
+  if (n_tiles && ctx->b_submaps) {
+    // submaps: every tile searched in the trees of its member's entries, each in its own stored frame (sgb_forest.cu)
+    CU(launch_submap_search(Bp, ctx->tgt_pnodes.as<float4>(), submap_view(ctx), n_tiles, ctx->kt_depth, search_bound(rejector, max_dist_sq),
+                            ctx->b_vcorr.as<uint32_t>(), ctx->stream));
+    ctx->launches += 1;
+  } else if (n_tiles && ctx->tgt_state == TargetState::KdTrees) {
     // many trees: every tile searched in its member's own tree, straight from the stored points at the member's pose (sgb_forest.cu)
     const bool view = paired_maps(ctx);
     const uint32_t* tab = (view ? ctx->v_tables : ctx->kt_tables).as<uint32_t>();
@@ -259,6 +320,84 @@ int reserve_members(sgb_ctx* ctx) {
   return reserve_query_scratch(ctx, nn);
 }
 
+// The batch's members become n_members replicas of its stored clouds (member p = cloud clouds[p], or cloud p), against map maps[p]
+// each if maps is given: what sgb_source_set_pairs does, and the member side of sgb_source_set_submaps.  who names the caller.
+int pair_members(sgb_ctx* ctx, const char* who, size_t n_members, const uint32_t* clouds, const uint32_t* maps) {
+  if (ctx->src_state != SourceState::Batch) return fail(ctx, 1, std::string(who) + ": the context holds no batch of sources (call sgb_source_set_batch)");
+  if (n_members > SGB_BATCH_MAX_MEMBERS)
+    return fail(ctx, 1, std::string(who) + ": " + std::to_string(n_members) + " members, at most " + std::to_string(SGB_BATCH_MAX_MEMBERS));
+  const std::vector<size_t>& coff = ctx->b_cloud_offsets;
+  const size_t N = coff.size() - 1, P = n_members;
+  if (!clouds && P != N)
+    return fail(ctx, 1, std::string(who) + ": without a cloud table member p is cloud p, so the member count (" + std::to_string(P) +
+                            ") must equal the cloud count (" + std::to_string(N) + ")");
+  // the device table: member offsets [P + 1] | cloud of each member [P] | map of each member [P] (only with maps)
+  std::vector<uint32_t> tab(2 * P + 1 + (maps ? P : 0));
+  std::vector<size_t> member_off(P + 1, 0);
+  uint32_t max_map = 0;
+  for (size_t p = 0; p < P; p++) {
+    const size_t c = clouds ? clouds[p] : p;
+    if (c >= N)
+      return fail(ctx, 1, std::string(who) + ": member " + std::to_string(p) + " names cloud " + std::to_string(c) + " but the batch holds " +
+                              std::to_string(N) + " clouds");
+    member_off[p + 1] = member_off[p] + (coff[c + 1] - coff[c]);
+    if (member_off[p + 1] >= (1ull << 31)) return fail(ctx, 1, std::string(who) + ": too many member points (at most 2^31 - 1 in all)");
+    tab[P + 1 + p] = static_cast<uint32_t>(c);
+    if (maps) {
+      tab[2 * P + 1 + p] = maps[p];
+      max_map = std::max(max_map, maps[p]);
+    }
+  }
+  for (size_t p = 0; p <= P; p++) tab[p] = static_cast<uint32_t>(member_off[p]);
+  const size_t n = member_off[P];
+  CU(cudaSetDevice(ctx->device));
+  begin_pairs(ctx);
+  ctx->b_offsets = member_off;
+  ctx->b_pair_has_maps = maps != nullptr;
+  if (maps) ctx->b_pair_maps.assign(maps, maps + P);
+  ctx->b_pair_max_map = max_map;
+  const size_t B = std::max<size_t>(P, 1), nn = std::max<size_t>(n, 1);
+  if (int rc = reserve_members(ctx)) return rc;
+  CU(ctx->p_tables.reserve(tab.size() * sizeof(uint32_t)));
+  CU(ctx->p_pts.reserve(nn * sizeof(float4)));
+  CU(ctx->p_perm.reserve(nn * sizeof(uint32_t)));
+  CU(ctx->p_centres.reserve(B * 4 * sizeof(double)));
+  CU(ctx->p_bounds.reserve(B * 6 * sizeof(double)));
+  if (ctx->src_has_covs) {
+    CU(ctx->p_covA.reserve(nn * sizeof(float4)));
+    CU(ctx->p_covB.reserve(nn * sizeof(float4)));
+  }
+  if (maps) {  // the view of whatever many-maps target the calls meet (pair_view)
+    CU(ctx->v_centres.reserve(B * 4 * sizeof(double)));
+    CU(ctx->v_tables.reserve((2 * B + 1) * sizeof(uint32_t)));
+    CU(ctx->v_regions.reserve(B * sizeof(uint4)));
+  }
+  if (P == 0) return 0;
+  // pageable host memory: the copy is staged before cudaMemcpyAsync returns
+  CU(cudaMemcpyAsync(ctx->p_tables.p, tab.data(), tab.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
+  PairGather g = {};
+  g.n = static_cast<uint32_t>(n);
+  g.n_members = static_cast<uint32_t>(P);
+  g.member_off = ctx->p_tables.as<uint32_t>();
+  g.clouds = g.member_off + P + 1;
+  g.cloud_off = ctx->b_cloud_off.as<uint32_t>();
+  g.pts = ctx->src_pts.as<float4>();
+  g.covA = ctx->src_has_covs ? ctx->src_covA.as<float4>() : nullptr;
+  g.covB = ctx->src_covB.as<float4>();
+  g.perm = ctx->src_perm.as<uint32_t>();
+  g.centres = ctx->b_centres.as<double>();
+  g.bounds = ctx->b_bounds.as<double>();
+  g.out_pts = ctx->p_pts.as<float4>();
+  g.out_covA = ctx->p_covA.as<float4>();
+  g.out_covB = ctx->p_covB.as<float4>();
+  g.out_perm = ctx->p_perm.as<uint32_t>();
+  g.out_centres = ctx->p_centres.as<double>();
+  g.out_bounds = ctx->p_bounds.as<double>();
+  CU(launch_pair_gather(g, ctx->sm_count, ctx->stream));
+  ctx->launches += 1;
+  return 0;
+}
+
 }  // namespace
 
 extern "C" {
@@ -336,87 +475,66 @@ int sgb_source_set_batch(sgb_ctx* ctx, size_t n_members, const size_t* offsets, 
 
 int sgb_source_set_pairs(sgb_ctx* ctx, size_t n_members, const uint32_t* clouds, const uint32_t* maps) {
   if (!ctx) return 1;
-  if (ctx->src_state != SourceState::Batch) return fail(ctx, 1, "sgb_source_set_pairs: the context holds no batch of sources (call sgb_source_set_batch)");
-  if (n_members > SGB_BATCH_MAX_MEMBERS)
-    return fail(ctx, 1, "sgb_source_set_pairs: " + std::to_string(n_members) + " members, at most " + std::to_string(SGB_BATCH_MAX_MEMBERS));
-  const std::vector<size_t>& coff = ctx->b_cloud_offsets;
-  const size_t N = coff.size() - 1, P = n_members;
-  if (!clouds && P != N)
-    return fail(ctx, 1, "sgb_source_set_pairs: without a cloud table member p is cloud p, so the member count (" + std::to_string(P) +
-                            ") must equal the cloud count (" + std::to_string(N) + ")");
-  // the device table: member offsets [P + 1] | cloud of each member [P] | map of each member [P] (only with maps)
-  std::vector<uint32_t> tab(2 * P + 1 + (maps ? P : 0));
-  std::vector<size_t> member_off(P + 1, 0);
-  uint32_t max_map = 0;
-  for (size_t p = 0; p < P; p++) {
-    const size_t c = clouds ? clouds[p] : p;
-    if (c >= N)
-      return fail(ctx, 1, "sgb_source_set_pairs: member " + std::to_string(p) + " names cloud " + std::to_string(c) + " but the batch holds " +
-                              std::to_string(N) + " clouds");
-    member_off[p + 1] = member_off[p] + (coff[c + 1] - coff[c]);
-    if (member_off[p + 1] >= (1ull << 31)) return fail(ctx, 1, "sgb_source_set_pairs: too many member points (at most 2^31 - 1 in all)");
-    tab[P + 1 + p] = static_cast<uint32_t>(c);
-    if (maps) {
-      tab[2 * P + 1 + p] = maps[p];
-      max_map = std::max(max_map, maps[p]);
-    }
-  }
-  for (size_t p = 0; p <= P; p++) tab[p] = static_cast<uint32_t>(member_off[p]);
-  const size_t n = member_off[P];
-  CU(cudaSetDevice(ctx->device));
-  begin_pairs(ctx);
-  ctx->b_offsets = member_off;
-  ctx->b_pair_has_maps = maps != nullptr;
-  if (maps) ctx->b_pair_maps.assign(maps, maps + P);
-  ctx->b_pair_max_map = max_map;
-  const size_t B = std::max<size_t>(P, 1), nn = std::max<size_t>(n, 1);
-  if (int rc = reserve_members(ctx)) return rc;
-  CU(ctx->p_tables.reserve(tab.size() * sizeof(uint32_t)));
-  CU(ctx->p_pts.reserve(nn * sizeof(float4)));
-  CU(ctx->p_perm.reserve(nn * sizeof(uint32_t)));
-  CU(ctx->p_centres.reserve(B * 4 * sizeof(double)));
-  CU(ctx->p_bounds.reserve(B * 6 * sizeof(double)));
-  if (ctx->src_has_covs) {
-    CU(ctx->p_covA.reserve(nn * sizeof(float4)));
-    CU(ctx->p_covB.reserve(nn * sizeof(float4)));
-  }
-  if (maps) {  // the view of whatever many-maps target the calls meet (pair_view)
-    CU(ctx->v_centres.reserve(B * 4 * sizeof(double)));
-    CU(ctx->v_tables.reserve((2 * B + 1) * sizeof(uint32_t)));
-    CU(ctx->v_regions.reserve(B * sizeof(uint4)));
-  }
-  if (P == 0) return 0;
-  // pageable host memory: the copy is staged before cudaMemcpyAsync returns
-  CU(cudaMemcpyAsync(ctx->p_tables.p, tab.data(), tab.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
-  PairGather g = {};
-  g.n = static_cast<uint32_t>(n);
-  g.n_members = static_cast<uint32_t>(P);
-  g.member_off = ctx->p_tables.as<uint32_t>();
-  g.clouds = g.member_off + P + 1;
-  g.cloud_off = ctx->b_cloud_off.as<uint32_t>();
-  g.pts = ctx->src_pts.as<float4>();
-  g.covA = ctx->src_has_covs ? ctx->src_covA.as<float4>() : nullptr;
-  g.covB = ctx->src_covB.as<float4>();
-  g.perm = ctx->src_perm.as<uint32_t>();
-  g.centres = ctx->b_centres.as<double>();
-  g.bounds = ctx->b_bounds.as<double>();
-  g.out_pts = ctx->p_pts.as<float4>();
-  g.out_covA = ctx->p_covA.as<float4>();
-  g.out_covB = ctx->p_covB.as<float4>();
-  g.out_perm = ctx->p_perm.as<uint32_t>();
-  g.out_centres = ctx->p_centres.as<double>();
-  g.out_bounds = ctx->p_bounds.as<double>();
-  CU(launch_pair_gather(g, ctx->sm_count, ctx->stream));
-  ctx->launches += 1;
-  return 0;
+  return pair_members(ctx, "sgb_source_set_pairs", n_members, clouds, maps);
 }
 
+int sgb_source_set_submaps(sgb_ctx* ctx, size_t n_members, const uint32_t* clouds, const size_t* list_off, const uint32_t* entry_maps, const double* entry_poses16) {
+  if (!ctx) return 1;
+  const std::string who = "sgb_source_set_submaps";
+  if (ctx->src_state != SourceState::Batch) return fail(ctx, 1, who + ": the context holds no batch of sources (call sgb_source_set_batch)");
+  if (n_members > SGB_BATCH_MAX_MEMBERS) return fail(ctx, 1, who + ": " + std::to_string(n_members) + " members, at most " + std::to_string(SGB_BATCH_MAX_MEMBERS));
+  if (!list_off) return fail(ctx, 1, who + ": null list offsets");
+  if (list_off[0] != 0) return fail(ctx, 1, who + ": list_off[0] must be 0");
+  for (size_t p = 0; p < n_members; p++)
+    if (list_off[p + 1] < list_off[p]) return fail(ctx, 1, who + ": list_off must be ascending (member " + std::to_string(p) + ")");
+  const size_t P = n_members, E = list_off[P];
+  if (E >= (1ull << 31)) return fail(ctx, 1, who + ": too many entries (at most 2^31 - 1 in all)");
+  if (E && !entry_maps) return fail(ctx, 1, who + ": null entry maps");
+  // the inverse of every placement, row-major R^T | -R^T t: the kernels carry the member's pose into the map's frame with it
+  std::vector<double> tables(12 * E + (P + 1 + E + 1) / 2);
+  for (size_t j = 0; j < E; j++) {
+    double R[12];
+    pose_from_colmajor(entry_poses16 ? entry_poses16 + 16 * j : kIdentity, R);
+    double dev = 0.0;
+    for (int a = 0; a < 3; a++)
+      for (int b = 0; b < 3; b++) dev = std::max(dev, std::fabs(R[a] * R[b] + R[3 + a] * R[3 + b] + R[6 + a] * R[6 + b] - (a == b ? 1.0 : 0.0)));
+    const double* M = entry_poses16 ? entry_poses16 + 16 * j : kIdentity;
+    const double det = R[0] * (R[4] * R[8] - R[5] * R[7]) - R[1] * (R[3] * R[8] - R[5] * R[6]) + R[2] * (R[3] * R[7] - R[4] * R[6]);
+    if (!(dev <= 1e-6) || !(det > 0.0) || M[3] != 0.0 || M[7] != 0.0 || M[11] != 0.0 || M[15] != 1.0 || !std::isfinite(R[9] + R[10] + R[11]))
+      return fail(ctx, 1, who + ": the pose of entry " + std::to_string(j) + " is not a rigid transformation (rotation block orthonormal to 1e-6, last row 0 0 0 1)");
+    double* inv = tables.data() + 12 * j;
+    for (int a = 0; a < 3; a++) {
+      for (int b = 0; b < 3; b++) inv[3 * a + b] = R[3 * b + a];
+      inv[9 + a] = -(R[a] * R[9] + R[3 + a] * R[10] + R[6 + a] * R[11]);
+    }
+  }
+  uint32_t* off = reinterpret_cast<uint32_t*>(tables.data() + 12 * E);
+  uint32_t max_map = 0;
+  for (size_t p = 0; p <= P; p++) off[p] = static_cast<uint32_t>(list_off[p]);
+  for (size_t j = 0; j < E; j++) {
+    off[P + 1 + j] = entry_maps[j];
+    max_map = std::max(max_map, entry_maps[j]);
+  }
+  if (int rc = pair_members(ctx, who.c_str(), P, clouds, nullptr)) return rc;
+  ctx->b_submaps = true;
+  ctx->b_sub_off.assign(off, off + P + 1);
+  ctx->b_sub_maps.assign(entry_maps, entry_maps + E);
+  ctx->b_pair_max_map = max_map;
+  CU(ctx->s_tables.reserve(tables.size() * sizeof(double)));
+  CU(ctx->s_entries.reserve(std::max<size_t>(E, 1) * sizeof(uint4)));
+  CU(ctx->s_centres.reserve(std::max<size_t>(E, 1) * 4 * sizeof(double)));
+  CU(ctx->b_centry.reserve(std::max<size_t>(batch_points(ctx), 1) * sizeof(uint32_t)));
+  // pageable host memory: the copy is staged before cudaMemcpyAsync returns
+  CU(cudaMemcpyAsync(ctx->s_tables.p, tables.data(), tables.size() * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
+  return 0;
+}
 int sgb_linearize_batch(sgb_ctx* ctx, int factor, int robust, double robust_c, int rejector, double max_dist_sq, const double* T, const uint8_t* active,
                         double* out44) {
   if (!ctx) return 1;
   if (int rc = batch_check(ctx, "sgb_linearize_batch", T)) return rc;
   if (factor < 0 || factor > 2 || robust < 0 || robust > 2 || rejector < 0 || rejector > 1) return fail(ctx, 1, "sgb_linearize_batch: invalid factor/robust/rejector kind");
   if (!out44) return fail(ctx, 1, "sgb_linearize_batch: null output");
+  if (int rc = submap_factor_check(ctx, "sgb_linearize_batch", factor)) return rc;
   const size_t B = batch_members(ctx);
   if (B == 0) return 0;
   if (batch_points(ctx) && ctx->n_tgt) {
@@ -450,6 +568,7 @@ int sgb_align_batch(sgb_ctx* ctx, const sgb_align_options* o, const double* init
   if (o->factor_kind < 0 || o->factor_kind > 2 || o->robust_kind < 0 || o->robust_kind > 2 || o->rejector_kind < 0 || o->rejector_kind > 1 ||
       o->optimizer_kind < 0 || o->optimizer_kind > 1)
     return fail(ctx, 1, "sgb_align_batch: invalid factor/robust/rejector/optimizer kind");
+  if (int rc = submap_factor_check(ctx, "sgb_align_batch", o->factor_kind)) return rc;
   const size_t B = batch_members(ctx);
   if (B == 0) return 0;
   if (batch_points(ctx) && ctx->n_tgt) {
@@ -539,7 +658,10 @@ int sgb_correspondences_batch(sgb_ctx* ctx, uint64_t* out) {
       continue;
     }
     // a multi-map target: the id within the member's own map (tgt_pts[k].w), as a context holding that map alone reports it
-    if (ctx->tgt_state == TargetState::VoxelMaps)
+    if (ctx->b_submaps)
+      CU(launch_submap_correspondences(ctx->b_corr.as<uint32_t>() + off, ctx->b_centry.as<uint32_t>() + off, perm + off, nm, ctx->tgt_pts.as<float4>(),
+                                       ctx->corr64.as<uint64_t>() + off, ctx->sm_count, ctx->stream));
+    else if (ctx->tgt_state == TargetState::VoxelMaps)
       CU(launch_voxelmaps_correspondences(ctx->b_corr.as<uint32_t>() + off, perm + off, nm, ctx->tgt_pts.as<float4>(), ctx->corr64.as<uint64_t>() + off, ctx->sm_count, ctx->stream));
     else
       CU(launch_correspondences(ctx->b_corr.as<uint32_t>() + off, perm + off, nm, ctx->tgt_pts.as<float4>(), voxel_target(ctx) ? 1 : 0, ctx->corr64.as<uint64_t>() + off, ctx->sm_count, ctx->stream));

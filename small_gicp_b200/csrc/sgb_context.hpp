@@ -195,12 +195,19 @@ struct sgb_ctx {
   bool b_paired = false;
   bool b_pair_has_maps = false;  // the pairing has a maps table (possibly of 0 members)
   std::vector<uint32_t> b_pair_maps;
-  uint32_t b_pair_max_map = 0;
+  uint32_t b_pair_max_map = 0;  // the largest map index the pairing names (b_pair_maps, or b_sub_maps of a submap pairing): the per-call check's fast path
   sgb::DevBuf p_tables;                    // uint32: member offsets [members + 1] | cloud of each member | map of each member
   sgb::DevBuf p_pts, p_covA, p_covB, p_perm, p_centres, p_bounds;
   // the many-maps target seen through b_pair_maps (PairView): rebuilt by the first batched call after the pairing or the target changed
   bool b_view_ok = false;
   sgb::DevBuf v_centres, v_tables, v_regions;  // [members][4] / pt_off [members + 1] | node_base [members] / [members]
+  // After sgb_source_set_submaps (b_submaps; also b_paired, without a maps table) member p is aligned against the union of the entries
+  // b_sub_off[p] .. b_sub_off[p + 1] - 1: entry j = map b_sub_maps[j] of a many-kd-trees target placed by a rigid pose.  s_tables is the
+  // one upload of the lists (SubmapTables in sgb_capi_batch.cu), s_entries / s_centres the target seen through them (SubmapView,
+  // rebuilt with b_view_ok), b_centry the entry of every cached correspondence (beside b_corr).
+  bool b_submaps = false;
+  std::vector<uint32_t> b_sub_off, b_sub_maps;
+  sgb::DevBuf s_tables, s_entries, s_centres, b_centry;
 };
 
 namespace sgb {
@@ -230,7 +237,7 @@ size_t target_maps(const sgb_ctx* ctx);
 int install_tree(sgb_ctx* ctx, int depth, size_t n_pnodes);
 /// a single cloud of n points, a batch (n = 0) or nothing replaces the source (and forgets any pairing of a batch)
 void begin_source(sgb_ctx* ctx, SourceState state, size_t n, bool covs);
-/// the batch's members become pairs of its stored clouds (the caller fills b_offsets, b_pair_maps and the replicas)
+/// the batch's members become pairs of its stored clouds (the caller fills b_offsets, b_pair_maps or the submap lists, and the replicas)
 void begin_pairs(sgb_ctx* ctx);
 /// normals and covariances (target) or covariances (source) were estimated on the device
 void features_changed(sgb_ctx* ctx, bool target);

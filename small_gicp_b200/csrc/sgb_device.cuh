@@ -104,6 +104,19 @@ __device__ __forceinline__ float3 centred_query_f32(const double* R, const doubl
   return make_float3(static_cast<float>(q.x), static_cast<float>(q.y), static_cast<float>(q.z));
 }
 
+/// The pose of a source relative to a placed map: out = Pinv * T, all row-major R (9) then t (3); Pinv = the inverse of the map's
+/// placement (R_P^T | -R_P^T t_P).  Submap members (sgb_source_set_submaps): the search and the factor kernels both derive a member's
+/// pose in the stored frame of an entry's map here, so a point is searched and linearised at the same pose.
+__device__ __forceinline__ void relative_pose(const double* __restrict__ Pinv, const double* __restrict__ T, double* out) {
+#pragma unroll
+  for (int r = 0; r < 3; r++) {
+    const double a = Pinv[3 * r + 0], b = Pinv[3 * r + 1], c = Pinv[3 * r + 2];
+#pragma unroll
+    for (int k = 0; k < 3; k++) out[3 * r + k] = a * T[k] + b * T[3 + k] + c * T[6 + k];
+    out[9 + r] = a * T[9] + b * T[10] + c * T[11] + Pinv[9 + r];
+  }
+}
+
 /// Squared distance of q to the box [lo, hi] (xyz; 0 inside): the pruning bound of the tree walks.
 __device__ __forceinline__ float box_dist2(float qx, float qy, float qz, const float4& lo, const float4& hi) {
   const float dx = fmaxf(fmaxf(lo.x - qx, qx - hi.x), 0.0f);

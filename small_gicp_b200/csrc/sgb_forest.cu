@@ -16,6 +16,8 @@
 // Search:
 //   forest_search_kernel        one CTA per BatchTile (128 consecutive stored points of ONE member): warp-cooperative exact nearest-
 //                               neighbour walk over that member's map, as packet_search_kernel walks one tree
+//   submap_search_kernel        the same for submap members (sgb_source_set_submaps, DESIGN.md §11 "Submaps"): the walk over every map
+//                               of the member's list, each in its own stored frame, the bound carried from map to map
 // The same build over the preprocessing scratch serves sgb_estimate_features_batch (forest_features_kernel, sgb_preprocess.cu).
 #include <algorithm>
 #include <cfloat>
@@ -324,6 +326,7 @@ __global__ void __launch_bounds__(kLinBlock, 8) forest_search_kernel(const __gri
     }
   }
 
+  // This walk exists twice: forest_walk below (used by submap_search_kernel) is a copy of it.  A change to one belongs in the other.
   int sp = 0;
   uint32_t cur = 0;    // inner node being expanded (index within the map's record block)
   bool expand = true;  // false: nothing to expand, take the next pending subtree
@@ -432,6 +435,182 @@ __global__ void __launch_bounds__(kLinBlock, 8) forest_search_kernel(const __gri
   if (valid) vcorr[v] = best;
 }
 
+// forest_search_kernel's walk of one tree's record block for the 32 queries of a warp, as a function: a copy, because calling it from
+// forest_search_kernel changes that kernel's register allocation (56 instead of 64 registers, other code).  best_d enters as each
+// lane's bound (< 0: an idle lane) and only a strictly nearer point replaces best.  Keep the two walks equal.
+__device__ __forceinline__ void forest_walk(const float4* __restrict__ pnodes, const float4* __restrict__ pts, float fx, float fy, float fz, float& best_d,
+                                            uint32_t& best, float* my_dist, uint2* my_child, uint32_t lane) {
+  int sp = 0;
+  uint32_t cur = 0;    // inner node being expanded (index within the map's record block)
+  bool expand = true;  // false: nothing to expand, take the next pending subtree
+  uint32_t leaf_first = 0, leaf_cnt = 0;
+  float leaf_d = 0.f;
+  for (;;) {
+    if (expand) {
+      const float4 n0 = __ldg(&pnodes[cur * 4 + 0]), n1 = __ldg(&pnodes[cur * 4 + 1]);
+      const float4 n2 = __ldg(&pnodes[cur * 4 + 2]), n3 = __ldg(&pnodes[cur * 4 + 3]);
+      const float dl = box_dist2(fx, fy, fz, n0, n1), dr = box_dist2(fx, fy, fz, n2, n3);
+      const bool wl = dl < best_d, wr = dr < best_d;
+      const unsigned ml = __ballot_sync(0xffffffffu, wl), mr = __ballot_sync(0xffffffffu, wr);
+      uint32_t ca, cb;
+      if (ml && mr) {
+        const unsigned closer_l = __ballot_sync(0xffffffffu, (wl || wr) && dl <= dr);
+        const bool left_first = 2 * __popc(closer_l) >= __popc(ml | mr);
+        my_dist[sp * kLinBlock] = left_first ? dr : dl;
+        if (lane == 0) my_child[sp] = left_first ? make_uint2(__float_as_uint(n2.w), __float_as_uint(n3.w)) : make_uint2(__float_as_uint(n0.w), __float_as_uint(n1.w));
+        sp++;
+        ca = left_first ? __float_as_uint(n0.w) : __float_as_uint(n2.w);
+        cb = left_first ? __float_as_uint(n1.w) : __float_as_uint(n3.w);
+        leaf_d = left_first ? dl : dr;
+      } else if (ml) {
+        ca = __float_as_uint(n0.w);
+        cb = __float_as_uint(n1.w);
+        leaf_d = dl;
+      } else if (mr) {
+        ca = __float_as_uint(n2.w);
+        cb = __float_as_uint(n3.w);
+        leaf_d = dr;
+      } else {
+        expand = false;
+        continue;
+      }
+      if (cb == 0u) {  // inner child
+        cur = ca;
+        continue;
+      }
+      leaf_first = ca;
+      leaf_cnt = cb;
+    } else {
+      bool got = false;
+      uint2 c = make_uint2(0u, 0u);
+      while (sp > 0) {
+        sp--;
+        const float d = my_dist[sp * kLinBlock];
+        if (__any_sync(0xffffffffu, d < best_d)) {
+          __syncwarp();  // lane 0's push of this entry is visible
+          c = my_child[sp];
+          __syncwarp();  // ... and every lane has read it before lane 0 may push over it
+          leaf_d = d;
+          got = true;
+          break;
+        }
+      }
+      if (!got) break;
+      if (c.y == 0u) {
+        cur = c.x;
+        expand = true;
+        continue;
+      }
+      leaf_first = c.x;
+      leaf_cnt = c.y;
+    }
+    // ---- leaf (global positions) ----
+    const unsigned want = __ballot_sync(0xffffffffu, leaf_d < best_d);
+    if (__popc(want) > kForestDenseLanes) {
+      const float4* lp = pts + leaf_first;
+#pragma unroll 4
+      for (uint32_t j = 0; j < leaf_cnt; j++) {
+        const float4 q = __ldg(&lp[j]);
+        const float dx = q.x - fx, dy = q.y - fy, dz = q.z - fz;
+        const float d = dx * dx + dy * dy + dz * dz;
+        if (d < best_d) {
+          best_d = d;
+          best = leaf_first + j;
+        }
+      }
+    } else {
+      for (uint32_t base = 0; base < leaf_cnt; base += 32u) {
+        const uint32_t j = base + lane;
+        float4 q = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (j < leaf_cnt) q = __ldg(&pts[leaf_first + j]);
+        unsigned todo = want;
+        while (todo) {
+          const int src = __ffs(todo) - 1;
+          todo &= todo - 1;
+          const float qx = __shfl_sync(0xffffffffu, fx, src), qy = __shfl_sync(0xffffffffu, fy, src), qz = __shfl_sync(0xffffffffu, fz, src);
+          const float dx = q.x - qx, dy = q.y - qy, dz = q.z - qz;
+          const uint32_t dbits = j < leaf_cnt ? __float_as_uint(dx * dx + dy * dy + dz * dz) : 0x7f800000u;
+          const uint32_t dmin = __reduce_min_sync(0xffffffffu, dbits);
+          const unsigned who = __ballot_sync(0xffffffffu, dbits == dmin);  // lowest lane = first point in scan order
+          if (static_cast<int>(lane) == src) {
+            const float d = __uint_as_float(dmin);
+            if (d < best_d) {
+              best_d = d;
+              best = leaf_first + base + (__ffs(who) - 1);
+            }
+          }
+        }
+      }
+    }
+    expand = false;
+  }
+}
+
+// The FP32 query of stored point sp of a member at pose T (centre cs) in the stored frame of submap entry e: the member's pose carried
+// through the inverse of the entry's placement, then centred on the entry's map as forest_search_kernel centres on map m.
+__device__ __forceinline__ float3 submap_query(const SubmapView& S, uint32_t e, const double* T, const double* cs, const float4& sp) {
+  double Tk[12];
+  relative_pose(S.inv_poses + 12 * static_cast<size_t>(e), T, Tk);
+  const double3 tp = centred_translation(Tk, cs[0], cs[1], cs[2], S.centres + 4 * static_cast<size_t>(e));
+  return centred_query_f32(Tk, tp, sp);
+}
+
+// forest_search_kernel for submap members (sgb_source_set_submaps): the warp still owns 32 consecutive stored points of ONE member, and
+// walks the tree of every entry of that member's list in list order, each in its map's own stored frame.  Rigid placements preserve
+// distances, so the nearest point of the placed union is the nearest over the entries, and best_d carried from entry to entry prunes
+// the later trees: one that no lane's ball reaches costs its root record's two box tests.  Only a strictly nearer point replaces the
+// best, so at an exact FP32 tie between two entries the earlier one wins.  The seed is evaluated in the frame of the entry that owned it.
+__global__ void __launch_bounds__(kLinBlock, 7) submap_search_kernel(const __grid_constant__ BatchParams B, const float4* __restrict__ all_pnodes,
+                                                                     const __grid_constant__ SubmapView S, float bound, uint32_t* __restrict__ vcorr) {
+  extern __shared__ float s_dist[];  // [max_depth][kLinBlock] per-lane box distance of each pending subtree
+  __shared__ uint2 s_child[kForestWarps][kForestStack];
+  const BatchTile t = B.tiles[blockIdx.x];
+  const uint32_t lane = threadIdx.x & 31u, wib = threadIdx.x >> 5;
+  if (wib * 32u >= t.count) return;  // warp-uniform; no CTA barrier below
+  const uint32_t m = t.member;
+  const bool valid = threadIdx.x < t.count;
+  const uint32_t i = t.first + threadIdx.x, v = t.vfirst + threadIdx.x;
+  const uint32_t e0 = __ldg(&S.entry_off[m]), e1 = __ldg(&S.entry_off[m + 1]);
+  const float4* __restrict__ pts = B.tgt.pts;
+  const double* T = B.poses + 12 * static_cast<size_t>(m);
+  const double* cs = B.centres + 4 * static_cast<size_t>(m);
+  float* my_dist = s_dist + threadIdx.x;
+  uint2* my_child = s_child[wib];
+
+  const float4 sp = valid ? __ldg(&B.pts[i]) : make_float4(0.f, 0.f, 0.f, 0.f);
+  float best_d = valid ? bound : -1.0f;  // an idle lane is never interested in anything
+  uint32_t best = kNone, best_e = 0;
+  if (valid && (B.members[m].z & kMemberSeeded)) {
+    // the member's previous correspondence: an upper bound only prunes
+    const uint32_t prev = B.corr[i];
+    if (prev != kNone) {
+      const uint32_t pe = S.centry[i];
+      const float3 f = submap_query(S, e0 + pe, T, cs, sp);
+      const float4 q = __ldg(&pts[prev]);
+      const float dx = q.x - f.x, dy = q.y - f.y, dz = q.z - f.z;
+      const float d = dx * dx + dy * dy + dz * dz;
+      if (d < best_d) {
+        best_d = d;
+        best = prev;
+        best_e = pe;
+      }
+    }
+  }
+  for (uint32_t e = e0; e < e1; e++) {
+    const uint4 ent = __ldg(&S.entries[e]);
+    if (ent.y == 0u) continue;  // an empty map
+    const float3 f = submap_query(S, e, T, cs, sp);
+    const float before = best_d;
+    forest_walk(all_pnodes + 4 * static_cast<size_t>(ent.z), pts, f.x, f.y, f.z, best_d, best, my_dist, my_child, lane);
+    if (best_d < before) best_e = e - e0;
+    __syncwarp();
+  }
+  if (valid) {
+    vcorr[v] = best;
+    S.centry[i] = best_e;
+  }
+}
+
 }  // namespace
 
 cudaError_t launch_forest_build(const ForestBuild& b, cudaStream_t st, int* launches) {
@@ -488,6 +667,14 @@ cudaError_t launch_forest_search(const BatchParams& B, const ForestView& F, uint
   if (max_depth < 1 || max_depth > kForestStack) return cudaErrorInvalidValue;
   const size_t smem = static_cast<size_t>(max_depth) * kLinBlock * sizeof(float);
   forest_search_kernel<<<n_tiles, kLinBlock, smem, st>>>(B, F, bound, vcorr);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_submap_search(const BatchParams& B, const float4* pnodes, const SubmapView& S, uint32_t n_tiles, int max_depth, float bound, uint32_t* vcorr,
+                                 cudaStream_t st) {
+  if (max_depth < 1 || max_depth > kForestStack) return cudaErrorInvalidValue;
+  const size_t smem = static_cast<size_t>(max_depth) * kLinBlock * sizeof(float);
+  submap_search_kernel<<<n_tiles, kLinBlock, smem, st>>>(B, pnodes, S, bound, vcorr);
   return cudaGetLastError();
 }
 

@@ -48,6 +48,14 @@ void set_general_factor(sgb_align_options& o, const GeneralFactor& g) {
     static_assert(dependent_false<GeneralFactor>::value, "BatchRegistration: NullFactor or RestrictDoFFactor");
   }
 }
+/// point-to-plane, with or without a robust kernel: its residual n o r is not rotation invariant, so it has no meaning against maps
+/// that each sit at a pose of their own (sgb_source_set_submaps)
+template <typename Factor>
+struct is_point_to_plane : std::false_type {};
+template <>
+struct is_point_to_plane<PointToPlaneICPFactor> : std::true_type {};
+template <typename Kernel>
+struct is_point_to_plane<RobustFactor<Kernel, PointToPlaneICPFactor>> : std::true_type {};
 }  // namespace detail
 
 template <typename PointFactor, typename GeneralFactor = NullFactor, typename CorrespondenceRejector = DistanceRejector,
@@ -135,6 +143,36 @@ struct BatchRegistration {
     check(ctx, sgb_source_set_batch(ctx, sources.size(), src.offsets.data(), src.points.data(), src.covs_or_null()));
     const std::vector<uint32_t> clouds = indices(cloud_of_member, sources.size(), "source");
     check(ctx, sgb_source_set_pairs(ctx, clouds.size(), clouds.data(), nullptr));
+    return run(ctx, init_Ts);
+  }
+
+  /// Submaps: one RegistrationResult per member, in order: sources[cloud_of_member[p]] from init_Ts[p] (source -> common frame) against
+  /// the UNION of submaps[p], a list of (index into maps, pose of that map in the common frame).  Each map's kd-tree is built once and
+  /// no map is transformed, however many lists name it and whatever its poses (sgb_source_set_submaps); all members in one
+  /// sgb_align_batch call.  ICP and GICP (the maps need covariances); point-to-plane does not compile.
+  template <typename Target, typename Source>
+  std::vector<RegistrationResult> align(const std::vector<Target>& maps, const std::vector<Source>& sources, const std::vector<size_t>& cloud_of_member,
+                                        const std::vector<std::vector<std::pair<size_t, Isometry3d>>>& submaps, const std::vector<Isometry3d>& init_Ts) const {
+    static_assert(!detail::is_point_to_plane<PointFactor>::value,
+                  "BatchRegistration: point-to-plane is not available against submaps (its element-wise residual n o r is not invariant under the map poses); use ICPFactor or GICPFactor");
+    if (cloud_of_member.size() != init_Ts.size() || submaps.size() != init_Ts.size()) throw std::runtime_error("BatchRegistration: one cloud, one submap list and one initial pose per member");
+    sgb_ctx* ctx = reduction.context();
+    reduction.invalidate();
+    const Concatenated tgt(maps), src(sources);
+    check(ctx, sgb_target_build_kdtrees(ctx, maps.size(), tgt.offsets.data(), tgt.points.data(), nullptr, tgt.covs_or_null()));
+    check(ctx, sgb_source_set_batch(ctx, sources.size(), src.offsets.data(), src.points.data(), src.covs_or_null()));
+    const std::vector<uint32_t> clouds = indices(cloud_of_member, sources.size(), "source");
+    std::vector<size_t> list_off(submaps.size() + 1, 0), entry_map;
+    std::vector<double> poses;
+    for (size_t p = 0; p < submaps.size(); p++) {
+      list_off[p + 1] = list_off[p] + submaps[p].size();
+      for (const auto& entry : submaps[p]) {
+        entry_map.push_back(entry.first);
+        poses.insert(poses.end(), entry.second.data(), entry.second.data() + 16);
+      }
+    }
+    const std::vector<uint32_t> entry_maps = indices(entry_map, maps.size(), "map");
+    check(ctx, sgb_source_set_submaps(ctx, clouds.size(), clouds.data(), list_off.data(), entry_maps.data(), poses.data()));
     return run(ctx, init_Ts);
   }
 

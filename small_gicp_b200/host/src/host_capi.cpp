@@ -164,6 +164,29 @@ struct PairsJob {
   }
 };
 
+struct SubmapsJob {
+  const Options& o;
+  const std::vector<PointCloud>& maps;
+  const std::vector<PointCloud>& sources;
+  const std::vector<size_t>& cloud_of_member;
+  const std::vector<std::vector<std::pair<size_t, Isometry3d>>>& submaps;
+  const std::vector<Isometry3d>& init;
+  std::vector<RegistrationResult> results;
+  template <typename Factor, typename General, typename Rejector, typename Optimizer, bool kRobust>
+  void call() {
+    if constexpr (detail::is_point_to_plane<Factor>::value) {  // the overload itself does not compile for it
+      throw std::runtime_error("sgbh_align_batch_submaps: point-to-plane is not available against submaps");
+    } else {
+      BatchRegistration<Factor, General, Rejector, Optimizer> reg;
+      configure(reg, o);
+      set_rejector(reg, o, std::is_same<Rejector, DistanceRejector>());
+      set_general(reg, o, std::is_same<General, RestrictDoFFactor>());
+      set_robust(reg.point_factor, o, std::integral_constant<bool, kRobust>());
+      results = reg.align(maps, sources, cloud_of_member, submaps, init);
+    }
+  }
+};
+
 template <typename Factor, bool kRobust, typename Job>
 void dispatch_rest(const Options& o, Job& job) {
   const int key = (o.restrict_dof ? 4 : 0) | (o.rejector == SGB_REJECT_DISTANCE ? 2 : 0) | (o.optimizer ? 1 : 0);
@@ -334,6 +357,49 @@ int sgbh_align_batch_pairs(size_t n_pairs, const size_t* target_offsets, const d
       return 1;
     }
     for (size_t m = 0; m < n_pairs; m++)
+      write_result(job.results[m], T_out16xB + 16 * m, scalars_out4xB + 4 * m, H_out36xB ? H_out36xB + 36 * m : nullptr, b_out6xB ? b_out6xB + 6 * m : nullptr);
+    return 0;
+  } catch (const std::exception& e) {
+    g_error = e.what();
+    return 2;
+  }
+}
+
+/// BatchRegistration<...>::align over submaps: the options of sgbh_align; map t = rows map_offsets[t] .. map_offsets[t+1] (covariances
+/// or none), source s likewise; member p = source cloud_of_member[p] against the entries list_off[p] .. list_off[p+1] - 1, entry j = map
+/// entry_maps[j] at the column-major pose entry_poses16[16 j ..].  One initial pose per member; outputs as sgbh_align_batch's.
+int sgbh_align_batch_submaps(size_t n_members, size_t n_maps, const size_t* map_offsets, const double* map_pts4, const double* map_covs16, size_t n_sources,
+                             const size_t* source_offsets, const double* source_pts4, const double* source_covs16, const size_t* cloud_of_member,
+                             const size_t* list_off, const size_t* entry_maps, const double* entry_poses16, const double* options21, const double* init_T16xB,
+                             double* T_out16xB, double* scalars_out4xB, double* H_out36xB, double* b_out6xB) {
+  try {
+    const Options o = parse_options(options21);
+    std::vector<PointCloud> maps(n_maps), sources(n_sources);
+    for (size_t t = 0; t < n_maps; t++) {
+      const size_t to = map_offsets[t], tn = map_offsets[t + 1] - to;
+      maps[t] = *make_cloud(tn, map_pts4 + 4 * to, nullptr, map_covs16 ? map_covs16 + 16 * to : nullptr);
+    }
+    for (size_t m = 0; m < n_sources; m++) {
+      const size_t so = source_offsets[m], sn = source_offsets[m + 1] - so;
+      sources[m] = *make_cloud(sn, source_pts4 + 4 * so, nullptr, source_covs16 ? source_covs16 + 16 * so : nullptr);
+    }
+    std::vector<Isometry3d> init(n_members);
+    std::vector<size_t> clouds(cloud_of_member, cloud_of_member + n_members);
+    std::vector<std::vector<std::pair<size_t, Isometry3d>>> submaps(n_members);
+    for (size_t p = 0; p < n_members; p++) {
+      std::memcpy(init[p].matrix().data(), init_T16xB + 16 * p, sizeof(double) * 16);
+      for (size_t j = list_off[p]; j < list_off[p + 1]; j++) {
+        Isometry3d P;
+        std::memcpy(P.matrix().data(), entry_poses16 + 16 * j, sizeof(double) * 16);
+        submaps[p].emplace_back(entry_maps[j], P);
+      }
+    }
+    SubmapsJob job{o, maps, sources, clouds, submaps, init, {}};
+    if (!dispatch(o, job)) {
+      g_error = "sgbh_align_batch_submaps: invalid factor kind";
+      return 1;
+    }
+    for (size_t m = 0; m < n_members; m++)
       write_result(job.results[m], T_out16xB + 16 * m, scalars_out4xB + 4 * m, H_out36xB ? H_out36xB + 36 * m : nullptr, b_out6xB ? b_out6xB + 6 * m : nullptr);
     return 0;
   } catch (const std::exception& e) {

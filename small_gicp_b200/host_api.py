@@ -228,6 +228,52 @@ def align_batch_pairs(
     return capi.BatchAlignResult(T[:B], sc4[:B], np.concatenate([H, b], axis=1)[:B])
 
 
+def align_batch_submaps(maps, sources, lists, poses, map_covs=None, source_covs=None, init_Ts=None, cloud_of_member=None, factor=capi.FACTOR_GICP,
+                        robust=capi.ROBUST_NONE, robust_c=1.0, rejector=capi.REJECT_DISTANCE, max_dist_sq=1.0, optimizer=OPT_LM, max_iterations=20,
+                        rotation_eps=0.1 * np.pi / 180.0, translation_eps=1e-3, dof_mask=None, device=0):
+    """BatchRegistration<...>::align(maps, sources, cloud_of_member, submaps, init_Ts) (C++ host mirror): member p = sources[cloud_of_member[p]]
+    (None: source p) from init_Ts[p] against the union of the maps lists[p], map lists[p][j] placed by the 4x4 pose poses[p][j] (map ->
+    common frame); each map's kd-tree is built once and none is transformed.  maps / sources: lists of (N_m, 3|4) arrays; map_covs /
+    source_covs: None or lists of (N_m, 4, 4).  ICP and GICP; point-to-plane raises.  Returns capi.BatchAlignResult."""
+    L = _lib()
+    szp = C.POINTER(C.c_size_t)
+    if not hasattr(L.sgbh_align_batch_submaps, "_typed"):
+        L.sgbh_align_batch_submaps.restype = C.c_int
+        L.sgbh_align_batch_submaps.argtypes = [C.c_size_t, C.c_size_t, szp, _dp, _dp, C.c_size_t, szp, _dp, _dp, szp, szp, szp, _dp, _dp, _dp, _dp, _dp, _dp, _dp]
+        L.sgbh_align_batch_submaps._typed = True
+    B = len(lists)
+
+    def concat(clouds, covs):
+        members = [capi._points4(c) for c in clouds]
+        offsets = np.zeros(len(members) + 1, dtype=np.uintp)
+        offsets[1:] = np.cumsum([m.shape[0] for m in members])
+        p = np.ascontiguousarray(np.concatenate(members) if members else np.zeros((0, 4)))
+        c = None if covs is None else np.ascontiguousarray(np.concatenate([_f64(x) for x in covs]) if members else np.zeros((0, 4, 4)))
+        return offsets, p, c
+
+    mo, mp, mc = concat(maps, map_covs)
+    so, sp, sc = concat(sources, source_covs)
+    cl = np.ascontiguousarray(np.arange(B) if cloud_of_member is None else cloud_of_member, dtype=np.uintp).reshape(B)
+    off = np.zeros(B + 1, dtype=np.uintp)
+    off[1:] = np.cumsum([len(l) for l in lists])
+    em = np.ascontiguousarray([k for l in lists for k in l], dtype=np.uintp)
+    assert all(len(poses[p]) == len(lists[p]) for p in range(B)), "one pose per list entry"
+    ep = np.ascontiguousarray(np.array([np.asarray(P, dtype=float).reshape(4, 4).T for ps in poses for P in ps]).reshape(-1, 16)) if em.size else np.zeros((1, 16))
+    opts = np.zeros(21)
+    opts[:13] = [factor, robust, robust_c, rejector, max_dist_sq, optimizer, max_iterations, rotation_eps, translation_eps, TREE_DEVICE_KDTREE, 1.0, 1,
+                 0 if dof_mask is None else 1]
+    opts[13:19] = 1.0 if dof_mask is None else np.asarray(dof_mask, dtype=float)
+    opts[19] = device
+    Ts = np.tile(np.eye(4), (B, 1, 1)) if init_Ts is None else np.asarray(init_Ts, dtype=float).reshape(B, 4, 4)
+    T0 = np.ascontiguousarray(Ts.transpose(0, 2, 1))
+    T, sc4, H, b = np.zeros((max(B, 1), 16)), np.zeros((max(B, 1), 4)), np.zeros((max(B, 1), 36)), np.zeros((max(B, 1), 6))
+    rc = L.sgbh_align_batch_submaps(B, len(maps), mo.ctypes.data_as(szp), _d(mp), _d(mc), len(sources), so.ctypes.data_as(szp), _d(sp), _d(sc),
+                                    cl.ctypes.data_as(szp), off.ctypes.data_as(szp), em.ctypes.data_as(szp), _d(ep), _d(opts), _d(T0), _d(T), _d(sc4), _d(H), _d(b))
+    if rc != 0:
+        raise capi.SgbError(L.sgbh_last_error().decode())
+    return capi.BatchAlignResult(T[:B], sc4[:B], np.concatenate([H, b], axis=1)[:B])
+
+
 ICP, PLANE_ICP, GICP, VGICP = 0, 1, 2, 3  # RegistrationSetting::RegistrationType
 
 
