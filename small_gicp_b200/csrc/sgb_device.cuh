@@ -376,6 +376,49 @@ __device__ __forceinline__ double comm_all_reduce(const CommParams& c, double v)
   return s;
 }
 
+/// Sum over the 32 lanes of a warp of N <= 32 values per lane (x[k]: this lane's term of sum k); lane k returns sum k (lanes >= N: 0).
+/// The transposing butterfly of block_reduce_and_finish with the lane bits taken from the lowest: every aligned group of eight sums is
+/// reduced over lane bits 0..2 (4 + 2 + 1 exchanges), which leaves one value per group and lane, and the (up to) four group values are
+/// then reduced over lane bits 3 and 4 (2 + 1 exchanges).  For 29 sums that is 30 exchanges, as few as one butterfly over all of them,
+/// but a group's terms are dead once the group is reduced: the compiler can produce and reduce the terms eight at a time.
+/// The order of the additions is fixed by the lane numbers: deterministic.
+template <int N>
+__device__ __forceinline__ double warp_sum_transposed(const double* x) {
+  static_assert(N <= 32, "one lane per sum");
+  const int lane = threadIdx.x & 31;
+  double g[4];
+#pragma unroll
+  for (int G = 0; G < 4; G++) {
+    double v[8];
+#pragma unroll
+    for (int k = 0; k < 8; k++) v[k] = 8 * G + k < N ? x[8 * G + k] : 0.0;
+#pragma unroll
+    for (int w = 1; w <= 4; w <<= 1) {  // lane bit w: slots k and k + w (k a multiple of 2w) -> slot k, this lane's half kept
+      const bool upper = (lane & w) != 0;
+#pragma unroll
+      for (int k = 0; k < 8; k += 2 * w) {
+        if (8 * G + k >= N) continue;  // both halves are padding
+        const double keep = upper ? v[k + w] : v[k];
+        const double send = upper ? v[k] : v[k + w];
+        v[k] = keep + __shfl_xor_sync(0xffffffffu, send, w);
+      }
+    }
+    g[G] = v[0];  // lane l: sum of slot 8 G + (l & 7) over the eight lanes l ^ 0..7
+  }
+#pragma unroll
+  for (int w = 1; w <= 2; w <<= 1) {  // lane bits 3 and 4 over the group values (group k and k + w -> group k)
+    const bool upper = (lane & (8 * w)) != 0;
+#pragma unroll
+    for (int k = 0; k < 4; k += 2 * w) {
+      if (8 * k >= N) continue;
+      const double keep = upper ? g[k + w] : g[k];
+      const double send = upper ? g[k] : g[k + w];
+      g[k] = keep + __shfl_xor_sync(0xffffffffu, send, 8 * w);
+    }
+  }
+  return g[0];
+}
+
 /// CTAs per group of the two-level final reduction (see block_reduce_and_finish)
 constexpr unsigned int kFinishGroup = 16;
 /// doubles / tickets the reduction needs for a grid of `grid` CTAs
@@ -389,13 +432,16 @@ __host__ __device__ inline size_t reduction_tickets(size_t grid) { return 1 + (g
 /// partials: reduction_partials_doubles(gridDim.x) doubles; ticket: reduction_tickets(gridDim.x) zeroed counters (left zeroed).
 /// comm.world > 1: the finishing CTA then exchanges the sums with the other ranks (comm_all_reduce) before writing `out`.
 /// tile_sum (sgb_batch.cu) is a copy of the CTA butterfly below: keep the two equal (sharing it changes this function's register allocation).
-template <int NACC, bool EXPAND>
+/// TRANSPOSED: the warps already hold their sums one per lane (acc[0] of lane k is the warp's sum k, e.g. from warp_sum_transposed): no butterfly.
+template <int NACC, bool EXPAND, bool TRANSPOSED = false>
 __device__ __forceinline__ void block_reduce_and_finish(double* acc, double* partials, unsigned int* ticket, double* out, const CommParams& comm) {
   static_assert(NACC <= 32, "one lane per accumulator");
   __shared__ double s_red[kLinBlock / 32][NACC];
   __shared__ bool s_last;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  if (NACC > 4) {
+  if (TRANSPOSED) {
+    if (lane < NACC) s_red[warp][lane] = acc[0];
+  } else if (NACC > 4) {
     // Transposing butterfly: at every step a lane keeps one half of the values it still owns and hands the other half to its partner,
     // so the 32 lanes end up with ONE fully reduced accumulator each (lane l holds sum l): 16 + 8 + 4 + 2 + 1 = 31 exchanges instead of
     // 5 per accumulator (145 for the 29 sums of linearize).  The order of

@@ -173,10 +173,10 @@ SGB_HD Sym3 plane_weight_source(const double* R, double nx, double ny, double nz
   return d;
 }
 
-/// Same sums as accumulate_factor, from the source-frame weight D = R^T M R and the source-frame residual rs = R^T r.
+/// One point's terms of the same sums as accumulate_factor (sum k gets t[k]), from the source-frame weight D = R^T M R and the
+/// source-frame residual rs = R^T r.
 template <int ROBUST>
-SGB_HD void accumulate_factor_source(const Sym3& D, double rsx, double rsy, double rsz, double px, double py, double pz, double robust_c,
-                                                         double* acc) {
+SGB_HD void factor_terms_source(const Sym3& D, double rsx, double rsy, double rsz, double px, double py, double pz, double robust_c, double* t) {
   const double mrx = D.xx * rsx + D.xy * rsy + D.xz * rsz;
   const double mry = D.xy * rsx + D.yy * rsy + D.yz * rsz;
   const double mrz = D.xz * rsx + D.yz * rsy + D.zz * rsz;
@@ -194,34 +194,74 @@ SGB_HD void accumulate_factor_source(const Sym3& D, double rsx, double rsy, doub
   const double u00 = py * d02 - pz * d01, u01 = py * d12 - pz * d11, u02 = py * d22 - pz * d12;
   const double u10 = pz * d00 - px * d02, u11 = pz * d01 - px * d12, u12 = pz * d02 - px * d22;
   const double u20 = px * d01 - py * d00, u21 = px * d11 - py * d01, u22 = px * d12 - py * d02;
-  acc[0] += py * u02 - pz * u01;
-  acc[1] += pz * u00 - px * u02;
-  acc[2] += px * u01 - py * u00;
-  acc[3] += pz * u10 - px * u12;
-  acc[4] += px * u11 - py * u10;
-  acc[5] += px * u21 - py * u20;
-  acc[6] += u00;
-  acc[7] += u01;
-  acc[8] += u02;
-  acc[9] += u10;
-  acc[10] += u11;
-  acc[11] += u12;
-  acc[12] += u20;
-  acc[13] += u21;
-  acc[14] += u22;
-  acc[15] += d00;
-  acc[16] += d01;
-  acc[17] += d02;
-  acc[18] += d11;
-  acc[19] += d12;
-  acc[20] += d22;
-  acc[21] += gy * pz - gz * py;
-  acc[22] += gz * px - gx * pz;
-  acc[23] += gx * py - gy * px;
-  acc[24] -= gx;
-  acc[25] -= gy;
-  acc[26] -= gz;
-  acc[27] += w * e;
+  t[0] = py * u02 - pz * u01;
+  t[1] = pz * u00 - px * u02;
+  t[2] = px * u01 - py * u00;
+  t[3] = pz * u10 - px * u12;
+  t[4] = px * u11 - py * u10;
+  t[5] = px * u21 - py * u20;
+  t[6] = u00;
+  t[7] = u01;
+  t[8] = u02;
+  t[9] = u10;
+  t[10] = u11;
+  t[11] = u12;
+  t[12] = u20;
+  t[13] = u21;
+  t[14] = u22;
+  t[15] = d00;
+  t[16] = d01;
+  t[17] = d02;
+  t[18] = d11;
+  t[19] = d12;
+  t[20] = d22;
+  t[21] = gy * pz - gz * py;
+  t[22] = gz * px - gx * pz;
+  t[23] = gx * py - gy * px;
+  t[24] = -gx;
+  t[25] = -gy;
+  t[26] = -gz;
+  t[27] = w * e;
+}
+
+/// Same sums as accumulate_factor, from the source-frame weight D = R^T M R and the source-frame residual rs = R^T r.
+template <int ROBUST>
+SGB_HD void accumulate_factor_source(const Sym3& D, double rsx, double rsy, double rsz, double px, double py, double pz, double robust_c,
+                                                         double* acc) {
+  double t[kAcc];
+  factor_terms_source<ROBUST>(D, rsx, rsy, rsz, px, py, pz, robust_c, t);
+#pragma unroll
+  for (int k = 0; k < kAcc; k++) acc[k] += t[k];
+}
+
+/// The part of point_linearize_source (below, same arguments) before the sums: false if rejected (D, rs, p untouched), else the
+/// source-frame weight D, the source-frame residual rs and the source point p (absolute, FP64) that factor_terms_source takes.
+template <int FACTOR>
+SGB_HD bool point_weight_source(const double* R, double tpx, double tpy, double tpz, double csx, double csy, double csz, double max_dist_sq_d,
+                                const float4& sp, const float4* sA, const float4* sB, const float4& tq, const float4* t1, const float4* t2, Sym3& D,
+                                double* rs, double* p) {
+  const double sx = sp.x, sy = sp.y, sz = sp.z;
+  const double qx = R[0] * sx + R[1] * sy + R[2] * sz + tpx;
+  const double qy = R[3] * sx + R[4] * sy + R[5] * sz + tpy;
+  const double qz = R[6] * sx + R[7] * sy + R[8] * sz + tpz;
+  const double rx = static_cast<double>(tq.x) - qx, ry = static_cast<double>(tq.y) - qy, rz = static_cast<double>(tq.z) - qz;
+  if (rx * rx + ry * ry + rz * rz > max_dist_sq_d) return false;  // DistanceRejector on the FP64 residual (rejector.hpp:24)
+  // weight and residual in the SOURCE frame (D = R^T M R, rs = R^T r): see gicp_precision_source
+  if (FACTOR == 0) {
+    D = Sym3{1.0, 0.0, 0.0, 1.0, 0.0, 1.0};
+  } else if (FACTOR == 1) {
+    const float4 nrm = *t1;
+    D = plane_weight_source(R, nrm.x, nrm.y, nrm.z);
+  } else {
+    D = gicp_precision_source(R, *sA, *sB, *t1, *t2);
+  }
+  rs[0] = R[0] * rx + R[3] * ry + R[6] * rz;
+  rs[1] = R[1] * rx + R[4] * ry + R[7] * rz;
+  rs[2] = R[2] * rx + R[5] * ry + R[8] * rz;
+  p[0] = csx + sx;
+  p[1] = csy + sy;
+  p[2] = csz + sz;
+  return true;
 }
 
 /// One accepted-or-rejected correspondence of `linearize`, evaluated exactly as factor_reduce_kernel does it:
@@ -236,24 +276,10 @@ template <int FACTOR, int ROBUST>
 SGB_HD bool point_linearize_source(const double* R, double tpx, double tpy, double tpz, double csx, double csy, double csz, double max_dist_sq_d,
                                    double robust_c, const float4& sp, const float4* sA, const float4* sB, const float4& tq, const float4* t1,
                                    const float4* t2, double* acc) {
-  const double sx = sp.x, sy = sp.y, sz = sp.z;
-  const double qx = R[0] * sx + R[1] * sy + R[2] * sz + tpx;
-  const double qy = R[3] * sx + R[4] * sy + R[5] * sz + tpy;
-  const double qz = R[6] * sx + R[7] * sy + R[8] * sz + tpz;
-  const double rx = static_cast<double>(tq.x) - qx, ry = static_cast<double>(tq.y) - qy, rz = static_cast<double>(tq.z) - qz;
-  if (rx * rx + ry * ry + rz * rz > max_dist_sq_d) return false;  // DistanceRejector on the FP64 residual (rejector.hpp:24)
-  // weight and residual in the SOURCE frame (D = R^T M R, rs = R^T r): see gicp_precision_source
   Sym3 D;
-  if (FACTOR == 0) {
-    D = Sym3{1.0, 0.0, 0.0, 1.0, 0.0, 1.0};
-  } else if (FACTOR == 1) {
-    const float4 nrm = *t1;
-    D = plane_weight_source(R, nrm.x, nrm.y, nrm.z);
-  } else {
-    D = gicp_precision_source(R, *sA, *sB, *t1, *t2);
-  }
-  const double rsx = R[0] * rx + R[3] * ry + R[6] * rz, rsy = R[1] * rx + R[4] * ry + R[7] * rz, rsz = R[2] * rx + R[5] * ry + R[8] * rz;
-  accumulate_factor_source<ROBUST>(D, rsx, rsy, rsz, csx + sx, csy + sy, csz + sz, robust_c, acc);
+  double rs[3], p[3];
+  if (!point_weight_source<FACTOR>(R, tpx, tpy, tpz, csx, csy, csz, max_dist_sq_d, sp, sA, sB, tq, t1, t2, D, rs, p)) return false;
+  accumulate_factor_source<ROBUST>(D, rs[0], rs[1], rs[2], p[0], p[1], p[2], robust_c, acc);
   acc[kAcc] += 1.0;
   return true;
 }
