@@ -321,6 +321,27 @@ typedef struct sgb_align_options {
  * out_Hb42xB (or NULL) = H(36) | b(6) per member (RegistrationResult).  max_iterations <= 0 returns the initial poses, not converged. */
 int sgb_align_batch(sgb_ctx* ctx, const sgb_align_options* options, const double* init_T16xB, double* out_T16xB, double* out_info4xB,
                     double* out_Hb42xB /*or NULL*/);
+/* sgb_align_batch enqueued on the context's stream (sgb_set_stream) with no host involvement after the call: the rounds are planned on
+ * the device and driven by a CUDA graph whose conditional WHILE node repeats one round (planner, search, factor, per-member sums, step)
+ * until no member has a round to go.  No host synchronisation, no device-to-host copy, no upload from pageable memory: the call returns
+ * once the work is enqueued, and a torch op (or any work) queued after it on the same stream sees the results.
+ *   - Inputs and outputs as sgb_align_batch (same layouts), but all of them device memory of the context's GPU; host, page-locked or
+ *     managed pointers fail with a message and nothing is enqueued.  Per member, T, info and H | b are bit-identical to sgb_align_batch with
+ *     the same options, poses, batch, pairing or submap lists and target, and the context is left as sgb_align_batch leaves it
+ *     (sgb_correspondences_batch, sgb_error_batch and sgb_linearize_batch behave alike afterwards).
+ *   - It fails with a message where sgb_align_batch does (no batch, connected comm, invalid kinds, point-to-plane on submaps, missing
+ *     normals or covariances), and where the driver has no conditional graph nodes.  Errors of the enqueued work surface at the next
+ *     synchronising call of the context (as for sgb_linearize_device).
+ *   - While the context's stream is being captured (cudaStreamIsCapturing, e.g. inside torch.cuda.graph) the align is added to the
+ *     capture instead: each replay re-runs it from what d_init_T16xB holds at replay time.  The captured work is only valid while the
+ *     context's batch, pairing, target and buffers are those of the capture; call it once outside the capture first (the first batched
+ *     call of a context allocates).  Outside a capture the loop's instantiated graph is cached in the context and rebuilt when the options,
+ *     the batch, the pairing, the target or any buffer it uses changes.
+ *   - sgb_kernel_launches counts 3 per call with max_iterations > 0 (initial state, one launch of the loop graph, outputs) and 2 without,
+ *     whatever the round count, plus 1 when the pairing's view of the target is rebuilt (as for sgb_align_batch); captured work counts
+ *     the same at capture and nothing at replay. */
+int sgb_align_batch_async(sgb_ctx* ctx, const sgb_align_options* options, const double* d_init_T16xB, double* d_out_T16xB, double* d_out_info4xB,
+                          double* d_out_Hb42xB /*or NULL*/);
 
 /* ---- per-cloud preparation on the device (SURVEY.md §8(f); not per-iteration) --------------------
  * sgb_estimate_features replaces estimate_normals / estimate_covariances / estimate_normals_covariances and

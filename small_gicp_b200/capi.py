@@ -84,6 +84,7 @@ _SIGNATURES = {
     "sgb_error_batch": (C.c_int, [_vp, _dp, C.POINTER(C.c_uint8), _dp]),
     "sgb_correspondences_batch": (C.c_int, [_vp, _u64p]),
     "sgb_align_batch": (C.c_int, [_vp, C.POINTER(AlignOptions), _dp, _dp, _dp, _dp]),
+    "sgb_align_batch_async": (C.c_int, [_vp, C.POINTER(AlignOptions), _dp, _dp, _dp, _dp]),
     "sgb_estimate_features": (C.c_int, [_vp, C.c_size_t, _dp, C.c_int, _dp, _dp]),
     "sgb_target_estimate_features": (C.c_int, [_vp, C.c_int]),
     "sgb_source_estimate_features": (C.c_int, [_vp, C.c_int]),
@@ -110,6 +111,24 @@ class BatchAlignResult:
         self.error = info4[:, 3].copy()
         self.H = np.ascontiguousarray(Hb42[:, :36].reshape(B, 6, 6).transpose(0, 2, 1))
         self.b = Hb42[:, 36:42].copy()
+
+
+class AsyncAlignResult:
+    """what Context.align_batch_async enqueued: CUDA float64 tensors filled in stream order.  T_target_source (B,4,4), H (B,6,6) and b
+    (B,6) as in BatchAlignResult; converged (1.0 / 0.0), iterations, num_inliers and error are (B,) float64 views of the info rows.  All
+    are views of the raw outputs T16 (B,16), info4 (B,4) and Hb42 (B,42), which pass as out= to reuse them (graph capture needs fixed
+    buffers)."""
+
+    def __init__(self, T16, info4, Hb42):
+        B = T16.shape[0]
+        self.T16, self.info4, self.Hb42 = T16, info4, Hb42
+        self.T_target_source = T16.view(B, 4, 4).transpose(1, 2)
+        self.converged = info4[:, 0]
+        self.iterations = info4[:, 1]
+        self.num_inliers = info4[:, 2]
+        self.error = info4[:, 3]
+        self.H = Hb42[:, :36].view(B, 6, 6).transpose(1, 2)
+        self.b = Hb42[:, 36:42]
 
 
 def library_path(profiling=False):
@@ -197,6 +216,8 @@ class Context:
             raise SgbError(self._L.sgb_last_error(None).decode())
         self._h = h
         self.device = int(device)
+        self._stream = None  # set_stream's stream (None: the context's own)
+        self._async_in = None  # align_batch_async's column-major poses
 
     def close(self):
         if getattr(self, "_h", None):
@@ -216,6 +237,7 @@ class Context:
     # ---- plumbing ----
     def set_stream(self, cuda_stream_ptr):
         self._check(self._L.sgb_set_stream(self._h, _vp(cuda_stream_ptr) if cuda_stream_ptr else None))
+        self._stream = int(cuda_stream_ptr) if cuda_stream_ptr else None
 
     def synchronize(self):
         self._check(self._L.sgb_synchronize(self._h))
@@ -537,6 +559,39 @@ class Context:
         Hb = np.zeros((max(B, 1), 42))
         self._check(self._L.sgb_align_batch(self._h, C.byref(o), _d(Tc), _d(T), _d(info), _d(Hb)))
         return BatchAlignResult(T[:B], info[:B], Hb[:B])
+
+    def align_batch_async(self, init_Ts, factor=FACTOR_GICP, robust=ROBUST_NONE, robust_c=1.0, rejector=REJECT_DISTANCE, max_dist_sq=1.0,
+                          optimizer=OPT_LEVENBERG_MARQUARDT, max_iterations=20, gn_lambda=1e-6, max_inner_iterations=10, init_lambda=1e-3,
+                          lambda_factor=10.0, rotation_eps=0.1 * np.pi / 180.0, translation_eps=1e-3, dof_mask=None, out=None):
+        """align_batch enqueued on the context's stream without a host synchronisation (sgb_align_batch_async).  init_Ts: CUDA float64
+        (B, 4, 4) row-major, on the context's device; the context's stream must have been set (set_stream) to a torch stream, on which the
+        poses are transposed into the library's column-major layout.  Returns an AsyncAlignResult of CUDA tensors (out: a previous result
+        whose buffers are reused).  Inside torch.cuda.graph (with the capture stream set) the align is captured: each replay re-runs it
+        from what init_Ts holds then."""
+        import torch
+
+        if self._stream is None:
+            raise SgbError("align_batch_async: set the context's stream to a torch stream first (set_stream): the poses are prepared on it")
+        offsets = getattr(self, "_batch_offsets", None)  # (no batch yet: the library says so)
+        B = int(offsets.size) - 1 if offsets is not None else int(init_Ts.shape[0])
+        if not (isinstance(init_Ts, torch.Tensor) and init_Ts.is_cuda and init_Ts.dtype == torch.float64 and tuple(init_Ts.shape) == (B, 4, 4)):
+            raise SgbError(f"align_batch_async: init_Ts must be a CUDA float64 tensor of shape ({B}, 4, 4)")
+        o = AlignOptions(int(factor), int(robust), float(robust_c), int(rejector), float(max_dist_sq), int(optimizer), int(max_iterations), float(gn_lambda),
+                         int(max_inner_iterations), float(init_lambda), float(lambda_factor), float(rotation_eps), float(translation_eps))
+        o.dof_mask[:] = [1.0] * 6 if dof_mask is None else [float(x) for x in dof_mask]
+        dev = init_Ts.device
+        with torch.cuda.stream(torch.cuda.ExternalStream(self._stream, device=dev)):
+            if out is None:
+                n = max(B, 1)
+                out = AsyncAlignResult(torch.zeros((n, 16), dtype=torch.float64, device=dev)[:B], torch.zeros((n, 4), dtype=torch.float64, device=dev)[:B],
+                                       torch.zeros((n, 42), dtype=torch.float64, device=dev)[:B])
+            elif tuple(out.T16.shape) != (B, 16):
+                raise SgbError(f"align_batch_async: out holds {out.T16.shape[0]} members, the batch {B}")
+            if self._async_in is None or self._async_in.shape[0] != B or self._async_in.device != dev:
+                self._async_in = torch.empty((max(B, 1), 16), dtype=torch.float64, device=dev)[:B]
+            self._async_in.view(B, 4, 4).copy_(init_Ts.transpose(1, 2))  # column-major
+        self._check(self._L.sgb_align_batch_async(self._h, C.byref(o), _d(self._async_in), _d(out.T16), _d(out.info4), _d(out.Hb42)))
+        return out
 
     # ---- multi-GPU: all-reduce of H|b|e fused into the reduction kernel (peer memory over NVLink) ----
     COMM_HANDLE_BYTES = 64

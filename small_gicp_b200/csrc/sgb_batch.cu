@@ -67,7 +67,8 @@ __device__ __forceinline__ double tile_sum(const double* acc) {
   return v;
 }
 
-__global__ void __launch_bounds__(kLinBlock) batch_transform_kernel(const __grid_constant__ BatchParams B, float4* vq, uint32_t* vcorr) {
+// (batch_transform_tile: the body of batch_transform_kernel and batch_transform_round_kernel)
+__device__ __forceinline__ void batch_transform_tile(const BatchParams& B, float4* vq, uint32_t* vcorr) {
   const BatchTile t = B.tiles[blockIdx.x];
   const uint32_t tid = threadIdx.x;
   if (tid >= t.count) return;
@@ -79,6 +80,10 @@ __global__ void __launch_bounds__(kLinBlock) batch_transform_kernel(const __grid
   vq[v] = make_float4(f.x, f.y, f.z, 0.f);
   // the member's previous correspondence seeds the search (seeds only prune: the result does not depend on them)
   vcorr[v] = (B.members[t.member].z & kMemberSeeded) ? B.corr[i] : kNone;
+}
+
+__global__ void __launch_bounds__(kLinBlock) batch_transform_kernel(const __grid_constant__ BatchParams B, float4* vq, uint32_t* vcorr) {
+  batch_transform_tile(B, vq, vcorr);
 }
 
 // One tile of batch_factor_kernel.  ERR = false: linearize (VOX: voxel-map probe here; else vcorr = what the search found); ERR = true:
@@ -211,7 +216,7 @@ __global__ void __launch_bounds__(kLinBlock, 4) batch_submap_factor_kernel(const
 // linearisation pose (read by later error() calls).
 constexpr int kSegWarps = 8;
 template <int NACC, bool LIN>
-__global__ void __launch_bounds__(kSegWarps * 32) batch_segment_kernel(const __grid_constant__ BatchParams B, double* out) {
+__device__ __forceinline__ void batch_segment(const BatchParams& B, double* out) {
   __shared__ double s_sum[kSegWarps][NACC];
   const uint32_t m = blockIdx.x, lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
   const uint4 mem = B.members[m];
@@ -236,16 +241,17 @@ __global__ void __launch_bounds__(kSegWarps * 32) batch_segment_kernel(const __g
   }
   if (LIN && (mem.z & kMemberActive) && threadIdx.x < 12) B.lin_poses[12 * static_cast<size_t>(m) + threadIdx.x] = B.poses[12 * static_cast<size_t>(m) + threadIdx.x];
 }
+template <int NACC, bool LIN>
+__global__ void __launch_bounds__(kSegWarps * 32) batch_segment_kernel(const __grid_constant__ BatchParams B, double* out) {
+  batch_segment<NACC, LIN>(B, out);
+}
 
 // One thread per member: the step is a sequential 6x6 solve and a few 4x4 products (about 2k FP64 operations), and at the 65536-member
 // limit that is 512 CTAs of 128 threads.  The state stays in global memory; only the solve's matrix is copied (to local memory: the
 // pivot indexes it at run time).
 constexpr int kStepBlock = 128;
-__global__ void __launch_bounds__(kStepBlock) batch_step_kernel(const __grid_constant__ AlignOptions o, uint32_t n_members, bool linearize,
-                                                                const double* __restrict__ out, MemberState* __restrict__ state,
-                                                                double* __restrict__ poses, uint8_t* __restrict__ phase) {
-  const uint32_t m = blockIdx.x * kStepBlock + threadIdx.x;
-  if (m >= n_members) return;
+__device__ __forceinline__ void batch_step_member(const AlignOptions& o, uint32_t m, bool linearize, const double* __restrict__ out,
+                                                  MemberState* __restrict__ state, double* __restrict__ poses, uint8_t* __restrict__ phase) {
   MemberState& s = state[m];
   if (linearize && s.phase == kPhaseLinearize)
     align_after_linearize(o, s, out + 44 * static_cast<size_t>(m));
@@ -258,6 +264,13 @@ __global__ void __launch_bounds__(kStepBlock) batch_step_kernel(const __grid_con
     p[9 + i] = T[12 + i];
   }
   phase[m] = static_cast<uint8_t>(s.phase);
+}
+__global__ void __launch_bounds__(kStepBlock) batch_step_kernel(const __grid_constant__ AlignOptions o, uint32_t n_members, bool linearize,
+                                                                const double* __restrict__ out, MemberState* __restrict__ state,
+                                                                double* __restrict__ poses, uint8_t* __restrict__ phase) {
+  const uint32_t m = blockIdx.x * kStepBlock + threadIdx.x;
+  if (m >= n_members) return;
+  batch_step_member(o, m, linearize, out, state, poses, phase);
 }
 
 cudaError_t launch_batch_step(const AlignOptions& o, uint32_t n_members, bool linearize, const double* out, MemberState* state, double* poses,
@@ -444,6 +457,236 @@ cudaError_t launch_batch_segment(const BatchParams& B, uint32_t n_members, bool 
     batch_segment_kernel<kAcc + 1, true><<<n_members, kSegWarps * 32, 0, st>>>(B, out);
   else
     batch_segment_kernel<1, false><<<n_members, kSegWarps * 32, 0, st>>>(B, out);
+  return cudaGetLastError();
+}
+
+// ---- sgb_align_batch_async: the rounds planned and sized on the device (DESIGN.md §11 "Asynchronous align") ----
+
+// The head of a round, one CTA: the host loop's rule (an error() round while any member has a pending trial, else a linearize round of
+// the members still iterating) and batch_tables' tables in the same order -- members in member order, each active non-empty member's
+// points in tiles of kLinBlock, the virtual source concatenating the active members -- then the round's sizes.  Members are taken
+// 1024 at a time: a CTA scan of the (tile, point) counts, then the chunk's tiles written by all threads (binary search for the owner).
+constexpr int kPlanBlock = 1024;
+__global__ void __launch_bounds__(kPlanBlock) batch_plan_kernel(const BatchPlan p) {
+  __shared__ uint32_t s_wt[32], s_wv[32], s_tot[2];
+  __shared__ uint32_t s_end[kPlanBlock], s_first[kPlanBlock], s_n[kPlanBlock], s_v0[kPlanBlock];
+  const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
+  if (tid == 0) cudaGraphSetConditional(p.loop, 0u);
+  for (int k = 0; k < 3; k++)
+    if (p.zero[k])
+      for (uint32_t j = tid; j < p.zero_n[k]; j += kPlanBlock) p.zero[k][j] = 0u;
+  int trial = 0;
+  for (uint32_t m = tid; m < p.n_members; m += kPlanBlock) trial |= p.phase[m] == kPhaseTrial;
+  const bool lin = !__syncthreads_or(trial);
+  const uint8_t want = lin ? kPhaseLinearize : kPhaseTrial;
+  uint32_t carry_t = 0, carry_v = 0;
+  for (uint32_t base = 0; base < p.n_members; base += kPlanBlock) {
+    const uint32_t m = base + tid;
+    bool act = false;
+    uint32_t first = 0, n = 0;
+    if (m < p.n_members) {
+      act = p.phase[m] == want;
+      first = p.member_off[m];
+      n = p.member_off[m + 1] - first;
+    }
+    const uint32_t nt = act ? (n + kLinBlock - 1u) / kLinBlock : 0u, nv = act ? n : 0u;
+    uint32_t it = nt, iv = nv;  // inclusive scan within the warp, then over the warp totals
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const uint32_t yt = __shfl_up_sync(0xffffffffu, it, o), yv = __shfl_up_sync(0xffffffffu, iv, o);
+      if (lane >= static_cast<uint32_t>(o)) {
+        it += yt;
+        iv += yv;
+      }
+    }
+    if (lane == 31u) {
+      s_wt[warp] = it;
+      s_wv[warp] = iv;
+    }
+    __syncthreads();
+    if (warp == 0) {
+      const uint32_t wt = s_wt[lane], wv = s_wv[lane];
+      uint32_t at = wt, av = wv;
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1) {
+        const uint32_t yt = __shfl_up_sync(0xffffffffu, at, o), yv = __shfl_up_sync(0xffffffffu, av, o);
+        if (lane >= static_cast<uint32_t>(o)) {
+          at += yt;
+          av += yv;
+        }
+      }
+      s_wt[lane] = at - wt;
+      s_wv[lane] = av - wv;
+      if (lane == 31u) {
+        s_tot[0] = at;
+        s_tot[1] = av;
+      }
+    }
+    __syncthreads();
+    const uint32_t et = s_wt[warp] + it - nt, ev = s_wv[warp] + iv - nv;  // exclusive within the chunk
+    if (m < p.n_members) {
+      const bool seeded = lin && p.seeds && p.seeded[m];
+      p.members[m] = p.no_target ? make_uint4(0u, 0u, lin && act ? kMemberActive : 0u, 0u)
+                                 : make_uint4(carry_t + et, nt, (act ? kMemberActive : 0u) | (seeded ? kMemberSeeded : 0u), 0u);
+      if (lin && act) p.seeded[m] = 1;  // its correspondences are cached by this round
+    }
+    s_end[tid] = et + nt;
+    s_first[tid] = first;
+    s_n[tid] = n;
+    s_v0[tid] = carry_v + ev;
+    __syncthreads();
+    const uint32_t tot_t = s_tot[0], tot_v = s_tot[1];
+    for (uint32_t k = tid; k < tot_t; k += kPlanBlock) {
+      uint32_t lo = 0, hi = kPlanBlock - 1;  // the owner: the first j with s_end[j] > k
+      while (lo < hi) {
+        const uint32_t mid = (lo + hi) >> 1;
+        if (s_end[mid] > k) hi = mid;
+        else lo = mid + 1;
+      }
+      const uint32_t j = (k - (lo ? s_end[lo - 1] : 0u)) * kLinBlock;
+      p.tiles[carry_t + k] = BatchTile{base + lo, s_first[lo] + j, min(static_cast<uint32_t>(kLinBlock), s_n[lo] - j), s_v0[lo] + j};
+    }
+    carry_t += tot_t;
+    carry_v += tot_v;
+    __syncthreads();  // the shared tables are reused by the next chunk
+  }
+  if (tid == 0) *p.round = BatchRound{lin ? 1u : 0u, p.no_target ? 0u : carry_t, lin && !p.no_target ? carry_v : 0u, lin && p.no_target ? carry_t : 0u};
+}
+
+__global__ void __launch_bounds__(kLinBlock) batch_transform_round_kernel(const __grid_constant__ BatchParams B, float4* vq, uint32_t* vcorr,
+                                                                          const BatchRound* __restrict__ round) {
+  const BatchRound r = *round;
+  if (!r.lin || blockIdx.x >= r.n_tiles) return;
+  batch_transform_tile(B, vq, vcorr);
+}
+
+// a linearize round against an empty target: every point of the active members is left without a correspondence
+__global__ void __launch_bounds__(kLinBlock) batch_unmatch_round_kernel(const __grid_constant__ BatchParams B, const BatchRound* __restrict__ round) {
+  if (blockIdx.x >= round->n_clear) return;
+  const BatchTile t = B.tiles[blockIdx.x];
+  if (threadIdx.x < t.count) B.corr[t.first + threadIdx.x] = kNone;
+}
+
+// The factor kernel of a round, linearize or error() as the planner decided, with the tile of the kernels launch_factor picks on the host
+// (KIND: 0 one point target, 1 one voxel map, 2 many voxel maps, 3 many kd-trees, 4 submaps).
+template <int FACTOR, int ROBUST, int KIND>
+__global__ void __launch_bounds__(kLinBlock, 4) batch_factor_round_kernel(const __grid_constant__ BatchParams B, const uint32_t* __restrict__ vcorr,
+                                                                         const double* __restrict__ map_centres, const uint4* __restrict__ map_regions,
+                                                                         const __grid_constant__ SubmapView S, const BatchRound* __restrict__ round) {
+  constexpr bool VOX = KIND == 1 || KIND == 2, MAPS = KIND == 2 || KIND == 3, SUB = KIND == 4;
+  const BatchRound r = *round;
+  if (blockIdx.x >= r.n_tiles) return;
+  if (r.lin)
+    batch_factor_tile<FACTOR, ROBUST, VOX, false, MAPS, SUB>(B, vcorr, map_centres, map_regions, &S);
+  else
+    batch_factor_tile<FACTOR, ROBUST, VOX, true, MAPS, SUB>(B, nullptr, map_centres, map_regions, &S);
+}
+
+__global__ void __launch_bounds__(kSegWarps * 32) batch_segment_round_kernel(const __grid_constant__ BatchParams B, double* out, const BatchRound* __restrict__ round) {
+  if (round->lin)
+    batch_segment<kAcc + 1, true>(B, out);
+  else
+    batch_segment<1, false>(B, out);
+}
+
+// the step of a round; the loop's condition becomes 1 if any member still has a round to go
+__global__ void __launch_bounds__(kStepBlock) batch_step_round_kernel(const __grid_constant__ AlignOptions o, uint32_t n_members, const BatchRound* __restrict__ round,
+                                                                      const double* __restrict__ out, MemberState* __restrict__ state,
+                                                                      double* __restrict__ poses, uint8_t* __restrict__ phase, cudaGraphConditionalHandle loop) {
+  const uint32_t m = blockIdx.x * kStepBlock + threadIdx.x;
+  int more = 0;
+  if (m < n_members) {
+    batch_step_member(o, m, round->lin != 0u, out, state, poses, phase);
+    more = phase[m] == kPhaseLinearize || phase[m] == kPhaseTrial;
+  }
+  if (__syncthreads_or(more) && threadIdx.x == 0) cudaGraphSetConditional(loop, 1u);
+}
+
+__global__ void __launch_bounds__(kStepBlock) batch_align_init_kernel(const __grid_constant__ AlignOptions o, uint32_t n_members, const double* __restrict__ init_T16,
+                                                                      MemberState* __restrict__ state, double* __restrict__ poses, uint8_t* __restrict__ phase,
+                                                                      uint8_t* __restrict__ seeded, int keep_seeds) {
+  const uint32_t m = blockIdx.x * kStepBlock + threadIdx.x;
+  if (m >= n_members) return;
+  const double* T = init_T16 + 16 * static_cast<size_t>(m);
+  align_init(o, T, state[m]);
+  double* p = poses + 12 * static_cast<size_t>(m);
+  for (int i = 0; i < 3; i++) {  // pose_from_colmajor
+    for (int j = 0; j < 3; j++) p[i * 3 + j] = T[j * 4 + i];
+    p[9 + i] = T[12 + i];
+  }
+  phase[m] = static_cast<uint8_t>(state[m].phase);
+  if (!keep_seeds) seeded[m] = 0;
+}
+
+__global__ void __launch_bounds__(kStepBlock) batch_align_finish_kernel(uint32_t n_members, const MemberState* __restrict__ state, double* __restrict__ out_T16,
+                                                                        double* __restrict__ out_info4, double* __restrict__ out_Hb42) {
+  const uint32_t m = blockIdx.x * kStepBlock + threadIdx.x;
+  if (m >= n_members) return;
+  const MemberState& s = state[m];
+  for (int i = 0; i < 16; i++) out_T16[16 * static_cast<size_t>(m) + i] = s.T[i];
+  double* info = out_info4 + 4 * static_cast<size_t>(m);
+  info[0] = s.converged ? 1.0 : 0.0;
+  info[1] = s.iterations;
+  info[2] = s.inliers;
+  info[3] = s.e;
+  if (out_Hb42) {
+    double* hb = out_Hb42 + 42 * static_cast<size_t>(m);
+    for (int i = 0; i < 36; i++) hb[i] = s.H[i];
+    for (int i = 0; i < 6; i++) hb[36 + i] = s.b[i];
+  }
+}
+
+cudaError_t launch_batch_plan(const BatchPlan& p, cudaStream_t st) {
+  batch_plan_kernel<<<1, kPlanBlock, 0, st>>>(p);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_batch_transform_round(const BatchParams& B, const BatchRound* round, uint32_t max_tiles, float4* vq, uint32_t* vcorr, cudaStream_t st) {
+  batch_transform_round_kernel<<<max_tiles, kLinBlock, 0, st>>>(B, vq, vcorr, round);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_batch_unmatch_round(const BatchParams& B, const BatchRound* round, uint32_t max_tiles, cudaStream_t st) {
+  batch_unmatch_round_kernel<<<max_tiles, kLinBlock, 0, st>>>(B, round);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_batch_factor_round(const BatchParams& B, int kind, int factor, int robust, const BatchRound* round, uint32_t max_tiles, const uint32_t* vcorr,
+                                      const double* map_centres, const uint4* map_regions, const SubmapView& S, cudaStream_t st) {
+  if (factor == 1 && (kind == 1 || kind == 2 || kind == 4)) return cudaErrorInvalidValue;  // no normals in a voxel map; no point-to-plane against a union
+  return dispatch_factor_robust(factor, robust, cudaErrorInvalidValue, [&](auto f, auto r) {
+    constexpr int F = f == 1 ? 0 : f;  // (the kinds without point-to-plane: one instantiation fewer each)
+    switch (kind) {
+      case 0: batch_factor_round_kernel<f, r, 0><<<max_tiles, kLinBlock, 0, st>>>(B, vcorr, map_centres, map_regions, S, round); break;
+      case 1: batch_factor_round_kernel<F, r, 1><<<max_tiles, kLinBlock, 0, st>>>(B, vcorr, map_centres, map_regions, S, round); break;
+      case 2: batch_factor_round_kernel<F, r, 2><<<max_tiles, kLinBlock, 0, st>>>(B, vcorr, map_centres, map_regions, S, round); break;
+      case 3: batch_factor_round_kernel<f, r, 3><<<max_tiles, kLinBlock, 0, st>>>(B, vcorr, map_centres, map_regions, S, round); break;
+      case 4: batch_factor_round_kernel<F, r, 4><<<max_tiles, kLinBlock, 0, st>>>(B, vcorr, map_centres, map_regions, S, round); break;
+      default: return cudaErrorInvalidValue;
+    }
+    return cudaGetLastError();
+  });
+}
+
+cudaError_t launch_batch_segment_round(const BatchParams& B, const BatchRound* round, uint32_t n_members, double* out, cudaStream_t st) {
+  batch_segment_round_kernel<<<n_members, kSegWarps * 32, 0, st>>>(B, out, round);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_batch_step_round(const AlignOptions& o, uint32_t n_members, const BatchRound* round, const double* out, MemberState* state, double* poses,
+                                    uint8_t* phase, cudaGraphConditionalHandle loop, cudaStream_t st) {
+  batch_step_round_kernel<<<(n_members + kStepBlock - 1) / kStepBlock, kStepBlock, 0, st>>>(o, n_members, round, out, state, poses, phase, loop);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_batch_align_init(const AlignOptions& o, uint32_t n_members, const double* init_T16, MemberState* state, double* poses, uint8_t* phase,
+                                    uint8_t* seeded, bool keep_seeds, cudaStream_t st) {
+  batch_align_init_kernel<<<(n_members + kStepBlock - 1) / kStepBlock, kStepBlock, 0, st>>>(o, n_members, init_T16, state, poses, phase, seeded, keep_seeds ? 1 : 0);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_batch_align_finish(uint32_t n_members, const MemberState* state, double* out_T16, double* out_info4, double* out_Hb42, cudaStream_t st) {
+  batch_align_finish_kernel<<<(n_members + kStepBlock - 1) / kStepBlock, kStepBlock, 0, st>>>(n_members, state, out_T16, out_info4, out_Hb42);
   return cudaGetLastError();
 }
 

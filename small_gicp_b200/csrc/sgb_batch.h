@@ -102,4 +102,44 @@ cudaError_t launch_batch_segment(const BatchParams& B, uint32_t n_members, bool 
 cudaError_t launch_batch_step(const AlignOptions& o, uint32_t n_members, bool linearize, const double* out, MemberState* state, double* poses,
                               uint8_t* phase, cudaStream_t st);
 
+// ---- sgb_align_batch_async (DESIGN.md §11 "Asynchronous align"): the rounds planned and sized on the device ----
+/// What a round does, written by batch_plan_kernel at its head and read by every kernel of the round.  lin: 1 = linearize of the members
+/// in kPhaseLinearize, 0 = error() of the members in kPhaseTrial; n_tiles: tiles the factor kernel and the tile searches process;
+/// n_search: queries of the virtual source (linearize rounds of a point target, else 0); n_clear: tiles whose points are left without a
+/// correspondence (a linearize round against an empty target).
+struct __align__(16) BatchRound {
+  uint32_t lin, n_tiles, n_search, n_clear;
+};
+/// The planner's inputs: the host loop's rule and batch_tables' tables, built on the device by one CTA.
+struct BatchPlan {
+  uint32_t n_members;
+  const uint32_t* member_off;  // [members + 1]
+  const uint8_t* phase;        // [members] kPhase* after the last step
+  uint8_t* seeded;             // [members] the device's copy of b_seeded: 1 = the member's cached correspondences may seed its search
+  int seeds;                   // linearize rounds mark seeded members (point targets; voxel maps have no search to seed)
+  int no_target;               // an empty target: no tiles to search or factor (the members still get zeros), n_clear instead
+  BatchTile* tiles;
+  uint4* members;
+  BatchRound* round;
+  uint32_t* zero[3];  // counters of the point search cleared at the head of every round (null: none)
+  uint32_t zero_n[3];
+  cudaGraphConditionalHandle loop;  // set to 0 here; the step kernel sets it to 1 while a member is still in a round
+};
+cudaError_t launch_batch_plan(const BatchPlan& p, cudaStream_t st);
+/// batch_transform_kernel / the factor kernel of the target's kind / batch_segment_kernel / batch_step_kernel in a planned round: the grids
+/// are sized for every tile (every member), the work is read from `round`, and the CTAs beyond it exit at once.  kind: 0 one point target,
+/// 1 one voxel map, 2 many voxel maps, 3 many kd-trees, 4 submaps.  The step kernel sets `loop` to 1 while a member is still in a round.
+cudaError_t launch_batch_transform_round(const BatchParams& B, const BatchRound* round, uint32_t max_tiles, float4* vq, uint32_t* vcorr, cudaStream_t st);
+cudaError_t launch_batch_unmatch_round(const BatchParams& B, const BatchRound* round, uint32_t max_tiles, cudaStream_t st);
+cudaError_t launch_batch_factor_round(const BatchParams& B, int kind, int factor, int robust, const BatchRound* round, uint32_t max_tiles, const uint32_t* vcorr,
+                                      const double* map_centres, const uint4* map_regions, const SubmapView& S, cudaStream_t st);
+cudaError_t launch_batch_segment_round(const BatchParams& B, const BatchRound* round, uint32_t n_members, double* out, cudaStream_t st);
+cudaError_t launch_batch_step_round(const AlignOptions& o, uint32_t n_members, const BatchRound* round, const double* out, MemberState* state, double* poses,
+                                    uint8_t* phase, cudaGraphConditionalHandle loop, cudaStream_t st);
+/// align_init of every member from its column-major initial pose: state, this call's pose and phase; seeded cleared unless keep_seeds
+cudaError_t launch_batch_align_init(const AlignOptions& o, uint32_t n_members, const double* init_T16, MemberState* state, double* poses, uint8_t* phase,
+                                    uint8_t* seeded, bool keep_seeds, cudaStream_t st);
+/// sgb_align_batch's outputs from the members' final state: T (16, column-major), info (converged, iterations, inliers, error), H | b (or null)
+cudaError_t launch_batch_align_finish(uint32_t n_members, const MemberState* state, double* out_T16, double* out_info4, double* out_Hb42, cudaStream_t st);
+
 }  // namespace sgb

@@ -85,6 +85,8 @@ void forget_linearisation(sgb_ctx* ctx) {
   ctx->have_lin = false;
   ctx->corr_seeds = false;
   ctx->b_view_ok = false;  // the target (or the pairing) it was built from may have changed
+  ctx->b_dseed_ok = false;
+  ctx->align_key.clear();  // sgb_align_batch_async rebuilds its loop graph
 }
 
 }  // namespace
@@ -634,6 +636,8 @@ void sgb_destroy(sgb_ctx* ctx) {
   if (ctx->ev_entry) cudaEventDestroy(ctx->ev_entry);
   for (int k = 0; k < sgb_ctx::kUploadChunks; k++)
     if (ctx->ev_upload[k]) cudaEventDestroy(ctx->ev_upload[k]);
+  if (ctx->align_exec) cudaGraphExecDestroy(ctx->align_exec);
+  if (ctx->cap_stream) cudaStreamDestroy(ctx->cap_stream);
   if (ctx->own_stream) cudaStreamDestroy(ctx->own_stream);
   delete ctx;  // every DevBuf member frees its allocation (the context's device is current)
 }
@@ -1071,6 +1075,7 @@ int sgb_num_inliers(sgb_ctx* ctx, size_t* n) {
 int sgb_drop_seeds(sgb_ctx* ctx) {
   if (!ctx) return 1;
   ctx->corr_seeds = false;
+  ctx->b_dseed_ok = false;
   return 0;
 }
 

@@ -1,6 +1,6 @@
 // SPDX-License-Identifier: MIT
 // C-ABI of batched registration (include/sgicp_b200.h: sgb_source_set_batch, sgb_source_set_pairs, sgb_source_set_submaps,
-// sgb_{linearize,error,align,correspondences}_batch).
+// sgb_{linearize,error,align,correspondences}_batch, sgb_align_batch_async).
 // Kernels in sgb_batch.cu (many kd-trees and submaps: the searches in sgb_forest.cu); DESIGN.md §11.
 #include <cuda_runtime.h>
 
@@ -317,6 +317,12 @@ int reserve_members(sgb_ctx* ctx) {
   CU(ctx->b_vq.reserve(nn * sizeof(float4)));
   CU(ctx->b_vcorr.reserve(nn * sizeof(uint32_t)));
   CU(cudaMemsetAsync(ctx->b_corr.p, 0xFF, nn * sizeof(uint32_t), ctx->stream));  // no correspondences before the first linearize
+  // sgb_align_batch_async: its per-member state, round descriptor and seed flags (cleared by its first call: b_dseed_ok)
+  CU(ctx->b_state.reserve(B * sizeof(MemberState)));
+  CU(ctx->b_phase.reserve(B));
+  CU(ctx->b_dseed.reserve(B));
+  CU(ctx->b_round.reserve(sizeof(BatchRound)));
+  ctx->b_dseed_ok = false;
   return reserve_query_scratch(ctx, nn);
 }
 
@@ -395,6 +401,215 @@ int pair_members(sgb_ctx* ctx, const char* who, size_t n_members, const uint32_t
   g.out_bounds = ctx->p_bounds.as<double>();
   CU(launch_pair_gather(g, ctx->sm_count, ctx->stream));
   ctx->launches += 1;
+  return 0;
+}
+
+// ---- sgb_align_batch_async (DESIGN.md §11 "Asynchronous align") ----
+
+// 0 one point target, 1 one voxel map, 2 many voxel maps, 3 many kd-trees, 4 submaps: the factor kernel family of launch_factor
+int factor_kind(const sgb_ctx* ctx) {
+  if (ctx->b_submaps) return 4;
+  if (ctx->tgt_state == TargetState::VoxelMaps) return 2;
+  if (ctx->tgt_state == TargetState::KdTrees) return 3;
+  return voxel_target(ctx) ? 1 : 0;
+}
+
+// the kernel parameters every round of the device loop shares (those of linearize_round; error() reads the same ones)
+void round_params(sgb_ctx* ctx, const sgb_align_options* o, LinParams& P, BatchParams& Bp) {
+  fill_params(ctx, P, kIdentity);
+  Bp = batch_params(ctx, P);
+  Bp.max_dist_sq_d = o->rejector_kind == SGB_REJECT_DISTANCE ? o->max_dist_sq : DBL_MAX;
+  Bp.robust_c = o->robust_c;
+}
+
+// The search of a point target over the virtual source in a round: launch_point_search with the query count read on the device.  The
+// counters do not alternate (a replayed graph cannot flip host state): the planner clears both pending counters, the class counters and
+// both queue counters at the head of every round.
+int point_search_round(sgb_ctx* ctx, const LinParams& P, const uint32_t* n_queries, int depth) {
+  const size_t n = P.src.n;
+  const int sgrid = one_wave_grid((n + 31) / 32 * 32, ctx->sm_count, packet_occupancy(depth));
+  const uint8_t* settled = nullptr;
+  const uint32_t* pending_count = nullptr;
+  ChunkClasses cc = {};
+  PendingParams pp = {};
+  if (ctx->grid_ready) {
+    GridParams g;
+    for (int a = 0; a < 3; a++) g.origin[a] = ctx->grid_origin[a];
+    g.inv_cell = ctx->grid_inv_cell;
+    g.settle_d2 = ctx->grid_settle_d2;
+    uint32_t* pbase = ctx->grid_pending.as<uint32_t>();
+    if (ctx->use_chunk_classes) {
+      const uint32_t nck = static_cast<uint32_t>((n + 31) / 32);
+      uint32_t* cbase = ctx->chunk_lists.as<uint32_t>();
+      cc.count = cbase;
+      cc.count_next = cbase + 4;
+      cc.lists = cbase + 8;
+      cc.n_chunks = nck;
+      const float cell = ctx->grid_cell;
+      cc.wide_r2 = ctx->class_wide_cells * ctx->class_wide_cells * cell * cell;
+      cc.mid_r2 = cell * cell;
+      cc.fallback_pct = ctx->class_fallback_pct;
+    }
+    CU(launch_grid_probe_round(P, n_queries, ctx->grid_pts.as<float4>(), ctx->grid_table.as<GridSlot>(), ctx->grid_capacity, g, ctx->grid_state.as<uint8_t>(), pbase,
+                               pbase + 2, ctx->grid_pending_q.as<float4>(), pbase + 1, cc, ctx->stream));
+    pp.list = pbase + 2;
+    pp.q = ctx->grid_pending_q.as<float4>();
+    pp.grid_pts = ctx->grid_pts.as<float4>();
+    pp.table = ctx->use_ring ? ctx->grid_table.as<GridSlot>() : nullptr;
+    pp.capacity = ctx->grid_capacity;
+    pp.g = g;
+    settled = ctx->grid_state.as<uint8_t>();
+    pending_count = pbase;
+  }
+  uint32_t* queue = ctx->use_packet_queue ? ctx->packet_queue.as<uint32_t>() : nullptr;
+  CU(launch_packet_search_round(P, n_queries, static_cast<uint32_t>(ctx->pending_div), ctx->tgt_pnodes.as<float4>(), sgrid, depth, settled, pending_count, queue,
+                                queue ? queue + 1 : nullptr, cc, pp, ctx->stream));
+  return 0;
+}
+
+// One round of the device loop on ctx->stream: planner, search, factor, per-member sums, step.  Every grid is sized for the worst case
+// (every tile, every point, every member); what the round does is read from b_round.
+int async_round(sgb_ctx* ctx, const sgb_align_options* o, const AlignOptions& ao, cudaGraphConditionalHandle loop) {
+  const size_t B = batch_members(ctx);
+  const uint32_t T = static_cast<uint32_t>(max_tiles(ctx));
+  const bool voxel = voxel_target(ctx), no_target = ctx->n_tgt == 0, point = !no_target && !voxel && !ctx->b_submaps && ctx->tgt_state != TargetState::KdTrees;
+  BatchRound* round = ctx->b_round.as<BatchRound>();
+  LinParams P;
+  BatchParams Bp;
+  round_params(ctx, o, P, Bp);
+  BatchPlan pl = {};
+  pl.n_members = static_cast<uint32_t>(B);
+  pl.member_off = (ctx->b_paired ? ctx->p_tables : ctx->b_cloud_off).as<uint32_t>();
+  pl.phase = ctx->b_phase.as<uint8_t>();
+  pl.seeded = ctx->b_dseed.as<uint8_t>();
+  pl.seeds = !voxel;
+  pl.no_target = no_target;
+  pl.tiles = ctx->b_tiles.as<BatchTile>();
+  pl.members = ctx->b_members.as<uint4>();
+  pl.round = round;
+  pl.loop = loop;
+  if (point) {
+    int k = 0;
+    if (ctx->grid_ready) {
+      pl.zero[k] = ctx->grid_pending.as<uint32_t>(), pl.zero_n[k++] = 2;
+      if (ctx->use_chunk_classes) pl.zero[k] = ctx->chunk_lists.as<uint32_t>(), pl.zero_n[k++] = 8;
+    }
+    if (ctx->use_packet_queue) pl.zero[k] = ctx->packet_queue.as<uint32_t>(), pl.zero_n[k++] = 2;
+  }
+  CU(launch_batch_plan(pl, ctx->stream));
+  const float bound = search_bound(o->rejector_kind, o->max_dist_sq);
+  uint32_t* vcorr = ctx->b_vcorr.as<uint32_t>();
+  if (no_target) {
+    CU(launch_batch_unmatch_round(Bp, round, T, ctx->stream));
+  } else if (ctx->b_submaps) {
+    CU(launch_submap_search_round(Bp, ctx->tgt_pnodes.as<float4>(), submap_view(ctx), round, T, ctx->kt_depth, bound, vcorr, ctx->stream));
+  } else if (ctx->tgt_state == TargetState::KdTrees) {
+    const bool view = paired_maps(ctx);
+    const uint32_t* tab = (view ? ctx->v_tables : ctx->kt_tables).as<uint32_t>();
+    const size_t M = view ? B : ctx->kt_maps;
+    const ForestView F{ctx->tgt_pnodes.as<float4>(), (view ? ctx->v_centres : ctx->kt_centres).as<double>(), tab, tab + (view ? M + 1 : 3 * (M + 1))};
+    CU(launch_forest_search_round(Bp, F, round, T, ctx->kt_depth, bound, vcorr, ctx->stream));
+  } else if (point) {
+    CU(launch_batch_transform_round(Bp, round, T, ctx->b_vq.as<float4>(), vcorr, ctx->stream));
+    LinParams Q = P;
+    Q.src.pts = ctx->b_vq.as<float4>();
+    Q.src.covA = Q.src.covB = nullptr;
+    Q.src.centre = ctx->tgt_centre.as<double>();
+    Q.src.n = static_cast<uint32_t>(batch_points(ctx));  // the most a round can have: the grids are sized for it
+    Q.src.run = 1;
+    Q.corr = vcorr;
+    Q.use_prev = 1;
+    Q.max_dist_sq = bound;
+    if (int rc = point_search_round(ctx, Q, &round->n_search, ctx->tree_depth > 0 ? ctx->tree_depth : 1)) return rc;
+  }
+  if (!no_target) {
+    const bool view = paired_maps(ctx);
+    const double* centres = nullptr;
+    const uint4* regions = nullptr;
+    if (ctx->tgt_state == TargetState::VoxelMaps) {
+      centres = (view ? ctx->v_centres : ctx->vm_centres).as<double>();
+      regions = (view ? ctx->v_regions : ctx->vm_regions).as<uint4>();
+    } else if (ctx->tgt_state == TargetState::KdTrees && !ctx->b_submaps) {
+      centres = (view ? ctx->v_centres : ctx->kt_centres).as<double>();
+    }
+    const SubmapView S = ctx->b_submaps ? submap_view(ctx) : SubmapView{};
+    CU(launch_batch_factor_round(Bp, factor_kind(ctx), o->factor_kind, o->robust_kind, round, T, vcorr, centres, regions, S, ctx->stream));
+  }
+  CU(launch_batch_segment_round(Bp, round, static_cast<uint32_t>(B), ctx->b_out.as<double>(), ctx->stream));
+  CU(launch_batch_step_round(ao, static_cast<uint32_t>(B), round, ctx->b_out.as<double>(), ctx->b_state.as<MemberState>(), ctx->b_poses.as<double>(),
+                             ctx->b_phase.as<uint8_t>(), loop, ctx->stream));
+  return 0;
+}
+
+// A WHILE node in g (after deps) whose body is one round, captured on the context's capture stream.  The condition starts at 1 at every
+// launch of g (every member starts in kPhaseLinearize when max_iterations > 0); the planner clears it and the step sets it again while a
+// member has a round to go.
+int add_loop(sgb_ctx* ctx, const sgb_align_options* o, const AlignOptions& ao, cudaGraph_t g, const std::vector<cudaGraphNode_t>& deps, cudaGraphNode_t* node) {
+  cudaGraphConditionalHandle h;
+  cudaError_t e = cudaGraphConditionalHandleCreate(&h, g, 1, cudaGraphCondAssignDefault);
+  if (e != cudaSuccess)
+    return fail(ctx, 2, std::string("sgb_align_batch_async: cudaGraphConditionalHandleCreate: ") + cudaGetErrorString(e) +
+                            " (the device loop needs conditional graph nodes: CUDA 12.4 or later, driver included)");
+  cudaGraphNodeParams np = {};
+  np.type = cudaGraphNodeTypeConditional;
+  np.conditional.handle = h;
+  np.conditional.type = cudaGraphCondTypeWhile;
+  np.conditional.size = 1;
+  CU(cudaGraphAddNode(node, g, deps.empty() ? nullptr : deps.data(), deps.size(), &np));
+  if (!ctx->cap_stream) CU(cudaStreamCreateWithFlags(&ctx->cap_stream, cudaStreamNonBlocking));
+  CU(cudaStreamBeginCaptureToGraph(ctx->cap_stream, np.conditional.phGraph_out[0], nullptr, nullptr, 0, cudaStreamCaptureModeRelaxed));
+  const cudaStream_t user = ctx->stream;
+  ctx->stream = ctx->cap_stream;
+  const int rc = async_round(ctx, o, ao, h);
+  ctx->stream = user;
+  cudaGraph_t body = nullptr;
+  e = cudaStreamEndCapture(ctx->cap_stream, &body);
+  if (rc) return rc;
+  CU(e);
+  return 0;
+}
+
+// Everything the cached loop graph captured: option values, sizes, the search configuration and every buffer address.
+template <typename T>
+void key_add(std::vector<unsigned char>& k, const T& v) {
+  const unsigned char* b = reinterpret_cast<const unsigned char*>(&v);
+  k.insert(k.end(), b, b + sizeof(T));
+}
+std::vector<unsigned char> loop_key(sgb_ctx* ctx, const sgb_align_options* o) {
+  std::vector<unsigned char> k;
+  for (int v : {o->factor_kind, o->robust_kind, o->rejector_kind, o->optimizer_kind, o->max_iterations, o->max_inner_iterations}) key_add(k, v);
+  for (double v : {o->robust_c, o->max_dist_sq, o->gn_lambda, o->init_lambda, o->lambda_factor, o->rotation_eps, o->translation_eps}) key_add(k, v);
+  for (int i = 0; i < 6; i++) key_add(k, o->dof_mask[i]);
+  LinParams P;
+  BatchParams Bp = {};
+  round_params(ctx, o, P, Bp);
+  key_add(k, P);
+  key_add(k, Bp);
+  for (size_t v : {batch_members(ctx), batch_points(ctx), ctx->n_tgt, ctx->kt_maps, ctx->vm_maps})
+    key_add(k, v);
+  for (int v : {static_cast<int>(ctx->tgt_state), static_cast<int>(ctx->b_submaps), static_cast<int>(ctx->b_paired), static_cast<int>(paired_maps(ctx)),
+                static_cast<int>(ctx->grid_ready), static_cast<int>(ctx->use_chunk_classes), static_cast<int>(ctx->use_packet_queue),
+                static_cast<int>(ctx->use_ring), ctx->pending_div, ctx->tree_depth, ctx->kt_depth, ctx->sm_count, static_cast<int>(ctx->grid_capacity),
+                static_cast<int>(ctx->class_fallback_pct)})
+    key_add(k, v);
+  for (float v : {ctx->grid_origin[0], ctx->grid_origin[1], ctx->grid_origin[2], ctx->grid_inv_cell, ctx->grid_settle_d2, ctx->grid_cell, ctx->class_wide_cells})
+    key_add(k, v);
+  for (const DevBuf* b : {&ctx->b_round, &ctx->b_dseed, &ctx->b_state, &ctx->b_phase, &ctx->b_vq, &ctx->b_vcorr, &ctx->b_out, &ctx->p_tables, &ctx->b_cloud_off,
+                          &ctx->grid_pts, &ctx->grid_table, &ctx->grid_state, &ctx->grid_pending, &ctx->grid_pending_q, &ctx->chunk_lists, &ctx->packet_queue,
+                          &ctx->tgt_pnodes, &ctx->kt_tables, &ctx->kt_centres, &ctx->vm_centres, &ctx->vm_regions, &ctx->v_tables, &ctx->v_centres,
+                          &ctx->v_regions, &ctx->s_tables, &ctx->s_entries, &ctx->s_centres, &ctx->b_centry})
+    key_add(k, b->p);
+  return k;
+}
+
+// p is device memory of the context's GPU (cudaPointerGetAttributes); what names it in the message
+int device_pointer(sgb_ctx* ctx, const void* p, const char* what) {
+  cudaPointerAttributes a = {};
+  const cudaError_t e = cudaPointerGetAttributes(&a, p);
+  if (e != cudaSuccess) cudaGetLastError();  // (not an error of the context: clear it)
+  if (e != cudaSuccess || a.type != cudaMemoryTypeDevice || a.device != ctx->device)
+    return fail(ctx, 1, std::string("sgb_align_batch_async: ") + what + " must be device memory of the context's GPU (cuda:" + std::to_string(ctx->device) +
+                            "); host, page-locked and managed memory are refused");
   return 0;
 }
 
@@ -652,6 +867,104 @@ int sgb_align_batch(sgb_ctx* ctx, const sgb_align_options* o, const double* init
       std::memcpy(out_Hb + 42 * m, s.H, 36 * sizeof(double));
       std::memcpy(out_Hb + 42 * m + 36, s.b, 6 * sizeof(double));
     }
+  }
+  return 0;
+}
+
+int sgb_align_batch_async(sgb_ctx* ctx, const sgb_align_options* o, const double* d_init_T, double* d_out_T, double* d_out_info, double* d_out_Hb) {
+  if (!ctx) return 1;
+  const char* who = "sgb_align_batch_async";
+  if (int rc = batch_check(ctx, who, d_init_T)) return rc;
+  if (!o) return fail(ctx, 1, std::string(who) + ": null options");
+  if (!d_out_T || !d_out_info) return fail(ctx, 1, std::string(who) + ": null output");
+  if (o->factor_kind < 0 || o->factor_kind > 2 || o->robust_kind < 0 || o->robust_kind > 2 || o->rejector_kind < 0 || o->rejector_kind > 1 ||
+      o->optimizer_kind < 0 || o->optimizer_kind > 1)
+    return fail(ctx, 1, std::string(who) + ": invalid factor/robust/rejector/optimizer kind");
+  if (int rc = submap_factor_check(ctx, who, o->factor_kind)) return rc;
+  const size_t B = batch_members(ctx);
+  if (B == 0) return 0;
+  if (batch_points(ctx) && ctx->n_tgt) {
+    if (int rc = check_target(ctx, who, o->factor_kind)) return rc;
+  }
+  CU(cudaSetDevice(ctx->device));
+  if (int rc = device_pointer(ctx, d_init_T, "init_T16xB")) return rc;
+  if (int rc = device_pointer(ctx, d_out_T, "out_T16xB")) return rc;
+  if (int rc = device_pointer(ctx, d_out_info, "out_info4xB")) return rc;
+  if (d_out_Hb) {
+    if (int rc = device_pointer(ctx, d_out_Hb, "out_Hb42xB")) return rc;
+  }
+  cudaStreamCaptureStatus capture = cudaStreamCaptureStatusNone;
+  CU(cudaStreamIsCapturing(ctx->stream, &capture));
+  if (capture == cudaStreamCaptureStatusInvalidated) return fail(ctx, 1, std::string(who) + ": the context's stream is in an invalidated capture");
+  const bool capturing = capture == cudaStreamCaptureStatusActive;
+  // nothing below allocates: a cudaMalloc may not run while the stream is captured (reserve_members sized everything for the batch)
+  if (ctx->use_packet_queue && !ctx->packet_queue.p) {
+    if (capturing) return fail(ctx, 1, std::string(who) + ": the first batched call of a context cannot be captured (it allocates); call it once before capturing");
+    CU(ctx->packet_queue.reserve(2 * sizeof(uint32_t)));
+    CU(cudaMemsetAsync(ctx->packet_queue.p, 0, 2 * sizeof(uint32_t), ctx->stream));
+  }
+  if (int rc = pair_view(ctx)) return rc;
+  AlignOptions ao;
+  ao.lm = o->optimizer_kind == SGB_OPT_LEVENBERG_MARQUARDT;
+  ao.max_iterations = o->max_iterations;
+  ao.max_inner_iterations = o->max_inner_iterations;
+  ao.gn_lambda = o->gn_lambda;
+  ao.init_lambda = o->init_lambda;
+  ao.lambda_factor = o->lambda_factor;
+  ao.rotation_eps = o->rotation_eps;
+  ao.translation_eps = o->translation_eps;
+  for (int i = 0; i < 6; i++) ao.dof_mask[i] = o->dof_mask[i];
+  const uint32_t nb = static_cast<uint32_t>(B);
+  // the device's seed flags are kept while the host's are valid (the same target, the cached correspondences not dropped)
+  CU(launch_batch_align_init(ao, nb, d_init_T, ctx->b_state.as<MemberState>(), ctx->b_poses.as<double>(), ctx->b_phase.as<uint8_t>(), ctx->b_dseed.as<uint8_t>(),
+                             ctx->corr_seeds && ctx->b_dseed_ok, ctx->stream));
+  ctx->launches += 2;  // the initial state here, the outputs below
+  if (o->max_iterations > 0) {
+    if (capturing) {
+      cudaGraph_t g = nullptr;
+      const cudaGraphNode_t* d = nullptr;
+      size_t nd = 0;
+      CU(cudaStreamGetCaptureInfo(ctx->stream, &capture, nullptr, &g, &d, &nd));
+      const std::vector<cudaGraphNode_t> deps(d, d + nd);
+      cudaGraphNode_t w = nullptr;
+      if (int rc = add_loop(ctx, o, ao, g, deps, &w)) return rc;
+      CU(cudaStreamUpdateCaptureDependencies(ctx->stream, &w, 1, cudaStreamSetCaptureDependencies));
+    } else {
+      std::vector<unsigned char> key = loop_key(ctx, o);
+      if (!ctx->align_exec || key != ctx->align_key) {
+        if (ctx->align_exec) cudaGraphExecDestroy(ctx->align_exec);
+        ctx->align_exec = nullptr;
+        ctx->align_key.clear();
+        cudaGraph_t g = nullptr;
+        CU(cudaGraphCreate(&g, 0));
+        cudaGraphNode_t w = nullptr;
+        const int rc = add_loop(ctx, o, ao, g, {}, &w);
+        const cudaError_t e = rc ? cudaSuccess : cudaGraphInstantiate(&ctx->align_exec, g, 0);
+        cudaGraphDestroy(g);
+        if (rc) return rc;
+        CU(e);
+        ctx->align_key.swap(key);
+      }
+      CU(cudaGraphLaunch(ctx->align_exec, ctx->stream));
+    }
+    ctx->launches += 1;
+    // the search counters are left cleared, as the synchronous calls expect them
+    if (ctx->grid_ready) {
+      CU(cudaMemsetAsync(ctx->grid_pending.p, 0, 2 * sizeof(uint32_t), ctx->stream));
+      if (ctx->use_chunk_classes) CU(cudaMemsetAsync(ctx->chunk_lists.p, 0, 8 * sizeof(uint32_t), ctx->stream));
+    }
+    if (ctx->use_packet_queue) CU(cudaMemsetAsync(ctx->packet_queue.p, 0, 2 * sizeof(uint32_t), ctx->stream));
+  }
+  CU(launch_batch_align_finish(nb, ctx->b_state.as<MemberState>(), d_out_T, d_out_info, d_out_Hb, ctx->stream));
+  ctx->b_dseed_ok = true;
+  if (o->max_iterations > 0) {  // round 1 linearised every member, as sgb_align_batch's does
+    std::fill(ctx->b_lin.begin(), ctx->b_lin.end(), 1);
+    std::fill(ctx->b_seeded.begin(), ctx->b_seeded.end(), 1);
+    ctx->have_lin = true;
+    ctx->corr_seeds = true;
+    ctx->lin_factor = o->factor_kind;
+    ctx->lin_robust = o->robust_kind;
+    ctx->lin_c = o->robust_c;
   }
   return 0;
 }

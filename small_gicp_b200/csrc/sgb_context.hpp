@@ -209,6 +209,13 @@ struct sgb_ctx {
   bool b_submaps = false;
   std::vector<uint32_t> b_sub_off, b_sub_maps;
   sgb::DevBuf s_tables, s_entries, s_centres, b_centry;
+  // sgb_align_batch_async: the round the planner made (BatchRound), the device's copy of b_seeded (b_dseed_ok: it never claims a seed
+  // the host's flags would not allow; cleared with them), the stream a round is captured on, and the instantiated loop with its key
+  sgb::DevBuf b_round, b_dseed;
+  bool b_dseed_ok = false;
+  cudaStream_t cap_stream = nullptr;
+  cudaGraphExec_t align_exec = nullptr;
+  std::vector<unsigned char> align_key;
 };
 
 namespace sgb {
