@@ -3,18 +3,19 @@
 //   batch_transform_kernel  member pose applied once per point: the FP32 query of every point of the active members (centred_query_f32,
 //                           as in the single-source search kernels), written as a "virtual source" (target-centred, identity pose) that
 //                           the single-source search kernels walk unchanged
-//   batch_factor_kernel     one CTA per 128-point tile of ONE member: FP64 rejector + factor (or error()) at that member's pose,
-//                           voxel-map probe for VGICP (vox_nearest, as in linearize_vox_kernel), CTA sum -> one partial per tile
-//   batch_maps_factor_kernel  the same for a multi-map voxel target: member m's tiles use map m's centre and table region
-//   batch_trees_factor_kernel the same for many kd-trees: member m's tiles use map m's centre and what the forest search found
+//   batch_factor_kernel     one CTA per 128-point tile of ONE member: FP64 rejector + factor (or error()) at that member's pose, CTA sum
+//                           -> one partial per tile.  Per target kind: the correspondence the search found (one point target, many
+//                           kd-trees with member m centred on map m), the voxel-map probe for VGICP (vox_nearest, as in
+//                           linearize_vox_kernel; many voxel maps: member m in map m's centre and table region), or submap members, each
+//                           point at the member's pose relative to the placement of the entry its correspondence lies in
 //   batch_segment_kernel    one CTA per member: its tiles' partials in tile order -> H|b|e|inliers (or e) of that member
 //   batch_step_kernel       batched align(): one thread per member, its Gauss-Newton / Levenberg-Marquardt step (sgb_math.cuh) after a
 //                           round, its next pose and phase
 //   pair_gather_kernel      sgb_source_set_pairs: every member's replica of its stored cloud, in one launch over all member points
 //   pair_view_kernel        the many-maps tables above seen through the pairing (member p -> map maps[p]), one CTA
-//   batch_submap_factor_kernel  batch_trees_factor_kernel for submap members (sgb_source_set_submaps): each point at the member's pose
-//                           relative to the placement of the entry its correspondence lies in, against that entry's map as stored
 //   submap_view_kernel      the per-entry tables of the submap lists from the target's per-map tables, one thread per entry
+// The transform, factor, segment and step kernels serve the rounds the host plans (sgb_{linearize,error,align}_batch) and, with ROUND /
+// kModeRound, the rounds batch_plan_kernel plans on the device (sgb_align_batch_async).
 // A member's sums depend on its own points, pose and correspondences only, added in an order fixed by its size: bit-identical whatever
 // else is in the batch.
 #include <algorithm>
@@ -67,8 +68,19 @@ __device__ __forceinline__ double tile_sum(const double* acc) {
   return v;
 }
 
-// (batch_transform_tile: the body of batch_transform_kernel and batch_transform_round_kernel)
-__device__ __forceinline__ void batch_transform_tile(const BatchParams& B, float4* vq, uint32_t* vcorr) {
+// What the factor and segment kernels compute: a linearize or an error() round planned on the host, or a round planned on the device
+// (either, as round->lin says).
+constexpr int kModeLinearize = 0, kModeError = 1, kModeRound = 2;
+
+// ROUND (every kernel below that has it): a round of sgb_align_batch_async, planned on the device -- the grid is sized for the worst
+// case, the round's size is read from `round`, and the CTAs beyond it exit at once.
+template <bool ROUND>
+__global__ void __launch_bounds__(kLinBlock) batch_transform_kernel(const __grid_constant__ BatchParams B, float4* vq, uint32_t* vcorr,
+                                                                    const BatchRound* __restrict__ round) {
+  if constexpr (ROUND) {
+    const BatchRound r = *round;
+    if (!r.lin || blockIdx.x >= r.n_tiles) return;
+  }
   const BatchTile t = B.tiles[blockIdx.x];
   const uint32_t tid = threadIdx.x;
   if (tid >= t.count) return;
@@ -80,10 +92,6 @@ __device__ __forceinline__ void batch_transform_tile(const BatchParams& B, float
   vq[v] = make_float4(f.x, f.y, f.z, 0.f);
   // the member's previous correspondence seeds the search (seeds only prune: the result does not depend on them)
   vcorr[v] = (B.members[t.member].z & kMemberSeeded) ? B.corr[i] : kNone;
-}
-
-__global__ void __launch_bounds__(kLinBlock) batch_transform_kernel(const __grid_constant__ BatchParams B, float4* vq, uint32_t* vcorr) {
-  batch_transform_tile(B, vq, vcorr);
 }
 
 // One tile of batch_factor_kernel.  ERR = false: linearize (VOX: voxel-map probe here; else vcorr = what the search found); ERR = true:
@@ -184,31 +192,25 @@ __device__ __forceinline__ void batch_factor_tile(const BatchParams& B, const ui
   if (tid < NACC) B.tile_partials[static_cast<size_t>(blockIdx.x) * kPartialStride + tid] = v;
 }
 
-template <int FACTOR, int ROBUST, bool VOX, bool ERR>
-__global__ void __launch_bounds__(kLinBlock, 4) batch_factor_kernel(const __grid_constant__ BatchParams B, const uint32_t* __restrict__ vcorr) {
-  batch_factor_tile<FACTOR, ROBUST, VOX, ERR, false>(B, vcorr, nullptr, nullptr);
-}
-
-// A multi-map voxel target (sgb_target_build_voxelmaps): member m against map m.  The per-map arrays are kernel arguments of their
-// own, so that BatchParams -- and with it the code of every other batch kernel -- stays as it is.
-template <int FACTOR, int ROBUST, bool ERR>
-__global__ void __launch_bounds__(kLinBlock, 4) batch_maps_factor_kernel(const __grid_constant__ BatchParams B, const double* __restrict__ map_centres,
-                                                                        const uint4* __restrict__ map_regions) {
-  batch_factor_tile<FACTOR, ROBUST, true, ERR, true>(B, nullptr, map_centres, map_regions);
-}
-
-// Many kd-trees (sgb_target_build_kdtrees): member m centred on map m's centre, vcorr = what forest_search_kernel found in map m.
-template <int FACTOR, int ROBUST, bool ERR>
-__global__ void __launch_bounds__(kLinBlock, 4) batch_trees_factor_kernel(const __grid_constant__ BatchParams B, const uint32_t* __restrict__ vcorr,
-                                                                         const double* __restrict__ map_centres) {
-  batch_factor_tile<FACTOR, ROBUST, false, ERR, true>(B, vcorr, map_centres, nullptr);
-}
-
-// Submap members (sgb_source_set_submaps) on many kd-trees: vcorr and S.centry = what submap_search_kernel found over the member's entries.
-template <int FACTOR, int ROBUST, bool ERR>
-__global__ void __launch_bounds__(kLinBlock, 4) batch_submap_factor_kernel(const __grid_constant__ BatchParams B, const uint32_t* __restrict__ vcorr,
-                                                                          const __grid_constant__ SubmapView S) {
-  batch_factor_tile<FACTOR, ROBUST, false, ERR, false, true>(B, vcorr, nullptr, nullptr, &S);  // MAPS = false: no per-member centre table is read
+// One CTA per tile of one member, for the target's KIND: 0 one point target, 1 one voxel map, 2 many voxel maps (member m against map m:
+// map_centres and map_regions), 3 many kd-trees (map_centres; vcorr = what forest_search_kernel found in map m), 4 submaps (S; vcorr and
+// S.centry = what submap_search_kernel found over the member's entries).  MODE: linearize, error() with the cached correspondences, or
+// either as the round's planner decided.
+template <int FACTOR, int ROBUST, int KIND, int MODE>
+__global__ void __launch_bounds__(kLinBlock, 4) batch_factor_kernel(const __grid_constant__ BatchParams B, const uint32_t* __restrict__ vcorr,
+                                                                   const double* __restrict__ map_centres, const uint4* __restrict__ map_regions,
+                                                                   const __grid_constant__ SubmapView S, const BatchRound* __restrict__ round) {
+  constexpr bool VOX = KIND == 1 || KIND == 2, MAPS = KIND == 2 || KIND == 3, SUB = KIND == 4;
+  bool lin = MODE == kModeLinearize;
+  if constexpr (MODE == kModeRound) {
+    const BatchRound r = *round;
+    if (blockIdx.x >= r.n_tiles) return;
+    lin = r.lin;
+  }
+  if (lin)
+    batch_factor_tile<FACTOR, ROBUST, VOX, false, MAPS, SUB>(B, vcorr, map_centres, map_regions, &S);
+  else
+    batch_factor_tile<FACTOR, ROBUST, VOX, true, MAPS, SUB>(B, nullptr, map_centres, map_regions, &S);
 }
 
 // One CTA per member: warp w adds tiles w, w + 8, ... of the member in order, then the 8 warp sums are added in warp order.  The order
@@ -241,9 +243,12 @@ __device__ __forceinline__ void batch_segment(const BatchParams& B, double* out)
   }
   if (LIN && (mem.z & kMemberActive) && threadIdx.x < 12) B.lin_poses[12 * static_cast<size_t>(m) + threadIdx.x] = B.poses[12 * static_cast<size_t>(m) + threadIdx.x];
 }
-template <int NACC, bool LIN>
-__global__ void __launch_bounds__(kSegWarps * 32) batch_segment_kernel(const __grid_constant__ BatchParams B, double* out) {
-  batch_segment<NACC, LIN>(B, out);
+template <int MODE>
+__global__ void __launch_bounds__(kSegWarps * 32) batch_segment_kernel(const __grid_constant__ BatchParams B, double* out, const BatchRound* __restrict__ round) {
+  if (MODE == kModeLinearize || (MODE == kModeRound && round->lin))
+    batch_segment<kAcc + 1, true>(B, out);
+  else
+    batch_segment<1, false>(B, out);
 }
 
 // One thread per member: the step is a sequential 6x6 solve and a few 4x4 products (about 2k FP64 operations), and at the 65536-member
@@ -265,17 +270,33 @@ __device__ __forceinline__ void batch_step_member(const AlignOptions& o, uint32_
   }
   phase[m] = static_cast<uint8_t>(s.phase);
 }
+// ROUND: the loop's condition becomes 1 if any member still has a round to go
+template <bool ROUND>
 __global__ void __launch_bounds__(kStepBlock) batch_step_kernel(const __grid_constant__ AlignOptions o, uint32_t n_members, bool linearize,
                                                                 const double* __restrict__ out, MemberState* __restrict__ state,
-                                                                double* __restrict__ poses, uint8_t* __restrict__ phase) {
+                                                                double* __restrict__ poses, uint8_t* __restrict__ phase, const BatchRound* __restrict__ round,
+                                                                cudaGraphConditionalHandle loop) {
   const uint32_t m = blockIdx.x * kStepBlock + threadIdx.x;
-  if (m >= n_members) return;
-  batch_step_member(o, m, linearize, out, state, poses, phase);
+  if constexpr (ROUND) {
+    int more = 0;
+    if (m < n_members) {
+      batch_step_member(o, m, round->lin != 0u, out, state, poses, phase);
+      more = phase[m] == kPhaseLinearize || phase[m] == kPhaseTrial;
+    }
+    if (__syncthreads_or(more) && threadIdx.x == 0) cudaGraphSetConditional(loop, 1u);
+  } else {
+    if (m >= n_members) return;
+    batch_step_member(o, m, linearize, out, state, poses, phase);
+  }
 }
 
-cudaError_t launch_batch_step(const AlignOptions& o, uint32_t n_members, bool linearize, const double* out, MemberState* state, double* poses,
-                              uint8_t* phase, cudaStream_t st) {
-  batch_step_kernel<<<(n_members + kStepBlock - 1) / kStepBlock, kStepBlock, 0, st>>>(o, n_members, linearize, out, state, poses, phase);
+cudaError_t launch_batch_step(const AlignOptions& o, uint32_t n_members, bool linearize, const BatchRound* round, cudaGraphConditionalHandle loop,
+                              const double* out, MemberState* state, double* poses, uint8_t* phase, cudaStream_t st) {
+  const uint32_t grid = (n_members + kStepBlock - 1) / kStepBlock;
+  if (round)
+    batch_step_kernel<true><<<grid, kStepBlock, 0, st>>>(o, n_members, linearize, out, state, poses, phase, round, loop);
+  else
+    batch_step_kernel<false><<<grid, kStepBlock, 0, st>>>(o, n_members, linearize, out, state, poses, phase, nullptr, loop);
   return cudaGetLastError();
 }
 
@@ -383,58 +404,39 @@ cudaError_t launch_pair_view(const PairView& v, cudaStream_t st) {
   return cudaGetLastError();
 }
 
-cudaError_t launch_batch_transform(const BatchParams& B, uint32_t n_tiles, float4* vq, uint32_t* vcorr, cudaStream_t st) {
-  batch_transform_kernel<<<n_tiles, kLinBlock, 0, st>>>(B, vq, vcorr);
+cudaError_t launch_batch_transform(const BatchParams& B, const BatchRound* round, uint32_t n_tiles, float4* vq, uint32_t* vcorr, cudaStream_t st) {
+  if (round)
+    batch_transform_kernel<true><<<n_tiles, kLinBlock, 0, st>>>(B, vq, vcorr, round);
+  else
+    batch_transform_kernel<false><<<n_tiles, kLinBlock, 0, st>>>(B, vq, vcorr, nullptr);
   return cudaGetLastError();
 }
 
-cudaError_t launch_batch_factor(const BatchParams& B, int factor, int robust, uint32_t n_tiles, bool voxel, bool err, const uint32_t* vcorr,
-                                cudaStream_t st) {
-  if (voxel && factor == 1 && !err) return cudaErrorInvalidValue;
-  return dispatch_factor_robust(factor, robust, cudaErrorInvalidValue, [&](auto f, auto r) {
-    if (err)
-      batch_factor_kernel<f, r, false, true><<<n_tiles, kLinBlock, 0, st>>>(B, vcorr);
-    else if (voxel)
-      batch_factor_kernel<(f == 1 ? 0 : f), r, true, false><<<n_tiles, kLinBlock, 0, st>>>(B, vcorr);
-    else
-      batch_factor_kernel<f, r, false, false><<<n_tiles, kLinBlock, 0, st>>>(B, vcorr);
-    return cudaGetLastError();
-  });
+// The factor kernel of one kind in one mode.  The kinds without point-to-plane (1, 2, 4: refused by the caller) compile FACTOR 1 as 0, one
+// instantiation fewer each.  error() reads the cached correspondences only, so the voxel kinds compute what the kinds with the same
+// centres compute there (1 -> 0, 2 -> 3).
+template <int F, int R, int MODE>
+auto factor_kernel(int kind) -> decltype(&batch_factor_kernel<0, 0, 0, kModeLinearize>) {
+  constexpr int G = F == 1 ? 0 : F;
+  switch (kind) {
+    case 0: return batch_factor_kernel<F, R, 0, MODE>;
+    case 1: if constexpr (MODE == kModeError) return batch_factor_kernel<G, R, 0, MODE>; else return batch_factor_kernel<G, R, 1, MODE>;
+    case 2: if constexpr (MODE == kModeError) return batch_factor_kernel<G, R, 3, MODE>; else return batch_factor_kernel<G, R, 2, MODE>;
+    case 3: return batch_factor_kernel<F, R, 3, MODE>;
+    case 4: return batch_factor_kernel<G, R, 4, MODE>;
+    default: return nullptr;
+  }
 }
 
-cudaError_t launch_batch_maps_factor(const BatchParams& B, int factor, int robust, uint32_t n_tiles, bool err, const double* map_centres,
-                                     const uint4* map_regions, cudaStream_t st) {
-  if (factor == 1) return cudaErrorInvalidValue;  // a voxel map has no normals
-  return dispatch_factor_robust(factor, robust, cudaErrorInvalidValue, [&](auto f, auto r) {
-    if (err)
-      batch_maps_factor_kernel<(f == 1 ? 0 : f), r, true><<<n_tiles, kLinBlock, 0, st>>>(B, map_centres, map_regions);
-    else
-      batch_maps_factor_kernel<(f == 1 ? 0 : f), r, false><<<n_tiles, kLinBlock, 0, st>>>(B, map_centres, map_regions);
-    return cudaGetLastError();
+cudaError_t launch_batch_factor(const BatchParams& B, int kind, int factor, int robust, bool err, const BatchRound* round, uint32_t n_tiles, const uint32_t* vcorr,
+                                const double* map_centres, const uint4* map_regions, const SubmapView& S, cudaStream_t st) {
+  if (factor == 1 && (kind == 1 || kind == 2 || kind == 4)) return cudaErrorInvalidValue;  // no normals in a voxel map; no point-to-plane against a union
+  const auto kernel = dispatch_factor_robust(factor, robust, decltype(&batch_factor_kernel<0, 0, 0, kModeLinearize>){}, [&](auto f, auto r) {
+    return round ? factor_kernel<f, r, kModeRound>(kind) : err ? factor_kernel<f, r, kModeError>(kind) : factor_kernel<f, r, kModeLinearize>(kind);
   });
-}
-
-cudaError_t launch_batch_trees_factor(const BatchParams& B, int factor, int robust, uint32_t n_tiles, bool err, const uint32_t* vcorr, const double* map_centres,
-                                      cudaStream_t st) {
-  return dispatch_factor_robust(factor, robust, cudaErrorInvalidValue, [&](auto f, auto r) {
-    if (err)
-      batch_trees_factor_kernel<f, r, true><<<n_tiles, kLinBlock, 0, st>>>(B, vcorr, map_centres);
-    else
-      batch_trees_factor_kernel<f, r, false><<<n_tiles, kLinBlock, 0, st>>>(B, vcorr, map_centres);
-    return cudaGetLastError();
-  });
-}
-
-cudaError_t launch_batch_submap_factor(const BatchParams& B, int factor, int robust, uint32_t n_tiles, bool err, const uint32_t* vcorr, const SubmapView& S,
-                                       cudaStream_t st) {
-  if (factor == 1) return cudaErrorInvalidValue;  // n o r is not invariant under a placement: no point-to-plane against a union
-  return dispatch_factor_robust(factor, robust, cudaErrorInvalidValue, [&](auto f, auto r) {
-    if (err)
-      batch_submap_factor_kernel<(f == 1 ? 0 : f), r, true><<<n_tiles, kLinBlock, 0, st>>>(B, vcorr, S);
-    else
-      batch_submap_factor_kernel<(f == 1 ? 0 : f), r, false><<<n_tiles, kLinBlock, 0, st>>>(B, vcorr, S);
-    return cudaGetLastError();
-  });
+  if (!kernel) return cudaErrorInvalidValue;
+  kernel<<<n_tiles, kLinBlock, 0, st>>>(B, vcorr, map_centres, map_regions, S, round);
+  return cudaGetLastError();
 }
 
 cudaError_t launch_submap_view(const SubmapViewBuild& v, int sm_count, cudaStream_t st) {
@@ -452,11 +454,13 @@ cudaError_t launch_submap_correspondences(const uint32_t* corr, const uint32_t* 
   return cudaGetLastError();
 }
 
-cudaError_t launch_batch_segment(const BatchParams& B, uint32_t n_members, bool linearize, double* out, cudaStream_t st) {
-  if (linearize)
-    batch_segment_kernel<kAcc + 1, true><<<n_members, kSegWarps * 32, 0, st>>>(B, out);
+cudaError_t launch_batch_segment(const BatchParams& B, uint32_t n_members, bool linearize, const BatchRound* round, double* out, cudaStream_t st) {
+  if (round)
+    batch_segment_kernel<kModeRound><<<n_members, kSegWarps * 32, 0, st>>>(B, out, round);
+  else if (linearize)
+    batch_segment_kernel<kModeLinearize><<<n_members, kSegWarps * 32, 0, st>>>(B, out, nullptr);
   else
-    batch_segment_kernel<1, false><<<n_members, kSegWarps * 32, 0, st>>>(B, out);
+    batch_segment_kernel<kModeError><<<n_members, kSegWarps * 32, 0, st>>>(B, out, nullptr);
   return cudaGetLastError();
 }
 
@@ -553,53 +557,11 @@ __global__ void __launch_bounds__(kPlanBlock) batch_plan_kernel(const BatchPlan 
   if (tid == 0) *p.round = BatchRound{lin ? 1u : 0u, p.no_target ? 0u : carry_t, lin && !p.no_target ? carry_v : 0u, lin && p.no_target ? carry_t : 0u};
 }
 
-__global__ void __launch_bounds__(kLinBlock) batch_transform_round_kernel(const __grid_constant__ BatchParams B, float4* vq, uint32_t* vcorr,
-                                                                          const BatchRound* __restrict__ round) {
-  const BatchRound r = *round;
-  if (!r.lin || blockIdx.x >= r.n_tiles) return;
-  batch_transform_tile(B, vq, vcorr);
-}
-
 // a linearize round against an empty target: every point of the active members is left without a correspondence
-__global__ void __launch_bounds__(kLinBlock) batch_unmatch_round_kernel(const __grid_constant__ BatchParams B, const BatchRound* __restrict__ round) {
+__global__ void __launch_bounds__(kLinBlock) batch_unmatch_kernel(const __grid_constant__ BatchParams B, const BatchRound* __restrict__ round) {
   if (blockIdx.x >= round->n_clear) return;
   const BatchTile t = B.tiles[blockIdx.x];
   if (threadIdx.x < t.count) B.corr[t.first + threadIdx.x] = kNone;
-}
-
-// The factor kernel of a round, linearize or error() as the planner decided, with the tile of the kernels launch_factor picks on the host
-// (KIND: 0 one point target, 1 one voxel map, 2 many voxel maps, 3 many kd-trees, 4 submaps).
-template <int FACTOR, int ROBUST, int KIND>
-__global__ void __launch_bounds__(kLinBlock, 4) batch_factor_round_kernel(const __grid_constant__ BatchParams B, const uint32_t* __restrict__ vcorr,
-                                                                         const double* __restrict__ map_centres, const uint4* __restrict__ map_regions,
-                                                                         const __grid_constant__ SubmapView S, const BatchRound* __restrict__ round) {
-  constexpr bool VOX = KIND == 1 || KIND == 2, MAPS = KIND == 2 || KIND == 3, SUB = KIND == 4;
-  const BatchRound r = *round;
-  if (blockIdx.x >= r.n_tiles) return;
-  if (r.lin)
-    batch_factor_tile<FACTOR, ROBUST, VOX, false, MAPS, SUB>(B, vcorr, map_centres, map_regions, &S);
-  else
-    batch_factor_tile<FACTOR, ROBUST, VOX, true, MAPS, SUB>(B, nullptr, map_centres, map_regions, &S);
-}
-
-__global__ void __launch_bounds__(kSegWarps * 32) batch_segment_round_kernel(const __grid_constant__ BatchParams B, double* out, const BatchRound* __restrict__ round) {
-  if (round->lin)
-    batch_segment<kAcc + 1, true>(B, out);
-  else
-    batch_segment<1, false>(B, out);
-}
-
-// the step of a round; the loop's condition becomes 1 if any member still has a round to go
-__global__ void __launch_bounds__(kStepBlock) batch_step_round_kernel(const __grid_constant__ AlignOptions o, uint32_t n_members, const BatchRound* __restrict__ round,
-                                                                      const double* __restrict__ out, MemberState* __restrict__ state,
-                                                                      double* __restrict__ poses, uint8_t* __restrict__ phase, cudaGraphConditionalHandle loop) {
-  const uint32_t m = blockIdx.x * kStepBlock + threadIdx.x;
-  int more = 0;
-  if (m < n_members) {
-    batch_step_member(o, m, round->lin != 0u, out, state, poses, phase);
-    more = phase[m] == kPhaseLinearize || phase[m] == kPhaseTrial;
-  }
-  if (__syncthreads_or(more) && threadIdx.x == 0) cudaGraphSetConditional(loop, 1u);
 }
 
 __global__ void __launch_bounds__(kStepBlock) batch_align_init_kernel(const __grid_constant__ AlignOptions o, uint32_t n_members, const double* __restrict__ init_T16,
@@ -641,41 +603,8 @@ cudaError_t launch_batch_plan(const BatchPlan& p, cudaStream_t st) {
   return cudaGetLastError();
 }
 
-cudaError_t launch_batch_transform_round(const BatchParams& B, const BatchRound* round, uint32_t max_tiles, float4* vq, uint32_t* vcorr, cudaStream_t st) {
-  batch_transform_round_kernel<<<max_tiles, kLinBlock, 0, st>>>(B, vq, vcorr, round);
-  return cudaGetLastError();
-}
-
-cudaError_t launch_batch_unmatch_round(const BatchParams& B, const BatchRound* round, uint32_t max_tiles, cudaStream_t st) {
-  batch_unmatch_round_kernel<<<max_tiles, kLinBlock, 0, st>>>(B, round);
-  return cudaGetLastError();
-}
-
-cudaError_t launch_batch_factor_round(const BatchParams& B, int kind, int factor, int robust, const BatchRound* round, uint32_t max_tiles, const uint32_t* vcorr,
-                                      const double* map_centres, const uint4* map_regions, const SubmapView& S, cudaStream_t st) {
-  if (factor == 1 && (kind == 1 || kind == 2 || kind == 4)) return cudaErrorInvalidValue;  // no normals in a voxel map; no point-to-plane against a union
-  return dispatch_factor_robust(factor, robust, cudaErrorInvalidValue, [&](auto f, auto r) {
-    constexpr int F = f == 1 ? 0 : f;  // (the kinds without point-to-plane: one instantiation fewer each)
-    switch (kind) {
-      case 0: batch_factor_round_kernel<f, r, 0><<<max_tiles, kLinBlock, 0, st>>>(B, vcorr, map_centres, map_regions, S, round); break;
-      case 1: batch_factor_round_kernel<F, r, 1><<<max_tiles, kLinBlock, 0, st>>>(B, vcorr, map_centres, map_regions, S, round); break;
-      case 2: batch_factor_round_kernel<F, r, 2><<<max_tiles, kLinBlock, 0, st>>>(B, vcorr, map_centres, map_regions, S, round); break;
-      case 3: batch_factor_round_kernel<f, r, 3><<<max_tiles, kLinBlock, 0, st>>>(B, vcorr, map_centres, map_regions, S, round); break;
-      case 4: batch_factor_round_kernel<F, r, 4><<<max_tiles, kLinBlock, 0, st>>>(B, vcorr, map_centres, map_regions, S, round); break;
-      default: return cudaErrorInvalidValue;
-    }
-    return cudaGetLastError();
-  });
-}
-
-cudaError_t launch_batch_segment_round(const BatchParams& B, const BatchRound* round, uint32_t n_members, double* out, cudaStream_t st) {
-  batch_segment_round_kernel<<<n_members, kSegWarps * 32, 0, st>>>(B, out, round);
-  return cudaGetLastError();
-}
-
-cudaError_t launch_batch_step_round(const AlignOptions& o, uint32_t n_members, const BatchRound* round, const double* out, MemberState* state, double* poses,
-                                    uint8_t* phase, cudaGraphConditionalHandle loop, cudaStream_t st) {
-  batch_step_round_kernel<<<(n_members + kStepBlock - 1) / kStepBlock, kStepBlock, 0, st>>>(o, n_members, round, out, state, poses, phase, loop);
+cudaError_t launch_batch_unmatch(const BatchParams& B, const BatchRound* round, uint32_t max_tiles, cudaStream_t st) {
+  batch_unmatch_kernel<<<max_tiles, kLinBlock, 0, st>>>(B, round);
   return cudaGetLastError();
 }
 

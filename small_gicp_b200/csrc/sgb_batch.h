@@ -32,16 +32,6 @@ struct BatchParams {
   double* tile_partials;  // [tiles][kPartialStride]
 };
 
-cudaError_t launch_batch_transform(const BatchParams& B, uint32_t n_tiles, float4* vq, uint32_t* vcorr, cudaStream_t st);
-cudaError_t launch_batch_factor(const BatchParams& B, int factor, int robust, uint32_t n_tiles, bool voxel, bool err, const uint32_t* vcorr, cudaStream_t st);
-/// The same over a multi-map voxel target (member m against map m): map_centres [maps][4], map_regions [maps] = (first table slot,
-/// mask, first voxel, voxel count) of each map (sgb_target_build_voxelmaps).  VGICP probe (err = false) or error() (err = true).
-cudaError_t launch_batch_maps_factor(const BatchParams& B, int factor, int robust, uint32_t n_tiles, bool err, const double* map_centres,
-                                     const uint4* map_regions, cudaStream_t st);
-/// The same over many kd-trees (member m against map m, sgb_target_build_kdtrees): map_centres [maps][4]; vcorr = the forest search's
-/// result over the call's virtual source (err = false) or unused (err = true).  ICP, point-to-plane or GICP.
-cudaError_t launch_batch_trees_factor(const BatchParams& B, int factor, int robust, uint32_t n_tiles, bool err, const uint32_t* vcorr, const double* map_centres,
-                                      cudaStream_t st);
 /// Members as (cloud, map) pairs (sgb_source_set_pairs): member p = a replica of stored cloud clouds[p], at member_off[p] .. member_off[p+1]
 /// of the member buffers; its centre and bounds too.  covA = null: no covariances.
 struct PairGather {
@@ -88,20 +78,9 @@ struct SubmapViewBuild {
   double* centres;
 };
 cudaError_t launch_submap_view(const SubmapViewBuild& v, int sm_count, cudaStream_t st);
-/// launch_batch_trees_factor for submap members: each point's correspondence is linearised (err = false; vcorr = what the submap search
-/// found) or re-evaluated (err = true) at the member's pose relative to the entry S.centry names.  ICP or GICP.
-cudaError_t launch_batch_submap_factor(const BatchParams& B, int factor, int robust, uint32_t n_tiles, bool err, const uint32_t* vcorr, const SubmapView& S,
-                                       cudaStream_t st);
 /// launch_correspondences for one submap member: out[perm[i]] = (entry << 32) | original index within the entry's map
 cudaError_t launch_submap_correspondences(const uint32_t* corr, const uint32_t* centry, const uint32_t* perm, size_t n, const float4* tgt_pts, uint64_t* out,
                                           int sm_count, cudaStream_t st);
-/// out: [members][44] (linearize) or [members] (error)
-cudaError_t launch_batch_segment(const BatchParams& B, uint32_t n_members, bool linearize, double* out, cudaStream_t st);
-/// batched align(): every member whose phase matches the round (linearize: kPhaseLinearize, else kPhaseTrial) takes its optimiser step
-/// from `out` (what launch_batch_segment wrote); then every member's next pose (row-major R | t) goes to poses and its phase to phase
-cudaError_t launch_batch_step(const AlignOptions& o, uint32_t n_members, bool linearize, const double* out, MemberState* state, double* poses,
-                              uint8_t* phase, cudaStream_t st);
-
 // ---- sgb_align_batch_async (DESIGN.md §11 "Asynchronous align"): the rounds planned and sized on the device ----
 /// What a round does, written by batch_plan_kernel at its head and read by every kernel of the round.  lin: 1 = linearize of the members
 /// in kPhaseLinearize, 0 = error() of the members in kPhaseTrial; n_tiles: tiles the factor kernel and the tile searches process;
@@ -126,16 +105,28 @@ struct BatchPlan {
   cudaGraphConditionalHandle loop;  // set to 0 here; the step kernel sets it to 1 while a member is still in a round
 };
 cudaError_t launch_batch_plan(const BatchPlan& p, cudaStream_t st);
-/// batch_transform_kernel / the factor kernel of the target's kind / batch_segment_kernel / batch_step_kernel in a planned round: the grids
-/// are sized for every tile (every member), the work is read from `round`, and the CTAs beyond it exit at once.  kind: 0 one point target,
-/// 1 one voxel map, 2 many voxel maps, 3 many kd-trees, 4 submaps.  The step kernel sets `loop` to 1 while a member is still in a round.
-cudaError_t launch_batch_transform_round(const BatchParams& B, const BatchRound* round, uint32_t max_tiles, float4* vq, uint32_t* vcorr, cudaStream_t st);
-cudaError_t launch_batch_unmatch_round(const BatchParams& B, const BatchRound* round, uint32_t max_tiles, cudaStream_t st);
-cudaError_t launch_batch_factor_round(const BatchParams& B, int kind, int factor, int robust, const BatchRound* round, uint32_t max_tiles, const uint32_t* vcorr,
-                                      const double* map_centres, const uint4* map_regions, const SubmapView& S, cudaStream_t st);
-cudaError_t launch_batch_segment_round(const BatchParams& B, const BatchRound* round, uint32_t n_members, double* out, cudaStream_t st);
-cudaError_t launch_batch_step_round(const AlignOptions& o, uint32_t n_members, const BatchRound* round, const double* out, MemberState* state, double* poses,
-                                    uint8_t* phase, cudaGraphConditionalHandle loop, cudaStream_t st);
+
+// ---- one launcher per step of a round.  round = null: a round planned on the host, with exact grids (n_tiles tiles of the call, n_members
+// members).  Else a round planned on the device (batch_plan_kernel): the grids are sized for every tile (n_tiles = the most a round can
+// have), what the round does is read from `round`, and the CTAs beyond it exit at once. ----
+/// The active members' queries as the virtual source of the point search (linearize rounds only)
+cudaError_t launch_batch_transform(const BatchParams& B, const BatchRound* round, uint32_t n_tiles, float4* vq, uint32_t* vcorr, cudaStream_t st);
+/// A linearize round against an empty target (planned on the device): every point of the active members is left without a correspondence
+cudaError_t launch_batch_unmatch(const BatchParams& B, const BatchRound* round, uint32_t n_tiles, cudaStream_t st);
+/// The factor kernel of the target's kind: 0 one point target (vcorr = the point search's result over the virtual source), 1 one voxel
+/// map (the VGICP probe), 2 many voxel maps (member m against map m: map_centres [maps][4], map_regions [maps] = (first table slot, mask,
+/// first voxel, voxel count) of each map), 3 many kd-trees (map_centres; vcorr = the forest search's result), 4 submaps (S; vcorr = the
+/// submap search's result).  Linearize (err = false), error() with the cached correspondences (err = true), or with a round what it
+/// says.  Point-to-plane only for kinds 0 and 3.
+cudaError_t launch_batch_factor(const BatchParams& B, int kind, int factor, int robust, bool err, const BatchRound* round, uint32_t n_tiles, const uint32_t* vcorr,
+                                const double* map_centres, const uint4* map_regions, const SubmapView& S, cudaStream_t st);
+/// out: [members][44] (linearize) or [members] (error)
+cudaError_t launch_batch_segment(const BatchParams& B, uint32_t n_members, bool linearize, const BatchRound* round, double* out, cudaStream_t st);
+/// batched align(): every member whose phase matches the round (linearize: kPhaseLinearize, else kPhaseTrial) takes its optimiser step
+/// from `out` (what launch_batch_segment wrote); then every member's next pose (row-major R | t) goes to poses and its phase to phase.
+/// With a round, the step sets `loop` to 1 while a member is still in a round.
+cudaError_t launch_batch_step(const AlignOptions& o, uint32_t n_members, bool linearize, const BatchRound* round, cudaGraphConditionalHandle loop,
+                              const double* out, MemberState* state, double* poses, uint8_t* phase, cudaStream_t st);
 /// align_init of every member from its column-major initial pose: state, this call's pose and phase; seeded cleared unless keep_seeds
 cudaError_t launch_batch_align_init(const AlignOptions& o, uint32_t n_members, const double* init_T16, MemberState* state, double* poses, uint8_t* phase,
                                     uint8_t* seeded, bool keep_seeds, cudaStream_t st);

@@ -382,6 +382,34 @@ int do_linearize_impl(sgb_ctx* ctx, int factor, int robust, double robust_c, int
 }
 }  // namespace
 
+// The grid front end's parameters for n queries (grid_ready, the buffers sized for them): the chunk class lists with the counters of
+// `parity`, and what the warp-per-query finish reads (pp.g: the cell grid of the probe).
+void sgb::point_search_params(const sgb_ctx* ctx, size_t n, int parity, ChunkClasses& cc, PendingParams& pp) {
+  GridParams g;
+  for (int a = 0; a < 3; a++) g.origin[a] = ctx->grid_origin[a];
+  g.inv_cell = ctx->grid_inv_cell;
+  g.settle_d2 = ctx->grid_settle_d2;
+  if (ctx->use_chunk_classes) {
+    // work lists of the packet search by cost class; two sets of counters alternate like the pending counters
+    uint32_t* cbase = ctx->chunk_lists.as<uint32_t>();
+    cc.count = cbase + 4 * parity;
+    cc.count_next = cbase + 4 * (parity ^ 1);
+    cc.lists = cbase + 8;
+    cc.n_chunks = static_cast<uint32_t>((n + 31) / 32);
+    const float cell = ctx->grid_cell;
+    cc.wide_r2 = ctx->class_wide_cells * ctx->class_wide_cells * cell * cell;  // search balls wider than two cells / one cell
+    cc.mid_r2 = cell * cell;
+    cc.fallback_pct = ctx->class_fallback_pct;
+  }
+  // the finishing kernel serves both regimes: few pending queries warp-per-query, many through the packet walk
+  pp.list = ctx->grid_pending.as<uint32_t>() + 2;
+  pp.q = ctx->grid_pending_q.as<float4>();
+  pp.grid_pts = ctx->grid_pts.as<float4>();
+  pp.table = ctx->use_ring ? ctx->grid_table.as<GridSlot>() : nullptr;
+  pp.capacity = ctx->grid_capacity;
+  pp.g = g;
+}
+
 // The search of a point target over P.src (P.src.n queries): grid probe, then the packet search / warp-per-query finish.  Fills P.corr.
 int sgb::launch_point_search(sgb_ctx* ctx, const LinParams& P, int depth) {
   const size_t n = P.src.n;
@@ -390,15 +418,9 @@ int sgb::launch_point_search(sgb_ctx* ctx, const LinParams& P, int depth) {
   const uint32_t* pending_count = nullptr;
   ChunkClasses cc = {};
   PendingParams pp = {};
-  // more pending queries than this: packet search over the chunk-ordered queries, else a warp per pending query
-  const uint32_t pending_split = static_cast<uint32_t>(n / static_cast<size_t>(ctx->pending_div));
   if (ctx->grid_ready) {
     // grid front end: settles every query whose nearest neighbour lies within half a cell (sgb_grid.cu)
     CU(ctx->grid_state.reserve(n));
-    GridParams g;
-    for (int a = 0; a < 3; a++) g.origin[a] = ctx->grid_origin[a];
-    g.inv_cell = ctx->grid_inv_cell;
-    g.settle_d2 = ctx->grid_settle_d2;
     // [0], [1]: two pending counters that alternate between calls (each probe clears the other one), [2..]: the list
     const void* before = ctx->grid_pending.p;
     CU(ctx->grid_pending.reserve((n + 2) * sizeof(uint32_t)));
@@ -406,42 +428,23 @@ int sgb::launch_point_search(sgb_ctx* ctx, const LinParams& P, int depth) {
       CU(cudaMemsetAsync(ctx->grid_pending.p, 0, 2 * sizeof(uint32_t), ctx->stream));
       ctx->pending_clean = true;
     }
-    uint32_t* pbase = ctx->grid_pending.as<uint32_t>();
-    uint32_t* pc = pbase + ctx->pending_parity;
-    uint32_t* plist = pbase + 2;
-    if (ctx->use_chunk_classes) {
-      // work lists of the packet search by cost class; counters alternate like the pending counters (sized in sgb_source_set_points)
-      const uint32_t nck = static_cast<uint32_t>((n + 31) / 32);
+    if (ctx->use_chunk_classes) {  // (sized in sgb_source_set_points)
       const void* cb = ctx->chunk_lists.p;
-      CU(ctx->chunk_lists.reserve((8 + static_cast<size_t>(kChunkClasses) * nck) * sizeof(uint32_t)));
+      CU(ctx->chunk_lists.reserve((8 + static_cast<size_t>(kChunkClasses) * ((n + 31) / 32)) * sizeof(uint32_t)));
       if (ctx->chunk_lists.p != cb || !ctx->chunk_lists_clean) {
         CU(cudaMemsetAsync(ctx->chunk_lists.p, 0, 8 * sizeof(uint32_t), ctx->stream));
         ctx->chunk_lists_clean = true;
       }
-      uint32_t* cbase = ctx->chunk_lists.as<uint32_t>();
-      cc.count = cbase + 4 * ctx->pending_parity;
-      cc.count_next = cbase + 4 * (ctx->pending_parity ^ 1);
-      cc.lists = cbase + 8;
-      cc.n_chunks = nck;
-      const float cell = ctx->grid_cell;
-      cc.wide_r2 = ctx->class_wide_cells * ctx->class_wide_cells * cell * cell;  // search balls wider than two cells / one cell
-      cc.mid_r2 = cell * cell;
-      cc.fallback_pct = ctx->class_fallback_pct;
     }
     CU(ctx->grid_pending_q.reserve(n * sizeof(float4)));
-    CU(launch_grid_probe(P, ctx->grid_pts.as<float4>(), ctx->grid_table.as<GridSlot>(), ctx->grid_capacity, g, ctx->grid_state.as<uint8_t>(), pc,
-                         plist, ctx->grid_pending_q.as<float4>(), pbase + (ctx->pending_parity ^ 1), cc, ctx->stream));
-    ctx->pending_parity ^= 1;
-    // the finishing kernel (below) serves both regimes: few pending queries warp-per-query, many through the packet walk
-    pp.list = plist;
-    pp.q = ctx->grid_pending_q.as<float4>();
-    pp.grid_pts = ctx->grid_pts.as<float4>();
-    pp.table = ctx->use_ring ? ctx->grid_table.as<GridSlot>() : nullptr;
-    pp.capacity = ctx->grid_capacity;
-    pp.g = g;
-    ctx->launches += 1;
+    point_search_params(ctx, n, ctx->pending_parity, cc, pp);
+    uint32_t* pbase = ctx->grid_pending.as<uint32_t>();
+    pending_count = pbase + ctx->pending_parity;
     settled = ctx->grid_state.as<uint8_t>();
-    pending_count = pc;
+    CU(launch_grid_probe(P, nullptr, ctx->grid_pts.as<float4>(), ctx->grid_table.as<GridSlot>(), ctx->grid_capacity, pp.g, ctx->grid_state.as<uint8_t>(),
+                         pbase + ctx->pending_parity, pbase + 2, ctx->grid_pending_q.as<float4>(), pbase + (ctx->pending_parity ^ 1), cc, ctx->stream));
+    ctx->pending_parity ^= 1;
+    ctx->launches += 1;
   }
   // many pending queries: the packet search walks the tree
   uint32_t *queue = nullptr, *queue_next = nullptr;
@@ -454,7 +457,8 @@ int sgb::launch_point_search(sgb_ctx* ctx, const LinParams& P, int depth) {
     queue_next = ctx->packet_queue.as<uint32_t>() + (ctx->packet_parity ^ 1);
     ctx->packet_parity ^= 1;
   }
-  CU(launch_packet_search(P, ctx->tgt_pnodes.as<float4>(), sgrid, depth, settled, pending_count, pending_split, queue, queue_next, cc, pp, ctx->tma_leaf, ctx->stream));
+  CU(launch_packet_search(P, nullptr, ctx->tgt_pnodes.as<float4>(), sgrid, depth, settled, pending_count, static_cast<uint32_t>(ctx->pending_div), queue, queue_next,
+                          cc, pp, ctx->tma_leaf, ctx->stream));
 #ifdef SGB_PROFILING
   if (ctx->debug_pending && pending_count) {  // profiling aid: synchronises
     uint32_t h = 0;

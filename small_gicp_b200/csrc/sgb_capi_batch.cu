@@ -97,19 +97,6 @@ SubmapView submap_view(const sgb_ctx* ctx) {
 
 bool voxel_target(const sgb_ctx* ctx) { return ctx->tgt_state == TargetState::VoxelMap || ctx->tgt_state == TargetState::VoxelMaps; }
 
-// the factor kernel of one round over the target's kind: one voxel map or a point target (launch_batch_factor), or many maps / trees
-// (with a pairing's map table: the member-indexed view of the maps instead of the map-indexed tables)
-cudaError_t launch_factor(sgb_ctx* ctx, const BatchParams& Bp, int factor, int robust, uint32_t n_tiles, bool err, const uint32_t* vcorr) {
-  const bool view = paired_maps(ctx);
-  if (ctx->b_submaps) return launch_batch_submap_factor(Bp, factor, robust, n_tiles, err, vcorr, submap_view(ctx), ctx->stream);
-  if (ctx->tgt_state == TargetState::VoxelMaps)
-    return launch_batch_maps_factor(Bp, factor, robust, n_tiles, err, (view ? ctx->v_centres : ctx->vm_centres).as<double>(),
-                                    (view ? ctx->v_regions : ctx->vm_regions).as<uint4>(), ctx->stream);
-  if (ctx->tgt_state == TargetState::KdTrees)
-    return launch_batch_trees_factor(Bp, factor, robust, n_tiles, err, vcorr, (view ? ctx->v_centres : ctx->kt_centres).as<double>(), ctx->stream);
-  return launch_batch_factor(Bp, factor, robust, n_tiles, voxel_target(ctx), err, vcorr, ctx->stream);
-}
-
 // Builds the pairing's view of the current target (one launch) unless it is up to date: forget_linearisation, which every target
 // transition and every pairing goes through, marks it stale.
 int pair_view(sgb_ctx* ctx) {
@@ -206,6 +193,87 @@ int copy_out(sgb_ctx* ctx, double* out, size_t doubles) {
   return 0;
 }
 
+// The search of a point target over the virtual source in a round planned on the device: launch_point_search with the query count read on
+// the device.  The counters do not alternate (a replayed graph cannot flip host state): the planner clears both pending counters, the
+// class counters and both queue counters at the head of every round.
+int point_search_round(sgb_ctx* ctx, const LinParams& P, const uint32_t* n_queries, int depth) {
+  const size_t n = P.src.n;
+  const int sgrid = one_wave_grid((n + 31) / 32 * 32, ctx->sm_count, packet_occupancy(depth));
+  const uint8_t* settled = nullptr;
+  const uint32_t* pending_count = nullptr;
+  ChunkClasses cc = {};
+  PendingParams pp = {};
+  if (ctx->grid_ready) {
+    point_search_params(ctx, n, 0, cc, pp);
+    uint32_t* pbase = ctx->grid_pending.as<uint32_t>();
+    settled = ctx->grid_state.as<uint8_t>();
+    pending_count = pbase;
+    CU(launch_grid_probe(P, n_queries, ctx->grid_pts.as<float4>(), ctx->grid_table.as<GridSlot>(), ctx->grid_capacity, pp.g, ctx->grid_state.as<uint8_t>(), pbase,
+                         pbase + 2, ctx->grid_pending_q.as<float4>(), pbase + 1, cc, ctx->stream));
+  }
+  uint32_t* queue = ctx->use_packet_queue ? ctx->packet_queue.as<uint32_t>() : nullptr;
+  CU(launch_packet_search(P, n_queries, ctx->tgt_pnodes.as<float4>(), sgrid, depth, settled, pending_count, static_cast<uint32_t>(ctx->pending_div), queue,
+                          queue ? queue + 1 : nullptr, cc, pp, false, ctx->stream));
+  return 0;
+}
+
+// The search and the factor kernel of one round against the current (non-empty) target, for its kind.  round = null: a round planned on
+// the host -- exact grids of n_tiles tiles and n_virtual queries, a linearize or (err) an error() round -- counted per launch; else a round
+// planned on the device (err = false), its grids sized for every tile (n_tiles = max_tiles) and point (n_virtual = batch_points), counted
+// with the graph that holds it.  P: the target's parameters (fill_params at the identity); bound: the FP32 search bound.
+int round_kernels(sgb_ctx* ctx, const LinParams& P, const BatchParams& Bp, const BatchRound* round, uint32_t n_tiles, uint32_t n_virtual, bool err, int factor,
+                  int robust, float bound) {
+  const int counted = round ? 0 : 1;
+  // the per-map tables: with a pairing's map table the member-indexed view of the maps, else the map-indexed tables
+  const bool view = paired_maps(ctx);
+  const double* centres = nullptr;
+  const uint4* regions = nullptr;
+  int kind = voxel_target(ctx) ? 1 : 0;
+  if (ctx->b_submaps) {
+    kind = 4;
+  } else if (ctx->tgt_state == TargetState::VoxelMaps) {
+    kind = 2;
+    centres = (view ? ctx->v_centres : ctx->vm_centres).as<double>();
+    regions = (view ? ctx->v_regions : ctx->vm_regions).as<uint4>();
+  } else if (ctx->tgt_state == TargetState::KdTrees) {
+    kind = 3;
+    centres = (view ? ctx->v_centres : ctx->kt_centres).as<double>();
+  }
+  const SubmapView S = ctx->b_submaps ? submap_view(ctx) : SubmapView{};
+  uint32_t* vcorr = ctx->b_vcorr.as<uint32_t>();
+  if (!err && kind == 4) {
+    // submaps: every tile searched in the trees of its member's entries, each in its own stored frame (sgb_forest.cu)
+    CU(launch_submap_search(Bp, ctx->tgt_pnodes.as<float4>(), S, round, n_tiles, ctx->kt_depth, bound, vcorr, ctx->stream));
+    ctx->launches += counted;
+  } else if (!err && kind == 3) {
+    // many trees: every tile searched in its member's own tree, straight from the stored points at the member's pose (sgb_forest.cu)
+    const uint32_t* tab = (view ? ctx->v_tables : ctx->kt_tables).as<uint32_t>();
+    const size_t M = view ? batch_members(ctx) : ctx->kt_maps;
+    const ForestView F{ctx->tgt_pnodes.as<float4>(), centres, tab, tab + (view ? M + 1 : 3 * (M + 1))};
+    CU(launch_forest_search(Bp, F, round, n_tiles, ctx->kt_depth, bound, vcorr, ctx->stream));
+    ctx->launches += counted;
+  } else if (!err && kind == 0) {
+    // the search runs over the virtual source: the active members' queries, already transformed into the target's frame
+    CU(launch_batch_transform(Bp, round, n_tiles, ctx->b_vq.as<float4>(), vcorr, ctx->stream));
+    ctx->launches += counted;
+    LinParams Q = P;
+    Q.src.pts = ctx->b_vq.as<float4>();
+    Q.src.covA = Q.src.covB = nullptr;
+    Q.src.centre = ctx->tgt_centre.as<double>();  // identity pose, source centre = target centre: the search takes the stored query as is
+    Q.src.n = n_virtual;
+    Q.src.run = 1;
+    Q.corr = vcorr;
+    Q.use_prev = 1;  // per member: its previous correspondences, or kNone
+    Q.max_dist_sq = bound;
+    const int depth = ctx->tree_depth > 0 ? ctx->tree_depth : 1;
+    if (int rc = round ? point_search_round(ctx, Q, &round->n_search, depth) : launch_point_search(ctx, Q, depth)) return rc;
+    ctx->launches += counted;
+  }
+  CU(launch_batch_factor(Bp, kind, factor, robust, err, round, n_tiles, err ? nullptr : vcorr, centres, regions, S, ctx->stream));
+  ctx->launches += counted;
+  return 0;
+}
+
 // One linearize of the active members (arguments checked by the caller) into b_out, asynchronous.  T = nullptr: poses already in b_poses.
 int linearize_round(sgb_ctx* ctx, int factor, int robust, double robust_c, int rejector, double max_dist_sq, const double* T, const uint8_t* active) {
   const size_t B = batch_members(ctx);
@@ -231,39 +299,10 @@ int linearize_round(sgb_ctx* ctx, int factor, int robust, double robust_c, int r
     for (size_t m = 0; m < B; m++) none[m].z = (!active || active[m]) ? kMemberActive : 0u;
     CU(cudaMemcpyAsync(ctx->b_members.p, none.data(), B * sizeof(uint4), cudaMemcpyHostToDevice, ctx->stream));
   }
-  if (n_tiles && ctx->b_submaps) {
-    // submaps: every tile searched in the trees of its member's entries, each in its own stored frame (sgb_forest.cu)
-    CU(launch_submap_search(Bp, ctx->tgt_pnodes.as<float4>(), submap_view(ctx), n_tiles, ctx->kt_depth, search_bound(rejector, max_dist_sq),
-                            ctx->b_vcorr.as<uint32_t>(), ctx->stream));
-    ctx->launches += 1;
-  } else if (n_tiles && ctx->tgt_state == TargetState::KdTrees) {
-    // many trees: every tile searched in its member's own tree, straight from the stored points at the member's pose (sgb_forest.cu)
-    const bool view = paired_maps(ctx);
-    const uint32_t* tab = (view ? ctx->v_tables : ctx->kt_tables).as<uint32_t>();
-    const size_t M = view ? B : ctx->kt_maps;
-    const ForestView F{ctx->tgt_pnodes.as<float4>(), (view ? ctx->v_centres : ctx->kt_centres).as<double>(), tab, tab + (view ? M + 1 : 3 * (M + 1))};
-    CU(launch_forest_search(Bp, F, n_tiles, ctx->kt_depth, search_bound(rejector, max_dist_sq), ctx->b_vcorr.as<uint32_t>(), ctx->stream));
-    ctx->launches += 1;
-  } else if (n_tiles && !voxel) {
-    // the search runs over the virtual source: the active members' queries, already transformed into the target's frame
-    CU(launch_batch_transform(Bp, n_tiles, ctx->b_vq.as<float4>(), ctx->b_vcorr.as<uint32_t>(), ctx->stream));
-    ctx->launches += 1;
-    P.src.pts = ctx->b_vq.as<float4>();
-    P.src.covA = P.src.covB = nullptr;
-    P.src.centre = ctx->tgt_centre.as<double>();  // identity pose, source centre = target centre: the search takes the stored query as is
-    P.src.n = n_virtual;
-    P.src.run = 1;
-    P.corr = ctx->b_vcorr.as<uint32_t>();
-    P.use_prev = 1;  // per member: its previous correspondences, or kNone
-    P.max_dist_sq = search_bound(rejector, max_dist_sq);
-    if (int rc = launch_point_search(ctx, P, ctx->tree_depth > 0 ? ctx->tree_depth : 1)) return rc;
-    ctx->launches += 1;
-  }
   if (n_tiles) {
-    CU(launch_factor(ctx, Bp, factor, robust, n_tiles, false, ctx->b_vcorr.as<uint32_t>()));
-    ctx->launches += 1;
+    if (int rc = round_kernels(ctx, P, Bp, nullptr, n_tiles, n_virtual, false, factor, robust, search_bound(rejector, max_dist_sq))) return rc;
   }
-  CU(launch_batch_segment(Bp, static_cast<uint32_t>(B), true, ctx->b_out.as<double>(), ctx->stream));
+  CU(launch_batch_segment(Bp, static_cast<uint32_t>(B), true, nullptr, ctx->b_out.as<double>(), ctx->stream));
   ctx->launches += 1;
   for (size_t m = 0; m < B; m++) {
     if (active && !active[m]) continue;
@@ -289,14 +328,13 @@ int error_round(sgb_ctx* ctx, const double* T, const uint8_t* active) {
   BatchParams Bp = batch_params(ctx, P);
   Bp.robust_c = ctx->lin_c;
   if (n_tiles && ctx->n_tgt) {
-    CU(launch_factor(ctx, Bp, ctx->lin_factor, ctx->lin_robust, n_tiles, true, nullptr));
-    ctx->launches += 1;
+    if (int rc = round_kernels(ctx, P, Bp, nullptr, n_tiles, 0, true, ctx->lin_factor, ctx->lin_robust, 0.f)) return rc;
   } else {
     n_tiles = 0;
     std::vector<uint4> none(B, make_uint4(0, 0, 0, 0));
     CU(cudaMemcpyAsync(ctx->b_members.p, none.data(), B * sizeof(uint4), cudaMemcpyHostToDevice, ctx->stream));
   }
-  CU(launch_batch_segment(Bp, static_cast<uint32_t>(B), false, ctx->b_out.as<double>(), ctx->stream));
+  CU(launch_batch_segment(Bp, static_cast<uint32_t>(B), false, nullptr, ctx->b_out.as<double>(), ctx->stream));
   ctx->launches += 1;
   return 0;
 }
@@ -406,65 +444,12 @@ int pair_members(sgb_ctx* ctx, const char* who, size_t n_members, const uint32_t
 
 // ---- sgb_align_batch_async (DESIGN.md §11 "Asynchronous align") ----
 
-// 0 one point target, 1 one voxel map, 2 many voxel maps, 3 many kd-trees, 4 submaps: the factor kernel family of launch_factor
-int factor_kind(const sgb_ctx* ctx) {
-  if (ctx->b_submaps) return 4;
-  if (ctx->tgt_state == TargetState::VoxelMaps) return 2;
-  if (ctx->tgt_state == TargetState::KdTrees) return 3;
-  return voxel_target(ctx) ? 1 : 0;
-}
-
 // the kernel parameters every round of the device loop shares (those of linearize_round; error() reads the same ones)
 void round_params(sgb_ctx* ctx, const sgb_align_options* o, LinParams& P, BatchParams& Bp) {
   fill_params(ctx, P, kIdentity);
   Bp = batch_params(ctx, P);
   Bp.max_dist_sq_d = o->rejector_kind == SGB_REJECT_DISTANCE ? o->max_dist_sq : DBL_MAX;
   Bp.robust_c = o->robust_c;
-}
-
-// The search of a point target over the virtual source in a round: launch_point_search with the query count read on the device.  The
-// counters do not alternate (a replayed graph cannot flip host state): the planner clears both pending counters, the class counters and
-// both queue counters at the head of every round.
-int point_search_round(sgb_ctx* ctx, const LinParams& P, const uint32_t* n_queries, int depth) {
-  const size_t n = P.src.n;
-  const int sgrid = one_wave_grid((n + 31) / 32 * 32, ctx->sm_count, packet_occupancy(depth));
-  const uint8_t* settled = nullptr;
-  const uint32_t* pending_count = nullptr;
-  ChunkClasses cc = {};
-  PendingParams pp = {};
-  if (ctx->grid_ready) {
-    GridParams g;
-    for (int a = 0; a < 3; a++) g.origin[a] = ctx->grid_origin[a];
-    g.inv_cell = ctx->grid_inv_cell;
-    g.settle_d2 = ctx->grid_settle_d2;
-    uint32_t* pbase = ctx->grid_pending.as<uint32_t>();
-    if (ctx->use_chunk_classes) {
-      const uint32_t nck = static_cast<uint32_t>((n + 31) / 32);
-      uint32_t* cbase = ctx->chunk_lists.as<uint32_t>();
-      cc.count = cbase;
-      cc.count_next = cbase + 4;
-      cc.lists = cbase + 8;
-      cc.n_chunks = nck;
-      const float cell = ctx->grid_cell;
-      cc.wide_r2 = ctx->class_wide_cells * ctx->class_wide_cells * cell * cell;
-      cc.mid_r2 = cell * cell;
-      cc.fallback_pct = ctx->class_fallback_pct;
-    }
-    CU(launch_grid_probe_round(P, n_queries, ctx->grid_pts.as<float4>(), ctx->grid_table.as<GridSlot>(), ctx->grid_capacity, g, ctx->grid_state.as<uint8_t>(), pbase,
-                               pbase + 2, ctx->grid_pending_q.as<float4>(), pbase + 1, cc, ctx->stream));
-    pp.list = pbase + 2;
-    pp.q = ctx->grid_pending_q.as<float4>();
-    pp.grid_pts = ctx->grid_pts.as<float4>();
-    pp.table = ctx->use_ring ? ctx->grid_table.as<GridSlot>() : nullptr;
-    pp.capacity = ctx->grid_capacity;
-    pp.g = g;
-    settled = ctx->grid_state.as<uint8_t>();
-    pending_count = pbase;
-  }
-  uint32_t* queue = ctx->use_packet_queue ? ctx->packet_queue.as<uint32_t>() : nullptr;
-  CU(launch_packet_search_round(P, n_queries, static_cast<uint32_t>(ctx->pending_div), ctx->tgt_pnodes.as<float4>(), sgrid, depth, settled, pending_count, queue,
-                                queue ? queue + 1 : nullptr, cc, pp, ctx->stream));
-  return 0;
 }
 
 // One round of the device loop on ctx->stream: planner, search, factor, per-member sums, step.  Every grid is sized for the worst case
@@ -497,47 +482,15 @@ int async_round(sgb_ctx* ctx, const sgb_align_options* o, const AlignOptions& ao
     if (ctx->use_packet_queue) pl.zero[k] = ctx->packet_queue.as<uint32_t>(), pl.zero_n[k++] = 2;
   }
   CU(launch_batch_plan(pl, ctx->stream));
-  const float bound = search_bound(o->rejector_kind, o->max_dist_sq);
-  uint32_t* vcorr = ctx->b_vcorr.as<uint32_t>();
   if (no_target) {
-    CU(launch_batch_unmatch_round(Bp, round, T, ctx->stream));
-  } else if (ctx->b_submaps) {
-    CU(launch_submap_search_round(Bp, ctx->tgt_pnodes.as<float4>(), submap_view(ctx), round, T, ctx->kt_depth, bound, vcorr, ctx->stream));
-  } else if (ctx->tgt_state == TargetState::KdTrees) {
-    const bool view = paired_maps(ctx);
-    const uint32_t* tab = (view ? ctx->v_tables : ctx->kt_tables).as<uint32_t>();
-    const size_t M = view ? B : ctx->kt_maps;
-    const ForestView F{ctx->tgt_pnodes.as<float4>(), (view ? ctx->v_centres : ctx->kt_centres).as<double>(), tab, tab + (view ? M + 1 : 3 * (M + 1))};
-    CU(launch_forest_search_round(Bp, F, round, T, ctx->kt_depth, bound, vcorr, ctx->stream));
-  } else if (point) {
-    CU(launch_batch_transform_round(Bp, round, T, ctx->b_vq.as<float4>(), vcorr, ctx->stream));
-    LinParams Q = P;
-    Q.src.pts = ctx->b_vq.as<float4>();
-    Q.src.covA = Q.src.covB = nullptr;
-    Q.src.centre = ctx->tgt_centre.as<double>();
-    Q.src.n = static_cast<uint32_t>(batch_points(ctx));  // the most a round can have: the grids are sized for it
-    Q.src.run = 1;
-    Q.corr = vcorr;
-    Q.use_prev = 1;
-    Q.max_dist_sq = bound;
-    if (int rc = point_search_round(ctx, Q, &round->n_search, ctx->tree_depth > 0 ? ctx->tree_depth : 1)) return rc;
+    CU(launch_batch_unmatch(Bp, round, T, ctx->stream));
+  } else if (int rc = round_kernels(ctx, P, Bp, round, T, static_cast<uint32_t>(batch_points(ctx)), false, o->factor_kind, o->robust_kind,
+                                    search_bound(o->rejector_kind, o->max_dist_sq))) {
+    return rc;
   }
-  if (!no_target) {
-    const bool view = paired_maps(ctx);
-    const double* centres = nullptr;
-    const uint4* regions = nullptr;
-    if (ctx->tgt_state == TargetState::VoxelMaps) {
-      centres = (view ? ctx->v_centres : ctx->vm_centres).as<double>();
-      regions = (view ? ctx->v_regions : ctx->vm_regions).as<uint4>();
-    } else if (ctx->tgt_state == TargetState::KdTrees && !ctx->b_submaps) {
-      centres = (view ? ctx->v_centres : ctx->kt_centres).as<double>();
-    }
-    const SubmapView S = ctx->b_submaps ? submap_view(ctx) : SubmapView{};
-    CU(launch_batch_factor_round(Bp, factor_kind(ctx), o->factor_kind, o->robust_kind, round, T, vcorr, centres, regions, S, ctx->stream));
-  }
-  CU(launch_batch_segment_round(Bp, round, static_cast<uint32_t>(B), ctx->b_out.as<double>(), ctx->stream));
-  CU(launch_batch_step_round(ao, static_cast<uint32_t>(B), round, ctx->b_out.as<double>(), ctx->b_state.as<MemberState>(), ctx->b_poses.as<double>(),
-                             ctx->b_phase.as<uint8_t>(), loop, ctx->stream));
+  CU(launch_batch_segment(Bp, static_cast<uint32_t>(B), true, round, ctx->b_out.as<double>(), ctx->stream));
+  CU(launch_batch_step(ao, static_cast<uint32_t>(B), true, round, loop, ctx->b_out.as<double>(), ctx->b_state.as<MemberState>(), ctx->b_poses.as<double>(),
+                       ctx->b_phase.as<uint8_t>(), ctx->stream));
   return 0;
 }
 
@@ -610,6 +563,31 @@ int device_pointer(sgb_ctx* ctx, const void* p, const char* what) {
   if (e != cudaSuccess || a.type != cudaMemoryTypeDevice || a.device != ctx->device)
     return fail(ctx, 1, std::string("sgb_align_batch_async: ") + what + " must be device memory of the context's GPU (cuda:" + std::to_string(ctx->device) +
                             "); host, page-locked and managed memory are refused");
+  return 0;
+}
+
+// The checks both align calls make before anything is launched (who names the caller), and the options of the optimiser's step
+int align_checks(sgb_ctx* ctx, const char* who, const sgb_align_options* o, const double* init_T, const double* out_T, const double* out_info,
+                 AlignOptions& ao) {
+  if (int rc = batch_check(ctx, who, init_T)) return rc;
+  if (!o) return fail(ctx, 1, std::string(who) + ": null options");
+  if (!out_T || !out_info) return fail(ctx, 1, std::string(who) + ": null output");
+  if (o->factor_kind < 0 || o->factor_kind > 2 || o->robust_kind < 0 || o->robust_kind > 2 || o->rejector_kind < 0 || o->rejector_kind > 1 ||
+      o->optimizer_kind < 0 || o->optimizer_kind > 1)
+    return fail(ctx, 1, std::string(who) + ": invalid factor/robust/rejector/optimizer kind");
+  if (int rc = submap_factor_check(ctx, who, o->factor_kind)) return rc;
+  if (batch_points(ctx) && ctx->n_tgt) {  // (an empty batch has no points)
+    if (int rc = check_target(ctx, who, o->factor_kind)) return rc;
+  }
+  ao.lm = o->optimizer_kind == SGB_OPT_LEVENBERG_MARQUARDT;
+  ao.max_iterations = o->max_iterations;
+  ao.max_inner_iterations = o->max_inner_iterations;
+  ao.gn_lambda = o->gn_lambda;
+  ao.init_lambda = o->init_lambda;
+  ao.lambda_factor = o->lambda_factor;
+  ao.rotation_eps = o->rotation_eps;
+  ao.translation_eps = o->translation_eps;
+  for (int i = 0; i < 6; i++) ao.dof_mask[i] = o->dof_mask[i];
   return 0;
 }
 
@@ -793,30 +771,12 @@ int sgb_error_batch(sgb_ctx* ctx, const double* T, const uint8_t* active, double
 
 int sgb_align_batch(sgb_ctx* ctx, const sgb_align_options* o, const double* init_T, double* out_T, double* out_info, double* out_Hb) {
   if (!ctx) return 1;
-  if (int rc = batch_check(ctx, "sgb_align_batch", init_T)) return rc;
-  if (!o) return fail(ctx, 1, "sgb_align_batch: null options");
-  if (!out_T || !out_info) return fail(ctx, 1, "sgb_align_batch: null output");
-  if (o->factor_kind < 0 || o->factor_kind > 2 || o->robust_kind < 0 || o->robust_kind > 2 || o->rejector_kind < 0 || o->rejector_kind > 1 ||
-      o->optimizer_kind < 0 || o->optimizer_kind > 1)
-    return fail(ctx, 1, "sgb_align_batch: invalid factor/robust/rejector/optimizer kind");
-  if (int rc = submap_factor_check(ctx, "sgb_align_batch", o->factor_kind)) return rc;
+  AlignOptions ao;
+  if (int rc = align_checks(ctx, "sgb_align_batch", o, init_T, out_T, out_info, ao)) return rc;
   const size_t B = batch_members(ctx);
   if (B == 0) return 0;
-  if (batch_points(ctx) && ctx->n_tgt) {
-    if (int rc = check_target(ctx, "sgb_align_batch", o->factor_kind)) return rc;
-  }
   CU(cudaSetDevice(ctx->device));
   if (int rc = pair_view(ctx)) return rc;
-  AlignOptions ao;
-  ao.lm = o->optimizer_kind == SGB_OPT_LEVENBERG_MARQUARDT;
-  ao.max_iterations = o->max_iterations;
-  ao.max_inner_iterations = o->max_inner_iterations;
-  ao.gn_lambda = o->gn_lambda;
-  ao.init_lambda = o->init_lambda;
-  ao.lambda_factor = o->lambda_factor;
-  ao.rotation_eps = o->rotation_eps;
-  ao.translation_eps = o->translation_eps;
-  for (int i = 0; i < 6; i++) ao.dof_mask[i] = o->dof_mask[i];
   // the initial state and poses: the only upload of poses in the whole align
   std::vector<MemberState> state(B);
   std::vector<double> poses(12 * B);
@@ -847,7 +807,7 @@ int sgb_align_batch(sgb_ctx* ctx, const sgb_align_options* o, const double* init
     } else {
       if (int rc = error_round(ctx, nullptr, active.data())) return rc;
     }
-    CU(launch_batch_step(ao, static_cast<uint32_t>(B), lin, ctx->b_out.as<double>(), ctx->b_state.as<MemberState>(), ctx->b_poses.as<double>(),
+    CU(launch_batch_step(ao, static_cast<uint32_t>(B), lin, nullptr, 0, ctx->b_out.as<double>(), ctx->b_state.as<MemberState>(), ctx->b_poses.as<double>(),
                          ctx->b_phase.as<uint8_t>(), ctx->stream));
     ctx->launches += 1;
     CU(cudaMemcpyAsync(phase.data(), ctx->b_phase.p, B, cudaMemcpyDeviceToHost, ctx->stream));
@@ -874,18 +834,10 @@ int sgb_align_batch(sgb_ctx* ctx, const sgb_align_options* o, const double* init
 int sgb_align_batch_async(sgb_ctx* ctx, const sgb_align_options* o, const double* d_init_T, double* d_out_T, double* d_out_info, double* d_out_Hb) {
   if (!ctx) return 1;
   const char* who = "sgb_align_batch_async";
-  if (int rc = batch_check(ctx, who, d_init_T)) return rc;
-  if (!o) return fail(ctx, 1, std::string(who) + ": null options");
-  if (!d_out_T || !d_out_info) return fail(ctx, 1, std::string(who) + ": null output");
-  if (o->factor_kind < 0 || o->factor_kind > 2 || o->robust_kind < 0 || o->robust_kind > 2 || o->rejector_kind < 0 || o->rejector_kind > 1 ||
-      o->optimizer_kind < 0 || o->optimizer_kind > 1)
-    return fail(ctx, 1, std::string(who) + ": invalid factor/robust/rejector/optimizer kind");
-  if (int rc = submap_factor_check(ctx, who, o->factor_kind)) return rc;
+  AlignOptions ao;
+  if (int rc = align_checks(ctx, who, o, d_init_T, d_out_T, d_out_info, ao)) return rc;
   const size_t B = batch_members(ctx);
   if (B == 0) return 0;
-  if (batch_points(ctx) && ctx->n_tgt) {
-    if (int rc = check_target(ctx, who, o->factor_kind)) return rc;
-  }
   CU(cudaSetDevice(ctx->device));
   if (int rc = device_pointer(ctx, d_init_T, "init_T16xB")) return rc;
   if (int rc = device_pointer(ctx, d_out_T, "out_T16xB")) return rc;
@@ -904,16 +856,6 @@ int sgb_align_batch_async(sgb_ctx* ctx, const sgb_align_options* o, const double
     CU(cudaMemsetAsync(ctx->packet_queue.p, 0, 2 * sizeof(uint32_t), ctx->stream));
   }
   if (int rc = pair_view(ctx)) return rc;
-  AlignOptions ao;
-  ao.lm = o->optimizer_kind == SGB_OPT_LEVENBERG_MARQUARDT;
-  ao.max_iterations = o->max_iterations;
-  ao.max_inner_iterations = o->max_inner_iterations;
-  ao.gn_lambda = o->gn_lambda;
-  ao.init_lambda = o->init_lambda;
-  ao.lambda_factor = o->lambda_factor;
-  ao.rotation_eps = o->rotation_eps;
-  ao.translation_eps = o->translation_eps;
-  for (int i = 0; i < 6; i++) ao.dof_mask[i] = o->dof_mask[i];
   const uint32_t nb = static_cast<uint32_t>(B);
   // the device's seed flags are kept while the host's are valid (the same target, the cached correspondences not dropped)
   CU(launch_batch_align_init(ao, nb, d_init_T, ctx->b_state.as<MemberState>(), ctx->b_poses.as<double>(), ctx->b_phase.as<uint8_t>(), ctx->b_dseed.as<uint8_t>(),

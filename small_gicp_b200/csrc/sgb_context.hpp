@@ -270,8 +270,12 @@ int check_target(sgb_ctx* ctx, const char* who, int factor);
 float search_bound(int rejector, double max_dist_sq);
 
 struct LinParams;
+struct ChunkClasses;
+struct PendingParams;
 /// kernel parameters of the current target and source at pose T (sgb_capi.cu)
 int fill_params(sgb_ctx* ctx, LinParams& P, const double* T_colmajor16);
+/// the grid front end's parameters of a point search over n queries with the class counters of `parity` (grid_ready; sgb_capi.cu)
+void point_search_params(const sgb_ctx* ctx, size_t n, int parity, ChunkClasses& cc, PendingParams& pp);
 /// nearest-neighbour search of the P.src.n queries of P.src in a point target: grid probe, then the packet search (sgb_capi.cu)
 int launch_point_search(sgb_ctx* ctx, const LinParams& P, int depth);
 

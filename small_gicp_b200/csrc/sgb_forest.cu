@@ -281,163 +281,15 @@ constexpr int kForestStack = 40;
 // them -- the walk of packet_search_kernel (sgb_kernels_packet.cu): one shared stack, warp votes, warp-uniform node and leaf loads, the
 // dense scan (every lane tests every point) or the sparse one (the whole warp serves one interested lane at a time).  Nothing of any
 // other member enters a warp, so a member's correspondences depend on its own points, pose and seeds only.
+// ROUND (a round of sgb_align_batch_async): the grid is sized for every tile, the round's tile count is read from the device and the CTAs
+// beyond it (all of them in an error() round) exit at once.
+template <bool ROUND>
 __global__ void __launch_bounds__(kLinBlock, 8) forest_search_kernel(const __grid_constant__ BatchParams B, const __grid_constant__ ForestView F,
-                                                                     float bound, uint32_t* __restrict__ vcorr) {
-  extern __shared__ float s_dist[];  // [max_depth][kLinBlock] per-lane box distance of each pending subtree
-  __shared__ uint2 s_child[kForestWarps][kForestStack];
-  const BatchTile t = B.tiles[blockIdx.x];
-  const uint32_t lane = threadIdx.x & 31u, wib = threadIdx.x >> 5;
-  if (wib * 32u >= t.count) return;  // warp-uniform; no CTA barrier below
-  const uint32_t m = t.member;
-  const bool valid = threadIdx.x < t.count;
-  const uint32_t i = t.first + threadIdx.x, v = t.vfirst + threadIdx.x;
-  const uint32_t n_map = F.pt_off[m + 1] - F.pt_off[m];
-  if (n_map == 0) {
-    if (valid) vcorr[v] = kNone;
-    return;
+                                                                     float bound, uint32_t* __restrict__ vcorr, const BatchRound* __restrict__ round) {
+  if constexpr (ROUND) {
+    const BatchRound r = *round;
+    if (!r.lin || blockIdx.x >= r.n_tiles) return;
   }
-  const float4* __restrict__ pnodes = F.pnodes + 4 * static_cast<size_t>(F.node_base[m]);
-  const float4* __restrict__ pts = B.tgt.pts;
-  float* my_dist = s_dist + threadIdx.x;
-  uint2* my_child = s_child[wib];
-
-  float fx = 0.f, fy = 0.f, fz = 0.f;
-  float best_d = -1.0f;  // an idle lane is never interested in anything
-  uint32_t best = kNone;
-  if (valid) {
-    const double* R = B.poses + 12 * static_cast<size_t>(m);
-    const double* cs = B.centres + 4 * static_cast<size_t>(m);
-    const double3 tp = centred_translation(R, cs[0], cs[1], cs[2], F.centres + 4 * static_cast<size_t>(m));
-    const float3 f = centred_query_f32(R, tp, __ldg(&B.pts[i]));
-    fx = f.x;
-    fy = f.y;
-    fz = f.z;
-    best_d = bound;
-    // the member's previous correspondence: an upper bound only prunes
-    const uint32_t prev = (B.members[m].z & kMemberSeeded) ? B.corr[i] : kNone;
-    if (prev != kNone) {
-      const float4 q = __ldg(&pts[prev]);
-      const float dx = q.x - fx, dy = q.y - fy, dz = q.z - fz;
-      const float d = dx * dx + dy * dy + dz * dz;
-      if (d < best_d) {
-        best_d = d;
-        best = prev;
-      }
-    }
-  }
-
-  // This walk exists twice: forest_walk below (used by submap_search_kernel) is a copy of it.  A change to one belongs in the other.
-  int sp = 0;
-  uint32_t cur = 0;    // inner node being expanded (index within the map's record block)
-  bool expand = true;  // false: nothing to expand, take the next pending subtree
-  uint32_t leaf_first = 0, leaf_cnt = 0;
-  float leaf_d = 0.f;
-  for (;;) {
-    if (expand) {
-      const float4 n0 = __ldg(&pnodes[cur * 4 + 0]), n1 = __ldg(&pnodes[cur * 4 + 1]);
-      const float4 n2 = __ldg(&pnodes[cur * 4 + 2]), n3 = __ldg(&pnodes[cur * 4 + 3]);
-      const float dl = box_dist2(fx, fy, fz, n0, n1), dr = box_dist2(fx, fy, fz, n2, n3);
-      const bool wl = dl < best_d, wr = dr < best_d;
-      const unsigned ml = __ballot_sync(0xffffffffu, wl), mr = __ballot_sync(0xffffffffu, wr);
-      uint32_t ca, cb;
-      if (ml && mr) {
-        const unsigned closer_l = __ballot_sync(0xffffffffu, (wl || wr) && dl <= dr);
-        const bool left_first = 2 * __popc(closer_l) >= __popc(ml | mr);
-        my_dist[sp * kLinBlock] = left_first ? dr : dl;
-        if (lane == 0) my_child[sp] = left_first ? make_uint2(__float_as_uint(n2.w), __float_as_uint(n3.w)) : make_uint2(__float_as_uint(n0.w), __float_as_uint(n1.w));
-        sp++;
-        ca = left_first ? __float_as_uint(n0.w) : __float_as_uint(n2.w);
-        cb = left_first ? __float_as_uint(n1.w) : __float_as_uint(n3.w);
-        leaf_d = left_first ? dl : dr;
-      } else if (ml) {
-        ca = __float_as_uint(n0.w);
-        cb = __float_as_uint(n1.w);
-        leaf_d = dl;
-      } else if (mr) {
-        ca = __float_as_uint(n2.w);
-        cb = __float_as_uint(n3.w);
-        leaf_d = dr;
-      } else {
-        expand = false;
-        continue;
-      }
-      if (cb == 0u) {  // inner child
-        cur = ca;
-        continue;
-      }
-      leaf_first = ca;
-      leaf_cnt = cb;
-    } else {
-      bool got = false;
-      uint2 c = make_uint2(0u, 0u);
-      while (sp > 0) {
-        sp--;
-        const float d = my_dist[sp * kLinBlock];
-        if (__any_sync(0xffffffffu, d < best_d)) {
-          __syncwarp();  // lane 0's push of this entry is visible
-          c = my_child[sp];
-          __syncwarp();  // ... and every lane has read it before lane 0 may push over it
-          leaf_d = d;
-          got = true;
-          break;
-        }
-      }
-      if (!got) break;
-      if (c.y == 0u) {
-        cur = c.x;
-        expand = true;
-        continue;
-      }
-      leaf_first = c.x;
-      leaf_cnt = c.y;
-    }
-    // ---- leaf (global positions) ----
-    const unsigned want = __ballot_sync(0xffffffffu, leaf_d < best_d);
-    if (__popc(want) > kForestDenseLanes) {
-      const float4* lp = pts + leaf_first;
-#pragma unroll 4
-      for (uint32_t j = 0; j < leaf_cnt; j++) {
-        const float4 q = __ldg(&lp[j]);
-        const float dx = q.x - fx, dy = q.y - fy, dz = q.z - fz;
-        const float d = dx * dx + dy * dy + dz * dz;
-        if (d < best_d) {
-          best_d = d;
-          best = leaf_first + j;
-        }
-      }
-    } else {
-      for (uint32_t base = 0; base < leaf_cnt; base += 32u) {
-        const uint32_t j = base + lane;
-        float4 q = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (j < leaf_cnt) q = __ldg(&pts[leaf_first + j]);
-        unsigned todo = want;
-        while (todo) {
-          const int src = __ffs(todo) - 1;
-          todo &= todo - 1;
-          const float qx = __shfl_sync(0xffffffffu, fx, src), qy = __shfl_sync(0xffffffffu, fy, src), qz = __shfl_sync(0xffffffffu, fz, src);
-          const float dx = q.x - qx, dy = q.y - qy, dz = q.z - qz;
-          const uint32_t dbits = j < leaf_cnt ? __float_as_uint(dx * dx + dy * dy + dz * dz) : 0x7f800000u;
-          const uint32_t dmin = __reduce_min_sync(0xffffffffu, dbits);
-          const unsigned who = __ballot_sync(0xffffffffu, dbits == dmin);  // lowest lane = first point in scan order
-          if (static_cast<int>(lane) == src) {
-            const float d = __uint_as_float(dmin);
-            if (d < best_d) {
-              best_d = d;
-              best = leaf_first + base + (__ffs(who) - 1);
-            }
-          }
-        }
-      }
-    }
-    expand = false;
-  }
-  __syncwarp();
-  if (valid) vcorr[v] = best;
-}
-
-// A copy of forest_search_kernel's body for forest_search_round_kernel, which serves the rounds of sgb_align_batch_async (calling one
-// shared body from both changed the instruction schedule of forest_search_kernel); a change to one belongs in the other.
-__device__ __forceinline__ void forest_search_tile(const BatchParams& B, const ForestView& F, float bound, uint32_t* __restrict__ vcorr) {
   extern __shared__ float s_dist[];  // [max_depth][kLinBlock] per-lane box distance of each pending subtree
   __shared__ uint2 s_child[kForestWarps][kForestStack];
   const BatchTile t = B.tiles[blockIdx.x];
@@ -715,8 +567,15 @@ __device__ __forceinline__ float3 submap_query(const SubmapView& S, uint32_t e, 
 // distances, so the nearest point of the placed union is the nearest over the entries, and best_d carried from entry to entry prunes
 // the later trees: one that no lane's ball reaches costs its root record's two box tests.  Only a strictly nearer point replaces the
 // best, so at an exact FP32 tie between two entries the earlier one wins.  The seed is evaluated in the frame of the entry that owned it.
-__device__ __forceinline__ void submap_search_tile(const BatchParams& B, const float4* __restrict__ all_pnodes, const SubmapView& S, float bound,
-                                                   uint32_t* __restrict__ vcorr) {
+// ROUND: as for forest_search_kernel.
+template <bool ROUND>
+__global__ void __launch_bounds__(kLinBlock, 7) submap_search_kernel(const __grid_constant__ BatchParams B, const float4* __restrict__ all_pnodes,
+                                                                     const __grid_constant__ SubmapView S, float bound, uint32_t* __restrict__ vcorr,
+                                                                     const BatchRound* __restrict__ round) {
+  if constexpr (ROUND) {
+    const BatchRound r = *round;
+    if (!r.lin || blockIdx.x >= r.n_tiles) return;
+  }
   extern __shared__ float s_dist[];  // [max_depth][kLinBlock] per-lane box distance of each pending subtree
   __shared__ uint2 s_child[kForestWarps][kForestStack];
   const BatchTile t = B.tiles[blockIdx.x];
@@ -764,27 +623,6 @@ __device__ __forceinline__ void submap_search_tile(const BatchParams& B, const f
     vcorr[v] = best;
     S.centry[i] = best_e;
   }
-}
-
-__global__ void __launch_bounds__(kLinBlock, 7) submap_search_kernel(const __grid_constant__ BatchParams B, const float4* __restrict__ all_pnodes,
-                                                                     const __grid_constant__ SubmapView S, float bound, uint32_t* __restrict__ vcorr) {
-  submap_search_tile(B, all_pnodes, S, bound, vcorr);
-}
-
-// The same searches in a round of sgb_align_batch_async: the grid is sized for every tile, the round's tile count is read from the device
-// and the CTAs beyond it (all of them in an error() round) exit at once.
-__global__ void __launch_bounds__(kLinBlock, 8) forest_search_round_kernel(const __grid_constant__ BatchParams B, const __grid_constant__ ForestView F,
-                                                                           float bound, uint32_t* __restrict__ vcorr, const BatchRound* __restrict__ round) {
-  const BatchRound r = *round;
-  if (!r.lin || blockIdx.x >= r.n_tiles) return;
-  forest_search_tile(B, F, bound, vcorr);
-}
-__global__ void __launch_bounds__(kLinBlock, 7) submap_search_round_kernel(const __grid_constant__ BatchParams B, const float4* __restrict__ all_pnodes,
-                                                                           const __grid_constant__ SubmapView S, float bound, uint32_t* __restrict__ vcorr,
-                                                                           const BatchRound* __restrict__ round) {
-  const BatchRound r = *round;
-  if (!r.lin || blockIdx.x >= r.n_tiles) return;
-  submap_search_tile(B, all_pnodes, S, bound, vcorr);
 }
 
 }  // namespace
@@ -839,34 +677,25 @@ cudaError_t launch_forest_build(const ForestBuild& b, cudaStream_t st, int* laun
   return cudaGetLastError();
 }
 
-cudaError_t launch_forest_search(const BatchParams& B, const ForestView& F, uint32_t n_tiles, int max_depth, float bound, uint32_t* vcorr, cudaStream_t st) {
-  if (max_depth < 1 || max_depth > kForestStack) return cudaErrorInvalidValue;
-  const size_t smem = static_cast<size_t>(max_depth) * kLinBlock * sizeof(float);
-  forest_search_kernel<<<n_tiles, kLinBlock, smem, st>>>(B, F, bound, vcorr);
-  return cudaGetLastError();
-}
-
-cudaError_t launch_submap_search(const BatchParams& B, const float4* pnodes, const SubmapView& S, uint32_t n_tiles, int max_depth, float bound, uint32_t* vcorr,
+cudaError_t launch_forest_search(const BatchParams& B, const ForestView& F, const BatchRound* round, uint32_t n_tiles, int max_depth, float bound, uint32_t* vcorr,
                                  cudaStream_t st) {
   if (max_depth < 1 || max_depth > kForestStack) return cudaErrorInvalidValue;
   const size_t smem = static_cast<size_t>(max_depth) * kLinBlock * sizeof(float);
-  submap_search_kernel<<<n_tiles, kLinBlock, smem, st>>>(B, pnodes, S, bound, vcorr);
+  if (round)
+    forest_search_kernel<true><<<n_tiles, kLinBlock, smem, st>>>(B, F, bound, vcorr, round);
+  else
+    forest_search_kernel<false><<<n_tiles, kLinBlock, smem, st>>>(B, F, bound, vcorr, nullptr);
   return cudaGetLastError();
 }
 
-cudaError_t launch_forest_search_round(const BatchParams& B, const ForestView& F, const BatchRound* round, uint32_t max_tiles, int max_depth, float bound,
-                                       uint32_t* vcorr, cudaStream_t st) {
+cudaError_t launch_submap_search(const BatchParams& B, const float4* pnodes, const SubmapView& S, const BatchRound* round, uint32_t n_tiles, int max_depth,
+                                 float bound, uint32_t* vcorr, cudaStream_t st) {
   if (max_depth < 1 || max_depth > kForestStack) return cudaErrorInvalidValue;
   const size_t smem = static_cast<size_t>(max_depth) * kLinBlock * sizeof(float);
-  forest_search_round_kernel<<<max_tiles, kLinBlock, smem, st>>>(B, F, bound, vcorr, round);
-  return cudaGetLastError();
-}
-
-cudaError_t launch_submap_search_round(const BatchParams& B, const float4* pnodes, const SubmapView& S, const BatchRound* round, uint32_t max_tiles, int max_depth,
-                                       float bound, uint32_t* vcorr, cudaStream_t st) {
-  if (max_depth < 1 || max_depth > kForestStack) return cudaErrorInvalidValue;
-  const size_t smem = static_cast<size_t>(max_depth) * kLinBlock * sizeof(float);
-  submap_search_round_kernel<<<max_tiles, kLinBlock, smem, st>>>(B, pnodes, S, bound, vcorr, round);
+  if (round)
+    submap_search_kernel<true><<<n_tiles, kLinBlock, smem, st>>>(B, pnodes, S, bound, vcorr, round);
+  else
+    submap_search_kernel<false><<<n_tiles, kLinBlock, smem, st>>>(B, pnodes, S, bound, vcorr, nullptr);
   return cudaGetLastError();
 }
 

@@ -57,16 +57,14 @@ struct ForestBuild {
 cudaError_t launch_forest_build(const ForestBuild& b, cudaStream_t st, int* launches);
 /// Exact nearest neighbour of every point of the call's tiles in its member's map; vcorr[vfirst + k] = global leaf position or kNone.
 /// max_depth: stack entries per lane (inner levels of the deepest tree + 1, at most 40); bound: the FP32 search bound (search_bound).
-cudaError_t launch_forest_search(const BatchParams& B, const ForestView& F, uint32_t n_tiles, int max_depth, float bound, uint32_t* vcorr, cudaStream_t st);
+/// round null: n_tiles tiles; else a round of sgb_align_batch_async: n_tiles CTAs, of which the first round->n_tiles search (none in an
+/// error() round).
+cudaError_t launch_forest_search(const BatchParams& B, const ForestView& F, const BatchRound* round, uint32_t n_tiles, int max_depth, float bound, uint32_t* vcorr,
+                                 cudaStream_t st);
 /// The same for submap members: the exact nearest neighbour of every point over ALL entries of its member's list, each entry's tree
 /// walked in its own stored frame with the bound the earlier entries left; vcorr as above, S.centry[stored position] = the entry.
-cudaError_t launch_submap_search(const BatchParams& B, const float4* pnodes, const SubmapView& S, uint32_t n_tiles, int max_depth, float bound, uint32_t* vcorr,
-                                 cudaStream_t st);
-/// The two searches in a round of sgb_align_batch_async: max_tiles CTAs, of which the first round->n_tiles search (none in an error() round).
-cudaError_t launch_forest_search_round(const BatchParams& B, const ForestView& F, const BatchRound* round, uint32_t max_tiles, int max_depth, float bound,
-                                       uint32_t* vcorr, cudaStream_t st);
-cudaError_t launch_submap_search_round(const BatchParams& B, const float4* pnodes, const SubmapView& S, const BatchRound* round, uint32_t max_tiles, int max_depth,
-                                       float bound, uint32_t* vcorr, cudaStream_t st);
+cudaError_t launch_submap_search(const BatchParams& B, const float4* pnodes, const SubmapView& S, const BatchRound* round, uint32_t n_tiles, int max_depth,
+                                 float bound, uint32_t* vcorr, cudaStream_t st);
 /// Normals (mode bit 0) / covariances (bit 1) of every point of a built forest from its k nearest neighbours in its own map, as
 /// launch_features computes them for one cloud (sgb_preprocess.cu): one thread per leaf-ordered point, outputs in the double layout at
 /// the point's global original position.  lo: the build's orig_lo, or null.  depth: stack entries (inner levels of the deepest tree + 1).

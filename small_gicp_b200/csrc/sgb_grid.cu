@@ -144,11 +144,20 @@ __global__ void grid_table_init_kernel(GridSlot* table, uint32_t capacity) {
 // ---------------------------------------------------------------------------------------------------------------
 // probe: the block anchored at floor(u - 1/2) covers [q - c/2, q + c/2]^3; one lookup, then its four contiguous runs
 // ---------------------------------------------------------------------------------------------------------------
-// A copy of grid_probe_blocks_kernel's body over n queries for grid_probe_round_kernel (calling one shared body from both changed the
-// register allocation of grid_probe_blocks_kernel); a change to one belongs in the other.
-__device__ __forceinline__ void grid_probe_blocks(const LinParams& P, uint32_t n, const float4* __restrict__ grid_pts, const GridSlot* __restrict__ table,
-                                                  uint32_t mask, const GridParams& g, uint8_t* state, uint32_t* pending_count, uint32_t* pending_list,
-                                                  float4* pending_q, uint32_t* next_count, const ChunkClasses& cc) {
+// 32 registers, no spills: 8 CTAs of 256 threads = full occupancy.  ROUND (a round of sgb_align_batch_async): the first *n_queries of the
+// grid's queries (written on the device by the round's planner), the CTAs beyond them exit at once; the planner cleared both pending
+// counters and the class counters at the head of the round.  The count read from memory does not fit 32 registers (at 8 or 7 CTAs of
+// 256 threads it spills 4 bytes): 39 registers, 6 CTAs.
+template <bool ROUND>
+__global__ void __launch_bounds__(256, ROUND ? 6 : 8) grid_probe_blocks_kernel(const __grid_constant__ LinParams P, const float4* __restrict__ grid_pts,
+                                                                               const GridSlot* __restrict__ table, uint32_t mask, GridParams g, uint8_t* state,
+                                                                               uint32_t* pending_count, uint32_t* pending_list, float4* pending_q,
+                                                                               uint32_t* next_count, ChunkClasses cc, const uint32_t* __restrict__ n_queries) {
+  uint32_t n = P.src.n;
+  if constexpr (ROUND) {
+    n = *n_queries;
+    if (blockIdx.x * blockDim.x >= n) return;
+  }
   const uint32_t gi = blockIdx.x * blockDim.x + threadIdx.x;
   const bool in_range = gi < n;
   if (gi == 0u) *next_count = 0u;  // the counter of the NEXT linearize (two counters alternate: no memset between launches)
@@ -256,131 +265,6 @@ __device__ __forceinline__ void grid_probe_blocks(const LinParams& P, uint32_t n
   }
 }
 
-// 32 registers, no spills: 8 CTAs of 256 threads = full occupancy.
-__global__ void __launch_bounds__(256, 8) grid_probe_blocks_kernel(const __grid_constant__ LinParams P, const float4* __restrict__ grid_pts,
-                                                                   const GridSlot* __restrict__ table, uint32_t mask, GridParams g, uint8_t* state,
-                                                                   uint32_t* pending_count, uint32_t* pending_list, float4* pending_q, uint32_t* next_count,
-                                                                   ChunkClasses cc) {
-  const uint32_t gi = blockIdx.x * blockDim.x + threadIdx.x;
-  const bool in_range = gi < P.src.n;
-  if (gi == 0u) *next_count = 0u;  // the counter of the NEXT linearize (two counters alternate: no memset between launches)
-  if (gi < kChunkClasses && cc.count_next) cc.count_next[gi] = 0u;
-  const uint32_t i = in_range ? gi : P.src.n - 1u;
-  const double3 tp = centred_translation(P.T, P.src.centre[0], P.src.centre[1], P.src.centre[2], P.tgt.centre);
-  const float3 f = centred_query_f32(P.T, tp, __ldg(&P.src.pts[i]));
-  const float fx = f.x, fy = f.y, fz = f.z;
-  const float ax = floorf((fx - g.origin[0]) * g.inv_cell - 0.5f), ay = floorf((fy - g.origin[1]) * g.inv_cell - 0.5f),
-              az = floorf((fz - g.origin[2]) * g.inv_cell - 0.5f);
-  // queries far outside the target's box cannot be settled anyway; clamping keeps the integer cell coordinates in range
-  const int bx = static_cast<int>(fminf(fmaxf(ax, -1e5f), 1e5f)), by = static_cast<int>(fminf(fmaxf(ay, -1e5f), 1e5f)),
-            bz = static_cast<int>(fminf(fmaxf(az, -1e5f), 1e5f));
-  const GridRuns e = grid_lookup(table, mask, bx, by, bz);
-  // The four runs are scanned as one sequence (run r starts at position p_r = count[0] + ... + count[r - 1], and o_r maps a position
-  // of run r to its point), unrolled by four so that four independent loads are in flight per thread.  The squared distance is
-  // fma(dz, dz, fma(dy, dy, dx * dx)) in FP32 with round-to-nearest, and the candidate is the lexicographic minimum of (distance, leaf
-  // position) -- within one block the same point the scan of a leaf-position-ordered list with a strict < keeps.
-  uint64_t best_key = grid_cand_key(P.max_dist_sq, 0u);
-  {
-    const uint32_t p1 = e.count[0], p2 = p1 + e.count[1], p3 = p2 + e.count[2], total = p3 + e.count[3];
-    const uint32_t o0 = e.start[0], o1 = e.start[1] - p1, o2 = e.start[2] - p2, o3 = e.start[3] - p3;
-#pragma unroll 4
-    for (uint32_t j = 0; j < total; j++) {
-      const uint32_t idx = j + (j >= p3 ? o3 : j >= p2 ? o2 : j >= p1 ? o1 : o0);
-      const float4 t = __ldg(&grid_pts[idx]);
-      const float dx = __fsub_rn(t.x, fx), dy = __fsub_rn(t.y, fy), dz = __fsub_rn(t.z, fz);
-      const uint64_t key = grid_cand_key(__fmaf_rn(dz, dz, __fmaf_rn(dy, dy, __fmul_rn(dx, dx))), __float_as_uint(t.w));
-      best_key = key < best_key ? key : best_key;
-    }
-  }
-  float best_d = P.max_dist_sq;
-  uint32_t best = kNone;
-  if (best_key != grid_cand_key(P.max_dist_sq, 0u)) {
-    best_d = __uint_as_float(static_cast<uint32_t>(best_key >> 32));
-    best = static_cast<uint32_t>(best_key);
-  }
-  const bool settled = best != kNone && best_d <= g.settle_d2;
-  if (!settled && P.use_prev) {  // keep the better of (grid candidate, previous correspondence) as the tree search's seed
-    const uint32_t prev = P.corr[i];
-    if (prev != kNone) {
-      const float4 t = __ldg(&P.tgt.pts[prev]);
-      const float dx = t.x - fx, dy = t.y - fy, dz = t.z - fz;
-      const float d = dx * dx + dy * dy + dz * dz;
-      if (d < best_d) {  // (a seed beyond the rejector's bound is no use: best_d starts there)
-        best = prev;
-        best_d = d;
-      }
-    }
-  }
-  if (in_range) {
-    P.corr[i] = best;
-    state[i] = settled ? 1 : 0;
-  }
-  // Pending queries go to a compact list, and -- for the packet search -- the CHUNK (one warp here = one 32-query chunk there) goes into
-  // the work list of its cost class = how far its widest search ball reaches (best_d is the squared radius a pending lane starts its
-  // walk with).  The packet search takes the wide classes first, so that what is left when the GPU drains are the cheap walks
-  // (otherwise a long tail of late-starting heavy chunks); chunks without a pending lane are in no list.
-  // Both appends are aggregated over the CTA's eight warps: at most four atomics per CTA -- one per warp and list made the hot
-  // counters the probe's own tail at the identity pose.
-  const bool pend = in_range && !settled;
-  const unsigned m = __ballot_sync(0xffffffffu, pend);
-  const uint32_t lane = threadIdx.x & 31u, wib = threadIdx.x >> 5;
-  __shared__ uint32_t s_cnt[8], s_cls[8], s_base[8];
-  {
-    const uint32_t r2 = __reduce_max_sync(0xffffffffu, pend ? __float_as_uint(best_d) : 0u);  // non-negative floats order like their bits
-    if (lane == 0) {
-      const float r = __uint_as_float(r2);
-      s_cnt[wib] = static_cast<uint32_t>(__popc(m));
-      s_cls[wib] = !m ? kChunkClasses : (r >= cc.wide_r2 ? 0u : (r >= cc.mid_r2 ? 1u : 2u));
-    }
-  }
-  __syncthreads();
-  if (wib == 0) {
-    const uint32_t nw = blockDim.x >> 5;
-    const uint32_t cnt = lane < nw ? s_cnt[lane] : 0u, cls = lane < nw ? s_cls[lane] : kChunkClasses;
-    uint32_t incl = cnt;  // inclusive prefix over the warps
-#pragma unroll
-    for (int o = 1; o < 8; o <<= 1) {
-      const uint32_t t = __shfl_up_sync(0xffffffffu, incl, o);
-      if (lane >= static_cast<uint32_t>(o)) incl += t;
-    }
-    const uint32_t total = __shfl_sync(0xffffffffu, incl, 7);
-    uint32_t pbase = 0;
-    if (lane == 0 && total) pbase = atomicAdd(pending_count, total);
-    pbase = __shfl_sync(0xffffffffu, pbase, 0);
-    if (lane < nw) s_base[lane] = pbase + incl - cnt;
-    if (cc.lists) {
-#pragma unroll
-      for (uint32_t c = 0; c < kChunkClasses; c++) {
-        const unsigned mc = __ballot_sync(0xffffffffu, cls == c);
-        if (!mc) continue;
-        uint32_t cb = 0;
-        if (lane == static_cast<uint32_t>(__ffs(mc) - 1)) cb = atomicAdd(&cc.count[c], static_cast<uint32_t>(__popc(mc)));
-        cb = __shfl_sync(0xffffffffu, cb, __ffs(mc) - 1);
-        if (cls == c) cc.lists[static_cast<size_t>(c) * cc.n_chunks + cb + __popc(mc & ((1u << lane) - 1u))] = (blockIdx.x * blockDim.x >> 5) + lane;
-      }
-    }
-  }
-  __syncthreads();
-  if (pend) {  // the pending record: who, where (transformed query) and how far its best candidate is -- the finishing kernel needs nothing else
-    const uint32_t slot = s_base[wib] + __popc(m & ((1u << lane) - 1u));
-    pending_list[slot] = i;
-    pending_q[slot] = make_float4(fx, fy, fz, best_d);
-  }
-}
-
-// The probe in a round of sgb_align_batch_async: *n_queries (written on the device by the round's planner) of the grid's queries; the
-// CTAs beyond them exit at once.  The planner cleared both pending counters and the class counters at the head of the round.  The count
-// read from memory does not fit grid_probe_blocks_kernel's 32 registers (at 8 or 7 CTAs of 256 threads it spills 4 bytes): 39 registers,
-// 6 CTAs.
-__global__ void __launch_bounds__(256, 6) grid_probe_round_kernel(const __grid_constant__ LinParams P, const uint32_t* __restrict__ n_queries,
-                                                                  const float4* __restrict__ grid_pts, const GridSlot* __restrict__ table, uint32_t mask,
-                                                                  GridParams g, uint8_t* state, uint32_t* pending_count, uint32_t* pending_list,
-                                                                  float4* pending_q, uint32_t* next_count, ChunkClasses cc) {
-  const uint32_t n = *n_queries;
-  if (blockIdx.x * blockDim.x >= n) return;
-  grid_probe_blocks(P, n, grid_pts, table, mask, g, state, pending_count, pending_list, pending_q, next_count, cc);
-}
-
 // per-leaf spacing estimate from the packet records (two largest box extents / count) for the choice of the cell size
 __global__ void grid_spacing_kernel(const float4* __restrict__ pnodes, uint32_t n_inner, float* out) {
   const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
@@ -428,19 +312,15 @@ cudaError_t launch_grid_fill(const uint64_t* akeys, const uint32_t* avals, uint3
   return cudaGetLastError();
 }
 
-cudaError_t launch_grid_probe(const LinParams& P, const float4* grid_pts, const GridSlot* table, uint32_t capacity, const GridParams& g, uint8_t* state,
-                              uint32_t* pending_count, uint32_t* pending_list, float4* pending_q, uint32_t* next_count, const ChunkClasses& cc, cudaStream_t st) {
+cudaError_t launch_grid_probe(const LinParams& P, const uint32_t* n_queries, const float4* grid_pts, const GridSlot* table, uint32_t capacity,
+                              const GridParams& g, uint8_t* state, uint32_t* pending_count, uint32_t* pending_list, float4* pending_q, uint32_t* next_count,
+                              const ChunkClasses& cc, cudaStream_t st) {
   // *pending_count must be zero on entry: the previous probe (or the context) cleared it
-  const uint32_t grid = (P.src.n + 255u) / 256u;
-  grid_probe_blocks_kernel<<<grid, 256, 0, st>>>(P, grid_pts, table, capacity - 1u, g, state, pending_count, pending_list, pending_q, next_count, cc);
-  return cudaGetLastError();
-}
-
-cudaError_t launch_grid_probe_round(const LinParams& P, const uint32_t* n_queries, const float4* grid_pts, const GridSlot* table, uint32_t capacity,
-                                    const GridParams& g, uint8_t* state, uint32_t* pending_count, uint32_t* pending_list, float4* pending_q,
-                                    uint32_t* next_count, const ChunkClasses& cc, cudaStream_t st) {
-  const uint32_t grid = (P.src.n + 255u) / 256u;  // P.src.n: the most queries a round can have
-  grid_probe_round_kernel<<<grid, 256, 0, st>>>(P, n_queries, grid_pts, table, capacity - 1u, g, state, pending_count, pending_list, pending_q, next_count, cc);
+  const uint32_t grid = (P.src.n + 255u) / 256u;  // with n_queries: P.src.n = the most queries a round can have
+  if (n_queries)
+    grid_probe_blocks_kernel<true><<<grid, 256, 0, st>>>(P, grid_pts, table, capacity - 1u, g, state, pending_count, pending_list, pending_q, next_count, cc, n_queries);
+  else
+    grid_probe_blocks_kernel<false><<<grid, 256, 0, st>>>(P, grid_pts, table, capacity - 1u, g, state, pending_count, pending_list, pending_q, next_count, cc, nullptr);
   return cudaGetLastError();
 }
 

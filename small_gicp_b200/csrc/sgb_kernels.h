@@ -156,13 +156,11 @@ struct PendingParams {
   GridParams g;
 };
 /// queue / queue_next: two alternating zero-initialised counters of the dynamic chunk queue (this launch clears queue_next), or null = static stride.
-/// pending_count <= min_pending: the launch finishes the pending queries warp-per-query (ring phase / tree walk); more: the packet walk.
-cudaError_t launch_packet_search(const LinParams& P, const float4* pnodes, int grid, int max_depth, const uint8_t* settled, const uint32_t* pending_count,
-                                 uint32_t min_pending, uint32_t* queue, uint32_t* queue_next, const ChunkClasses& cc, const PendingParams& pp, bool tma_leaf, cudaStream_t st);
-/// The same in a round of sgb_align_batch_async: *n_queries of the P.src.n queries (read on the device), min_pending = *n_queries / pending_div.
-cudaError_t launch_packet_search_round(const LinParams& P, const uint32_t* n_queries, uint32_t pending_div, const float4* pnodes, int grid, int max_depth,
-                                       const uint8_t* settled, const uint32_t* pending_count, uint32_t* queue, uint32_t* queue_next, const ChunkClasses& cc,
-                                       const PendingParams& pp, cudaStream_t st);
+/// pending_count <= P.src.n / pending_div: the launch finishes the pending queries warp-per-query (ring phase / tree walk); more: the packet walk.
+/// n_queries non-null: a round of sgb_align_batch_async, *n_queries of the P.src.n queries (read on the device) in place of P.src.n.
+cudaError_t launch_packet_search(const LinParams& P, const uint32_t* n_queries, const float4* pnodes, int grid, int max_depth, const uint8_t* settled,
+                                 const uint32_t* pending_count, uint32_t pending_div, uint32_t* queue, uint32_t* queue_next, const ChunkClasses& cc,
+                                 const PendingParams& pp, bool tma_leaf, cudaStream_t st);
 cudaError_t launch_grid_spacing(const float4* pnodes, uint32_t n_inner, float* out, cudaStream_t st);
 /// Cell-ordered points + block table (sgb_grid.cu), sorted by compact raster keys of 3 `bits` bits.  build: cell keys of the n
 /// leaf-ordered points, radix sort, the points in cell order into grid_pts (n float4), cell sizes into cnt (n), the eight block anchors
@@ -175,12 +173,10 @@ cudaError_t launch_grid_fill(const uint64_t* akeys, const uint32_t* avals, uint3
 /// largest block (points, the sum of its four runs) the grid front end accepts: beyond it a single query's scan would dominate (a cluster of near-duplicate
 /// points, or a few far outliers stretching the box so that the cell-count bound inflates the cell) and the exact tree search alone is used
 constexpr uint32_t kGridMaxList = 2048;
-cudaError_t launch_grid_probe(const LinParams& P, const float4* grid_pts, const GridSlot* table, uint32_t capacity, const GridParams& g, uint8_t* state,
-                              uint32_t* pending_count, uint32_t* pending_list, float4* pending_q, uint32_t* next_count, const ChunkClasses& cc, cudaStream_t st);
-/// The probe in a round of sgb_align_batch_async: a grid for P.src.n queries, of which the first *n_queries (read on the device) are probed.
-cudaError_t launch_grid_probe_round(const LinParams& P, const uint32_t* n_queries, const float4* grid_pts, const GridSlot* table, uint32_t capacity,
-                                    const GridParams& g, uint8_t* state, uint32_t* pending_count, uint32_t* pending_list, float4* pending_q,
-                                    uint32_t* next_count, const ChunkClasses& cc, cudaStream_t st);
+/// n_queries non-null: a round of sgb_align_batch_async, a grid for P.src.n queries of which the first *n_queries (read on the device) are probed.
+cudaError_t launch_grid_probe(const LinParams& P, const uint32_t* n_queries, const float4* grid_pts, const GridSlot* table, uint32_t capacity,
+                              const GridParams& g, uint8_t* state, uint32_t* pending_count, uint32_t* pending_list, float4* pending_q, uint32_t* next_count,
+                              const ChunkClasses& cc, cudaStream_t st);
 /// what the 27-block ring is guaranteed to cover: squared radius ((2.5 - slack) cells)^2
 inline float ring_cover_sq(float cell) {
   const float c = (2.5f - 4e-3f) * cell;
