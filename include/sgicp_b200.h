@@ -295,6 +295,25 @@ int sgb_error_batch(sgb_ctx* ctx, const double* T_colmajor16xB, const uint8_t* a
 /* Correspondences of every member's last linearize, concatenated in the caller's order (offsets of sgb_source_set_batch), original
  * target indices; SGB_NO_CORRESPONDENCE = rejected or never linearised. */
 int sgb_correspondences_batch(sgb_ctx* ctx, uint64_t* out);
+/* Per-point terms: sgb_linearize_batch / sgb_error_batch that also return every source point's share of its member's sums, e.g. to flag
+ * points whose error stays large after an align, to score an alignment per member, or to weight the points in a solver of one's own.
+ *   - Each call does exactly what the plain call does (search, correspondences, seeds, cached linearisation and the state it leaves) and
+ *     out44xB / out_e are bit-identical to it.  sgb_kernel_launches counts the same launches: the factor kernel writes the rows itself.
+ *   - One row per source point, in the layout of sgb_correspondences_batch: members concatenated (pair and submap members in the
+ *     pairing's member order), each in its cloud's original order.
+ *   - out_point_e[i]: the point's share of its member's e.  linearize: w e as RobustFactor::linearize returns it; error(): Factor::error
+ *     at the trial pose with the cached correspondence (GICP: the precision matrix of the member's linearisation pose), robust-weighted.
+ *   - out_point_Hb42[42 i ..]: the point's H (36, row-major, symmetric) | b (6).  A member's rows add up to its H | b | e.
+ *   - Zero rows: rejected points, points without a correspondence, every point of an inactive member, and every point against an
+ *     empty target.
+ *   - Outputs in host, page-locked or device memory; the call returns when the results are there.  Device memory of the context's GPU is
+ *     written by the kernel directly, any other memory through one copy.
+ *   - They fail where the plain calls fail, and also when out_point_e and out_point_Hb42 are both NULL (linearize) or out_point_e is
+ *     NULL (error). */
+int sgb_linearize_batch_points(sgb_ctx* ctx, int factor_kind, int robust_kind, double robust_c, int rejector_kind, double max_dist_sq,
+                               const double* T_colmajor16xB, const uint8_t* active /*or NULL*/, double* out44xB, double* out_point_e /*or NULL*/,
+                               double* out_point_Hb42 /*or NULL*/);
+int sgb_error_batch_points(sgb_ctx* ctx, const double* T_colmajor16xB, const uint8_t* active /*or NULL*/, double* out_e, double* out_point_e);
 
 /* Batched align(): Registration<Factor, ..., GeneralFactor, Rejector, Optimizer>::align (registration.hpp:17-54, optimizer.hpp:10-158) of
  * every member from its own initial pose, in lockstep.  A round is one sgb_linearize_batch over the members still iterating or, for

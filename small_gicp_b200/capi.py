@@ -83,6 +83,8 @@ _SIGNATURES = {
     "sgb_linearize_batch": (C.c_int, [_vp, C.c_int, C.c_int, C.c_double, C.c_int, C.c_double, _dp, C.POINTER(C.c_uint8), _dp]),
     "sgb_error_batch": (C.c_int, [_vp, _dp, C.POINTER(C.c_uint8), _dp]),
     "sgb_correspondences_batch": (C.c_int, [_vp, _u64p]),
+    "sgb_linearize_batch_points": (C.c_int, [_vp, C.c_int, C.c_int, C.c_double, C.c_int, C.c_double, _dp, C.POINTER(C.c_uint8), _dp, _dp, _dp]),
+    "sgb_error_batch_points": (C.c_int, [_vp, _dp, C.POINTER(C.c_uint8), _dp, _dp]),
     "sgb_align_batch": (C.c_int, [_vp, C.POINTER(AlignOptions), _dp, _dp, _dp, _dp]),
     "sgb_align_batch_async": (C.c_int, [_vp, C.POINTER(AlignOptions), _dp, _dp, _dp, _dp]),
     "sgb_estimate_features": (C.c_int, [_vp, C.c_size_t, _dp, C.c_int, _dp, _dp]),
@@ -111,6 +113,20 @@ class BatchAlignResult:
         self.error = info4[:, 3].copy()
         self.H = np.ascontiguousarray(Hb42[:, :36].reshape(B, 6, 6).transpose(0, 2, 1))
         self.b = Hb42[:, 36:42].copy()
+
+
+class BatchPointTerms:
+    """what Context.linearize_batch_points returns: the member arrays of linearize_batch, H (B,6,6), b (B,6), e (B,) and num_inliers (B,),
+    and one row per source point in the layout of correspondences_batch (member m's rows are offsets[m] .. offsets[m + 1], in its
+    cloud's original order): point_e (N,), point_H (N,6,6) and point_b (N,6) (None with hessians=False).  The point arrays are views of
+    the raw rows point_e and point_Hb42 (N,42) = H (36, row-major) | b, numpy arrays or the CUDA tensors passed as out_e / out_Hb42."""
+
+    def __init__(self, H, b, e, num_inliers, offsets, point_e, point_Hb42):
+        self.H, self.b, self.e, self.num_inliers, self.offsets = H, b, e, num_inliers, offsets
+        self.point_e, self.point_Hb42 = point_e, point_Hb42
+        n = point_e.shape[0]
+        self.point_H = None if point_Hb42 is None else point_Hb42[:, :36].reshape(n, 6, 6)
+        self.point_b = None if point_Hb42 is None else point_Hb42[:, 36:42]
 
 
 class AsyncAlignResult:
@@ -537,6 +553,45 @@ class Context:
         out = np.zeros(max(B, 1))
         self._check(self._L.sgb_error_batch(self._h, _d(Tc), ap, _d(out)))
         return out[:B].copy()
+
+    def _rows(self, out, cols, who):
+        """a per-point output: a new numpy array, or `out` (numpy or torch, CUDA tensors included) checked for shape and layout"""
+        n = int(self._batch_offsets[-1])
+        shape = (n,) if cols == 1 else (n, cols)
+        if out is None:
+            return np.zeros((max(n, 1),) + shape[1:])[:n]
+        if tuple(out.shape) != shape:
+            raise SgbError(f"{who}: the per-point output must have shape {shape}")
+        if _is_dev(out):
+            _f64(out)
+        elif not (out.dtype == np.float64 and out.flags.c_contiguous):
+            raise SgbError(f"{who}: the per-point output must be contiguous float64")
+        return out
+
+    def linearize_batch_points(self, Ts, active=None, factor=FACTOR_GICP, robust=ROBUST_NONE, robust_c=1.0, rejector=REJECT_DISTANCE, max_dist_sq=1.0,
+                               hessians=True, out_e=None, out_Hb42=None):
+        """linearize_batch plus every source point's terms (sgb_linearize_batch_points) -> BatchPointTerms.  The member sums are
+        bit-identical to linearize_batch's.  point_e = the point's w e, point_H / point_b its J^T M J / J^T M r (robust-weighted); zero rows
+        for rejected or unmatched points and inactive members.  hessians=False: point_e only (H | b rows not computed).  out_e (N,) and
+        out_Hb42 (N, 42): float64 outputs to write in place (numpy, or CUDA tensors on the context's device, written by the kernel)."""
+        B, Tc, a, ap = self._batch_args(Ts, active)
+        e_rows = self._rows(out_e, 1, "linearize_batch_points")
+        hb_rows = self._rows(out_Hb42, 42, "linearize_batch_points") if hessians else None
+        out = np.zeros((max(B, 1), 44))
+        self._check(self._L.sgb_linearize_batch_points(self._h, factor, robust, float(robust_c), rejector, float(max_dist_sq), _d(Tc), ap, _d(out),
+                                                       _d(e_rows), _d(hb_rows)))
+        out = out[:B]
+        return BatchPointTerms(out[:, :36].reshape(B, 6, 6).copy(), out[:, 36:42].copy(), out[:, 42].copy(), out[:, 43].astype(np.int64),
+                               self._batch_offsets.copy(), e_rows, hb_rows)
+
+    def error_batch_points(self, Ts, active=None, out_e=None):
+        """error_batch plus every source point's share of its member's e (sgb_error_batch_points) -> (e (B,), point_e (N,)), point_e in the
+        layout of correspondences_batch; out_e as in linearize_batch_points"""
+        B, Tc, a, ap = self._batch_args(Ts, active)
+        e_rows = self._rows(out_e, 1, "error_batch_points")
+        out = np.zeros(max(B, 1))
+        self._check(self._L.sgb_error_batch_points(self._h, _d(Tc), ap, _d(out), _d(e_rows)))
+        return out[:B].copy(), e_rows
 
     def correspondences_batch(self):
         """list of per-member correspondence arrays (original target indices, NO_CORRESPONDENCE = rejected)"""

@@ -7,7 +7,8 @@
 //                           -> one partial per tile.  Per target kind: the correspondence the search found (one point target, many
 //                           kd-trees with member m centred on map m), the voxel-map probe for VGICP (vox_nearest, as in
 //                           linearize_vox_kernel; many voxel maps: member m in map m's centre and table region), or submap members, each
-//                           point at the member's pose relative to the placement of the entry its correspondence lies in
+//                           point at the member's pose relative to the placement of the entry its correspondence lies in; for the
+//                           _points calls also each point's row of terms (BatchRows)
 //   batch_segment_kernel    one CTA per member: its tiles' partials in tile order -> H|b|e|inliers (or e) of that member
 //   batch_step_kernel       batched align(): one thread per member, its Gauss-Newton / Levenberg-Marquardt step (sgb_math.cuh) after a
 //                           round, its next pose and phase
@@ -100,9 +101,11 @@ __global__ void __launch_bounds__(kLinBlock) batch_transform_kernel(const __grid
 // SUB: submap members (S, sgb_source_set_submaps) -- the correspondence lies in entry S->centry[i] of the member's list, and the point is
 // linearised at the member's pose relative to that entry's placement against the entry's map as stored.  r^T M r and its derivatives by
 // the right perturbation of the pose are invariant under the placement, so this IS the point's share of the sums against the union.
-template <int FACTOR, int ROBUST, bool VOX, bool ERR, bool MAPS, bool SUB = false>
+// POINTS: the point's row too (rows).  A thread takes one point of the tile, so its acc is 0 + that point's terms: the very summands of
+// the tile sum, written before it, whatever the kind (factor_terms_source or accumulate_factor); zeros where the point has no term.
+template <int FACTOR, int ROBUST, bool VOX, bool ERR, bool MAPS, bool SUB = false, bool POINTS = false>
 __device__ __forceinline__ void batch_factor_tile(const BatchParams& B, const uint32_t* __restrict__ vcorr, const double* __restrict__ map_centres,
-                                                  const uint4* __restrict__ map_regions, const SubmapView* S = nullptr) {
+                                                  const uint4* __restrict__ map_regions, const SubmapView* S = nullptr, const BatchRows* rows = nullptr) {
   constexpr int NACC = ERR ? 1 : kAcc + 1;
   double acc[NACC];
 #pragma unroll
@@ -187,6 +190,23 @@ __device__ __forceinline__ void batch_factor_tile(const BatchParams& B, const ui
       }
       B.corr[i] = best;
     }
+    if constexpr (POINTS) {
+      const size_t row = static_cast<size_t>(__ldg(&rows->member_off[t.member])) + __ldg(&rows->perm[i]);
+      if constexpr (ERR) {
+        rows->e[row] = acc[0];
+      } else {
+        if (rows->e) rows->e[row] = acc[kAcc - 1];
+        if (rows->Hb) {
+          double* o = rows->Hb + 42 * row;
+#pragma unroll
+          for (int k = 0; k < kAcc - 1; k++) {
+            int p0, p1;
+            if (expand_positions(k, p0, p1) == 2) o[p1] = acc[k];
+            o[p0] = acc[k];
+          }
+        }
+      }
+    }
   }
   const double v = tile_sum<NACC>(acc);
   if (tid < NACC) B.tile_partials[static_cast<size_t>(blockIdx.x) * kPartialStride + tid] = v;
@@ -195,11 +215,12 @@ __device__ __forceinline__ void batch_factor_tile(const BatchParams& B, const ui
 // One CTA per tile of one member, for the target's KIND: 0 one point target, 1 one voxel map, 2 many voxel maps (member m against map m:
 // map_centres and map_regions), 3 many kd-trees (map_centres; vcorr = what forest_search_kernel found in map m), 4 submaps (S; vcorr and
 // S.centry = what submap_search_kernel found over the member's entries).  MODE: linearize, error() with the cached correspondences, or
-// either as the round's planner decided.
-template <int FACTOR, int ROBUST, int KIND, int MODE>
+// either as the round's planner decided.  POINTS (host-planned modes only): every processed point's row to `rows` too.
+template <int FACTOR, int ROBUST, int KIND, int MODE, bool POINTS = false>
 __global__ void __launch_bounds__(kLinBlock, 4) batch_factor_kernel(const __grid_constant__ BatchParams B, const uint32_t* __restrict__ vcorr,
                                                                    const double* __restrict__ map_centres, const uint4* __restrict__ map_regions,
-                                                                   const __grid_constant__ SubmapView S, const BatchRound* __restrict__ round) {
+                                                                   const __grid_constant__ SubmapView S, const BatchRound* __restrict__ round,
+                                                                   const __grid_constant__ BatchRows rows) {
   constexpr bool VOX = KIND == 1 || KIND == 2, MAPS = KIND == 2 || KIND == 3, SUB = KIND == 4;
   bool lin = MODE == kModeLinearize;
   if constexpr (MODE == kModeRound) {
@@ -208,9 +229,9 @@ __global__ void __launch_bounds__(kLinBlock, 4) batch_factor_kernel(const __grid
     lin = r.lin;
   }
   if (lin)
-    batch_factor_tile<FACTOR, ROBUST, VOX, false, MAPS, SUB>(B, vcorr, map_centres, map_regions, &S);
+    batch_factor_tile<FACTOR, ROBUST, VOX, false, MAPS, SUB, POINTS>(B, vcorr, map_centres, map_regions, &S, &rows);
   else
-    batch_factor_tile<FACTOR, ROBUST, VOX, true, MAPS, SUB>(B, nullptr, map_centres, map_regions, &S);
+    batch_factor_tile<FACTOR, ROBUST, VOX, true, MAPS, SUB, POINTS>(B, nullptr, map_centres, map_regions, &S, &rows);
 }
 
 // One CTA per member: warp w adds tiles w, w + 8, ... of the member in order, then the 8 warp sums are added in warp order.  The order
@@ -415,27 +436,29 @@ cudaError_t launch_batch_transform(const BatchParams& B, const BatchRound* round
 // The factor kernel of one kind in one mode.  The kinds without point-to-plane (1, 2, 4: refused by the caller) compile FACTOR 1 as 0, one
 // instantiation fewer each.  error() reads the cached correspondences only, so the voxel kinds compute what the kinds with the same
 // centres compute there (1 -> 0, 2 -> 3).
-template <int F, int R, int MODE>
+template <int F, int R, int MODE, bool POINTS = false>
 auto factor_kernel(int kind) -> decltype(&batch_factor_kernel<0, 0, 0, kModeLinearize>) {
   constexpr int G = F == 1 ? 0 : F;
   switch (kind) {
-    case 0: return batch_factor_kernel<F, R, 0, MODE>;
-    case 1: if constexpr (MODE == kModeError) return batch_factor_kernel<G, R, 0, MODE>; else return batch_factor_kernel<G, R, 1, MODE>;
-    case 2: if constexpr (MODE == kModeError) return batch_factor_kernel<G, R, 3, MODE>; else return batch_factor_kernel<G, R, 2, MODE>;
-    case 3: return batch_factor_kernel<F, R, 3, MODE>;
-    case 4: return batch_factor_kernel<G, R, 4, MODE>;
+    case 0: return batch_factor_kernel<F, R, 0, MODE, POINTS>;
+    case 1: if constexpr (MODE == kModeError) return batch_factor_kernel<G, R, 0, MODE, POINTS>; else return batch_factor_kernel<G, R, 1, MODE, POINTS>;
+    case 2: if constexpr (MODE == kModeError) return batch_factor_kernel<G, R, 3, MODE, POINTS>; else return batch_factor_kernel<G, R, 2, MODE, POINTS>;
+    case 3: return batch_factor_kernel<F, R, 3, MODE, POINTS>;
+    case 4: return batch_factor_kernel<G, R, 4, MODE, POINTS>;
     default: return nullptr;
   }
 }
 
 cudaError_t launch_batch_factor(const BatchParams& B, int kind, int factor, int robust, bool err, const BatchRound* round, uint32_t n_tiles, const uint32_t* vcorr,
-                                const double* map_centres, const uint4* map_regions, const SubmapView& S, cudaStream_t st) {
+                                const double* map_centres, const uint4* map_regions, const SubmapView& S, const BatchRows* rows, cudaStream_t st) {
   if (factor == 1 && (kind == 1 || kind == 2 || kind == 4)) return cudaErrorInvalidValue;  // no normals in a voxel map; no point-to-plane against a union
+  if (round && rows) return cudaErrorInvalidValue;
   const auto kernel = dispatch_factor_robust(factor, robust, decltype(&batch_factor_kernel<0, 0, 0, kModeLinearize>){}, [&](auto f, auto r) {
+    if (rows) return err ? factor_kernel<f, r, kModeError, true>(kind) : factor_kernel<f, r, kModeLinearize, true>(kind);
     return round ? factor_kernel<f, r, kModeRound>(kind) : err ? factor_kernel<f, r, kModeError>(kind) : factor_kernel<f, r, kModeLinearize>(kind);
   });
   if (!kernel) return cudaErrorInvalidValue;
-  kernel<<<n_tiles, kLinBlock, 0, st>>>(B, vcorr, map_centres, map_regions, S, round);
+  kernel<<<n_tiles, kLinBlock, 0, st>>>(B, vcorr, map_centres, map_regions, S, round, rows ? *rows : BatchRows{});
   return cudaGetLastError();
 }
 

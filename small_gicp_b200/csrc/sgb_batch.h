@@ -32,6 +32,17 @@ struct BatchParams {
   double* tile_partials;  // [tiles][kPartialStride]
 };
 
+/// Per-point rows of sgb_linearize_batch_points / sgb_error_batch_points, written by the factor kernel beside its sums: stored point i of
+/// member m writes row member_off[m] + perm[i], the caller's order of sgb_correspondences_batch.  e: [points] the point's share of the
+/// member's e (or null); Hb: [points][42] its H (36, row-major) | b (6) (or null; linearize only).  Kept out of BatchParams, which keys
+/// the cached graph of sgb_align_batch_async.
+struct BatchRows {
+  const uint32_t* perm;        // stored position -> original index within the member's cloud
+  const uint32_t* member_off;  // [members + 1]
+  double* e;
+  double* Hb;
+};
+
 /// Members as (cloud, map) pairs (sgb_source_set_pairs): member p = a replica of stored cloud clouds[p], at member_off[p] .. member_off[p+1]
 /// of the member buffers; its centre and bounds too.  covA = null: no covariances.
 struct PairGather {
@@ -117,9 +128,9 @@ cudaError_t launch_batch_unmatch(const BatchParams& B, const BatchRound* round, 
 /// map (the VGICP probe), 2 many voxel maps (member m against map m: map_centres [maps][4], map_regions [maps] = (first table slot, mask,
 /// first voxel, voxel count) of each map), 3 many kd-trees (map_centres; vcorr = the forest search's result), 4 submaps (S; vcorr = the
 /// submap search's result).  Linearize (err = false), error() with the cached correspondences (err = true), or with a round what it
-/// says.  Point-to-plane only for kinds 0 and 3.
+/// says.  Point-to-plane only for kinds 0 and 3.  rows (rounds planned on the host only; null: none): every processed point's row too.
 cudaError_t launch_batch_factor(const BatchParams& B, int kind, int factor, int robust, bool err, const BatchRound* round, uint32_t n_tiles, const uint32_t* vcorr,
-                                const double* map_centres, const uint4* map_regions, const SubmapView& S, cudaStream_t st);
+                                const double* map_centres, const uint4* map_regions, const SubmapView& S, const BatchRows* rows, cudaStream_t st);
 /// out: [members][44] (linearize) or [members] (error)
 cudaError_t launch_batch_segment(const BatchParams& B, uint32_t n_members, bool linearize, const BatchRound* round, double* out, cudaStream_t st);
 /// batched align(): every member whose phase matches the round (linearize: kPhaseLinearize, else kPhaseTrial) takes its optimiser step

@@ -1,6 +1,6 @@
 // SPDX-License-Identifier: MIT
 // C-ABI of batched registration (include/sgicp_b200.h: sgb_source_set_batch, sgb_source_set_pairs, sgb_source_set_submaps,
-// sgb_{linearize,error,align,correspondences}_batch, sgb_align_batch_async).
+// sgb_{linearize,error,align,correspondences}_batch, sgb_{linearize,error}_batch_points, sgb_align_batch_async).
 // Kernels in sgb_batch.cu (many kd-trees and submaps: the searches in sgb_forest.cu); DESIGN.md §11.
 #include <cuda_runtime.h>
 
@@ -222,7 +222,7 @@ int point_search_round(sgb_ctx* ctx, const LinParams& P, const uint32_t* n_queri
 // planned on the device (err = false), its grids sized for every tile (n_tiles = max_tiles) and point (n_virtual = batch_points), counted
 // with the graph that holds it.  P: the target's parameters (fill_params at the identity); bound: the FP32 search bound.
 int round_kernels(sgb_ctx* ctx, const LinParams& P, const BatchParams& Bp, const BatchRound* round, uint32_t n_tiles, uint32_t n_virtual, bool err, int factor,
-                  int robust, float bound) {
+                  int robust, float bound, const BatchRows* rows = nullptr) {
   const int counted = round ? 0 : 1;
   // the per-map tables: with a pairing's map table the member-indexed view of the maps, else the map-indexed tables
   const bool view = paired_maps(ctx);
@@ -269,13 +269,15 @@ int round_kernels(sgb_ctx* ctx, const LinParams& P, const BatchParams& Bp, const
     if (int rc = round ? point_search_round(ctx, Q, &round->n_search, depth) : launch_point_search(ctx, Q, depth)) return rc;
     ctx->launches += counted;
   }
-  CU(launch_batch_factor(Bp, kind, factor, robust, err, round, n_tiles, err ? nullptr : vcorr, centres, regions, S, ctx->stream));
+  CU(launch_batch_factor(Bp, kind, factor, robust, err, round, n_tiles, err ? nullptr : vcorr, centres, regions, S, rows, ctx->stream));
   ctx->launches += counted;
   return 0;
 }
 
 // One linearize of the active members (arguments checked by the caller) into b_out, asynchronous.  T = nullptr: poses already in b_poses.
-int linearize_round(sgb_ctx* ctx, int factor, int robust, double robust_c, int rejector, double max_dist_sq, const double* T, const uint8_t* active) {
+// rows: the factor kernel's per-point rows too (the rows it does not reach are the caller's to clear: point_rows).
+int linearize_round(sgb_ctx* ctx, int factor, int robust, double robust_c, int rejector, double max_dist_sq, const double* T, const uint8_t* active,
+                    const BatchRows* rows = nullptr) {
   const size_t B = batch_members(ctx);
   CU(cudaSetDevice(ctx->device));
   const bool voxel = voxel_target(ctx);
@@ -300,7 +302,7 @@ int linearize_round(sgb_ctx* ctx, int factor, int robust, double robust_c, int r
     CU(cudaMemcpyAsync(ctx->b_members.p, none.data(), B * sizeof(uint4), cudaMemcpyHostToDevice, ctx->stream));
   }
   if (n_tiles) {
-    if (int rc = round_kernels(ctx, P, Bp, nullptr, n_tiles, n_virtual, false, factor, robust, search_bound(rejector, max_dist_sq))) return rc;
+    if (int rc = round_kernels(ctx, P, Bp, nullptr, n_tiles, n_virtual, false, factor, robust, search_bound(rejector, max_dist_sq), rows)) return rc;
   }
   CU(launch_batch_segment(Bp, static_cast<uint32_t>(B), true, nullptr, ctx->b_out.as<double>(), ctx->stream));
   ctx->launches += 1;
@@ -317,8 +319,8 @@ int linearize_round(sgb_ctx* ctx, int factor, int robust, double robust_c, int r
   return 0;
 }
 
-// One error() of the active members (every one linearised against the current target) into b_out[0, B), asynchronous.  T as above.
-int error_round(sgb_ctx* ctx, const double* T, const uint8_t* active) {
+// One error() of the active members (every one linearised against the current target) into b_out[0, B), asynchronous.  T, rows as above.
+int error_round(sgb_ctx* ctx, const double* T, const uint8_t* active, const BatchRows* rows = nullptr) {
   const size_t B = batch_members(ctx);
   CU(cudaSetDevice(ctx->device));
   uint32_t n_tiles = 0, n_virtual = 0;
@@ -328,7 +330,7 @@ int error_round(sgb_ctx* ctx, const double* T, const uint8_t* active) {
   BatchParams Bp = batch_params(ctx, P);
   Bp.robust_c = ctx->lin_c;
   if (n_tiles && ctx->n_tgt) {
-    if (int rc = round_kernels(ctx, P, Bp, nullptr, n_tiles, 0, true, ctx->lin_factor, ctx->lin_robust, 0.f)) return rc;
+    if (int rc = round_kernels(ctx, P, Bp, nullptr, n_tiles, 0, true, ctx->lin_factor, ctx->lin_robust, 0.f, rows)) return rc;
   } else {
     n_tiles = 0;
     std::vector<uint4> none(B, make_uint4(0, 0, 0, 0));
@@ -555,12 +557,17 @@ std::vector<unsigned char> loop_key(sgb_ctx* ctx, const sgb_align_options* o) {
   return k;
 }
 
-// p is device memory of the context's GPU (cudaPointerGetAttributes); what names it in the message
-int device_pointer(sgb_ctx* ctx, const void* p, const char* what) {
+// p is device memory of the context's GPU (cudaPointerGetAttributes)
+bool on_device(const sgb_ctx* ctx, const void* p) {
   cudaPointerAttributes a = {};
   const cudaError_t e = cudaPointerGetAttributes(&a, p);
   if (e != cudaSuccess) cudaGetLastError();  // (not an error of the context: clear it)
-  if (e != cudaSuccess || a.type != cudaMemoryTypeDevice || a.device != ctx->device)
+  return e == cudaSuccess && a.type == cudaMemoryTypeDevice && a.device == ctx->device;
+}
+
+// the same as a check; what names p in the message
+int device_pointer(sgb_ctx* ctx, const void* p, const char* what) {
+  if (!on_device(ctx, p))
     return fail(ctx, 1, std::string("sgb_align_batch_async: ") + what + " must be device memory of the context's GPU (cuda:" + std::to_string(ctx->device) +
                             "); host, page-locked and managed memory are refused");
   return 0;
@@ -589,6 +596,103 @@ int align_checks(sgb_ctx* ctx, const char* who, const sgb_align_options* o, cons
   ao.translation_eps = o->translation_eps;
   for (int i = 0; i < 6; i++) ao.dof_mask[i] = o->dof_mask[i];
   return 0;
+}
+
+// ---- sgb_linearize_batch_points / sgb_error_batch_points (DESIGN.md §11 "Per-point terms") ----
+
+// Where the factor kernel writes the rows of one call: the caller's buffers when they are device memory of the context's GPU, else the
+// context's staging buffers (copy_rows copies them out).  The rows the kernel does not reach -- every point of an inactive member, and of
+// every member against an empty target -- are cleared here; rejected and unmatched points get zero rows from the kernel itself.
+int point_rows(sgb_ctx* ctx, const uint8_t* active, double* out_e, double* out_Hb, BatchRows& rows) {
+  const size_t B = batch_members(ctx), nn = std::max<size_t>(batch_points(ctx), 1);
+  rows.perm = (ctx->b_paired ? ctx->p_perm : ctx->src_perm).as<uint32_t>();
+  rows.member_off = (ctx->b_paired ? ctx->p_tables : ctx->b_cloud_off).as<uint32_t>();
+  rows.e = rows.Hb = nullptr;
+  if (out_e && on_device(ctx, out_e)) {
+    rows.e = out_e;
+  } else if (out_e) {
+    CU(ctx->b_rows_e.reserve(nn * sizeof(double)));
+    rows.e = ctx->b_rows_e.as<double>();
+  }
+  if (out_Hb && on_device(ctx, out_Hb)) {
+    rows.Hb = out_Hb;
+  } else if (out_Hb) {
+    CU(ctx->b_rows_hb.reserve(nn * 42 * sizeof(double)));
+    rows.Hb = ctx->b_rows_hb.as<double>();
+  }
+  const auto reached = [&](size_t m) { return ctx->n_tgt && (!active || active[m]); };
+  for (size_t m = 0; m < B;) {  // runs of consecutive members the kernel does not reach: their rows are contiguous
+    size_t end = m;
+    while (end < B && !reached(end)) end++;
+    if (end == m) {
+      m++;
+      continue;
+    }
+    const size_t first = ctx->b_offsets[m], n = ctx->b_offsets[end] - first;
+    if (n && rows.e) CU(cudaMemsetAsync(rows.e + first, 0, n * sizeof(double), ctx->stream));
+    if (n && rows.Hb) CU(cudaMemsetAsync(rows.Hb + 42 * first, 0, 42 * n * sizeof(double), ctx->stream));
+    m = end;
+  }
+  return 0;
+}
+
+int copy_rows(sgb_ctx* ctx, const BatchRows& rows, double* out_e, double* out_Hb) {
+  const size_t n = batch_points(ctx);
+  if (n && out_e && rows.e != out_e) CU(cudaMemcpyAsync(out_e, rows.e, n * sizeof(double), cudaMemcpyDefault, ctx->stream));
+  if (n && out_Hb && rows.Hb != out_Hb) CU(cudaMemcpyAsync(out_Hb, rows.Hb, 42 * n * sizeof(double), cudaMemcpyDefault, ctx->stream));
+  return 0;
+}
+
+// sgb_linearize_batch (who, no rows) and sgb_linearize_batch_points (points: rows to out_e and / or out_Hb)
+int linearize_batch(sgb_ctx* ctx, const char* who, bool points, int factor, int robust, double robust_c, int rejector, double max_dist_sq, const double* T,
+                    const uint8_t* active, double* out44, double* out_e, double* out_Hb) {
+  if (!ctx) return 1;
+  const std::string w = who;
+  if (int rc = batch_check(ctx, who, T)) return rc;
+  if (factor < 0 || factor > 2 || robust < 0 || robust > 2 || rejector < 0 || rejector > 1) return fail(ctx, 1, w + ": invalid factor/robust/rejector kind");
+  if (!out44) return fail(ctx, 1, w + ": null output");
+  if (points && !out_e && !out_Hb) return fail(ctx, 1, w + ": null per-point outputs (out_point_e and out_point_Hb42 both NULL; sgb_linearize_batch gives the sums alone)");
+  if (int rc = submap_factor_check(ctx, who, factor)) return rc;
+  const size_t B = batch_members(ctx);
+  if (B == 0) return 0;
+  if (batch_points(ctx) && ctx->n_tgt) {
+    if (int rc = check_target(ctx, who, factor)) return rc;
+  }
+  if (int rc = pair_view(ctx)) return rc;
+  BatchRows rows;
+  if (points) {
+    if (int rc = point_rows(ctx, active, out_e, out_Hb, rows)) return rc;
+  }
+  if (int rc = linearize_round(ctx, factor, robust, robust_c, rejector, max_dist_sq, T, active, points ? &rows : nullptr)) return rc;
+  if (points) {
+    if (int rc = copy_rows(ctx, rows, out_e, out_Hb)) return rc;
+  }
+  return copy_out(ctx, out44, 44 * B);
+}
+
+// sgb_error_batch (who, no rows) and sgb_error_batch_points (points: rows to out_e)
+int error_batch(sgb_ctx* ctx, const char* who, bool points, const double* T, const uint8_t* active, double* out, double* out_e) {
+  if (!ctx) return 1;
+  const std::string w = who;
+  if (int rc = batch_check(ctx, who, T)) return rc;
+  if (!out) return fail(ctx, 1, w + ": null output");
+  if (points && !out_e) return fail(ctx, 1, w + ": null per-point output (out_point_e; sgb_error_batch gives the sums alone)");
+  const size_t B = batch_members(ctx);
+  if (B == 0) return 0;
+  if (!ctx->have_lin) return fail(ctx, 1, w + ": no preceding sgb_linearize_batch (the correspondences are cached there)");
+  for (size_t m = 0; m < B; m++)
+    if ((!active || active[m]) && !ctx->b_lin[m])
+      return fail(ctx, 1, w + ": member " + std::to_string(m) + " is active but has not been linearised against the current target");
+  if (int rc = pair_view(ctx)) return rc;
+  BatchRows rows;
+  if (points) {
+    if (int rc = point_rows(ctx, active, out_e, nullptr, rows)) return rc;
+  }
+  if (int rc = error_round(ctx, T, active, points ? &rows : nullptr)) return rc;
+  if (points) {
+    if (int rc = copy_rows(ctx, rows, out_e, nullptr)) return rc;
+  }
+  return copy_out(ctx, out, B);
 }
 
 }  // namespace
@@ -739,34 +843,20 @@ int sgb_source_set_submaps(sgb_ctx* ctx, size_t n_members, const uint32_t* cloud
 }
 int sgb_linearize_batch(sgb_ctx* ctx, int factor, int robust, double robust_c, int rejector, double max_dist_sq, const double* T, const uint8_t* active,
                         double* out44) {
-  if (!ctx) return 1;
-  if (int rc = batch_check(ctx, "sgb_linearize_batch", T)) return rc;
-  if (factor < 0 || factor > 2 || robust < 0 || robust > 2 || rejector < 0 || rejector > 1) return fail(ctx, 1, "sgb_linearize_batch: invalid factor/robust/rejector kind");
-  if (!out44) return fail(ctx, 1, "sgb_linearize_batch: null output");
-  if (int rc = submap_factor_check(ctx, "sgb_linearize_batch", factor)) return rc;
-  const size_t B = batch_members(ctx);
-  if (B == 0) return 0;
-  if (batch_points(ctx) && ctx->n_tgt) {
-    if (int rc = check_target(ctx, "sgb_linearize_batch", factor)) return rc;
-  }
-  if (int rc = pair_view(ctx)) return rc;
-  if (int rc = linearize_round(ctx, factor, robust, robust_c, rejector, max_dist_sq, T, active)) return rc;
-  return copy_out(ctx, out44, 44 * B);
+  return linearize_batch(ctx, "sgb_linearize_batch", false, factor, robust, robust_c, rejector, max_dist_sq, T, active, out44, nullptr, nullptr);
+}
+
+int sgb_linearize_batch_points(sgb_ctx* ctx, int factor, int robust, double robust_c, int rejector, double max_dist_sq, const double* T, const uint8_t* active,
+                               double* out44, double* out_point_e, double* out_point_Hb42) {
+  return linearize_batch(ctx, "sgb_linearize_batch_points", true, factor, robust, robust_c, rejector, max_dist_sq, T, active, out44, out_point_e, out_point_Hb42);
 }
 
 int sgb_error_batch(sgb_ctx* ctx, const double* T, const uint8_t* active, double* out_e) {
-  if (!ctx) return 1;
-  if (int rc = batch_check(ctx, "sgb_error_batch", T)) return rc;
-  if (!out_e) return fail(ctx, 1, "sgb_error_batch: null output");
-  const size_t B = batch_members(ctx);
-  if (B == 0) return 0;
-  if (!ctx->have_lin) return fail(ctx, 1, "sgb_error_batch: no preceding sgb_linearize_batch (the correspondences are cached there)");
-  for (size_t m = 0; m < B; m++)
-    if ((!active || active[m]) && !ctx->b_lin[m])
-      return fail(ctx, 1, "sgb_error_batch: member " + std::to_string(m) + " is active but has not been linearised against the current target");
-  if (int rc = pair_view(ctx)) return rc;
-  if (int rc = error_round(ctx, T, active)) return rc;
-  return copy_out(ctx, out_e, B);
+  return error_batch(ctx, "sgb_error_batch", false, T, active, out_e, nullptr);
+}
+
+int sgb_error_batch_points(sgb_ctx* ctx, const double* T, const uint8_t* active, double* out_e, double* out_point_e) {
+  return error_batch(ctx, "sgb_error_batch_points", true, T, active, out_e, out_point_e);
 }
 
 int sgb_align_batch(sgb_ctx* ctx, const sgb_align_options* o, const double* init_T, double* out_T, double* out_info, double* out_Hb) {

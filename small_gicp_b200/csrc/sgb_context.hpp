@@ -188,6 +188,7 @@ struct sgb_ctx {
   sgb::DevBuf b_vq, b_vcorr;               // virtual source of the search: transformed queries of the active members and what the search found
   sgb::DevBuf b_partials, b_out;           // per-tile partial sums, per-member results
   sgb::DevBuf b_state, b_phase;            // sgb_align_batch: per member MemberState / next round (kPhase*, one byte)
+  sgb::DevBuf b_rows_e, b_rows_hb;         // sgb_*_batch_points: the per-point rows staged for outputs that are not device memory
   // The clouds of sgb_source_set_batch are stored once (src_* and b_centres / b_bounds, cloud after cloud).  Without a pairing the
   // members are those clouds.  After sgb_source_set_pairs (b_paired) member p is a replica of one stored cloud in p_*, b_offsets are
   // the members' offsets, and b_pair_maps (empty: member m against map m) names each member's map.
