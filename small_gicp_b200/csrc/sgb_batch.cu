@@ -214,7 +214,7 @@ __device__ __forceinline__ void batch_factor_tile(const BatchParams& B, const ui
 
 // One CTA per tile of one member, for the target's KIND: 0 one point target, 1 one voxel map, 2 many voxel maps (member m against map m:
 // map_centres and map_regions), 3 many kd-trees (map_centres; vcorr = what forest_search_kernel found in map m), 4 submaps (S; vcorr and
-// S.centry = what submap_search_kernel found over the member's entries).  MODE: linearize, error() with the cached correspondences, or
+// S.centry = what forest_search_kernel<SUBMAP> found over the member's entries).  MODE: linearize, error() with the cached correspondences, or
 // either as the round's planner decided.  POINTS (host-planned modes only): every processed point's row to `rows` too.
 template <int FACTOR, int ROBUST, int KIND, int MODE, bool POINTS = false>
 __global__ void __launch_bounds__(kLinBlock, 4) batch_factor_kernel(const __grid_constant__ BatchParams B, const uint32_t* __restrict__ vcorr,

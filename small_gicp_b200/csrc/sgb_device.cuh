@@ -261,6 +261,151 @@ __device__ __forceinline__ void cta_box_centre(const double4* __restrict__ pts, 
   }
 }
 
+// ---------------------------------------------------------------------------------------------
+// kd-tree construction, shared by the single tree (sgb_kernels.cu) and many trees at once (sgb_forest.cu): a tree over n points is the
+// implicit balanced tree whose nodes at a level with `count` nodes own contiguous position ranges; its records are 64-byte packets.
+// ---------------------------------------------------------------------------------------------
+/// first point of node j at a level with `count` nodes (balanced implicit tree over n points)
+__device__ __forceinline__ uint32_t tree_bound(uint32_t j, uint32_t count, uint32_t n) {
+  return static_cast<uint32_t>((static_cast<uint64_t>(j) * n) / count);
+}
+/// node (at a level with `count` nodes) that owns position i
+__device__ __forceinline__ uint32_t tree_node_of(uint32_t i, uint32_t count, uint32_t n) {
+  return static_cast<uint32_t>(((static_cast<uint64_t>(i) + 1u) * count + n - 1u) / n) - 1u;
+}
+
+// boxes: count x 6 floats stored as order-preserving uints (lo xyz, hi xyz)
+__device__ __forceinline__ uint32_t float_flip(float f) {
+  const uint32_t u = __float_as_uint(f);
+  return u ^ ((u >> 31) ? 0xFFFFFFFFu : 0x80000000u);
+}
+__device__ __forceinline__ float float_unflip(uint32_t u) { return __uint_as_float(u ^ ((u >> 31) ? 0x80000000u : 0xFFFFFFFFu)); }
+
+/// the child record of heap node child_heap (> 0) in its parent's packet: box [lo, hi], a | b in the w lanes
+__device__ __forceinline__ void lbvh_store_child(float4* pnodes, uint32_t child_heap, const float lo[3], const float hi[3], uint32_t a, uint32_t b) {
+  const uint32_t parent = (child_heap - 1u) >> 1, side = (child_heap & 1u) ? 0u : 1u;  // odd heap index = left child
+  pnodes[parent * 4 + side * 2 + 0] = make_float4(lo[0], lo[1], lo[2], __uint_as_float(a));
+  pnodes[parent * 4 + side * 2 + 1] = make_float4(hi[0], hi[1], hi[2], __uint_as_float(b));
+}
+
+/// The bounding box of a leaf slot's (at most 32) consecutive points pts[base + first, base + last), one per lane of the warp: lo / hi in
+/// every lane (inverted for an empty slot, which no query enters).
+__device__ __forceinline__ void lbvh_leaf_box(const float4* __restrict__ pts, uint32_t base, uint32_t first, uint32_t last, uint32_t lane, float lo[3], float hi[3]) {
+  const uint32_t idx = first + lane;
+#pragma unroll
+  for (int a = 0; a < 3; a++) {
+    lo[a] = INFINITY;
+    hi[a] = -INFINITY;
+  }
+  if (idx < last) {
+    const float4 p = pts[base + idx];
+    lo[0] = hi[0] = p.x;
+    lo[1] = hi[1] = p.y;
+    lo[2] = hi[2] = p.z;
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+#pragma unroll
+    for (int a = 0; a < 3; a++) {
+      lo[a] = fminf(lo[a], __shfl_xor_sync(0xffffffffu, lo[a], o));
+      hi[a] = fmaxf(hi[a], __shfl_xor_sync(0xffffffffu, hi[a], o));
+    }
+  }
+}
+
+/// inner node `node` whose children's records are complete: their union box -> the parent's child record (a = node index, b = 0)
+__device__ __forceinline__ void lbvh_inner_record(float4* pnodes, uint32_t node) {
+  const float4 l0 = pnodes[node * 4 + 0], l1 = pnodes[node * 4 + 1], r0 = pnodes[node * 4 + 2], r1 = pnodes[node * 4 + 3];
+  const float lo[3] = {fminf(l0.x, r0.x), fminf(l0.y, r0.y), fminf(l0.z, r0.z)};
+  const float hi[3] = {fmaxf(l1.x, r1.x), fmaxf(l1.y, r1.y), fmaxf(l1.z, r1.z)};
+  lbvh_store_child(pnodes, node, lo, hi, node, 0u);
+}
+
+/// Shared-memory refinement: a node of at most kKdSegMax points, and at most kKdSegNodes nodes of it at one level, refined by one CTA.
+constexpr uint32_t kKdSegMax = 2048;
+constexpr uint32_t kKdSegNodes = 128;
+/// its dynamic shared memory: two point buffers, the keys and slots of the sort, the boxes of one level
+constexpr size_t kKdRefineSmem = 2 * kKdSegMax * sizeof(float4) + kKdSegMax * (sizeof(unsigned long long) + sizeof(uint32_t)) + kKdSegNodes * 6 * sizeof(uint32_t);
+
+/// The median-split refinement of a whole SUBTREE of at most kKdSegMax points by one CTA: node b of level `level0` of a tree of `levels`
+/// inner levels over the n points pts[0 .. n) (a contiguous position range) is loaded into shared memory and every remaining level runs
+/// there -- per level: node boxes (shared-memory atomics on order-preserving integer images of the floats), key = (node, coordinate along
+/// the node's widest axis), bitonic sort of (key, slot), permutation of the points.  The same keys and balanced position boundaries as one
+/// radix sort per level (ties may land differently -- any order is a valid tree).  The points go back to pts; perm[base + k] receives
+/// base + the w (original index within the tree) of the point at position k.
+__device__ __forceinline__ void kd_refine_segment(float4* __restrict__ pts, uint32_t* __restrict__ perm, uint32_t base, uint32_t b, uint32_t n, uint32_t level0,
+                                                  uint32_t levels) {
+  extern __shared__ __align__(16) unsigned char s_raw[];
+  float4* s_pts = reinterpret_cast<float4*>(s_raw);                                            // [2][kKdSegMax]
+  unsigned long long* s_key = reinterpret_cast<unsigned long long*>(s_raw + 2 * kKdSegMax * sizeof(float4));  // [kKdSegMax]
+  uint32_t* s_idx = reinterpret_cast<uint32_t*>(s_key + kKdSegMax);                            // [kKdSegMax]
+  uint32_t* s_box = s_idx + kKdSegMax;                                                         // [kKdSegNodes][6]
+  const uint32_t tid = threadIdx.x;
+  const uint32_t first = tree_bound(b, 1u << level0, n), last = tree_bound(b + 1u, 1u << level0, n), m = last - first;
+  for (uint32_t t = tid; t < m; t += blockDim.x) s_pts[t] = pts[first + t];
+  uint32_t cur = 0;
+  __syncthreads();
+  for (uint32_t level = level0; level < levels; level++) {
+    const uint32_t count = 1u << level, node_first = b << (level - level0), n_nodes = 1u << (level - level0);
+    for (uint32_t t = tid; t < n_nodes * 6u; t += blockDim.x) s_box[t] = (t % 6u) < 3u ? 0xFFFFFFFFu : 0u;
+    __syncthreads();
+    const float4* P0 = s_pts + cur * kKdSegMax;
+    for (uint32_t t = tid; t < m; t += blockDim.x) {
+      const float4 p = P0[t];
+      uint32_t* bx = s_box + (tree_node_of(first + t, count, n) - node_first) * 6u;
+      atomicMin(&bx[0], float_flip(p.x));
+      atomicMin(&bx[1], float_flip(p.y));
+      atomicMin(&bx[2], float_flip(p.z));
+      atomicMax(&bx[3], float_flip(p.x));
+      atomicMax(&bx[4], float_flip(p.y));
+      atomicMax(&bx[5], float_flip(p.z));
+    }
+    __syncthreads();
+    for (uint32_t t = tid; t < kKdSegMax; t += blockDim.x) {
+      unsigned long long key = ~0ull;  // padding sorts to the end
+      if (t < m) {
+        const uint32_t node = tree_node_of(first + t, count, n) - node_first;
+        const uint32_t* bx = s_box + node * 6u;
+        const float ex = float_unflip(bx[3]) - float_unflip(bx[0]), ey = float_unflip(bx[4]) - float_unflip(bx[1]), ez = float_unflip(bx[5]) - float_unflip(bx[2]);
+        const float4 p = P0[t];
+        const float c = ex >= ey ? (ex >= ez ? p.x : p.z) : (ey >= ez ? p.y : p.z);
+        key = (static_cast<unsigned long long>(node) << 32) | float_flip(c);
+      }
+      s_key[t] = key;
+      s_idx[t] = t;
+    }
+    __syncthreads();
+    // bitonic sort of (key, slot) over kKdSegMax entries: one compare-exchange per thread and step
+    for (uint32_t k = 2; k <= kKdSegMax; k <<= 1) {
+      for (uint32_t j = k >> 1; j > 0; j >>= 1) {
+        for (uint32_t t = tid; t < kKdSegMax / 2u; t += blockDim.x) {
+          const uint32_t lo = ((t & ~(j - 1u)) << 1) | (t & (j - 1u)), hi = lo | j;
+          const bool up = (lo & k) == 0u;
+          const unsigned long long a = s_key[lo], c = s_key[hi];
+          if ((a > c) == up) {
+            s_key[lo] = c;
+            s_key[hi] = a;
+            const uint32_t ia = s_idx[lo];
+            s_idx[lo] = s_idx[hi];
+            s_idx[hi] = ia;
+          }
+        }
+        __syncthreads();
+      }
+    }
+    float4* P1 = s_pts + (cur ^ 1u) * kKdSegMax;
+    for (uint32_t t = tid; t < m; t += blockDim.x) P1[t] = P0[s_idx[t]];
+    cur ^= 1u;
+    __syncthreads();
+  }
+  const float4* Pf = s_pts + cur * kKdSegMax;
+  for (uint32_t t = tid; t < m; t += blockDim.x) {
+    const float4 p = Pf[t];
+    pts[first + t] = p;
+    perm[base + first + t] = base + static_cast<uint32_t>(__float_as_int(p.w));  // w carries the original index through every permutation
+  }
+}
+
 // Sym3, the factor algebra and the per-point helpers live in sgb_math.cuh (also compiled for the host by tests/host_math).
 
 /// Exact nearest neighbour of q in the flattened kd-tree (restates the visiting order of

@@ -13,11 +13,12 @@
 //                               the caller sorts by (global node, coordinate along the node's widest axis) and re-gathers
 //   forest_refine_smem_kernel   every (map, subtree of <= kKdSegMax points) segment refined in shared memory, one CTA each
 //   forest_leaf_kernel / forest_level_kernel   the packet records of every map, one launch per tree level
+// The refinement and the record kernels run the single tree's helpers and bodies (sgb_device.cuh) on each map's part of the arrays.
 // Search:
 //   forest_search_kernel        one CTA per BatchTile (128 consecutive stored points of ONE member): warp-cooperative exact nearest-
-//                               neighbour walk over that member's map, as packet_search_kernel walks one tree
-//   submap_search_kernel        the same for submap members (sgb_source_set_submaps, DESIGN.md §11 "Submaps"): the walk over every map
-//                               of the member's list, each in its own stored frame, the bound carried from map to map
+//                               neighbour walk over that member's map, as packet_search_kernel walks one tree; with SUBMAP, the same
+//                               walk for submap members (sgb_source_set_submaps, DESIGN.md §11 "Submaps") over every map of the
+//                               member's list, each in its own stored frame, the bound carried from map to map
 // The same build over the preprocessing scratch serves sgb_estimate_features_batch (forest_features_kernel, sgb_preprocess.cu).
 #include <algorithm>
 #include <cfloat>
@@ -31,31 +32,12 @@ namespace sgb {
 
 namespace {
 
-// The helpers below are copies of tree_bound / tree_node_of / float_flip / float_unflip / lbvh_store_child in sgb_kernels.cu: sharing
-// them would change the code of the single-tree build kernels there.
-__device__ __forceinline__ uint32_t forest_bound(uint32_t j, uint32_t count, uint32_t n) {
-  return static_cast<uint32_t>((static_cast<uint64_t>(j) * n) / count);
-}
-__device__ __forceinline__ uint32_t forest_node_of(uint32_t i, uint32_t count, uint32_t n) {
-  return static_cast<uint32_t>(((static_cast<uint64_t>(i) + 1u) * count + n - 1u) / n) - 1u;
-}
-__device__ __forceinline__ uint32_t forest_flip(float f) {
-  const uint32_t u = __float_as_uint(f);
-  return u ^ ((u >> 31) ? 0xFFFFFFFFu : 0x80000000u);
-}
-__device__ __forceinline__ float forest_unflip(uint32_t u) { return __uint_as_float(u ^ ((u >> 31) ? 0x80000000u : 0xFFFFFFFFu)); }
-__device__ __forceinline__ void forest_store_child(float4* pnodes, uint32_t child_heap, const float lo[3], const float hi[3], uint32_t a, uint32_t b) {
-  const uint32_t parent = (child_heap - 1u) >> 1, side = (child_heap & 1u) ? 0u : 1u;  // odd heap index = left child
-  pnodes[parent * 4 + side * 2 + 0] = make_float4(lo[0], lo[1], lo[2], __uint_as_float(a));
-  pnodes[parent * 4 + side * 2 + 1] = make_float4(hi[0], hi[1], hi[2], __uint_as_float(b));
-}
-
 /// the node of map-local position `local` at radix level `level` as a global box / key id: the first shared-memory segment it covers
 /// (segments are map m's nodes at its level level0, numbered from seg_off[m]); ~0: the map is past its radix levels
 __device__ __forceinline__ uint32_t forest_level_node(const ForestTables& F, uint32_t m, uint32_t local, uint32_t n, uint32_t level) {
   const uint32_t l0 = __ldg(&F.level0[m]);
   if (level >= l0) return ~0u;
-  return __ldg(&F.seg_off[m]) + (forest_node_of(local, 1u << level, n) << (l0 - level));
+  return __ldg(&F.seg_off[m]) + (tree_node_of(local, 1u << level, n) << (l0 - level));
 }
 
 // one CTA per map: the centre of its box
@@ -104,7 +86,7 @@ __global__ void forest_boxes_kernel(const float4* __restrict__ pts, uint32_t n, 
   const uint32_t m = owner_of(F.pt_off, F.n_maps, idx), first = F.pt_off[m];
   const uint32_t node = forest_level_node(F, m, idx - first, F.pt_off[m + 1] - first, level);
   const float4 p = pts[idx];
-  uint32_t v[6] = {forest_flip(p.x), forest_flip(p.y), forest_flip(p.z), forest_flip(p.x), forest_flip(p.y), forest_flip(p.z)};
+  uint32_t v[6] = {float_flip(p.x), float_flip(p.y), float_flip(p.z), float_flip(p.x), float_flip(p.y), float_flip(p.z)};
   const uint32_t node0 = __shfl_sync(0xffffffffu, node, 0);
   if (__all_sync(0xffffffffu, node == node0)) {
     if (node0 == ~0u) return;
@@ -141,134 +123,47 @@ __global__ void forest_keys_kernel(const float4* __restrict__ pts, uint32_t n, c
     keys[i] = static_cast<uint64_t>(F.seg_off[m]) << 32;
     return;
   }
-  const float ex = forest_unflip(boxes[node * 6 + 3]) - forest_unflip(boxes[node * 6 + 0]);
-  const float ey = forest_unflip(boxes[node * 6 + 4]) - forest_unflip(boxes[node * 6 + 1]);
-  const float ez = forest_unflip(boxes[node * 6 + 5]) - forest_unflip(boxes[node * 6 + 2]);
+  const float ex = float_unflip(boxes[node * 6 + 3]) - float_unflip(boxes[node * 6 + 0]);
+  const float ey = float_unflip(boxes[node * 6 + 4]) - float_unflip(boxes[node * 6 + 1]);
+  const float ez = float_unflip(boxes[node * 6 + 5]) - float_unflip(boxes[node * 6 + 2]);
   const float4 p = pts[i];
   const float c = ex >= ey ? (ex >= ez ? p.x : p.z) : (ey >= ez ? p.y : p.z);
-  keys[i] = (static_cast<uint64_t>(node) << 32) | forest_flip(c);
+  keys[i] = (static_cast<uint64_t>(node) << 32) | float_flip(c);
 }
 
-// A copy of kd_refine_smem_kernel (sgb_kernels.cu) over every map's segments: CTA b owns segment b - seg_off[m] of map m (a node of
-// its level level0 with at most kKdSegMax points) and runs its remaining levels down to the leaves in shared memory.  perm receives
-// global original positions (the map's first position + w).
+// kd_refine_smem_kernel over every map's segments: CTA b refines segment b - seg_off[m] of map m (a node of its level level0 with at
+// most kKdSegMax points).  perm receives global original positions (the map's first position + w).
 __global__ void __launch_bounds__(1024) forest_refine_smem_kernel(float4* __restrict__ leaf_pts, uint32_t* __restrict__ perm, const ForestTables F) {
-  extern __shared__ __align__(16) unsigned char s_raw[];
-  float4* s_pts = reinterpret_cast<float4*>(s_raw);                                                        // [2][kForestSegMax]
-  unsigned long long* s_key = reinterpret_cast<unsigned long long*>(s_raw + 2 * kForestSegMax * sizeof(float4));  // [kForestSegMax]
-  uint32_t* s_idx = reinterpret_cast<uint32_t*>(s_key + kForestSegMax);                                   // [kForestSegMax]
-  uint32_t* s_box = s_idx + kForestSegMax;                                                                // [kForestSegNodes][6]
-  const uint32_t tid = threadIdx.x;
   const uint32_t map = owner_of(F.seg_off, F.n_maps, blockIdx.x);
   const uint32_t b = blockIdx.x - F.seg_off[map], base = F.pt_off[map], n = F.pt_off[map + 1] - base;
-  const uint32_t level0 = F.level0[map], levels = F.depth[map];
-  const uint32_t first = forest_bound(b, 1u << level0, n), last = forest_bound(b + 1u, 1u << level0, n), m = last - first;
-  float4* pts = leaf_pts + base;
-  for (uint32_t t = tid; t < m; t += blockDim.x) s_pts[t] = pts[first + t];
-  uint32_t cur = 0;
-  __syncthreads();
-  for (uint32_t level = level0; level < levels; level++) {
-    const uint32_t count = 1u << level, node_first = b << (level - level0), n_nodes = 1u << (level - level0);
-    for (uint32_t t = tid; t < n_nodes * 6u; t += blockDim.x) s_box[t] = (t % 6u) < 3u ? 0xFFFFFFFFu : 0u;
-    __syncthreads();
-    const float4* P0 = s_pts + cur * kForestSegMax;
-    for (uint32_t t = tid; t < m; t += blockDim.x) {
-      const float4 p = P0[t];
-      uint32_t* bx = s_box + (forest_node_of(first + t, count, n) - node_first) * 6u;
-      atomicMin(&bx[0], forest_flip(p.x));
-      atomicMin(&bx[1], forest_flip(p.y));
-      atomicMin(&bx[2], forest_flip(p.z));
-      atomicMax(&bx[3], forest_flip(p.x));
-      atomicMax(&bx[4], forest_flip(p.y));
-      atomicMax(&bx[5], forest_flip(p.z));
-    }
-    __syncthreads();
-    for (uint32_t t = tid; t < kForestSegMax; t += blockDim.x) {
-      unsigned long long key = ~0ull;  // padding sorts to the end
-      if (t < m) {
-        const uint32_t node = forest_node_of(first + t, count, n) - node_first;
-        const uint32_t* bx = s_box + node * 6u;
-        const float ex = forest_unflip(bx[3]) - forest_unflip(bx[0]), ey = forest_unflip(bx[4]) - forest_unflip(bx[1]), ez = forest_unflip(bx[5]) - forest_unflip(bx[2]);
-        const float4 p = P0[t];
-        const float c = ex >= ey ? (ex >= ez ? p.x : p.z) : (ey >= ez ? p.y : p.z);
-        key = (static_cast<unsigned long long>(node) << 32) | forest_flip(c);
-      }
-      s_key[t] = key;
-      s_idx[t] = t;
-    }
-    __syncthreads();
-    for (uint32_t k = 2; k <= kForestSegMax; k <<= 1) {
-      for (uint32_t j = k >> 1; j > 0; j >>= 1) {
-        for (uint32_t t = tid; t < kForestSegMax / 2u; t += blockDim.x) {
-          const uint32_t lo = ((t & ~(j - 1u)) << 1) | (t & (j - 1u)), hi = lo | j;
-          const bool up = (lo & k) == 0u;
-          const unsigned long long a = s_key[lo], c = s_key[hi];
-          if ((a > c) == up) {
-            s_key[lo] = c;
-            s_key[hi] = a;
-            const uint32_t ia = s_idx[lo];
-            s_idx[lo] = s_idx[hi];
-            s_idx[hi] = ia;
-          }
-        }
-        __syncthreads();
-      }
-    }
-    float4* P1 = s_pts + (cur ^ 1u) * kForestSegMax;
-    for (uint32_t t = tid; t < m; t += blockDim.x) P1[t] = P0[s_idx[t]];
-    cur ^= 1u;
-    __syncthreads();
-  }
-  const float4* Pf = s_pts + cur * kForestSegMax;
-  for (uint32_t t = tid; t < m; t += blockDim.x) {
-    const float4 p = Pf[t];
-    pts[first + t] = p;
-    perm[base + first + t] = base + static_cast<uint32_t>(__float_as_int(p.w));
-  }
+  kd_refine_segment(leaf_pts + base, perm, base, b, n, F.level0[map], F.depth[map]);
 }
 
-// one warp per leaf slot of any map (lbvh_leaf_kernel in sgb_kernels.cu): bounding box of its points -> the parent's child record in the
-// map's record block; a = the leaf's first GLOBAL position
+// one warp per leaf slot of any map (lbvh_leaf_kernel in sgb_kernels.cu): the record in the map's record block, a = the leaf's first
+// GLOBAL position
 __global__ void forest_leaf_kernel(const float4* __restrict__ leaf_pts, const ForestTables F, uint32_t n_slots, float4* pnodes) {
   const uint32_t slot = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31u;
   if (slot >= n_slots) return;
   const uint32_t m = owner_of(F.slot_off, F.n_maps, slot);
   const uint32_t j = slot - F.slot_off[m], P = F.slot_off[m + 1] - F.slot_off[m];
   const uint32_t base = F.pt_off[m], n = F.pt_off[m + 1] - base;
-  const uint32_t first = forest_bound(j, P, n), last = forest_bound(j + 1u, P, n), idx = first + lane;
-  float lo[3] = {INFINITY, INFINITY, INFINITY}, hi[3] = {-INFINITY, -INFINITY, -INFINITY};
-  if (idx < last) {
-    const float4 p = leaf_pts[base + idx];
-    lo[0] = hi[0] = p.x;
-    lo[1] = hi[1] = p.y;
-    lo[2] = hi[2] = p.z;
-  }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-#pragma unroll
-    for (int a = 0; a < 3; a++) {
-      lo[a] = fminf(lo[a], __shfl_xor_sync(0xffffffffu, lo[a], o));
-      hi[a] = fmaxf(hi[a], __shfl_xor_sync(0xffffffffu, hi[a], o));
-    }
-  }
+  const uint32_t first = tree_bound(j, P, n), last = tree_bound(j + 1u, P, n);
+  float lo[3], hi[3];
+  lbvh_leaf_box(leaf_pts, base, first, last, lane, lo, hi);
   if (lane == 0) {
     const uint32_t cnt = last - first;
-    forest_store_child(pnodes + 4 * static_cast<size_t>(F.node_base[m]), (P - 1u) + j, lo, hi, cnt ? base + first : 0u, cnt);
+    lbvh_store_child(pnodes + 4 * static_cast<size_t>(F.node_base[m]), (P - 1u) + j, lo, hi, cnt ? base + first : 0u, cnt);
   }
 }
 
-// the inner nodes at `level` of every map that has that level (lbvh_level_kernel in sgb_kernels.cu): union box -> the parent's record
+// the inner nodes at `level` of every map that has that level (lbvh_level_kernel in sgb_kernels.cu)
 __global__ void forest_level_kernel(const ForestTables F, uint32_t level, float4* pnodes) {
   const uint64_t total = static_cast<uint64_t>(F.n_maps) << level;
   for (uint64_t t = blockIdx.x * static_cast<uint64_t>(blockDim.x) + threadIdx.x; t < total; t += static_cast<uint64_t>(gridDim.x) * blockDim.x) {
     const uint32_t m = static_cast<uint32_t>(t >> level);
     if (F.depth[m] <= level) continue;  // the map's inner levels are 0 .. depth - 1
     const uint32_t node = ((1u << level) - 1u) + static_cast<uint32_t>(t & ((1ull << level) - 1ull));
-    float4* nodes = pnodes + 4 * static_cast<size_t>(F.node_base[m]);
-    const float4 l0 = nodes[node * 4 + 0], l1 = nodes[node * 4 + 1], r0 = nodes[node * 4 + 2], r1 = nodes[node * 4 + 3];
-    const float lo[3] = {fminf(l0.x, r0.x), fminf(l0.y, r0.y), fminf(l0.z, r0.z)};
-    const float hi[3] = {fmaxf(l1.x, r1.x), fmaxf(l1.y, r1.y), fmaxf(l1.z, r1.z)};
-    forest_store_child(nodes, node, lo, hi, node, 0u);
+    lbvh_inner_record(pnodes + 4 * static_cast<size_t>(F.node_base[m]), node);
   }
 }
 
@@ -277,15 +172,32 @@ constexpr int kForestWarps = kLinBlock / 32;
 constexpr int kForestDenseLanes = 18;  // as kPacketDenseLanes (sgb_kernels_packet.cu)
 constexpr int kForestStack = 40;
 
+// The FP32 query of stored point sp of member m in the stored frame of submap entry e: the member's pose carried through the inverse of
+// the entry's placement, then centred on the entry's map as forest_search_kernel centres on map m.
+__device__ __forceinline__ float3 submap_query(const SubmapView& S, uint32_t e, const BatchParams& B, uint32_t m, const float4& sp) {
+  const double* cs = B.centres + 4 * static_cast<size_t>(m);
+  double Tk[12];
+  relative_pose(S.inv_poses + 12 * static_cast<size_t>(e), B.poses + 12 * static_cast<size_t>(m), Tk);
+  const double3 tp = centred_translation(Tk, cs[0], cs[1], cs[2], S.centres + 4 * static_cast<size_t>(e));
+  return centred_query_f32(Tk, tp, sp);
+}
+
 // One CTA per BatchTile: warp w takes the tile's points 32 w .. 32 w + 31, all of ONE member m, and walks map m's tree once for all of
 // them -- the walk of packet_search_kernel (sgb_kernels_packet.cu): one shared stack, warp votes, warp-uniform node and leaf loads, the
 // dense scan (every lane tests every point) or the sparse one (the whole warp serves one interested lane at a time).  Nothing of any
 // other member enters a warp, so a member's correspondences depend on its own points, pose and seeds only.
+// SUBMAP (submap members, sgb_source_set_submaps; F.pnodes = every map's records, F's tables unused): the same walk over the tree of
+// every entry of the member's list in list order, each in its map's own stored frame.  Rigid placements preserve distances, so the
+// nearest point of the placed union is the nearest over the entries, and best_d carried from entry to entry prunes the later trees: one
+// that no lane's ball reaches costs its root record's two box tests.  Only a strictly nearer point replaces the best, so at an exact FP32
+// tie between two entries the earlier one wins.  The seed is evaluated in the frame of the entry that owned it.  Without SUBMAP, S is
+// not read.
 // ROUND (a round of sgb_align_batch_async): the grid is sized for every tile, the round's tile count is read from the device and the CTAs
 // beyond it (all of them in an error() round) exit at once.
-template <bool ROUND>
-__global__ void __launch_bounds__(kLinBlock, 8) forest_search_kernel(const __grid_constant__ BatchParams B, const __grid_constant__ ForestView F,
-                                                                     float bound, uint32_t* __restrict__ vcorr, const BatchRound* __restrict__ round) {
+template <bool ROUND, bool SUBMAP>
+__global__ void __launch_bounds__(kLinBlock, SUBMAP ? 7 : 8) forest_search_kernel(const __grid_constant__ BatchParams B, const __grid_constant__ ForestView F,
+                                                                                  float bound, uint32_t* __restrict__ vcorr, const BatchRound* __restrict__ round,
+                                                                                  const __grid_constant__ SubmapView S) {
   if constexpr (ROUND) {
     const BatchRound r = *round;
     if (!r.lin || blockIdx.x >= r.n_tiles) return;
@@ -298,310 +210,47 @@ __global__ void __launch_bounds__(kLinBlock, 8) forest_search_kernel(const __gri
   const uint32_t m = t.member;
   const bool valid = threadIdx.x < t.count;
   const uint32_t i = t.first + threadIdx.x, v = t.vfirst + threadIdx.x;
-  const uint32_t n_map = F.pt_off[m + 1] - F.pt_off[m];
-  if (n_map == 0) {
-    if (valid) vcorr[v] = kNone;
-    return;
+  const uint32_t e0 = SUBMAP ? __ldg(&S.entry_off[m]) : 0u, e1 = SUBMAP ? __ldg(&S.entry_off[m + 1]) : 1u;  // the member's entries
+  if constexpr (!SUBMAP) {
+    const uint32_t n_map = F.pt_off[m + 1] - F.pt_off[m];
+    if (n_map == 0) {
+      if (valid) vcorr[v] = kNone;
+      return;
+    }
   }
-  const float4* __restrict__ pnodes = F.pnodes + 4 * static_cast<size_t>(F.node_base[m]);
+  const float4* __restrict__ pnodes = SUBMAP ? F.pnodes : F.pnodes + 4 * static_cast<size_t>(F.node_base[m]);
   const float4* __restrict__ pts = B.tgt.pts;
   float* my_dist = s_dist + threadIdx.x;
   uint2* my_child = s_child[wib];
 
   float fx = 0.f, fy = 0.f, fz = 0.f;
   float best_d = -1.0f;  // an idle lane is never interested in anything
-  uint32_t best = kNone;
+  uint32_t best = kNone, best_e = 0;
+  const float4 p = (SUBMAP && valid) ? __ldg(&B.pts[i]) : make_float4(0.f, 0.f, 0.f, 0.f);  // SUBMAP: the stored point
   if (valid) {
-    const double* R = B.poses + 12 * static_cast<size_t>(m);
-    const double* cs = B.centres + 4 * static_cast<size_t>(m);
-    const double3 tp = centred_translation(R, cs[0], cs[1], cs[2], F.centres + 4 * static_cast<size_t>(m));
-    const float3 f = centred_query_f32(R, tp, __ldg(&B.pts[i]));
-    fx = f.x;
-    fy = f.y;
-    fz = f.z;
+    if constexpr (!SUBMAP) {
+      const double* R = B.poses + 12 * static_cast<size_t>(m);
+      const double* cs = B.centres + 4 * static_cast<size_t>(m);
+      const double3 tp = centred_translation(R, cs[0], cs[1], cs[2], F.centres + 4 * static_cast<size_t>(m));
+      const float3 f = centred_query_f32(R, tp, __ldg(&B.pts[i]));
+      fx = f.x;
+      fy = f.y;
+      fz = f.z;
+    }
     best_d = bound;
     // the member's previous correspondence: an upper bound only prunes
     const uint32_t prev = (B.members[m].z & kMemberSeeded) ? B.corr[i] : kNone;
     if (prev != kNone) {
+      uint32_t pe = 0;  // SUBMAP: the entry it lies in
+      if constexpr (SUBMAP) {
+        pe = S.centry[i];
+        const float3 f = submap_query(S, e0 + pe, B, m, p);
+        fx = f.x;
+        fy = f.y;
+        fz = f.z;
+      }
       const float4 q = __ldg(&pts[prev]);
       const float dx = q.x - fx, dy = q.y - fy, dz = q.z - fz;
-      const float d = dx * dx + dy * dy + dz * dz;
-      if (d < best_d) {
-        best_d = d;
-        best = prev;
-      }
-    }
-  }
-
-  // This walk exists twice: forest_walk below (used by submap_search_kernel) is a copy of it.  A change to one belongs in the other.
-  int sp = 0;
-  uint32_t cur = 0;    // inner node being expanded (index within the map's record block)
-  bool expand = true;  // false: nothing to expand, take the next pending subtree
-  uint32_t leaf_first = 0, leaf_cnt = 0;
-  float leaf_d = 0.f;
-  for (;;) {
-    if (expand) {
-      const float4 n0 = __ldg(&pnodes[cur * 4 + 0]), n1 = __ldg(&pnodes[cur * 4 + 1]);
-      const float4 n2 = __ldg(&pnodes[cur * 4 + 2]), n3 = __ldg(&pnodes[cur * 4 + 3]);
-      const float dl = box_dist2(fx, fy, fz, n0, n1), dr = box_dist2(fx, fy, fz, n2, n3);
-      const bool wl = dl < best_d, wr = dr < best_d;
-      const unsigned ml = __ballot_sync(0xffffffffu, wl), mr = __ballot_sync(0xffffffffu, wr);
-      uint32_t ca, cb;
-      if (ml && mr) {
-        const unsigned closer_l = __ballot_sync(0xffffffffu, (wl || wr) && dl <= dr);
-        const bool left_first = 2 * __popc(closer_l) >= __popc(ml | mr);
-        my_dist[sp * kLinBlock] = left_first ? dr : dl;
-        if (lane == 0) my_child[sp] = left_first ? make_uint2(__float_as_uint(n2.w), __float_as_uint(n3.w)) : make_uint2(__float_as_uint(n0.w), __float_as_uint(n1.w));
-        sp++;
-        ca = left_first ? __float_as_uint(n0.w) : __float_as_uint(n2.w);
-        cb = left_first ? __float_as_uint(n1.w) : __float_as_uint(n3.w);
-        leaf_d = left_first ? dl : dr;
-      } else if (ml) {
-        ca = __float_as_uint(n0.w);
-        cb = __float_as_uint(n1.w);
-        leaf_d = dl;
-      } else if (mr) {
-        ca = __float_as_uint(n2.w);
-        cb = __float_as_uint(n3.w);
-        leaf_d = dr;
-      } else {
-        expand = false;
-        continue;
-      }
-      if (cb == 0u) {  // inner child
-        cur = ca;
-        continue;
-      }
-      leaf_first = ca;
-      leaf_cnt = cb;
-    } else {
-      bool got = false;
-      uint2 c = make_uint2(0u, 0u);
-      while (sp > 0) {
-        sp--;
-        const float d = my_dist[sp * kLinBlock];
-        if (__any_sync(0xffffffffu, d < best_d)) {
-          __syncwarp();  // lane 0's push of this entry is visible
-          c = my_child[sp];
-          __syncwarp();  // ... and every lane has read it before lane 0 may push over it
-          leaf_d = d;
-          got = true;
-          break;
-        }
-      }
-      if (!got) break;
-      if (c.y == 0u) {
-        cur = c.x;
-        expand = true;
-        continue;
-      }
-      leaf_first = c.x;
-      leaf_cnt = c.y;
-    }
-    // ---- leaf (global positions) ----
-    const unsigned want = __ballot_sync(0xffffffffu, leaf_d < best_d);
-    if (__popc(want) > kForestDenseLanes) {
-      const float4* lp = pts + leaf_first;
-#pragma unroll 4
-      for (uint32_t j = 0; j < leaf_cnt; j++) {
-        const float4 q = __ldg(&lp[j]);
-        const float dx = q.x - fx, dy = q.y - fy, dz = q.z - fz;
-        const float d = dx * dx + dy * dy + dz * dz;
-        if (d < best_d) {
-          best_d = d;
-          best = leaf_first + j;
-        }
-      }
-    } else {
-      for (uint32_t base = 0; base < leaf_cnt; base += 32u) {
-        const uint32_t j = base + lane;
-        float4 q = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (j < leaf_cnt) q = __ldg(&pts[leaf_first + j]);
-        unsigned todo = want;
-        while (todo) {
-          const int src = __ffs(todo) - 1;
-          todo &= todo - 1;
-          const float qx = __shfl_sync(0xffffffffu, fx, src), qy = __shfl_sync(0xffffffffu, fy, src), qz = __shfl_sync(0xffffffffu, fz, src);
-          const float dx = q.x - qx, dy = q.y - qy, dz = q.z - qz;
-          const uint32_t dbits = j < leaf_cnt ? __float_as_uint(dx * dx + dy * dy + dz * dz) : 0x7f800000u;
-          const uint32_t dmin = __reduce_min_sync(0xffffffffu, dbits);
-          const unsigned who = __ballot_sync(0xffffffffu, dbits == dmin);  // lowest lane = first point in scan order
-          if (static_cast<int>(lane) == src) {
-            const float d = __uint_as_float(dmin);
-            if (d < best_d) {
-              best_d = d;
-              best = leaf_first + base + (__ffs(who) - 1);
-            }
-          }
-        }
-      }
-    }
-    expand = false;
-  }
-  __syncwarp();
-  if (valid) vcorr[v] = best;
-}
-
-// forest_search_kernel's walk of one tree's record block for the 32 queries of a warp, as a function: a copy, because calling it from
-// forest_search_kernel changes that kernel's register allocation (56 instead of 64 registers, other code).  best_d enters as each
-// lane's bound (< 0: an idle lane) and only a strictly nearer point replaces best.  Keep the two walks equal.
-__device__ __forceinline__ void forest_walk(const float4* __restrict__ pnodes, const float4* __restrict__ pts, float fx, float fy, float fz, float& best_d,
-                                            uint32_t& best, float* my_dist, uint2* my_child, uint32_t lane) {
-  int sp = 0;
-  uint32_t cur = 0;    // inner node being expanded (index within the map's record block)
-  bool expand = true;  // false: nothing to expand, take the next pending subtree
-  uint32_t leaf_first = 0, leaf_cnt = 0;
-  float leaf_d = 0.f;
-  for (;;) {
-    if (expand) {
-      const float4 n0 = __ldg(&pnodes[cur * 4 + 0]), n1 = __ldg(&pnodes[cur * 4 + 1]);
-      const float4 n2 = __ldg(&pnodes[cur * 4 + 2]), n3 = __ldg(&pnodes[cur * 4 + 3]);
-      const float dl = box_dist2(fx, fy, fz, n0, n1), dr = box_dist2(fx, fy, fz, n2, n3);
-      const bool wl = dl < best_d, wr = dr < best_d;
-      const unsigned ml = __ballot_sync(0xffffffffu, wl), mr = __ballot_sync(0xffffffffu, wr);
-      uint32_t ca, cb;
-      if (ml && mr) {
-        const unsigned closer_l = __ballot_sync(0xffffffffu, (wl || wr) && dl <= dr);
-        const bool left_first = 2 * __popc(closer_l) >= __popc(ml | mr);
-        my_dist[sp * kLinBlock] = left_first ? dr : dl;
-        if (lane == 0) my_child[sp] = left_first ? make_uint2(__float_as_uint(n2.w), __float_as_uint(n3.w)) : make_uint2(__float_as_uint(n0.w), __float_as_uint(n1.w));
-        sp++;
-        ca = left_first ? __float_as_uint(n0.w) : __float_as_uint(n2.w);
-        cb = left_first ? __float_as_uint(n1.w) : __float_as_uint(n3.w);
-        leaf_d = left_first ? dl : dr;
-      } else if (ml) {
-        ca = __float_as_uint(n0.w);
-        cb = __float_as_uint(n1.w);
-        leaf_d = dl;
-      } else if (mr) {
-        ca = __float_as_uint(n2.w);
-        cb = __float_as_uint(n3.w);
-        leaf_d = dr;
-      } else {
-        expand = false;
-        continue;
-      }
-      if (cb == 0u) {  // inner child
-        cur = ca;
-        continue;
-      }
-      leaf_first = ca;
-      leaf_cnt = cb;
-    } else {
-      bool got = false;
-      uint2 c = make_uint2(0u, 0u);
-      while (sp > 0) {
-        sp--;
-        const float d = my_dist[sp * kLinBlock];
-        if (__any_sync(0xffffffffu, d < best_d)) {
-          __syncwarp();  // lane 0's push of this entry is visible
-          c = my_child[sp];
-          __syncwarp();  // ... and every lane has read it before lane 0 may push over it
-          leaf_d = d;
-          got = true;
-          break;
-        }
-      }
-      if (!got) break;
-      if (c.y == 0u) {
-        cur = c.x;
-        expand = true;
-        continue;
-      }
-      leaf_first = c.x;
-      leaf_cnt = c.y;
-    }
-    // ---- leaf (global positions) ----
-    const unsigned want = __ballot_sync(0xffffffffu, leaf_d < best_d);
-    if (__popc(want) > kForestDenseLanes) {
-      const float4* lp = pts + leaf_first;
-#pragma unroll 4
-      for (uint32_t j = 0; j < leaf_cnt; j++) {
-        const float4 q = __ldg(&lp[j]);
-        const float dx = q.x - fx, dy = q.y - fy, dz = q.z - fz;
-        const float d = dx * dx + dy * dy + dz * dz;
-        if (d < best_d) {
-          best_d = d;
-          best = leaf_first + j;
-        }
-      }
-    } else {
-      for (uint32_t base = 0; base < leaf_cnt; base += 32u) {
-        const uint32_t j = base + lane;
-        float4 q = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (j < leaf_cnt) q = __ldg(&pts[leaf_first + j]);
-        unsigned todo = want;
-        while (todo) {
-          const int src = __ffs(todo) - 1;
-          todo &= todo - 1;
-          const float qx = __shfl_sync(0xffffffffu, fx, src), qy = __shfl_sync(0xffffffffu, fy, src), qz = __shfl_sync(0xffffffffu, fz, src);
-          const float dx = q.x - qx, dy = q.y - qy, dz = q.z - qz;
-          const uint32_t dbits = j < leaf_cnt ? __float_as_uint(dx * dx + dy * dy + dz * dz) : 0x7f800000u;
-          const uint32_t dmin = __reduce_min_sync(0xffffffffu, dbits);
-          const unsigned who = __ballot_sync(0xffffffffu, dbits == dmin);  // lowest lane = first point in scan order
-          if (static_cast<int>(lane) == src) {
-            const float d = __uint_as_float(dmin);
-            if (d < best_d) {
-              best_d = d;
-              best = leaf_first + base + (__ffs(who) - 1);
-            }
-          }
-        }
-      }
-    }
-    expand = false;
-  }
-}
-
-// The FP32 query of stored point sp of a member at pose T (centre cs) in the stored frame of submap entry e: the member's pose carried
-// through the inverse of the entry's placement, then centred on the entry's map as forest_search_kernel centres on map m.
-__device__ __forceinline__ float3 submap_query(const SubmapView& S, uint32_t e, const double* T, const double* cs, const float4& sp) {
-  double Tk[12];
-  relative_pose(S.inv_poses + 12 * static_cast<size_t>(e), T, Tk);
-  const double3 tp = centred_translation(Tk, cs[0], cs[1], cs[2], S.centres + 4 * static_cast<size_t>(e));
-  return centred_query_f32(Tk, tp, sp);
-}
-
-// forest_search_kernel for submap members (sgb_source_set_submaps): the warp still owns 32 consecutive stored points of ONE member, and
-// walks the tree of every entry of that member's list in list order, each in its map's own stored frame.  Rigid placements preserve
-// distances, so the nearest point of the placed union is the nearest over the entries, and best_d carried from entry to entry prunes
-// the later trees: one that no lane's ball reaches costs its root record's two box tests.  Only a strictly nearer point replaces the
-// best, so at an exact FP32 tie between two entries the earlier one wins.  The seed is evaluated in the frame of the entry that owned it.
-// ROUND: as for forest_search_kernel.
-template <bool ROUND>
-__global__ void __launch_bounds__(kLinBlock, 7) submap_search_kernel(const __grid_constant__ BatchParams B, const float4* __restrict__ all_pnodes,
-                                                                     const __grid_constant__ SubmapView S, float bound, uint32_t* __restrict__ vcorr,
-                                                                     const BatchRound* __restrict__ round) {
-  if constexpr (ROUND) {
-    const BatchRound r = *round;
-    if (!r.lin || blockIdx.x >= r.n_tiles) return;
-  }
-  extern __shared__ float s_dist[];  // [max_depth][kLinBlock] per-lane box distance of each pending subtree
-  __shared__ uint2 s_child[kForestWarps][kForestStack];
-  const BatchTile t = B.tiles[blockIdx.x];
-  const uint32_t lane = threadIdx.x & 31u, wib = threadIdx.x >> 5;
-  if (wib * 32u >= t.count) return;  // warp-uniform; no CTA barrier below
-  const uint32_t m = t.member;
-  const bool valid = threadIdx.x < t.count;
-  const uint32_t i = t.first + threadIdx.x, v = t.vfirst + threadIdx.x;
-  const uint32_t e0 = __ldg(&S.entry_off[m]), e1 = __ldg(&S.entry_off[m + 1]);
-  const float4* __restrict__ pts = B.tgt.pts;
-  const double* T = B.poses + 12 * static_cast<size_t>(m);
-  const double* cs = B.centres + 4 * static_cast<size_t>(m);
-  float* my_dist = s_dist + threadIdx.x;
-  uint2* my_child = s_child[wib];
-
-  const float4 sp = valid ? __ldg(&B.pts[i]) : make_float4(0.f, 0.f, 0.f, 0.f);
-  float best_d = valid ? bound : -1.0f;  // an idle lane is never interested in anything
-  uint32_t best = kNone, best_e = 0;
-  if (valid && (B.members[m].z & kMemberSeeded)) {
-    // the member's previous correspondence: an upper bound only prunes
-    const uint32_t prev = B.corr[i];
-    if (prev != kNone) {
-      const uint32_t pe = S.centry[i];
-      const float3 f = submap_query(S, e0 + pe, T, cs, sp);
-      const float4 q = __ldg(&pts[prev]);
-      const float dx = q.x - f.x, dy = q.y - f.y, dz = q.z - f.z;
       const float d = dx * dx + dy * dy + dz * dz;
       if (d < best_d) {
         best_d = d;
@@ -610,18 +259,132 @@ __global__ void __launch_bounds__(kLinBlock, 7) submap_search_kernel(const __gri
       }
     }
   }
-  for (uint32_t e = e0; e < e1; e++) {
-    const uint4 ent = __ldg(&S.entries[e]);
-    if (ent.y == 0u) continue;  // an empty map
-    const float3 f = submap_query(S, e, T, cs, sp);
+
+  // One walk per entry.  Without SUBMAP the loop condition is constant false, so no loop is emitted around the walk: a loop there, even
+  // one that runs once, changes the code of the one-map-per-member search.
+  uint32_t e = e0;
+  if (e < e1) do {
+    const float4* __restrict__ tree = pnodes;  // the records walked
+    if constexpr (SUBMAP) {
+      const uint4 ent = __ldg(&S.entries[e]);
+      if (ent.y == 0u) continue;  // an empty map
+      const float3 f = submap_query(S, e, B, m, p);
+      fx = f.x;
+      fy = f.y;
+      fz = f.z;
+      tree = pnodes + 4 * static_cast<size_t>(ent.z);
+    }
     const float before = best_d;
-    forest_walk(all_pnodes + 4 * static_cast<size_t>(ent.z), pts, f.x, f.y, f.z, best_d, best, my_dist, my_child, lane);
+    int sp = 0;
+    uint32_t cur = 0;    // inner node being expanded (index within the map's record block)
+    bool expand = true;  // false: nothing to expand, take the next pending subtree
+    uint32_t leaf_first = 0, leaf_cnt = 0;
+    float leaf_d = 0.f;
+    for (;;) {
+      if (expand) {
+        const float4 n0 = __ldg(&tree[cur * 4 + 0]), n1 = __ldg(&tree[cur * 4 + 1]);
+        const float4 n2 = __ldg(&tree[cur * 4 + 2]), n3 = __ldg(&tree[cur * 4 + 3]);
+        const float dl = box_dist2(fx, fy, fz, n0, n1), dr = box_dist2(fx, fy, fz, n2, n3);
+        const bool wl = dl < best_d, wr = dr < best_d;
+        const unsigned ml = __ballot_sync(0xffffffffu, wl), mr = __ballot_sync(0xffffffffu, wr);
+        uint32_t ca, cb;
+        if (ml && mr) {
+          const unsigned closer_l = __ballot_sync(0xffffffffu, (wl || wr) && dl <= dr);
+          const bool left_first = 2 * __popc(closer_l) >= __popc(ml | mr);
+          my_dist[sp * kLinBlock] = left_first ? dr : dl;
+          if (lane == 0) my_child[sp] = left_first ? make_uint2(__float_as_uint(n2.w), __float_as_uint(n3.w)) : make_uint2(__float_as_uint(n0.w), __float_as_uint(n1.w));
+          sp++;
+          ca = left_first ? __float_as_uint(n0.w) : __float_as_uint(n2.w);
+          cb = left_first ? __float_as_uint(n1.w) : __float_as_uint(n3.w);
+          leaf_d = left_first ? dl : dr;
+        } else if (ml) {
+          ca = __float_as_uint(n0.w);
+          cb = __float_as_uint(n1.w);
+          leaf_d = dl;
+        } else if (mr) {
+          ca = __float_as_uint(n2.w);
+          cb = __float_as_uint(n3.w);
+          leaf_d = dr;
+        } else {
+          expand = false;
+          continue;
+        }
+        if (cb == 0u) {  // inner child
+          cur = ca;
+          continue;
+        }
+        leaf_first = ca;
+        leaf_cnt = cb;
+      } else {
+        bool got = false;
+        uint2 c = make_uint2(0u, 0u);
+        while (sp > 0) {
+          sp--;
+          const float d = my_dist[sp * kLinBlock];
+          if (__any_sync(0xffffffffu, d < best_d)) {
+            __syncwarp();  // lane 0's push of this entry is visible
+            c = my_child[sp];
+            __syncwarp();  // ... and every lane has read it before lane 0 may push over it
+            leaf_d = d;
+            got = true;
+            break;
+          }
+        }
+        if (!got) break;
+        if (c.y == 0u) {
+          cur = c.x;
+          expand = true;
+          continue;
+        }
+        leaf_first = c.x;
+        leaf_cnt = c.y;
+      }
+      // ---- leaf (global positions) ----
+      const unsigned want = __ballot_sync(0xffffffffu, leaf_d < best_d);
+      if (__popc(want) > kForestDenseLanes) {
+        const float4* lp = pts + leaf_first;
+#pragma unroll 4
+        for (uint32_t j = 0; j < leaf_cnt; j++) {
+          const float4 q = __ldg(&lp[j]);
+          const float dx = q.x - fx, dy = q.y - fy, dz = q.z - fz;
+          const float d = dx * dx + dy * dy + dz * dz;
+          if (d < best_d) {
+            best_d = d;
+            best = leaf_first + j;
+          }
+        }
+      } else {
+        for (uint32_t base = 0; base < leaf_cnt; base += 32u) {
+          const uint32_t j = base + lane;
+          float4 q = make_float4(0.f, 0.f, 0.f, 0.f);
+          if (j < leaf_cnt) q = __ldg(&pts[leaf_first + j]);
+          unsigned todo = want;
+          while (todo) {
+            const int src = __ffs(todo) - 1;
+            todo &= todo - 1;
+            const float qx = __shfl_sync(0xffffffffu, fx, src), qy = __shfl_sync(0xffffffffu, fy, src), qz = __shfl_sync(0xffffffffu, fz, src);
+            const float dx = q.x - qx, dy = q.y - qy, dz = q.z - qz;
+            const uint32_t dbits = j < leaf_cnt ? __float_as_uint(dx * dx + dy * dy + dz * dz) : 0x7f800000u;
+            const uint32_t dmin = __reduce_min_sync(0xffffffffu, dbits);
+            const unsigned who = __ballot_sync(0xffffffffu, dbits == dmin);  // lowest lane = first point in scan order
+            if (static_cast<int>(lane) == src) {
+              const float d = __uint_as_float(dmin);
+              if (d < best_d) {
+                best_d = d;
+                best = leaf_first + base + (__ffs(who) - 1);
+              }
+            }
+          }
+        }
+      }
+      expand = false;
+    }
     if (best_d < before) best_e = e - e0;
     __syncwarp();
-  }
+  } while (SUBMAP && ++e < e1);
   if (valid) {
     vcorr[v] = best;
-    S.centry[i] = best_e;
+    if constexpr (SUBMAP) S.centry[i] = best_e;
   }
 }
 
@@ -638,7 +401,7 @@ cudaError_t launch_forest_build(const ForestBuild& b, cudaStream_t st, int* laun
   count += 2;
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return e;
-  // radix levels: every map whose nodes at this level still hold more than kForestSegMax points
+  // radix levels: every map whose nodes at this level still hold more than kKdSegMax points
   for (uint32_t level = 0; level < b.radix_levels; level++) {
     forest_boxes_init_kernel<<<(b.n_segments * 6u + 255u) / 256u, 256, 0, st>>>(b.boxes, b.n_segments);
     forest_boxes_kernel<<<(n + 255u) / 256u, 256, 0, st>>>(b.leaf_pts, n, F, level, b.boxes);
@@ -650,13 +413,12 @@ cudaError_t launch_forest_build(const ForestBuild& b, cudaStream_t st, int* laun
     count += 6;
   }
   // every (map, segment) below: one CTA each
-  const size_t smem = 2 * kForestSegMax * sizeof(float4) + kForestSegMax * (sizeof(unsigned long long) + sizeof(uint32_t)) + kForestSegNodes * 6 * sizeof(uint32_t);
   static bool configured = false;
   if (!configured) {
-    if ((e = cudaFuncSetAttribute(forest_refine_smem_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem))) != cudaSuccess) return e;
+    if ((e = cudaFuncSetAttribute(forest_refine_smem_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(kKdRefineSmem))) != cudaSuccess) return e;
     configured = true;
   }
-  forest_refine_smem_kernel<<<b.n_segments, 1024, smem, st>>>(b.leaf_pts, b.perm, F);
+  forest_refine_smem_kernel<<<b.n_segments, 1024, kKdRefineSmem, st>>>(b.leaf_pts, b.perm, F);
   count += 1;
   if (b.orig_normals || b.orig_covA) {
     if ((e = launch_gather(b.perm, n, nullptr, nullptr, b.orig_normals, b.leaf_normals, b.orig_covA, b.leaf_covA, b.orig_covB, b.leaf_covB, b.sm_count, st)) !=
@@ -682,9 +444,9 @@ cudaError_t launch_forest_search(const BatchParams& B, const ForestView& F, cons
   if (max_depth < 1 || max_depth > kForestStack) return cudaErrorInvalidValue;
   const size_t smem = static_cast<size_t>(max_depth) * kLinBlock * sizeof(float);
   if (round)
-    forest_search_kernel<true><<<n_tiles, kLinBlock, smem, st>>>(B, F, bound, vcorr, round);
+    forest_search_kernel<true, false><<<n_tiles, kLinBlock, smem, st>>>(B, F, bound, vcorr, round, SubmapView{});
   else
-    forest_search_kernel<false><<<n_tiles, kLinBlock, smem, st>>>(B, F, bound, vcorr, nullptr);
+    forest_search_kernel<false, false><<<n_tiles, kLinBlock, smem, st>>>(B, F, bound, vcorr, nullptr, SubmapView{});
   return cudaGetLastError();
 }
 
@@ -692,10 +454,11 @@ cudaError_t launch_submap_search(const BatchParams& B, const float4* pnodes, con
                                  float bound, uint32_t* vcorr, cudaStream_t st) {
   if (max_depth < 1 || max_depth > kForestStack) return cudaErrorInvalidValue;
   const size_t smem = static_cast<size_t>(max_depth) * kLinBlock * sizeof(float);
+  const ForestView F{pnodes, nullptr, nullptr, nullptr};
   if (round)
-    submap_search_kernel<true><<<n_tiles, kLinBlock, smem, st>>>(B, pnodes, S, bound, vcorr, round);
+    forest_search_kernel<true, true><<<n_tiles, kLinBlock, smem, st>>>(B, F, bound, vcorr, round, S);
   else
-    submap_search_kernel<false><<<n_tiles, kLinBlock, smem, st>>>(B, pnodes, S, bound, vcorr, nullptr);
+    forest_search_kernel<false, true><<<n_tiles, kLinBlock, smem, st>>>(B, F, bound, vcorr, nullptr, S);
   return cudaGetLastError();
 }
 

@@ -9,10 +9,6 @@
 
 namespace sgb {
 
-/// shared-memory segment of the refinement (points) and its most nodes at one level: kKdSegMax / kKdSegNodes of sgb_kernels.cu
-constexpr uint32_t kForestSegMax = 2048;
-constexpr uint32_t kForestSegNodes = 128;
-
 /// Per-map tables on the device, all derived on the host from the map offsets.  Prefix arrays have n_maps + 1 entries.
 struct ForestTables {
   const uint32_t* pt_off;     // first point of map m (points concatenated in map order)
@@ -20,7 +16,7 @@ struct ForestTables {
   const uint32_t* seg_off;    // first shared-memory segment of map m (2^level0 segments, 0 for an empty map)
   const uint32_t* node_base;  // [n_maps] first packet record of map m in the record array (P_m - 1 records)
   const uint32_t* depth;      // [n_maps] inner levels of map m's tree (0: empty map)
-  const uint32_t* level0;     // [n_maps] first level whose nodes hold at most kForestSegMax points
+  const uint32_t* level0;     // [n_maps] first level whose nodes hold at most kKdSegMax points
   uint32_t n_maps;
 };
 

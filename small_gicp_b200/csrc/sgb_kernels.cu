@@ -467,32 +467,10 @@ __global__ void curve_keys_kernel(const float4* __restrict__ pts, size_t n, cons
 // consecutive points, hierarchy = the implicit perfect binary tree over P = 2^ceil(log2(#leaves)) leaf slots (node i has
 // children 2i+1, 2i+2; missing leaves are empty boxes that no query ever enters).  Every step is a data-parallel kernel;
 // the output is the same 64-byte packet record array the search kernel consumes.
-// sgb_forest.cu keeps copies of the helpers and kernels below (tree_bound ... lbvh_level_kernel) for many trees at once (forest_*): a
-// change to one side belongs in the other.
+// The helpers and the bodies of the shared-memory refinement and of the record kernels are in sgb_device.cuh, which the many-tree
+// build (sgb_forest.cu) shares.
 // ---------------------------------------------------------------------------------------------
-__device__ __forceinline__ void lbvh_store_child(float4* pnodes, uint32_t child_heap, const float lo[3], const float hi[3], uint32_t a, uint32_t b) {
-  const uint32_t parent = (child_heap - 1u) >> 1, side = (child_heap & 1u) ? 0u : 1u;  // odd heap index = left child
-  pnodes[parent * 4 + side * 2 + 0] = make_float4(lo[0], lo[1], lo[2], __uint_as_float(a));
-  pnodes[parent * 4 + side * 2 + 1] = make_float4(hi[0], hi[1], hi[2], __uint_as_float(b));
-}
-
-/// first point of node j at a level with `count` nodes (balanced implicit tree over n points)
-__device__ __forceinline__ uint32_t tree_bound(uint32_t j, uint32_t count, uint32_t n) {
-  return static_cast<uint32_t>((static_cast<uint64_t>(j) * n) / count);
-}
-/// node (at a level with `count` nodes) that owns position i
-__device__ __forceinline__ uint32_t tree_node_of(uint32_t i, uint32_t count, uint32_t n) {
-  return static_cast<uint32_t>(((static_cast<uint64_t>(i) + 1u) * count + n - 1u) / n) - 1u;
-}
-
 // ---- median-split refinement (device-side kd construction): one pass per level ------------------------------------
-// boxes: count x 6 floats stored as order-preserving uints (lo xyz, hi xyz)
-__device__ __forceinline__ uint32_t float_flip(float f) {
-  const uint32_t u = __float_as_uint(f);
-  return u ^ ((u >> 31) ? 0xFFFFFFFFu : 0x80000000u);
-}
-__device__ __forceinline__ float float_unflip(uint32_t u) { return __uint_as_float(u ^ ((u >> 31) ? 0x80000000u : 0xFFFFFFFFu)); }
-
 __global__ void kd_boxes_init_kernel(uint32_t* boxes, uint32_t count) {
   const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
   if (t < count * 6u) boxes[t] = (t % 6u) < 3u ? 0xFFFFFFFFu : 0u;
@@ -557,107 +535,20 @@ __global__ void kd_keys_kernel(const float4* __restrict__ pts, uint32_t n, uint3
   keys[i] = (static_cast<uint64_t>(node) << 32) | float_flip(c);
 }
 
-// The same median-split refinement for a whole SUBTREE of at most kKdSegMax points in ONE launch: CTA b owns node b of level `level0`
-// (a contiguous position range), keeps its points in shared memory and runs every remaining level there -- per level: node boxes
-// (shared-memory atomics on order-preserving integer images of the floats), key = (node, coordinate along the node's widest axis),
-// bitonic sort of (key, slot), permutation of the points.  Above level0 a level is ~12 launches (boxes, keys, radix sort, gather); for a
-// 16k-point frame that was 9 levels = ~110 launches of pure launch latency, now 3 levels + this kernel.  Same keys, same balanced
-// position boundaries as the per-level path (ties may land differently -- any order is a valid tree).  forest_refine_smem_kernel
-// (sgb_forest.cu) is its copy over many maps' segments.
-constexpr uint32_t kKdSegMax = 2048;
-constexpr uint32_t kKdSegNodes = 128;
+// The same median-split refinement for every subtree of at most kKdSegMax points in ONE launch: CTA b refines node b of level `level0`
+// in shared memory (kd_refine_segment).  Above level0 a level is ~12 launches (boxes, keys, radix sort, gather); for a 16k-point frame
+// that was 9 levels = ~110 launches of pure launch latency, now 3 levels + this kernel.
 __global__ void __launch_bounds__(1024) kd_refine_smem_kernel(float4* __restrict__ leaf_pts, uint32_t* __restrict__ perm, uint32_t n, uint32_t level0, uint32_t levels) {
-  extern __shared__ __align__(16) unsigned char s_raw[];
-  float4* s_pts = reinterpret_cast<float4*>(s_raw);                                            // [2][kKdSegMax]
-  unsigned long long* s_key = reinterpret_cast<unsigned long long*>(s_raw + 2 * kKdSegMax * sizeof(float4));  // [kKdSegMax]
-  uint32_t* s_idx = reinterpret_cast<uint32_t*>(s_key + kKdSegMax);                            // [kKdSegMax]
-  uint32_t* s_box = s_idx + kKdSegMax;                                                         // [kKdSegNodes][6]
-  const uint32_t b = blockIdx.x, tid = threadIdx.x;
-  const uint32_t first = tree_bound(b, 1u << level0, n), last = tree_bound(b + 1u, 1u << level0, n), m = last - first;
-  for (uint32_t t = tid; t < m; t += blockDim.x) s_pts[t] = leaf_pts[first + t];
-  uint32_t cur = 0;
-  __syncthreads();
-  for (uint32_t level = level0; level < levels; level++) {
-    const uint32_t count = 1u << level, node_first = b << (level - level0), n_nodes = 1u << (level - level0);
-    for (uint32_t t = tid; t < n_nodes * 6u; t += blockDim.x) s_box[t] = (t % 6u) < 3u ? 0xFFFFFFFFu : 0u;
-    __syncthreads();
-    const float4* P0 = s_pts + cur * kKdSegMax;
-    for (uint32_t t = tid; t < m; t += blockDim.x) {
-      const float4 p = P0[t];
-      uint32_t* bx = s_box + (tree_node_of(first + t, count, n) - node_first) * 6u;
-      atomicMin(&bx[0], float_flip(p.x));
-      atomicMin(&bx[1], float_flip(p.y));
-      atomicMin(&bx[2], float_flip(p.z));
-      atomicMax(&bx[3], float_flip(p.x));
-      atomicMax(&bx[4], float_flip(p.y));
-      atomicMax(&bx[5], float_flip(p.z));
-    }
-    __syncthreads();
-    for (uint32_t t = tid; t < kKdSegMax; t += blockDim.x) {
-      unsigned long long key = ~0ull;  // padding sorts to the end
-      if (t < m) {
-        const uint32_t node = tree_node_of(first + t, count, n) - node_first;
-        const uint32_t* bx = s_box + node * 6u;
-        const float ex = float_unflip(bx[3]) - float_unflip(bx[0]), ey = float_unflip(bx[4]) - float_unflip(bx[1]), ez = float_unflip(bx[5]) - float_unflip(bx[2]);
-        const float4 p = P0[t];
-        const float c = ex >= ey ? (ex >= ez ? p.x : p.z) : (ey >= ez ? p.y : p.z);
-        key = (static_cast<unsigned long long>(node) << 32) | float_flip(c);
-      }
-      s_key[t] = key;
-      s_idx[t] = t;
-    }
-    __syncthreads();
-    // bitonic sort of (key, slot) over kKdSegMax entries: one compare-exchange per thread and step
-    for (uint32_t k = 2; k <= kKdSegMax; k <<= 1) {
-      for (uint32_t j = k >> 1; j > 0; j >>= 1) {
-        for (uint32_t t = tid; t < kKdSegMax / 2u; t += blockDim.x) {
-          const uint32_t lo = ((t & ~(j - 1u)) << 1) | (t & (j - 1u)), hi = lo | j;
-          const bool up = (lo & k) == 0u;
-          const unsigned long long a = s_key[lo], c = s_key[hi];
-          if ((a > c) == up) {
-            s_key[lo] = c;
-            s_key[hi] = a;
-            const uint32_t ia = s_idx[lo];
-            s_idx[lo] = s_idx[hi];
-            s_idx[hi] = ia;
-          }
-        }
-        __syncthreads();
-      }
-    }
-    float4* P1 = s_pts + (cur ^ 1u) * kKdSegMax;
-    for (uint32_t t = tid; t < m; t += blockDim.x) P1[t] = P0[s_idx[t]];
-    cur ^= 1u;
-    __syncthreads();
-  }
-  const float4* Pf = s_pts + cur * kKdSegMax;
-  for (uint32_t t = tid; t < m; t += blockDim.x) {
-    const float4 p = Pf[t];
-    leaf_pts[first + t] = p;
-    perm[first + t] = static_cast<uint32_t>(__float_as_int(p.w));  // w carries the original index through every permutation
-  }
+  kd_refine_segment(leaf_pts, perm, 0u, blockIdx.x, n, level0, levels);
 }
 
 // one warp per leaf slot: bounding box of its (at most 32) consecutive points -> the parent's child record
 __global__ void lbvh_leaf_kernel(const float4* __restrict__ leaf_pts, uint32_t n, uint32_t P, float4* pnodes) {
   const uint32_t slot = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31u;
   if (slot >= P) return;
-  const uint32_t first = tree_bound(slot, P, n), last = tree_bound(slot + 1u, P, n), idx = first + lane;
-  float lo[3] = {INFINITY, INFINITY, INFINITY}, hi[3] = {-INFINITY, -INFINITY, -INFINITY};
-  if (idx < last) {
-    const float4 p = leaf_pts[idx];
-    lo[0] = hi[0] = p.x;
-    lo[1] = hi[1] = p.y;
-    lo[2] = hi[2] = p.z;
-  }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-#pragma unroll
-    for (int a = 0; a < 3; a++) {
-      lo[a] = fminf(lo[a], __shfl_xor_sync(0xffffffffu, lo[a], o));
-      hi[a] = fmaxf(hi[a], __shfl_xor_sync(0xffffffffu, hi[a], o));
-    }
-  }
+  const uint32_t first = tree_bound(slot, P, n), last = tree_bound(slot + 1u, P, n);
+  float lo[3], hi[3];
+  lbvh_leaf_box(leaf_pts, 0u, first, last, lane, lo, hi);
   if (lane == 0) {
     const uint32_t cnt = last - first;
     lbvh_store_child(pnodes, (P - 1u) + slot, lo, hi, cnt ? first : 0u, cnt);  // cnt == 0: inverted box, never entered
@@ -668,11 +559,7 @@ __global__ void lbvh_leaf_kernel(const float4* __restrict__ leaf_pts, uint32_t n
 __global__ void lbvh_level_kernel(uint32_t level_first, uint32_t level_count, float4* pnodes) {
   const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
   if (t >= level_count) return;
-  const uint32_t node = level_first + t;
-  const float4 l0 = pnodes[node * 4 + 0], l1 = pnodes[node * 4 + 1], r0 = pnodes[node * 4 + 2], r1 = pnodes[node * 4 + 3];
-  const float lo[3] = {fminf(l0.x, r0.x), fminf(l0.y, r0.y), fminf(l0.z, r0.z)};
-  const float hi[3] = {fmaxf(l1.x, r1.x), fmaxf(l1.y, r1.y), fmaxf(l1.z, r1.z)};
-  lbvh_store_child(pnodes, node, lo, hi, node, 0u);  // inner child: a = node index, b = 0
+  lbvh_inner_record(pnodes, level_first + t);
 }
 
 cudaError_t launch_curve_keys(const float4* pts, size_t n, const double* centre4, uint64_t* keys, uint32_t* vals, int sm_count, cudaStream_t st) {
@@ -714,14 +601,13 @@ uint32_t kd_smem_first_level(uint32_t n, uint32_t levels) {
 }
 cudaError_t launch_kd_refine_smem(float4* leaf_pts, uint32_t* perm, uint32_t n, uint32_t level0, uint32_t levels, cudaStream_t st) {
   if (level0 >= levels) return cudaSuccess;
-  const size_t smem = 2 * kKdSegMax * sizeof(float4) + kKdSegMax * (sizeof(unsigned long long) + sizeof(uint32_t)) + kKdSegNodes * 6 * sizeof(uint32_t);
   static bool configured = false;
   if (!configured) {
-    cudaError_t e = cudaFuncSetAttribute(kd_refine_smem_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
+    cudaError_t e = cudaFuncSetAttribute(kd_refine_smem_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(kKdRefineSmem));
     if (e != cudaSuccess) return e;
     configured = true;
   }
-  kd_refine_smem_kernel<<<1u << level0, 1024, smem, st>>>(leaf_pts, perm, n, level0, levels);
+  kd_refine_smem_kernel<<<1u << level0, 1024, kKdRefineSmem, st>>>(leaf_pts, perm, n, level0, levels);
   return cudaGetLastError();
 }
 
