@@ -340,6 +340,31 @@ typedef struct sgb_align_options {
  * out_Hb42xB (or NULL) = H(36) | b(6) per member (RegistrationResult).  max_iterations <= 0 returns the initial poses, not converged. */
 int sgb_align_batch(sgb_ctx* ctx, const sgb_align_options* options, const double* init_T16xB, double* out_T16xB, double* out_info4xB,
                     double* out_Hb42xB /*or NULL*/);
+/* Joint window registration: every frame pose of a window of scans solved against all the window's pairwise edges at once, many windows
+ * per call.  Frame k is cloud k of the last sgb_source_set_batch with map k of a many-kd-trees or many-voxel-maps target, both in frame k's
+ * own coordinates (cloud count == map count).  The edges are the members of the pairing of sgb_source_set_pairs with a maps table: member
+ * p is the edge "cloud clouds[p] against map maps[p]" (clouds[p] != maps[p]).  Windows partition the frames: window_off has n_windows + 1
+ * ascending entries from 0 to the frame count, at most 32 frames per window; both frames of an edge lie in one window.  fixed[k] = 1 holds
+ * frame k at its initial pose (NULL: the first frame of each window); a window with an edge needs a fixed frame.
+ *   - Each window minimises E(X) = sum over its edges (i, j) of the factor error of the edge at T_e = X_j^-1 X_i (factor, robust kernel and
+ *     rejector of the options).  With the right perturbations X <- X exp(delta), delta_e = delta_i + A_e delta_j, A_e = -Ad(T_e^-1), and
+ *     the window's system over its free frames is assembled from the edges' H | b (H_ii += H_e, H_ij += H_e A_e, H_jj += A_e^T H_e A_e,
+ *     b_i += b_e, b_j += A_e^T b_e, in member order), plus 1e9 |mask - 1| on every free frame's diagonal.  The step (H + lambda I) delta = -b
+ *     updates every free frame at once: Gauss-Newton with gn_lambda, or Levenberg-Marquardt with the reference's lambda schedule on the
+ *     window's summed error().  Converged: the termination criteria hold for every free frame's step.
+ *   - init_X16xK / out_X16xK: column-major 4x4 per frame, host memory; fixed frames come back bit for bit.  out_info4xW: per window
+ *     converged, iterations, num_inliers, error (both summed over its edges), as sgb_align_batch's per member.  A window without an edge or
+ *     without a free frame returns its initial poses, not converged, 0 iterations; a free frame without an edge stays put.
+ *   - Rounds as sgb_align_batch's, per window: a round is the pairs round of the active edges (those of the windows in that round's phase)
+ *     plus one joint_step_kernel launch, whatever the counts of windows, frames and edges; plus 1 set-up launch for the initial edge poses
+ *     (and 1 when the pairing's view of the target is rebuilt).  The context is left as sgb_align_batch leaves it: sgb_correspondences_batch
+ *     gives each edge's correspondences of its last linearize, and the batched calls work on the edges afterwards.
+ *   - Fails with a message, the context still usable, on: no batch, no pairing with a maps table or a submap pairing, a target that is not
+ *     many maps, cloud count != map count, a self-edge, an edge across windows, a window with edges but no fixed frame, a window of more than
+ *     32 frames, window_off not ascending from 0 to the frame count, more than SGB_BATCH_MAX_MEMBERS windows, and wherever sgb_align_batch
+ *     fails. */
+int sgb_align_joint(sgb_ctx* ctx, const sgb_align_options* options, size_t n_windows, const size_t* window_off, const uint8_t* fixed /*or NULL*/,
+                    const double* init_X16xK, double* out_X16xK, double* out_info4xW);
 /* sgb_align_batch enqueued on the context's stream (sgb_set_stream) with no host involvement after the call: the rounds are planned on
  * the device and driven by a CUDA graph whose conditional WHILE node repeats one round (planner, search, factor, per-member sums, step)
  * until no member has a round to go.  No host synchronisation, no device-to-host copy, no upload from pageable memory: the call returns

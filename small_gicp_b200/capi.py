@@ -87,6 +87,7 @@ _SIGNATURES = {
     "sgb_error_batch_points": (C.c_int, [_vp, _dp, C.POINTER(C.c_uint8), _dp, _dp]),
     "sgb_align_batch": (C.c_int, [_vp, C.POINTER(AlignOptions), _dp, _dp, _dp, _dp]),
     "sgb_align_batch_async": (C.c_int, [_vp, C.POINTER(AlignOptions), _dp, _dp, _dp, _dp]),
+    "sgb_align_joint": (C.c_int, [_vp, C.POINTER(AlignOptions), C.c_size_t, C.POINTER(C.c_size_t), C.POINTER(C.c_uint8), _dp, _dp, _dp]),
     "sgb_estimate_features": (C.c_int, [_vp, C.c_size_t, _dp, C.c_int, _dp, _dp]),
     "sgb_target_estimate_features": (C.c_int, [_vp, C.c_int]),
     "sgb_source_estimate_features": (C.c_int, [_vp, C.c_int]),
@@ -127,6 +128,19 @@ class BatchPointTerms:
         n = point_e.shape[0]
         self.point_H = None if point_Hb42 is None else point_Hb42[:, :36].reshape(n, 6, 6)
         self.point_b = None if point_Hb42 is None else point_Hb42[:, 36:42]
+
+
+class JointAlignResult:
+    """what Context.align_joint returns: per frame X (K,4,4); per window converged (W,) bool, iterations (W,), num_inliers (W,) and error
+    (W,), the last two summed over the window's edges"""
+
+    def __init__(self, X16, info4):
+        K = X16.shape[0]
+        self.X = np.ascontiguousarray(X16.reshape(K, 4, 4).transpose(0, 2, 1))
+        self.converged = info4[:, 0] != 0
+        self.iterations = info4[:, 1].astype(np.int64)
+        self.num_inliers = info4[:, 2].astype(np.int64)
+        self.error = info4[:, 3].copy()
 
 
 class AsyncAlignResult:
@@ -614,6 +628,35 @@ class Context:
         Hb = np.zeros((max(B, 1), 42))
         self._check(self._L.sgb_align_batch(self._h, C.byref(o), _d(Tc), _d(T), _d(info), _d(Hb)))
         return BatchAlignResult(T[:B], info[:B], Hb[:B])
+
+    def align_joint(self, init_X, windows=None, fixed=None, factor=FACTOR_GICP, robust=ROBUST_NONE, robust_c=1.0, rejector=REJECT_DISTANCE, max_dist_sq=1.0,
+                    optimizer=OPT_LEVENBERG_MARQUARDT, max_iterations=20, gn_lambda=1e-6, max_inner_iterations=10, init_lambda=1e-3,
+                    lambda_factor=10.0, rotation_eps=0.1 * np.pi / 180.0, translation_eps=1e-3, dof_mask=None):
+        """Joint registration of windows of frames (sgb_align_joint) -> a JointAlignResult.  Frame k is cloud k of set_source_batch with map k
+        of the many-maps target; the edges are the members of set_source_pairs(clouds, maps), edge p = cloud clouds[p] against map maps[p] at
+        X_j^-1 X_i.  init_X (K,4,4) row-major frame poses; windows: the window offsets (W + 1,) from 0 to K (None: one window of all
+        frames); fixed (K,) flags of frames held at their initial pose (None: the first frame of each window); the other keywords as in
+        align_batch."""
+        X = np.asarray(init_X, dtype=np.float64)
+        K = self._cloud_offsets.size - 1 if hasattr(self, "_cloud_offsets") else 0
+        if X.shape != (K, 4, 4):
+            raise SgbError(f"align_joint: need ({K}, 4, 4) frame poses")
+        Xc = np.ascontiguousarray(X.transpose(0, 2, 1))
+        off = np.ascontiguousarray(np.array([0, K] if windows is None else windows, dtype=np.uintp).reshape(-1))
+        if off.size < 1:
+            raise SgbError("align_joint: windows needs at least one entry")
+        W = off.size - 1
+        fx = None if fixed is None else np.ascontiguousarray(np.asarray(fixed).astype(np.uint8).reshape(-1))
+        if fx is not None and fx.size != K:
+            raise SgbError(f"align_joint: fixed needs {K} entries")
+        o = AlignOptions(int(factor), int(robust), float(robust_c), int(rejector), float(max_dist_sq), int(optimizer), int(max_iterations), float(gn_lambda),
+                         int(max_inner_iterations), float(init_lambda), float(lambda_factor), float(rotation_eps), float(translation_eps))
+        o.dof_mask[:] = [1.0] * 6 if dof_mask is None else [float(x) for x in dof_mask]
+        out = np.zeros((max(K, 1), 16))
+        info = np.zeros((max(W, 1), 4))
+        self._check(self._L.sgb_align_joint(self._h, C.byref(o), W, off.ctypes.data_as(C.POINTER(C.c_size_t)),
+                                            None if fx is None else fx.ctypes.data_as(C.POINTER(C.c_uint8)), _d(Xc), _d(out), _d(info)))
+        return JointAlignResult(out[:K], info[:W])
 
     def align_batch_async(self, init_Ts, factor=FACTOR_GICP, robust=ROBUST_NONE, robust_c=1.0, rejector=REJECT_DISTANCE, max_dist_sq=1.0,
                           optimizer=OPT_LEVENBERG_MARQUARDT, max_iterations=20, gn_lambda=1e-6, max_inner_iterations=10, init_lambda=1e-3,

@@ -642,4 +642,76 @@ cudaError_t launch_batch_align_finish(uint32_t n_members, const MemberState* sta
   return cudaGetLastError();
 }
 
+// ---- sgb_align_joint (DESIGN.md §11 "Joint windows") ----
+
+__device__ __forceinline__ void joint_write_edge_pose(const JointParams& J, uint32_t q, const double* X) {
+  double T[16];
+  edge_pose(X + 16 * J.edge_i[q], X + 16 * J.edge_j[q], T);
+  double* p = J.poses + 12 * static_cast<size_t>(J.edge_member[q]);
+  for (int i = 0; i < 3; i++) {  // pose_from_colmajor
+    for (int j = 0; j < 3; j++) p[i * 3 + j] = T[j * 4 + i];
+    p[9 + i] = T[12 + i];
+  }
+}
+
+__global__ void joint_edge_poses_kernel(const __grid_constant__ JointParams J) {
+  for (uint32_t q = blockIdx.x * blockDim.x + threadIdx.x; q < J.n_edges; q += gridDim.x * blockDim.x)
+    joint_write_edge_pose(J, q, J.X + 16 * static_cast<size_t>(J.frame_off[J.edge_win[q]]));
+}
+
+// One CTA per window; the window's system (packed lower triangle, up to 192 x 192) and the solve's scratch in dynamic shared memory.
+// Threads take the rows of each column of the factorisation (n <= 192 < kJointBlock), the entries of each edge's blocks, the frames.
+constexpr int kJointBlock = 256;
+__global__ void __launch_bounds__(kJointBlock) joint_step_kernel(const __grid_constant__ AlignOptions o, const __grid_constant__ JointParams J, bool linearize,
+                                                                 const double* __restrict__ out) {
+  extern __shared__ double s_work[];
+  const uint32_t w = blockIdx.x;
+  const int tid = threadIdx.x, nt = blockDim.x;
+  WindowState* s = J.state + w;
+  if (s->phase != (linearize ? kPhaseLinearize : kPhaseTrial)) return;
+  const uint32_t f0 = J.frame_off[w], e0 = J.edge_off[w];
+  JointWindow win;
+  win.n_frames = static_cast<int>(J.frame_off[w + 1] - f0);
+  win.n_free = static_cast<int>(J.n_free[w]);
+  win.n_edges = static_cast<int>(J.edge_off[w + 1] - e0);
+  win.free = J.free + f0;
+  win.ei = J.edge_i + e0;
+  win.ej = J.edge_j + e0;
+  win.sums = J.sums + 44 * static_cast<size_t>(e0);
+  win.X = J.X + 16 * static_cast<size_t>(f0);
+  win.cand = J.cand + 16 * static_cast<size_t>(f0);
+  win.delta = J.delta + 6 * static_cast<size_t>(f0);
+  win.s = s;
+  win.work = s_work;
+  if (linearize) {
+    // the edges' sums are kept: error() rounds overwrite `out`, and every further trial re-assembles the system from them
+    for (uint32_t k = tid; k < 44u * win.n_edges; k += nt) J.sums[44 * static_cast<size_t>(e0) + k] = out[44 * static_cast<size_t>(J.edge_member[e0 + k / 44u]) + k % 44u];
+    __syncthreads();
+    joint_after_linearize(o, win, tid, nt);
+  } else {
+    double ce = 0.0;
+    for (int q = 0; q < win.n_edges; q++) ce += out[J.edge_member[e0 + q]];
+    joint_after_error(o, win, ce, tid, nt);
+  }
+  const double* X = s->phase == kPhaseTrial ? win.cand : win.X;
+  for (int q = tid; q < win.n_edges; q += nt) joint_write_edge_pose(J, e0 + q, X);
+  if (tid == 0) J.phase[w] = static_cast<uint8_t>(s->phase);
+}
+
+cudaError_t launch_joint_edge_poses(const JointParams& J, cudaStream_t st) {
+  if (!J.n_edges) return cudaSuccess;
+  joint_edge_poses_kernel<<<(J.n_edges + 127u) / 128u, 128, 0, st>>>(J);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_joint_step(const AlignOptions& o, const JointParams& J, int max_free, bool linearize, const double* out, cudaStream_t st) {
+  const size_t smem = joint_step_smem(max_free);
+  if (smem > 48 * 1024) {
+    const cudaError_t e = cudaFuncSetAttribute(joint_step_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
+    if (e != cudaSuccess) return e;
+  }
+  joint_step_kernel<<<J.n_windows, kJointBlock, smem, st>>>(o, J, linearize, out);
+  return cudaGetLastError();
+}
+
 }  // namespace sgb

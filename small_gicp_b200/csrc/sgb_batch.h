@@ -144,4 +144,26 @@ cudaError_t launch_batch_align_init(const AlignOptions& o, uint32_t n_members, c
 /// sgb_align_batch's outputs from the members' final state: T (16, column-major), info (converged, iterations, inliers, error), H | b (or null)
 cudaError_t launch_batch_align_finish(uint32_t n_members, const MemberState* state, double* out_T16, double* out_info4, double* out_Hb42, cudaStream_t st);
 
+// ---- sgb_align_joint (DESIGN.md §11 "Joint windows"): windows of frames, each edge a pair member ----
+/// The call's tables (built once per call) and state.  Window w holds frames frame_off[w] .. frame_off[w + 1] - 1 and the edges
+/// edge_off[w] .. edge_off[w + 1] - 1 of the edge list (member order within each window); edge q is member edge_member[q], cloud frame
+/// edge_i[q] against map frame edge_j[q] (local to the window).  free[k]: index of frame k among its window's free frames, or -1.
+struct JointParams {
+  uint32_t n_windows, n_edges;
+  const uint32_t *frame_off, *edge_off, *n_free, *edge_member, *edge_win;
+  const int *edge_i, *edge_j, *free;
+  double *X, *cand, *delta;  // [frames][16] / [frames][16] / [frames][6] (window w's steps from 6 frame_off[w])
+  double* sums;              // [edges][44]: each edge's H | b | e | inliers of its last linearize
+  WindowState* state;        // [windows]
+  uint8_t* phase;            // [windows]
+  double* poses;             // BatchParams::poses: [members][12]
+};
+/// the scratch of joint_step_kernel for windows of up to max_free free frames (dynamic shared memory)
+inline size_t joint_step_smem(int max_free) { return static_cast<size_t>(joint_work_doubles(max_free)) * sizeof(double); }
+/// every edge's pose X_j^-1 X_i (row-major R | t) from the frames' X
+cudaError_t launch_joint_edge_poses(const JointParams& J, cudaStream_t st);
+/// one CTA per window: every window in the round's phase (linearize: kPhaseLinearize, else kPhaseTrial) takes its step from `out` (what
+/// launch_batch_segment wrote for the edges), then writes its edges' next poses and its phase
+cudaError_t launch_joint_step(const AlignOptions& o, const JointParams& J, int max_free, bool linearize, const double* out, cudaStream_t st);
+
 }  // namespace sgb

@@ -401,6 +401,8 @@ int pair_members(sgb_ctx* ctx, const char* who, size_t n_members, const uint32_t
   ctx->b_offsets = member_off;
   ctx->b_pair_has_maps = maps != nullptr;
   if (maps) ctx->b_pair_maps.assign(maps, maps + P);
+  ctx->b_pair_clouds.resize(P);
+  for (size_t p = 0; p < P; p++) ctx->b_pair_clouds[p] = clouds ? clouds[p] : static_cast<uint32_t>(p);
   ctx->b_pair_max_map = max_map;
   const size_t B = std::max<size_t>(P, 1), nn = std::max<size_t>(n, 1);
   if (int rc = reserve_members(ctx)) return rc;
@@ -917,6 +919,169 @@ int sgb_align_batch(sgb_ctx* ctx, const sgb_align_options* o, const double* init
       std::memcpy(out_Hb + 42 * m, s.H, 36 * sizeof(double));
       std::memcpy(out_Hb + 42 * m + 36, s.b, 6 * sizeof(double));
     }
+  }
+  return 0;
+}
+
+int sgb_align_joint(sgb_ctx* ctx, const sgb_align_options* o, size_t n_windows, const size_t* window_off, const uint8_t* fixed, const double* init_X,
+                    double* out_X, double* out_info) {
+  if (!ctx) return 1;
+  const std::string who = "sgb_align_joint";
+  if (ctx->src_state != SourceState::Batch) return fail(ctx, 1, who + ": the context holds no batch of sources (call sgb_source_set_batch)");
+  if (ctx->b_submaps) return fail(ctx, 1, who + ": the members are submap members (sgb_source_set_submaps); joint windows need (cloud, map) edges");
+  if (!ctx->b_paired || !ctx->b_pair_has_maps)
+    return fail(ctx, 1, who + ": the edges are the members of a pairing with a maps table (sgb_source_set_pairs with maps); there is none");
+  if (!many_maps(ctx))
+    return fail(ctx, 1, who + ": the frames are the maps of a many-kd-trees or many-voxel-maps target (sgb_target_build_kdtrees / sgb_target_build_voxelmaps); "
+                              "the current target is not one");
+  const size_t K = ctx->b_cloud_offsets.size() - 1, E = batch_members(ctx);
+  if (K != target_maps(ctx))
+    return fail(ctx, 1, who + ": frame k is cloud k with map k, but the batch holds " + std::to_string(K) + " clouds and the target " +
+                            std::to_string(target_maps(ctx)) + " maps");
+  AlignOptions ao;
+  if (int rc = align_checks(ctx, who.c_str(), o, init_X, out_X, out_info, ao)) return rc;
+  if (!window_off) return fail(ctx, 1, who + ": null window offsets");
+  if (n_windows > SGB_BATCH_MAX_MEMBERS)
+    return fail(ctx, 1, who + ": " + std::to_string(n_windows) + " windows, at most " + std::to_string(SGB_BATCH_MAX_MEMBERS));
+  if (window_off[0] != 0 || window_off[n_windows] != K)
+    return fail(ctx, 1, who + ": window_off must run from 0 to the frame count " + std::to_string(K));
+  for (size_t w = 0; w < n_windows; w++) {
+    if (window_off[w + 1] < window_off[w]) return fail(ctx, 1, who + ": window_off must be ascending (window " + std::to_string(w) + ")");
+    if (window_off[w + 1] - window_off[w] > static_cast<size_t>(kJointMaxFrames))
+      return fail(ctx, 1, who + ": window " + std::to_string(w) + " has " + std::to_string(window_off[w + 1] - window_off[w]) + " frames, at most " +
+                              std::to_string(kJointMaxFrames));
+  }
+  // window of every frame; the edges of every window in member order
+  std::vector<uint32_t> win_of(K);
+  for (size_t w = 0; w < n_windows; w++)
+    for (size_t k = window_off[w]; k < window_off[w + 1]; k++) win_of[k] = static_cast<uint32_t>(w);
+  std::vector<uint32_t> edge_count(n_windows, 0);
+  for (size_t p = 0; p < E; p++) {
+    const uint32_t i = ctx->b_pair_clouds[p], j = ctx->b_pair_maps[p];
+    if (i == j) return fail(ctx, 1, who + ": member " + std::to_string(p) + " pairs cloud " + std::to_string(i) + " with map " + std::to_string(j) + " of its own frame");
+    if (win_of[i] != win_of[j])
+      return fail(ctx, 1, who + ": member " + std::to_string(p) + " joins frame " + std::to_string(i) + " (window " + std::to_string(win_of[i]) + ") and frame " +
+                              std::to_string(j) + " (window " + std::to_string(win_of[j]) + "); both frames of an edge must lie in one window");
+    edge_count[win_of[i]]++;
+  }
+  std::vector<uint8_t> fix(K);
+  for (size_t k = 0; k < K; k++) fix[k] = fixed ? (fixed[k] != 0) : (k == window_off[win_of[k]]);
+  std::vector<uint32_t> n_free(n_windows, 0);
+  std::vector<int32_t> free_of(K);
+  for (size_t w = 0; w < n_windows; w++) {
+    for (size_t k = window_off[w]; k < window_off[w + 1]; k++) free_of[k] = fix[k] ? -1 : static_cast<int32_t>(n_free[w]++);
+    if (edge_count[w] && n_free[w] == window_off[w + 1] - window_off[w])
+      return fail(ctx, 1, who + ": window " + std::to_string(w) + " has edges but no fixed frame (its gauge would be free)");
+  }
+  CU(cudaSetDevice(ctx->device));
+  if (E) {
+    if (int rc = pair_view(ctx)) return rc;
+  }
+  // the tables: frame_off [W + 1] | edge_off [W + 1] | n_free [W] | edge_member [E] | edge_win [E] | edge_i [E] | edge_j [E] | free [K]
+  const size_t W = n_windows;
+  std::vector<uint32_t> tab(2 * (W + 1) + W + 4 * E + K);
+  uint32_t* frame_off = tab.data();
+  uint32_t* edge_off = frame_off + W + 1;
+  uint32_t* nf = edge_off + W + 1;
+  uint32_t* edge_member = nf + W;
+  uint32_t* edge_win = edge_member + E;
+  int32_t* edge_i = reinterpret_cast<int32_t*>(edge_win + E);
+  int32_t* edge_j = edge_i + E;
+  int32_t* freeidx = edge_j + E;
+  for (size_t w = 0; w <= W; w++) frame_off[w] = static_cast<uint32_t>(window_off[w]);
+  edge_off[0] = 0;
+  for (size_t w = 0; w < W; w++) edge_off[w + 1] = edge_off[w] + edge_count[w];
+  std::vector<uint32_t> fill(edge_off, edge_off + W);
+  for (size_t p = 0; p < E; p++) {  // member order within each window
+    const uint32_t i = ctx->b_pair_clouds[p], j = ctx->b_pair_maps[p], w = win_of[i], q = fill[w]++;
+    edge_member[q] = static_cast<uint32_t>(p);
+    edge_win[q] = w;
+    edge_i[q] = static_cast<int32_t>(i - window_off[w]);
+    edge_j[q] = static_cast<int32_t>(j - window_off[w]);
+  }
+  int max_free = 0;
+  for (size_t w = 0; w < W; w++) {
+    nf[w] = n_free[w];
+    if (edge_count[w]) max_free = std::max(max_free, static_cast<int>(n_free[w]));
+  }
+  std::copy(free_of.begin(), free_of.end(), freeidx);
+  std::vector<WindowState> state(W);
+  std::vector<uint8_t> phase(W);
+  for (size_t w = 0; w < W; w++) {
+    joint_init(ao, static_cast<int>(n_free[w]), static_cast<int>(edge_count[w]), state[w]);
+    phase[w] = static_cast<uint8_t>(state[w].phase);
+  }
+  const size_t K1 = std::max<size_t>(K, 1), W1 = std::max<size_t>(W, 1);
+  CU(ctx->j_tables.reserve(tab.size() * sizeof(uint32_t)));
+  CU(ctx->j_X.reserve(K1 * 16 * sizeof(double)));
+  CU(ctx->j_cand.reserve(K1 * 16 * sizeof(double)));
+  CU(ctx->j_delta.reserve(K1 * 6 * sizeof(double)));
+  CU(ctx->j_sums.reserve(std::max<size_t>(E, 1) * 44 * sizeof(double)));
+  CU(ctx->j_state.reserve(W1 * sizeof(WindowState)));
+  CU(ctx->j_phase.reserve(W1));
+  JointParams J = {};
+  J.n_windows = static_cast<uint32_t>(W);
+  J.n_edges = static_cast<uint32_t>(E);
+  const uint32_t* dt = ctx->j_tables.as<uint32_t>();
+  J.frame_off = dt;
+  J.edge_off = dt + W + 1;
+  J.n_free = J.edge_off + W + 1;
+  J.edge_member = J.n_free + W;
+  J.edge_win = J.edge_member + E;
+  J.edge_i = reinterpret_cast<const int*>(J.edge_win + E);
+  J.edge_j = J.edge_i + E;
+  J.free = J.edge_j + E;
+  J.X = ctx->j_X.as<double>();
+  J.cand = ctx->j_cand.as<double>();
+  J.delta = ctx->j_delta.as<double>();
+  J.sums = ctx->j_sums.as<double>();
+  J.state = ctx->j_state.as<WindowState>();
+  J.phase = ctx->j_phase.as<uint8_t>();
+  J.poses = ctx->b_poses.as<double>();
+  // pageable host memory: the copies are staged before cudaMemcpyAsync returns
+  CU(cudaMemcpyAsync(ctx->j_tables.p, tab.data(), tab.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
+  if (K) CU(cudaMemcpyAsync(ctx->j_X.p, init_X, K * 16 * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
+  if (W) {  // the phases too: a window done from the start is never stepped, and the host reads every window's phase after each round
+    CU(cudaMemcpyAsync(ctx->j_state.p, state.data(), W * sizeof(WindowState), cudaMemcpyHostToDevice, ctx->stream));
+    CU(cudaMemcpyAsync(ctx->j_phase.p, phase.data(), W, cudaMemcpyHostToDevice, ctx->stream));
+  }
+  if (E) {
+    CU(launch_joint_edge_poses(J, ctx->stream));
+    ctx->launches += 1;
+  }
+  // Rounds in lockstep as in sgb_align_batch, per window: error() for the edges of every window with a pending trial until none has one,
+  // else a linearize of the edges of every window still iterating; each round ends with one joint step launch.
+  std::vector<uint8_t> active(E);
+  for (;;) {
+    bool any_trial = false, any_lin = false;
+    for (size_t w = 0; w < W; w++) {
+      any_trial |= phase[w] == kPhaseTrial;
+      any_lin |= phase[w] == kPhaseLinearize;
+    }
+    if (!any_trial && !any_lin) break;
+    const bool lin = !any_trial;
+    for (size_t q = 0; q < E; q++) active[edge_member[q]] = phase[edge_win[q]] == (lin ? kPhaseLinearize : kPhaseTrial);
+    if (lin) {
+      if (int rc = linearize_round(ctx, o->factor_kind, o->robust_kind, o->robust_c, o->rejector_kind, o->max_dist_sq, nullptr, active.data())) return rc;
+    } else {
+      if (int rc = error_round(ctx, nullptr, active.data())) return rc;
+    }
+    CU(launch_joint_step(ao, J, max_free, lin, ctx->b_out.as<double>(), ctx->stream));
+    ctx->launches += 1;
+    CU(cudaMemcpyAsync(phase.data(), ctx->j_phase.p, W, cudaMemcpyDeviceToHost, ctx->stream));
+    CU(cudaStreamSynchronize(ctx->stream));
+  }
+  std::vector<double> X(16 * K);
+  if (K) CU(cudaMemcpyAsync(X.data(), ctx->j_X.p, K * 16 * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+  if (W) CU(cudaMemcpyAsync(state.data(), ctx->j_state.p, W * sizeof(WindowState), cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));
+  for (size_t k = 0; k < K; k++) std::memcpy(out_X + 16 * k, fix[k] ? init_X + 16 * k : X.data() + 16 * k, 16 * sizeof(double));
+  for (size_t w = 0; w < W; w++) {
+    double* info = out_info + 4 * w;
+    info[0] = state[w].converged ? 1.0 : 0.0;
+    info[1] = state[w].iterations;
+    info[2] = state[w].inliers;
+    info[3] = state[w].e;
   }
   return 0;
 }

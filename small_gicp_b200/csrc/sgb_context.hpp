@@ -197,6 +197,7 @@ struct sgb_ctx {
   bool b_paired = false;
   bool b_pair_has_maps = false;  // the pairing has a maps table (possibly of 0 members)
   std::vector<uint32_t> b_pair_maps;
+  std::vector<uint32_t> b_pair_clouds;  // the cloud of each pair member
   uint32_t b_pair_max_map = 0;  // the largest map index the pairing names (b_pair_maps, or b_sub_maps of a submap pairing): the per-call check's fast path
   sgb::DevBuf p_tables;                    // uint32: member offsets [members + 1] | cloud of each member | map of each member
   sgb::DevBuf p_pts, p_covA, p_covB, p_perm, p_centres, p_bounds;
@@ -217,6 +218,9 @@ struct sgb_ctx {
   cudaStream_t cap_stream = nullptr;
   cudaGraphExec_t align_exec = nullptr;
   std::vector<unsigned char> align_key;
+  // sgb_align_joint: the call's window / edge tables (JointParams), the frames' poses, candidates and steps, the edges' last sums, the
+  // windows' WindowState and phase
+  sgb::DevBuf j_tables, j_X, j_cand, j_delta, j_sums, j_state, j_phase;
 };
 
 namespace sgb {

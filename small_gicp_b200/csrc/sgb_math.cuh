@@ -678,4 +678,359 @@ SGB_HD void align_after_error(const AlignOptions& o, MemberState& s, double cand
   s.phase = kPhaseDone;
 }
 
+// ---------------------------------------------------------------------------------------------------------------------------------
+// Joint window registration (sgb_align_joint, joint_step_kernel in sgb_batch.cu; DESIGN.md §11 "Joint windows").  The frames X_k of a
+// window are solved together against every edge (i, j) of the window, each edge a pair member at T_e = X_j^-1 X_i.  The functions below
+// are run by every thread of one CTA (tid of nt threads, CTA barriers between phases); compiled for the host (tests/host_joint) they run
+// with tid = 0, nt = 1 and no barrier.
+// ---------------------------------------------------------------------------------------------------------------------------------
+#if defined(__CUDA_ARCH__)
+#define SGB_CTA_SYNC() __syncthreads()
+#else
+#define SGB_CTA_SYNC() ((void)0)
+#endif
+
+constexpr int kJointMaxFrames = 32;
+constexpr int kJointMaxN = 6 * kJointMaxFrames;
+
+/// position of entry (r, c) of a symmetric n x n matrix stored as its packed lower triangle, row after row
+SGB_HD int packed_index(int r, int c) { return r >= c ? r * (r + 1) / 2 + c : c * (c + 1) / 2 + r; }
+
+/// solve_ldlt6 for a symmetric n x n A given as its packed lower triangle L (destroyed), n <= kJointMaxN: the same diagonal pivoting and
+/// the same operations in the same order for every entry (each entry's j-sum sequential), so n = 6 gives solve_ldlt6's bits.  The rows of
+/// each column are spread over the threads; the back substitution, whose order chains every entry, is thread 0's.  perm [n] and y [n] are
+/// scratch of the CTA (shared memory on the device).  solve_ldlt6 swaps whole rows and columns; only the lower triangle is ever read, and
+/// the symmetric swap below moves its entries exactly as the full swap does (the trailing block is still symmetric when it is swapped).
+SGB_HD void solve_ldlt_n(int n, double* L, const double* rhs, double* x, int* perm, double* y, int tid, int nt) {
+  for (int i = tid; i < n; i += nt) perm[i] = i;
+  SGB_CTA_SYNC();
+  for (int k = 0; k < n; k++) {
+    int piv = k;
+    for (int i = k + 1; i < n; i++)
+      if (fabs(L[packed_index(i, i)]) > fabs(L[packed_index(piv, piv)])) piv = i;
+    SGB_CTA_SYNC();  // every thread has read the diagonal before it is swapped
+    if (piv != k) {
+      for (int m = tid; m < n; m += nt) {
+        int a, b;
+        if (m < k) {
+          a = packed_index(k, m), b = packed_index(piv, m);
+        } else if (m == k) {
+          a = packed_index(k, k), b = packed_index(piv, piv);
+        } else if (m < piv) {
+          a = packed_index(m, k), b = packed_index(piv, m);
+        } else if (m > piv) {
+          a = packed_index(m, k), b = packed_index(m, piv);
+        } else {
+          continue;  // (piv, k) maps onto itself
+        }
+        const double t = L[a];
+        L[a] = L[b];
+        L[b] = t;
+      }
+      if (tid == 0) {
+        const int t = perm[k];
+        perm[k] = perm[piv];
+        perm[piv] = t;
+      }
+      SGB_CTA_SYNC();
+    }
+    for (int i = k + tid; i < n; i += nt) {  // the sums of column k, each in place (the divisions wait for the new pivot)
+      const int ik = packed_index(i, k);
+      double s = L[ik];
+      for (int j = 0; j < k; j++) s -= L[packed_index(i, j)] * L[packed_index(k, j)] * L[packed_index(j, j)];
+      L[ik] = s;
+    }
+    SGB_CTA_SYNC();
+    const double d = L[packed_index(k, k)];
+    for (int i = k + 1 + tid; i < n; i += nt) {
+      const int ik = packed_index(i, k);
+      L[ik] = d != 0.0 ? L[ik] / d : 0.0;
+    }
+    SGB_CTA_SYNC();
+  }
+  for (int i = tid; i < n; i += nt) y[i] = rhs[perm[i]];
+  SGB_CTA_SYNC();
+  for (int j = 0; j < n; j++) {  // y[i] -= L(i, j) y[j] for j = 0 .. i - 1 in that order, column by column
+    for (int i = j + 1 + tid; i < n; i += nt) y[i] -= L[packed_index(i, j)] * y[j];
+    SGB_CTA_SYNC();
+  }
+  for (int i = tid; i < n; i += nt) {
+    const double d = L[packed_index(i, i)];
+    y[i] = fabs(d) > 0.0 ? y[i] / d : 0.0;
+  }
+  SGB_CTA_SYNC();
+  if (tid == 0)
+    for (int i = n - 1; i >= 0; i--)
+      for (int j = i + 1; j < n; j++) y[i] -= L[packed_index(j, i)] * y[j];
+  SGB_CTA_SYNC();
+  for (int i = tid; i < n; i += nt) x[perm[i]] = y[i];
+  SGB_CTA_SYNC();
+}
+
+/// inverse of a rigid 4x4 pose (column-major): R^T | -R^T t
+SGB_HD void pose_inverse(const double* X, double* out) {
+  for (int c = 0; c < 3; c++) {
+    for (int r = 0; r < 3; r++) out[c * 4 + r] = X[r * 4 + c];
+    out[c * 4 + 3] = 0.0;
+  }
+  for (int r = 0; r < 3; r++) out[12 + r] = -(X[r * 4 + 0] * X[12] + X[r * 4 + 1] * X[13] + X[r * 4 + 2] * X[14]);
+  out[15] = 1.0;
+}
+
+/// the pose of edge (i, j): T_e = X_j^-1 X_i
+SGB_HD void edge_pose(const double* Xi, const double* Xj, double* T) {
+  double inv[16];
+  pose_inverse(Xj, inv);
+  pose_mul(inv, Xi, T);
+}
+
+/// A_e = -Ad(T_e^-1), 6x6 row-major, Ad(R, t) = [[R, 0], [[t]x R, R]] for twists [r; t]: the right perturbations of the frames move the
+/// edge by delta_e = delta_i + A_e delta_j
+SGB_HD void edge_adjoint(const double* T, double* A) {
+  double inv[16];
+  pose_inverse(T, inv);
+  const double* t = inv + 12;
+  for (int r = 0; r < 3; r++)
+    for (int c = 0; c < 3; c++) {
+      const double R = inv[c * 4 + r];
+      // ([t]x R)(r, c) = sum_k [t]x(r, k) R(k, c)
+      const double tx = r == 0 ? t[1] * inv[c * 4 + 2] - t[2] * inv[c * 4 + 1]
+                               : (r == 1 ? t[2] * inv[c * 4 + 0] - t[0] * inv[c * 4 + 2] : t[0] * inv[c * 4 + 1] - t[1] * inv[c * 4 + 0]);
+      A[r * 6 + c] = -R;
+      A[r * 6 + 3 + c] = 0.0;
+      A[(3 + r) * 6 + c] = -tx;
+      A[(3 + r) * 6 + 3 + c] = -R;
+    }
+}
+
+/// One window's optimiser between rounds (beside MemberState: the scalars; the frames' poses, candidates and steps are arrays of the call).
+struct WindowState {
+  double e, inliers;  // summed over the window's edges at the last linearize (e: LM's e / the result's error)
+  double lambda;
+  int phase, it, trial, converged, iterations;
+};
+
+/// One window as the step sees it.  Frames 0 .. n_frames - 1 (local), free[k] = index of frame k among the free frames or -1 (fixed);
+/// edges 0 .. n_edges - 1 in member order, edge q = cloud ei[q] against map ej[q] (local frames), sums [n_edges][44] = its H | b | e | inliers
+/// of the last linearize.  X, cand: [n_frames][16]; delta: [6 n_free].  work: the CTA's scratch of joint_work_doubles(n_free) doubles.
+struct JointWindow {
+  int n_frames, n_free, n_edges;
+  const int* free;
+  const int *ei, *ej;
+  const double* sums;
+  double *X, *cand, *delta;
+  WindowState* s;
+  double* work;
+};
+
+SGB_HHD int joint_work_doubles(int n_free) {
+  const int n = 6 * n_free;
+  return n * (n + 1) / 2 + 3 * n + 36 * 3 + 6 + (n + 1) / 2 + 4;  // L | b | rhs | y | A, P, Q | c | perm (ints) | flags
+}
+
+SGB_HHD void joint_init(const AlignOptions& o, int n_free, int n_edges, WindowState& s) {
+  s.e = s.inliers = 0.0;
+  s.lambda = o.init_lambda;
+  s.phase = o.max_iterations > 0 && n_free > 0 && n_edges > 0 ? kPhaseLinearize : kPhaseDone;
+  s.it = s.trial = s.converged = s.iterations = 0;
+}
+
+/// L | b of the window from its edges' sums: H_ii += H_e, H_ij += H_e A_e, H_jj += A_e^T H_e A_e, b_i += b_e, b_j += A_e^T b_e for the free
+/// frames among i, j, edge after edge in member order; then 1e9 |mask - 1| on every free frame's diagonal and lambda on every diagonal entry.
+SGB_HD void joint_assemble(const AlignOptions& o, const JointWindow& w, double lambda, int tid, int nt) {
+  const int n = 6 * w.n_free;
+  double* L = w.work;
+  double* b = L + n * (n + 1) / 2;
+  double* A = b + 3 * n;
+  double* P = A + 36;
+  double* Q = P + 36;
+  double* c = Q + 36;
+  for (int k = tid; k < n * (n + 1) / 2 + n; k += nt) L[k] = 0.0;  // L and b are contiguous
+  SGB_CTA_SYNC();
+  for (int q = 0; q < w.n_edges; q++) {
+    const int fi = w.free[w.ei[q]], fj = w.free[w.ej[q]];
+    const double* H = w.sums + 44 * static_cast<size_t>(q);  // symmetric: row- and column-major agree
+    if (fj >= 0) {
+      if (tid == 0) {
+        double T[16];
+        edge_pose(w.X + 16 * w.ei[q], w.X + 16 * w.ej[q], T);
+        edge_adjoint(T, A);
+      }
+      SGB_CTA_SYNC();
+      for (int k = tid; k < 36; k += nt) {  // P = H A
+        const int r = k / 6, cc = k % 6;
+        double v = 0.0;
+        for (int m = 0; m < 6; m++) v += H[r * 6 + m] * A[m * 6 + cc];
+        P[k] = v;
+      }
+      SGB_CTA_SYNC();
+      for (int k = tid; k < 42; k += nt) {  // Q = A^T P, c = A^T b
+        if (k < 36) {
+          const int r = k / 6, cc = k % 6;
+          double v = 0.0;
+          for (int m = 0; m < 6; m++) v += A[m * 6 + r] * P[m * 6 + cc];
+          Q[k] = v;
+        } else {
+          const int r = k - 36;
+          double v = 0.0;
+          for (int m = 0; m < 6; m++) v += A[m * 6 + r] * H[36 + m];
+          c[r] = v;
+        }
+      }
+      SGB_CTA_SYNC();
+    }
+    for (int k = tid; k < 36 * 3 + 12; k += nt) {  // every target entry is one thread's
+      if (k < 36) {
+        const int r = k / 6, cc = k % 6;
+        if (fi >= 0 && r >= cc) L[packed_index(6 * fi + r, 6 * fi + cc)] += H[r * 6 + cc];
+      } else if (k < 72) {
+        const int r = (k - 36) / 6, cc = (k - 36) % 6;
+        if (fj >= 0 && r >= cc) L[packed_index(6 * fj + r, 6 * fj + cc)] += Q[r * 6 + cc];
+      } else if (k < 108) {
+        const int r = (k - 72) / 6, cc = (k - 72) % 6;
+        if (fi >= 0 && fj >= 0) {
+          if (fi > fj)
+            L[packed_index(6 * fi + r, 6 * fj + cc)] += P[r * 6 + cc];  // H_ij = H_e A_e
+          else
+            L[packed_index(6 * fj + r, 6 * fi + cc)] += P[cc * 6 + r];  // H_ji = A_e^T H_e = P^T
+        }
+      } else if (k < 114) {
+        if (fi >= 0) b[6 * fi + k - 108] += H[36 + k - 108];
+      } else {
+        if (fj >= 0) b[6 * fj + k - 114] += c[k - 114];
+      }
+    }
+    SGB_CTA_SYNC();
+  }
+  for (int k = tid; k < n; k += nt) {
+    const int d = packed_index(k, k);
+    L[d] += 1e9 * fabs(o.dof_mask[k % 6] - 1.0);
+  }
+  SGB_CTA_SYNC();
+  for (int k = tid; k < n; k += nt) L[packed_index(k, k)] += lambda;
+  SGB_CTA_SYNC();
+}
+
+/// delta = (H + lambda I)^-1 (-b) over the window's free frames; returns whether every free frame's step meets the termination criteria
+SGB_HD bool joint_solve(const AlignOptions& o, const JointWindow& w, double lambda, int tid, int nt) {
+  const int n = 6 * w.n_free;
+  joint_assemble(o, w, lambda, tid, nt);
+  double* L = w.work;
+  double* b = L + n * (n + 1) / 2;
+  double* rhs = b + n;
+  double* y = rhs + n;
+  int* perm = reinterpret_cast<int*>(y + n + 36 * 3 + 6);
+  int* flag = perm + n + (n & 1);
+  for (int k = tid; k < n; k += nt) rhs[k] = -b[k];
+  if (tid == 0) *flag = 1;
+  SGB_CTA_SYNC();
+  solve_ldlt_n(n, L, rhs, w.delta, perm, y, tid, nt);
+  for (int f = tid; f < w.n_free; f += nt)
+    if (!step_converged(w.delta + 6 * f, o.rotation_eps, o.translation_eps)) *flag = 0;
+  SGB_CTA_SYNC();
+  const bool conv = *flag != 0;
+  SGB_CTA_SYNC();
+  return conv;
+}
+
+/// out = X exp(delta_k) for the free frames, X for the fixed ones
+SGB_HD void joint_update(const JointWindow& w, const double* X, double* out, int tid, int nt) {
+  for (int k = tid; k < w.n_frames; k += nt) {
+    const int f = w.free[k];
+    if (f < 0) {
+      for (int i = 0; i < 16; i++) out[16 * k + i] = X[16 * k + i];
+      continue;
+    }
+    double E[16], T[16];
+    se3_exp6(w.delta + 6 * f, E);
+    pose_mul(X + 16 * k, E, T);
+    for (int i = 0; i < 16; i++) out[16 * k + i] = T[i];
+  }
+  SGB_CTA_SYNC();
+}
+
+SGB_HD void joint_end_iteration(const AlignOptions& o, WindowState& s) {
+  s.iterations = s.it;
+  s.it++;
+  s.phase = (s.it < o.max_iterations && !s.converged) ? kPhaseLinearize : kPhaseDone;
+}
+
+/// align_after_linearize for a window: the edges' sums of the linearize at X are in w.sums
+SGB_HD void joint_after_linearize(const AlignOptions& o, JointWindow& w, int tid, int nt) {
+  WindowState& s = *w.s;
+  if (tid == 0) {
+    double e = 0.0, inl = 0.0;
+    for (int q = 0; q < w.n_edges; q++) {
+      e += w.sums[44 * static_cast<size_t>(q) + 42];
+      inl += w.sums[44 * static_cast<size_t>(q) + 43];
+    }
+    s.e = e;
+    s.inliers = inl;
+  }
+  SGB_CTA_SYNC();
+  if (!o.lm) {
+    const bool conv = joint_solve(o, w, o.gn_lambda, tid, nt);
+    joint_update(w, w.X, w.cand, tid, nt);
+    for (int k = tid; k < 16 * w.n_frames; k += nt) w.X[k] = w.cand[k];
+    if (tid == 0) {
+      s.converged = conv;
+      joint_end_iteration(o, s);
+    }
+    SGB_CTA_SYNC();
+    return;
+  }
+  if (o.max_inner_iterations <= 0) {  // no trial: nothing accepted
+    if (tid == 0) {
+      s.trial = 0;
+      s.iterations = s.it;
+      s.phase = kPhaseDone;
+    }
+    SGB_CTA_SYNC();
+    return;
+  }
+  const double lambda = s.lambda;
+  joint_solve(o, w, lambda, tid, nt);
+  joint_update(w, w.X, w.cand, tid, nt);
+  if (tid == 0) {
+    s.trial = 0;
+    s.phase = kPhaseTrial;
+  }
+  SGB_CTA_SYNC();
+}
+
+/// align_after_error for a window: candidate_e = the window's error() at w.cand, summed over its edges in member order
+SGB_HD void joint_after_error(const AlignOptions& o, JointWindow& w, double candidate_e, int tid, int nt) {
+  WindowState& s = *w.s;
+  const double e = s.e, lambda = s.lambda;
+  const int trial = s.trial;
+  SGB_CTA_SYNC();
+  if (candidate_e <= e) {
+    bool conv = true;
+    for (int f = 0; f < w.n_free; f++) conv = conv && step_converged(w.delta + 6 * f, o.rotation_eps, o.translation_eps);
+    for (int k = tid; k < 16 * w.n_frames; k += nt) w.X[k] = w.cand[k];
+    if (tid == 0) {
+      s.converged = conv;
+      s.lambda = lambda / o.lambda_factor;
+      s.e = candidate_e;
+      joint_end_iteration(o, s);
+    }
+    SGB_CTA_SYNC();
+    return;
+  }
+  const double next = lambda * o.lambda_factor;
+  if (trial + 1 < o.max_inner_iterations) {
+    joint_solve(o, w, next, tid, nt);
+    joint_update(w, w.X, w.cand, tid, nt);
+  }
+  if (tid == 0) {
+    s.lambda = next;
+    s.trial = trial + 1;
+    if (s.trial >= o.max_inner_iterations) {
+      s.iterations = s.it;  // every trial rejected: the reference breaks out of the outer loop
+      s.phase = kPhaseDone;
+    }
+  }
+  SGB_CTA_SYNC();
+}
+
 }  // namespace sgb
