@@ -386,6 +386,24 @@ int sgb_align_joint(sgb_ctx* ctx, const sgb_align_options* options, size_t n_win
  *     the same at capture and nothing at replay. */
 int sgb_align_batch_async(sgb_ctx* ctx, const sgb_align_options* options, const double* d_init_T16xB, double* d_out_T16xB, double* d_out_info4xB,
                           double* d_out_Hb42xB /*or NULL*/);
+/* sgb_align_joint enqueued on the context's stream with no host involvement after the call, as sgb_align_batch_async enqueues
+ * sgb_align_batch: the edges are the members of the device loop's rounds, each edge's phase its window's, and one joint step per round
+ * (one CTA per window) writes the windows' new phases to their edges and keeps the loop running while a window has a round to go.
+ *   - Arguments, checks, messages and results as sgb_align_joint: for the same inputs out_X16xK and out_info4xW are bit-identical to it,
+ *     fixed frames come back bit for bit from d_init_X16xK, and the context is left as sgb_align_joint leaves it (sgb_correspondences_batch,
+ *     sgb_error_batch and sgb_linearize_batch on the edges afterwards).  window_off and fixed are host memory, read during the call; poses
+ *     and outputs are device memory of the context's GPU (host, page-locked or managed pointers fail with a message, nothing enqueued).
+ *   - The window tables built from window_off, fixed and the pairing are cached in the context, apart from sgb_align_joint's: a call whose
+ *     tables are unchanged uploads nothing; one whose tables changed uploads them once.
+ *   - While the context's stream is being captured the align is added to the capture (each replay re-runs it from what d_init_X16xK holds
+ *     then); a call that would have to allocate or to upload its window tables fails with a message instead: call it once outside the
+ *     capture first.  The captured work is only valid while the context's batch, pairing, target, windows and fixed flags are those of
+ *     the capture.  Outside a capture the loop's instantiated graph is cached and rebuilt when anything it captured changes.
+ *   - sgb_kernel_launches counts 3 per call with max_iterations > 0 and at least one edge (initial state, one launch of the loop graph,
+ *     outputs) and 2 otherwise, whatever the round count, plus 1 when the pairing's view of the target is rebuilt; captured work counts at
+ *     capture, not at replay.  A call with no window enqueues nothing. */
+int sgb_align_joint_async(sgb_ctx* ctx, const sgb_align_options* options, size_t n_windows, const size_t* window_off, const uint8_t* fixed /*or NULL*/,
+                          const double* d_init_X16xK, double* d_out_X16xK, double* d_out_info4xW);
 
 /* ---- per-cloud preparation on the device (SURVEY.md §8(f); not per-iteration) --------------------
  * sgb_estimate_features replaces estimate_normals / estimate_covariances / estimate_normals_covariances and

@@ -88,6 +88,7 @@ _SIGNATURES = {
     "sgb_align_batch": (C.c_int, [_vp, C.POINTER(AlignOptions), _dp, _dp, _dp, _dp]),
     "sgb_align_batch_async": (C.c_int, [_vp, C.POINTER(AlignOptions), _dp, _dp, _dp, _dp]),
     "sgb_align_joint": (C.c_int, [_vp, C.POINTER(AlignOptions), C.c_size_t, C.POINTER(C.c_size_t), C.POINTER(C.c_uint8), _dp, _dp, _dp]),
+    "sgb_align_joint_async": (C.c_int, [_vp, C.POINTER(AlignOptions), C.c_size_t, C.POINTER(C.c_size_t), C.POINTER(C.c_uint8), _dp, _dp, _dp]),
     "sgb_estimate_features": (C.c_int, [_vp, C.c_size_t, _dp, C.c_int, _dp, _dp]),
     "sgb_target_estimate_features": (C.c_int, [_vp, C.c_int]),
     "sgb_source_estimate_features": (C.c_int, [_vp, C.c_int]),
@@ -159,6 +160,21 @@ class AsyncAlignResult:
         self.error = info4[:, 3]
         self.H = Hb42[:, :36].view(B, 6, 6).transpose(1, 2)
         self.b = Hb42[:, 36:42]
+
+
+class AsyncJointAlignResult:
+    """what Context.align_joint_async enqueued: CUDA float64 tensors filled in stream order.  X (K,4,4) per frame; converged (1.0 / 0.0),
+    iterations, num_inliers and error (W,) per window, as in JointAlignResult.  All are views of the raw outputs X16 (K,16) and info4 (W,4),
+    which pass as out= to reuse them (graph capture needs fixed buffers)."""
+
+    def __init__(self, X16, info4):
+        K = X16.shape[0]
+        self.X16, self.info4 = X16, info4
+        self.X = X16.view(K, 4, 4).transpose(1, 2)
+        self.converged = info4[:, 0]
+        self.iterations = info4[:, 1]
+        self.num_inliers = info4[:, 2]
+        self.error = info4[:, 3]
 
 
 def library_path(profiling=False):
@@ -248,6 +264,7 @@ class Context:
         self.device = int(device)
         self._stream = None  # set_stream's stream (None: the context's own)
         self._async_in = None  # align_batch_async's column-major poses
+        self._joint_in = None  # align_joint_async's column-major frame poses
 
     def close(self):
         if getattr(self, "_h", None):
@@ -689,6 +706,45 @@ class Context:
                 self._async_in = torch.empty((max(B, 1), 16), dtype=torch.float64, device=dev)[:B]
             self._async_in.view(B, 4, 4).copy_(init_Ts.transpose(1, 2))  # column-major
         self._check(self._L.sgb_align_batch_async(self._h, C.byref(o), _d(self._async_in), _d(out.T16), _d(out.info4), _d(out.Hb42)))
+        return out
+
+    def align_joint_async(self, init_X, windows=None, fixed=None, factor=FACTOR_GICP, robust=ROBUST_NONE, robust_c=1.0, rejector=REJECT_DISTANCE,
+                          max_dist_sq=1.0, optimizer=OPT_LEVENBERG_MARQUARDT, max_iterations=20, gn_lambda=1e-6, max_inner_iterations=10, init_lambda=1e-3,
+                          lambda_factor=10.0, rotation_eps=0.1 * np.pi / 180.0, translation_eps=1e-3, dof_mask=None, out=None):
+        """align_joint enqueued on the context's stream without a host synchronisation (sgb_align_joint_async).  init_X: CUDA float64 (K, 4, 4)
+        row-major frame poses on the context's device, transposed on the context's stream (set_stream: a torch stream); windows, fixed and the
+        other keywords as in align_joint.  Returns an AsyncJointAlignResult of CUDA tensors (out: a previous result whose buffers are reused).
+        Inside torch.cuda.graph (with the capture stream set) the align is captured: each replay re-runs it from what init_X holds then."""
+        import torch
+
+        if self._stream is None:
+            raise SgbError("align_joint_async: set the context's stream to a torch stream first (set_stream): the poses are prepared on it")
+        K = self._cloud_offsets.size - 1 if hasattr(self, "_cloud_offsets") else 0
+        if not (isinstance(init_X, torch.Tensor) and init_X.is_cuda and init_X.dtype == torch.float64 and tuple(init_X.shape) == (K, 4, 4)):
+            raise SgbError(f"align_joint_async: init_X must be a CUDA float64 tensor of shape ({K}, 4, 4)")
+        off = np.ascontiguousarray(np.array([0, K] if windows is None else windows, dtype=np.uintp).reshape(-1))
+        if off.size < 1:
+            raise SgbError("align_joint_async: windows needs at least one entry")
+        W = off.size - 1
+        fx = None if fixed is None else np.ascontiguousarray(np.asarray(fixed).astype(np.uint8).reshape(-1))
+        if fx is not None and fx.size != K:
+            raise SgbError(f"align_joint_async: fixed needs {K} entries")
+        o = AlignOptions(int(factor), int(robust), float(robust_c), int(rejector), float(max_dist_sq), int(optimizer), int(max_iterations), float(gn_lambda),
+                         int(max_inner_iterations), float(init_lambda), float(lambda_factor), float(rotation_eps), float(translation_eps))
+        o.dof_mask[:] = [1.0] * 6 if dof_mask is None else [float(x) for x in dof_mask]
+        dev = init_X.device
+        with torch.cuda.stream(torch.cuda.ExternalStream(self._stream, device=dev)):
+            if out is None:
+                out = AsyncJointAlignResult(torch.zeros((max(K, 1), 16), dtype=torch.float64, device=dev)[:K],
+                                            torch.zeros((max(W, 1), 4), dtype=torch.float64, device=dev)[:W])
+            elif tuple(out.X16.shape) != (K, 16) or tuple(out.info4.shape) != (W, 4):
+                raise SgbError(f"align_joint_async: out holds {out.X16.shape[0]} frames and {out.info4.shape[0]} windows, the call {K} and {W}")
+            if self._joint_in is None or self._joint_in.shape[0] != K or self._joint_in.device != dev:
+                self._joint_in = torch.empty((max(K, 1), 16), dtype=torch.float64, device=dev)[:K]
+            self._joint_in.view(K, 4, 4).copy_(init_X.transpose(1, 2))  # column-major
+        self._check(self._L.sgb_align_joint_async(self._h, C.byref(o), W, off.ctypes.data_as(C.POINTER(C.c_size_t)),
+                                                  None if fx is None else fx.ctypes.data_as(C.POINTER(C.c_uint8)), _d(self._joint_in), _d(out.X16),
+                                                  _d(out.info4)))
         return out
 
     # ---- multi-GPU: all-reduce of H|b|e fused into the reduction kernel (peer memory over NVLink) ----

@@ -15,8 +15,11 @@
 //   pair_gather_kernel      sgb_source_set_pairs: every member's replica of its stored cloud, in one launch over all member points
 //   pair_view_kernel        the many-maps tables above seen through the pairing (member p -> map maps[p]), one CTA
 //   submap_view_kernel      the per-entry tables of the submap lists from the target's per-map tables, one thread per entry
-// The transform, factor, segment and step kernels serve the rounds the host plans (sgb_{linearize,error,align}_batch) and, with ROUND /
-// kModeRound, the rounds batch_plan_kernel plans on the device (sgb_align_batch_async).
+//   joint_step_kernel       joint windows: one CTA per window, its system assembled from its edges' sums and solved, its state machine,
+//                           its edges' next poses (sgb_align_joint; joint_align_init_kernel / joint_align_finish_kernel: the asynchronous
+//                           call's set-up and outputs)
+// The transform, factor, segment and step kernels serve the rounds the host plans (sgb_{linearize,error,align}_batch, sgb_align_joint) and,
+// with ROUND / kModeRound, the rounds batch_plan_kernel plans on the device (sgb_align_batch_async, sgb_align_joint_async).
 // A member's sums depend on its own points, pose and correspondences only, added in an order fixed by its size: bit-identical whatever
 // else is in the batch.
 #include <algorithm>
@@ -661,13 +664,25 @@ __global__ void joint_edge_poses_kernel(const __grid_constant__ JointParams J) {
 
 // One CTA per window; the window's system (packed lower triangle, up to 192 x 192) and the solve's scratch in dynamic shared memory.
 // Threads take the rows of each column of the factorisation (n <= 192 < kJointBlock), the entries of each edge's blocks, the frames.
+// ROUND (a round of sgb_align_joint_async): the round's kind is read from `round`; a window outside it sets `loop` to 1 if it still has a
+// round to go, a stepped window writes its new phase to its edges' member_phase (what the next round's planner reads) and sets `loop` too.
 constexpr int kJointBlock = 256;
+template <bool ROUND>
 __global__ void __launch_bounds__(kJointBlock) joint_step_kernel(const __grid_constant__ AlignOptions o, const __grid_constant__ JointParams J, bool linearize,
-                                                                 const double* __restrict__ out) {
+                                                                 const double* __restrict__ out, const BatchRound* __restrict__ round,
+                                                                 cudaGraphConditionalHandle loop, uint8_t* __restrict__ member_phase) {
   extern __shared__ double s_work[];
   const uint32_t w = blockIdx.x;
   const int tid = threadIdx.x, nt = blockDim.x;
   WindowState* s = J.state + w;
+  if constexpr (ROUND) {
+    linearize = round->lin != 0u;
+    const int ph = s->phase;
+    if (ph != (linearize ? kPhaseLinearize : kPhaseTrial)) {
+      if (tid == 0 && (ph == kPhaseLinearize || ph == kPhaseTrial)) cudaGraphSetConditional(loop, 1u);
+      return;
+    }
+  }
   if (s->phase != (linearize ? kPhaseLinearize : kPhaseTrial)) return;
   const uint32_t f0 = J.frame_off[w], e0 = J.edge_off[w];
   JointWindow win;
@@ -696,6 +711,11 @@ __global__ void __launch_bounds__(kJointBlock) joint_step_kernel(const __grid_co
   const double* X = s->phase == kPhaseTrial ? win.cand : win.X;
   for (int q = tid; q < win.n_edges; q += nt) joint_write_edge_pose(J, e0 + q, X);
   if (tid == 0) J.phase[w] = static_cast<uint8_t>(s->phase);
+  if constexpr (ROUND) {
+    const int ph = s->phase;
+    for (int q = tid; q < win.n_edges; q += nt) member_phase[J.edge_member[e0 + q]] = static_cast<uint8_t>(ph);
+    if (tid == 0 && (ph == kPhaseLinearize || ph == kPhaseTrial)) cudaGraphSetConditional(loop, 1u);
+  }
 }
 
 cudaError_t launch_joint_edge_poses(const JointParams& J, cudaStream_t st) {
@@ -704,13 +724,70 @@ cudaError_t launch_joint_edge_poses(const JointParams& J, cudaStream_t st) {
   return cudaGetLastError();
 }
 
-cudaError_t launch_joint_step(const AlignOptions& o, const JointParams& J, int max_free, bool linearize, const double* out, cudaStream_t st) {
+cudaError_t launch_joint_step(const AlignOptions& o, const JointParams& J, int max_free, bool linearize, const BatchRound* round, cudaGraphConditionalHandle loop,
+                              uint8_t* member_phase, const double* out, cudaStream_t st) {
+  const auto kernel = round ? joint_step_kernel<true> : joint_step_kernel<false>;
   const size_t smem = joint_step_smem(max_free);
   if (smem > 48 * 1024) {
-    const cudaError_t e = cudaFuncSetAttribute(joint_step_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
+    const cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
     if (e != cudaSuccess) return e;
   }
-  joint_step_kernel<<<J.n_windows, kJointBlock, smem, st>>>(o, J, linearize, out);
+  kernel<<<J.n_windows, kJointBlock, smem, st>>>(o, J, linearize, out, round, loop, member_phase);
+  return cudaGetLastError();
+}
+
+// ---- sgb_align_joint_async (DESIGN.md §11 "Asynchronous joint windows") ----
+
+// One CTA per window: sgb_align_joint's set-up on the device.  Thread 0 runs joint_init; the frames' X are copied from init_X16; then
+// every edge gets its initial pose (joint_write_edge_pose, as joint_edge_poses_kernel), its window's phase as its member phase (what the
+// planner reads) and, unless keep_seeds, a cleared seed flag (as batch_align_init_kernel clears a member's).
+__global__ void __launch_bounds__(kStepBlock) joint_align_init_kernel(const __grid_constant__ AlignOptions o, const __grid_constant__ JointParams J,
+                                                                      const double* __restrict__ init_X16, uint8_t* __restrict__ member_phase,
+                                                                      uint8_t* __restrict__ seeded, int keep_seeds) {
+  __shared__ uint8_t s_phase;
+  const uint32_t w = blockIdx.x, f0 = J.frame_off[w], f1 = J.frame_off[w + 1], e0 = J.edge_off[w], e1 = J.edge_off[w + 1];
+  if (threadIdx.x == 0) {
+    joint_init(o, static_cast<int>(J.n_free[w]), static_cast<int>(e1 - e0), J.state[w]);
+    s_phase = static_cast<uint8_t>(J.state[w].phase);
+    J.phase[w] = s_phase;
+  }
+  for (size_t k = 16 * static_cast<size_t>(f0) + threadIdx.x; k < 16 * static_cast<size_t>(f1); k += kStepBlock) J.X[k] = init_X16[k];
+  __syncthreads();
+  for (uint32_t q = e0 + threadIdx.x; q < e1; q += kStepBlock) {
+    joint_write_edge_pose(J, q, J.X + 16 * static_cast<size_t>(f0));
+    const uint32_t m = J.edge_member[q];
+    member_phase[m] = s_phase;
+    if (!keep_seeds) seeded[m] = 0;
+  }
+}
+
+// sgb_align_joint's outputs: thread i writes frame i's X (a fixed frame's from init_X16, bit for bit) and window i's info
+__global__ void __launch_bounds__(kStepBlock) joint_align_finish_kernel(const __grid_constant__ JointParams J, uint32_t n_frames, const double* __restrict__ init_X16,
+                                                                        double* __restrict__ out_X16, double* __restrict__ out_info4) {
+  const uint32_t i = blockIdx.x * kStepBlock + threadIdx.x;
+  if (i < n_frames) {
+    const double* X = (J.free[i] < 0 ? init_X16 : J.X) + 16 * static_cast<size_t>(i);
+    for (int k = 0; k < 16; k++) out_X16[16 * static_cast<size_t>(i) + k] = X[k];
+  }
+  if (i < J.n_windows) {
+    const WindowState& s = J.state[i];
+    double* info = out_info4 + 4 * static_cast<size_t>(i);
+    info[0] = s.converged ? 1.0 : 0.0;
+    info[1] = s.iterations;
+    info[2] = s.inliers;
+    info[3] = s.e;
+  }
+}
+
+cudaError_t launch_joint_align_init(const AlignOptions& o, const JointParams& J, const double* init_X16, uint8_t* member_phase, uint8_t* seeded, bool keep_seeds,
+                                    cudaStream_t st) {
+  joint_align_init_kernel<<<J.n_windows, kStepBlock, 0, st>>>(o, J, init_X16, member_phase, seeded, keep_seeds ? 1 : 0);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_joint_align_finish(const JointParams& J, uint32_t n_frames, const double* init_X16, double* out_X16, double* out_info4, cudaStream_t st) {
+  const uint32_t n = std::max(n_frames, J.n_windows);
+  joint_align_finish_kernel<<<(n + kStepBlock - 1) / kStepBlock, kStepBlock, 0, st>>>(J, n_frames, init_X16, out_X16, out_info4);
   return cudaGetLastError();
 }
 

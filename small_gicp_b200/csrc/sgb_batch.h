@@ -163,7 +163,19 @@ inline size_t joint_step_smem(int max_free) { return static_cast<size_t>(joint_w
 /// every edge's pose X_j^-1 X_i (row-major R | t) from the frames' X
 cudaError_t launch_joint_edge_poses(const JointParams& J, cudaStream_t st);
 /// one CTA per window: every window in the round's phase (linearize: kPhaseLinearize, else kPhaseTrial) takes its step from `out` (what
-/// launch_batch_segment wrote for the edges), then writes its edges' next poses and its phase
-cudaError_t launch_joint_step(const AlignOptions& o, const JointParams& J, int max_free, bool linearize, const double* out, cudaStream_t st);
+/// launch_batch_segment wrote for the edges), then writes its edges' next poses and its phase.  With a round (planned on the device) the
+/// kind is the round's, every stepped window's phase goes to its edges' member_phase too, and `loop` is set to 1 while a window still
+/// has a round to go.
+cudaError_t launch_joint_step(const AlignOptions& o, const JointParams& J, int max_free, bool linearize, const BatchRound* round, cudaGraphConditionalHandle loop,
+                              uint8_t* member_phase, const double* out, cudaStream_t st);
+
+// ---- sgb_align_joint_async (DESIGN.md §11 "Asynchronous joint windows"): the rounds of sgb_align_joint planned on the device ----
+/// one CTA per window: joint_init, the frames' X from init_X16 (column-major), every edge's initial pose, its window's phase as its member
+/// phase, and its seed flag cleared unless keep_seeds
+cudaError_t launch_joint_align_init(const AlignOptions& o, const JointParams& J, const double* init_X16, uint8_t* member_phase, uint8_t* seeded, bool keep_seeds,
+                                    cudaStream_t st);
+/// sgb_align_joint's outputs from the windows' final state: X (16, column-major) per frame, fixed frames copied from init_X16; info
+/// (converged, iterations, inliers, error) per window
+cudaError_t launch_joint_align_finish(const JointParams& J, uint32_t n_frames, const double* init_X16, double* out_X16, double* out_info4, cudaStream_t st);
 
 }  // namespace sgb

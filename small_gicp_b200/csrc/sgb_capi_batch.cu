@@ -1,6 +1,7 @@
 // SPDX-License-Identifier: MIT
 // C-ABI of batched registration (include/sgicp_b200.h: sgb_source_set_batch, sgb_source_set_pairs, sgb_source_set_submaps,
-// sgb_{linearize,error,align,correspondences}_batch, sgb_{linearize,error}_batch_points, sgb_align_batch_async).
+// sgb_{linearize,error,align,correspondences}_batch, sgb_{linearize,error}_batch_points, sgb_align_batch_async, sgb_align_joint,
+// sgb_align_joint_async).
 // Kernels in sgb_batch.cu (many kd-trees and submaps: the searches in sgb_forest.cu); DESIGN.md §11.
 #include <cuda_runtime.h>
 
@@ -446,7 +447,7 @@ int pair_members(sgb_ctx* ctx, const char* who, size_t n_members, const uint32_t
   return 0;
 }
 
-// ---- sgb_align_batch_async (DESIGN.md §11 "Asynchronous align") ----
+// ---- the device loop of sgb_align_batch_async and sgb_align_joint_async (DESIGN.md §11 "Asynchronous align", "Asynchronous joint windows") ----
 
 // the kernel parameters every round of the device loop shares (those of linearize_round; error() reads the same ones)
 void round_params(sgb_ctx* ctx, const sgb_align_options* o, LinParams& P, BatchParams& Bp) {
@@ -456,9 +457,9 @@ void round_params(sgb_ctx* ctx, const sgb_align_options* o, LinParams& P, BatchP
   Bp.robust_c = o->robust_c;
 }
 
-// One round of the device loop on ctx->stream: planner, search, factor, per-member sums, step.  Every grid is sized for the worst case
-// (every tile, every point, every member); what the round does is read from b_round.
-int async_round(sgb_ctx* ctx, const sgb_align_options* o, const AlignOptions& ao, cudaGraphConditionalHandle loop) {
+// The head of one round of a device loop on ctx->stream: planner, search, factor, per-member sums into b_out.  Every grid is sized for
+// the worst case (every tile, every point, every member); what the round does is read from b_round.  The caller's step follows.
+int round_head(sgb_ctx* ctx, const sgb_align_options* o, cudaGraphConditionalHandle loop) {
   const size_t B = batch_members(ctx);
   const uint32_t T = static_cast<uint32_t>(max_tiles(ctx));
   const bool voxel = voxel_target(ctx), no_target = ctx->n_tgt == 0, point = !no_target && !voxel && !ctx->b_submaps && ctx->tgt_state != TargetState::KdTrees;
@@ -493,19 +494,17 @@ int async_round(sgb_ctx* ctx, const sgb_align_options* o, const AlignOptions& ao
     return rc;
   }
   CU(launch_batch_segment(Bp, static_cast<uint32_t>(B), true, round, ctx->b_out.as<double>(), ctx->stream));
-  CU(launch_batch_step(ao, static_cast<uint32_t>(B), true, round, loop, ctx->b_out.as<double>(), ctx->b_state.as<MemberState>(), ctx->b_poses.as<double>(),
-                       ctx->b_phase.as<uint8_t>(), ctx->stream));
   return 0;
 }
 
-// A WHILE node in g (after deps) whose body is one round, captured on the context's capture stream.  The condition starts at 1 at every
-// launch of g (every member starts in kPhaseLinearize when max_iterations > 0); the planner clears it and the step sets it again while a
-// member has a round to go.
-int add_loop(sgb_ctx* ctx, const sgb_align_options* o, const AlignOptions& ao, cudaGraph_t g, const std::vector<cudaGraphNode_t>& deps, cudaGraphNode_t* node) {
+// A WHILE node in g (after deps) whose body is one round -- round_head, then step(loop) -- captured on the context's capture stream.  The
+// condition starts at 1 at every launch of g; the planner clears it and the step sets it again while a member (or window) has a round to go.
+template <typename Step>
+int add_loop(sgb_ctx* ctx, const char* who, const sgb_align_options* o, cudaGraph_t g, const std::vector<cudaGraphNode_t>& deps, cudaGraphNode_t* node, Step step) {
   cudaGraphConditionalHandle h;
   cudaError_t e = cudaGraphConditionalHandleCreate(&h, g, 1, cudaGraphCondAssignDefault);
   if (e != cudaSuccess)
-    return fail(ctx, 2, std::string("sgb_align_batch_async: cudaGraphConditionalHandleCreate: ") + cudaGetErrorString(e) +
+    return fail(ctx, 2, std::string(who) + ": cudaGraphConditionalHandleCreate: " + cudaGetErrorString(e) +
                             " (the device loop needs conditional graph nodes: CUDA 12.4 or later, driver included)");
   cudaGraphNodeParams np = {};
   np.type = cudaGraphNodeTypeConditional;
@@ -517,12 +516,59 @@ int add_loop(sgb_ctx* ctx, const sgb_align_options* o, const AlignOptions& ao, c
   CU(cudaStreamBeginCaptureToGraph(ctx->cap_stream, np.conditional.phGraph_out[0], nullptr, nullptr, 0, cudaStreamCaptureModeRelaxed));
   const cudaStream_t user = ctx->stream;
   ctx->stream = ctx->cap_stream;
-  const int rc = async_round(ctx, o, ao, h);
+  int rc = round_head(ctx, o, h);
+  if (!rc) rc = step(h);
   ctx->stream = user;
   cudaGraph_t body = nullptr;
   e = cudaStreamEndCapture(ctx->cap_stream, &body);
   if (rc) return rc;
   CU(e);
+  return 0;
+}
+
+// One launch of a device loop (add_loop) on ctx->stream.  While the stream is captured the WHILE node joins the capture after what it
+// already holds; otherwise the instantiated graph cached in exec under cached_key is launched, rebuilt first when key (everything the
+// loop captured) differs from it.
+template <typename Step>
+int launch_loop(sgb_ctx* ctx, const char* who, const sgb_align_options* o, bool capturing, std::vector<unsigned char> key, cudaGraphExec_t& exec,
+                std::vector<unsigned char>& cached_key, Step step) {
+  if (capturing) {
+    cudaStreamCaptureStatus capture = cudaStreamCaptureStatusNone;
+    cudaGraph_t g = nullptr;
+    const cudaGraphNode_t* d = nullptr;
+    size_t nd = 0;
+    CU(cudaStreamGetCaptureInfo(ctx->stream, &capture, nullptr, &g, &d, &nd));
+    const std::vector<cudaGraphNode_t> deps(d, d + nd);
+    cudaGraphNode_t w = nullptr;
+    if (int rc = add_loop(ctx, who, o, g, deps, &w, step)) return rc;
+    CU(cudaStreamUpdateCaptureDependencies(ctx->stream, &w, 1, cudaStreamSetCaptureDependencies));
+    return 0;
+  }
+  if (!exec || key != cached_key) {
+    if (exec) cudaGraphExecDestroy(exec);
+    exec = nullptr;
+    cached_key.clear();
+    cudaGraph_t g = nullptr;
+    CU(cudaGraphCreate(&g, 0));
+    cudaGraphNode_t w = nullptr;
+    const int rc = add_loop(ctx, who, o, g, {}, &w, step);
+    const cudaError_t e = rc ? cudaSuccess : cudaGraphInstantiate(&exec, g, 0);
+    cudaGraphDestroy(g);
+    if (rc) return rc;
+    CU(e);
+    cached_key.swap(key);
+  }
+  CU(cudaGraphLaunch(exec, ctx->stream));
+  return 0;
+}
+
+// the search counters are left cleared after a device loop, as the synchronous calls expect them
+int clear_search_counters(sgb_ctx* ctx) {
+  if (ctx->grid_ready) {
+    CU(cudaMemsetAsync(ctx->grid_pending.p, 0, 2 * sizeof(uint32_t), ctx->stream));
+    if (ctx->use_chunk_classes) CU(cudaMemsetAsync(ctx->chunk_lists.p, 0, 8 * sizeof(uint32_t), ctx->stream));
+  }
+  if (ctx->use_packet_queue && ctx->packet_queue.p) CU(cudaMemsetAsync(ctx->packet_queue.p, 0, 2 * sizeof(uint32_t), ctx->stream));
   return 0;
 }
 
@@ -567,10 +613,10 @@ bool on_device(const sgb_ctx* ctx, const void* p) {
   return e == cudaSuccess && a.type == cudaMemoryTypeDevice && a.device == ctx->device;
 }
 
-// the same as a check; what names p in the message
-int device_pointer(sgb_ctx* ctx, const void* p, const char* what) {
+// the same as a check of who's argument; what names p in the message
+int device_pointer(sgb_ctx* ctx, const char* who, const void* p, const char* what) {
   if (!on_device(ctx, p))
-    return fail(ctx, 1, std::string("sgb_align_batch_async: ") + what + " must be device memory of the context's GPU (cuda:" + std::to_string(ctx->device) +
+    return fail(ctx, 1, std::string(who) + ": " + what + " must be device memory of the context's GPU (cuda:" + std::to_string(ctx->device) +
                             "); host, page-locked and managed memory are refused");
   return 0;
 }
@@ -923,10 +969,27 @@ int sgb_align_batch(sgb_ctx* ctx, const sgb_align_options* o, const double* init
   return 0;
 }
 
-int sgb_align_joint(sgb_ctx* ctx, const sgb_align_options* o, size_t n_windows, const size_t* window_off, const uint8_t* fixed, const double* init_X,
-                    double* out_X, double* out_info) {
-  if (!ctx) return 1;
-  const std::string who = "sgb_align_joint";
+}  // extern "C"
+
+namespace {
+
+// ---- joint windows (DESIGN.md §11 "Joint windows", "Asynchronous joint windows") ----
+
+// What both joint aligns build from their arguments: the window tables, each window's free frame and edge counts, and the most free
+// frames of a window with an edge (which sizes the step's shared memory).  tab = frame_off [W + 1] | edge_off [W + 1] | n_free [W] |
+// edge_member [E] | edge_win [E] | edge_i [E] | edge_j [E] | free [K], the layout JointParams reads.
+struct JointLayout {
+  size_t W = 0, K = 0, E = 0;
+  std::vector<uint32_t> tab, n_free, edge_count;
+  int max_free = 0;
+  const uint32_t* edge_member() const { return tab.data() + 3 * W + 2; }
+  const uint32_t* edge_win() const { return edge_member() + E; }
+  const int32_t* free() const { return reinterpret_cast<const int32_t*>(edge_win() + 3 * E); }
+};
+
+// The checks both joint aligns make before anything is enqueued (who names the caller), and their layout
+int joint_layout(sgb_ctx* ctx, const std::string& who, const sgb_align_options* o, size_t n_windows, const size_t* window_off, const uint8_t* fixed,
+                 const double* init_X, const double* out_X, const double* out_info, AlignOptions& ao, JointLayout& L) {
   if (ctx->src_state != SourceState::Batch) return fail(ctx, 1, who + ": the context holds no batch of sources (call sgb_source_set_batch)");
   if (ctx->b_submaps) return fail(ctx, 1, who + ": the members are submap members (sgb_source_set_submaps); joint windows need (cloud, map) edges");
   if (!ctx->b_paired || !ctx->b_pair_has_maps)
@@ -938,7 +1001,6 @@ int sgb_align_joint(sgb_ctx* ctx, const sgb_align_options* o, size_t n_windows, 
   if (K != target_maps(ctx))
     return fail(ctx, 1, who + ": frame k is cloud k with map k, but the batch holds " + std::to_string(K) + " clouds and the target " +
                             std::to_string(target_maps(ctx)) + " maps");
-  AlignOptions ao;
   if (int rc = align_checks(ctx, who.c_str(), o, init_X, out_X, out_info, ao)) return rc;
   if (!window_off) return fail(ctx, 1, who + ": null window offsets");
   if (n_windows > SGB_BATCH_MAX_MEMBERS)
@@ -973,11 +1035,6 @@ int sgb_align_joint(sgb_ctx* ctx, const sgb_align_options* o, size_t n_windows, 
     if (edge_count[w] && n_free[w] == window_off[w + 1] - window_off[w])
       return fail(ctx, 1, who + ": window " + std::to_string(w) + " has edges but no fixed frame (its gauge would be free)");
   }
-  CU(cudaSetDevice(ctx->device));
-  if (E) {
-    if (int rc = pair_view(ctx)) return rc;
-  }
-  // the tables: frame_off [W + 1] | edge_off [W + 1] | n_free [W] | edge_member [E] | edge_win [E] | edge_i [E] | edge_j [E] | free [K]
   const size_t W = n_windows;
   std::vector<uint32_t> tab(2 * (W + 1) + W + 4 * E + K);
   uint32_t* frame_off = tab.data();
@@ -999,30 +1056,35 @@ int sgb_align_joint(sgb_ctx* ctx, const sgb_align_options* o, size_t n_windows, 
     edge_i[q] = static_cast<int32_t>(i - window_off[w]);
     edge_j[q] = static_cast<int32_t>(j - window_off[w]);
   }
-  int max_free = 0;
+  L.max_free = 0;
   for (size_t w = 0; w < W; w++) {
     nf[w] = n_free[w];
-    if (edge_count[w]) max_free = std::max(max_free, static_cast<int>(n_free[w]));
+    if (edge_count[w]) L.max_free = std::max(L.max_free, static_cast<int>(n_free[w]));
   }
   std::copy(free_of.begin(), free_of.end(), freeidx);
-  std::vector<WindowState> state(W);
-  std::vector<uint8_t> phase(W);
-  for (size_t w = 0; w < W; w++) {
-    joint_init(ao, static_cast<int>(n_free[w]), static_cast<int>(edge_count[w]), state[w]);
-    phase[w] = static_cast<uint8_t>(state[w].phase);
-  }
-  const size_t K1 = std::max<size_t>(K, 1), W1 = std::max<size_t>(W, 1);
-  CU(ctx->j_tables.reserve(tab.size() * sizeof(uint32_t)));
-  CU(ctx->j_X.reserve(K1 * 16 * sizeof(double)));
-  CU(ctx->j_cand.reserve(K1 * 16 * sizeof(double)));
-  CU(ctx->j_delta.reserve(K1 * 6 * sizeof(double)));
-  CU(ctx->j_sums.reserve(std::max<size_t>(E, 1) * 44 * sizeof(double)));
-  CU(ctx->j_state.reserve(W1 * sizeof(WindowState)));
-  CU(ctx->j_phase.reserve(W1));
+  L.W = W;
+  L.K = K;
+  L.E = E;
+  L.tab.swap(tab);
+  L.n_free.swap(n_free);
+  L.edge_count.swap(edge_count);
+  return 0;
+}
+
+// the bytes of each of b's buffers a call of layout L uses, in JointBufs order
+std::vector<size_t> joint_bytes(const JointLayout& L) {
+  const size_t K1 = std::max<size_t>(L.K, 1), W1 = std::max<size_t>(L.W, 1);
+  return {L.tab.size() * sizeof(uint32_t), K1 * 16 * sizeof(double), K1 * 16 * sizeof(double), K1 * 6 * sizeof(double),
+          std::max<size_t>(L.E, 1) * 44 * sizeof(double), W1 * sizeof(WindowState), W1};
+}
+std::vector<DevBuf*> joint_buffers(JointBufs& b) { return {&b.tables, &b.X, &b.cand, &b.delta, &b.sums, &b.state, &b.phase}; }
+
+// JointParams over b (its tables laid out as JointLayout::tab)
+JointParams joint_params(sgb_ctx* ctx, const JointBufs& b, size_t W, size_t E) {
   JointParams J = {};
   J.n_windows = static_cast<uint32_t>(W);
   J.n_edges = static_cast<uint32_t>(E);
-  const uint32_t* dt = ctx->j_tables.as<uint32_t>();
+  const uint32_t* dt = b.tables.as<uint32_t>();
   J.frame_off = dt;
   J.edge_off = dt + W + 1;
   J.n_free = J.edge_off + W + 1;
@@ -1031,19 +1093,47 @@ int sgb_align_joint(sgb_ctx* ctx, const sgb_align_options* o, size_t n_windows, 
   J.edge_i = reinterpret_cast<const int*>(J.edge_win + E);
   J.edge_j = J.edge_i + E;
   J.free = J.edge_j + E;
-  J.X = ctx->j_X.as<double>();
-  J.cand = ctx->j_cand.as<double>();
-  J.delta = ctx->j_delta.as<double>();
-  J.sums = ctx->j_sums.as<double>();
-  J.state = ctx->j_state.as<WindowState>();
-  J.phase = ctx->j_phase.as<uint8_t>();
+  J.X = b.X.as<double>();
+  J.cand = b.cand.as<double>();
+  J.delta = b.delta.as<double>();
+  J.sums = b.sums.as<double>();
+  J.state = b.state.as<WindowState>();
+  J.phase = b.phase.as<uint8_t>();
   J.poses = ctx->b_poses.as<double>();
+  return J;
+}
+
+}  // namespace
+
+extern "C" {
+
+int sgb_align_joint(sgb_ctx* ctx, const sgb_align_options* o, size_t n_windows, const size_t* window_off, const uint8_t* fixed, const double* init_X,
+                    double* out_X, double* out_info) {
+  if (!ctx) return 1;
+  AlignOptions ao;
+  JointLayout L;
+  if (int rc = joint_layout(ctx, "sgb_align_joint", o, n_windows, window_off, fixed, init_X, out_X, out_info, ao, L)) return rc;
+  const size_t W = L.W, K = L.K, E = L.E;
+  CU(cudaSetDevice(ctx->device));
+  if (E) {
+    if (int rc = pair_view(ctx)) return rc;
+  }
+  std::vector<WindowState> state(W);
+  std::vector<uint8_t> phase(W);
+  for (size_t w = 0; w < W; w++) {
+    joint_init(ao, static_cast<int>(L.n_free[w]), static_cast<int>(L.edge_count[w]), state[w]);
+    phase[w] = static_cast<uint8_t>(state[w].phase);
+  }
+  const std::vector<size_t> bytes = joint_bytes(L);
+  const std::vector<DevBuf*> bufs = joint_buffers(ctx->joint);
+  for (size_t i = 0; i < bufs.size(); i++) CU(bufs[i]->reserve(bytes[i]));
+  const JointParams J = joint_params(ctx, ctx->joint, W, E);
   // pageable host memory: the copies are staged before cudaMemcpyAsync returns
-  CU(cudaMemcpyAsync(ctx->j_tables.p, tab.data(), tab.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
-  if (K) CU(cudaMemcpyAsync(ctx->j_X.p, init_X, K * 16 * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
+  CU(cudaMemcpyAsync(ctx->joint.tables.p, L.tab.data(), L.tab.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
+  if (K) CU(cudaMemcpyAsync(ctx->joint.X.p, init_X, K * 16 * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
   if (W) {  // the phases too: a window done from the start is never stepped, and the host reads every window's phase after each round
-    CU(cudaMemcpyAsync(ctx->j_state.p, state.data(), W * sizeof(WindowState), cudaMemcpyHostToDevice, ctx->stream));
-    CU(cudaMemcpyAsync(ctx->j_phase.p, phase.data(), W, cudaMemcpyHostToDevice, ctx->stream));
+    CU(cudaMemcpyAsync(ctx->joint.state.p, state.data(), W * sizeof(WindowState), cudaMemcpyHostToDevice, ctx->stream));
+    CU(cudaMemcpyAsync(ctx->joint.phase.p, phase.data(), W, cudaMemcpyHostToDevice, ctx->stream));
   }
   if (E) {
     CU(launch_joint_edge_poses(J, ctx->stream));
@@ -1051,6 +1141,8 @@ int sgb_align_joint(sgb_ctx* ctx, const sgb_align_options* o, size_t n_windows, 
   }
   // Rounds in lockstep as in sgb_align_batch, per window: error() for the edges of every window with a pending trial until none has one,
   // else a linearize of the edges of every window still iterating; each round ends with one joint step launch.
+  const uint32_t* edge_member = L.edge_member();
+  const uint32_t* edge_win = L.edge_win();
   std::vector<uint8_t> active(E);
   for (;;) {
     bool any_trial = false, any_lin = false;
@@ -1066,16 +1158,17 @@ int sgb_align_joint(sgb_ctx* ctx, const sgb_align_options* o, size_t n_windows, 
     } else {
       if (int rc = error_round(ctx, nullptr, active.data())) return rc;
     }
-    CU(launch_joint_step(ao, J, max_free, lin, ctx->b_out.as<double>(), ctx->stream));
+    CU(launch_joint_step(ao, J, L.max_free, lin, nullptr, 0, nullptr, ctx->b_out.as<double>(), ctx->stream));
     ctx->launches += 1;
-    CU(cudaMemcpyAsync(phase.data(), ctx->j_phase.p, W, cudaMemcpyDeviceToHost, ctx->stream));
+    CU(cudaMemcpyAsync(phase.data(), ctx->joint.phase.p, W, cudaMemcpyDeviceToHost, ctx->stream));
     CU(cudaStreamSynchronize(ctx->stream));
   }
   std::vector<double> X(16 * K);
-  if (K) CU(cudaMemcpyAsync(X.data(), ctx->j_X.p, K * 16 * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
-  if (W) CU(cudaMemcpyAsync(state.data(), ctx->j_state.p, W * sizeof(WindowState), cudaMemcpyDeviceToHost, ctx->stream));
+  if (K) CU(cudaMemcpyAsync(X.data(), ctx->joint.X.p, K * 16 * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+  if (W) CU(cudaMemcpyAsync(state.data(), ctx->joint.state.p, W * sizeof(WindowState), cudaMemcpyDeviceToHost, ctx->stream));
   CU(cudaStreamSynchronize(ctx->stream));
-  for (size_t k = 0; k < K; k++) std::memcpy(out_X + 16 * k, fix[k] ? init_X + 16 * k : X.data() + 16 * k, 16 * sizeof(double));
+  const int32_t* freeidx = L.free();
+  for (size_t k = 0; k < K; k++) std::memcpy(out_X + 16 * k, freeidx[k] < 0 ? init_X + 16 * k : X.data() + 16 * k, 16 * sizeof(double));
   for (size_t w = 0; w < W; w++) {
     double* info = out_info + 4 * w;
     info[0] = state[w].converged ? 1.0 : 0.0;
@@ -1094,11 +1187,11 @@ int sgb_align_batch_async(sgb_ctx* ctx, const sgb_align_options* o, const double
   const size_t B = batch_members(ctx);
   if (B == 0) return 0;
   CU(cudaSetDevice(ctx->device));
-  if (int rc = device_pointer(ctx, d_init_T, "init_T16xB")) return rc;
-  if (int rc = device_pointer(ctx, d_out_T, "out_T16xB")) return rc;
-  if (int rc = device_pointer(ctx, d_out_info, "out_info4xB")) return rc;
+  if (int rc = device_pointer(ctx, who, d_init_T, "init_T16xB")) return rc;
+  if (int rc = device_pointer(ctx, who, d_out_T, "out_T16xB")) return rc;
+  if (int rc = device_pointer(ctx, who, d_out_info, "out_info4xB")) return rc;
   if (d_out_Hb) {
-    if (int rc = device_pointer(ctx, d_out_Hb, "out_Hb42xB")) return rc;
+    if (int rc = device_pointer(ctx, who, d_out_Hb, "out_Hb42xB")) return rc;
   }
   cudaStreamCaptureStatus capture = cudaStreamCaptureStatusNone;
   CU(cudaStreamIsCapturing(ctx->stream, &capture));
@@ -1117,46 +1210,107 @@ int sgb_align_batch_async(sgb_ctx* ctx, const sgb_align_options* o, const double
                              ctx->corr_seeds && ctx->b_dseed_ok, ctx->stream));
   ctx->launches += 2;  // the initial state here, the outputs below
   if (o->max_iterations > 0) {
-    if (capturing) {
-      cudaGraph_t g = nullptr;
-      const cudaGraphNode_t* d = nullptr;
-      size_t nd = 0;
-      CU(cudaStreamGetCaptureInfo(ctx->stream, &capture, nullptr, &g, &d, &nd));
-      const std::vector<cudaGraphNode_t> deps(d, d + nd);
-      cudaGraphNode_t w = nullptr;
-      if (int rc = add_loop(ctx, o, ao, g, deps, &w)) return rc;
-      CU(cudaStreamUpdateCaptureDependencies(ctx->stream, &w, 1, cudaStreamSetCaptureDependencies));
-    } else {
-      std::vector<unsigned char> key = loop_key(ctx, o);
-      if (!ctx->align_exec || key != ctx->align_key) {
-        if (ctx->align_exec) cudaGraphExecDestroy(ctx->align_exec);
-        ctx->align_exec = nullptr;
-        ctx->align_key.clear();
-        cudaGraph_t g = nullptr;
-        CU(cudaGraphCreate(&g, 0));
-        cudaGraphNode_t w = nullptr;
-        const int rc = add_loop(ctx, o, ao, g, {}, &w);
-        const cudaError_t e = rc ? cudaSuccess : cudaGraphInstantiate(&ctx->align_exec, g, 0);
-        cudaGraphDestroy(g);
-        if (rc) return rc;
-        CU(e);
-        ctx->align_key.swap(key);
-      }
-      CU(cudaGraphLaunch(ctx->align_exec, ctx->stream));
-    }
+    const auto step = [&](cudaGraphConditionalHandle h) {
+      CU(launch_batch_step(ao, nb, true, ctx->b_round.as<BatchRound>(), h, ctx->b_out.as<double>(), ctx->b_state.as<MemberState>(), ctx->b_poses.as<double>(),
+                           ctx->b_phase.as<uint8_t>(), ctx->stream));
+      return 0;
+    };
+    if (int rc = launch_loop(ctx, who, o, capturing, capturing ? std::vector<unsigned char>() : loop_key(ctx, o), ctx->align_exec, ctx->align_key, step)) return rc;
     ctx->launches += 1;
-    // the search counters are left cleared, as the synchronous calls expect them
-    if (ctx->grid_ready) {
-      CU(cudaMemsetAsync(ctx->grid_pending.p, 0, 2 * sizeof(uint32_t), ctx->stream));
-      if (ctx->use_chunk_classes) CU(cudaMemsetAsync(ctx->chunk_lists.p, 0, 8 * sizeof(uint32_t), ctx->stream));
-    }
-    if (ctx->use_packet_queue) CU(cudaMemsetAsync(ctx->packet_queue.p, 0, 2 * sizeof(uint32_t), ctx->stream));
+    if (int rc = clear_search_counters(ctx)) return rc;
   }
   CU(launch_batch_align_finish(nb, ctx->b_state.as<MemberState>(), d_out_T, d_out_info, d_out_Hb, ctx->stream));
   ctx->b_dseed_ok = true;
   if (o->max_iterations > 0) {  // round 1 linearised every member, as sgb_align_batch's does
     std::fill(ctx->b_lin.begin(), ctx->b_lin.end(), 1);
     std::fill(ctx->b_seeded.begin(), ctx->b_seeded.end(), 1);
+    ctx->have_lin = true;
+    ctx->corr_seeds = true;
+    ctx->lin_factor = o->factor_kind;
+    ctx->lin_robust = o->robust_kind;
+    ctx->lin_c = o->robust_c;
+  }
+  return 0;
+}
+
+int sgb_align_joint_async(sgb_ctx* ctx, const sgb_align_options* o, size_t n_windows, const size_t* window_off, const uint8_t* fixed, const double* d_init_X,
+                          double* d_out_X, double* d_out_info) {
+  if (!ctx) return 1;
+  const char* who = "sgb_align_joint_async";
+  AlignOptions ao;
+  JointLayout L;
+  if (int rc = joint_layout(ctx, who, o, n_windows, window_off, fixed, d_init_X, d_out_X, d_out_info, ao, L)) return rc;
+  const size_t W = L.W, K = L.K, E = L.E;
+  if (W == 0) return 0;
+  CU(cudaSetDevice(ctx->device));
+  if (int rc = device_pointer(ctx, who, d_init_X, "init_X16xK")) return rc;
+  if (int rc = device_pointer(ctx, who, d_out_X, "out_X16xK")) return rc;
+  if (int rc = device_pointer(ctx, who, d_out_info, "out_info4xW")) return rc;
+  cudaStreamCaptureStatus capture = cudaStreamCaptureStatusNone;
+  CU(cudaStreamIsCapturing(ctx->stream, &capture));
+  if (capture == cudaStreamCaptureStatusInvalidated) return fail(ctx, 1, std::string(who) + ": the context's stream is in an invalidated capture");
+  const bool capturing = capture == cudaStreamCaptureStatusActive;
+  const bool loop = o->max_iterations > 0 && E > 0;
+  // A capture can hold neither an allocation nor an upload from pageable memory: the buffers, the capture stream and the window tables
+  // must come from an earlier call.  Outside a capture the tables are uploaded only when they changed (windows, fixed flags or pairing).
+  const std::vector<size_t> bytes = joint_bytes(L);
+  const std::vector<DevBuf*> bufs = joint_buffers(ctx->joint_async);
+  bool grow = false;
+  for (size_t i = 0; i < bufs.size(); i++) grow = grow || bytes[i] > bufs[i]->cap;
+  const bool upload = grow || L.tab != ctx->ja_tab;
+  if (capturing && (upload || (loop && !ctx->cap_stream)))
+    return fail(ctx, 1, std::string(who) + ": these windows need an allocation or an upload of their tables, which a capture cannot hold; call it once "
+                                           "outside the capture first");
+  // ja_tab claims what joint_async.tables holds.  The claim is dropped before anything that can replace or lose that content: a
+  // reservation frees the old buffer before it allocates the new one, and any step below may fail.  So a failed call leaves no claim
+  // behind, and the next call uploads its tables again.
+  if (upload) ctx->ja_tab.clear();
+  for (size_t i = 0; i < bufs.size(); i++) CU(bufs[i]->reserve(bytes[i]));
+  if (upload) {
+    // pageable host memory: the copy is staged before cudaMemcpyAsync returns
+    CU(cudaMemcpyAsync(ctx->joint_async.tables.p, L.tab.data(), L.tab.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
+    ctx->ja_tab = L.tab;
+  }
+  if (E) {
+    if (int rc = pair_view(ctx)) return rc;
+  }
+  const JointParams J = joint_params(ctx, ctx->joint_async, W, E);
+  // the edges are the members: each edge's member phase is its window's, which the planner reads as sgb_align_joint's host loop reads
+  // the windows' phases; the device's seed flags are kept as sgb_align_batch_async keeps them
+  uint8_t* member_phase = ctx->b_phase.as<uint8_t>();
+  CU(launch_joint_align_init(ao, J, d_init_X, member_phase, ctx->b_dseed.as<uint8_t>(), ctx->corr_seeds && ctx->b_dseed_ok, ctx->stream));
+  ctx->launches += 2;  // the initial state here, the outputs below
+  if (loop) {
+    const auto step = [&](cudaGraphConditionalHandle h) {
+      CU(launch_joint_step(ao, J, L.max_free, true, ctx->b_round.as<BatchRound>(), h, member_phase, ctx->b_out.as<double>(), ctx->stream));
+      return 0;
+    };
+    std::vector<unsigned char> key;
+    if (!capturing) {  // loop_key, plus JointParams (window and edge counts, every buffer), the frame count and max_free (the step's shared memory)
+      key = loop_key(ctx, o);
+      key_add(key, J);
+      for (size_t v : {K, static_cast<size_t>(L.max_free)}) key_add(key, v);
+    }
+    if (int rc = launch_loop(ctx, who, o, capturing, std::move(key), ctx->joint_exec, ctx->joint_key, step)) return rc;
+    ctx->launches += 1;
+    if (int rc = clear_search_counters(ctx)) return rc;
+  }
+  CU(launch_joint_align_finish(J, static_cast<uint32_t>(K), d_init_X, d_out_X, d_out_info, ctx->stream));
+  ctx->b_dseed_ok = true;
+  // Round 1 linearised the edges of every window that started in kPhaseLinearize (one with a free frame and an edge), as sgb_align_joint's
+  // first round does; no other edge was ever linearised.  Their flags are set as linearize_round sets them, the others left as they were.
+  const uint32_t* edge_member = L.edge_member();
+  const uint32_t* edge_win = L.edge_win();
+  bool any = false;
+  for (size_t q = 0; loop && q < E && !any; q++) any = L.n_free[edge_win[q]] > 0;
+  if (any) {
+    if (!ctx->have_lin) std::fill(ctx->b_lin.begin(), ctx->b_lin.end(), 0);
+    if (!ctx->corr_seeds) std::fill(ctx->b_seeded.begin(), ctx->b_seeded.end(), 0);
+    for (size_t q = 0; q < E; q++) {
+      if (!L.n_free[edge_win[q]]) continue;
+      ctx->b_lin[edge_member[q]] = 1;
+      ctx->b_seeded[edge_member[q]] = 1;
+    }
     ctx->have_lin = true;
     ctx->corr_seeds = true;
     ctx->lin_factor = o->factor_kind;

@@ -47,6 +47,12 @@ struct DevBuf {
   }
 };
 
+/// The device side of a joint window align (JointParams in sgb_batch.h): the window / edge tables, the frames' poses, candidates and
+/// steps, the edges' last sums, the windows' WindowState and phase
+struct JointBufs {
+  DevBuf tables, X, cand, delta, sums, state, phase;
+};
+
 /// What the target is.  Points: tgt_orig_* hold n_tgt points in original order, no search structure yet.  Tree: the points are still
 /// resident, and tgt_perm / tgt_pts / tgt_pnodes (+ the grid front end when grid_ready) are their search structure.  VoxelMap: tgt_pts /
 /// tgt_cov* hold n_tgt voxels and vox_table indexes them; tgt_orig_* belong to no one.  VoxelMaps: vm_maps voxel maps for batched calls
@@ -218,9 +224,13 @@ struct sgb_ctx {
   cudaStream_t cap_stream = nullptr;
   cudaGraphExec_t align_exec = nullptr;
   std::vector<unsigned char> align_key;
-  // sgb_align_joint: the call's window / edge tables (JointParams), the frames' poses, candidates and steps, the edges' last sums, the
-  // windows' WindowState and phase
-  sgb::DevBuf j_tables, j_X, j_cand, j_delta, j_sums, j_state, j_phase;
+  // sgb_align_joint: the buffers of its JointParams.  sgb_align_joint_async has its own (joint_async), which no other call writes: its
+  // tables are uploaded only when they differ from ja_tab, the host copy of what joint_async.tables holds.  Its instantiated loop is
+  // cached with its key beside align_exec's.
+  sgb::JointBufs joint, joint_async;
+  std::vector<uint32_t> ja_tab;
+  cudaGraphExec_t joint_exec = nullptr;
+  std::vector<unsigned char> joint_key;
 };
 
 namespace sgb {
