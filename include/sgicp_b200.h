@@ -314,6 +314,29 @@ int sgb_linearize_batch_points(sgb_ctx* ctx, int factor_kind, int robust_kind, d
                                const double* T_colmajor16xB, const uint8_t* active /*or NULL*/, double* out44xB, double* out_point_e /*or NULL*/,
                                double* out_point_Hb42 /*or NULL*/);
 int sgb_error_batch_points(sgb_ctx* ctx, const double* T_colmajor16xB, const uint8_t* active /*or NULL*/, double* out_e, double* out_point_e);
+/* Per-point weights: the caller's weight w_i on every source point's terms in every batched call, e.g. to suppress points of moving
+ * objects flagged by their per-point error, to apply semantic or intensity confidences or overlap masks, or to run IRLS / graduated
+ * non-convexity with a robust kernel of one's own (align, read the rows of sgb_error_batch_points, compute weights, align again).
+ *   - weights: one double per member point in the row layout of sgb_correspondences_batch and the _points calls (member m's rows are its
+ *     offsets' range, in its cloud's original order; pair and submap members in the pairing's member order, so two members of one cloud
+ *     may carry different weights).  The count is the batch's point count.  Host, page-locked or device memory of the context's GPU.
+ *     NULL clears the weights: the batched calls are unweighted again.
+ *   - Meaning: after the factor and the robust kernel, each of a point's terms (H, b and e of a linearize, its error() share) is
+ *     multiplied by w_i, one FP64 multiply per term; the robust weight is still computed from the unweighted residual.  The correspondence
+ *     search, the rejector and num_inliers do not change: a zero-weight point that has a correspondence still counts as an inlier.  The
+ *     rows of the _points calls are the weighted terms, the exact summands of the member sums.  With all weights 1 every result is
+ *     bit-identical to an unweighted call.
+ *   - Honoured by sgb_linearize_batch, sgb_error_batch, both _points calls, sgb_align_batch, sgb_align_batch_async, sgb_align_joint and
+ *     sgb_align_joint_async, against every target kind; not by the single-source calls (sgb_linearize, sgb_error, their _device variants)
+ *     nor the k-NN calls.
+ *   - Every weight must be finite and >= 0 (-0.0 passes).  The weights are gathered into the stored order and checked in 1 launch, and the
+ *     call synchronises once to read the check: a failing weight fails the call with a message naming its row, and the weights in force
+ *     stay.  Fails with a message too without a batch and while the context's stream is being captured.  The batched calls never check
+ *     again, and keep their launch counts.  Weights set again with the same count keep their device address, so a cached or captured
+ *     asynchronous align reads the new ones at its next launch or replay.
+ *   - sgb_source_set_batch, sgb_source_set_pairs, sgb_source_set_submaps and sgb_source_set_points clear the weights; target changes and
+ *     sgb_drop_seeds keep them. */
+int sgb_source_set_weights(sgb_ctx* ctx, const double* weights /*or NULL*/);
 
 /* Batched align(): Registration<Factor, ..., GeneralFactor, Rejector, Optimizer>::align (registration.hpp:17-54, optimizer.hpp:10-158) of
  * every member from its own initial pose, in lockstep.  A round is one sgb_linearize_batch over the members still iterating or, for

@@ -80,6 +80,7 @@ _SIGNATURES = {
     "sgb_source_set_batch": (C.c_int, [_vp, C.c_size_t, C.POINTER(C.c_size_t), _dp, _dp]),
     "sgb_source_set_pairs": (C.c_int, [_vp, C.c_size_t, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32)]),
     "sgb_source_set_submaps": (C.c_int, [_vp, C.c_size_t, C.POINTER(C.c_uint32), C.POINTER(C.c_size_t), C.POINTER(C.c_uint32), _dp]),
+    "sgb_source_set_weights": (C.c_int, [_vp, _dp]),
     "sgb_linearize_batch": (C.c_int, [_vp, C.c_int, C.c_int, C.c_double, C.c_int, C.c_double, _dp, C.POINTER(C.c_uint8), _dp]),
     "sgb_error_batch": (C.c_int, [_vp, _dp, C.POINTER(C.c_uint8), _dp]),
     "sgb_correspondences_batch": (C.c_int, [_vp, _u64p]),
@@ -562,6 +563,30 @@ class Context:
         sizes = np.diff(self._cloud_offsets)
         self._batch_offsets = np.concatenate([[0], np.cumsum(sizes[cl] if cl is not None else sizes)]).astype(np.int64)
 
+    def set_source_weights(self, w):
+        """per-point weights of every batched call (sgb_source_set_weights): w (N,) float64 in the row layout of correspondences_batch
+        (member m's rows are offsets m .. m + 1, in its cloud's original order), a numpy array or a contiguous float64 torch tensor (CUDA on
+        the context's device, or host / page-locked); None clears them.  Each point's H | b | e (and its error() share) is multiplied by its
+        weight after the robust kernel; correspondences and num_inliers do not change.  Every weight must be finite and >= 0, else the call
+        fails naming the row and the weights in force stay.  set_source_batch / _pairs / _submaps / set_source clear the weights."""
+        if w is None:
+            self._check(self._L.sgb_source_set_weights(self._h, None))
+            return
+        offsets = getattr(self, "_batch_offsets", None)
+        n = int(offsets[-1]) if offsets is not None else None
+        if _is_dev(w):
+            import torch
+
+            if w.dtype != torch.float64 or not w.is_contiguous():
+                raise SgbError("set_source_weights: a torch tensor of weights must be contiguous float64")
+            if w.is_cuda and w.device.index != self.device:
+                raise SgbError(f"set_source_weights: the weights are on {w.device}, the context on cuda:{self.device}")
+        else:
+            w = np.ascontiguousarray(w, dtype=np.float64)
+        if n is not None and tuple(w.shape) != (n,):
+            raise SgbError(f"set_source_weights: need ({n},) weights, one per member point in the layout of correspondences_batch; got {tuple(w.shape)}")
+        self._check(self._L.sgb_source_set_weights(self._h, _d(w)))
+
     def _batch_args(self, Ts, active):
         Ts = np.asarray(Ts, dtype=np.float64)
         B = self._batch_offsets.size - 1
@@ -571,7 +596,8 @@ class Context:
         return B, Tc, a, (None if a is None else a.ctypes.data_as(C.POINTER(C.c_uint8)))
 
     def linearize_batch(self, Ts, active=None, factor=FACTOR_GICP, robust=ROBUST_NONE, robust_c=1.0, rejector=REJECT_DISTANCE, max_dist_sq=1.0):
-        """Reduction::linearize of every member at its pose -> (H (B,6,6), b (B,6), e (B,), inliers (B,)); inactive members: zeros"""
+        """Reduction::linearize of every member at its pose -> (H (B,6,6), b (B,6), e (B,), inliers (B,)); inactive members: zeros.  The
+        weights in force (set_source_weights) apply."""
         B, Tc, a, ap = self._batch_args(Ts, active)
         out = np.zeros((max(B, 1), 44))
         self._check(self._L.sgb_linearize_batch(self._h, factor, robust, float(robust_c), rejector, float(max_dist_sq), _d(Tc), ap, _d(out)))
@@ -579,7 +605,7 @@ class Context:
         return out[:, :36].reshape(B, 6, 6).copy(), out[:, 36:42].copy(), out[:, 42].copy(), out[:, 43].astype(np.int64)
 
     def error_batch(self, Ts, active=None):
-        """Reduction::error of every active member at its trial pose (cached correspondences) -> (B,)"""
+        """Reduction::error of every active member at its trial pose (cached correspondences) -> (B,); the weights in force apply"""
         B, Tc, a, ap = self._batch_args(Ts, active)
         out = np.zeros(max(B, 1))
         self._check(self._L.sgb_error_batch(self._h, _d(Tc), ap, _d(out)))
@@ -604,7 +630,8 @@ class Context:
         """linearize_batch plus every source point's terms (sgb_linearize_batch_points) -> BatchPointTerms.  The member sums are
         bit-identical to linearize_batch's.  point_e = the point's w e, point_H / point_b its J^T M J / J^T M r (robust-weighted); zero rows
         for rejected or unmatched points and inactive members.  hessians=False: point_e only (H | b rows not computed).  out_e (N,) and
-        out_Hb42 (N, 42): float64 outputs to write in place (numpy, or CUDA tensors on the context's device, written by the kernel)."""
+        out_Hb42 (N, 42): float64 outputs to write in place (numpy, or CUDA tensors on the context's device, written by the kernel).  With
+        weights in force (set_source_weights) the rows are the weighted terms."""
         B, Tc, a, ap = self._batch_args(Ts, active)
         e_rows = self._rows(out_e, 1, "linearize_batch_points")
         hb_rows = self._rows(out_Hb42, 42, "linearize_batch_points") if hessians else None
@@ -617,7 +644,7 @@ class Context:
 
     def error_batch_points(self, Ts, active=None, out_e=None):
         """error_batch plus every source point's share of its member's e (sgb_error_batch_points) -> (e (B,), point_e (N,)), point_e in the
-        layout of correspondences_batch; out_e as in linearize_batch_points"""
+        layout of correspondences_batch; out_e as in linearize_batch_points; the weights in force apply to both"""
         B, Tc, a, ap = self._batch_args(Ts, active)
         e_rows = self._rows(out_e, 1, "error_batch_points")
         out = np.zeros(max(B, 1))
@@ -635,7 +662,8 @@ class Context:
                     optimizer=OPT_LEVENBERG_MARQUARDT, max_iterations=20, gn_lambda=1e-6, max_inner_iterations=10, init_lambda=1e-3,
                     lambda_factor=10.0, rotation_eps=0.1 * np.pi / 180.0, translation_eps=1e-3, dof_mask=None):
         """Registration<...>::align of every member from its initial pose (sgb_align_batch) -> a Result with per-member arrays
-        T_target_source (B,4,4), converged (B,) bool, iterations (B,), num_inliers (B,), error (B,), H (B,6,6), b (B,6)"""
+        T_target_source (B,4,4), converged (B,) bool, iterations (B,), num_inliers (B,), error (B,), H (B,6,6), b (B,6).  The weights in
+        force (set_source_weights) apply to every round."""
         B, Tc, _, _ = self._batch_args(init_Ts, None)
         o = AlignOptions(int(factor), int(robust), float(robust_c), int(rejector), float(max_dist_sq), int(optimizer), int(max_iterations), float(gn_lambda),
                          int(max_inner_iterations), float(init_lambda), float(lambda_factor), float(rotation_eps), float(translation_eps))
@@ -653,7 +681,7 @@ class Context:
         of the many-maps target; the edges are the members of set_source_pairs(clouds, maps), edge p = cloud clouds[p] against map maps[p] at
         X_j^-1 X_i.  init_X (K,4,4) row-major frame poses; windows: the window offsets (W + 1,) from 0 to K (None: one window of all
         frames); fixed (K,) flags of frames held at their initial pose (None: the first frame of each window); the other keywords as in
-        align_batch."""
+        align_batch.  The weights in force (set_source_weights, one per edge point) apply."""
         X = np.asarray(init_X, dtype=np.float64)
         K = self._cloud_offsets.size - 1 if hasattr(self, "_cloud_offsets") else 0
         if X.shape != (K, 4, 4):
@@ -682,7 +710,7 @@ class Context:
         (B, 4, 4) row-major, on the context's device; the context's stream must have been set (set_stream) to a torch stream, on which the
         poses are transposed into the library's column-major layout.  Returns an AsyncAlignResult of CUDA tensors (out: a previous result
         whose buffers are reused).  Inside torch.cuda.graph (with the capture stream set) the align is captured: each replay re-runs it
-        from what init_Ts holds then."""
+        from what init_Ts holds then, with the weights in force then (set_source_weights)."""
         import torch
 
         if self._stream is None:
@@ -714,7 +742,8 @@ class Context:
         """align_joint enqueued on the context's stream without a host synchronisation (sgb_align_joint_async).  init_X: CUDA float64 (K, 4, 4)
         row-major frame poses on the context's device, transposed on the context's stream (set_stream: a torch stream); windows, fixed and the
         other keywords as in align_joint.  Returns an AsyncJointAlignResult of CUDA tensors (out: a previous result whose buffers are reused).
-        Inside torch.cuda.graph (with the capture stream set) the align is captured: each replay re-runs it from what init_X holds then."""
+        Inside torch.cuda.graph (with the capture stream set) the align is captured: each replay re-runs it from what init_X holds then.
+        The weights in force (set_source_weights) apply, at a replay those in force then."""
         import torch
 
         if self._stream is None:

@@ -8,7 +8,9 @@
 //                           kd-trees with member m centred on map m), the voxel-map probe for VGICP (vox_nearest, as in
 //                           linearize_vox_kernel; many voxel maps: member m in map m's centre and table region), or submap members, each
 //                           point at the member's pose relative to the placement of the entry its correspondence lies in; for the
-//                           _points calls also each point's row of terms (BatchRows)
+//                           _points calls also each point's row of terms (BatchRows), and with weights in force each point's terms
+//                           times its weight
+//   weight_gather_kernel    sgb_source_set_weights: the caller's per-point weights into stored order, each checked finite and >= 0
 //   batch_segment_kernel    one CTA per member: its tiles' partials in tile order -> H|b|e|inliers (or e) of that member
 //   batch_step_kernel       batched align(): one thread per member, its Gauss-Newton / Levenberg-Marquardt step (sgb_math.cuh) after a
 //                           round, its next pose and phase
@@ -106,7 +108,9 @@ __global__ void __launch_bounds__(kLinBlock) batch_transform_kernel(const __grid
 // the right perturbation of the pose are invariant under the placement, so this IS the point's share of the sums against the union.
 // POINTS: the point's row too (rows).  A thread takes one point of the tile, so its acc is 0 + that point's terms: the very summands of
 // the tile sum, written before it, whatever the kind (factor_terms_source or accumulate_factor); zeros where the point has no term.
-template <int FACTOR, int ROBUST, bool VOX, bool ERR, bool MAPS, bool SUB = false, bool POINTS = false>
+// WEIGHTED: the point's terms (H | b | e, or its error()) times its weight rows->w[i] (sgb_source_set_weights), after the robust kernel and
+// before its row and the tile sum; the inlier count stays as it is.
+template <int FACTOR, int ROBUST, bool VOX, bool ERR, bool MAPS, bool SUB = false, bool POINTS = false, bool WEIGHTED = false>
 __device__ __forceinline__ void batch_factor_tile(const BatchParams& B, const uint32_t* __restrict__ vcorr, const double* __restrict__ map_centres,
                                                   const uint4* __restrict__ map_regions, const SubmapView* S = nullptr, const BatchRows* rows = nullptr) {
   constexpr int NACC = ERR ? 1 : kAcc + 1;
@@ -193,8 +197,13 @@ __device__ __forceinline__ void batch_factor_tile(const BatchParams& B, const ui
       }
       B.corr[i] = best;
     }
+    if constexpr (WEIGHTED) {
+      const double w = __ldg(&rows->w[i]);
+#pragma unroll
+      for (int k = 0; k < (ERR ? 1 : kAcc); k++) acc[k] *= w;
+    }
     if constexpr (POINTS) {
-      const size_t row = static_cast<size_t>(__ldg(&rows->member_off[t.member])) + __ldg(&rows->perm[i]);
+      const size_t row = batch_row(rows->member_off, rows->perm, t.member, i);
       if constexpr (ERR) {
         rows->e[row] = acc[0];
       } else {
@@ -218,8 +227,9 @@ __device__ __forceinline__ void batch_factor_tile(const BatchParams& B, const ui
 // One CTA per tile of one member, for the target's KIND: 0 one point target, 1 one voxel map, 2 many voxel maps (member m against map m:
 // map_centres and map_regions), 3 many kd-trees (map_centres; vcorr = what forest_search_kernel found in map m), 4 submaps (S; vcorr and
 // S.centry = what forest_search_kernel<SUBMAP> found over the member's entries).  MODE: linearize, error() with the cached correspondences, or
-// either as the round's planner decided.  POINTS (host-planned modes only): every processed point's row to `rows` too.
-template <int FACTOR, int ROBUST, int KIND, int MODE, bool POINTS = false>
+// either as the round's planner decided.  POINTS (host-planned modes only): every processed point's row to `rows` too.  WEIGHTED (any
+// mode): each point's terms times its weight rows.w[i].
+template <int FACTOR, int ROBUST, int KIND, int MODE, bool POINTS = false, bool WEIGHTED = false>
 __global__ void __launch_bounds__(kLinBlock, 4) batch_factor_kernel(const __grid_constant__ BatchParams B, const uint32_t* __restrict__ vcorr,
                                                                    const double* __restrict__ map_centres, const uint4* __restrict__ map_regions,
                                                                    const __grid_constant__ SubmapView S, const BatchRound* __restrict__ round,
@@ -232,9 +242,9 @@ __global__ void __launch_bounds__(kLinBlock, 4) batch_factor_kernel(const __grid
     lin = r.lin;
   }
   if (lin)
-    batch_factor_tile<FACTOR, ROBUST, VOX, false, MAPS, SUB, POINTS>(B, vcorr, map_centres, map_regions, &S, &rows);
+    batch_factor_tile<FACTOR, ROBUST, VOX, false, MAPS, SUB, POINTS, WEIGHTED>(B, vcorr, map_centres, map_regions, &S, &rows);
   else
-    batch_factor_tile<FACTOR, ROBUST, VOX, true, MAPS, SUB, POINTS>(B, nullptr, map_centres, map_regions, &S, &rows);
+    batch_factor_tile<FACTOR, ROBUST, VOX, true, MAPS, SUB, POINTS, WEIGHTED>(B, nullptr, map_centres, map_regions, &S, &rows);
 }
 
 // One CTA per member: warp w adds tiles w, w + 8, ... of the member in order, then the 8 warp sums are added in warp order.  The order
@@ -439,29 +449,57 @@ cudaError_t launch_batch_transform(const BatchParams& B, const BatchRound* round
 // The factor kernel of one kind in one mode.  The kinds without point-to-plane (1, 2, 4: refused by the caller) compile FACTOR 1 as 0, one
 // instantiation fewer each.  error() reads the cached correspondences only, so the voxel kinds compute what the kinds with the same
 // centres compute there (1 -> 0, 2 -> 3).
-template <int F, int R, int MODE, bool POINTS = false>
+template <int F, int R, int MODE, bool POINTS = false, bool WEIGHTED = false>
 auto factor_kernel(int kind) -> decltype(&batch_factor_kernel<0, 0, 0, kModeLinearize>) {
   constexpr int G = F == 1 ? 0 : F;
   switch (kind) {
-    case 0: return batch_factor_kernel<F, R, 0, MODE, POINTS>;
-    case 1: if constexpr (MODE == kModeError) return batch_factor_kernel<G, R, 0, MODE, POINTS>; else return batch_factor_kernel<G, R, 1, MODE, POINTS>;
-    case 2: if constexpr (MODE == kModeError) return batch_factor_kernel<G, R, 3, MODE, POINTS>; else return batch_factor_kernel<G, R, 2, MODE, POINTS>;
-    case 3: return batch_factor_kernel<F, R, 3, MODE, POINTS>;
-    case 4: return batch_factor_kernel<G, R, 4, MODE, POINTS>;
+    case 0: return batch_factor_kernel<F, R, 0, MODE, POINTS, WEIGHTED>;
+    case 1: if constexpr (MODE == kModeError) return batch_factor_kernel<G, R, 0, MODE, POINTS, WEIGHTED>; else return batch_factor_kernel<G, R, 1, MODE, POINTS, WEIGHTED>;
+    case 2: if constexpr (MODE == kModeError) return batch_factor_kernel<G, R, 3, MODE, POINTS, WEIGHTED>; else return batch_factor_kernel<G, R, 2, MODE, POINTS, WEIGHTED>;
+    case 3: return batch_factor_kernel<F, R, 3, MODE, POINTS, WEIGHTED>;
+    case 4: return batch_factor_kernel<G, R, 4, MODE, POINTS, WEIGHTED>;
     default: return nullptr;
   }
 }
 
+// the factor kernel of one kind for a round (device-planned), or for a host-planned mode with or without rows
+template <int F, int R, bool WEIGHTED>
+auto factor_kernel(int kind, bool err, bool round, bool rows) -> decltype(&batch_factor_kernel<0, 0, 0, kModeLinearize>) {
+  if (rows) return err ? factor_kernel<F, R, kModeError, true, WEIGHTED>(kind) : factor_kernel<F, R, kModeLinearize, true, WEIGHTED>(kind);
+  return round ? factor_kernel<F, R, kModeRound, false, WEIGHTED>(kind) : err ? factor_kernel<F, R, kModeError, false, WEIGHTED>(kind)
+                                                                               : factor_kernel<F, R, kModeLinearize, false, WEIGHTED>(kind);
+}
+
 cudaError_t launch_batch_factor(const BatchParams& B, int kind, int factor, int robust, bool err, const BatchRound* round, uint32_t n_tiles, const uint32_t* vcorr,
-                                const double* map_centres, const uint4* map_regions, const SubmapView& S, const BatchRows* rows, cudaStream_t st) {
+                                const double* map_centres, const uint4* map_regions, const SubmapView& S, const BatchRows* rows, const double* weights,
+                                cudaStream_t st) {
   if (factor == 1 && (kind == 1 || kind == 2 || kind == 4)) return cudaErrorInvalidValue;  // no normals in a voxel map; no point-to-plane against a union
   if (round && rows) return cudaErrorInvalidValue;
   const auto kernel = dispatch_factor_robust(factor, robust, decltype(&batch_factor_kernel<0, 0, 0, kModeLinearize>){}, [&](auto f, auto r) {
-    if (rows) return err ? factor_kernel<f, r, kModeError, true>(kind) : factor_kernel<f, r, kModeLinearize, true>(kind);
-    return round ? factor_kernel<f, r, kModeRound>(kind) : err ? factor_kernel<f, r, kModeError>(kind) : factor_kernel<f, r, kModeLinearize>(kind);
+    return weights ? factor_kernel<f, r, true>(kind, err, round, rows) : factor_kernel<f, r, false>(kind, err, round, rows);
   });
   if (!kernel) return cudaErrorInvalidValue;
-  kernel<<<n_tiles, kLinBlock, 0, st>>>(B, vcorr, map_centres, map_regions, S, round, rows ? *rows : BatchRows{});
+  BatchRows R = rows ? *rows : BatchRows{};
+  R.w = weights;
+  kernel<<<n_tiles, kLinBlock, 0, st>>>(B, vcorr, map_centres, map_regions, S, round, R);
+  return cudaGetLastError();
+}
+
+// One thread per stored point: its weight fetched from the caller's row (batch_row, as the POINTS row write) and checked
+__global__ void weight_gather_kernel(const WeightGather g) {
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < g.n; i += gridDim.x * blockDim.x) {
+    const uint32_t m = owner_of(g.member_off, g.n_members, i);
+    const size_t row = batch_row(g.member_off, g.perm, m, i);
+    const double w = g.src[row];
+    g.dst[i] = w;
+    if (!(w >= 0.0 && w <= DBL_MAX)) atomicMin(g.bad, static_cast<uint32_t>(row));  // NaN, negative or infinite (-0.0 passes)
+  }
+}
+
+cudaError_t launch_weight_gather(const WeightGather& g, int sm_count, cudaStream_t st) {
+  if (g.n == 0) return cudaSuccess;
+  const uint32_t grid = std::min<uint32_t>((g.n + 255u) / 256u, static_cast<uint32_t>(sm_count) * 8u);
+  weight_gather_kernel<<<grid, 256, 0, st>>>(g);
   return cudaGetLastError();
 }
 

@@ -33,15 +33,31 @@ struct BatchParams {
 };
 
 /// Per-point rows of sgb_linearize_batch_points / sgb_error_batch_points, written by the factor kernel beside its sums: stored point i of
-/// member m writes row member_off[m] + perm[i], the caller's order of sgb_correspondences_batch.  e: [points] the point's share of the
-/// member's e (or null); Hb: [points][42] its H (36, row-major) | b (6) (or null; linearize only).  Kept out of BatchParams, which keys
-/// the cached graph of sgb_align_batch_async.
+/// member m writes row batch_row(member_off, perm, m, i), the caller's order of sgb_correspondences_batch.  e: [points] the point's share
+/// of the member's e (or null); Hb: [points][42] its H (36, row-major) | b (6) (or null; linearize only).  w: the weights in force
+/// (sgb_source_set_weights), [points] in stored order, read by the weighted instantiations only (any mode, the rows' fields unused
+/// without POINTS).  Kept out of BatchParams, which keys the cached graph of sgb_align_batch_async.
 struct BatchRows {
   const uint32_t* perm;        // stored position -> original index within the member's cloud
   const uint32_t* member_off;  // [members + 1]
   double* e;
   double* Hb;
+  const double* w;
 };
+/// the caller's row of stored point i of member m: the member's first row plus the point's original index within its cloud
+__device__ __forceinline__ size_t batch_row(const uint32_t* __restrict__ member_off, const uint32_t* __restrict__ perm, uint32_t m, uint32_t i) {
+  return static_cast<size_t>(__ldg(&member_off[m])) + __ldg(&perm[i]);
+}
+/// sgb_source_set_weights: the caller's weights (src, row layout) gathered into stored order (dst), n stored points of n_members members
+/// (member_off / perm as BatchRows); the first row whose weight is not finite and >= 0 goes to *bad (atomicMin; ~0u: none)
+struct WeightGather {
+  uint32_t n, n_members;
+  const uint32_t *member_off, *perm;
+  const double* src;
+  double* dst;
+  uint32_t* bad;
+};
+cudaError_t launch_weight_gather(const WeightGather& g, int sm_count, cudaStream_t st);
 
 /// Members as (cloud, map) pairs (sgb_source_set_pairs): member p = a replica of stored cloud clouds[p], at member_off[p] .. member_off[p+1]
 /// of the member buffers; its centre and bounds too.  covA = null: no covariances.
@@ -129,8 +145,10 @@ cudaError_t launch_batch_unmatch(const BatchParams& B, const BatchRound* round, 
 /// first voxel, voxel count) of each map), 3 many kd-trees (map_centres; vcorr = the forest search's result), 4 submaps (S; vcorr = the
 /// submap search's result).  Linearize (err = false), error() with the cached correspondences (err = true), or with a round what it
 /// says.  Point-to-plane only for kinds 0 and 3.  rows (rounds planned on the host only; null: none): every processed point's row too.
+/// weights (null: none): each point's terms scaled by its weight (stored order) before its row and the sums.
 cudaError_t launch_batch_factor(const BatchParams& B, int kind, int factor, int robust, bool err, const BatchRound* round, uint32_t n_tiles, const uint32_t* vcorr,
-                                const double* map_centres, const uint4* map_regions, const SubmapView& S, const BatchRows* rows, cudaStream_t st);
+                                const double* map_centres, const uint4* map_regions, const SubmapView& S, const BatchRows* rows, const double* weights,
+                                cudaStream_t st);
 /// out: [members][44] (linearize) or [members] (error)
 cudaError_t launch_batch_segment(const BatchParams& B, uint32_t n_members, bool linearize, const BatchRound* round, double* out, cudaStream_t st);
 /// batched align(): every member whose phase matches the round (linearize: kPhaseLinearize, else kPhaseTrial) takes its optimiser step

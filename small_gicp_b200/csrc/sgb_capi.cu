@@ -198,6 +198,7 @@ void sgb::begin_source(sgb_ctx* ctx, SourceState state, size_t n, bool covs) {
   ctx->src_has_lo = ctx->src_tree_valid = ctx->src_cov_orig_valid = false;
   ctx->b_paired = ctx->b_pair_has_maps = ctx->b_submaps = false;
   ctx->b_pair_maps.clear();
+  ctx->b_weighted = false;  // the weights belonged to the rows of the old members
   forget_linearisation(ctx);
 }
 
@@ -205,6 +206,7 @@ void sgb::begin_pairs(sgb_ctx* ctx) {
   ctx->b_paired = true;
   ctx->b_pair_has_maps = ctx->b_submaps = false;
   ctx->b_pair_maps.clear();
+  ctx->b_weighted = false;
   forget_linearisation(ctx);
 }
 

@@ -1,6 +1,6 @@
 // SPDX-License-Identifier: MIT
 // C-ABI of batched registration (include/sgicp_b200.h: sgb_source_set_batch, sgb_source_set_pairs, sgb_source_set_submaps,
-// sgb_{linearize,error,align,correspondences}_batch, sgb_{linearize,error}_batch_points, sgb_align_batch_async, sgb_align_joint,
+// sgb_source_set_weights, sgb_{linearize,error,align,correspondences}_batch, sgb_{linearize,error}_batch_points, sgb_align_batch_async, sgb_align_joint,
 // sgb_align_joint_async).
 // Kernels in sgb_batch.cu (many kd-trees and submaps: the searches in sgb_forest.cu); DESIGN.md §11.
 #include <cuda_runtime.h>
@@ -8,6 +8,7 @@
 #include <algorithm>
 #include <cfloat>
 #include <cmath>
+#include <cstdio>
 #include <cstring>
 #include <string>
 #include <vector>
@@ -270,7 +271,8 @@ int round_kernels(sgb_ctx* ctx, const LinParams& P, const BatchParams& Bp, const
     if (int rc = round ? point_search_round(ctx, Q, &round->n_search, depth) : launch_point_search(ctx, Q, depth)) return rc;
     ctx->launches += counted;
   }
-  CU(launch_batch_factor(Bp, kind, factor, robust, err, round, n_tiles, err ? nullptr : vcorr, centres, regions, S, rows, ctx->stream));
+  const double* weights = ctx->b_weighted ? ctx->b_weights.as<double>() : nullptr;  // (sgb_source_set_weights)
+  CU(launch_batch_factor(Bp, kind, factor, robust, err, round, n_tiles, err ? nullptr : vcorr, centres, regions, S, rows, weights, ctx->stream));
   ctx->launches += counted;
   return 0;
 }
@@ -602,6 +604,9 @@ std::vector<unsigned char> loop_key(sgb_ctx* ctx, const sgb_align_options* o) {
                           &ctx->tgt_pnodes, &ctx->kt_tables, &ctx->kt_centres, &ctx->vm_centres, &ctx->vm_regions, &ctx->v_tables, &ctx->v_centres,
                           &ctx->v_regions, &ctx->s_tables, &ctx->s_entries, &ctx->s_centres, &ctx->b_centry})
     key_add(k, b->p);
+  // the weighted factor kernel and the address it reads: a replay reads whatever weights are in force there
+  key_add(k, static_cast<int>(ctx->b_weighted));
+  key_add(k, ctx->b_weights.p);
   return k;
 }
 
@@ -648,14 +653,19 @@ int align_checks(sgb_ctx* ctx, const char* who, const sgb_align_options* o, cons
 
 // ---- sgb_linearize_batch_points / sgb_error_batch_points (DESIGN.md §11 "Per-point terms") ----
 
+// the tables that map a stored point to the caller's row (batch_row): the pairing's member offsets and replicas' order, else the clouds'
+void row_layout(const sgb_ctx* ctx, const uint32_t*& member_off, const uint32_t*& perm) {
+  member_off = (ctx->b_paired ? ctx->p_tables : ctx->b_cloud_off).as<uint32_t>();
+  perm = (ctx->b_paired ? ctx->p_perm : ctx->src_perm).as<uint32_t>();
+}
+
 // Where the factor kernel writes the rows of one call: the caller's buffers when they are device memory of the context's GPU, else the
 // context's staging buffers (copy_rows copies them out).  The rows the kernel does not reach -- every point of an inactive member, and of
 // every member against an empty target -- are cleared here; rejected and unmatched points get zero rows from the kernel itself.
 int point_rows(sgb_ctx* ctx, const uint8_t* active, double* out_e, double* out_Hb, BatchRows& rows) {
   const size_t B = batch_members(ctx), nn = std::max<size_t>(batch_points(ctx), 1);
-  rows.perm = (ctx->b_paired ? ctx->p_perm : ctx->src_perm).as<uint32_t>();
-  rows.member_off = (ctx->b_paired ? ctx->p_tables : ctx->b_cloud_off).as<uint32_t>();
-  rows.e = rows.Hb = nullptr;
+  rows = BatchRows{};
+  row_layout(ctx, rows.member_off, rows.perm);
   if (out_e && on_device(ctx, out_e)) {
     rows.e = out_e;
   } else if (out_e) {
@@ -887,6 +897,62 @@ int sgb_source_set_submaps(sgb_ctx* ctx, size_t n_members, const uint32_t* cloud
   CU(ctx->b_centry.reserve(std::max<size_t>(batch_points(ctx), 1) * sizeof(uint32_t)));
   // pageable host memory: the copy is staged before cudaMemcpyAsync returns
   CU(cudaMemcpyAsync(ctx->s_tables.p, tables.data(), tables.size() * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
+  return 0;
+}
+
+int sgb_source_set_weights(sgb_ctx* ctx, const double* weights) {
+  if (!ctx) return 1;
+  const std::string who = "sgb_source_set_weights";
+  if (ctx->src_state != SourceState::Batch) return fail(ctx, 1, who + ": the context holds no batch of sources (call sgb_source_set_batch)");
+  if (!weights) {
+    ctx->b_weighted = false;
+    return 0;
+  }
+  CU(cudaSetDevice(ctx->device));
+  cudaStreamCaptureStatus capture = cudaStreamCaptureStatusNone;
+  CU(cudaStreamIsCapturing(ctx->stream, &capture));
+  if (capture != cudaStreamCaptureStatusNone)
+    return fail(ctx, 1, who + ": the context's stream is being captured, and the call synchronises to check the weights; set them outside the capture "
+                              "(a replay reads the weights in force)");
+  const size_t n = batch_points(ctx);
+  if (n == 0) {
+    ctx->b_weighted = true;
+    return 0;
+  }
+  // Gathered into stored order and checked in one launch, into b_wnext: the weights in force stay until every new one has passed.  The
+  // weights in force always have the batch's count, so b_weights never reallocates here while they are.
+  const double* src = weights;
+  if (!on_device(ctx, weights)) {  // host or page-locked memory: one copy to the device first (b_rows_e: scratch of the _points calls)
+    CU(ctx->b_rows_e.reserve(n * sizeof(double)));
+    CU(cudaMemcpyAsync(ctx->b_rows_e.p, weights, n * sizeof(double), cudaMemcpyDefault, ctx->stream));
+    src = ctx->b_rows_e.as<double>();
+  }
+  CU(ctx->b_wnext.reserve(n * sizeof(double)));
+  CU(ctx->b_wbad.reserve(sizeof(uint32_t)));
+  CU(cudaMemsetAsync(ctx->b_wbad.p, 0xFF, sizeof(uint32_t), ctx->stream));
+  WeightGather g = {};
+  g.n = static_cast<uint32_t>(n);
+  g.n_members = static_cast<uint32_t>(batch_members(ctx));
+  row_layout(ctx, g.member_off, g.perm);
+  g.src = src;
+  g.dst = ctx->b_wnext.as<double>();
+  g.bad = ctx->b_wbad.as<uint32_t>();
+  CU(launch_weight_gather(g, ctx->sm_count, ctx->stream));
+  ctx->launches += 1;
+  uint32_t bad = ~0u;
+  CU(cudaMemcpyAsync(&bad, ctx->b_wbad.p, sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));
+  if (bad != ~0u) {
+    double v = 0.0;
+    CU(cudaMemcpy(&v, weights + bad, sizeof(double), cudaMemcpyDefault));
+    char val[32];
+    std::snprintf(val, sizeof(val), "%g", v);
+    return fail(ctx, 1, who + ": the weight of row " + std::to_string(bad) + " is " + val + "; every weight must be finite and >= 0 (the weights in force "
+                                  "are unchanged)");
+  }
+  CU(ctx->b_weights.reserve(n * sizeof(double)));
+  CU(cudaMemcpyAsync(ctx->b_weights.p, ctx->b_wnext.p, n * sizeof(double), cudaMemcpyDeviceToDevice, ctx->stream));
+  ctx->b_weighted = true;
   return 0;
 }
 int sgb_linearize_batch(sgb_ctx* ctx, int factor, int robust, double robust_c, int rejector, double max_dist_sq, const double* T, const uint8_t* active,

@@ -195,6 +195,11 @@ struct sgb_ctx {
   sgb::DevBuf b_partials, b_out;           // per-tile partial sums, per-member results
   sgb::DevBuf b_state, b_phase;            // sgb_align_batch: per member MemberState / next round (kPhase*, one byte)
   sgb::DevBuf b_rows_e, b_rows_hb;         // sgb_*_batch_points: the per-point rows staged for outputs that are not device memory
+  // sgb_source_set_weights: b_weighted = the batched calls scale each point's terms by b_weights (per stored point, stored order, every
+  // one checked finite and >= 0); b_wnext / b_wbad = the gather's output and its first offending row, before the check lets it in force.
+  // The source setters and pairings clear b_weighted (begin_source, begin_pairs); the buffer keeps its address while the count does.
+  bool b_weighted = false;
+  sgb::DevBuf b_weights, b_wnext, b_wbad;
   // The clouds of sgb_source_set_batch are stored once (src_* and b_centres / b_bounds, cloud after cloud).  Without a pairing the
   // members are those clouds.  After sgb_source_set_pairs (b_paired) member p is a replica of one stored cloud in p_*, b_offsets are
   // the members' offsets, and b_pair_maps (empty: member m against map m) names each member's map.
