@@ -363,6 +363,45 @@ typedef struct sgb_align_options {
  * out_Hb42xB (or NULL) = H(36) | b(6) per member (RegistrationResult).  max_iterations <= 0 returns the initial poses, not converged. */
 int sgb_align_batch(sgb_ctx* ctx, const sgb_align_options* options, const double* init_T16xB, double* out_T16xB, double* out_info4xB,
                     double* out_Hb42xB /*or NULL*/);
+/* Graduated non-convexity (GNC; Yang, Antonante, Tzoumas, Carlone, RA-L 2020): outlier-robust batched align, for moving objects, partial
+ * overlap, clutter or wrong loop-closure candidates, where a fixed-width robust kernel breaks down.  Each member alternates a weighted
+ * sgb_align_batch with a closed-form update of its per-point weights, annealing a surrogate of the Geman-McClure or truncated-least-squares
+ * cost from convex to the true cost; the weights stay on the device.  Per member, stage s (s = 0, 1, ...) from its current pose T_s (T_0 =
+ * its initial pose):
+ *   1. Reweighting linearize: one unweighted linearize at T_s with the options' factor and rejector and no robust kernel.  A point with a
+ *      correspondence has r_i^2 = 2 e_i (e_i: its row of sgb_linearize_batch_points without weights; c^2 is on this scale: ICP m^2, GICP
+ *      Mahalanobis); a point without one gets g_i = 0 for the stage.
+ *   2. Stage 0: r_max^2 = the member's largest r_i^2 (0 without any).  GM: mu = 2 r_max^2 / c^2, or 1 if that is <= 1.  TLS: if
+ *      2 r_max^2 <= c^2 the member has no outliers: every point with a correspondence gets g_i = 1, this stage is its last, and its mu is
+ *      reported as 0; else mu = c^2 / (2 r_max^2 - c^2).  Later stages: GM mu = max(mu / 1.4, 1), TLS mu = 1.4 mu.
+ *   3. Weights: GM g = (mu c^2 / (r^2 + mu c^2))^2; TLS g = 1 if r^2 <= mu / (mu + 1) c^2, 0 if r^2 >= (mu + 1) / mu c^2, else
+ *      c / r sqrt(mu (mu + 1)) - mu (clamped to [0, 1]).  The stage's align uses w_i g_i, w_i = the weight in force (1 without).  Every
+ *      formula is FP64 with a fixed operation order and no contraction (sgb_math.cuh): numpy reproduces every bit.
+ *   4. The stage is the member's last when GM's mu is 1, when TLS's weights are all binary (every g in {0, 1}), or at s = max_stages - 1.
+ *   5. Weighted align: sgb_align_batch's algorithm from T_s (a fresh start, the options as given) with the stage's weights and max_iterations
+ *      = stage_iterations, or options->max_iterations at the last stage; its result is T_{s+1}.
+ * Outputs (host memory; out_point_w may also be device memory of the context's GPU): T, H | b and info of the last stage's align (converged,
+ * iterations summed over all stages, inliers and the weighted error), out_gnc2xB = the stages run and the last stage's mu, out_point_w =
+ * each point's final g (without the weights in force) in the row layout of sgb_correspondences_batch.  Each member's results are
+ * bit-identical to this loop driven from the host on a context holding that member alone: sgb_source_set_weights(NULL),
+ * sgb_linearize_batch_points, the formulas, sgb_source_set_weights(w * g), sgb_align_batch (the exact-FP32-tie caveat above applies).
+ * Afterwards the context is as sgb_align_batch leaves it after each member's last stage (sgb_correspondences_batch, sgb_error_batch), and
+ * the weights in force are unchanged: the stage weights live in a buffer of the call.
+ * Launches per stage: the reweighting linearize round (its search launches, the factor kernel, the segment kernel), 1 for the largest
+ * residual (stage 0 only), 3 (mu and last stage, weights, align_init), then the align's rounds as in sgb_align_batch, each ending with one
+ * step launch.  The host reads one byte per member per round, and one more per member per stage ("still in GNC").
+ * Fails with a message, enqueuing nothing, for robust_kind != SGB_ROBUST_NONE (the GNC weights are the robust kernel), an invalid kind,
+ * noise_bound_sq not finite or <= 0, max_stages < 1, stage_iterations < 1, while the context's stream is being captured (the call
+ * synchronises), and for everything sgb_align_batch refuses. */
+enum sgb_gnc_kind { SGB_GNC_GEMAN_MCCLURE = 0, SGB_GNC_TLS = 1 };
+typedef struct sgb_gnc_options {
+  int kind;               /* sgb_gnc_kind */
+  double noise_bound_sq;  /* c^2, on the factor's own r^2 = 2 e scale (ICP: m^2; GICP: Mahalanobis) */
+  int max_stages;         /* hard bound on the stage count, >= 1 */
+  int stage_iterations;   /* max_iterations of every stage but the last (>= 1); the last uses options->max_iterations */
+} sgb_gnc_options;
+int sgb_align_batch_gnc(sgb_ctx* ctx, const sgb_align_options* options, const sgb_gnc_options* gnc, const double* init_T16xB, double* out_T16xB,
+                        double* out_info4xB, double* out_Hb42xB /*or NULL*/, double* out_gnc2xB /*or NULL*/, double* out_point_w /*or NULL*/);
 /* Joint window registration: every frame pose of a window of scans solved against all the window's pairwise edges at once, many windows
  * per call.  Frame k is cloud k of the last sgb_source_set_batch with map k of a many-kd-trees or many-voxel-maps target, both in frame k's
  * own coordinates (cloud count == map count).  The edges are the members of the pairing of sgb_source_set_pairs with a maps table: member

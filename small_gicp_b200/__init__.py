@@ -15,6 +15,8 @@ from .capi import (  # noqa: F401
     REJECT_NONE,
     REJECT_DISTANCE,
     NO_CORRESPONDENCE,
+    GNC_GEMAN_MCCLURE,
+    GNC_TLS,
     library_path,
     exported_symbols,
 )

@@ -12,6 +12,7 @@ FACTOR_ICP, FACTOR_PLANE_ICP, FACTOR_GICP = 0, 1, 2
 ROBUST_NONE, ROBUST_HUBER, ROBUST_CAUCHY = 0, 1, 2
 REJECT_NONE, REJECT_DISTANCE = 0, 1
 OPT_GAUSS_NEWTON, OPT_LEVENBERG_MARQUARDT = 0, 1
+GNC_GEMAN_MCCLURE, GNC_TLS = 0, 1
 NO_CORRESPONDENCE = np.uint64(0xFFFFFFFFFFFFFFFF)
 
 _dp = C.POINTER(C.c_double)
@@ -39,6 +40,22 @@ class AlignOptions(C.Structure):
         ("translation_eps", C.c_double),
         ("dof_mask", C.c_double * 6),
     ]
+
+
+def _align_options(factor=FACTOR_GICP, robust=ROBUST_NONE, robust_c=1.0, rejector=REJECT_DISTANCE, max_dist_sq=1.0, optimizer=OPT_LEVENBERG_MARQUARDT,
+                   max_iterations=20, gn_lambda=1e-6, max_inner_iterations=10, init_lambda=1e-3, lambda_factor=10.0, rotation_eps=0.1 * np.pi / 180.0,
+                   translation_eps=1e-3, dof_mask=None):
+    """the sgb_align_options of the align_batch keywords"""
+    o = AlignOptions(int(factor), int(robust), float(robust_c), int(rejector), float(max_dist_sq), int(optimizer), int(max_iterations), float(gn_lambda),
+                     int(max_inner_iterations), float(init_lambda), float(lambda_factor), float(rotation_eps), float(translation_eps))
+    o.dof_mask[:] = [1.0] * 6 if dof_mask is None else [float(x) for x in dof_mask]
+    return o
+
+
+class GncOptions(C.Structure):
+    """sgb_gnc_options"""
+
+    _fields_ = [("kind", C.c_int), ("noise_bound_sq", C.c_double), ("max_stages", C.c_int), ("stage_iterations", C.c_int)]
 
 # name -> (restype, argtypes): every symbol include/sgicp_b200.h declares
 _SIGNATURES = {
@@ -88,6 +105,7 @@ _SIGNATURES = {
     "sgb_error_batch_points": (C.c_int, [_vp, _dp, C.POINTER(C.c_uint8), _dp, _dp]),
     "sgb_align_batch": (C.c_int, [_vp, C.POINTER(AlignOptions), _dp, _dp, _dp, _dp]),
     "sgb_align_batch_async": (C.c_int, [_vp, C.POINTER(AlignOptions), _dp, _dp, _dp, _dp]),
+    "sgb_align_batch_gnc": (C.c_int, [_vp, C.POINTER(AlignOptions), C.POINTER(GncOptions), _dp, _dp, _dp, _dp, _dp, _dp]),
     "sgb_align_joint": (C.c_int, [_vp, C.POINTER(AlignOptions), C.c_size_t, C.POINTER(C.c_size_t), C.POINTER(C.c_uint8), _dp, _dp, _dp]),
     "sgb_align_joint_async": (C.c_int, [_vp, C.POINTER(AlignOptions), C.c_size_t, C.POINTER(C.c_size_t), C.POINTER(C.c_uint8), _dp, _dp, _dp]),
     "sgb_estimate_features": (C.c_int, [_vp, C.c_size_t, _dp, C.c_int, _dp, _dp]),
@@ -116,6 +134,18 @@ class BatchAlignResult:
         self.error = info4[:, 3].copy()
         self.H = np.ascontiguousarray(Hb42[:, :36].reshape(B, 6, 6).transpose(0, 2, 1))
         self.b = Hb42[:, 36:42].copy()
+
+
+class GncAlignResult(BatchAlignResult):
+    """what Context.align_batch_gnc returns: the BatchAlignResult fields of each member's last stage (iterations summed over its stages),
+    stages (B,) the stages it ran, mu (B,) the surrogate's shape at its last stage (TLS without outliers: 0), and point_w (N,) each point's
+    final GNC weight g in the layout of correspondences_batch (None unless requested)"""
+
+    def __init__(self, T16, info4, Hb42, gnc2, point_w):
+        super().__init__(T16, info4, Hb42)
+        self.stages = gnc2[:, 0].astype(np.int64)
+        self.mu = gnc2[:, 1].copy()
+        self.point_w = point_w
 
 
 class BatchPointTerms:
@@ -665,14 +695,30 @@ class Context:
         T_target_source (B,4,4), converged (B,) bool, iterations (B,), num_inliers (B,), error (B,), H (B,6,6), b (B,6).  The weights in
         force (set_source_weights) apply to every round."""
         B, Tc, _, _ = self._batch_args(init_Ts, None)
-        o = AlignOptions(int(factor), int(robust), float(robust_c), int(rejector), float(max_dist_sq), int(optimizer), int(max_iterations), float(gn_lambda),
-                         int(max_inner_iterations), float(init_lambda), float(lambda_factor), float(rotation_eps), float(translation_eps))
-        o.dof_mask[:] = [1.0] * 6 if dof_mask is None else [float(x) for x in dof_mask]
+        o = _align_options(factor, robust, robust_c, rejector, max_dist_sq, optimizer, max_iterations, gn_lambda, max_inner_iterations, init_lambda,
+                           lambda_factor, rotation_eps, translation_eps, dof_mask)
         T = np.zeros((max(B, 1), 16))
         info = np.zeros((max(B, 1), 4))
         Hb = np.zeros((max(B, 1), 42))
         self._check(self._L.sgb_align_batch(self._h, C.byref(o), _d(Tc), _d(T), _d(info), _d(Hb)))
         return BatchAlignResult(T[:B], info[:B], Hb[:B])
+
+    def align_batch_gnc(self, init_Ts, noise_bound_sq, gnc=GNC_TLS, max_stages=64, stage_iterations=3, point_weights=False, **align):
+        """Graduated non-convexity over every member (sgb_align_batch_gnc) -> a GncAlignResult.  Each stage re-estimates every point's weight
+        g on the device from its residual r^2 = 2 e at the member's pose (gnc: GNC_GEMAN_MCCLURE or GNC_TLS, noise_bound_sq = c^2 on that
+        scale), then runs align_batch from there with the weights w * g (w: the weights in force, which the call leaves unchanged) and
+        max_iterations = stage_iterations, or align's max_iterations at the member's last stage.  At most max_stages stages.
+        point_weights=True: each point's final g too.  align: the keywords of align_batch (robust must stay ROBUST_NONE)."""
+        B, Tc, _, _ = self._batch_args(init_Ts, None)
+        o = _align_options(**align)
+        g = GncOptions(int(gnc), float(noise_bound_sq), int(max_stages), int(stage_iterations))
+        T = np.zeros((max(B, 1), 16))
+        info = np.zeros((max(B, 1), 4))
+        Hb = np.zeros((max(B, 1), 42))
+        gnc2 = np.zeros((max(B, 1), 2))
+        pw = np.zeros(max(int(self._batch_offsets[-1]), 1)) if point_weights else None
+        self._check(self._L.sgb_align_batch_gnc(self._h, C.byref(o), C.byref(g), _d(Tc), _d(T), _d(info), _d(Hb), _d(gnc2), _d(pw)))
+        return GncAlignResult(T[:B], info[:B], Hb[:B], gnc2[:B], None if pw is None else pw[: int(self._batch_offsets[-1])])
 
     def align_joint(self, init_X, windows=None, fixed=None, factor=FACTOR_GICP, robust=ROBUST_NONE, robust_c=1.0, rejector=REJECT_DISTANCE, max_dist_sq=1.0,
                     optimizer=OPT_LEVENBERG_MARQUARDT, max_iterations=20, gn_lambda=1e-6, max_inner_iterations=10, init_lambda=1e-3,

@@ -20,6 +20,9 @@
 //   joint_step_kernel       joint windows: one CTA per window, its system assembled from its edges' sums and solved, its state machine,
 //                           its edges' next poses (sgb_align_joint; joint_align_init_kernel / joint_align_finish_kernel: the asynchronous
 //                           call's set-up and outputs)
+//   gnc_*_kernel            sgb_align_batch_gnc: the largest residual of stage 0, each member's mu and last-stage decision, each point's
+//                           GNC weight from its row of the reweighting linearize, each stage's align_init, and the step with each member's
+//                           stage iterations
 // The transform, factor, segment and step kernels serve the rounds the host plans (sgb_{linearize,error,align}_batch, sgb_align_joint) and,
 // with ROUND / kModeRound, the rounds batch_plan_kernel plans on the device (sgb_align_batch_async, sgb_align_joint_async).
 // A member's sums depend on its own points, pose and correspondences only, added in an order fixed by its size: bit-identical whatever
@@ -680,6 +683,112 @@ cudaError_t launch_batch_align_init(const AlignOptions& o, uint32_t n_members, c
 
 cudaError_t launch_batch_align_finish(uint32_t n_members, const MemberState* state, double* out_T16, double* out_info4, double* out_Hb42, cudaStream_t st) {
   batch_align_finish_kernel<<<(n_members + kStepBlock - 1) / kStepBlock, kStepBlock, 0, st>>>(n_members, state, out_T16, out_info4, out_Hb42);
+  return cudaGetLastError();
+}
+
+// ---- sgb_align_batch_gnc (DESIGN.md §11 "Graduated non-convexity") ----
+
+// the grid of a one-thread-per-stored-point GNC kernel (at least one CTA: the launch count does not depend on the point count)
+uint32_t gnc_point_grid(uint32_t n, int sm_count) { return std::max<uint32_t>(1u, std::min<uint32_t>((n + 255u) / 256u, static_cast<uint32_t>(sm_count) * 8u)); }
+
+__global__ void gnc_rmax_kernel(const GncParams p) {
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < p.n; i += gridDim.x * blockDim.x) {
+    const uint32_t m = owner_of(p.member_off, p.n_members, i);
+    if (!p.live[m] || p.corr[i] == kNone) continue;
+    const double r2 = rn_mul(2.0, p.e[batch_row(p.member_off, p.perm, m, i)]);
+    // a non-negative double orders as its bit pattern; -0.0, rounding's tiny negatives and NaN never enter
+    if (r2 > 0.0) atomicMax(reinterpret_cast<unsigned long long*>(&p.gnc[m].r2max), static_cast<unsigned long long>(__double_as_longlong(r2)));
+  }
+}
+
+__global__ void __launch_bounds__(kStepBlock) gnc_stage_kernel(const GncParams p) {
+  const uint32_t m = blockIdx.x * kStepBlock + threadIdx.x;
+  if (m >= p.n_members || !p.live[m]) return;
+  gnc_stage_begin(p.kind, p.c2, p.max_stages, p.gnc[m]);
+}
+
+template <int KIND>
+__global__ void gnc_weight_kernel(const GncParams p) {
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < p.n; i += gridDim.x * blockDim.x) {
+    const uint32_t m = owner_of(p.member_off, p.n_members, i);
+    if (!p.live[m]) continue;
+    const size_t row = batch_row(p.member_off, p.perm, m, i);
+    double g = 0.0;
+    if (p.corr[i] != kNone) {
+      const GncState& s = p.gnc[m];
+      g = s.ones ? 1.0 : gnc_weight<KIND>(rn_mul(2.0, p.e[row]), s.mu, p.c2);
+      if (KIND == kGncTls && g != 0.0 && g != 1.0) atomicOr(&p.gnc[m].not_binary, 1u);
+    }
+    p.e[row] = g;
+    p.wstage[i] = p.w ? rn_mul(__ldg(&p.w[i]), g) : g;
+  }
+}
+
+// the options of member m's align in the current stage
+__device__ __forceinline__ AlignOptions gnc_stage_options(const AlignOptions& o, const GncParams& p, uint32_t m) {
+  AlignOptions om = o;
+  if (!p.gnc[m].last) om.max_iterations = p.stage_iterations;
+  return om;
+}
+
+__global__ void __launch_bounds__(kStepBlock) gnc_init_kernel(const GncParams p, const __grid_constant__ AlignOptions o, MemberState* __restrict__ state,
+                                                              double* __restrict__ poses, uint8_t* __restrict__ phase) {
+  const uint32_t m = blockIdx.x * kStepBlock + threadIdx.x;
+  if (m >= p.n_members) return;
+  MemberState& s = state[m];
+  if (!p.live[m]) {  // finished earlier: its state holds its last stage's result
+    s.phase = kPhaseDone;
+    phase[m] = kPhaseDone;
+    return;
+  }
+  GncState& g = p.gnc[m];
+  if (p.kind == kGncTls && !g.not_binary) g.last = 1;
+  p.live[m] = g.last ? 0 : 1;
+  g.iterations += s.iterations;
+  double T[16];
+  for (int i = 0; i < 16; i++) T[i] = s.T[i];
+  align_init(gnc_stage_options(o, p, m), T, s);
+  double* q = poses + 12 * static_cast<size_t>(m);
+  for (int i = 0; i < 3; i++) {  // pose_from_colmajor
+    for (int j = 0; j < 3; j++) q[i * 3 + j] = T[j * 4 + i];
+    q[9 + i] = T[12 + i];
+  }
+  phase[m] = static_cast<uint8_t>(s.phase);
+}
+
+__global__ void __launch_bounds__(kStepBlock) gnc_step_kernel(const GncParams p, const __grid_constant__ AlignOptions o, bool linearize, const double* __restrict__ out,
+                                                              MemberState* __restrict__ state, double* __restrict__ poses, uint8_t* __restrict__ phase) {
+  const uint32_t m = blockIdx.x * kStepBlock + threadIdx.x;
+  if (m >= p.n_members) return;
+  batch_step_member(gnc_stage_options(o, p, m), m, linearize, out, state, poses, phase);
+}
+
+cudaError_t launch_gnc_rmax(const GncParams& p, int sm_count, cudaStream_t st) {
+  gnc_rmax_kernel<<<gnc_point_grid(p.n, sm_count), 256, 0, st>>>(p);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_gnc_stage(const GncParams& p, cudaStream_t st) {
+  gnc_stage_kernel<<<(p.n_members + kStepBlock - 1) / kStepBlock, kStepBlock, 0, st>>>(p);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_gnc_weight(const GncParams& p, int sm_count, cudaStream_t st) {
+  if (p.kind == kGncTls)
+    gnc_weight_kernel<kGncTls><<<gnc_point_grid(p.n, sm_count), 256, 0, st>>>(p);
+  else
+    gnc_weight_kernel<kGncGemanMcClure><<<gnc_point_grid(p.n, sm_count), 256, 0, st>>>(p);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_gnc_init(const GncParams& p, const AlignOptions& o, MemberState* state, double* poses, uint8_t* phase, cudaStream_t st) {
+  gnc_init_kernel<<<(p.n_members + kStepBlock - 1) / kStepBlock, kStepBlock, 0, st>>>(p, o, state, poses, phase);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_gnc_step(const GncParams& p, const AlignOptions& o, bool linearize, const double* out, MemberState* state, double* poses, uint8_t* phase,
+                            cudaStream_t st) {
+  gnc_step_kernel<<<(p.n_members + kStepBlock - 1) / kStepBlock, kStepBlock, 0, st>>>(p, o, linearize, out, state, poses, phase);
   return cudaGetLastError();
 }
 

@@ -162,6 +162,37 @@ cudaError_t launch_batch_align_init(const AlignOptions& o, uint32_t n_members, c
 /// sgb_align_batch's outputs from the members' final state: T (16, column-major), info (converged, iterations, inliers, error), H | b (or null)
 cudaError_t launch_batch_align_finish(uint32_t n_members, const MemberState* state, double* out_T16, double* out_info4, double* out_Hb42, cudaStream_t st);
 
+// ---- sgb_align_batch_gnc (DESIGN.md §11 "Graduated non-convexity"): the stages' reweighting between host-planned aligns ----
+/// What the GNC kernels of one stage share.  The members in the stage are those with live[m] = 1.  e: [rows] in the row layout of BatchRows
+/// (member_off, perm): the reweighting linearize's e rows in, each point's g of the stage out.  corr: BatchParams::corr after that
+/// linearize.  w: the weights in force in stored order (null: none); wstage: [points] w_i g_i in stored order, the weights of the stage's align.
+struct GncParams {
+  uint32_t n, n_members;
+  int kind;        // kGncGemanMcClure / kGncTls
+  double c2;       // the noise bound c^2
+  int max_stages, stage_iterations;
+  const uint32_t *member_off, *perm;
+  const uint32_t* corr;
+  double* e;
+  const double* w;
+  double* wstage;
+  GncState* gnc;   // [members]
+  uint8_t* live;   // [members] in: in this stage; the init kernel leaves 1 for a member with a stage to go
+};
+/// stage 0: every member's largest r^2 = 2 e_i > 0 over its points with a correspondence (gnc[m].r2max, cleared by the caller)
+cudaError_t launch_gnc_rmax(const GncParams& p, int sm_count, cudaStream_t st);
+/// one thread per member in the stage: gnc_stage_begin
+cudaError_t launch_gnc_stage(const GncParams& p, cudaStream_t st);
+/// one thread per stored point of a member in the stage: its g (0 without a correspondence) to e, w_i g_i to wstage, TLS's not_binary flag
+cudaError_t launch_gnc_weight(const GncParams& p, int sm_count, cudaStream_t st);
+/// one thread per member: a member in the stage ends GNC after it if the stage is its last (TLS: or its weights are all binary), adds
+/// the previous stage's iterations and starts its align from its current pose (align_init of o with max_iterations = stage_iterations
+/// unless last; pose and phase as the align's rounds read them); every other member is left done
+cudaError_t launch_gnc_init(const GncParams& p, const AlignOptions& o, MemberState* state, double* poses, uint8_t* phase, cudaStream_t st);
+/// launch_batch_step for a host-planned round of a GNC stage: each member steps with its stage's max_iterations (as launch_gnc_init chose)
+cudaError_t launch_gnc_step(const GncParams& p, const AlignOptions& o, bool linearize, const double* out, MemberState* state, double* poses, uint8_t* phase,
+                            cudaStream_t st);
+
 // ---- sgb_align_joint (DESIGN.md §11 "Joint windows"): windows of frames, each edge a pair member ----
 /// The call's tables (built once per call) and state.  Window w holds frames frame_off[w] .. frame_off[w + 1] - 1 and the edges
 /// edge_off[w] .. edge_off[w + 1] - 1 of the edge list (member order within each window); edge q is member edge_member[q], cloud frame

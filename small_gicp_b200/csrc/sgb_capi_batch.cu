@@ -1,7 +1,7 @@
 // SPDX-License-Identifier: MIT
 // C-ABI of batched registration (include/sgicp_b200.h: sgb_source_set_batch, sgb_source_set_pairs, sgb_source_set_submaps,
 // sgb_source_set_weights, sgb_{linearize,error,align,correspondences}_batch, sgb_{linearize,error}_batch_points, sgb_align_batch_async, sgb_align_joint,
-// sgb_align_joint_async).
+// sgb_align_joint_async, sgb_align_batch_gnc).
 // Kernels in sgb_batch.cu (many kd-trees and submaps: the searches in sgb_forest.cu); DESIGN.md §11.
 #include <cuda_runtime.h>
 
@@ -271,7 +271,8 @@ int round_kernels(sgb_ctx* ctx, const LinParams& P, const BatchParams& Bp, const
     if (int rc = round ? point_search_round(ctx, Q, &round->n_search, depth) : launch_point_search(ctx, Q, depth)) return rc;
     ctx->launches += counted;
   }
-  const double* weights = ctx->b_weighted ? ctx->b_weights.as<double>() : nullptr;  // (sgb_source_set_weights)
+  // the weights in force (sgb_source_set_weights), or those of an sgb_align_batch_gnc round (RoundWeights)
+  const double* weights = ctx->b_wround ? ctx->b_wuse : ctx->b_weighted ? ctx->b_weights.as<double>() : nullptr;
   CU(launch_batch_factor(Bp, kind, factor, robust, err, round, n_tiles, err ? nullptr : vcorr, centres, regions, S, rows, weights, ctx->stream));
   ctx->launches += counted;
   return 0;
@@ -753,6 +754,80 @@ int error_batch(sgb_ctx* ctx, const char* who, bool points, const double* T, con
   return copy_out(ctx, out, B);
 }
 
+// The initial state and poses of sgb_align_batch (and of stage 0 of sgb_align_batch_gnc): the only upload of poses in the whole align
+int align_start(sgb_ctx* ctx, const AlignOptions& ao, const double* init_T, std::vector<MemberState>& state, std::vector<uint8_t>& phase) {
+  const size_t B = batch_members(ctx);
+  state.resize(B);
+  phase.resize(B);
+  std::vector<double> poses(12 * B);
+  for (size_t m = 0; m < B; m++) {
+    align_init(ao, init_T + 16 * m, state[m]);
+    pose_from_colmajor(init_T + 16 * m, poses.data() + 12 * m);
+    phase[m] = static_cast<uint8_t>(state[m].phase);
+  }
+  CU(ctx->b_state.reserve(B * sizeof(MemberState)));
+  CU(ctx->b_phase.reserve(B));
+  CU(cudaMemcpyAsync(ctx->b_state.p, state.data(), B * sizeof(MemberState), cudaMemcpyHostToDevice, ctx->stream));
+  CU(cudaMemcpyAsync(ctx->b_poses.p, poses.data(), poses.size() * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
+  return 0;
+}
+
+// The outputs of an align from the members' final state; gnc (or null): the iterations of their earlier GNC stages are added
+void align_results(const std::vector<MemberState>& state, const GncState* gnc, double* out_T, double* out_info, double* out_Hb) {
+  for (size_t m = 0; m < state.size(); m++) {
+    const MemberState& s = state[m];
+    std::memcpy(out_T + 16 * m, s.T, 16 * sizeof(double));
+    double* info = out_info + 4 * m;
+    info[0] = s.converged ? 1.0 : 0.0;
+    info[1] = s.iterations + (gnc ? gnc[m].iterations : 0);
+    info[2] = s.inliers;
+    info[3] = s.e;
+    if (out_Hb) {
+      std::memcpy(out_Hb + 42 * m, s.H, 36 * sizeof(double));
+      std::memcpy(out_Hb + 42 * m + 36, s.b, 6 * sizeof(double));
+    }
+  }
+}
+
+// The rounds of sgb_align_batch from the members' phases (read back after each round), in lockstep: error() for every member with a
+// pending trial until none has one, else a linearize of every member still iterating; each round ends with one step launch, step(lin).
+// The host only reads the phases to build the next round's tile tables.
+template <typename Step>
+int align_rounds(sgb_ctx* ctx, const sgb_align_options* o, std::vector<uint8_t>& phase, Step step) {
+  const size_t B = batch_members(ctx);
+  std::vector<uint8_t> active(B);
+  for (;;) {
+    bool any_trial = false, any_lin = false;
+    for (size_t m = 0; m < B; m++) {
+      any_trial |= phase[m] == kPhaseTrial;
+      any_lin |= phase[m] == kPhaseLinearize;
+    }
+    if (!any_trial && !any_lin) return 0;
+    const bool lin = !any_trial;
+    for (size_t m = 0; m < B; m++) active[m] = phase[m] == (lin ? kPhaseLinearize : kPhaseTrial);
+    if (lin) {
+      if (int rc = linearize_round(ctx, o->factor_kind, o->robust_kind, o->robust_c, o->rejector_kind, o->max_dist_sq, nullptr, active.data())) return rc;
+    } else {
+      if (int rc = error_round(ctx, nullptr, active.data())) return rc;
+    }
+    CU(step(lin));
+    ctx->launches += 1;
+    CU(cudaMemcpyAsync(phase.data(), ctx->b_phase.p, B, cudaMemcpyDeviceToHost, ctx->stream));
+    CU(cudaStreamSynchronize(ctx->stream));
+  }
+}
+
+// sgb_align_batch_gnc: the weights its rounds use in place of those in force, until the call returns however it returns
+struct RoundWeights {
+  sgb_ctx* ctx;
+  explicit RoundWeights(sgb_ctx* c) : ctx(c) { ctx->b_wround = true; }
+  ~RoundWeights() {
+    ctx->b_wround = false;
+    ctx->b_wuse = nullptr;
+  }
+  void use(const double* w) { ctx->b_wuse = w; }
+};
+
 }  // namespace
 
 extern "C" {
@@ -981,55 +1056,106 @@ int sgb_align_batch(sgb_ctx* ctx, const sgb_align_options* o, const double* init
   if (B == 0) return 0;
   CU(cudaSetDevice(ctx->device));
   if (int rc = pair_view(ctx)) return rc;
-  // the initial state and poses: the only upload of poses in the whole align
-  std::vector<MemberState> state(B);
-  std::vector<double> poses(12 * B);
-  std::vector<uint8_t> phase(B);
-  for (size_t m = 0; m < B; m++) {
-    align_init(ao, init_T + 16 * m, state[m]);
-    pose_from_colmajor(init_T + 16 * m, poses.data() + 12 * m);
-    phase[m] = static_cast<uint8_t>(state[m].phase);
-  }
-  CU(ctx->b_state.reserve(B * sizeof(MemberState)));
-  CU(ctx->b_phase.reserve(B));
-  CU(cudaMemcpyAsync(ctx->b_state.p, state.data(), B * sizeof(MemberState), cudaMemcpyHostToDevice, ctx->stream));
-  CU(cudaMemcpyAsync(ctx->b_poses.p, poses.data(), poses.size() * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
-  // Rounds in lockstep: error() for every member with a pending trial until none has one, else a linearize of every member still
-  // iterating; each round ends with one step launch.  The host only reads the phases to build the next round's tile tables.
-  std::vector<uint8_t> active(B);
-  for (;;) {
-    bool any_trial = false, any_lin = false;
-    for (size_t m = 0; m < B; m++) {
-      any_trial |= phase[m] == kPhaseTrial;
-      any_lin |= phase[m] == kPhaseLinearize;
-    }
-    if (!any_trial && !any_lin) break;
-    const bool lin = !any_trial;
-    for (size_t m = 0; m < B; m++) active[m] = phase[m] == (lin ? kPhaseLinearize : kPhaseTrial);
-    if (lin) {
-      if (int rc = linearize_round(ctx, o->factor_kind, o->robust_kind, o->robust_c, o->rejector_kind, o->max_dist_sq, nullptr, active.data())) return rc;
-    } else {
-      if (int rc = error_round(ctx, nullptr, active.data())) return rc;
-    }
-    CU(launch_batch_step(ao, static_cast<uint32_t>(B), lin, nullptr, 0, ctx->b_out.as<double>(), ctx->b_state.as<MemberState>(), ctx->b_poses.as<double>(),
-                         ctx->b_phase.as<uint8_t>(), ctx->stream));
-    ctx->launches += 1;
-    CU(cudaMemcpyAsync(phase.data(), ctx->b_phase.p, B, cudaMemcpyDeviceToHost, ctx->stream));
-    CU(cudaStreamSynchronize(ctx->stream));
-  }
+  std::vector<MemberState> state;
+  std::vector<uint8_t> phase;
+  if (int rc = align_start(ctx, ao, init_T, state, phase)) return rc;
+  if (int rc = align_rounds(ctx, o, phase, [&](bool lin) {
+        return launch_batch_step(ao, static_cast<uint32_t>(B), lin, nullptr, 0, ctx->b_out.as<double>(), ctx->b_state.as<MemberState>(),
+                                 ctx->b_poses.as<double>(), ctx->b_phase.as<uint8_t>(), ctx->stream);
+      }))
+    return rc;
   CU(cudaMemcpyAsync(state.data(), ctx->b_state.p, B * sizeof(MemberState), cudaMemcpyDeviceToHost, ctx->stream));
   CU(cudaStreamSynchronize(ctx->stream));
-  for (size_t m = 0; m < B; m++) {
-    const MemberState& s = state[m];
-    std::memcpy(out_T + 16 * m, s.T, 16 * sizeof(double));
-    double* info = out_info + 4 * m;
-    info[0] = s.converged ? 1.0 : 0.0;
-    info[1] = s.iterations;
-    info[2] = s.inliers;
-    info[3] = s.e;
-    if (out_Hb) {
-      std::memcpy(out_Hb + 42 * m, s.H, 36 * sizeof(double));
-      std::memcpy(out_Hb + 42 * m + 36, s.b, 6 * sizeof(double));
+  align_results(state, nullptr, out_T, out_info, out_Hb);
+  return 0;
+}
+
+int sgb_align_batch_gnc(sgb_ctx* ctx, const sgb_align_options* o, const sgb_gnc_options* gnc, const double* init_T, double* out_T, double* out_info,
+                        double* out_Hb, double* out_gnc2, double* out_point_w) {
+  if (!ctx) return 1;
+  const std::string who = "sgb_align_batch_gnc";
+  AlignOptions ao;
+  if (int rc = align_checks(ctx, who.c_str(), o, init_T, out_T, out_info, ao)) return rc;
+  if (!gnc) return fail(ctx, 1, who + ": null GNC options");
+  if (o->robust_kind != SGB_ROBUST_NONE)
+    return fail(ctx, 1, who + ": robust_kind must be SGB_ROBUST_NONE: the GNC weights are the robust kernel (a fixed-width kernel on top would change the cost "
+                              "they anneal)");
+  if (gnc->kind != SGB_GNC_GEMAN_MCCLURE && gnc->kind != SGB_GNC_TLS) return fail(ctx, 1, who + ": invalid GNC kind (SGB_GNC_GEMAN_MCCLURE or SGB_GNC_TLS)");
+  if (!(std::isfinite(gnc->noise_bound_sq) && gnc->noise_bound_sq > 0.0)) return fail(ctx, 1, who + ": noise_bound_sq must be finite and > 0");
+  if (gnc->max_stages < 1) return fail(ctx, 1, who + ": max_stages must be >= 1");
+  if (gnc->stage_iterations < 1) return fail(ctx, 1, who + ": stage_iterations must be >= 1");
+  CU(cudaSetDevice(ctx->device));
+  cudaStreamCaptureStatus capture = cudaStreamCaptureStatusNone;
+  CU(cudaStreamIsCapturing(ctx->stream, &capture));
+  if (capture != cudaStreamCaptureStatusNone)
+    return fail(ctx, 1, who + ": the context's stream is being captured, and the call synchronises at every round and stage to plan the next one; call it "
+                              "outside the capture");
+  const size_t B = batch_members(ctx), n = batch_points(ctx);
+  if (B == 0) return 0;
+  if (int rc = pair_view(ctx)) return rc;
+  CU(ctx->g_w.reserve(std::max<size_t>(n, 1) * sizeof(double)));
+  CU(ctx->g_e.reserve(std::max<size_t>(n, 1) * sizeof(double)));
+  CU(ctx->g_state.reserve(B * (sizeof(GncState) + 1)));
+  std::vector<MemberState> state;
+  std::vector<uint8_t> phase;
+  if (int rc = align_start(ctx, ao, init_T, state, phase)) return rc;
+  // every member starts its stage 0: zero GNC state (r2max = 0, no stage begun), live
+  std::vector<unsigned char> g0(B * (sizeof(GncState) + 1), 0);
+  std::fill(g0.begin() + B * sizeof(GncState), g0.end(), 1);
+  CU(cudaMemcpyAsync(ctx->g_state.p, g0.data(), g0.size(), cudaMemcpyHostToDevice, ctx->stream));
+  GncParams gp = {};
+  gp.n = static_cast<uint32_t>(n);
+  gp.n_members = static_cast<uint32_t>(B);
+  gp.kind = gnc->kind;
+  gp.c2 = gnc->noise_bound_sq;
+  gp.max_stages = gnc->max_stages;
+  gp.stage_iterations = gnc->stage_iterations;
+  row_layout(ctx, gp.member_off, gp.perm);
+  gp.corr = ctx->b_corr.as<uint32_t>();
+  gp.e = ctx->g_e.as<double>();
+  gp.w = ctx->b_weighted ? ctx->b_weights.as<double>() : nullptr;
+  gp.wstage = ctx->g_w.as<double>();
+  gp.gnc = ctx->g_state.as<GncState>();
+  gp.live = reinterpret_cast<uint8_t*>(gp.gnc + B);
+  BatchRows rows = {};
+  rows.member_off = gp.member_off;
+  rows.perm = gp.perm;
+  rows.e = gp.e;
+  RoundWeights weights(ctx);
+  std::vector<uint8_t> live(B, 1);
+  for (int stage = 0; std::find(live.begin(), live.end(), 1) != live.end(); stage++) {
+    // the reweighting linearize of the members in the stage at their current pose: unweighted, no robust kernel, its e rows to g_e
+    weights.use(nullptr);
+    if (int rc = linearize_round(ctx, o->factor_kind, SGB_ROBUST_NONE, o->robust_c, o->rejector_kind, o->max_dist_sq, nullptr, live.data(), &rows)) return rc;
+    if (stage == 0) {
+      CU(launch_gnc_rmax(gp, ctx->sm_count, ctx->stream));
+      ctx->launches += 1;
+    }
+    CU(launch_gnc_stage(gp, ctx->stream));
+    CU(launch_gnc_weight(gp, ctx->sm_count, ctx->stream));
+    CU(launch_gnc_init(gp, ao, ctx->b_state.as<MemberState>(), ctx->b_poses.as<double>(), ctx->b_phase.as<uint8_t>(), ctx->stream));
+    ctx->launches += 3;
+    CU(cudaMemcpyAsync(phase.data(), ctx->b_phase.p, B, cudaMemcpyDeviceToHost, ctx->stream));
+    CU(cudaMemcpyAsync(live.data(), gp.live, B, cudaMemcpyDeviceToHost, ctx->stream));
+    CU(cudaStreamSynchronize(ctx->stream));
+    // the stage's align with its weights
+    weights.use(gp.wstage);
+    if (int rc = align_rounds(ctx, o, phase, [&](bool lin) {
+          return launch_gnc_step(gp, ao, lin, ctx->b_out.as<double>(), ctx->b_state.as<MemberState>(), ctx->b_poses.as<double>(), ctx->b_phase.as<uint8_t>(),
+                                 ctx->stream);
+        }))
+      return rc;
+  }
+  std::vector<GncState> g(B);
+  CU(cudaMemcpyAsync(state.data(), ctx->b_state.p, B * sizeof(MemberState), cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaMemcpyAsync(g.data(), gp.gnc, B * sizeof(GncState), cudaMemcpyDeviceToHost, ctx->stream));
+  if (out_point_w && n) CU(cudaMemcpyAsync(out_point_w, gp.e, n * sizeof(double), cudaMemcpyDefault, ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));
+  align_results(state, g.data(), out_T, out_info, out_Hb);
+  if (out_gnc2) {
+    for (size_t m = 0; m < B; m++) {
+      out_gnc2[2 * m] = g[m].stages;
+      out_gnc2[2 * m + 1] = g[m].mu;
     }
   }
   return 0;

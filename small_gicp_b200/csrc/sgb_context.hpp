@@ -200,6 +200,12 @@ struct sgb_ctx {
   // The source setters and pairings clear b_weighted (begin_source, begin_pairs); the buffer keeps its address while the count does.
   bool b_weighted = false;
   sgb::DevBuf b_weights, b_wnext, b_wbad;
+  // sgb_align_batch_gnc, for the call's duration: b_wround = its rounds use b_wuse (null: unweighted) instead of the weights in force.
+  // Its own grow-only buffers: g_w = the stage's weights (stored order), g_e = the reweighting linearize's e rows and then each point's g
+  // (row layout), g_state = GncState [members] | live flags [members].
+  bool b_wround = false;
+  const double* b_wuse = nullptr;
+  sgb::DevBuf g_w, g_e, g_state;
   // The clouds of sgb_source_set_batch are stored once (src_* and b_centres / b_bounds, cloud after cloud).  Without a pairing the
   // members are those clouds.  After sgb_source_set_pairs (b_paired) member p is a replica of one stored cloud in p_*, b_offsets are
   // the members' offsets, and b_pair_maps (empty: member m against map m) names each member's map.

@@ -679,6 +679,86 @@ SGB_HD void align_after_error(const AlignOptions& o, MemberState& s, double cand
 }
 
 // ---------------------------------------------------------------------------------------------------------------------------------
+// Graduated non-convexity (sgb_align_batch_gnc, the gnc_* kernels in sgb_batch.cu; DESIGN.md §11 "Graduated non-convexity"): the
+// closed-form weight of a point of squared residual r2 under the surrogate of shape mu, and the mu schedule.  Every operation is an
+// explicitly rounded FP64 one in a fixed order, so nothing is contracted into an FMA and numpy reproduces every bit (tests/np_gnc.py;
+// compiled for the host in tests/host_gnc, where the plain operators are built without contraction).
+// ---------------------------------------------------------------------------------------------------------------------------------
+#if defined(__CUDA_ARCH__)
+SGB_HD double rn_add(double a, double b) { return __dadd_rn(a, b); }
+SGB_HD double rn_sub(double a, double b) { return __dsub_rn(a, b); }
+SGB_HD double rn_mul(double a, double b) { return __dmul_rn(a, b); }
+SGB_HD double rn_div(double a, double b) { return __ddiv_rn(a, b); }
+SGB_HD double rn_sqrt(double a) { return __dsqrt_rn(a); }
+#else
+SGB_HD double rn_add(double a, double b) { return a + b; }
+SGB_HD double rn_sub(double a, double b) { return a - b; }
+SGB_HD double rn_mul(double a, double b) { return a * b; }
+SGB_HD double rn_div(double a, double b) { return a / b; }
+SGB_HD double rn_sqrt(double a) { return std::sqrt(a); }
+#endif
+
+enum : int { kGncGemanMcClure = 0, kGncTls = 1 };  // sgb_gnc_kind
+constexpr double kGncFactor = 1.4;                  // the annealing factor of Yang et al. (RA-L 2020)
+
+/// The weight of a point with squared residual r2 (>= 0 up to rounding) under the surrogate of shape mu, noise bound c2:
+///   Geman-McClure  (mu c2 / (r2 + mu c2))^2
+///   TLS            1 if r2 <= mu / (mu + 1) c2, 0 if r2 >= (mu + 1) / mu c2, else min(max(sqrt(c2) / sqrt(r2) sqrt(mu (mu + 1)) - mu, 0), 1)
+/// (the clamp only catches the rounding of the middle branch at its two edges, where it is 1 and 0).
+template <int KIND>
+SGB_HD double gnc_weight(double r2, double mu, double c2) {
+  if constexpr (KIND == kGncGemanMcClure) {
+    const double a = rn_mul(mu, c2);
+    const double q = rn_div(a, rn_add(r2, a));
+    return rn_mul(q, q);
+  } else {
+    const double mu1 = rn_add(mu, 1.0);
+    if (r2 <= rn_mul(rn_div(mu, mu1), c2)) return 1.0;
+    if (r2 >= rn_mul(rn_div(mu1, mu), c2)) return 0.0;
+    const double g = rn_sub(rn_mul(rn_div(rn_sqrt(c2), rn_sqrt(r2)), rn_sqrt(rn_mul(mu, mu1))), mu);
+    return g < 0.0 ? 0.0 : (g > 1.0 ? 1.0 : g);
+  }
+}
+
+/// One member's GNC between stages.  r2max: the largest r^2 > 0 of stage 0's reweighting linearize (0: none), kept as the bits of a
+/// non-negative double so that atomicMax on them is an exact, order-free maximum.
+struct GncState {
+  double mu;          // the surrogate's shape of the current (after the loop: the last) stage
+  double r2max;
+  int stages;         // stages begun
+  int last;           // the current stage is the member's last
+  int ones;           // TLS without outliers (2 r2max <= c2): every weight of its only stage is 1
+  unsigned not_binary;  // TLS: a weight of the current stage lies strictly between 0 and 1
+  int iterations;     // the iterations of the member's finished stages
+};
+
+/// The start of a member's next stage: mu_0 from r2max at stage 0 (GM: 2 r2max / c2, at least 1; TLS: c2 / (2 r2max - c2), or none
+/// without outliers), else the schedule's next mu (GM: max(mu / 1.4, 1); TLS: 1.4 mu).  The stage is the last when GM reaches mu = 1,
+/// TLS has no outliers, or it is stage max_stages - 1; TLS also ends at a stage whose weights are all binary (decided after them).
+SGB_HD void gnc_stage_begin(int kind, double c2, int max_stages, GncState& g) {
+  if (g.stages == 0) {
+    const double t = rn_mul(2.0, g.r2max);
+    if (kind == kGncGemanMcClure) {
+      g.mu = rn_div(t, c2);
+      if (g.mu <= 1.0) g.mu = 1.0;
+    } else if (t <= c2) {
+      g.mu = 0.0;
+      g.ones = 1;
+    } else {
+      g.mu = rn_div(c2, rn_sub(t, c2));
+    }
+  } else if (kind == kGncGemanMcClure) {
+    const double m = rn_div(g.mu, kGncFactor);
+    g.mu = m > 1.0 ? m : 1.0;
+  } else {
+    g.mu = rn_mul(kGncFactor, g.mu);
+  }
+  g.last = g.ones || (kind == kGncGemanMcClure && g.mu == 1.0) || g.stages == max_stages - 1;
+  g.stages++;
+  g.not_binary = 0u;
+}
+
+// ---------------------------------------------------------------------------------------------------------------------------------
 // Joint window registration (sgb_align_joint, joint_step_kernel in sgb_batch.cu; DESIGN.md §11 "Joint windows").  The frames X_k of a
 // window are solved together against every edge (i, j) of the window, each edge a pair member at T_e = X_j^-1 X_i.  The functions below
 // are run by every thread of one CTA (tid of nt threads, CTA barriers between phases); compiled for the host (tests/host_joint) they run
