@@ -3,17 +3,13 @@
      iterations, inliers, error, correspondences afterwards), on many kd-trees (ICP, point-to-plane, GICP) and many voxel maps (ICP,
      GICP), every robust kernel, GN and LM, a DoF mask, max_iterations 0 / 1 / 20;
   2. a star window (edges i -> 0, frame 0 fixed: H block diagonal) after one GN iteration is the pairwise align of every edge;
-  3. round by round: the GN step of every window after k iterations is np_joint's step from the edges relinearised on a second context,
-     for windows of 3, 8 and 32 frames with chains and a loop edge;
+  3. round by round, GN and LM, every option and window shapes beyond these: tests/test_gpu_align_joint_replay.py;
   4. ground truth: 8 LiDAR frames perturbed by ~2 deg / 0.3 m come within 0.5 deg / 0.05 m (GICP on kd-trees and on voxel maps);
   5. a window's results do not depend on the other windows of the call; empty windows, edge-less frames, all-fixed windows;
   6. the launch count per round is the pairs round's plus one, for 1 and 1024 windows;
   7. misuse fails with its message and leaves the context usable."""
 import numpy as np
 import pytest
-
-import np_joint as J
-from np_align import Options
 
 pytestmark = pytest.mark.gpu
 
@@ -135,35 +131,6 @@ def _window_edges(F, loop=True):
     if loop and F > 2:
         e.append((0, F - 1))
     return e
-
-
-@pytest.mark.parametrize("F", [3, 8, 32])
-@pytest.mark.parametrize("kind", ["kdtree", "voxelmap"])
-def test_gn_rounds_replay_against_the_model(frames, F, kind):
-    """X_{k+1} of the joint GN is np_joint's step from X_k with the edges relinearised at X_j^-1 X_i on a second context"""
-    idx = list(range(F))
-    edges = _window_edges(F)
-    cl, mp = [e[0] for e in edges], [e[1] for e in edges]
-    X0 = _perturbed(frames, idx, 3)
-    fixed = [1] + [0] * (F - 1)
-    ctx = _context(frames, idx, kind, cl, mp)
-    lin = _context(frames, idx, kind, cl, mp)
-    kw = dict(factor=2, optimizer=GN, max_dist_sq=1.0)
-    o = Options(lm=False)
-    Xk = X0
-    for k in range(3):
-        r = ctx.align_joint(X0, **kw, max_iterations=k + 1)
-        Ts = np.array([J.edge_pose(Xk[i], Xk[j]) for i, j in edges])
-        H, b, e, inl = lin.linearize_batch(Ts, factor=2, max_dist_sq=1.0)
-        Hw, bw = J.assemble(list(Xk), edges, fixed, list(H), list(b), o.dof_mask)
-        d = J.damped_solve(Hw, bw, o.gn_lambda)
-        pred = [Xk[0]] + [Xk[m] @ _exp(d[6 * (m - 1) : 6 * m]) for m in range(1, F)]
-        if r.iterations[0] == k:  # the window ran iteration k (not converged before it)
-            for m in range(F):
-                np.testing.assert_allclose(r.X[m], pred[m], rtol=1e-9, atol=1e-9)
-            np.testing.assert_allclose(r.error[0], e.sum(), rtol=1e-12)
-            assert r.num_inliers[0] == inl.sum()
-        Xk = r.X
 
 
 def _rot_deg(R):
