@@ -13,8 +13,11 @@
 #pragma once
 #include <cstdint>
 #include <cstring>
+#include <iterator>
 #include <limits>
+#include <map>
 #include <memory>
+#include <mutex>
 #include <stdexcept>
 #include <string>
 #include <tuple>
@@ -98,6 +101,25 @@ struct DeviceMirror {
     if (ctx && owned) sgb_destroy(ctx);
   }
 };
+
+/// The one mirror record of a borrowed context.  Reductions that share a context through use_context() share what they believe it
+/// holds: with a record each, one would keep searching a target another has since replaced on the device.  Attaching forgets the
+/// record's clouds (a context created at the address of a destroyed one must not inherit its record).
+inline std::shared_ptr<DeviceMirror> borrowed_mirror(sgb_ctx* ctx) {
+  static std::mutex lock;
+  static std::map<sgb_ctx*, std::weak_ptr<DeviceMirror>> by_ctx;
+  std::lock_guard<std::mutex> guard(lock);
+  for (auto it = by_ctx.begin(); it != by_ctx.end();) it = it->second.expired() ? by_ctx.erase(it) : std::next(it);
+  std::shared_ptr<DeviceMirror> m = by_ctx[ctx].lock();
+  if (!m) {
+    m = std::make_shared<DeviceMirror>();
+    m->ctx = ctx;
+    m->owned = false;
+    by_ctx[ctx] = m;
+  }
+  m->target_valid = m->source_valid = false;
+  return m;
+}
 
 /// Contiguous views of a cloud in the C-ABI's layout (N x 4 / N x 16 doubles).  small_gicp::PointCloud's three std::vectors ARE
 /// that layout and are passed through without a copy; any other cloud type is gathered through its traits first.
@@ -226,11 +248,8 @@ struct ParallelReductionCUDA {
 
   /// Run on a context the caller owns (and keeps alive) instead of creating one: creating a context costs milliseconds (stream, page-locked
   /// result slot, first allocations) -- code that constructs a Registration<> per align() call shares one long-lived context this way.
-  void use_context(sgb_ctx* ctx) const {
-    mirror_ = std::make_shared<cuda_detail::DeviceMirror>();
-    mirror_->ctx = ctx;
-    mirror_->owned = false;
-  }
+  /// Every reduction given the same context shares one record of what the context holds (cuda_detail::borrowed_mirror).
+  void use_context(sgb_ctx* ctx) const { mirror_ = cuda_detail::borrowed_mirror(ctx); }
 
   sgb_ctx* context() const {
     if (!mirror_) mirror_ = std::make_shared<cuda_detail::DeviceMirror>();
@@ -313,9 +332,29 @@ private:
       covs[i] = v.second.cov;
     }
     check(ctx, sgb_target_set_voxelmap(ctx, 1.0 / target.inv_leaf_size, n, coords.data(), n ? means[0].data() : nullptr, n ? covs[0].data() : nullptr,
-                                       static_cast<int>(target.search_offsets.size())));
+                                       offset_pattern(target.search_offsets)));
     mirror_->target = mirror_->tree = key;
     mirror_->target_valid = true;
+  }
+
+  /// The probe pattern of a map's search_offsets: 1, 7 or 27.  Counted by distinct offsets, not by size(): set_search_offsets(27)
+  /// appends the cube to the centre the constructor put there (incremental_voxelmap.hpp:46,176-183), which leaves 28 entries.
+  template <typename Offsets>
+  static int offset_pattern(const Offsets& offsets) {
+    bool seen[27] = {};
+    int distinct = 0, axis = 0;
+    for (const auto& o : offsets) {
+      if (o[0] < -1 || o[0] > 1 || o[1] < -1 || o[1] > 1 || o[2] < -1 || o[2] > 1) throw std::runtime_error("ParallelReductionCUDA: voxel search offset outside the 3x3x3 cube");
+      const int k = (o[0] + 1) * 9 + (o[1] + 1) * 3 + (o[2] + 1);
+      if (seen[k]) continue;
+      seen[k] = true;
+      distinct++;
+      axis += (o[0] != 0) + (o[1] != 0) + (o[2] != 0) == 1;
+    }
+    if (distinct == 1 && seen[13]) return 1;
+    if (distinct == 7 && seen[13] && axis == 6) return 7;
+    if (distinct == 27) return 27;
+    throw std::runtime_error("ParallelReductionCUDA: voxel search_offsets must be one of the patterns of set_search_offsets (1, 7 or 27)");
   }
 
   mutable std::shared_ptr<cuda_detail::DeviceMirror> mirror_;
