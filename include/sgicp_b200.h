@@ -466,6 +466,26 @@ int sgb_align_batch_async(sgb_ctx* ctx, const sgb_align_options* options, const 
  *     capture, not at replay.  A call with no window enqueues nothing. */
 int sgb_align_joint_async(sgb_ctx* ctx, const sgb_align_options* options, size_t n_windows, const size_t* window_off, const uint8_t* fixed /*or NULL*/,
                           const double* d_init_X16xK, double* d_out_X16xK, double* d_out_info4xW);
+/* sgb_align_batch_gnc enqueued on the context's stream with no host involvement after the call, as sgb_align_batch_async enqueues
+ * sgb_align_batch: a CUDA graph whose outer WHILE node runs one GNC stage per iteration (the reweighting linearize of the members still
+ * in GNC, planned on the device; the stage's mu, weights and align_init) and whose body holds an inner WHILE node repeating the stage's
+ * align rounds (planner, search, factor with the stage's weights, per-member sums, step) until no member has a round to go.  Members run
+ * their stages in lockstep in sgb_align_batch_gnc's order.
+ *   - Arguments, checks, messages and results as sgb_align_batch_gnc, except that every pose and output is device memory of the context's
+ *     GPU (host, page-locked or managed pointers fail with a message, nothing enqueued).  For the same inputs T, info, H | b, gnc2 and
+ *     out_point_w are bit-identical to it, the context is left as it leaves it (sgb_correspondences_batch, sgb_error_batch and
+ *     sgb_linearize_batch behave alike afterwards), and the weights in force are unchanged.  Errors of the enqueued work surface at the next
+ *     synchronising call of the context.
+ *   - While the context's stream is being captured the whole GNC is added to the capture: each replay re-runs it from what d_init_T16xB
+ *     and the weights in force hold at replay time.  A call that would have to allocate (the GNC buffers for the batch, the first batched
+ *     call's search queue, the capture streams) fails with a message instead: call it once outside the capture first.  The captured work
+ *     is only valid while the context's batch, pairing, target and buffers are those of the capture.  Outside a capture the instantiated
+ *     graph is cached in the context and rebuilt when the align or GNC options, the batch, the pairing, the target or any buffer it uses
+ *     changes.
+ *   - sgb_kernel_launches counts 4 per call (initial state, one launch of the graph, two for the outputs), whatever the stage and round
+ *     counts, plus 1 when the pairing's view of the target is rebuilt; captured work counts at capture, not at replay. */
+int sgb_align_batch_gnc_async(sgb_ctx* ctx, const sgb_align_options* options, const sgb_gnc_options* gnc, const double* d_init_T16xB, double* d_out_T16xB,
+                              double* d_out_info4xB, double* d_out_Hb42xB /*or NULL*/, double* d_out_gnc2xB /*or NULL*/, double* d_out_point_w /*or NULL*/);
 
 /* ---- per-cloud preparation on the device (SURVEY.md §8(f); not per-iteration) --------------------
  * sgb_estimate_features replaces estimate_normals / estimate_covariances / estimate_normals_covariances and

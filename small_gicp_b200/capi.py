@@ -106,6 +106,7 @@ _SIGNATURES = {
     "sgb_align_batch": (C.c_int, [_vp, C.POINTER(AlignOptions), _dp, _dp, _dp, _dp]),
     "sgb_align_batch_async": (C.c_int, [_vp, C.POINTER(AlignOptions), _dp, _dp, _dp, _dp]),
     "sgb_align_batch_gnc": (C.c_int, [_vp, C.POINTER(AlignOptions), C.POINTER(GncOptions), _dp, _dp, _dp, _dp, _dp, _dp]),
+    "sgb_align_batch_gnc_async": (C.c_int, [_vp, C.POINTER(AlignOptions), C.POINTER(GncOptions), _dp, _dp, _dp, _dp, _dp, _dp]),
     "sgb_align_joint": (C.c_int, [_vp, C.POINTER(AlignOptions), C.c_size_t, C.POINTER(C.c_size_t), C.POINTER(C.c_uint8), _dp, _dp, _dp]),
     "sgb_align_joint_async": (C.c_int, [_vp, C.POINTER(AlignOptions), C.c_size_t, C.POINTER(C.c_size_t), C.POINTER(C.c_uint8), _dp, _dp, _dp]),
     "sgb_estimate_features": (C.c_int, [_vp, C.c_size_t, _dp, C.c_int, _dp, _dp]),
@@ -191,6 +192,18 @@ class AsyncAlignResult:
         self.error = info4[:, 3]
         self.H = Hb42[:, :36].view(B, 6, 6).transpose(1, 2)
         self.b = Hb42[:, 36:42]
+
+
+class AsyncGncAlignResult(AsyncAlignResult):
+    """what Context.align_batch_gnc_async enqueued: the AsyncAlignResult views (iterations summed over the stages), stages (B,) and mu (B,)
+    as float64 views of the raw gnc2 (B,2), and point_w (N,) each point's final g (None unless requested).  The raw outputs T16, info4,
+    Hb42, gnc2 and point_w pass as out= to reuse them (graph capture needs fixed buffers)."""
+
+    def __init__(self, T16, info4, Hb42, gnc2, point_w):
+        super().__init__(T16, info4, Hb42)
+        self.gnc2, self.point_w = gnc2, point_w
+        self.stages = gnc2[:, 0]
+        self.mu = gnc2[:, 1]
 
 
 class AsyncJointAlignResult:
@@ -780,6 +793,45 @@ class Context:
                 self._async_in = torch.empty((max(B, 1), 16), dtype=torch.float64, device=dev)[:B]
             self._async_in.view(B, 4, 4).copy_(init_Ts.transpose(1, 2))  # column-major
         self._check(self._L.sgb_align_batch_async(self._h, C.byref(o), _d(self._async_in), _d(out.T16), _d(out.info4), _d(out.Hb42)))
+        return out
+
+    def align_batch_gnc_async(self, init_Ts, noise_bound_sq, gnc=GNC_TLS, max_stages=64, stage_iterations=3, point_weights=False, out=None, **align):
+        """align_batch_gnc enqueued on the context's stream without a host synchronisation (sgb_align_batch_gnc_async): every stage and round
+        runs on the device.  init_Ts and the stream as in align_batch_async; the other arguments as in align_batch_gnc.  Returns an
+        AsyncGncAlignResult of CUDA tensors (out: a previous result whose buffers are reused; it must hold point_w if point_weights).  Inside
+        torch.cuda.graph (with the capture stream set) the whole GNC is captured: each replay re-runs it from what init_Ts holds then, with
+        the weights in force then (set_source_weights)."""
+        import torch
+
+        if self._stream is None:
+            raise SgbError("align_batch_gnc_async: set the context's stream to a torch stream first (set_stream): the poses are prepared on it")
+        offsets = getattr(self, "_batch_offsets", None)  # (no batch yet: the library says so)
+        B = int(offsets.size) - 1 if offsets is not None else int(init_Ts.shape[0])
+        N = int(offsets[-1]) if offsets is not None else 0
+        if not (isinstance(init_Ts, torch.Tensor) and init_Ts.is_cuda and init_Ts.dtype == torch.float64 and tuple(init_Ts.shape) == (B, 4, 4)):
+            raise SgbError(f"align_batch_gnc_async: init_Ts must be a CUDA float64 tensor of shape ({B}, 4, 4)")
+        o = _align_options(**align)
+        g = GncOptions(int(gnc), float(noise_bound_sq), int(max_stages), int(stage_iterations))
+        dev = init_Ts.device
+        with torch.cuda.stream(torch.cuda.ExternalStream(self._stream, device=dev)):
+            if out is None:
+                n = max(B, 1)
+
+                def zeros(rows, cols):
+                    return torch.zeros((n, cols), dtype=torch.float64, device=dev)[:rows]
+
+                pw = torch.zeros(max(N, 1), dtype=torch.float64, device=dev)[:N] if point_weights else None
+                out = AsyncGncAlignResult(zeros(B, 16), zeros(B, 4), zeros(B, 42), zeros(B, 2), pw)
+            elif tuple(out.T16.shape) != (B, 16):
+                raise SgbError(f"align_batch_gnc_async: out holds {out.T16.shape[0]} members, the batch {B}")
+            elif point_weights and (out.point_w is None or tuple(out.point_w.shape) != (N,)):
+                raise SgbError(f"align_batch_gnc_async: point_weights needs out.point_w of {N} rows")
+            if self._async_in is None or self._async_in.shape[0] != B or self._async_in.device != dev:
+                self._async_in = torch.empty((max(B, 1), 16), dtype=torch.float64, device=dev)[:B]
+            self._async_in.view(B, 4, 4).copy_(init_Ts.transpose(1, 2))  # column-major
+        pw = out.point_w if point_weights else None
+        self._check(self._L.sgb_align_batch_gnc_async(self._h, C.byref(o), C.byref(g), _d(self._async_in), _d(out.T16), _d(out.info4), _d(out.Hb42),
+                                                      _d(out.gnc2), _d(pw)))
         return out
 
     def align_joint_async(self, init_X, windows=None, fixed=None, factor=FACTOR_GICP, robust=ROBUST_NONE, robust_c=1.0, rejector=REJECT_DISTANCE,

@@ -22,9 +22,11 @@
 //                           call's set-up and outputs)
 //   gnc_*_kernel            sgb_align_batch_gnc: the largest residual of stage 0, each member's mu and last-stage decision, each point's
 //                           GNC weight from its row of the reweighting linearize, each stage's align_init, and the step with each member's
-//                           stage iterations
+//                           stage iterations (sgb_align_batch_gnc_async: gnc_reweigh_kernel / gnc_loops_kernel / gnc_finish_kernel,
+//                           each stage's phases, the loops' conditions and the outputs)
 // The transform, factor, segment and step kernels serve the rounds the host plans (sgb_{linearize,error,align}_batch, sgb_align_joint) and,
-// with ROUND / kModeRound, the rounds batch_plan_kernel plans on the device (sgb_align_batch_async, sgb_align_joint_async).
+// with ROUND / kModeRound, the rounds batch_plan_kernel plans on the device (sgb_align_batch_async, sgb_align_joint_async,
+// sgb_align_batch_gnc_async).
 // A member's sums depend on its own points, pose and correspondences only, added in an order fixed by its size: bit-identical whatever
 // else is in the batch.
 #include <algorithm>
@@ -230,8 +232,8 @@ __device__ __forceinline__ void batch_factor_tile(const BatchParams& B, const ui
 // One CTA per tile of one member, for the target's KIND: 0 one point target, 1 one voxel map, 2 many voxel maps (member m against map m:
 // map_centres and map_regions), 3 many kd-trees (map_centres; vcorr = what forest_search_kernel found in map m), 4 submaps (S; vcorr and
 // S.centry = what forest_search_kernel<SUBMAP> found over the member's entries).  MODE: linearize, error() with the cached correspondences, or
-// either as the round's planner decided.  POINTS (host-planned modes only): every processed point's row to `rows` too.  WEIGHTED (any
-// mode): each point's terms times its weight rows.w[i].
+// either as the round's planner decided.  POINTS: every processed point's row to `rows` too (in a round: the reweighting round of
+// sgb_align_batch_gnc_async only).  WEIGHTED (any mode): each point's terms times its weight rows.w[i].
 template <int FACTOR, int ROBUST, int KIND, int MODE, bool POINTS = false, bool WEIGHTED = false>
 __global__ void __launch_bounds__(kLinBlock, 4) batch_factor_kernel(const __grid_constant__ BatchParams B, const uint32_t* __restrict__ vcorr,
                                                                    const double* __restrict__ map_centres, const uint4* __restrict__ map_regions,
@@ -465,9 +467,14 @@ auto factor_kernel(int kind) -> decltype(&batch_factor_kernel<0, 0, 0, kModeLine
   }
 }
 
-// the factor kernel of one kind for a round (device-planned), or for a host-planned mode with or without rows
+// the factor kernel of one kind for a round (device-planned), or for a host-planned mode with or without rows.  A device-planned round
+// with rows is the reweighting round of sgb_align_batch_gnc_async: unweighted, no robust kernel (GNC refuses one), its e rows wanted.
 template <int F, int R, bool WEIGHTED>
 auto factor_kernel(int kind, bool err, bool round, bool rows) -> decltype(&batch_factor_kernel<0, 0, 0, kModeLinearize>) {
+  if (round && rows) {
+    if constexpr (R == 0 && !WEIGHTED) return factor_kernel<F, R, kModeRound, true, false>(kind);
+    else return nullptr;
+  }
   if (rows) return err ? factor_kernel<F, R, kModeError, true, WEIGHTED>(kind) : factor_kernel<F, R, kModeLinearize, true, WEIGHTED>(kind);
   return round ? factor_kernel<F, R, kModeRound, false, WEIGHTED>(kind) : err ? factor_kernel<F, R, kModeError, false, WEIGHTED>(kind)
                                                                                : factor_kernel<F, R, kModeLinearize, false, WEIGHTED>(kind);
@@ -477,7 +484,6 @@ cudaError_t launch_batch_factor(const BatchParams& B, int kind, int factor, int 
                                 const double* map_centres, const uint4* map_regions, const SubmapView& S, const BatchRows* rows, const double* weights,
                                 cudaStream_t st) {
   if (factor == 1 && (kind == 1 || kind == 2 || kind == 4)) return cudaErrorInvalidValue;  // no normals in a voxel map; no point-to-plane against a union
-  if (round && rows) return cudaErrorInvalidValue;
   const auto kernel = dispatch_factor_robust(factor, robust, decltype(&batch_factor_kernel<0, 0, 0, kModeLinearize>){}, [&](auto f, auto r) {
     return weights ? factor_kernel<f, r, true>(kind, err, round, rows) : factor_kernel<f, r, false>(kind, err, round, rows);
   });
@@ -691,10 +697,13 @@ cudaError_t launch_batch_align_finish(uint32_t n_members, const MemberState* sta
 // the grid of a one-thread-per-stored-point GNC kernel (at least one CTA: the launch count does not depend on the point count)
 uint32_t gnc_point_grid(uint32_t n, int sm_count) { return std::max<uint32_t>(1u, std::min<uint32_t>((n + 255u) / 256u, static_cast<uint32_t>(sm_count) * 8u)); }
 
+// ROUND (sgb_align_batch_gnc_async, launched at every stage of its loop): only the members before their stage 0 (no stage begun)
+template <bool ROUND>
 __global__ void gnc_rmax_kernel(const GncParams p) {
   for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < p.n; i += gridDim.x * blockDim.x) {
     const uint32_t m = owner_of(p.member_off, p.n_members, i);
     if (!p.live[m] || p.corr[i] == kNone) continue;
+    if (ROUND && p.gnc[m].stages != 0) continue;
     const double r2 = rn_mul(2.0, p.e[batch_row(p.member_off, p.perm, m, i)]);
     // a non-negative double orders as its bit pattern; -0.0, rounding's tiny negatives and NaN never enter
     if (r2 > 0.0) atomicMax(reinterpret_cast<unsigned long long*>(&p.gnc[m].r2max), static_cast<unsigned long long>(__double_as_longlong(r2)));
@@ -755,16 +764,68 @@ __global__ void __launch_bounds__(kStepBlock) gnc_init_kernel(const GncParams p,
   }
   phase[m] = static_cast<uint8_t>(s.phase);
 }
-
+// ROUND: a round of a stage of sgb_align_batch_gnc_async, its kind read from `round`; `loop` becomes 1 while a member has a round to go
+template <bool ROUND>
 __global__ void __launch_bounds__(kStepBlock) gnc_step_kernel(const GncParams p, const __grid_constant__ AlignOptions o, bool linearize, const double* __restrict__ out,
-                                                              MemberState* __restrict__ state, double* __restrict__ poses, uint8_t* __restrict__ phase) {
+                                                              MemberState* __restrict__ state, double* __restrict__ poses, uint8_t* __restrict__ phase,
+                                                              const BatchRound* __restrict__ round, cudaGraphConditionalHandle loop) {
   const uint32_t m = blockIdx.x * kStepBlock + threadIdx.x;
-  if (m >= p.n_members) return;
-  batch_step_member(gnc_stage_options(o, p, m), m, linearize, out, state, poses, phase);
+  if constexpr (ROUND) {
+    int more = 0;
+    if (m < p.n_members) {
+      batch_step_member(gnc_stage_options(o, p, m), m, round->lin != 0u, out, state, poses, phase);
+      more = phase[m] == kPhaseLinearize || phase[m] == kPhaseTrial;
+    }
+    if (__syncthreads_or(more) && threadIdx.x == 0) cudaGraphSetConditional(loop, 1u);
+  } else {
+    if (m >= p.n_members) return;
+    batch_step_member(gnc_stage_options(o, p, m), m, linearize, out, state, poses, phase);
+  }
 }
 
-cudaError_t launch_gnc_rmax(const GncParams& p, int sm_count, cudaStream_t st) {
-  gnc_rmax_kernel<<<gnc_point_grid(p.n, sm_count), 256, 0, st>>>(p);
+// ---- sgb_align_batch_gnc_async (DESIGN.md §11 "Asynchronous graduated non-convexity") ----
+
+// The head of a stage: the members still in GNC in kPhaseLinearize, the others done, so that the planner plans the reweighting linearize
+// of exactly the members in the stage; `rounds` cleared (gnc_loops_kernel sets it)
+__global__ void __launch_bounds__(kStepBlock) gnc_reweigh_kernel(uint32_t n_members, const uint8_t* __restrict__ live, uint8_t* __restrict__ phase,
+                                                                 cudaGraphConditionalHandle rounds) {
+  const uint32_t m = blockIdx.x * kStepBlock + threadIdx.x;
+  if (m == 0) cudaGraphSetConditional(rounds, 0u);
+  if (m < n_members) phase[m] = live[m] ? kPhaseLinearize : kPhaseDone;
+}
+
+// After gnc_init_kernel: `stages` becomes 1 if a member has a stage to go after this one, `rounds` (cleared by gnc_reweigh_kernel) 1 if
+// a member's align has a round to go
+__global__ void __launch_bounds__(kStepBlock) gnc_loops_kernel(uint32_t n_members, const uint8_t* __restrict__ live, const uint8_t* __restrict__ phase,
+                                                               cudaGraphConditionalHandle stages, cudaGraphConditionalHandle rounds) {
+  const uint32_t m = blockIdx.x * kStepBlock + threadIdx.x;
+  int more_stages = 0, more_rounds = 0;
+  if (m < n_members) {
+    more_stages = live[m];
+    more_rounds = phase[m] == kPhaseLinearize || phase[m] == kPhaseTrial;
+  }
+  if (__syncthreads_or(more_stages) && threadIdx.x == 0) cudaGraphSetConditional(stages, 1u);
+  if (__syncthreads_or(more_rounds) && threadIdx.x == 0) cudaGraphSetConditional(rounds, 1u);
+}
+
+// what sgb_align_batch_gnc adds to batch_align_finish_kernel's outputs: the iterations of the earlier stages, the stages and last mu
+__global__ void __launch_bounds__(kStepBlock) gnc_finish_kernel(uint32_t n_members, const MemberState* __restrict__ state, const GncState* __restrict__ gnc,
+                                                                double* __restrict__ out_info4, double* __restrict__ out_gnc2) {
+  const uint32_t m = blockIdx.x * kStepBlock + threadIdx.x;
+  if (m >= n_members) return;
+  const GncState& g = gnc[m];
+  out_info4[4 * static_cast<size_t>(m) + 1] = state[m].iterations + g.iterations;
+  if (out_gnc2) {
+    out_gnc2[2 * static_cast<size_t>(m)] = g.stages;
+    out_gnc2[2 * static_cast<size_t>(m) + 1] = g.mu;
+  }
+}
+
+cudaError_t launch_gnc_rmax(const GncParams& p, bool round, int sm_count, cudaStream_t st) {
+  if (round)
+    gnc_rmax_kernel<true><<<gnc_point_grid(p.n, sm_count), 256, 0, st>>>(p);
+  else
+    gnc_rmax_kernel<false><<<gnc_point_grid(p.n, sm_count), 256, 0, st>>>(p);
   return cudaGetLastError();
 }
 
@@ -786,9 +847,29 @@ cudaError_t launch_gnc_init(const GncParams& p, const AlignOptions& o, MemberSta
   return cudaGetLastError();
 }
 
-cudaError_t launch_gnc_step(const GncParams& p, const AlignOptions& o, bool linearize, const double* out, MemberState* state, double* poses, uint8_t* phase,
-                            cudaStream_t st) {
-  gnc_step_kernel<<<(p.n_members + kStepBlock - 1) / kStepBlock, kStepBlock, 0, st>>>(p, o, linearize, out, state, poses, phase);
+cudaError_t launch_gnc_step(const GncParams& p, const AlignOptions& o, bool linearize, const BatchRound* round, cudaGraphConditionalHandle loop, const double* out,
+                            MemberState* state, double* poses, uint8_t* phase, cudaStream_t st) {
+  const uint32_t grid = (p.n_members + kStepBlock - 1) / kStepBlock;
+  if (round)
+    gnc_step_kernel<true><<<grid, kStepBlock, 0, st>>>(p, o, linearize, out, state, poses, phase, round, loop);
+  else
+    gnc_step_kernel<false><<<grid, kStepBlock, 0, st>>>(p, o, linearize, out, state, poses, phase, nullptr, loop);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_gnc_reweigh(uint32_t n_members, const uint8_t* live, uint8_t* phase, cudaGraphConditionalHandle rounds, cudaStream_t st) {
+  gnc_reweigh_kernel<<<(n_members + kStepBlock - 1) / kStepBlock, kStepBlock, 0, st>>>(n_members, live, phase, rounds);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_gnc_loops(uint32_t n_members, const uint8_t* live, const uint8_t* phase, cudaGraphConditionalHandle stages, cudaGraphConditionalHandle rounds,
+                             cudaStream_t st) {
+  gnc_loops_kernel<<<(n_members + kStepBlock - 1) / kStepBlock, kStepBlock, 0, st>>>(n_members, live, phase, stages, rounds);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_gnc_finish(uint32_t n_members, const MemberState* state, const GncState* gnc, double* out_info4, double* out_gnc2, cudaStream_t st) {
+  gnc_finish_kernel<<<(n_members + kStepBlock - 1) / kStepBlock, kStepBlock, 0, st>>>(n_members, state, gnc, out_info4, out_gnc2);
   return cudaGetLastError();
 }
 

@@ -144,8 +144,9 @@ cudaError_t launch_batch_unmatch(const BatchParams& B, const BatchRound* round, 
 /// map (the VGICP probe), 2 many voxel maps (member m against map m: map_centres [maps][4], map_regions [maps] = (first table slot, mask,
 /// first voxel, voxel count) of each map), 3 many kd-trees (map_centres; vcorr = the forest search's result), 4 submaps (S; vcorr = the
 /// submap search's result).  Linearize (err = false), error() with the cached correspondences (err = true), or with a round what it
-/// says.  Point-to-plane only for kinds 0 and 3.  rows (rounds planned on the host only; null: none): every processed point's row too.
-/// weights (null: none): each point's terms scaled by its weight (stored order) before its row and the sums.
+/// says.  Point-to-plane only for kinds 0 and 3.  rows (null: none): every processed point's row too; with a round only unweighted and
+/// without a robust kernel (the reweighting round of sgb_align_batch_gnc_async).  weights (null: none): each point's terms scaled by its
+/// weight (stored order) before its row and the sums.
 cudaError_t launch_batch_factor(const BatchParams& B, int kind, int factor, int robust, bool err, const BatchRound* round, uint32_t n_tiles, const uint32_t* vcorr,
                                 const double* map_centres, const uint4* map_regions, const SubmapView& S, const BatchRows* rows, const double* weights,
                                 cudaStream_t st);
@@ -179,8 +180,9 @@ struct GncParams {
   GncState* gnc;   // [members]
   uint8_t* live;   // [members] in: in this stage; the init kernel leaves 1 for a member with a stage to go
 };
-/// stage 0: every member's largest r^2 = 2 e_i > 0 over its points with a correspondence (gnc[m].r2max, cleared by the caller)
-cudaError_t launch_gnc_rmax(const GncParams& p, int sm_count, cudaStream_t st);
+/// stage 0: every member's largest r^2 = 2 e_i > 0 over its points with a correspondence (gnc[m].r2max, cleared by the caller).  round:
+/// launched at every stage of the device loop, for the members that have begun no stage only
+cudaError_t launch_gnc_rmax(const GncParams& p, bool round, int sm_count, cudaStream_t st);
 /// one thread per member in the stage: gnc_stage_begin
 cudaError_t launch_gnc_stage(const GncParams& p, cudaStream_t st);
 /// one thread per stored point of a member in the stage: its g (0 without a correspondence) to e, w_i g_i to wstage, TLS's not_binary flag
@@ -189,9 +191,20 @@ cudaError_t launch_gnc_weight(const GncParams& p, int sm_count, cudaStream_t st)
 /// the previous stage's iterations and starts its align from its current pose (align_init of o with max_iterations = stage_iterations
 /// unless last; pose and phase as the align's rounds read them); every other member is left done
 cudaError_t launch_gnc_init(const GncParams& p, const AlignOptions& o, MemberState* state, double* poses, uint8_t* phase, cudaStream_t st);
-/// launch_batch_step for a host-planned round of a GNC stage: each member steps with its stage's max_iterations (as launch_gnc_init chose)
-cudaError_t launch_gnc_step(const GncParams& p, const AlignOptions& o, bool linearize, const double* out, MemberState* state, double* poses, uint8_t* phase,
-                            cudaStream_t st);
+/// launch_batch_step for a round of a GNC stage: each member steps with its stage's max_iterations (as launch_gnc_init chose).  round = null:
+/// a host-planned round; else a round planned on the device, its kind read from `round`, `loop` set to 1 while a member has a round to go
+cudaError_t launch_gnc_step(const GncParams& p, const AlignOptions& o, bool linearize, const BatchRound* round, cudaGraphConditionalHandle loop, const double* out,
+                            MemberState* state, double* poses, uint8_t* phase, cudaStream_t st);
+
+// ---- sgb_align_batch_gnc_async (DESIGN.md §11 "Asynchronous graduated non-convexity"): the stages and their rounds on the device ----
+/// the head of a stage: phase[m] = kPhaseLinearize for the members still in GNC (live), kPhaseDone for the others; `rounds` set to 0
+cudaError_t launch_gnc_reweigh(uint32_t n_members, const uint8_t* live, uint8_t* phase, cudaGraphConditionalHandle rounds, cudaStream_t st);
+/// after launch_gnc_init: `stages` set to 1 if a member has a stage to go after this one (live), `rounds` to 1 if a member's align has a
+/// round to go
+cudaError_t launch_gnc_loops(uint32_t n_members, const uint8_t* live, const uint8_t* phase, cudaGraphConditionalHandle stages, cudaGraphConditionalHandle rounds,
+                             cudaStream_t st);
+/// after launch_batch_align_finish: info's iterations summed over the stages, and gnc2 (or null) = the stages run and the last stage's mu
+cudaError_t launch_gnc_finish(uint32_t n_members, const MemberState* state, const GncState* gnc, double* out_info4, double* out_gnc2, cudaStream_t st);
 
 // ---- sgb_align_joint (DESIGN.md §11 "Joint windows"): windows of frames, each edge a pair member ----
 /// The call's tables (built once per call) and state.  Window w holds frames frame_off[w] .. frame_off[w + 1] - 1 and the edges

@@ -1,7 +1,7 @@
 // SPDX-License-Identifier: MIT
 // C-ABI of batched registration (include/sgicp_b200.h: sgb_source_set_batch, sgb_source_set_pairs, sgb_source_set_submaps,
 // sgb_source_set_weights, sgb_{linearize,error,align,correspondences}_batch, sgb_{linearize,error}_batch_points, sgb_align_batch_async, sgb_align_joint,
-// sgb_align_joint_async, sgb_align_batch_gnc).
+// sgb_align_joint_async, sgb_align_batch_gnc, sgb_align_batch_gnc_async).
 // Kernels in sgb_batch.cu (many kd-trees and submaps: the searches in sgb_forest.cu); DESIGN.md §11.
 #include <cuda_runtime.h>
 
@@ -450,7 +450,8 @@ int pair_members(sgb_ctx* ctx, const char* who, size_t n_members, const uint32_t
   return 0;
 }
 
-// ---- the device loop of sgb_align_batch_async and sgb_align_joint_async (DESIGN.md §11 "Asynchronous align", "Asynchronous joint windows") ----
+// ---- the device loops of sgb_align_batch_async, sgb_align_joint_async and sgb_align_batch_gnc_async (DESIGN.md §11 "Asynchronous align",
+// "Asynchronous joint windows", "Asynchronous graduated non-convexity") ----
 
 // the kernel parameters every round of the device loop shares (those of linearize_round; error() reads the same ones)
 void round_params(sgb_ctx* ctx, const sgb_align_options* o, LinParams& P, BatchParams& Bp) {
@@ -461,8 +462,9 @@ void round_params(sgb_ctx* ctx, const sgb_align_options* o, LinParams& P, BatchP
 }
 
 // The head of one round of a device loop on ctx->stream: planner, search, factor, per-member sums into b_out.  Every grid is sized for
-// the worst case (every tile, every point, every member); what the round does is read from b_round.  The caller's step follows.
-int round_head(sgb_ctx* ctx, const sgb_align_options* o, cudaGraphConditionalHandle loop) {
+// the worst case (every tile, every point, every member); what the round does is read from b_round.  The caller's step follows.  rows
+// (null: none): the factor kernel's per-point rows too (sgb_align_batch_gnc_async's reweighting round).
+int round_head(sgb_ctx* ctx, const sgb_align_options* o, cudaGraphConditionalHandle loop, const BatchRows* rows = nullptr) {
   const size_t B = batch_members(ctx);
   const uint32_t T = static_cast<uint32_t>(max_tiles(ctx));
   const bool voxel = voxel_target(ctx), no_target = ctx->n_tgt == 0, point = !no_target && !voxel && !ctx->b_submaps && ctx->tgt_state != TargetState::KdTrees;
@@ -493,59 +495,85 @@ int round_head(sgb_ctx* ctx, const sgb_align_options* o, cudaGraphConditionalHan
   if (no_target) {
     CU(launch_batch_unmatch(Bp, round, T, ctx->stream));
   } else if (int rc = round_kernels(ctx, P, Bp, round, T, static_cast<uint32_t>(batch_points(ctx)), false, o->factor_kind, o->robust_kind,
-                                    search_bound(o->rejector_kind, o->max_dist_sq))) {
+                                    search_bound(o->rejector_kind, o->max_dist_sq), rows)) {
     return rc;
   }
   CU(launch_batch_segment(Bp, static_cast<uint32_t>(B), true, round, ctx->b_out.as<double>(), ctx->stream));
   return 0;
 }
 
-// A WHILE node in g (after deps) whose body is one round -- round_head, then step(loop) -- captured on the context's capture stream.  The
-// condition starts at 1 at every launch of g; the planner clears it and the step sets it again while a member (or window) has a round to go.
-template <typename Step>
-int add_loop(sgb_ctx* ctx, const char* who, const sgb_align_options* o, cudaGraph_t g, const std::vector<cudaGraphNode_t>& deps, cudaGraphNode_t* node, Step step) {
-  cudaGraphConditionalHandle h;
-  cudaError_t e = cudaGraphConditionalHandleCreate(&h, g, 1, cudaGraphCondAssignDefault);
+// A conditional handle for a WHILE node of g (null: the graph ctx->stream is being captured into); its condition starts at 1 at every
+// launch of g.  Made before the node when kernels captured ahead of the node set it (a loop nested in a loop's body).
+int loop_handle(sgb_ctx* ctx, const char* who, cudaGraph_t g, cudaGraphConditionalHandle* h) {
+  if (!g) {
+    cudaStreamCaptureStatus capture = cudaStreamCaptureStatusNone;
+    CU(cudaStreamGetCaptureInfo(ctx->stream, &capture, nullptr, &g, nullptr, nullptr));
+  }
+  const cudaError_t e = cudaGraphConditionalHandleCreate(h, g, 1, cudaGraphCondAssignDefault);
   if (e != cudaSuccess)
     return fail(ctx, 2, std::string(who) + ": cudaGraphConditionalHandleCreate: " + cudaGetErrorString(e) +
                             " (the device loop needs conditional graph nodes: CUDA 12.4 or later, driver included)");
+  return 0;
+}
+
+// A WHILE node of h in g (after deps) whose body is whatever body(h) enqueues on ctx->stream, captured on a capture stream of the context:
+// cap_stream, or cap_stream_nested for the body of a loop nested in a body being captured on cap_stream.
+template <typename Body>
+int add_loop(sgb_ctx* ctx, cudaGraph_t g, const std::vector<cudaGraphNode_t>& deps, cudaGraphConditionalHandle h, cudaGraphNode_t* node, Body body) {
   cudaGraphNodeParams np = {};
   np.type = cudaGraphNodeTypeConditional;
   np.conditional.handle = h;
   np.conditional.type = cudaGraphCondTypeWhile;
   np.conditional.size = 1;
   CU(cudaGraphAddNode(node, g, deps.empty() ? nullptr : deps.data(), deps.size(), &np));
-  if (!ctx->cap_stream) CU(cudaStreamCreateWithFlags(&ctx->cap_stream, cudaStreamNonBlocking));
-  CU(cudaStreamBeginCaptureToGraph(ctx->cap_stream, np.conditional.phGraph_out[0], nullptr, nullptr, 0, cudaStreamCaptureModeRelaxed));
+  cudaStream_t& cap = ctx->cap_stream && ctx->stream == ctx->cap_stream ? ctx->cap_stream_nested : ctx->cap_stream;
+  if (!cap) CU(cudaStreamCreateWithFlags(&cap, cudaStreamNonBlocking));
+  CU(cudaStreamBeginCaptureToGraph(cap, np.conditional.phGraph_out[0], nullptr, nullptr, 0, cudaStreamCaptureModeRelaxed));
   const cudaStream_t user = ctx->stream;
-  ctx->stream = ctx->cap_stream;
-  int rc = round_head(ctx, o, h);
-  if (!rc) rc = step(h);
+  ctx->stream = cap;
+  const int rc = body(h);
   ctx->stream = user;
-  cudaGraph_t body = nullptr;
-  e = cudaStreamEndCapture(ctx->cap_stream, &body);
+  cudaGraph_t captured = nullptr;
+  const cudaError_t e = cudaStreamEndCapture(cap, &captured);
   if (rc) return rc;
   CU(e);
   return 0;
 }
 
-// One launch of a device loop (add_loop) on ctx->stream.  While the stream is captured the WHILE node joins the capture after what it
-// already holds; otherwise the instantiated graph cached in exec under cached_key is launched, rebuilt first when key (everything the
-// loop captured) differs from it.
+// While ctx->stream is being captured: a WHILE node of h (add_loop) joins the capture after what it already holds
+template <typename Body>
+int capture_loop(sgb_ctx* ctx, cudaGraphConditionalHandle h, Body body) {
+  cudaStreamCaptureStatus capture = cudaStreamCaptureStatusNone;
+  cudaGraph_t g = nullptr;
+  const cudaGraphNode_t* d = nullptr;
+  size_t nd = 0;
+  CU(cudaStreamGetCaptureInfo(ctx->stream, &capture, nullptr, &g, &d, &nd));
+  const std::vector<cudaGraphNode_t> deps(d, d + nd);
+  cudaGraphNode_t w = nullptr;
+  if (int rc = add_loop(ctx, g, deps, h, &w, body)) return rc;
+  CU(cudaStreamUpdateCaptureDependencies(ctx->stream, &w, 1, cudaStreamSetCaptureDependencies));
+  return 0;
+}
+
+// The body of a loop of rounds: round_head, then step(loop), which sets the condition again while a member (or window) has a round to
+// go (the planner clears it)
 template <typename Step>
-int launch_loop(sgb_ctx* ctx, const char* who, const sgb_align_options* o, bool capturing, std::vector<unsigned char> key, cudaGraphExec_t& exec,
-                std::vector<unsigned char>& cached_key, Step step) {
+auto round_loop(sgb_ctx* ctx, const sgb_align_options* o, Step step) {
+  return [=](cudaGraphConditionalHandle h) {
+    if (int rc = round_head(ctx, o, h)) return rc;
+    return step(h);
+  };
+}
+
+// One launch of a device loop on ctx->stream.  While the stream is captured the WHILE node joins the capture (capture_loop); otherwise
+// the instantiated graph cached in exec under cached_key is launched, rebuilt first when key (everything the loop captured) differs from it.
+template <typename Body>
+int launch_loop(sgb_ctx* ctx, const char* who, bool capturing, std::vector<unsigned char> key, cudaGraphExec_t& exec, std::vector<unsigned char>& cached_key,
+                Body body) {
   if (capturing) {
-    cudaStreamCaptureStatus capture = cudaStreamCaptureStatusNone;
-    cudaGraph_t g = nullptr;
-    const cudaGraphNode_t* d = nullptr;
-    size_t nd = 0;
-    CU(cudaStreamGetCaptureInfo(ctx->stream, &capture, nullptr, &g, &d, &nd));
-    const std::vector<cudaGraphNode_t> deps(d, d + nd);
-    cudaGraphNode_t w = nullptr;
-    if (int rc = add_loop(ctx, who, o, g, deps, &w, step)) return rc;
-    CU(cudaStreamUpdateCaptureDependencies(ctx->stream, &w, 1, cudaStreamSetCaptureDependencies));
-    return 0;
+    cudaGraphConditionalHandle h;
+    if (int rc = loop_handle(ctx, who, nullptr, &h)) return rc;
+    return capture_loop(ctx, h, body);
   }
   if (!exec || key != cached_key) {
     if (exec) cudaGraphExecDestroy(exec);
@@ -553,8 +581,10 @@ int launch_loop(sgb_ctx* ctx, const char* who, const sgb_align_options* o, bool 
     cached_key.clear();
     cudaGraph_t g = nullptr;
     CU(cudaGraphCreate(&g, 0));
+    cudaGraphConditionalHandle h;
     cudaGraphNode_t w = nullptr;
-    const int rc = add_loop(ctx, who, o, g, {}, &w, step);
+    int rc = loop_handle(ctx, who, g, &h);
+    if (!rc) rc = add_loop(ctx, g, {}, h, &w, body);
     const cudaError_t e = rc ? cudaSuccess : cudaGraphInstantiate(&exec, g, 0);
     cudaGraphDestroy(g);
     if (rc) return rc;
@@ -828,6 +858,44 @@ struct RoundWeights {
   void use(const double* w) { ctx->b_wuse = w; }
 };
 
+// The checks both GNC aligns make before anything is enqueued (who names the caller): align_checks', then the GNC options'
+int gnc_checks(sgb_ctx* ctx, const std::string& who, const sgb_align_options* o, const sgb_gnc_options* gnc, const double* init_T, const double* out_T,
+               const double* out_info, AlignOptions& ao) {
+  if (int rc = align_checks(ctx, who.c_str(), o, init_T, out_T, out_info, ao)) return rc;
+  if (!gnc) return fail(ctx, 1, who + ": null GNC options");
+  if (o->robust_kind != SGB_ROBUST_NONE)
+    return fail(ctx, 1, who + ": robust_kind must be SGB_ROBUST_NONE: the GNC weights are the robust kernel (a fixed-width kernel on top would change the cost "
+                              "they anneal)");
+  if (gnc->kind != SGB_GNC_GEMAN_MCCLURE && gnc->kind != SGB_GNC_TLS) return fail(ctx, 1, who + ": invalid GNC kind (SGB_GNC_GEMAN_MCCLURE or SGB_GNC_TLS)");
+  if (!(std::isfinite(gnc->noise_bound_sq) && gnc->noise_bound_sq > 0.0)) return fail(ctx, 1, who + ": noise_bound_sq must be finite and > 0");
+  if (gnc->max_stages < 1) return fail(ctx, 1, who + ": max_stages must be >= 1");
+  if (gnc->stage_iterations < 1) return fail(ctx, 1, who + ": stage_iterations must be >= 1");
+  return 0;
+}
+
+// the bytes of g_w, g_e and g_state a GNC align of the batch uses
+size_t gnc_w_bytes(const sgb_ctx* ctx) { return std::max<size_t>(batch_points(ctx), 1) * sizeof(double); }
+size_t gnc_state_bytes(const sgb_ctx* ctx) { return batch_members(ctx) * (sizeof(GncState) + 1); }
+
+// The GNC kernels' parameters of a call over g_w, g_e and g_state (reserved for the batch)
+GncParams gnc_params(sgb_ctx* ctx, const sgb_gnc_options* gnc) {
+  GncParams gp = {};
+  gp.n = static_cast<uint32_t>(batch_points(ctx));
+  gp.n_members = static_cast<uint32_t>(batch_members(ctx));
+  gp.kind = gnc->kind;
+  gp.c2 = gnc->noise_bound_sq;
+  gp.max_stages = gnc->max_stages;
+  gp.stage_iterations = gnc->stage_iterations;
+  row_layout(ctx, gp.member_off, gp.perm);
+  gp.corr = ctx->b_corr.as<uint32_t>();
+  gp.e = ctx->g_e.as<double>();
+  gp.w = ctx->b_weighted ? ctx->b_weights.as<double>() : nullptr;
+  gp.wstage = ctx->g_w.as<double>();
+  gp.gnc = ctx->g_state.as<GncState>();
+  gp.live = reinterpret_cast<uint8_t*>(gp.gnc + gp.n_members);
+  return gp;
+}
+
 }  // namespace
 
 extern "C" {
@@ -1075,15 +1143,7 @@ int sgb_align_batch_gnc(sgb_ctx* ctx, const sgb_align_options* o, const sgb_gnc_
   if (!ctx) return 1;
   const std::string who = "sgb_align_batch_gnc";
   AlignOptions ao;
-  if (int rc = align_checks(ctx, who.c_str(), o, init_T, out_T, out_info, ao)) return rc;
-  if (!gnc) return fail(ctx, 1, who + ": null GNC options");
-  if (o->robust_kind != SGB_ROBUST_NONE)
-    return fail(ctx, 1, who + ": robust_kind must be SGB_ROBUST_NONE: the GNC weights are the robust kernel (a fixed-width kernel on top would change the cost "
-                              "they anneal)");
-  if (gnc->kind != SGB_GNC_GEMAN_MCCLURE && gnc->kind != SGB_GNC_TLS) return fail(ctx, 1, who + ": invalid GNC kind (SGB_GNC_GEMAN_MCCLURE or SGB_GNC_TLS)");
-  if (!(std::isfinite(gnc->noise_bound_sq) && gnc->noise_bound_sq > 0.0)) return fail(ctx, 1, who + ": noise_bound_sq must be finite and > 0");
-  if (gnc->max_stages < 1) return fail(ctx, 1, who + ": max_stages must be >= 1");
-  if (gnc->stage_iterations < 1) return fail(ctx, 1, who + ": stage_iterations must be >= 1");
+  if (int rc = gnc_checks(ctx, who, o, gnc, init_T, out_T, out_info, ao)) return rc;
   CU(cudaSetDevice(ctx->device));
   cudaStreamCaptureStatus capture = cudaStreamCaptureStatusNone;
   CU(cudaStreamIsCapturing(ctx->stream, &capture));
@@ -1093,9 +1153,9 @@ int sgb_align_batch_gnc(sgb_ctx* ctx, const sgb_align_options* o, const sgb_gnc_
   const size_t B = batch_members(ctx), n = batch_points(ctx);
   if (B == 0) return 0;
   if (int rc = pair_view(ctx)) return rc;
-  CU(ctx->g_w.reserve(std::max<size_t>(n, 1) * sizeof(double)));
-  CU(ctx->g_e.reserve(std::max<size_t>(n, 1) * sizeof(double)));
-  CU(ctx->g_state.reserve(B * (sizeof(GncState) + 1)));
+  CU(ctx->g_w.reserve(gnc_w_bytes(ctx)));
+  CU(ctx->g_e.reserve(gnc_w_bytes(ctx)));
+  CU(ctx->g_state.reserve(gnc_state_bytes(ctx)));
   std::vector<MemberState> state;
   std::vector<uint8_t> phase;
   if (int rc = align_start(ctx, ao, init_T, state, phase)) return rc;
@@ -1103,20 +1163,7 @@ int sgb_align_batch_gnc(sgb_ctx* ctx, const sgb_align_options* o, const sgb_gnc_
   std::vector<unsigned char> g0(B * (sizeof(GncState) + 1), 0);
   std::fill(g0.begin() + B * sizeof(GncState), g0.end(), 1);
   CU(cudaMemcpyAsync(ctx->g_state.p, g0.data(), g0.size(), cudaMemcpyHostToDevice, ctx->stream));
-  GncParams gp = {};
-  gp.n = static_cast<uint32_t>(n);
-  gp.n_members = static_cast<uint32_t>(B);
-  gp.kind = gnc->kind;
-  gp.c2 = gnc->noise_bound_sq;
-  gp.max_stages = gnc->max_stages;
-  gp.stage_iterations = gnc->stage_iterations;
-  row_layout(ctx, gp.member_off, gp.perm);
-  gp.corr = ctx->b_corr.as<uint32_t>();
-  gp.e = ctx->g_e.as<double>();
-  gp.w = ctx->b_weighted ? ctx->b_weights.as<double>() : nullptr;
-  gp.wstage = ctx->g_w.as<double>();
-  gp.gnc = ctx->g_state.as<GncState>();
-  gp.live = reinterpret_cast<uint8_t*>(gp.gnc + B);
+  const GncParams gp = gnc_params(ctx, gnc);
   BatchRows rows = {};
   rows.member_off = gp.member_off;
   rows.perm = gp.perm;
@@ -1128,7 +1175,7 @@ int sgb_align_batch_gnc(sgb_ctx* ctx, const sgb_align_options* o, const sgb_gnc_
     weights.use(nullptr);
     if (int rc = linearize_round(ctx, o->factor_kind, SGB_ROBUST_NONE, o->robust_c, o->rejector_kind, o->max_dist_sq, nullptr, live.data(), &rows)) return rc;
     if (stage == 0) {
-      CU(launch_gnc_rmax(gp, ctx->sm_count, ctx->stream));
+      CU(launch_gnc_rmax(gp, false, ctx->sm_count, ctx->stream));
       ctx->launches += 1;
     }
     CU(launch_gnc_stage(gp, ctx->stream));
@@ -1141,8 +1188,8 @@ int sgb_align_batch_gnc(sgb_ctx* ctx, const sgb_align_options* o, const sgb_gnc_
     // the stage's align with its weights
     weights.use(gp.wstage);
     if (int rc = align_rounds(ctx, o, phase, [&](bool lin) {
-          return launch_gnc_step(gp, ao, lin, ctx->b_out.as<double>(), ctx->b_state.as<MemberState>(), ctx->b_poses.as<double>(), ctx->b_phase.as<uint8_t>(),
-                                 ctx->stream);
+          return launch_gnc_step(gp, ao, lin, nullptr, 0, ctx->b_out.as<double>(), ctx->b_state.as<MemberState>(), ctx->b_poses.as<double>(),
+                                 ctx->b_phase.as<uint8_t>(), ctx->stream);
         }))
       return rc;
   }
@@ -1158,6 +1205,110 @@ int sgb_align_batch_gnc(sgb_ctx* ctx, const sgb_align_options* o, const sgb_gnc_
       out_gnc2[2 * m + 1] = g[m].mu;
     }
   }
+  return 0;
+}
+
+int sgb_align_batch_gnc_async(sgb_ctx* ctx, const sgb_align_options* o, const sgb_gnc_options* gnc, const double* d_init_T, double* d_out_T, double* d_out_info,
+                              double* d_out_Hb, double* d_out_gnc2, double* d_out_point_w) {
+  if (!ctx) return 1;
+  const char* who = "sgb_align_batch_gnc_async";
+  AlignOptions ao;
+  if (int rc = gnc_checks(ctx, who, o, gnc, d_init_T, d_out_T, d_out_info, ao)) return rc;
+  const size_t B = batch_members(ctx), n = batch_points(ctx);
+  if (B == 0) return 0;
+  CU(cudaSetDevice(ctx->device));
+  if (int rc = device_pointer(ctx, who, d_init_T, "init_T16xB")) return rc;
+  if (int rc = device_pointer(ctx, who, d_out_T, "out_T16xB")) return rc;
+  if (int rc = device_pointer(ctx, who, d_out_info, "out_info4xB")) return rc;
+  if (d_out_Hb) {
+    if (int rc = device_pointer(ctx, who, d_out_Hb, "out_Hb42xB")) return rc;
+  }
+  if (d_out_gnc2) {
+    if (int rc = device_pointer(ctx, who, d_out_gnc2, "out_gnc2xB")) return rc;
+  }
+  if (d_out_point_w) {
+    if (int rc = device_pointer(ctx, who, d_out_point_w, "out_point_w")) return rc;
+  }
+  cudaStreamCaptureStatus capture = cudaStreamCaptureStatusNone;
+  CU(cudaStreamIsCapturing(ctx->stream, &capture));
+  if (capture == cudaStreamCaptureStatusInvalidated) return fail(ctx, 1, std::string(who) + ": the context's stream is in an invalidated capture");
+  const bool capturing = capture == cudaStreamCaptureStatusActive;
+  // A capture can hold no allocation: the GNC buffers, the packet queue and both capture streams (the stages' loop and the rounds' loop
+  // nested in it) must come from an earlier call
+  const bool allocates = ctx->g_w.cap < gnc_w_bytes(ctx) || ctx->g_e.cap < gnc_w_bytes(ctx) || ctx->g_state.cap < gnc_state_bytes(ctx) ||
+                         (ctx->use_packet_queue && !ctx->packet_queue.p) || !ctx->cap_stream || !ctx->cap_stream_nested;
+  if (capturing && allocates)
+    return fail(ctx, 1, std::string(who) + ": this call needs an allocation, which a capture cannot hold; call it once outside the capture first");
+  if (ctx->use_packet_queue && !ctx->packet_queue.p) {
+    CU(ctx->packet_queue.reserve(2 * sizeof(uint32_t)));
+    CU(cudaMemsetAsync(ctx->packet_queue.p, 0, 2 * sizeof(uint32_t), ctx->stream));
+  }
+  CU(ctx->g_w.reserve(gnc_w_bytes(ctx)));
+  CU(ctx->g_e.reserve(gnc_w_bytes(ctx)));
+  CU(ctx->g_state.reserve(gnc_state_bytes(ctx)));
+  if (int rc = pair_view(ctx)) return rc;
+  const GncParams gp = gnc_params(ctx, gnc);
+  BatchRows rows = {};
+  rows.member_off = gp.member_off;
+  rows.perm = gp.perm;
+  rows.e = gp.e;
+  const uint32_t nb = static_cast<uint32_t>(B);
+  MemberState* state = ctx->b_state.as<MemberState>();
+  double* poses = ctx->b_poses.as<double>();
+  uint8_t* phase = ctx->b_phase.as<uint8_t>();
+  // sgb_align_batch_gnc's initial state: every member's align_init at its initial pose, zero GNC state, every member live (the seed flags
+  // kept as sgb_align_batch_async keeps them)
+  CU(launch_batch_align_init(ao, nb, d_init_T, state, poses, phase, ctx->b_dseed.as<uint8_t>(), ctx->corr_seeds && ctx->b_dseed_ok, ctx->stream));
+  CU(cudaMemsetAsync(gp.gnc, 0, B * sizeof(GncState), ctx->stream));
+  CU(cudaMemsetAsync(gp.live, 1, B, ctx->stream));
+  ctx->launches += 3;  // the initial state here, the outputs below
+  // One stage per iteration of the outer loop, in sgb_align_batch_gnc's order: the reweighting linearize of the members in the stage
+  // (planned by batch_plan_kernel from their phases), the stage kernels, then the stage's align as an inner loop of rounds.  After
+  // gnc_init, gnc_loops sets both conditions: the stages' while a member has a stage to go, the rounds' while a member's align has a round
+  // to go.
+  RoundWeights weights(ctx);
+  const auto stage = [&](cudaGraphConditionalHandle stages) {
+    cudaGraphConditionalHandle rounds;
+    if (int rc = loop_handle(ctx, who, nullptr, &rounds)) return rc;
+    CU(launch_gnc_reweigh(nb, gp.live, phase, rounds, ctx->stream));
+    weights.use(nullptr);
+    if (int rc = round_head(ctx, o, stages, &rows)) return rc;
+    CU(launch_gnc_rmax(gp, true, ctx->sm_count, ctx->stream));
+    CU(launch_gnc_stage(gp, ctx->stream));
+    CU(launch_gnc_weight(gp, ctx->sm_count, ctx->stream));
+    CU(launch_gnc_init(gp, ao, state, poses, phase, ctx->stream));
+    CU(launch_gnc_loops(nb, gp.live, phase, stages, rounds, ctx->stream));
+    weights.use(gp.wstage);
+    return capture_loop(ctx, rounds, round_loop(ctx, o, [&](cudaGraphConditionalHandle h) {
+                          CU(launch_gnc_step(gp, ao, true, ctx->b_round.as<BatchRound>(), h, ctx->b_out.as<double>(), state, poses, phase, ctx->stream));
+                          return 0;
+                        }));
+  };
+  std::vector<unsigned char> key;
+  if (!capturing) {  // loop_key, plus the GNC options and every buffer the GNC kernels use
+    key = loop_key(ctx, o);
+    for (int v : {gp.kind, gp.max_stages, gp.stage_iterations}) key_add(key, v);
+    key_add(key, gp.c2);
+    for (const void* v : {static_cast<const void*>(gp.member_off), static_cast<const void*>(gp.perm), static_cast<const void*>(gp.corr),
+                          static_cast<const void*>(gp.e), static_cast<const void*>(gp.w), static_cast<const void*>(gp.wstage),
+                          static_cast<const void*>(gp.gnc)})
+      key_add(key, v);
+  }
+  if (int rc = launch_loop(ctx, who, capturing, std::move(key), ctx->gnc_exec, ctx->gnc_key, stage)) return rc;
+  ctx->launches += 1;
+  if (int rc = clear_search_counters(ctx)) return rc;
+  CU(launch_batch_align_finish(nb, state, d_out_T, d_out_info, d_out_Hb, ctx->stream));
+  CU(launch_gnc_finish(nb, state, gp.gnc, d_out_info, d_out_gnc2, ctx->stream));
+  if (d_out_point_w && n) CU(cudaMemcpyAsync(d_out_point_w, gp.e, n * sizeof(double), cudaMemcpyDeviceToDevice, ctx->stream));
+  ctx->b_dseed_ok = true;
+  // stage 0's reweighting round linearised every member, as sgb_align_batch_gnc's does; every round since used robust_kind (NONE)
+  std::fill(ctx->b_lin.begin(), ctx->b_lin.end(), 1);
+  std::fill(ctx->b_seeded.begin(), ctx->b_seeded.end(), 1);
+  ctx->have_lin = true;
+  ctx->corr_seeds = true;
+  ctx->lin_factor = o->factor_kind;
+  ctx->lin_robust = o->robust_kind;
+  ctx->lin_c = o->robust_c;
   return 0;
 }
 
@@ -1407,7 +1558,9 @@ int sgb_align_batch_async(sgb_ctx* ctx, const sgb_align_options* o, const double
                            ctx->b_phase.as<uint8_t>(), ctx->stream));
       return 0;
     };
-    if (int rc = launch_loop(ctx, who, o, capturing, capturing ? std::vector<unsigned char>() : loop_key(ctx, o), ctx->align_exec, ctx->align_key, step)) return rc;
+    if (int rc = launch_loop(ctx, who, capturing, capturing ? std::vector<unsigned char>() : loop_key(ctx, o), ctx->align_exec, ctx->align_key,
+                             round_loop(ctx, o, step)))
+      return rc;
     ctx->launches += 1;
     if (int rc = clear_search_counters(ctx)) return rc;
   }
@@ -1483,7 +1636,7 @@ int sgb_align_joint_async(sgb_ctx* ctx, const sgb_align_options* o, size_t n_win
       key_add(key, J);
       for (size_t v : {K, static_cast<size_t>(L.max_free)}) key_add(key, v);
     }
-    if (int rc = launch_loop(ctx, who, o, capturing, std::move(key), ctx->joint_exec, ctx->joint_key, step)) return rc;
+    if (int rc = launch_loop(ctx, who, capturing, std::move(key), ctx->joint_exec, ctx->joint_key, round_loop(ctx, o, step))) return rc;
     ctx->launches += 1;
     if (int rc = clear_search_counters(ctx)) return rc;
   }

@@ -233,6 +233,7 @@ struct sgb_ctx {
   sgb::DevBuf b_round, b_dseed;
   bool b_dseed_ok = false;
   cudaStream_t cap_stream = nullptr;
+  cudaStream_t cap_stream_nested = nullptr;  // the stream the body of a loop nested in a loop's body is captured on
   cudaGraphExec_t align_exec = nullptr;
   std::vector<unsigned char> align_key;
   // sgb_align_joint: the buffers of its JointParams.  sgb_align_joint_async has its own (joint_async), which no other call writes: its
@@ -242,6 +243,9 @@ struct sgb_ctx {
   std::vector<uint32_t> ja_tab;
   cudaGraphExec_t joint_exec = nullptr;
   std::vector<unsigned char> joint_key;
+  // sgb_align_batch_gnc_async: its instantiated loop of stages, with its key (it uses g_w, g_e and g_state as sgb_align_batch_gnc does)
+  cudaGraphExec_t gnc_exec = nullptr;
+  std::vector<unsigned char> gnc_key;
 };
 
 namespace sgb {
