@@ -5,6 +5,7 @@
  * One context = one GPU = one CUDA stream.  A context is NOT thread-safe; distinct contexts are
  * (the reference runs several align() calls concurrently from TBB flow-graph nodes,
  * src/benchmark/odometry_benchmark_small_gicp_tbb_flow.cpp:81-98 -- give each its own context).
+ * Distinct contexts may also be on distinct devices of one process, used at the same time.
  *
  * Every entry point returns 0 on success and a non-zero code on failure; sgb_last_error() then
  * returns a description.  There is NO CPU fallback: without a CUDA device sgb_create() fails.

@@ -956,10 +956,8 @@ cudaError_t launch_joint_step(const AlignOptions& o, const JointParams& J, int m
                               uint8_t* member_phase, const double* out, cudaStream_t st) {
   const auto kernel = round ? joint_step_kernel<true> : joint_step_kernel<false>;
   const size_t smem = joint_step_smem(max_free);
-  if (smem > 48 * 1024) {
-    const cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
-    if (e != cudaSuccess) return e;
-  }
+  const cudaError_t e = allow_dynamic_smem(kernel, smem);
+  if (e != cudaSuccess) return e;
   kernel<<<J.n_windows, kJointBlock, smem, st>>>(o, J, linearize, out, round, loop, member_phase);
   return cudaGetLastError();
 }

@@ -413,11 +413,7 @@ cudaError_t launch_forest_build(const ForestBuild& b, cudaStream_t st, int* laun
     count += 6;
   }
   // every (map, segment) below: one CTA each
-  static bool configured = false;
-  if (!configured) {
-    if ((e = cudaFuncSetAttribute(forest_refine_smem_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(kKdRefineSmem))) != cudaSuccess) return e;
-    configured = true;
-  }
+  if ((e = allow_dynamic_smem(forest_refine_smem_kernel, kKdRefineSmem)) != cudaSuccess) return e;
   forest_refine_smem_kernel<<<b.n_segments, 1024, kKdRefineSmem, st>>>(b.leaf_pts, b.perm, F);
   count += 1;
   if (b.orig_normals || b.orig_covA) {

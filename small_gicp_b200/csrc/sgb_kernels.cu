@@ -172,10 +172,8 @@ static cudaError_t launch_lin(const LinParams& P, bool voxel, int grid, size_t s
     linearize_vox_kernel<(FACTOR == 1 ? 0 : FACTOR), ROBUST><<<grid, kLinBlock, 0, st>>>(P);
   } else {
 #ifdef SGB_PROFILING
-    if (smem > 48 * 1024) {
-      cudaError_t e = cudaFuncSetAttribute(linearize_kd_kernel<FACTOR, ROBUST>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
-      if (e != cudaSuccess) return e;
-    }
+    const cudaError_t e = allow_dynamic_smem(linearize_kd_kernel<FACTOR, ROBUST>, smem);
+    if (e != cudaSuccess) return e;
     linearize_kd_kernel<FACTOR, ROBUST><<<grid, kLinBlock, smem, st>>>(P);
 #else
     return cudaErrorNotSupported;  // point targets go through the search + factor kernels (sgb_grid.cu, sgb_kernels_packet.cu, sgb_kernels_split.cu)
@@ -222,17 +220,40 @@ int linearize_occupancy(int stack_depth) {
   return ctas_per_sm(linearize_vox_kernel<2, 0>, kLinBlock, 0, false, false);
 }
 
+// Kernel attributes belong to the kernel on a device, not to a context: every context of the process on that device shares them.  One mutex
+// guards both caches below, and the dynamic shared-memory limit only ever grows, so a launch at or below the limit it asked for can never be
+// undercut by another thread lowering it between that thread's set and its launch.
+static std::mutex g_attr_mu;
+static std::map<std::pair<int, const void*>, size_t> g_smem_limit;  // (device, kernel) -> largest opt-in limit set so far
+
+static cudaError_t allow_dynamic_smem_locked(int device, const void* kernel, size_t bytes) {
+  if (bytes <= 48 * 1024) return cudaSuccess;  // within every kernel's default limit
+  size_t& limit = g_smem_limit[std::make_pair(device, kernel)];
+  if (bytes <= limit) return cudaSuccess;
+  const cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(bytes));
+  if (e == cudaSuccess) limit = bytes;
+  return e;
+}
+
+cudaError_t allow_dynamic_smem(const void* kernel, size_t bytes) {
+  if (bytes <= 48 * 1024) return cudaSuccess;
+  int device = 0;
+  cudaError_t e = cudaGetDevice(&device);
+  if (e != cudaSuccess) return e;
+  const std::lock_guard<std::mutex> lock(g_attr_mu);
+  return allow_dynamic_smem_locked(device, kernel, bytes);
+}
+
 int ctas_per_sm(const void* kernel, int block, size_t smem, bool max_shared_carveout, bool smem_limit) {
-  static std::mutex mu;
   static std::map<std::tuple<int, const void*, int, size_t>, int> cache;
   int device = 0;
   cudaGetDevice(&device);
   const auto key = std::make_tuple(device, kernel, block, smem);
-  const std::lock_guard<std::mutex> lock(mu);
+  const std::lock_guard<std::mutex> lock(g_attr_mu);
   const auto it = cache.find(key);
   if (it != cache.end()) return it->second;
   if (max_shared_carveout) cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-  if (smem_limit) cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
+  if (smem_limit) allow_dynamic_smem_locked(device, kernel, smem);
   int nb = 0;
   if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, kernel, block, smem) != cudaSuccess || nb < 1) nb = 1;
   cache.emplace(key, nb);
@@ -601,12 +622,8 @@ uint32_t kd_smem_first_level(uint32_t n, uint32_t levels) {
 }
 cudaError_t launch_kd_refine_smem(float4* leaf_pts, uint32_t* perm, uint32_t n, uint32_t level0, uint32_t levels, cudaStream_t st) {
   if (level0 >= levels) return cudaSuccess;
-  static bool configured = false;
-  if (!configured) {
-    cudaError_t e = cudaFuncSetAttribute(kd_refine_smem_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(kKdRefineSmem));
-    if (e != cudaSuccess) return e;
-    configured = true;
-  }
+  const cudaError_t e = allow_dynamic_smem(kd_refine_smem_kernel, kKdRefineSmem);
+  if (e != cudaSuccess) return e;
   kd_refine_smem_kernel<<<1u << level0, 1024, kKdRefineSmem, st>>>(leaf_pts, perm, n, level0, levels);
   return cudaGetLastError();
 }

@@ -57,9 +57,17 @@ inline Ret dispatch_factor_robust(int factor, int robust, Ret invalid, Fn&& fn) 
   }
 }
 
+/// Lets `kernel` launch on the current device with `bytes` of dynamic shared memory: the one place that sets its opt-in limit.  The limit is
+/// per (device, kernel) and shared by every context of the process, so it is only ever raised, never lowered, under one mutex; a launch at or
+/// below the size it allowed stays valid whatever other threads allow meanwhile.  Nothing to do up to 48 KiB.
+cudaError_t allow_dynamic_smem(const void* kernel, size_t bytes);
+template <typename... KArgs>
+inline cudaError_t allow_dynamic_smem(void (*kernel)(KArgs...), size_t bytes) {
+  return allow_dynamic_smem(reinterpret_cast<const void*>(kernel), bytes);
+}
 /// Resident CTAs per SM (at least 1) of `kernel` launched with `block` threads and `smem` bytes of dynamic shared memory, asked once per
 /// device, kernel, block and smem.  Before the query: max_shared_carveout prefers the largest shared-memory carveout, smem_limit raises the
-/// kernel's dynamic shared-memory limit to `smem` (needed beyond 48 KiB).
+/// kernel's dynamic shared-memory limit to at least `smem` through allow_dynamic_smem.
 int ctas_per_sm(const void* kernel, int block, size_t smem, bool max_shared_carveout, bool smem_limit);
 template <typename... KArgs>
 inline int ctas_per_sm(void (*kernel)(KArgs...), int block, size_t smem, bool max_shared_carveout, bool smem_limit) {

@@ -334,10 +334,8 @@ int search_occupancy(int stack_depth) {
 
 cudaError_t launch_search(const LinParams& P, int grid, int stack_depth, cudaStream_t st) {
   const size_t smem = static_cast<size_t>(stack_depth) * kLinBlock * sizeof(uint2);
-  if (smem > 48 * 1024) {
-    cudaError_t e = cudaFuncSetAttribute(nn_search_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
-    if (e != cudaSuccess) return e;
-  }
+  const cudaError_t e = allow_dynamic_smem(nn_search_kernel, smem);
+  if (e != cudaSuccess) return e;
   nn_search_kernel<<<grid, kLinBlock, smem, st>>>(P);
   return cudaGetLastError();
 }

@@ -272,10 +272,8 @@ static cudaError_t launch_forest_features_t(const float4* pnodes, const float4* 
                                             double* ond, double* ocd, int depth, const float4* lo, cudaStream_t st) {
   if (depth < 1) depth = 1;
   const size_t smem = static_cast<size_t>(depth) * kLinBlock * (sizeof(uint2) + sizeof(float));
-  if (smem > 48 * 1024) {
-    cudaError_t e = cudaFuncSetAttribute(forest_features_kernel<KMAX>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
-    if (e != cudaSuccess) return e;
-  }
+  const cudaError_t e = allow_dynamic_smem(forest_features_kernel<KMAX>, smem);
+  if (e != cudaSuccess) return e;
   const int grid = static_cast<int>((n + kLinBlock - 1) / kLinBlock);
   forest_features_kernel<KMAX><<<grid, kLinBlock, smem, st>>>(pnodes, pts, n, k, F.pt_off, F.node_base, F.n_maps, centres, mode, ond, ocd, depth, lo);
   return cudaGetLastError();
@@ -295,10 +293,8 @@ static cudaError_t launch_features_t(const float4* nodes, const float4* pts, uin
                                      double* ond, double* ocd, int depth, int leaf_order_out, cudaStream_t st, const float4* lo) {
   if (depth < 1) depth = 1;
   const size_t smem = static_cast<size_t>(depth) * kLinBlock * (sizeof(uint2) + sizeof(float));
-  if (smem > 48 * 1024) {
-    cudaError_t e = cudaFuncSetAttribute(features_kernel<KMAX>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
-    if (e != cudaSuccess) return e;
-  }
+  const cudaError_t e = allow_dynamic_smem(features_kernel<KMAX>, smem);
+  if (e != cudaSuccess) return e;
   const int grid = static_cast<int>((n + kLinBlock - 1) / kLinBlock);
   features_kernel<KMAX><<<grid, kLinBlock, smem, st>>>(nodes, pts, n, k, centre, mode, on, oa, ob, ond, ocd, leaf_order_out, depth, lo);
   return cudaGetLastError();
@@ -474,10 +470,8 @@ static cudaError_t launch_batch_knn_t(const float4* pnodes, const float4* pts, c
                                       unsigned long long* out_idx, double* out_d, int depth, cudaStream_t st) {
   if (depth < 1) depth = 1;
   const size_t smem = static_cast<size_t>(depth) * kLinBlock * (sizeof(uint2) + sizeof(float));
-  if (smem > 48 * 1024) {
-    cudaError_t e = cudaFuncSetAttribute(batch_knn_kernel<KMAX>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
-    if (e != cudaSuccess) return e;
-  }
+  const cudaError_t e = allow_dynamic_smem(batch_knn_kernel<KMAX>, smem);
+  if (e != cudaSuccess) return e;
   batch_knn_kernel<KMAX><<<(n + kLinBlock - 1) / kLinBlock, kLinBlock, smem, st>>>(pnodes, pts, reinterpret_cast<const double4*>(queries4), n, k, centre, out_idx,
                                                                                   out_d, depth);
   return cudaGetLastError();
@@ -497,10 +491,8 @@ template <int KMAX>
 static cudaError_t launch_forest_knn_t(const ForestKnn& P, uint32_t n, int k, unsigned long long* out_idx, double* out_d, int depth, cudaStream_t st) {
   if (depth < 1) depth = 1;
   const size_t smem = static_cast<size_t>(depth) * kLinBlock * (sizeof(uint2) + sizeof(float));
-  if (smem > 48 * 1024) {
-    cudaError_t e = cudaFuncSetAttribute(forest_knn_kernel<KMAX>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
-    if (e != cudaSuccess) return e;
-  }
+  const cudaError_t e = allow_dynamic_smem(forest_knn_kernel<KMAX>, smem);
+  if (e != cudaSuccess) return e;
   forest_knn_kernel<KMAX><<<(n + kLinBlock - 1) / kLinBlock, kLinBlock, smem, st>>>(P, n, k, out_idx, out_d, depth);
   return cudaGetLastError();
 }
