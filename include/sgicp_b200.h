@@ -428,6 +428,45 @@ int sgb_align_batch_gnc(sgb_ctx* ctx, const sgb_align_options* options, const sg
  *     fails. */
 int sgb_align_joint(sgb_ctx* ctx, const sgb_align_options* options, size_t n_windows, const size_t* window_off, const uint8_t* fixed /*or NULL*/,
                     const double* init_X16xK, double* out_X16xK, double* out_info4xW);
+/* The edge poses sgb_align_joint linearises at: per member p of the pairing (in member order), T_p = X_j^-1 X_i for its cloud i and map
+ * j, column-major 4x4 into out_T16xE, computed on the device by the joint align's own kernel and tables, so its bits are those of the
+ * poses the joint align and sgb_align_joint_gnc use (a host X_j^-1 X_i differs in the last bits).  The layout of the poses that
+ * sgb_linearize_batch_points takes.  X16xK and out_T16xE are host memory.  Checks and messages as sgb_align_joint's for the windows and
+ * the pairing (fixed frames do not enter); no pairing member: nothing to do.  1 launch. */
+int sgb_joint_edge_poses(sgb_ctx* ctx, size_t n_windows, const size_t* window_off, const double* X16xK, double* out_T16xE);
+/* Graduated non-convexity for joint windows: sgb_align_batch_gnc's stages with the window as the GNC unit, one mu annealing the window's
+ * whole objective.  Frames, windows, fixed flags, edges, targets and options as sgb_align_joint; gnc as sgb_align_batch_gnc.  Per window,
+ * stage s (s = 0, 1, ...) from its frames X_s (X_0 = init_X16xK):
+ *   1. Edge poses: every edge's T_e from X_s (sgb_joint_edge_poses' bits).
+ *   2. Reweighting linearize: one unweighted linearize of the window's edges at those poses, the options' factor and rejector, no robust
+ *      kernel.  A point with a correspondence has r_i^2 = 2 e_i; one without gets g_i = 0 for the stage.
+ *   3. Stage 0: r_max^2 = the largest r_i^2 over all the window's edges; mu_0 from it as in sgb_align_batch_gnc (TLS without outliers,
+ *      2 r_max^2 <= c^2, per window).  Later stages: the schedule's next mu.
+ *   4. Weights g_i of sgb_align_batch_gnc's formulas with the window's mu; the stage's align uses w_i g_i (w_i: the weight in force).
+ *   5. The stage is the window's last when GM's mu is 1, when TLS's weights are all binary over the whole window or it has no outliers, or
+ *      at s = max_stages - 1.
+ *   6. Joint align: sgb_align_joint's algorithm from X_s (a fresh start, lambda = init_lambda) with the stage's weights and max_iterations
+ *      = stage_iterations, or options->max_iterations at the last stage; its frames are X_{s+1}.
+ * Outputs (host memory; out_point_w may also be device memory of the context's GPU): out_X16xK the frames after the last stage (fixed
+ * frames bit for bit); out_info4xW per window converged, iterations summed over all stages, inliers and weighted error (summed over its
+ * edges) of the last stage; out_gnc2xW the stages run and the last mu; out_point_w each edge point's final g (without the weights in
+ * force) in the row layout of sgb_correspondences_batch.  Each window's results are bit-identical to this loop driven from the host on a
+ * context holding that window alone: sgb_source_set_weights(NULL), sgb_joint_edge_poses, sgb_linearize_batch_points at those poses (no
+ * robust kernel), the formulas, sgb_source_set_weights(w * g), sgb_align_joint (the exact-FP32-tie caveat above applies).  A window with
+ * no edge, which no such context can hold, returns its initial poses, not converged, 0 iterations, and the stage count and mu of r_max^2 =
+ * 0 (GM: 1 stage, mu 1; TLS: 1 stage, mu 0).  Afterwards the context is as sgb_align_joint leaves it after each window's last stage
+ * (sgb_correspondences_batch, sgb_error_batch on the edges), and the weights in force are unchanged.
+ * Launches: per stage 1 for the edge poses (whenever the call has an edge, even at a stage whose windows have none), the reweighting
+ * linearize round of the edges of the windows in the stage (its search launches, the factor kernel, the segment kernel; none when those
+ * windows have no edge), 1 for the largest residual (stage 0 only), 3 (mu and last stage, weights, joint_init), then the joint align's
+ * rounds as in sgb_align_joint, each ending with one joint step launch; plus 1 when the pairing's view of the target is rebuilt.  The host
+ * reads one byte per window per round, and one more per window per stage ("still in GNC").
+ * Fails with a message, enqueuing nothing, where sgb_align_batch_gnc refuses its GNC options (robust_kind != SGB_ROBUST_NONE, an invalid
+ * kind, noise_bound_sq not finite or <= 0, max_stages < 1, stage_iterations < 1), while the context's stream is being captured, and for
+ * everything sgb_align_joint refuses. */
+int sgb_align_joint_gnc(sgb_ctx* ctx, const sgb_align_options* options, const sgb_gnc_options* gnc, size_t n_windows, const size_t* window_off,
+                        const uint8_t* fixed /*or NULL*/, const double* init_X16xK, double* out_X16xK, double* out_info4xW, double* out_gnc2xW /*or NULL*/,
+                        double* out_point_w /*or NULL*/);
 /* sgb_align_batch enqueued on the context's stream (sgb_set_stream) with no host involvement after the call: the rounds are planned on
  * the device and driven by a CUDA graph whose conditional WHILE node repeats one round (planner, search, factor, per-member sums, step)
  * until no member has a round to go.  No host synchronisation, no device-to-host copy, no upload from pageable memory: the call returns

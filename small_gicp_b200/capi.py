@@ -109,6 +109,9 @@ _SIGNATURES = {
     "sgb_align_batch_gnc_async": (C.c_int, [_vp, C.POINTER(AlignOptions), C.POINTER(GncOptions), _dp, _dp, _dp, _dp, _dp, _dp]),
     "sgb_align_joint": (C.c_int, [_vp, C.POINTER(AlignOptions), C.c_size_t, C.POINTER(C.c_size_t), C.POINTER(C.c_uint8), _dp, _dp, _dp]),
     "sgb_align_joint_async": (C.c_int, [_vp, C.POINTER(AlignOptions), C.c_size_t, C.POINTER(C.c_size_t), C.POINTER(C.c_uint8), _dp, _dp, _dp]),
+    "sgb_joint_edge_poses": (C.c_int, [_vp, C.c_size_t, C.POINTER(C.c_size_t), _dp, _dp]),
+    "sgb_align_joint_gnc": (C.c_int, [_vp, C.POINTER(AlignOptions), C.POINTER(GncOptions), C.c_size_t, C.POINTER(C.c_size_t), C.POINTER(C.c_uint8), _dp,
+                                      _dp, _dp, _dp, _dp]),
     "sgb_estimate_features": (C.c_int, [_vp, C.c_size_t, _dp, C.c_int, _dp, _dp]),
     "sgb_target_estimate_features": (C.c_int, [_vp, C.c_int]),
     "sgb_source_estimate_features": (C.c_int, [_vp, C.c_int]),
@@ -174,6 +177,18 @@ class JointAlignResult:
         self.iterations = info4[:, 1].astype(np.int64)
         self.num_inliers = info4[:, 2].astype(np.int64)
         self.error = info4[:, 3].copy()
+
+
+class JointGncAlignResult(JointAlignResult):
+    """what Context.align_joint_gnc returns: the JointAlignResult fields of each window's last stage (iterations summed over its stages),
+    stages (W,) the stages it ran, mu (W,) the surrogate's shape at its last stage (TLS without outliers: 0), and point_w (N,) each edge
+    point's final GNC weight g in the layout of correspondences_batch (None unless requested)"""
+
+    def __init__(self, X16, info4, gnc2, point_w):
+        super().__init__(X16, info4)
+        self.stages = gnc2[:, 0].astype(np.int64)
+        self.mu = gnc2[:, 1].copy()
+        self.point_w = point_w
 
 
 class AsyncAlignResult:
@@ -741,18 +756,8 @@ class Context:
         X_j^-1 X_i.  init_X (K,4,4) row-major frame poses; windows: the window offsets (W + 1,) from 0 to K (None: one window of all
         frames); fixed (K,) flags of frames held at their initial pose (None: the first frame of each window); the other keywords as in
         align_batch.  The weights in force (set_source_weights, one per edge point) apply."""
-        X = np.asarray(init_X, dtype=np.float64)
-        K = self._cloud_offsets.size - 1 if hasattr(self, "_cloud_offsets") else 0
-        if X.shape != (K, 4, 4):
-            raise SgbError(f"align_joint: need ({K}, 4, 4) frame poses")
-        Xc = np.ascontiguousarray(X.transpose(0, 2, 1))
-        off = np.ascontiguousarray(np.array([0, K] if windows is None else windows, dtype=np.uintp).reshape(-1))
-        if off.size < 1:
-            raise SgbError("align_joint: windows needs at least one entry")
+        K, Xc, off, fx = self._joint_args(init_X, windows, fixed, "align_joint")
         W = off.size - 1
-        fx = None if fixed is None else np.ascontiguousarray(np.asarray(fixed).astype(np.uint8).reshape(-1))
-        if fx is not None and fx.size != K:
-            raise SgbError(f"align_joint: fixed needs {K} entries")
         o = AlignOptions(int(factor), int(robust), float(robust_c), int(rejector), float(max_dist_sq), int(optimizer), int(max_iterations), float(gn_lambda),
                          int(max_inner_iterations), float(init_lambda), float(lambda_factor), float(rotation_eps), float(translation_eps))
         o.dof_mask[:] = [1.0] * 6 if dof_mask is None else [float(x) for x in dof_mask]
@@ -761,6 +766,52 @@ class Context:
         self._check(self._L.sgb_align_joint(self._h, C.byref(o), W, off.ctypes.data_as(C.POINTER(C.c_size_t)),
                                             None if fx is None else fx.ctypes.data_as(C.POINTER(C.c_uint8)), _d(Xc), _d(out), _d(info)))
         return JointAlignResult(out[:K], info[:W])
+
+    def _joint_args(self, X, windows, fixed, who):
+        """the column-major frame poses, window offsets and fixed flags of a joint call"""
+        X = np.asarray(X, dtype=np.float64)
+        K = self._cloud_offsets.size - 1 if hasattr(self, "_cloud_offsets") else 0
+        if X.shape != (K, 4, 4):
+            raise SgbError(f"{who}: need ({K}, 4, 4) frame poses")
+        off = np.ascontiguousarray(np.array([0, K] if windows is None else windows, dtype=np.uintp).reshape(-1))
+        if off.size < 1:
+            raise SgbError(f"{who}: windows needs at least one entry")
+        fx = None if fixed is None else np.ascontiguousarray(np.asarray(fixed).astype(np.uint8).reshape(-1))
+        if fx is not None and fx.size != K:
+            raise SgbError(f"{who}: fixed needs {K} entries")
+        return K, np.ascontiguousarray(X.transpose(0, 2, 1)), off, fx
+
+    def joint_edge_poses(self, X, windows=None):
+        """The edge poses the joint aligns linearise at (sgb_joint_edge_poses) -> (E, 4, 4) row-major, T_p = X_j^-1 X_i for pairing member p
+        (cloud i against map j), computed on the device with the joint align's own kernel: bit for bit the poses align_joint and
+        align_joint_gnc use, ready for linearize_batch_points.  X (K,4,4) row-major frame poses; windows as in align_joint."""
+        K, Xc, off, _ = self._joint_args(X, windows, None, "joint_edge_poses")
+        E = self._batch_offsets.size - 1
+        out = np.zeros((max(E, 1), 16))
+        self._check(self._L.sgb_joint_edge_poses(self._h, off.size - 1, off.ctypes.data_as(C.POINTER(C.c_size_t)), _d(Xc), _d(out)))
+        return np.ascontiguousarray(out[:E].reshape(E, 4, 4).transpose(0, 2, 1))
+
+    def align_joint_gnc(self, init_X, noise_bound_sq, windows=None, fixed=None, gnc=GNC_TLS, max_stages=64, stage_iterations=3, point_weights=False,
+                        **align):
+        """Graduated non-convexity over joint windows (sgb_align_joint_gnc) -> a JointGncAlignResult.  Per window, each stage re-estimates every
+        edge point's weight g on the device from its residual r^2 = 2 e at the window's edge poses (one mu per window; gnc: GNC_GEMAN_MCCLURE
+        or GNC_TLS, noise_bound_sq = c^2 on that scale), then runs align_joint from there with the weights w * g (w: the weights in force,
+        which the call leaves unchanged) and max_iterations = stage_iterations, or align's max_iterations at the window's last stage.  At
+        most max_stages stages.  point_weights=True: each point's final g too.  init_X, windows and fixed as in align_joint; align: the
+        keywords of align_joint (robust must stay ROBUST_NONE)."""
+        K, Xc, off, fx = self._joint_args(init_X, windows, fixed, "align_joint_gnc")
+        W = off.size - 1
+        o = _align_options(**align)
+        g = GncOptions(int(gnc), float(noise_bound_sq), int(max_stages), int(stage_iterations))
+        out = np.zeros((max(K, 1), 16))
+        info = np.zeros((max(W, 1), 4))
+        gnc2 = np.zeros((max(W, 1), 2))
+        n = int(self._batch_offsets[-1]) if hasattr(self, "_batch_offsets") else 0
+        pw = np.zeros(max(n, 1)) if point_weights else None
+        self._check(self._L.sgb_align_joint_gnc(self._h, C.byref(o), C.byref(g), W, off.ctypes.data_as(C.POINTER(C.c_size_t)),
+                                                None if fx is None else fx.ctypes.data_as(C.POINTER(C.c_uint8)), _d(Xc), _d(out), _d(info), _d(gnc2),
+                                                _d(pw)))
+        return JointGncAlignResult(out[:K], info[:W], gnc2[:W], None if pw is None else pw[:n])
 
     def align_batch_async(self, init_Ts, factor=FACTOR_GICP, robust=ROBUST_NONE, robust_c=1.0, rejector=REJECT_DISTANCE, max_dist_sq=1.0,
                           optimizer=OPT_LEVENBERG_MARQUARDT, max_iterations=20, gn_lambda=1e-6, max_inner_iterations=10, init_lambda=1e-3,

@@ -24,6 +24,8 @@
 //                           GNC weight from its row of the reweighting linearize, each stage's align_init, and the step with each member's
 //                           stage iterations (sgb_align_batch_gnc_async: gnc_reweigh_kernel / gnc_loops_kernel / gnc_finish_kernel,
 //                           each stage's phases, the loops' conditions and the outputs)
+//   joint_gnc_*_kernel      sgb_align_joint_gnc: the same GNC with the window as its unit (each point's window through its edge), each
+//                           window's stage start (joint_init) and the joint step with each window's stage iterations
 // The transform, factor, segment and step kernels serve the rounds the host plans (sgb_{linearize,error,align}_batch, sgb_align_joint) and,
 // with ROUND / kModeRound, the rounds batch_plan_kernel plans on the device (sgb_align_batch_async, sgb_align_joint_async,
 // sgb_align_batch_gnc_async).
@@ -697,17 +699,34 @@ cudaError_t launch_batch_align_finish(uint32_t n_members, const MemberState* sta
 // the grid of a one-thread-per-stored-point GNC kernel (at least one CTA: the launch count does not depend on the point count)
 uint32_t gnc_point_grid(uint32_t n, int sm_count) { return std::max<uint32_t>(1u, std::min<uint32_t>((n + 255u) / 256u, static_cast<uint32_t>(sm_count) * 8u)); }
 
+// The GNC unit of member m, whose GncState and live flag its points use: the member itself (sgb_align_batch_gnc), or the window of the
+// edge it is (sgb_align_joint_gnc: win[m])
+struct GncMemberUnit {
+  __device__ __forceinline__ uint32_t operator()(uint32_t m) const { return m; }
+};
+struct GncWindowUnit {
+  const uint32_t* __restrict__ win;
+  __device__ __forceinline__ uint32_t operator()(uint32_t m) const { return __ldg(&win[m]); }
+};
+
+// every unit's largest r^2 over its points (the loop of gnc_rmax_kernel and joint_gnc_rmax_kernel)
+template <bool ROUND, typename Unit>
+__device__ __forceinline__ void gnc_rmax_points(const GncParams& p, Unit unit) {
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < p.n; i += gridDim.x * blockDim.x) {
+    const uint32_t m = owner_of(p.member_off, p.n_members, i);
+    const uint32_t u = unit(m);
+    if (!p.live[u] || p.corr[i] == kNone) continue;
+    if (ROUND && p.gnc[u].stages != 0) continue;
+    const double r2 = rn_mul(2.0, p.e[batch_row(p.member_off, p.perm, m, i)]);
+    // a non-negative double orders as its bit pattern; -0.0, rounding's tiny negatives and NaN never enter
+    if (r2 > 0.0) atomicMax(reinterpret_cast<unsigned long long*>(&p.gnc[u].r2max), static_cast<unsigned long long>(__double_as_longlong(r2)));
+  }
+}
+
 // ROUND (sgb_align_batch_gnc_async, launched at every stage of its loop): only the members before their stage 0 (no stage begun)
 template <bool ROUND>
 __global__ void gnc_rmax_kernel(const GncParams p) {
-  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < p.n; i += gridDim.x * blockDim.x) {
-    const uint32_t m = owner_of(p.member_off, p.n_members, i);
-    if (!p.live[m] || p.corr[i] == kNone) continue;
-    if (ROUND && p.gnc[m].stages != 0) continue;
-    const double r2 = rn_mul(2.0, p.e[batch_row(p.member_off, p.perm, m, i)]);
-    // a non-negative double orders as its bit pattern; -0.0, rounding's tiny negatives and NaN never enter
-    if (r2 > 0.0) atomicMax(reinterpret_cast<unsigned long long*>(&p.gnc[m].r2max), static_cast<unsigned long long>(__double_as_longlong(r2)));
-  }
+  gnc_rmax_points<ROUND>(p, GncMemberUnit{});
 }
 
 __global__ void __launch_bounds__(kStepBlock) gnc_stage_kernel(const GncParams p) {
@@ -716,21 +735,28 @@ __global__ void __launch_bounds__(kStepBlock) gnc_stage_kernel(const GncParams p
   gnc_stage_begin(p.kind, p.c2, p.max_stages, p.gnc[m]);
 }
 
-template <int KIND>
-__global__ void gnc_weight_kernel(const GncParams p) {
+// every point's g of its unit's stage (the loop of gnc_weight_kernel and joint_gnc_weight_kernel)
+template <int KIND, typename Unit>
+__device__ __forceinline__ void gnc_weight_points(const GncParams& p, Unit unit) {
   for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < p.n; i += gridDim.x * blockDim.x) {
     const uint32_t m = owner_of(p.member_off, p.n_members, i);
-    if (!p.live[m]) continue;
+    const uint32_t u = unit(m);
+    if (!p.live[u]) continue;
     const size_t row = batch_row(p.member_off, p.perm, m, i);
     double g = 0.0;
     if (p.corr[i] != kNone) {
-      const GncState& s = p.gnc[m];
+      const GncState& s = p.gnc[u];
       g = s.ones ? 1.0 : gnc_weight<KIND>(rn_mul(2.0, p.e[row]), s.mu, p.c2);
-      if (KIND == kGncTls && g != 0.0 && g != 1.0) atomicOr(&p.gnc[m].not_binary, 1u);
+      if (KIND == kGncTls && g != 0.0 && g != 1.0) atomicOr(&p.gnc[u].not_binary, 1u);
     }
     p.e[row] = g;
     p.wstage[i] = p.w ? rn_mul(__ldg(&p.w[i]), g) : g;
   }
+}
+
+template <int KIND>
+__global__ void gnc_weight_kernel(const GncParams p) {
+  gnc_weight_points<KIND>(p, GncMemberUnit{});
 }
 
 // the options of member m's align in the current stage
@@ -896,9 +922,8 @@ __global__ void joint_edge_poses_kernel(const __grid_constant__ JointParams J) {
 // round to go, a stepped window writes its new phase to its edges' member_phase (what the next round's planner reads) and sets `loop` too.
 constexpr int kJointBlock = 256;
 template <bool ROUND>
-__global__ void __launch_bounds__(kJointBlock) joint_step_kernel(const __grid_constant__ AlignOptions o, const __grid_constant__ JointParams J, bool linearize,
-                                                                 const double* __restrict__ out, const BatchRound* __restrict__ round,
-                                                                 cudaGraphConditionalHandle loop, uint8_t* __restrict__ member_phase) {
+__device__ __forceinline__ void joint_step_window(const AlignOptions& o, const JointParams& J, bool linearize, const double* __restrict__ out,
+                                                  const BatchRound* __restrict__ round, cudaGraphConditionalHandle loop, uint8_t* __restrict__ member_phase) {
   extern __shared__ double s_work[];
   const uint32_t w = blockIdx.x;
   const int tid = threadIdx.x, nt = blockDim.x;
@@ -944,6 +969,12 @@ __global__ void __launch_bounds__(kJointBlock) joint_step_kernel(const __grid_co
     for (int q = tid; q < win.n_edges; q += nt) member_phase[J.edge_member[e0 + q]] = static_cast<uint8_t>(ph);
     if (tid == 0 && (ph == kPhaseLinearize || ph == kPhaseTrial)) cudaGraphSetConditional(loop, 1u);
   }
+}
+template <bool ROUND>
+__global__ void __launch_bounds__(kJointBlock) joint_step_kernel(const __grid_constant__ AlignOptions o, const __grid_constant__ JointParams J, bool linearize,
+                                                                 const double* __restrict__ out, const BatchRound* __restrict__ round,
+                                                                 cudaGraphConditionalHandle loop, uint8_t* __restrict__ member_phase) {
+  joint_step_window<ROUND>(o, J, linearize, out, round, loop, member_phase);
 }
 
 cudaError_t launch_joint_edge_poses(const JointParams& J, cudaStream_t st) {
@@ -1014,6 +1045,71 @@ cudaError_t launch_joint_align_init(const AlignOptions& o, const JointParams& J,
 cudaError_t launch_joint_align_finish(const JointParams& J, uint32_t n_frames, const double* init_X16, double* out_X16, double* out_info4, cudaStream_t st) {
   const uint32_t n = std::max(n_frames, J.n_windows);
   joint_align_finish_kernel<<<(n + kStepBlock - 1) / kStepBlock, kStepBlock, 0, st>>>(J, n_frames, init_X16, out_X16, out_info4);
+  return cudaGetLastError();
+}
+
+// ---- sgb_align_joint_gnc (DESIGN.md §11 "Graduated non-convexity for joint windows"): the GNC unit is the window.  p.gnc and p.live are
+// per window; the point kernels reach a point's window through its member (edge), member_win[m] ----
+
+__global__ void joint_gnc_rmax_kernel(const GncParams p, const uint32_t* __restrict__ member_win) {
+  gnc_rmax_points<false>(p, GncWindowUnit{member_win});
+}
+
+template <int KIND>
+__global__ void joint_gnc_weight_kernel(const GncParams p, const uint32_t* __restrict__ member_win) {
+  gnc_weight_points<KIND>(p, GncWindowUnit{member_win});
+}
+
+// One thread per window (p.n_members = the windows), as gnc_init_kernel per member: a window in the stage ends GNC after it if the stage
+// is its last (TLS: or its weights are all binary), adds the previous stage's iterations and starts its joint align from its current X
+// (joint_init with max_iterations = stage_iterations unless last); every other window is left done.  Its edges' poses are those of its X
+// already: the stage's reweighting linearize ran at them.
+__global__ void __launch_bounds__(kStepBlock) joint_gnc_init_kernel(const GncParams p, const __grid_constant__ AlignOptions o, const __grid_constant__ JointParams J) {
+  const uint32_t w = blockIdx.x * kStepBlock + threadIdx.x;
+  if (w >= J.n_windows) return;
+  WindowState& s = J.state[w];
+  if (!p.live[w]) {  // finished earlier: its state holds its last stage's result
+    s.phase = kPhaseDone;
+    J.phase[w] = kPhaseDone;
+    return;
+  }
+  GncState& g = p.gnc[w];
+  if (p.kind == kGncTls && !g.not_binary) g.last = 1;
+  p.live[w] = g.last ? 0 : 1;
+  g.iterations += s.iterations;
+  joint_init(gnc_stage_options(o, p, w), static_cast<int>(J.n_free[w]), static_cast<int>(J.edge_off[w + 1] - J.edge_off[w]), s);
+  J.phase[w] = static_cast<uint8_t>(s.phase);
+}
+
+// joint_step_kernel<false> for a round of a GNC stage: each window steps with its stage's max_iterations (as joint_gnc_init_kernel chose)
+__global__ void __launch_bounds__(kJointBlock) joint_gnc_step_kernel(const __grid_constant__ AlignOptions o, const __grid_constant__ JointParams J, bool linearize,
+                                                                     const double* __restrict__ out, const GncParams p) {
+  joint_step_window<false>(gnc_stage_options(o, p, blockIdx.x), J, linearize, out, nullptr, 0, nullptr);
+}
+
+cudaError_t launch_joint_gnc_rmax(const GncParams& p, const uint32_t* member_win, int sm_count, cudaStream_t st) {
+  joint_gnc_rmax_kernel<<<gnc_point_grid(p.n, sm_count), 256, 0, st>>>(p, member_win);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_joint_gnc_weight(const GncParams& p, const uint32_t* member_win, int sm_count, cudaStream_t st) {
+  if (p.kind == kGncTls)
+    joint_gnc_weight_kernel<kGncTls><<<gnc_point_grid(p.n, sm_count), 256, 0, st>>>(p, member_win);
+  else
+    joint_gnc_weight_kernel<kGncGemanMcClure><<<gnc_point_grid(p.n, sm_count), 256, 0, st>>>(p, member_win);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_joint_gnc_init(const GncParams& pw, const AlignOptions& o, const JointParams& J, cudaStream_t st) {
+  joint_gnc_init_kernel<<<(J.n_windows + kStepBlock - 1) / kStepBlock, kStepBlock, 0, st>>>(pw, o, J);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_joint_gnc_step(const AlignOptions& o, const JointParams& J, int max_free, bool linearize, const double* out, const GncParams& pw, cudaStream_t st) {
+  const size_t smem = joint_step_smem(max_free);
+  const cudaError_t e = allow_dynamic_smem(joint_gnc_step_kernel, smem);
+  if (e != cudaSuccess) return e;
+  joint_gnc_step_kernel<<<J.n_windows, kJointBlock, smem, st>>>(o, J, linearize, out, pw);
   return cudaGetLastError();
 }
 

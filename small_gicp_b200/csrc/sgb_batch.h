@@ -240,4 +240,17 @@ cudaError_t launch_joint_align_init(const AlignOptions& o, const JointParams& J,
 /// (converged, iterations, inliers, error) per window
 cudaError_t launch_joint_align_finish(const JointParams& J, uint32_t n_frames, const double* init_X16, double* out_X16, double* out_info4, cudaStream_t st);
 
+// ---- sgb_align_joint_gnc (DESIGN.md §11 "Graduated non-convexity for joint windows"): sgb_align_batch_gnc's stages with the window as the
+// GNC unit.  GncState and live flags per window: p (the point kernels) has n_members = the edges, each point's window member_win[its edge];
+// pw (the window kernels, and launch_gnc_stage) the same with n_members = the windows. ----
+/// stage 0: every window's largest r^2 = 2 e_i > 0 over its edges' points with a correspondence (gnc[w].r2max, cleared by the caller)
+cudaError_t launch_joint_gnc_rmax(const GncParams& p, const uint32_t* member_win, int sm_count, cudaStream_t st);
+/// launch_gnc_weight with each point's window's mu (TLS: not_binary per window)
+cudaError_t launch_joint_gnc_weight(const GncParams& p, const uint32_t* member_win, int sm_count, cudaStream_t st);
+/// launch_gnc_init per window: joint_init of a window in the stage from its current X (max_iterations = stage_iterations unless last),
+/// its phase to J.phase; every other window is left done
+cudaError_t launch_joint_gnc_init(const GncParams& pw, const AlignOptions& o, const JointParams& J, cudaStream_t st);
+/// launch_joint_step of a host-planned round of a GNC stage: each window steps with its stage's max_iterations
+cudaError_t launch_joint_gnc_step(const AlignOptions& o, const JointParams& J, int max_free, bool linearize, const double* out, const GncParams& pw, cudaStream_t st);
+
 }  // namespace sgb

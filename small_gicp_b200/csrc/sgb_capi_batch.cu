@@ -1,7 +1,7 @@
 // SPDX-License-Identifier: MIT
 // C-ABI of batched registration (include/sgicp_b200.h: sgb_source_set_batch, sgb_source_set_pairs, sgb_source_set_submaps,
 // sgb_source_set_weights, sgb_{linearize,error,align,correspondences}_batch, sgb_{linearize,error}_batch_points, sgb_align_batch_async, sgb_align_joint,
-// sgb_align_joint_async, sgb_align_batch_gnc, sgb_align_batch_gnc_async).
+// sgb_align_joint_async, sgb_align_batch_gnc, sgb_align_batch_gnc_async, sgb_joint_edge_poses, sgb_align_joint_gnc).
 // Kernels in sgb_batch.cu (many kd-trees and submaps: the searches in sgb_forest.cu); DESIGN.md §11.
 #include <cuda_runtime.h>
 
@@ -858,10 +858,8 @@ struct RoundWeights {
   void use(const double* w) { ctx->b_wuse = w; }
 };
 
-// The checks both GNC aligns make before anything is enqueued (who names the caller): align_checks', then the GNC options'
-int gnc_checks(sgb_ctx* ctx, const std::string& who, const sgb_align_options* o, const sgb_gnc_options* gnc, const double* init_T, const double* out_T,
-               const double* out_info, AlignOptions& ao) {
-  if (int rc = align_checks(ctx, who.c_str(), o, init_T, out_T, out_info, ao)) return rc;
+// The checks of the GNC options every GNC align makes (who names the caller), after those of its align
+int gnc_option_checks(sgb_ctx* ctx, const std::string& who, const sgb_align_options* o, const sgb_gnc_options* gnc) {
   if (!gnc) return fail(ctx, 1, who + ": null GNC options");
   if (o->robust_kind != SGB_ROBUST_NONE)
     return fail(ctx, 1, who + ": robust_kind must be SGB_ROBUST_NONE: the GNC weights are the robust kernel (a fixed-width kernel on top would change the cost "
@@ -870,6 +868,23 @@ int gnc_checks(sgb_ctx* ctx, const std::string& who, const sgb_align_options* o,
   if (!(std::isfinite(gnc->noise_bound_sq) && gnc->noise_bound_sq > 0.0)) return fail(ctx, 1, who + ": noise_bound_sq must be finite and > 0");
   if (gnc->max_stages < 1) return fail(ctx, 1, who + ": max_stages must be >= 1");
   if (gnc->stage_iterations < 1) return fail(ctx, 1, who + ": stage_iterations must be >= 1");
+  return 0;
+}
+
+// The checks both batch GNC aligns make before anything is enqueued (who names the caller): align_checks', then the GNC options'
+int gnc_checks(sgb_ctx* ctx, const std::string& who, const sgb_align_options* o, const sgb_gnc_options* gnc, const double* init_T, const double* out_T,
+               const double* out_info, AlignOptions& ao) {
+  if (int rc = align_checks(ctx, who.c_str(), o, init_T, out_T, out_info, ao)) return rc;
+  return gnc_option_checks(ctx, who, o, gnc);
+}
+
+// A synchronous GNC call refuses a captured stream: it synchronises at every round and stage to plan the next one
+int gnc_capture_check(sgb_ctx* ctx, const std::string& who) {
+  cudaStreamCaptureStatus capture = cudaStreamCaptureStatusNone;
+  CU(cudaStreamIsCapturing(ctx->stream, &capture));
+  if (capture != cudaStreamCaptureStatusNone)
+    return fail(ctx, 1, who + ": the context's stream is being captured, and the call synchronises at every round and stage to plan the next one; call it "
+                              "outside the capture");
   return 0;
 }
 
@@ -1145,11 +1160,7 @@ int sgb_align_batch_gnc(sgb_ctx* ctx, const sgb_align_options* o, const sgb_gnc_
   AlignOptions ao;
   if (int rc = gnc_checks(ctx, who, o, gnc, init_T, out_T, out_info, ao)) return rc;
   CU(cudaSetDevice(ctx->device));
-  cudaStreamCaptureStatus capture = cudaStreamCaptureStatusNone;
-  CU(cudaStreamIsCapturing(ctx->stream, &capture));
-  if (capture != cudaStreamCaptureStatusNone)
-    return fail(ctx, 1, who + ": the context's stream is being captured, and the call synchronises at every round and stage to plan the next one; call it "
-                              "outside the capture");
+  if (int rc = gnc_capture_check(ctx, who)) return rc;
   const size_t B = batch_members(ctx), n = batch_points(ctx);
   if (B == 0) return 0;
   if (int rc = pair_view(ctx)) return rc;
@@ -1320,7 +1331,8 @@ namespace {
 
 // What both joint aligns build from their arguments: the window tables, each window's free frame and edge counts, and the most free
 // frames of a window with an edge (which sizes the step's shared memory).  tab = frame_off [W + 1] | edge_off [W + 1] | n_free [W] |
-// edge_member [E] | edge_win [E] | edge_i [E] | edge_j [E] | free [K], the layout JointParams reads.
+// edge_member [E] | edge_win [E] | edge_i [E] | edge_j [E] | free [K], the layout JointParams reads, then member_win [E] (the window of
+// member p, which sgb_align_joint_gnc's point kernels read).
 struct JointLayout {
   size_t W = 0, K = 0, E = 0;
   std::vector<uint32_t> tab, n_free, edge_count;
@@ -1328,11 +1340,13 @@ struct JointLayout {
   const uint32_t* edge_member() const { return tab.data() + 3 * W + 2; }
   const uint32_t* edge_win() const { return edge_member() + E; }
   const int32_t* free() const { return reinterpret_cast<const int32_t*>(edge_win() + 3 * E); }
+  size_t member_win_at() const { return tab.size() - E; }  // (in uint32_t of tab)
 };
 
-// The checks both joint aligns make before anything is enqueued (who names the caller), and their layout
+// The checks every joint call makes before anything is enqueued (who names the caller), and their layout.  align = false: no align
+// (sgb_joint_edge_poses; o, out_info and ao unused), the checks of the windows and the pairing alone.
 int joint_layout(sgb_ctx* ctx, const std::string& who, const sgb_align_options* o, size_t n_windows, const size_t* window_off, const uint8_t* fixed,
-                 const double* init_X, const double* out_X, const double* out_info, AlignOptions& ao, JointLayout& L) {
+                 const double* init_X, const double* out_X, const double* out_info, AlignOptions& ao, JointLayout& L, bool align = true) {
   if (ctx->src_state != SourceState::Batch) return fail(ctx, 1, who + ": the context holds no batch of sources (call sgb_source_set_batch)");
   if (ctx->b_submaps) return fail(ctx, 1, who + ": the members are submap members (sgb_source_set_submaps); joint windows need (cloud, map) edges");
   if (!ctx->b_paired || !ctx->b_pair_has_maps)
@@ -1344,7 +1358,11 @@ int joint_layout(sgb_ctx* ctx, const std::string& who, const sgb_align_options* 
   if (K != target_maps(ctx))
     return fail(ctx, 1, who + ": frame k is cloud k with map k, but the batch holds " + std::to_string(K) + " clouds and the target " +
                             std::to_string(target_maps(ctx)) + " maps");
-  if (int rc = align_checks(ctx, who.c_str(), o, init_X, out_X, out_info, ao)) return rc;
+  if (align) {
+    if (int rc = align_checks(ctx, who.c_str(), o, init_X, out_X, out_info, ao)) return rc;
+  } else if (!init_X || !out_X) {
+    return fail(ctx, 1, who + ": null poses or output");
+  }
   if (!window_off) return fail(ctx, 1, who + ": null window offsets");
   if (n_windows > SGB_BATCH_MAX_MEMBERS)
     return fail(ctx, 1, who + ": " + std::to_string(n_windows) + " windows, at most " + std::to_string(SGB_BATCH_MAX_MEMBERS));
@@ -1379,7 +1397,7 @@ int joint_layout(sgb_ctx* ctx, const std::string& who, const sgb_align_options* 
       return fail(ctx, 1, who + ": window " + std::to_string(w) + " has edges but no fixed frame (its gauge would be free)");
   }
   const size_t W = n_windows;
-  std::vector<uint32_t> tab(2 * (W + 1) + W + 4 * E + K);
+  std::vector<uint32_t> tab(2 * (W + 1) + W + 5 * E + K);
   uint32_t* frame_off = tab.data();
   uint32_t* edge_off = frame_off + W + 1;
   uint32_t* nf = edge_off + W + 1;
@@ -1388,6 +1406,7 @@ int joint_layout(sgb_ctx* ctx, const std::string& who, const sgb_align_options* 
   int32_t* edge_i = reinterpret_cast<int32_t*>(edge_win + E);
   int32_t* edge_j = edge_i + E;
   int32_t* freeidx = edge_j + E;
+  uint32_t* member_win = reinterpret_cast<uint32_t*>(freeidx + K);
   for (size_t w = 0; w <= W; w++) frame_off[w] = static_cast<uint32_t>(window_off[w]);
   edge_off[0] = 0;
   for (size_t w = 0; w < W; w++) edge_off[w + 1] = edge_off[w] + edge_count[w];
@@ -1396,6 +1415,7 @@ int joint_layout(sgb_ctx* ctx, const std::string& who, const sgb_align_options* 
     const uint32_t i = ctx->b_pair_clouds[p], j = ctx->b_pair_maps[p], w = win_of[i], q = fill[w]++;
     edge_member[q] = static_cast<uint32_t>(p);
     edge_win[q] = w;
+    member_win[p] = w;
     edge_i[q] = static_cast<int32_t>(i - window_off[w]);
     edge_j[q] = static_cast<int32_t>(j - window_off[w]);
   }
@@ -1446,6 +1466,47 @@ JointParams joint_params(sgb_ctx* ctx, const JointBufs& b, size_t W, size_t E) {
   return J;
 }
 
+// The rounds of sgb_align_joint from the windows' phases (read back after each round), in lockstep as in sgb_align_batch, per window:
+// error() for the edges of every window with a pending trial until none has one, else a linearize of the edges of every window still
+// iterating; each round ends with one joint step launch, step(lin).
+template <typename Step>
+int joint_rounds(sgb_ctx* ctx, const sgb_align_options* o, const JointLayout& L, std::vector<uint8_t>& phase, Step step) {
+  const size_t W = L.W, E = L.E;
+  const uint32_t* edge_member = L.edge_member();
+  const uint32_t* edge_win = L.edge_win();
+  std::vector<uint8_t> active(E);
+  for (;;) {
+    bool any_trial = false, any_lin = false;
+    for (size_t w = 0; w < W; w++) {
+      any_trial |= phase[w] == kPhaseTrial;
+      any_lin |= phase[w] == kPhaseLinearize;
+    }
+    if (!any_trial && !any_lin) return 0;
+    const bool lin = !any_trial;
+    for (size_t q = 0; q < E; q++) active[edge_member[q]] = phase[edge_win[q]] == (lin ? kPhaseLinearize : kPhaseTrial);
+    if (lin) {
+      if (int rc = linearize_round(ctx, o->factor_kind, o->robust_kind, o->robust_c, o->rejector_kind, o->max_dist_sq, nullptr, active.data())) return rc;
+    } else {
+      if (int rc = error_round(ctx, nullptr, active.data())) return rc;
+    }
+    CU(step(lin));
+    ctx->launches += 1;
+    CU(cudaMemcpyAsync(phase.data(), ctx->joint.phase.p, W, cudaMemcpyDeviceToHost, ctx->stream));
+    CU(cudaStreamSynchronize(ctx->stream));
+  }
+}
+
+// The window tables of layout L and the frames' X (host memory, column-major) uploaded to ctx->joint, its buffers reserved for L
+int joint_upload(sgb_ctx* ctx, const JointLayout& L, const double* X) {
+  const std::vector<size_t> bytes = joint_bytes(L);
+  const std::vector<DevBuf*> bufs = joint_buffers(ctx->joint);
+  for (size_t i = 0; i < bufs.size(); i++) CU(bufs[i]->reserve(bytes[i]));
+  // pageable host memory: the copies are staged before cudaMemcpyAsync returns
+  CU(cudaMemcpyAsync(ctx->joint.tables.p, L.tab.data(), L.tab.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
+  if (L.K) CU(cudaMemcpyAsync(ctx->joint.X.p, X, L.K * 16 * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
+  return 0;
+}
+
 }  // namespace
 
 extern "C" {
@@ -1467,13 +1528,8 @@ int sgb_align_joint(sgb_ctx* ctx, const sgb_align_options* o, size_t n_windows, 
     joint_init(ao, static_cast<int>(L.n_free[w]), static_cast<int>(L.edge_count[w]), state[w]);
     phase[w] = static_cast<uint8_t>(state[w].phase);
   }
-  const std::vector<size_t> bytes = joint_bytes(L);
-  const std::vector<DevBuf*> bufs = joint_buffers(ctx->joint);
-  for (size_t i = 0; i < bufs.size(); i++) CU(bufs[i]->reserve(bytes[i]));
+  if (int rc = joint_upload(ctx, L, init_X)) return rc;
   const JointParams J = joint_params(ctx, ctx->joint, W, E);
-  // pageable host memory: the copies are staged before cudaMemcpyAsync returns
-  CU(cudaMemcpyAsync(ctx->joint.tables.p, L.tab.data(), L.tab.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
-  if (K) CU(cudaMemcpyAsync(ctx->joint.X.p, init_X, K * 16 * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
   if (W) {  // the phases too: a window done from the start is never stepped, and the host reads every window's phase after each round
     CU(cudaMemcpyAsync(ctx->joint.state.p, state.data(), W * sizeof(WindowState), cudaMemcpyHostToDevice, ctx->stream));
     CU(cudaMemcpyAsync(ctx->joint.phase.p, phase.data(), W, cudaMemcpyHostToDevice, ctx->stream));
@@ -1482,30 +1538,10 @@ int sgb_align_joint(sgb_ctx* ctx, const sgb_align_options* o, size_t n_windows, 
     CU(launch_joint_edge_poses(J, ctx->stream));
     ctx->launches += 1;
   }
-  // Rounds in lockstep as in sgb_align_batch, per window: error() for the edges of every window with a pending trial until none has one,
-  // else a linearize of the edges of every window still iterating; each round ends with one joint step launch.
-  const uint32_t* edge_member = L.edge_member();
-  const uint32_t* edge_win = L.edge_win();
-  std::vector<uint8_t> active(E);
-  for (;;) {
-    bool any_trial = false, any_lin = false;
-    for (size_t w = 0; w < W; w++) {
-      any_trial |= phase[w] == kPhaseTrial;
-      any_lin |= phase[w] == kPhaseLinearize;
-    }
-    if (!any_trial && !any_lin) break;
-    const bool lin = !any_trial;
-    for (size_t q = 0; q < E; q++) active[edge_member[q]] = phase[edge_win[q]] == (lin ? kPhaseLinearize : kPhaseTrial);
-    if (lin) {
-      if (int rc = linearize_round(ctx, o->factor_kind, o->robust_kind, o->robust_c, o->rejector_kind, o->max_dist_sq, nullptr, active.data())) return rc;
-    } else {
-      if (int rc = error_round(ctx, nullptr, active.data())) return rc;
-    }
-    CU(launch_joint_step(ao, J, L.max_free, lin, nullptr, 0, nullptr, ctx->b_out.as<double>(), ctx->stream));
-    ctx->launches += 1;
-    CU(cudaMemcpyAsync(phase.data(), ctx->joint.phase.p, W, cudaMemcpyDeviceToHost, ctx->stream));
-    CU(cudaStreamSynchronize(ctx->stream));
-  }
+  if (int rc = joint_rounds(ctx, o, L, phase, [&](bool lin) {
+        return launch_joint_step(ao, J, L.max_free, lin, nullptr, 0, nullptr, ctx->b_out.as<double>(), ctx->stream);
+      }))
+    return rc;
   std::vector<double> X(16 * K);
   if (K) CU(cudaMemcpyAsync(X.data(), ctx->joint.X.p, K * 16 * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
   if (W) CU(cudaMemcpyAsync(state.data(), ctx->joint.state.p, W * sizeof(WindowState), cudaMemcpyDeviceToHost, ctx->stream));
@@ -1518,6 +1554,128 @@ int sgb_align_joint(sgb_ctx* ctx, const sgb_align_options* o, size_t n_windows, 
     info[1] = state[w].iterations;
     info[2] = state[w].inliers;
     info[3] = state[w].e;
+  }
+  return 0;
+}
+
+int sgb_joint_edge_poses(sgb_ctx* ctx, size_t n_windows, const size_t* window_off, const double* X, double* out_T) {
+  if (!ctx) return 1;
+  AlignOptions ao;
+  JointLayout L;
+  if (int rc = joint_layout(ctx, "sgb_joint_edge_poses", nullptr, n_windows, window_off, nullptr, X, out_T, nullptr, ao, L, false)) return rc;
+  const size_t E = L.E;
+  if (E == 0) return 0;
+  CU(cudaSetDevice(ctx->device));
+  if (int rc = joint_upload(ctx, L, X)) return rc;
+  // joint_edge_poses_kernel writes the poses where the joint align's rounds read them (b_poses, row-major R | t per member)
+  CU(launch_joint_edge_poses(joint_params(ctx, ctx->joint, L.W, E), ctx->stream));
+  ctx->launches += 1;
+  std::vector<double> poses(12 * E);
+  CU(cudaMemcpyAsync(poses.data(), ctx->b_poses.p, poses.size() * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));
+  for (size_t p = 0; p < E; p++) {
+    const double* q = poses.data() + 12 * p;
+    double* T = out_T + 16 * p;
+    for (int i = 0; i < 3; i++) {
+      for (int j = 0; j < 3; j++) T[j * 4 + i] = q[i * 3 + j];
+      T[12 + i] = q[9 + i];
+      T[i * 4 + 3] = 0.0;
+    }
+    T[15] = 1.0;
+  }
+  return 0;
+}
+
+int sgb_align_joint_gnc(sgb_ctx* ctx, const sgb_align_options* o, const sgb_gnc_options* gnc, size_t n_windows, const size_t* window_off, const uint8_t* fixed,
+                        const double* init_X, double* out_X, double* out_info, double* out_gnc2, double* out_point_w) {
+  if (!ctx) return 1;
+  const std::string who = "sgb_align_joint_gnc";
+  AlignOptions ao;
+  JointLayout L;
+  if (int rc = joint_layout(ctx, who, o, n_windows, window_off, fixed, init_X, out_X, out_info, ao, L)) return rc;
+  if (int rc = gnc_option_checks(ctx, who, o, gnc)) return rc;
+  CU(cudaSetDevice(ctx->device));
+  if (int rc = gnc_capture_check(ctx, who)) return rc;
+  const size_t W = L.W, K = L.K, E = L.E, n = batch_points(ctx);
+  if (W == 0) return 0;
+  if (E) {
+    if (int rc = pair_view(ctx)) return rc;
+  }
+  CU(ctx->g_w.reserve(gnc_w_bytes(ctx)));
+  CU(ctx->g_e.reserve(gnc_w_bytes(ctx)));
+  CU(ctx->g_state.reserve(W * (sizeof(GncState) + 1)));
+  if (int rc = joint_upload(ctx, L, init_X)) return rc;
+  const JointParams J = joint_params(ctx, ctx->joint, W, E);
+  const uint32_t* member_win = ctx->joint.tables.as<uint32_t>() + L.member_win_at();
+  // the GNC state per window: p for the point kernels (over the edges' points), pw for the window kernels; every window starts its
+  // stage 0 with zero GNC and window state (r2max = 0, no stage begun, no iterations), live
+  GncParams p = gnc_params(ctx, gnc);
+  p.live = reinterpret_cast<uint8_t*>(p.gnc + W);
+  GncParams pw = p;
+  pw.n_members = static_cast<uint32_t>(W);
+  std::vector<unsigned char> g0(W * (sizeof(GncState) + 1), 0);
+  std::fill(g0.begin() + W * sizeof(GncState), g0.end(), 1);
+  CU(cudaMemcpyAsync(ctx->g_state.p, g0.data(), g0.size(), cudaMemcpyHostToDevice, ctx->stream));
+  CU(cudaMemsetAsync(ctx->joint.state.p, 0, W * sizeof(WindowState), ctx->stream));
+  BatchRows rows = {};
+  rows.member_off = p.member_off;
+  rows.perm = p.perm;
+  rows.e = p.e;
+  RoundWeights weights(ctx);
+  const uint32_t* edge_member = L.edge_member();
+  const uint32_t* edge_win = L.edge_win();
+  std::vector<uint8_t> live(W, 1), phase(W), active(E);
+  for (int stage = 0; std::find(live.begin(), live.end(), 1) != live.end(); stage++) {
+    // the edge poses of every window's X, then the reweighting linearize of the edges of the windows in the stage at them: unweighted,
+    // no robust kernel, its e rows to g_e
+    bool any = false;
+    for (size_t q = 0; q < E; q++) any |= (active[edge_member[q]] = live[edge_win[q]]) != 0;
+    if (E) {
+      CU(launch_joint_edge_poses(J, ctx->stream));
+      ctx->launches += 1;
+    }
+    weights.use(nullptr);
+    if (any) {
+      if (int rc = linearize_round(ctx, o->factor_kind, SGB_ROBUST_NONE, o->robust_c, o->rejector_kind, o->max_dist_sq, nullptr, active.data(), &rows)) return rc;
+    }
+    if (stage == 0) {
+      CU(launch_joint_gnc_rmax(p, member_win, ctx->sm_count, ctx->stream));
+      ctx->launches += 1;
+    }
+    CU(launch_gnc_stage(pw, ctx->stream));
+    CU(launch_joint_gnc_weight(p, member_win, ctx->sm_count, ctx->stream));
+    CU(launch_joint_gnc_init(pw, ao, J, ctx->stream));
+    ctx->launches += 3;
+    CU(cudaMemcpyAsync(phase.data(), ctx->joint.phase.p, W, cudaMemcpyDeviceToHost, ctx->stream));
+    CU(cudaMemcpyAsync(live.data(), p.live, W, cudaMemcpyDeviceToHost, ctx->stream));
+    CU(cudaStreamSynchronize(ctx->stream));
+    // the stage's joint align with its weights
+    weights.use(p.wstage);
+    if (int rc = joint_rounds(ctx, o, L, phase, [&](bool lin) {
+          return launch_joint_gnc_step(ao, J, L.max_free, lin, ctx->b_out.as<double>(), pw, ctx->stream);
+        }))
+      return rc;
+  }
+  std::vector<double> X(16 * K);
+  std::vector<WindowState> state(W);
+  std::vector<GncState> g(W);
+  if (K) CU(cudaMemcpyAsync(X.data(), ctx->joint.X.p, K * 16 * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaMemcpyAsync(state.data(), ctx->joint.state.p, W * sizeof(WindowState), cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaMemcpyAsync(g.data(), p.gnc, W * sizeof(GncState), cudaMemcpyDeviceToHost, ctx->stream));
+  if (out_point_w && n) CU(cudaMemcpyAsync(out_point_w, p.e, n * sizeof(double), cudaMemcpyDefault, ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));
+  const int32_t* freeidx = L.free();
+  for (size_t k = 0; k < K; k++) std::memcpy(out_X + 16 * k, freeidx[k] < 0 ? init_X + 16 * k : X.data() + 16 * k, 16 * sizeof(double));
+  for (size_t w = 0; w < W; w++) {
+    double* info = out_info + 4 * w;
+    info[0] = state[w].converged ? 1.0 : 0.0;
+    info[1] = state[w].iterations + g[w].iterations;
+    info[2] = state[w].inliers;
+    info[3] = state[w].e;
+    if (out_gnc2) {
+      out_gnc2[2 * w] = g[w].stages;
+      out_gnc2[2 * w + 1] = g[w].mu;
+    }
   }
   return 0;
 }
