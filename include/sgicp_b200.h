@@ -27,6 +27,21 @@
  *   poses            : 16 doubles, COLUMN-major 4x4 = Eigen::Isometry3d::data()
  *   H | b | e        : 36 + 6 + 1 doubles (H symmetric)          -- the tuple returned by
  *                      Reduction::linearize, registration/reduction.hpp:20-27
+ *
+ * Non-finite points.  A point whose x, y or z is NaN or +-Inf (organized LiDAR clouds mark missing
+ * returns so) is INERT, in every call that takes points:
+ *   - box and storage: it takes no part in its cloud's box, centre, extent, curve keys, tree boxes or
+ *     grid; every finite point is stored bit for bit as it is in the cloud without it;
+ *   - sgb_voxelgrid_sampling(_batch) and sgb_target_build_voxelmap(s) drop it, as the reference does;
+ *   - in a target (single kd-tree, many kd-trees, pairs, submaps, the grid front end) it is never a
+ *     correspondence and never a k-NN entry (sgb_target_batch_knn, sgb_target_knn_maps / _submaps);
+ *   - in a source (single, batch, pairs, submaps, joint frames) it has no correspondence and zero
+ *     per-point rows: it adds nothing to H | b | e, the inlier count or error(); in GNC its weight is 0;
+ *   - in sgb_estimate_features(_batch) it is never another point's neighbour, and its own row gets what a
+ *     point with fewer than 5 neighbours gets (zero normal, identity covariance).
+ * So the results for the finite rows equal the results for the cloud with the non-finite rows removed,
+ * indices mapped back.  Non-finite normals, covariances or poses supplied by the caller are not covered:
+ * they propagate, as in the reference.
  */
 #ifndef SGICP_B200_H_
 #define SGICP_B200_H_

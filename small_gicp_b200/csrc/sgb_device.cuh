@@ -212,14 +212,29 @@ __device__ __forceinline__ uint32_t owner_of(const uint32_t* __restrict__ prefix
   return lo;
 }
 
+/// Non-finite input points (a NaN or +-Inf in x, y or z) are inert (sgicp_b200.h): they take no part in a cloud's box, and the store
+/// writes them as NaN in all three lanes, so that no infinity survives centring.  A NaN point's squared distance to anything is NaN,
+/// which no `d < best` accepts and whose bits order above every finite bound, so the searches never return one; leaf boxes leave it
+/// out.  Its own query (NaN) is never searched: box_dist2 would be 0 for every box and nothing would prune the walk, so the grid probe
+/// settles it without a correspondence, the tree walks run it as an idle lane and the k-NN returns before walking.
+__device__ __forceinline__ bool point_is_finite(double x, double y, double z) { return isfinite(x) && isfinite(y) && isfinite(z); }
+/// the stored (centred FP32) point: x - c in each lane, or NaN in all three for a non-finite input point
+__device__ __forceinline__ float4 centred_store_point(const double4& p, double x, double y, double z, uint32_t w) {
+  const bool ok = point_is_finite(p.x, p.y, p.z);
+  return make_float4(ok ? (float)x : __int_as_float(0x7fffffff), ok ? (float)y : __int_as_float(0x7fffffff), ok ? (float)z : __int_as_float(0x7fffffff),
+                     __int_as_float(static_cast<int>(w)));
+}
+
 /// One CTA of kBoxBlock threads over pts[first, last): the exact box into bounds[6] (unless null) and the centre [4] that centre_kernel
-/// derives from it.  Min / max are exact, so both equal what the atomics of launch_bounds_centre give for these points alone.
+/// derives from it.  Min / max are exact, so both equal what the atomics of launch_bounds_centre give for these points alone.  Only
+/// finite points count (point_is_finite).
 constexpr int kBoxBlock = 256;
 __device__ __forceinline__ void cta_box_centre(const double4* __restrict__ pts, uint32_t first, uint32_t last, double* bounds, double* centre) {
   __shared__ double s_red[kBoxBlock / 32][6];
   double lo[3] = {DBL_MAX, DBL_MAX, DBL_MAX}, hi[3] = {-DBL_MAX, -DBL_MAX, -DBL_MAX};
   for (uint32_t i = first + threadIdx.x; i < last; i += kBoxBlock) {
     const double4 p = pts[i];
+    if (!point_is_finite(p.x, p.y, p.z)) continue;
     lo[0] = fmin(lo[0], p.x); lo[1] = fmin(lo[1], p.y); lo[2] = fmin(lo[2], p.z);
     hi[0] = fmax(hi[0], p.x); hi[1] = fmax(hi[1], p.y); hi[2] = fmax(hi[2], p.z);
   }
@@ -280,6 +295,10 @@ __device__ __forceinline__ uint32_t float_flip(float f) {
   return u ^ ((u >> 31) ? 0xFFFFFFFFu : 0x80000000u);
 }
 __device__ __forceinline__ float float_unflip(uint32_t u) { return __uint_as_float(u ^ ((u >> 31) ? 0x80000000u : 0xFFFFFFFFu)); }
+/// a coordinate's contribution to the min / max words of a box: the empty box's word for NaN (a stored non-finite point), which
+/// float_flip would order above +Inf (or below -Inf with its sign bit set)
+__device__ __forceinline__ uint32_t box_lo_word(float f) { return isnan(f) ? 0xFFFFFFFFu : float_flip(f); }
+__device__ __forceinline__ uint32_t box_hi_word(float f) { return isnan(f) ? 0u : float_flip(f); }
 
 /// the child record of heap node child_heap (> 0) in its parent's packet: box [lo, hi], a | b in the w lanes
 __device__ __forceinline__ void lbvh_store_child(float4* pnodes, uint32_t child_heap, const float lo[3], const float hi[3], uint32_t a, uint32_t b) {
@@ -297,8 +316,8 @@ __device__ __forceinline__ void lbvh_leaf_box(const float4* __restrict__ pts, ui
     lo[a] = INFINITY;
     hi[a] = -INFINITY;
   }
-  if (idx < last) {
-    const float4 p = pts[base + idx];
+  const float4 p = idx < last ? pts[base + idx] : make_float4(0.f, 0.f, 0.f, 0.f);
+  if (idx < last && !isnan(p.x)) {  // a stored non-finite point (NaN in every lane) leaves the box as it is
     lo[0] = hi[0] = p.x;
     lo[1] = hi[1] = p.y;
     lo[2] = hi[2] = p.z;
@@ -353,12 +372,12 @@ __device__ __forceinline__ void kd_refine_segment(float4* __restrict__ pts, uint
     for (uint32_t t = tid; t < m; t += blockDim.x) {
       const float4 p = P0[t];
       uint32_t* bx = s_box + (tree_node_of(first + t, count, n) - node_first) * 6u;
-      atomicMin(&bx[0], float_flip(p.x));
-      atomicMin(&bx[1], float_flip(p.y));
-      atomicMin(&bx[2], float_flip(p.z));
-      atomicMax(&bx[3], float_flip(p.x));
-      atomicMax(&bx[4], float_flip(p.y));
-      atomicMax(&bx[5], float_flip(p.z));
+      atomicMin(&bx[0], box_lo_word(p.x));
+      atomicMin(&bx[1], box_lo_word(p.y));
+      atomicMin(&bx[2], box_lo_word(p.z));
+      atomicMax(&bx[3], box_hi_word(p.x));
+      atomicMax(&bx[4], box_hi_word(p.y));
+      atomicMax(&bx[5], box_hi_word(p.z));
     }
     __syncthreads();
     for (uint32_t t = tid; t < kKdSegMax; t += blockDim.x) {

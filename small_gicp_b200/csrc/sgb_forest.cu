@@ -56,7 +56,7 @@ __global__ void forest_convert_kernel(const double4* __restrict__ pts, const dou
     const double* c = centres + 4 * static_cast<size_t>(m);
     const double4 p = pts[i];
     const double x = p.x - c[0], y = p.y - c[1], z = p.z - c[2];
-    const float4 f = make_float4((float)x, (float)y, (float)z, __int_as_float(static_cast<int>(i - F.pt_off[m])));
+    const float4 f = centred_store_point(p, x, y, z, i - F.pt_off[m]);
     out_pts[i] = f;
     work_pts[i] = f;
     perm[i] = i;
@@ -86,7 +86,7 @@ __global__ void forest_boxes_kernel(const float4* __restrict__ pts, uint32_t n, 
   const uint32_t m = owner_of(F.pt_off, F.n_maps, idx), first = F.pt_off[m];
   const uint32_t node = forest_level_node(F, m, idx - first, F.pt_off[m + 1] - first, level);
   const float4 p = pts[idx];
-  uint32_t v[6] = {float_flip(p.x), float_flip(p.y), float_flip(p.z), float_flip(p.x), float_flip(p.y), float_flip(p.z)};
+  uint32_t v[6] = {box_lo_word(p.x), box_lo_word(p.y), box_lo_word(p.z), box_hi_word(p.x), box_hi_word(p.y), box_hi_word(p.z)};
   const uint32_t node0 = __shfl_sync(0xffffffffu, node, 0);
   if (__all_sync(0xffffffffu, node == node0)) {
     if (node0 == ~0u) return;
@@ -237,7 +237,7 @@ __global__ void __launch_bounds__(kLinBlock, SUBMAP ? 7 : 8) forest_search_kerne
       fy = f.y;
       fz = f.z;
     }
-    best_d = bound;
+    best_d = isnan(SUBMAP ? p.x : fx) ? -1.0f : bound;  // a stored non-finite point (NaN query): no search, as an idle lane
     // the member's previous correspondence: an upper bound only prunes
     const uint32_t prev = (B.members[m].z & kMemberSeeded) ? B.corr[i] : kNone;
     if (prev != kNone) {

@@ -40,21 +40,22 @@ __device__ __forceinline__ void grid_sort_coords(uint64_t k, int bits, int& ix, 
 }
 __device__ __forceinline__ uint64_t grid_sort_pad(int bits) { return (1ull << (3 * bits)) - 1ull; }
 
-// cell key of every target point (leaf-ordered, centred FP32); value = leaf position
+// cell key of every target point (leaf-ordered, centred FP32); value = leaf position.  A stored non-finite point (NaN) gets the pad:
+// it sorts after every cell and is in no block
 __global__ void grid_cell_keys_kernel(const float4* __restrict__ pts, uint32_t n, GridParams g, int bits, uint64_t* keys, uint32_t* vals) {
   const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   const float4 p = pts[i];
   const int ix = __float2int_rd((p.x - g.origin[0]) * g.inv_cell), iy = __float2int_rd((p.y - g.origin[1]) * g.inv_cell),
             iz = __float2int_rd((p.z - g.origin[2]) * g.inv_cell);
-  keys[i] = grid_sort_key(ix, iy, iz, bits);
+  keys[i] = isnan(p.x) || isnan(p.y) || isnan(p.z) ? grid_sort_pad(bits) : grid_sort_key(ix, iy, iz, bits);
   vals[i] = i;
 }
 
 // after the (stable) sort: the points in cell order -- within a cell in ascending leaf position -- and, at position j, the eight
 // anchor entries of the cell that starts at j: every cell c is part of the blocks anchored at c - o, o in {0, 1}^3, in run
 // r = oy + 2 oz of each (value 4 j + r).  cnt[j] = points of that cell (measured up to kGridMaxList + 1: beyond it build_grid drops
-// the front end anyway).  Positions that start no cell write eight pads.
+// the front end anyway).  Positions that start no cell, and the non-finite points at the end, write eight pads.
 __global__ void grid_cell_heads_kernel(const uint64_t* __restrict__ keys, const uint32_t* __restrict__ leaf_pos, const float4* __restrict__ leaf_pts, uint32_t n,
                                        int bits, float4* grid_pts, uint32_t* cnt, uint64_t* akeys, uint32_t* avals) {
   const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
@@ -63,7 +64,7 @@ __global__ void grid_cell_heads_kernel(const uint64_t* __restrict__ keys, const 
   const float4 p = leaf_pts[l];
   grid_pts[j] = make_float4(p.x, p.y, p.z, __uint_as_float(l));
   const uint64_t k = keys[j];
-  if (j != 0 && keys[j - 1] == k) {
+  if ((j != 0 && keys[j - 1] == k) || k == grid_sort_pad(bits)) {  // not the head of a cell, or a non-finite point
 #pragma unroll
     for (uint32_t o = 0; o < 8u; o++) {
       akeys[8u * j + o] = grid_sort_pad(bits);
@@ -195,7 +196,8 @@ __global__ void __launch_bounds__(256, ROUND ? 6 : 8) grid_probe_blocks_kernel(c
     best_d = __uint_as_float(static_cast<uint32_t>(best_key >> 32));
     best = static_cast<uint32_t>(best_key);
   }
-  const bool settled = best != kNone && best_d <= g.settle_d2;
+  // a stored non-finite point (NaN query) is settled without a correspondence: no walk ever starts for it
+  const bool settled = (best != kNone && best_d <= g.settle_d2) || isnan(fx);
   if (!settled && P.use_prev) {  // keep the better of (grid candidate, previous correspondence) as the tree search's seed
     const uint32_t prev = P.corr[i];
     if (prev != kNone) {

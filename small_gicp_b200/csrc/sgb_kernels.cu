@@ -292,6 +292,7 @@ __global__ void bounds_kernel(const double4* __restrict__ pts, size_t n, double*
   double lo[3] = {DBL_MAX, DBL_MAX, DBL_MAX}, hi[3] = {-DBL_MAX, -DBL_MAX, -DBL_MAX};
   for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < n; i += static_cast<size_t>(gridDim.x) * blockDim.x) {
     const double4 p = pts[i];
+    if (!point_is_finite(p.x, p.y, p.z)) continue;  // inert: no part in the box
     lo[0] = fmin(lo[0], p.x); lo[1] = fmin(lo[1], p.y); lo[2] = fmin(lo[2], p.z);
     hi[0] = fmax(hi[0], p.x); hi[1] = fmax(hi[1], p.y); hi[2] = fmax(hi[2], p.z);
   }
@@ -339,8 +340,8 @@ __device__ __forceinline__ uint64_t spread21(uint64_t x) {  // 21 bits -> every 
 }
 
 
-/// 63-bit space-filling-curve key of a centred point (h = half extent of the cloud's box, inv_ext = (2^21 - 1) / extent).
-__device__ __forceinline__ uint64_t curve_key(double x, double y, double z, double h, double inv_ext) {
+/// 63-bit space-filling-curve key of a finite centred point (h = half extent of the cloud's box, inv_ext = (2^21 - 1) / extent).
+__device__ __forceinline__ uint64_t curve_key_finite(double x, double y, double z, double h, double inv_ext) {
   const uint64_t kx = static_cast<uint64_t>(fmin(fmax((x + h) * inv_ext, 0.0), 2097151.0));
   const uint64_t ky = static_cast<uint64_t>(fmin(fmax((y + h) * inv_ext, 0.0), 2097151.0));
   const uint64_t kz = static_cast<uint64_t>(fmin(fmax((z + h) * inv_ext, 0.0), 2097151.0));
@@ -372,6 +373,15 @@ __device__ __forceinline__ uint64_t curve_key(double x, double y, double z, doub
   X[2] ^= t;
   return (spread21(X[0]) << 2) | (spread21(X[1]) << 1) | spread21(X[2]);
 }
+/// The sort key of a point: a non-finite point gets the largest 63-bit key and every finite point a smaller one, so that the stable
+/// sort stores the non-finite points after every finite point of their cloud, and the finite points at the positions they have in the
+/// cloud without them.
+constexpr uint64_t kCurveKeyNonFinite = (1ull << 63) - 1ull;
+__device__ __forceinline__ uint64_t curve_key(double x, double y, double z, double h, double inv_ext) {
+  if (!point_is_finite(x, y, z)) return kCurveKeyNonFinite;
+  const uint64_t k = curve_key_finite(x, y, z, h, inv_ext);
+  return k < kCurveKeyNonFinite ? k : kCurveKeyNonFinite - 1ull;
+}
 
 // raw (double AoS) -> centred float4 in ORIGINAL order (w = index), optional features, optional curve key
 __global__ void convert_kernel(const double4* __restrict__ pts, const double4* __restrict__ normals, const double* __restrict__ covs, size_t n,
@@ -382,7 +392,7 @@ __global__ void convert_kernel(const double4* __restrict__ pts, const double4* _
   for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < n; i += static_cast<size_t>(gridDim.x) * blockDim.x) {
     const double4 p = pts[i];
     const double x = p.x - cx, y = p.y - cy, z = p.z - cz;
-    out_pts[i] = make_float4((float)x, (float)y, (float)z, __int_as_float(static_cast<int>(i)));
+    out_pts[i] = centred_store_point(p, x, y, z, static_cast<uint32_t>(i));
     // what the rounding to FP32 dropped (hi + lo carries ~48 bits of x - c): the feature estimation ranks its neighbour candidates and
     // sums its covariances on the exact coordinates, so that its neighbour SETS are the reference's, not FP32 near-tie variants of them
     if (out_lo) out_lo[i] = make_float4((float)(x - (double)(float)x), (float)(y - (double)(float)y), (float)(z - (double)(float)z), 0.f);
@@ -443,7 +453,7 @@ __global__ void clouds_convert_kernel(const double4* __restrict__ pts, uint32_t 
     const double inv_ext = 2097151.0 / centre[3];
     const double4 p = pts[i];
     const double x = p.x - cx, y = p.y - cy, z = p.z - cz;
-    out_pts[i] = make_float4((float)x, (float)y, (float)z, __int_as_float(static_cast<int>(i - off[c])));
+    out_pts[i] = centred_store_point(p, x, y, z, i - off[c]);
     keys[i] = curve_key(x, y, z, 0.5 * centre[3], inv_ext);
     vals[i] = i;
   }
@@ -503,7 +513,7 @@ __global__ void kd_boxes_kernel(const float4* __restrict__ pts, uint32_t n, uint
   const uint32_t idx = valid ? i : n - 1u;
   const float4 p = pts[idx];
   const uint32_t node = tree_node_of(idx, count, n);
-  uint32_t v[6] = {float_flip(p.x), float_flip(p.y), float_flip(p.z), float_flip(p.x), float_flip(p.y), float_flip(p.z)};
+  uint32_t v[6] = {box_lo_word(p.x), box_lo_word(p.y), box_lo_word(p.z), box_hi_word(p.x), box_hi_word(p.y), box_hi_word(p.z)};
   // pre-reduction: whole CTA in one node (upper levels: otherwise thousands of atomics hit the same six words), else
   // whole warp in one node, else per-thread atomics (deepest levels, little contention)
   __shared__ uint32_t s_box[6];

@@ -147,7 +147,7 @@ __global__ void __launch_bounds__(kLinBlock, MIN_CTAS) packet_search_kernel(cons
       fx = f.x;
       fy = f.y;
       fz = f.z;
-      best_d = P.max_dist_sq;
+      best_d = isnan(fx) ? -1.0f : P.max_dist_sq;  // a stored non-finite point (NaN query): no search, as an idle lane
       const uint32_t prev = (P.use_prev || settled) ? P.corr[i] : kNone;  // seed: an upper bound only prunes
       if (prev != kNone) {
         const float4 t = __ldg(&pts[prev]);

@@ -64,6 +64,7 @@ struct KnnList {
 template <int KMAX, typename I = uint32_t>
 __device__ __forceinline__ void bvh_knn(const float4* __restrict__ pnodes, const float4* __restrict__ pts, float qx, float qy, float qz,
                                         KnnList<KMAX, float, I>& L, uint2* desc, float* dist, I tag = 0) {
+  if (!(isfinite(qx) && isfinite(qy) && isfinite(qz))) return;  // a non-finite query has no neighbours: no walk
   int sp = 0;
   uint2* my_desc = desc + threadIdx.x;
   float* my_dist = dist + threadIdx.x;
@@ -529,8 +530,10 @@ __global__ void voxel_keys_kernel(const double4* __restrict__ pts, size_t n, dou
     const int64_t cx = static_cast<int64_t>(floor(p.x * inv_leaf)) + coord_offset;
     const int64_t cy = static_cast<int64_t>(floor(p.y * inv_leaf)) + coord_offset;
     const int64_t cz = static_cast<int64_t>(floor(p.z * inv_leaf)) + coord_offset;
-    uint64_t key = ~0ull;  // out of the 21-bit range: dropped (downsampling.hpp:41-45 warns and marks them invalid)
-    if (cx >= 0 && cy >= 0 && cz >= 0 && cx <= coord_bit_mask && cy <= coord_bit_mask && cz <= coord_bit_mask)
+    // out of the 21-bit range, or non-finite (the reference's fast_floor gives INT_MIN there; the cast here gives 0 for NaN): dropped
+    // (downsampling.hpp:41-45 warns and marks them invalid)
+    uint64_t key = ~0ull;
+    if (point_is_finite(p.x, p.y, p.z) && cx >= 0 && cy >= 0 && cz >= 0 && cx <= coord_bit_mask && cy <= coord_bit_mask && cz <= coord_bit_mask)
       key = static_cast<uint64_t>(cx) | (static_cast<uint64_t>(cy) << coord_bit_size) | (static_cast<uint64_t>(cz) << (2 * coord_bit_size));
     keys[i] = key;
     vals[i] = static_cast<uint32_t>(i);

@@ -17,18 +17,28 @@ def _f32(a):
     return np.asarray(a, dtype=np.float64).astype(np.float32).astype(np.float64)
 
 
+def finite_rows(pts):
+    """rows whose x, y and z are all finite; a row with a NaN or an infinity is inert (include/sgicp_b200.h)"""
+    return np.isfinite(np.asarray(pts, dtype=np.float64)[:, :3]).all(1)
+
+
 def box_centre(pts):
-    """the centre every upload (source, target, voxel means) is stored relative to: 0.5 (min + max) per axis in FP64, 0 if empty"""
-    if len(pts) == 0:
+    """the centre every upload (source, target, voxel means) is stored relative to: 0.5 (min + max) per axis in FP64 over the finite
+    rows, 0 if there are none"""
+    p = np.asarray(pts, dtype=np.float64)[:, :3]
+    p = p[finite_rows(p)] if len(p) else p
+    if len(p) == 0:
         return np.zeros(3)
-    return 0.5 * (pts[:, :3].min(0) + pts[:, :3].max(0))
+    return 0.5 * (p.min(0) + p.max(0))
 
 
 def stored_points(pts, centre=None):
-    """convert_kernel: float32(p - c) with round-to-nearest, read back as that + c in FP64; c = box_centre of the whole upload"""
+    """convert_kernel: float32(p - c) with round-to-nearest, read back as that + c in FP64; c = box_centre of the whole upload.  A
+    non-finite row is stored as NaN in all three coordinates."""
     c = box_centre(pts) if centre is None else centre
     out = np.array(pts, dtype=np.float64)
-    out[:, :3] = _f32(out[:, :3] - c) + c
+    fin = finite_rows(out)
+    out[:, :3] = np.where(fin[:, None], _f32(np.where(fin[:, None], out[:, :3], 0.0) - c) + c, np.nan)
     return out
 
 
@@ -107,8 +117,18 @@ def weights(T, factor, src_pts, src_covs, tgt_pts, tgt_normals, tgt_covs, idx, k
     return np.linalg.inv(RCR)
 
 
+def _check_inert(corr, src_pts, tgt_pts):
+    """a non-finite source row has no correspondence, and no correspondence names a non-finite target row"""
+    corr = np.asarray(corr, dtype=np.uint64)
+    hit = corr != NO
+    assert not (hit & ~finite_rows(src_pts)).any(), ("non-finite source rows with a correspondence", np.nonzero(hit & ~finite_rows(src_pts))[0][:10])
+    k = corr[hit].astype(np.int64)
+    assert finite_rows(np.asarray(tgt_pts)[k]).all() if len(k) else True, "a correspondence names a non-finite target row"
+
+
 def linearize(T, corr, factor, robust, robust_c, src_pts, src_covs, tgt_pts, tgt_normals, tgt_covs):
     """sum over accepted correspondences of J^T M J, J^T M r, 1/2 r^T M r (robust-weighted)"""
+    _check_inert(corr, src_pts, tgt_pts)
     idx = np.nonzero(corr != NO)[0]
     if len(idx) == 0:
         return np.zeros((6, 6)), np.zeros(6), 0.0
@@ -130,6 +150,7 @@ def linearize(T, corr, factor, robust, robust_c, src_pts, src_covs, tgt_pts, tgt
 
 def error(T_trial, T_lin, corr, factor, robust, robust_c, src_pts, src_covs, tgt_pts, tgt_normals, tgt_covs):
     """Reduction::error: residuals at T_trial, GICP precision frozen at T_lin (gicp_factor.hpp:81-89)"""
+    _check_inert(corr, src_pts, tgt_pts)
     idx = np.nonzero(corr != NO)[0]
     if len(idx) == 0:
         return 0.0

@@ -18,8 +18,14 @@ COORD_MASK = (1 << COORD_BITS) - 1
 
 
 def voxel_coords(points, leaf):
-    """integer voxel coordinates floor(p * (1 / leaf)): a multiply by the FP64 reciprocal, as the kernels and the reference compute it"""
-    return np.floor(np.asarray(points, dtype=np.float64)[:, :3] * (1.0 / leaf)).astype(np.int64)
+    """integer voxel coordinates floor(p * (1 / leaf)): a multiply by the FP64 reciprocal, as the kernels and the reference compute it.
+    A row with a non-finite coordinate (or one whose scaled coordinate overflows) gets coordinates outside the 21-bit range, so that
+    coord_keys drops it, as the reference's fast_floor (INT_MIN) does; numpy's cast of NaN to int64 is not relied on."""
+    c = np.floor(np.asarray(points, dtype=np.float64)[:, :3] * (1.0 / leaf))
+    fin = np.isfinite(c).all(1)
+    out = np.where(fin[:, None], np.clip(np.where(fin[:, None], c, 0.0), -(1 << 40), 1 << 40), 0.0).astype(np.int64)
+    out[~fin] = COORD_MASK + 1
+    return out
 
 
 def coord_keys(c):

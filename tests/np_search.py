@@ -20,7 +20,7 @@ band, and rows are padded with UINT64_MAX / DBL_MAX when the target has fewer th
 import numpy as np
 from scipy.spatial import cKDTree
 
-from np_factors import NO, _f32, box_centre
+from np_factors import NO, _f32, box_centre, finite_rows
 
 BAND = 32 * 2.0**-24
 DBL_MAX = np.finfo(np.float64).max
@@ -33,14 +33,30 @@ def search_bound(max_dist_sq):
 
 
 class Target:
-    """the stored target: FP32 coordinates centred on the box centre (held as FP64) and a cKDTree over them"""
+    """the stored target: FP32 coordinates centred on the box centre (held as FP64) and a cKDTree over them.  Non-finite rows are
+    inert (include/sgicp_b200.h): f holds NaN there, the tree holds only the finite rows, and every index the tree returns is mapped
+    back to the row it came from (tree.query's answers go through .rows)."""
 
     def __init__(self, pts):
         pts = np.asarray(pts, dtype=np.float64)[:, :3]
         self.n = len(pts)
         self.centre = box_centre(pts)
-        self.f = _f32(pts - self.centre)
-        self.tree = cKDTree(self.f) if self.n else None
+        fin = finite_rows(pts)
+        self.f = np.where(fin[:, None], _f32(np.where(fin[:, None], pts, 0.0) - self.centre), np.nan)
+        self.rows = np.nonzero(fin)[0]
+        self.n_finite = len(self.rows)
+        self.tree = _RowTree(self.f[self.rows], self.rows, self.n) if self.n_finite else None
+
+
+class _RowTree:
+    """cKDTree over the finite rows whose query returns row indices of the whole target (n where cKDTree reports a missing neighbour)"""
+
+    def __init__(self, f, rows, n):
+        self._t, self._rows = cKDTree(f), np.append(rows, n)
+
+    def query(self, x, k=1, **kw):
+        d, j = self._t.query(x, k=k, **kw)
+        return d, self._rows[j]
 
 
 def _rows(T, x):
@@ -75,13 +91,13 @@ def _d2(a, b):
 def _band_points(tgt, q32, dmin):
     """indices of every target point within the tie band of one query"""
     lim = dmin * (1.0 + BAND)
-    k = min(8, tgt.n)
+    k = min(8, tgt.n_finite)
     while True:
         d, j = tgt.tree.query(q32, k=k)
         d, j = np.atleast_1d(d) ** 2, np.atleast_1d(j)
-        if d[-1] > lim or k == tgt.n:
+        if d[-1] > lim or k == tgt.n_finite:
             return j[d <= lim * (1 + 1e-15)]
-        k = min(4 * k, tgt.n)
+        k = min(4 * k, tgt.n_finite)
 
 
 def _check_nn(tgt, corr, q, q32, max_d):
@@ -141,11 +157,18 @@ def check_correspondences(corr, T, src_pts, tgt, max_dist_sq=1.0, src_centre=Non
     report.queries += n
     if n == 0:
         return 0
-    if tgt.n == 0:
+    fin = finite_rows(src_pts)
+    assert (corr[~fin] == NO).all(), ("non-finite queries with a correspondence", np.nonzero(~fin & (corr != NO))[0][:10])
+    if tgt.n_finite == 0:
         assert (corr == NO).all()
         return n
-    q, q32, amb, other = queries(T, src_pts, tgt.centre, src_centre)
+    cs = box_centre(src_pts) if src_centre is None else src_centre
+    src = np.where(fin[:, None], np.asarray(src_pts, dtype=np.float64)[:, :3], cs)  # (checked above; the finite rows are the queries)
+    q, q32, amb, other = queries(T, src, tgt.centre, cs)
     status, ratio = _check_nn(tgt, corr, q, q32, max_dist_sq)
+    status[~fin] = 0
+    ratio[~fin] = 0.0
+    amb[~fin] = False
     bad = np.nonzero(status < 0)[0]
     amb_any = amb.any(1)
     report.ambiguous += int(amb_any.sum())
@@ -189,10 +212,15 @@ def check_knn(idx, d2, queries_xyz, k, tgt, report=REPORT):
     n = len(qw)
     assert idx.shape == (n, k) and d2.shape == (n, k)
     report.queries += n
-    m = min(k, tgt.n)
+    # a non-finite query has no neighbours: its row is all padding
+    fin = finite_rows(qw)
+    assert (idx[~fin] == NO).all() and (d2[~fin] == DBL_MAX).all(), ("non-finite queries with neighbours", np.nonzero(~fin & (idx[:, 0] != NO))[0][:10])
+    idx, d2, qw = idx[fin], d2[fin], qw[fin]
+    n = len(qw)
+    m = min(k, tgt.n_finite)
     # padding
     assert (idx[:, m:] == NO).all() and (d2[:, m:] == DBL_MAX).all(), "padding"
-    if m == 0:
+    if m == 0 or n == 0:
         return n
     assert (idx[:, :m] < tgt.n).all(), "index out of range or missing"
     qc = qw - tgt.centre  # the device's FP64 centred query
@@ -202,7 +230,7 @@ def check_knn(idx, d2, queries_xyz, k, tgt, report=REPORT):
     assert np.all(np.diff(d2, axis=1) >= 0), ("rows not ascending", np.nonzero((np.diff(d2, axis=1) < 0).any(1))[0][:10])
     assert all(len(set(row)) == m for row in j.tolist()), "duplicate index in a row"
     # the model's FP64 k-set: k + 8 candidates re-ranked by the exact FP64 distance
-    kk = min(tgt.n, m + 8)
+    kk = min(tgt.n_finite, m + 8)
     _, cand = tgt.tree.query(qc, k=kk, workers=-1)
     cand = cand.reshape(n, kk)
     cd = _d2(tgt.f[cand], qc[:, None, :])
