@@ -541,6 +541,33 @@ int sgb_align_joint_async(sgb_ctx* ctx, const sgb_align_options* options, size_t
  *     counts, plus 1 when the pairing's view of the target is rebuilt; captured work counts at capture, not at replay. */
 int sgb_align_batch_gnc_async(sgb_ctx* ctx, const sgb_align_options* options, const sgb_gnc_options* gnc, const double* d_init_T16xB, double* d_out_T16xB,
                               double* d_out_info4xB, double* d_out_Hb42xB /*or NULL*/, double* d_out_gnc2xB /*or NULL*/, double* d_out_point_w /*or NULL*/);
+/* sgb_align_joint_gnc enqueued on the context's stream with no host involvement after the call, as sgb_align_batch_gnc_async enqueues
+ * sgb_align_batch_gnc: a CUDA graph whose outer WHILE node runs one GNC stage per iteration (every edge's pose from its window's X, the
+ * reweighting linearize of the edges of the windows still in GNC, planned on the device; the stage's mu, weights and joint_init per
+ * window) and whose body holds an inner WHILE node repeating the stage's joint rounds (planner, search, factor with the stage's weights,
+ * per-edge sums, one joint step per window) until no window has a round to go.  Windows run their stages in lockstep in
+ * sgb_align_joint_gnc's order.
+ *   - Arguments, checks, messages and results as sgb_align_joint_gnc, except that the poses and every output are device memory of the
+ *     context's GPU (host, page-locked or managed pointers fail with a message, nothing enqueued); window_off and fixed are host memory,
+ *     read during the call.  For the same inputs X, info, gnc2 and out_point_w are bit-identical to it (a window with no edge, and a call
+ *     with no edge at all, included; a call made from other seeds -- the correspondences an earlier call left -- may differ at exact FP32
+ *     distance ties, as above), fixed frames come back bit for bit from d_init_X16xK, the context is left as it leaves it
+ *     (sgb_correspondences_batch, sgb_error_batch and sgb_linearize_batch on the edges behave alike afterwards), and the weights in force
+ *     are unchanged.  Errors of the enqueued work surface at the next synchronising call of the context.
+ *   - The window tables are those of sgb_align_joint_async, cached in the context once for both calls: a call whose tables are unchanged
+ *     uploads nothing; one whose tables changed uploads them once.
+ *   - While the context's stream is being captured the whole GNC is added to the capture: each replay re-runs it from what d_init_X16xK
+ *     and the weights in force hold at replay time.  A call that would have to allocate or upload (the GNC buffers for its windows, the
+ *     first batched call's search queue, the capture streams, window tables that differ from the cached ones) fails with a message
+ *     instead: call it once outside the capture first.  The captured work is only valid while the context's batch, pairing, target,
+ *     windows, fixed flags and buffers are those of the capture.  Outside a capture the instantiated graph is cached in the context and
+ *     rebuilt when the align or GNC options, the windows, the batch, the pairing, the target or any buffer it uses changes.
+ *   - sgb_kernel_launches counts 3 per call with at least one edge (one launch of the graph, two for the outputs) and 4 without (the stage
+ *     kernels of the one stage, two for the outputs), whatever the stage and round counts, plus 1 when the pairing's view of the target
+ *     is rebuilt; captured work counts at capture, not at replay.  A call with no window enqueues nothing. */
+int sgb_align_joint_gnc_async(sgb_ctx* ctx, const sgb_align_options* options, const sgb_gnc_options* gnc, size_t n_windows, const size_t* window_off,
+                              const uint8_t* fixed /*or NULL*/, const double* d_init_X16xK, double* d_out_X16xK, double* d_out_info4xW,
+                              double* d_out_gnc2xW /*or NULL*/, double* d_out_point_w /*or NULL*/);
 
 /* ---- per-cloud preparation on the device (SURVEY.md §8(f); not per-iteration) --------------------
  * sgb_estimate_features replaces estimate_normals / estimate_covariances / estimate_normals_covariances and

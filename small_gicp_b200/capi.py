@@ -109,6 +109,8 @@ _SIGNATURES = {
     "sgb_align_batch_gnc_async": (C.c_int, [_vp, C.POINTER(AlignOptions), C.POINTER(GncOptions), _dp, _dp, _dp, _dp, _dp, _dp]),
     "sgb_align_joint": (C.c_int, [_vp, C.POINTER(AlignOptions), C.c_size_t, C.POINTER(C.c_size_t), C.POINTER(C.c_uint8), _dp, _dp, _dp]),
     "sgb_align_joint_async": (C.c_int, [_vp, C.POINTER(AlignOptions), C.c_size_t, C.POINTER(C.c_size_t), C.POINTER(C.c_uint8), _dp, _dp, _dp]),
+    "sgb_align_joint_gnc_async": (C.c_int, [_vp, C.POINTER(AlignOptions), C.POINTER(GncOptions), C.c_size_t, C.POINTER(C.c_size_t), C.POINTER(C.c_uint8),
+                                            _dp, _dp, _dp, _dp, _dp]),
     "sgb_joint_edge_poses": (C.c_int, [_vp, C.c_size_t, C.POINTER(C.c_size_t), _dp, _dp]),
     "sgb_align_joint_gnc": (C.c_int, [_vp, C.POINTER(AlignOptions), C.POINTER(GncOptions), C.c_size_t, C.POINTER(C.c_size_t), C.POINTER(C.c_uint8), _dp,
                                       _dp, _dp, _dp, _dp]),
@@ -234,6 +236,18 @@ class AsyncJointAlignResult:
         self.iterations = info4[:, 1]
         self.num_inliers = info4[:, 2]
         self.error = info4[:, 3]
+
+
+class AsyncJointGncAlignResult(AsyncJointAlignResult):
+    """what Context.align_joint_gnc_async enqueued: the AsyncJointAlignResult views (iterations summed over each window's stages), stages
+    (W,) and mu (W,) as float64 views of the raw gnc2 (W,2), and point_w (N,) each edge point's final g (None unless requested).  The raw
+    outputs X16, info4, gnc2 and point_w pass as out= to reuse them (graph capture needs fixed buffers)."""
+
+    def __init__(self, X16, info4, gnc2, point_w):
+        super().__init__(X16, info4)
+        self.gnc2, self.point_w = gnc2, point_w
+        self.stages = gnc2[:, 0]
+        self.mu = gnc2[:, 1]
 
 
 def library_path(profiling=False):
@@ -893,37 +907,74 @@ class Context:
         other keywords as in align_joint.  Returns an AsyncJointAlignResult of CUDA tensors (out: a previous result whose buffers are reused).
         Inside torch.cuda.graph (with the capture stream set) the align is captured: each replay re-runs it from what init_X holds then.
         The weights in force (set_source_weights) apply, at a replay those in force then."""
-        import torch
-
-        if self._stream is None:
-            raise SgbError("align_joint_async: set the context's stream to a torch stream first (set_stream): the poses are prepared on it")
-        K = self._cloud_offsets.size - 1 if hasattr(self, "_cloud_offsets") else 0
-        if not (isinstance(init_X, torch.Tensor) and init_X.is_cuda and init_X.dtype == torch.float64 and tuple(init_X.shape) == (K, 4, 4)):
-            raise SgbError(f"align_joint_async: init_X must be a CUDA float64 tensor of shape ({K}, 4, 4)")
-        off = np.ascontiguousarray(np.array([0, K] if windows is None else windows, dtype=np.uintp).reshape(-1))
-        if off.size < 1:
-            raise SgbError("align_joint_async: windows needs at least one entry")
-        W = off.size - 1
-        fx = None if fixed is None else np.ascontiguousarray(np.asarray(fixed).astype(np.uint8).reshape(-1))
-        if fx is not None and fx.size != K:
-            raise SgbError(f"align_joint_async: fixed needs {K} entries")
         o = AlignOptions(int(factor), int(robust), float(robust_c), int(rejector), float(max_dist_sq), int(optimizer), int(max_iterations), float(gn_lambda),
                          int(max_inner_iterations), float(init_lambda), float(lambda_factor), float(rotation_eps), float(translation_eps))
         o.dof_mask[:] = [1.0] * 6 if dof_mask is None else [float(x) for x in dof_mask]
+
+        def outputs(K, W, zeros):
+            if out is None:
+                return AsyncJointAlignResult(zeros(K, 16), zeros(W, 4))
+            if tuple(out.X16.shape) != (K, 16) or tuple(out.info4.shape) != (W, 4):
+                raise SgbError(f"align_joint_async: out holds {out.X16.shape[0]} frames and {out.info4.shape[0]} windows, the call {K} and {W}")
+            return out
+
+        W, off, fx, res = self._joint_async_in(init_X, windows, fixed, "align_joint_async", outputs)
+        self._check(self._L.sgb_align_joint_async(self._h, C.byref(o), W, off.ctypes.data_as(C.POINTER(C.c_size_t)),
+                                                  None if fx is None else fx.ctypes.data_as(C.POINTER(C.c_uint8)), _d(self._joint_in), _d(res.X16),
+                                                  _d(res.info4)))
+        return res
+
+    def _joint_async_in(self, init_X, windows, fixed, who, outputs):
+        """the window offsets, fixed flags and outputs of a stream-ordered joint call, with init_X transposed into _joint_in (column-major) on
+        the context's stream; outputs(K, W, zeros) returns the call's result buffers, zeros(rows, cols) a new float64 tensor there"""
+        import torch
+
+        if self._stream is None:
+            raise SgbError(f"{who}: set the context's stream to a torch stream first (set_stream): the poses are prepared on it")
+        K = self._cloud_offsets.size - 1 if hasattr(self, "_cloud_offsets") else 0
+        if not (isinstance(init_X, torch.Tensor) and init_X.is_cuda and init_X.dtype == torch.float64 and tuple(init_X.shape) == (K, 4, 4)):
+            raise SgbError(f"{who}: init_X must be a CUDA float64 tensor of shape ({K}, 4, 4)")
+        off = np.ascontiguousarray(np.array([0, K] if windows is None else windows, dtype=np.uintp).reshape(-1))
+        if off.size < 1:
+            raise SgbError(f"{who}: windows needs at least one entry")
+        W = off.size - 1
+        fx = None if fixed is None else np.ascontiguousarray(np.asarray(fixed).astype(np.uint8).reshape(-1))
+        if fx is not None and fx.size != K:
+            raise SgbError(f"{who}: fixed needs {K} entries")
         dev = init_X.device
         with torch.cuda.stream(torch.cuda.ExternalStream(self._stream, device=dev)):
-            if out is None:
-                out = AsyncJointAlignResult(torch.zeros((max(K, 1), 16), dtype=torch.float64, device=dev)[:K],
-                                            torch.zeros((max(W, 1), 4), dtype=torch.float64, device=dev)[:W])
-            elif tuple(out.X16.shape) != (K, 16) or tuple(out.info4.shape) != (W, 4):
-                raise SgbError(f"align_joint_async: out holds {out.X16.shape[0]} frames and {out.info4.shape[0]} windows, the call {K} and {W}")
+            res = outputs(K, W, lambda rows, cols: torch.zeros((max(rows, 1), cols), dtype=torch.float64, device=dev)[:rows])
             if self._joint_in is None or self._joint_in.shape[0] != K or self._joint_in.device != dev:
                 self._joint_in = torch.empty((max(K, 1), 16), dtype=torch.float64, device=dev)[:K]
             self._joint_in.view(K, 4, 4).copy_(init_X.transpose(1, 2))  # column-major
-        self._check(self._L.sgb_align_joint_async(self._h, C.byref(o), W, off.ctypes.data_as(C.POINTER(C.c_size_t)),
-                                                  None if fx is None else fx.ctypes.data_as(C.POINTER(C.c_uint8)), _d(self._joint_in), _d(out.X16),
-                                                  _d(out.info4)))
-        return out
+        return W, off, fx, res
+
+    def align_joint_gnc_async(self, init_X, noise_bound_sq, windows=None, fixed=None, gnc=GNC_TLS, max_stages=64, stage_iterations=3, point_weights=False,
+                              out=None, **align):
+        """align_joint_gnc enqueued on the context's stream without a host synchronisation (sgb_align_joint_gnc_async): every stage and joint
+        round runs on the device.  init_X and the stream as in align_joint_async; the other arguments as in align_joint_gnc.  Returns an
+        AsyncJointGncAlignResult of CUDA tensors (out: a previous result whose buffers are reused; it must hold point_w if point_weights).
+        Inside torch.cuda.graph (with the capture stream set) the whole GNC is captured: each replay re-runs it from what init_X holds then,
+        with the weights in force then (set_source_weights)."""
+        o = _align_options(**align)
+        g = GncOptions(int(gnc), float(noise_bound_sq), int(max_stages), int(stage_iterations))
+        N = int(self._batch_offsets[-1]) if hasattr(self, "_batch_offsets") else 0
+
+        def outputs(K, W, zeros):
+            if out is None:
+                return AsyncJointGncAlignResult(zeros(K, 16), zeros(W, 4), zeros(W, 2), zeros(N, 1)[:, 0] if point_weights else None)
+            if tuple(out.X16.shape) != (K, 16) or tuple(out.info4.shape) != (W, 4):
+                raise SgbError(f"align_joint_gnc_async: out holds {out.X16.shape[0]} frames and {out.info4.shape[0]} windows, the call {K} and {W}")
+            if point_weights and (out.point_w is None or tuple(out.point_w.shape) != (N,)):
+                raise SgbError(f"align_joint_gnc_async: point_weights needs out.point_w of {N} rows")
+            return out
+
+        W, off, fx, res = self._joint_async_in(init_X, windows, fixed, "align_joint_gnc_async", outputs)
+        pw = res.point_w if point_weights else None
+        self._check(self._L.sgb_align_joint_gnc_async(self._h, C.byref(o), C.byref(g), W, off.ctypes.data_as(C.POINTER(C.c_size_t)),
+                                                      None if fx is None else fx.ctypes.data_as(C.POINTER(C.c_uint8)), _d(self._joint_in), _d(res.X16),
+                                                      _d(res.info4), _d(res.gnc2), _d(pw)))
+        return res
 
     # ---- multi-GPU: all-reduce of H|b|e fused into the reduction kernel (peer memory over NVLink) ----
     COMM_HANDLE_BYTES = 64

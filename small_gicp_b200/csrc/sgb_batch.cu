@@ -26,9 +26,11 @@
 //                           each stage's phases, the loops' conditions and the outputs)
 //   joint_gnc_*_kernel      sgb_align_joint_gnc: the same GNC with the window as its unit (each point's window through its edge), each
 //                           window's stage start (joint_init) and the joint step with each window's stage iterations
+//                           (sgb_align_joint_gnc_async: joint_gnc_reweigh_kernel / joint_gnc_loops_kernel / joint_gnc_finish_kernel, each
+//                           stage's edge phases, the loops' conditions and the outputs)
 // The transform, factor, segment and step kernels serve the rounds the host plans (sgb_{linearize,error,align}_batch, sgb_align_joint) and,
 // with ROUND / kModeRound, the rounds batch_plan_kernel plans on the device (sgb_align_batch_async, sgb_align_joint_async,
-// sgb_align_batch_gnc_async).
+// sgb_align_batch_gnc_async, sgb_align_joint_gnc_async).
 // A member's sums depend on its own points, pose and correspondences only, added in an order fixed by its size: bit-identical whatever
 // else is in the batch.
 #include <algorithm>
@@ -1051,8 +1053,10 @@ cudaError_t launch_joint_align_finish(const JointParams& J, uint32_t n_frames, c
 // ---- sgb_align_joint_gnc (DESIGN.md §11 "Graduated non-convexity for joint windows"): the GNC unit is the window.  p.gnc and p.live are
 // per window; the point kernels reach a point's window through its member (edge), member_win[m] ----
 
+// ROUND (sgb_align_joint_gnc_async, launched at every stage of its loop): only the windows before their stage 0 (no stage begun)
+template <bool ROUND>
 __global__ void joint_gnc_rmax_kernel(const GncParams p, const uint32_t* __restrict__ member_win) {
-  gnc_rmax_points<false>(p, GncWindowUnit{member_win});
+  gnc_rmax_points<ROUND>(p, GncWindowUnit{member_win});
 }
 
 template <int KIND>
@@ -1081,14 +1085,24 @@ __global__ void __launch_bounds__(kStepBlock) joint_gnc_init_kernel(const GncPar
   J.phase[w] = static_cast<uint8_t>(s.phase);
 }
 
-// joint_step_kernel<false> for a round of a GNC stage: each window steps with its stage's max_iterations (as joint_gnc_init_kernel chose)
+// joint_step_kernel for a round of a GNC stage: each window steps with its stage's max_iterations (as joint_gnc_init_kernel chose).  ROUND: a
+// round of a stage of sgb_align_joint_gnc_async, as joint_step_kernel<true> (its kind read from `round`, each stepped window's phase to its
+// edges' member_phase, `loop` set to 1 while a window has a round to go)
+template <bool ROUND>
 __global__ void __launch_bounds__(kJointBlock) joint_gnc_step_kernel(const __grid_constant__ AlignOptions o, const __grid_constant__ JointParams J, bool linearize,
-                                                                     const double* __restrict__ out, const GncParams p) {
-  joint_step_window<false>(gnc_stage_options(o, p, blockIdx.x), J, linearize, out, nullptr, 0, nullptr);
+                                                                     const double* __restrict__ out, const GncParams p, const BatchRound* __restrict__ round,
+                                                                     cudaGraphConditionalHandle loop, uint8_t* __restrict__ member_phase) {
+  if constexpr (ROUND)
+    joint_step_window<true>(gnc_stage_options(o, p, blockIdx.x), J, linearize, out, round, loop, member_phase);
+  else
+    joint_step_window<false>(gnc_stage_options(o, p, blockIdx.x), J, linearize, out, nullptr, 0, nullptr);
 }
 
-cudaError_t launch_joint_gnc_rmax(const GncParams& p, const uint32_t* member_win, int sm_count, cudaStream_t st) {
-  joint_gnc_rmax_kernel<<<gnc_point_grid(p.n, sm_count), 256, 0, st>>>(p, member_win);
+cudaError_t launch_joint_gnc_rmax(const GncParams& p, const uint32_t* member_win, bool round, int sm_count, cudaStream_t st) {
+  if (round)
+    joint_gnc_rmax_kernel<true><<<gnc_point_grid(p.n, sm_count), 256, 0, st>>>(p, member_win);
+  else
+    joint_gnc_rmax_kernel<false><<<gnc_point_grid(p.n, sm_count), 256, 0, st>>>(p, member_win);
   return cudaGetLastError();
 }
 
@@ -1105,11 +1119,72 @@ cudaError_t launch_joint_gnc_init(const GncParams& pw, const AlignOptions& o, co
   return cudaGetLastError();
 }
 
-cudaError_t launch_joint_gnc_step(const AlignOptions& o, const JointParams& J, int max_free, bool linearize, const double* out, const GncParams& pw, cudaStream_t st) {
+cudaError_t launch_joint_gnc_step(const AlignOptions& o, const JointParams& J, int max_free, bool linearize, const double* out, const GncParams& pw,
+                                  const BatchRound* round, cudaGraphConditionalHandle loop, uint8_t* member_phase, cudaStream_t st) {
+  const auto kernel = round ? joint_gnc_step_kernel<true> : joint_gnc_step_kernel<false>;
   const size_t smem = joint_step_smem(max_free);
-  const cudaError_t e = allow_dynamic_smem(joint_gnc_step_kernel, smem);
+  const cudaError_t e = allow_dynamic_smem(kernel, smem);
   if (e != cudaSuccess) return e;
-  joint_gnc_step_kernel<<<J.n_windows, kJointBlock, smem, st>>>(o, J, linearize, out, pw);
+  kernel<<<J.n_windows, kJointBlock, smem, st>>>(o, J, linearize, out, pw, round, loop, member_phase);
+  return cudaGetLastError();
+}
+
+// ---- sgb_align_joint_gnc_async (DESIGN.md §11 "Asynchronous graduated non-convexity for joint windows"): the stages and their joint rounds
+// on the device.  The edges are the members of the rounds, each edge's member phase its window's. ----
+
+// The head of a stage, one thread per edge: the edges of the windows still in GNC in kPhaseLinearize, every other edge done, so that the
+// planner plans the reweighting linearize of exactly the edges of the windows in the stage; `rounds` cleared (joint_gnc_loops_kernel sets it)
+__global__ void __launch_bounds__(kStepBlock) joint_gnc_reweigh_kernel(const __grid_constant__ JointParams J, const uint8_t* __restrict__ live,
+                                                                       uint8_t* __restrict__ member_phase, cudaGraphConditionalHandle rounds) {
+  const uint32_t q = blockIdx.x * kStepBlock + threadIdx.x;
+  if (q == 0) cudaGraphSetConditional(rounds, 0u);
+  if (q < J.n_edges) member_phase[J.edge_member[q]] = live[J.edge_win[q]] ? kPhaseLinearize : kPhaseDone;
+}
+
+// After joint_gnc_init_kernel, one thread per edge and per window: each edge's member phase becomes its window's new phase (what the
+// rounds' planner reads; joint_gnc_init_kernel writes J.phase only); `stages` becomes 1 if a window has a stage to go after this one,
+// `rounds` (cleared by joint_gnc_reweigh_kernel) 1 if a window's joint align has a round to go
+__global__ void __launch_bounds__(kStepBlock) joint_gnc_loops_kernel(const __grid_constant__ JointParams J, const uint8_t* __restrict__ live,
+                                                                     uint8_t* __restrict__ member_phase, cudaGraphConditionalHandle stages,
+                                                                     cudaGraphConditionalHandle rounds) {
+  const uint32_t i = blockIdx.x * kStepBlock + threadIdx.x;
+  if (i < J.n_edges) member_phase[J.edge_member[i]] = J.phase[J.edge_win[i]];
+  int more_stages = 0, more_rounds = 0;
+  if (i < J.n_windows) {
+    more_stages = live[i];
+    more_rounds = J.phase[i] == kPhaseLinearize || J.phase[i] == kPhaseTrial;
+  }
+  if (__syncthreads_or(more_stages) && threadIdx.x == 0) cudaGraphSetConditional(stages, 1u);
+  if (__syncthreads_or(more_rounds) && threadIdx.x == 0) cudaGraphSetConditional(rounds, 1u);
+}
+
+// what sgb_align_joint_gnc adds to joint_align_finish_kernel's outputs, per window: the iterations of its earlier stages, its stages and last mu
+__global__ void __launch_bounds__(kStepBlock) joint_gnc_finish_kernel(uint32_t n_windows, const WindowState* __restrict__ state, const GncState* __restrict__ gnc,
+                                                                      double* __restrict__ out_info4, double* __restrict__ out_gnc2) {
+  const uint32_t w = blockIdx.x * kStepBlock + threadIdx.x;
+  if (w >= n_windows) return;
+  const GncState& g = gnc[w];
+  out_info4[4 * static_cast<size_t>(w) + 1] = state[w].iterations + g.iterations;
+  if (out_gnc2) {
+    out_gnc2[2 * static_cast<size_t>(w)] = g.stages;
+    out_gnc2[2 * static_cast<size_t>(w) + 1] = g.mu;
+  }
+}
+
+cudaError_t launch_joint_gnc_reweigh(const JointParams& J, const uint8_t* live, uint8_t* member_phase, cudaGraphConditionalHandle rounds, cudaStream_t st) {
+  joint_gnc_reweigh_kernel<<<(J.n_edges + kStepBlock - 1) / kStepBlock, kStepBlock, 0, st>>>(J, live, member_phase, rounds);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_joint_gnc_loops(const JointParams& J, const uint8_t* live, uint8_t* member_phase, cudaGraphConditionalHandle stages,
+                                   cudaGraphConditionalHandle rounds, cudaStream_t st) {
+  const uint32_t n = std::max(J.n_edges, J.n_windows);
+  joint_gnc_loops_kernel<<<(n + kStepBlock - 1) / kStepBlock, kStepBlock, 0, st>>>(J, live, member_phase, stages, rounds);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_joint_gnc_finish(const JointParams& J, const GncState* gnc, double* out_info4, double* out_gnc2, cudaStream_t st) {
+  joint_gnc_finish_kernel<<<(J.n_windows + kStepBlock - 1) / kStepBlock, kStepBlock, 0, st>>>(J.n_windows, J.state, gnc, out_info4, out_gnc2);
   return cudaGetLastError();
 }
 

@@ -243,14 +243,29 @@ cudaError_t launch_joint_align_finish(const JointParams& J, uint32_t n_frames, c
 // ---- sgb_align_joint_gnc (DESIGN.md §11 "Graduated non-convexity for joint windows"): sgb_align_batch_gnc's stages with the window as the
 // GNC unit.  GncState and live flags per window: p (the point kernels) has n_members = the edges, each point's window member_win[its edge];
 // pw (the window kernels, and launch_gnc_stage) the same with n_members = the windows. ----
-/// stage 0: every window's largest r^2 = 2 e_i > 0 over its edges' points with a correspondence (gnc[w].r2max, cleared by the caller)
-cudaError_t launch_joint_gnc_rmax(const GncParams& p, const uint32_t* member_win, int sm_count, cudaStream_t st);
+/// stage 0: every window's largest r^2 = 2 e_i > 0 over its edges' points with a correspondence (gnc[w].r2max, cleared by the caller).
+/// round: launched at every stage of the device loop, for the windows that have begun no stage only
+cudaError_t launch_joint_gnc_rmax(const GncParams& p, const uint32_t* member_win, bool round, int sm_count, cudaStream_t st);
 /// launch_gnc_weight with each point's window's mu (TLS: not_binary per window)
 cudaError_t launch_joint_gnc_weight(const GncParams& p, const uint32_t* member_win, int sm_count, cudaStream_t st);
 /// launch_gnc_init per window: joint_init of a window in the stage from its current X (max_iterations = stage_iterations unless last),
 /// its phase to J.phase; every other window is left done
 cudaError_t launch_joint_gnc_init(const GncParams& pw, const AlignOptions& o, const JointParams& J, cudaStream_t st);
-/// launch_joint_step of a host-planned round of a GNC stage: each window steps with its stage's max_iterations
-cudaError_t launch_joint_gnc_step(const AlignOptions& o, const JointParams& J, int max_free, bool linearize, const double* out, const GncParams& pw, cudaStream_t st);
+/// launch_joint_step for a round of a GNC stage: each window steps with its stage's max_iterations.  round = null: a host-planned round;
+/// else a round planned on the device, as launch_joint_step's (member_phase, loop)
+cudaError_t launch_joint_gnc_step(const AlignOptions& o, const JointParams& J, int max_free, bool linearize, const double* out, const GncParams& pw,
+                                  const BatchRound* round, cudaGraphConditionalHandle loop, uint8_t* member_phase, cudaStream_t st);
+
+// ---- sgb_align_joint_gnc_async (DESIGN.md §11 "Asynchronous graduated non-convexity for joint windows"): the stages and their joint rounds
+// on the device, the edges the members of the rounds ----
+/// the head of a stage: member_phase of every edge of a window still in GNC (live) = kPhaseLinearize, of every other edge kPhaseDone;
+/// `rounds` set to 0
+cudaError_t launch_joint_gnc_reweigh(const JointParams& J, const uint8_t* live, uint8_t* member_phase, cudaGraphConditionalHandle rounds, cudaStream_t st);
+/// after launch_joint_gnc_init: every edge's member_phase = its window's phase; `stages` set to 1 if a window has a stage to go after this
+/// one (live), `rounds` to 1 if a window's joint align has a round to go
+cudaError_t launch_joint_gnc_loops(const JointParams& J, const uint8_t* live, uint8_t* member_phase, cudaGraphConditionalHandle stages,
+                                   cudaGraphConditionalHandle rounds, cudaStream_t st);
+/// after launch_joint_align_finish: info's iterations summed over each window's stages, and gnc2 (or null) = the stages run and the last mu
+cudaError_t launch_joint_gnc_finish(const JointParams& J, const GncState* gnc, double* out_info4, double* out_gnc2, cudaStream_t st);
 
 }  // namespace sgb

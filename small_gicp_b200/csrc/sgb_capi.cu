@@ -89,6 +89,7 @@ void forget_linearisation(sgb_ctx* ctx) {
   ctx->align_key.clear();  // sgb_align_batch_async rebuilds its loop graph
   ctx->joint_key.clear();  // and sgb_align_joint_async its own
   ctx->gnc_key.clear();    // and sgb_align_batch_gnc_async its own
+  ctx->joint_gnc_key.clear();  // and sgb_align_joint_gnc_async its own
 }
 
 }  // namespace
@@ -647,6 +648,7 @@ void sgb_destroy(sgb_ctx* ctx) {
   if (ctx->align_exec) cudaGraphExecDestroy(ctx->align_exec);
   if (ctx->joint_exec) cudaGraphExecDestroy(ctx->joint_exec);
   if (ctx->gnc_exec) cudaGraphExecDestroy(ctx->gnc_exec);
+  if (ctx->joint_gnc_exec) cudaGraphExecDestroy(ctx->joint_gnc_exec);
   if (ctx->cap_stream) cudaStreamDestroy(ctx->cap_stream);
   if (ctx->cap_stream_nested) cudaStreamDestroy(ctx->cap_stream_nested);
   if (ctx->own_stream) cudaStreamDestroy(ctx->own_stream);

@@ -1,7 +1,7 @@
 // SPDX-License-Identifier: MIT
 // C-ABI of batched registration (include/sgicp_b200.h: sgb_source_set_batch, sgb_source_set_pairs, sgb_source_set_submaps,
 // sgb_source_set_weights, sgb_{linearize,error,align,correspondences}_batch, sgb_{linearize,error}_batch_points, sgb_align_batch_async, sgb_align_joint,
-// sgb_align_joint_async, sgb_align_batch_gnc, sgb_align_batch_gnc_async, sgb_joint_edge_poses, sgb_align_joint_gnc).
+// sgb_align_joint_async, sgb_align_batch_gnc, sgb_align_batch_gnc_async, sgb_joint_edge_poses, sgb_align_joint_gnc, sgb_align_joint_gnc_async).
 // Kernels in sgb_batch.cu (many kd-trees and submaps: the searches in sgb_forest.cu); DESIGN.md §11.
 #include <cuda_runtime.h>
 
@@ -450,8 +450,8 @@ int pair_members(sgb_ctx* ctx, const char* who, size_t n_members, const uint32_t
   return 0;
 }
 
-// ---- the device loops of sgb_align_batch_async, sgb_align_joint_async and sgb_align_batch_gnc_async (DESIGN.md §11 "Asynchronous align",
-// "Asynchronous joint windows", "Asynchronous graduated non-convexity") ----
+// ---- the device loops of sgb_align_batch_async, sgb_align_joint_async, sgb_align_batch_gnc_async and sgb_align_joint_gnc_async (DESIGN.md
+// §11 "Asynchronous align", "Asynchronous joint windows", "Asynchronous graduated non-convexity", "... for joint windows") ----
 
 // the kernel parameters every round of the device loop shares (those of linearize_round; error() reads the same ones)
 void round_params(sgb_ctx* ctx, const sgb_align_options* o, LinParams& P, BatchParams& Bp) {
@@ -1507,6 +1507,33 @@ int joint_upload(sgb_ctx* ctx, const JointLayout& L, const double* X) {
   return 0;
 }
 
+// The window tables and buffers of sgb_align_joint_async (ctx->joint_async), which sgb_align_joint_gnc_async shares: a call of layout L
+// must reserve or upload (neither of which a capture can hold) when a buffer must grow or the tables differ from ja_tab, the host copy of
+// what joint_async.tables holds
+bool joint_async_stale(sgb_ctx* ctx, const JointLayout& L) {
+  const std::vector<size_t> bytes = joint_bytes(L);
+  const std::vector<DevBuf*> bufs = joint_buffers(ctx->joint_async);
+  for (size_t i = 0; i < bufs.size(); i++)
+    if (bytes[i] > bufs[i]->cap) return true;
+  return L.tab != ctx->ja_tab;
+}
+
+// joint_async reserved for layout L, and its tables uploaded when upload (joint_async_stale).  ja_tab claims what joint_async.tables holds.
+// The claim is dropped before anything that can replace or lose that content: a reservation frees the old buffer before it allocates the
+// new one, and any step below may fail.  So a failed call leaves no claim behind, and the next call uploads its tables again.
+int joint_async_tables(sgb_ctx* ctx, const JointLayout& L, bool upload) {
+  const std::vector<size_t> bytes = joint_bytes(L);
+  const std::vector<DevBuf*> bufs = joint_buffers(ctx->joint_async);
+  if (upload) ctx->ja_tab.clear();
+  for (size_t i = 0; i < bufs.size(); i++) CU(bufs[i]->reserve(bytes[i]));
+  if (upload) {
+    // pageable host memory: the copy is staged before cudaMemcpyAsync returns
+    CU(cudaMemcpyAsync(ctx->joint_async.tables.p, L.tab.data(), L.tab.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
+    ctx->ja_tab = L.tab;
+  }
+  return 0;
+}
+
 }  // namespace
 
 extern "C" {
@@ -1639,7 +1666,7 @@ int sgb_align_joint_gnc(sgb_ctx* ctx, const sgb_align_options* o, const sgb_gnc_
       if (int rc = linearize_round(ctx, o->factor_kind, SGB_ROBUST_NONE, o->robust_c, o->rejector_kind, o->max_dist_sq, nullptr, active.data(), &rows)) return rc;
     }
     if (stage == 0) {
-      CU(launch_joint_gnc_rmax(p, member_win, ctx->sm_count, ctx->stream));
+      CU(launch_joint_gnc_rmax(p, member_win, false, ctx->sm_count, ctx->stream));
       ctx->launches += 1;
     }
     CU(launch_gnc_stage(pw, ctx->stream));
@@ -1652,7 +1679,7 @@ int sgb_align_joint_gnc(sgb_ctx* ctx, const sgb_align_options* o, const sgb_gnc_
     // the stage's joint align with its weights
     weights.use(p.wstage);
     if (int rc = joint_rounds(ctx, o, L, phase, [&](bool lin) {
-          return launch_joint_gnc_step(ao, J, L.max_free, lin, ctx->b_out.as<double>(), pw, ctx->stream);
+          return launch_joint_gnc_step(ao, J, L.max_free, lin, ctx->b_out.as<double>(), pw, nullptr, 0, nullptr, ctx->stream);
         }))
       return rc;
   }
@@ -1756,24 +1783,11 @@ int sgb_align_joint_async(sgb_ctx* ctx, const sgb_align_options* o, size_t n_win
   const bool loop = o->max_iterations > 0 && E > 0;
   // A capture can hold neither an allocation nor an upload from pageable memory: the buffers, the capture stream and the window tables
   // must come from an earlier call.  Outside a capture the tables are uploaded only when they changed (windows, fixed flags or pairing).
-  const std::vector<size_t> bytes = joint_bytes(L);
-  const std::vector<DevBuf*> bufs = joint_buffers(ctx->joint_async);
-  bool grow = false;
-  for (size_t i = 0; i < bufs.size(); i++) grow = grow || bytes[i] > bufs[i]->cap;
-  const bool upload = grow || L.tab != ctx->ja_tab;
+  const bool upload = joint_async_stale(ctx, L);
   if (capturing && (upload || (loop && !ctx->cap_stream)))
     return fail(ctx, 1, std::string(who) + ": these windows need an allocation or an upload of their tables, which a capture cannot hold; call it once "
                                            "outside the capture first");
-  // ja_tab claims what joint_async.tables holds.  The claim is dropped before anything that can replace or lose that content: a
-  // reservation frees the old buffer before it allocates the new one, and any step below may fail.  So a failed call leaves no claim
-  // behind, and the next call uploads its tables again.
-  if (upload) ctx->ja_tab.clear();
-  for (size_t i = 0; i < bufs.size(); i++) CU(bufs[i]->reserve(bytes[i]));
-  if (upload) {
-    // pageable host memory: the copy is staged before cudaMemcpyAsync returns
-    CU(cudaMemcpyAsync(ctx->joint_async.tables.p, L.tab.data(), L.tab.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
-    ctx->ja_tab = L.tab;
-  }
+  if (int rc = joint_async_tables(ctx, L, upload)) return rc;
   if (E) {
     if (int rc = pair_view(ctx)) return rc;
   }
@@ -1814,6 +1828,136 @@ int sgb_align_joint_async(sgb_ctx* ctx, const sgb_align_options* o, size_t n_win
       ctx->b_lin[edge_member[q]] = 1;
       ctx->b_seeded[edge_member[q]] = 1;
     }
+    ctx->have_lin = true;
+    ctx->corr_seeds = true;
+    ctx->lin_factor = o->factor_kind;
+    ctx->lin_robust = o->robust_kind;
+    ctx->lin_c = o->robust_c;
+  }
+  return 0;
+}
+
+int sgb_align_joint_gnc_async(sgb_ctx* ctx, const sgb_align_options* o, const sgb_gnc_options* gnc, size_t n_windows, const size_t* window_off,
+                              const uint8_t* fixed, const double* d_init_X, double* d_out_X, double* d_out_info, double* d_out_gnc2, double* d_out_point_w) {
+  if (!ctx) return 1;
+  const std::string who = "sgb_align_joint_gnc_async";
+  AlignOptions ao;
+  JointLayout L;
+  if (int rc = joint_layout(ctx, who, o, n_windows, window_off, fixed, d_init_X, d_out_X, d_out_info, ao, L)) return rc;
+  if (int rc = gnc_option_checks(ctx, who, o, gnc)) return rc;
+  const size_t W = L.W, K = L.K, E = L.E, n = batch_points(ctx);
+  if (W == 0) return 0;
+  CU(cudaSetDevice(ctx->device));
+  if (int rc = device_pointer(ctx, who.c_str(), d_init_X, "init_X16xK")) return rc;
+  if (int rc = device_pointer(ctx, who.c_str(), d_out_X, "out_X16xK")) return rc;
+  if (int rc = device_pointer(ctx, who.c_str(), d_out_info, "out_info4xW")) return rc;
+  if (d_out_gnc2) {
+    if (int rc = device_pointer(ctx, who.c_str(), d_out_gnc2, "out_gnc2xW")) return rc;
+  }
+  if (d_out_point_w) {
+    if (int rc = device_pointer(ctx, who.c_str(), d_out_point_w, "out_point_w")) return rc;
+  }
+  cudaStreamCaptureStatus capture = cudaStreamCaptureStatusNone;
+  CU(cudaStreamIsCapturing(ctx->stream, &capture));
+  if (capture == cudaStreamCaptureStatusInvalidated) return fail(ctx, 1, who + ": the context's stream is in an invalidated capture");
+  const bool capturing = capture == cudaStreamCaptureStatusActive;
+  // A capture can hold neither an allocation nor an upload from pageable memory: the GNC buffers for W windows, the window tables and
+  // buffers (uploaded only when they changed, as sgb_align_joint_async's), and with an edge the first batched call's search queue and both
+  // capture streams (the stages' loop and the rounds' loop nested in it) must come from an earlier call
+  const size_t w_bytes = gnc_w_bytes(ctx), state_bytes = W * (sizeof(GncState) + 1);
+  const bool upload = joint_async_stale(ctx, L);
+  const bool allocates = upload || ctx->g_w.cap < w_bytes || ctx->g_e.cap < w_bytes || ctx->g_state.cap < state_bytes ||
+                         (E && ((ctx->use_packet_queue && !ctx->packet_queue.p) || !ctx->cap_stream || !ctx->cap_stream_nested));
+  if (capturing && allocates)
+    return fail(ctx, 1, who + ": this call needs an allocation or an upload of its window tables, which a capture cannot hold; call it once outside the "
+                              "capture first");
+  if (E && ctx->use_packet_queue && !ctx->packet_queue.p) {
+    CU(ctx->packet_queue.reserve(2 * sizeof(uint32_t)));
+    CU(cudaMemsetAsync(ctx->packet_queue.p, 0, 2 * sizeof(uint32_t), ctx->stream));
+  }
+  CU(ctx->g_w.reserve(w_bytes));
+  CU(ctx->g_e.reserve(w_bytes));
+  CU(ctx->g_state.reserve(state_bytes));
+  if (int rc = joint_async_tables(ctx, L, upload)) return rc;
+  if (E) {
+    if (int rc = pair_view(ctx)) return rc;
+  }
+  const JointParams J = joint_params(ctx, ctx->joint_async, W, E);
+  const uint32_t* member_win = ctx->joint_async.tables.as<uint32_t>() + L.member_win_at();
+  // the GNC state per window, as sgb_align_joint_gnc's: p for the point kernels (over the edges' points), pw for the window kernels
+  GncParams p = gnc_params(ctx, gnc);
+  p.live = reinterpret_cast<uint8_t*>(p.gnc + W);
+  GncParams pw = p;
+  pw.n_members = static_cast<uint32_t>(W);
+  uint8_t* member_phase = ctx->b_phase.as<uint8_t>();
+  // sgb_align_joint_gnc's initial state: the frames' X from d_init_X, zero window and GNC state (r2max = 0, no stage begun, no iterations),
+  // every window live; the device's seed flags kept as sgb_align_joint_async keeps them
+  if (K) CU(cudaMemcpyAsync(J.X, d_init_X, K * 16 * sizeof(double), cudaMemcpyDeviceToDevice, ctx->stream));
+  CU(cudaMemsetAsync(J.state, 0, W * sizeof(WindowState), ctx->stream));
+  CU(cudaMemsetAsync(p.gnc, 0, W * sizeof(GncState), ctx->stream));
+  CU(cudaMemsetAsync(p.live, 1, W, ctx->stream));
+  if (E && !(ctx->corr_seeds && ctx->b_dseed_ok)) CU(cudaMemsetAsync(ctx->b_dseed.p, 0, E, ctx->stream));
+  if (!E) {
+    // No edge, so no point: sgb_align_joint_gnc's one stage of the stage kernels (r_max^2 = 0 makes it every window's last; the largest
+    // residual and the weights have nothing to visit) and no round
+    CU(launch_gnc_stage(pw, ctx->stream));
+    CU(launch_joint_gnc_init(pw, ao, J, ctx->stream));
+    ctx->launches += 2;
+  } else {
+    // One stage per iteration of the outer loop, in sgb_align_joint_gnc's order: the edge poses of every window's X, the reweighting
+    // linearize of the edges of the windows in the stage (planned by batch_plan_kernel from their member phases), the stage kernels, then
+    // the stage's joint align as an inner loop of rounds.  After joint_gnc_init, joint_gnc_loops gives every edge its window's phase and
+    // sets both conditions: the stages' while a window has a stage to go, the rounds' while a window's align has a round to go.
+    BatchRows rows = {};
+    rows.member_off = p.member_off;
+    rows.perm = p.perm;
+    rows.e = p.e;
+    RoundWeights weights(ctx);
+    const auto stage = [&](cudaGraphConditionalHandle stages) {
+      cudaGraphConditionalHandle rounds;
+      if (int rc = loop_handle(ctx, who.c_str(), nullptr, &rounds)) return rc;
+      CU(launch_joint_edge_poses(J, ctx->stream));
+      CU(launch_joint_gnc_reweigh(J, p.live, member_phase, rounds, ctx->stream));
+      weights.use(nullptr);
+      if (int rc = round_head(ctx, o, stages, &rows)) return rc;
+      CU(launch_joint_gnc_rmax(p, member_win, true, ctx->sm_count, ctx->stream));
+      CU(launch_gnc_stage(pw, ctx->stream));
+      CU(launch_joint_gnc_weight(p, member_win, ctx->sm_count, ctx->stream));
+      CU(launch_joint_gnc_init(pw, ao, J, ctx->stream));
+      CU(launch_joint_gnc_loops(J, p.live, member_phase, stages, rounds, ctx->stream));
+      weights.use(p.wstage);
+      return capture_loop(ctx, rounds, round_loop(ctx, o, [&](cudaGraphConditionalHandle h) {
+                            CU(launch_joint_gnc_step(ao, J, L.max_free, true, ctx->b_out.as<double>(), pw, ctx->b_round.as<BatchRound>(), h, member_phase,
+                                                     ctx->stream));
+                            return 0;
+                          }));
+    };
+    std::vector<unsigned char> key;
+    if (!capturing) {  // loop_key, plus the GNC options, JointParams, the frame count, max_free and every buffer the GNC kernels use
+      key = loop_key(ctx, o);
+      for (int v : {p.kind, p.max_stages, p.stage_iterations}) key_add(key, v);
+      key_add(key, p.c2);
+      key_add(key, J);
+      for (size_t v : {K, static_cast<size_t>(L.max_free)}) key_add(key, v);
+      for (const void* v : {static_cast<const void*>(p.member_off), static_cast<const void*>(p.perm), static_cast<const void*>(p.corr),
+                            static_cast<const void*>(p.e), static_cast<const void*>(p.w), static_cast<const void*>(p.wstage),
+                            static_cast<const void*>(p.gnc), static_cast<const void*>(p.live), static_cast<const void*>(member_win)})
+        key_add(key, v);
+    }
+    if (int rc = launch_loop(ctx, who.c_str(), capturing, std::move(key), ctx->joint_gnc_exec, ctx->joint_gnc_key, stage)) return rc;
+    ctx->launches += 1;
+    if (int rc = clear_search_counters(ctx)) return rc;
+  }
+  CU(launch_joint_align_finish(J, static_cast<uint32_t>(K), d_init_X, d_out_X, d_out_info, ctx->stream));
+  CU(launch_joint_gnc_finish(J, p.gnc, d_out_info, d_out_gnc2, ctx->stream));
+  ctx->launches += 2;
+  if (d_out_point_w && n) CU(cudaMemcpyAsync(d_out_point_w, p.e, n * sizeof(double), cudaMemcpyDeviceToDevice, ctx->stream));
+  if (E) {
+    ctx->b_dseed_ok = true;
+    // stage 0's reweighting round linearised every edge (every window is in stage 0), as sgb_align_joint_gnc's does; every round since used
+    // robust_kind (NONE)
+    std::fill(ctx->b_lin.begin(), ctx->b_lin.end(), 1);
+    std::fill(ctx->b_seeded.begin(), ctx->b_seeded.end(), 1);
     ctx->have_lin = true;
     ctx->corr_seeds = true;
     ctx->lin_factor = o->factor_kind;

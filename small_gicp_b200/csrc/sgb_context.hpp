@@ -246,6 +246,10 @@ struct sgb_ctx {
   // sgb_align_batch_gnc_async: its instantiated loop of stages, with its key (it uses g_w, g_e and g_state as sgb_align_batch_gnc does)
   cudaGraphExec_t gnc_exec = nullptr;
   std::vector<unsigned char> gnc_key;
+  // sgb_align_joint_gnc_async: its instantiated loop of stages, with its key (it uses g_w, g_e and g_state as sgb_align_joint_gnc does, and
+  // joint_async with its ja_tab as sgb_align_joint_async does)
+  cudaGraphExec_t joint_gnc_exec = nullptr;
+  std::vector<unsigned char> joint_gnc_key;
 };
 
 namespace sgb {
