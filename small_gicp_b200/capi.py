@@ -52,6 +52,17 @@ def _align_options(factor=FACTOR_GICP, robust=ROBUST_NONE, robust_c=1.0, rejecto
     return o
 
 
+def _windows(windows, fixed, K, who):
+    """the window offsets and fixed flags of a joint call over K frames"""
+    off = np.ascontiguousarray(np.array([0, K] if windows is None else windows, dtype=np.uintp).reshape(-1))
+    if off.size < 1:
+        raise SgbError(f"{who}: windows needs at least one entry")
+    fx = None if fixed is None else np.ascontiguousarray(np.asarray(fixed).astype(np.uint8).reshape(-1))
+    if fx is not None and fx.size != K:
+        raise SgbError(f"{who}: fixed needs {K} entries")
+    return off, fx
+
+
 class GncOptions(C.Structure):
     """sgb_gnc_options"""
 
@@ -772,9 +783,8 @@ class Context:
         align_batch.  The weights in force (set_source_weights, one per edge point) apply."""
         K, Xc, off, fx = self._joint_args(init_X, windows, fixed, "align_joint")
         W = off.size - 1
-        o = AlignOptions(int(factor), int(robust), float(robust_c), int(rejector), float(max_dist_sq), int(optimizer), int(max_iterations), float(gn_lambda),
-                         int(max_inner_iterations), float(init_lambda), float(lambda_factor), float(rotation_eps), float(translation_eps))
-        o.dof_mask[:] = [1.0] * 6 if dof_mask is None else [float(x) for x in dof_mask]
+        o = _align_options(factor, robust, robust_c, rejector, max_dist_sq, optimizer, max_iterations, gn_lambda, max_inner_iterations, init_lambda,
+                           lambda_factor, rotation_eps, translation_eps, dof_mask)
         out = np.zeros((max(K, 1), 16))
         info = np.zeros((max(W, 1), 4))
         self._check(self._L.sgb_align_joint(self._h, C.byref(o), W, off.ctypes.data_as(C.POINTER(C.c_size_t)),
@@ -787,12 +797,7 @@ class Context:
         K = self._cloud_offsets.size - 1 if hasattr(self, "_cloud_offsets") else 0
         if X.shape != (K, 4, 4):
             raise SgbError(f"{who}: need ({K}, 4, 4) frame poses")
-        off = np.ascontiguousarray(np.array([0, K] if windows is None else windows, dtype=np.uintp).reshape(-1))
-        if off.size < 1:
-            raise SgbError(f"{who}: windows needs at least one entry")
-        fx = None if fixed is None else np.ascontiguousarray(np.asarray(fixed).astype(np.uint8).reshape(-1))
-        if fx is not None and fx.size != K:
-            raise SgbError(f"{who}: fixed needs {K} entries")
+        off, fx = _windows(windows, fixed, K, who)
         return K, np.ascontiguousarray(X.transpose(0, 2, 1)), off, fx
 
     def joint_edge_poses(self, X, windows=None):
@@ -835,30 +840,39 @@ class Context:
         poses are transposed into the library's column-major layout.  Returns an AsyncAlignResult of CUDA tensors (out: a previous result
         whose buffers are reused).  Inside torch.cuda.graph (with the capture stream set) the align is captured: each replay re-runs it
         from what init_Ts holds then, with the weights in force then (set_source_weights)."""
+
+        def outputs(B, N, zeros):
+            if out is None:
+                return AsyncAlignResult(zeros(B, 16), zeros(B, 4), zeros(B, 42))
+            if tuple(out.T16.shape) != (B, 16):
+                raise SgbError(f"align_batch_async: out holds {out.T16.shape[0]} members, the batch {B}")
+            return out
+
+        res = self._batch_async_in(init_Ts, "align_batch_async", outputs)
+        o = _align_options(factor, robust, robust_c, rejector, max_dist_sq, optimizer, max_iterations, gn_lambda, max_inner_iterations, init_lambda,
+                           lambda_factor, rotation_eps, translation_eps, dof_mask)
+        self._check(self._L.sgb_align_batch_async(self._h, C.byref(o), _d(self._async_in), _d(res.T16), _d(res.info4), _d(res.Hb42)))
+        return res
+
+    def _batch_async_in(self, init_Ts, who, outputs):
+        """the outputs of a stream-ordered batch call, with init_Ts transposed into _async_in (column-major) on the context's stream;
+        outputs(B, N, zeros) returns the call's result buffers for B members of N points in all, zeros(rows, cols) a new float64 tensor there"""
         import torch
 
         if self._stream is None:
-            raise SgbError("align_batch_async: set the context's stream to a torch stream first (set_stream): the poses are prepared on it")
+            raise SgbError(f"{who}: set the context's stream to a torch stream first (set_stream): the poses are prepared on it")
         offsets = getattr(self, "_batch_offsets", None)  # (no batch yet: the library says so)
         B = int(offsets.size) - 1 if offsets is not None else int(init_Ts.shape[0])
+        N = int(offsets[-1]) if offsets is not None else 0
         if not (isinstance(init_Ts, torch.Tensor) and init_Ts.is_cuda and init_Ts.dtype == torch.float64 and tuple(init_Ts.shape) == (B, 4, 4)):
-            raise SgbError(f"align_batch_async: init_Ts must be a CUDA float64 tensor of shape ({B}, 4, 4)")
-        o = AlignOptions(int(factor), int(robust), float(robust_c), int(rejector), float(max_dist_sq), int(optimizer), int(max_iterations), float(gn_lambda),
-                         int(max_inner_iterations), float(init_lambda), float(lambda_factor), float(rotation_eps), float(translation_eps))
-        o.dof_mask[:] = [1.0] * 6 if dof_mask is None else [float(x) for x in dof_mask]
+            raise SgbError(f"{who}: init_Ts must be a CUDA float64 tensor of shape ({B}, 4, 4)")
         dev = init_Ts.device
         with torch.cuda.stream(torch.cuda.ExternalStream(self._stream, device=dev)):
-            if out is None:
-                n = max(B, 1)
-                out = AsyncAlignResult(torch.zeros((n, 16), dtype=torch.float64, device=dev)[:B], torch.zeros((n, 4), dtype=torch.float64, device=dev)[:B],
-                                       torch.zeros((n, 42), dtype=torch.float64, device=dev)[:B])
-            elif tuple(out.T16.shape) != (B, 16):
-                raise SgbError(f"align_batch_async: out holds {out.T16.shape[0]} members, the batch {B}")
+            res = outputs(B, N, lambda rows, cols: torch.zeros((max(rows, 1), cols), dtype=torch.float64, device=dev)[:rows])
             if self._async_in is None or self._async_in.shape[0] != B or self._async_in.device != dev:
                 self._async_in = torch.empty((max(B, 1), 16), dtype=torch.float64, device=dev)[:B]
             self._async_in.view(B, 4, 4).copy_(init_Ts.transpose(1, 2))  # column-major
-        self._check(self._L.sgb_align_batch_async(self._h, C.byref(o), _d(self._async_in), _d(out.T16), _d(out.info4), _d(out.Hb42)))
-        return out
+        return res
 
     def align_batch_gnc_async(self, init_Ts, noise_bound_sq, gnc=GNC_TLS, max_stages=64, stage_iterations=3, point_weights=False, out=None, **align):
         """align_batch_gnc enqueued on the context's stream without a host synchronisation (sgb_align_batch_gnc_async): every stage and round
@@ -866,38 +880,23 @@ class Context:
         AsyncGncAlignResult of CUDA tensors (out: a previous result whose buffers are reused; it must hold point_w if point_weights).  Inside
         torch.cuda.graph (with the capture stream set) the whole GNC is captured: each replay re-runs it from what init_Ts holds then, with
         the weights in force then (set_source_weights)."""
-        import torch
 
-        if self._stream is None:
-            raise SgbError("align_batch_gnc_async: set the context's stream to a torch stream first (set_stream): the poses are prepared on it")
-        offsets = getattr(self, "_batch_offsets", None)  # (no batch yet: the library says so)
-        B = int(offsets.size) - 1 if offsets is not None else int(init_Ts.shape[0])
-        N = int(offsets[-1]) if offsets is not None else 0
-        if not (isinstance(init_Ts, torch.Tensor) and init_Ts.is_cuda and init_Ts.dtype == torch.float64 and tuple(init_Ts.shape) == (B, 4, 4)):
-            raise SgbError(f"align_batch_gnc_async: init_Ts must be a CUDA float64 tensor of shape ({B}, 4, 4)")
+        def outputs(B, N, zeros):
+            if out is None:
+                return AsyncGncAlignResult(zeros(B, 16), zeros(B, 4), zeros(B, 42), zeros(B, 2), zeros(N, 1)[:, 0] if point_weights else None)
+            if tuple(out.T16.shape) != (B, 16):
+                raise SgbError(f"align_batch_gnc_async: out holds {out.T16.shape[0]} members, the batch {B}")
+            if point_weights and (out.point_w is None or tuple(out.point_w.shape) != (N,)):
+                raise SgbError(f"align_batch_gnc_async: point_weights needs out.point_w of {N} rows")
+            return out
+
+        res = self._batch_async_in(init_Ts, "align_batch_gnc_async", outputs)
         o = _align_options(**align)
         g = GncOptions(int(gnc), float(noise_bound_sq), int(max_stages), int(stage_iterations))
-        dev = init_Ts.device
-        with torch.cuda.stream(torch.cuda.ExternalStream(self._stream, device=dev)):
-            if out is None:
-                n = max(B, 1)
-
-                def zeros(rows, cols):
-                    return torch.zeros((n, cols), dtype=torch.float64, device=dev)[:rows]
-
-                pw = torch.zeros(max(N, 1), dtype=torch.float64, device=dev)[:N] if point_weights else None
-                out = AsyncGncAlignResult(zeros(B, 16), zeros(B, 4), zeros(B, 42), zeros(B, 2), pw)
-            elif tuple(out.T16.shape) != (B, 16):
-                raise SgbError(f"align_batch_gnc_async: out holds {out.T16.shape[0]} members, the batch {B}")
-            elif point_weights and (out.point_w is None or tuple(out.point_w.shape) != (N,)):
-                raise SgbError(f"align_batch_gnc_async: point_weights needs out.point_w of {N} rows")
-            if self._async_in is None or self._async_in.shape[0] != B or self._async_in.device != dev:
-                self._async_in = torch.empty((max(B, 1), 16), dtype=torch.float64, device=dev)[:B]
-            self._async_in.view(B, 4, 4).copy_(init_Ts.transpose(1, 2))  # column-major
-        pw = out.point_w if point_weights else None
-        self._check(self._L.sgb_align_batch_gnc_async(self._h, C.byref(o), C.byref(g), _d(self._async_in), _d(out.T16), _d(out.info4), _d(out.Hb42),
-                                                      _d(out.gnc2), _d(pw)))
-        return out
+        pw = res.point_w if point_weights else None
+        self._check(self._L.sgb_align_batch_gnc_async(self._h, C.byref(o), C.byref(g), _d(self._async_in), _d(res.T16), _d(res.info4), _d(res.Hb42),
+                                                      _d(res.gnc2), _d(pw)))
+        return res
 
     def align_joint_async(self, init_X, windows=None, fixed=None, factor=FACTOR_GICP, robust=ROBUST_NONE, robust_c=1.0, rejector=REJECT_DISTANCE,
                           max_dist_sq=1.0, optimizer=OPT_LEVENBERG_MARQUARDT, max_iterations=20, gn_lambda=1e-6, max_inner_iterations=10, init_lambda=1e-3,
@@ -907,9 +906,8 @@ class Context:
         other keywords as in align_joint.  Returns an AsyncJointAlignResult of CUDA tensors (out: a previous result whose buffers are reused).
         Inside torch.cuda.graph (with the capture stream set) the align is captured: each replay re-runs it from what init_X holds then.
         The weights in force (set_source_weights) apply, at a replay those in force then."""
-        o = AlignOptions(int(factor), int(robust), float(robust_c), int(rejector), float(max_dist_sq), int(optimizer), int(max_iterations), float(gn_lambda),
-                         int(max_inner_iterations), float(init_lambda), float(lambda_factor), float(rotation_eps), float(translation_eps))
-        o.dof_mask[:] = [1.0] * 6 if dof_mask is None else [float(x) for x in dof_mask]
+        o = _align_options(factor, robust, robust_c, rejector, max_dist_sq, optimizer, max_iterations, gn_lambda, max_inner_iterations, init_lambda,
+                           lambda_factor, rotation_eps, translation_eps, dof_mask)
 
         def outputs(K, W, zeros):
             if out is None:
@@ -934,13 +932,8 @@ class Context:
         K = self._cloud_offsets.size - 1 if hasattr(self, "_cloud_offsets") else 0
         if not (isinstance(init_X, torch.Tensor) and init_X.is_cuda and init_X.dtype == torch.float64 and tuple(init_X.shape) == (K, 4, 4)):
             raise SgbError(f"{who}: init_X must be a CUDA float64 tensor of shape ({K}, 4, 4)")
-        off = np.ascontiguousarray(np.array([0, K] if windows is None else windows, dtype=np.uintp).reshape(-1))
-        if off.size < 1:
-            raise SgbError(f"{who}: windows needs at least one entry")
+        off, fx = _windows(windows, fixed, K, who)
         W = off.size - 1
-        fx = None if fixed is None else np.ascontiguousarray(np.asarray(fixed).astype(np.uint8).reshape(-1))
-        if fx is not None and fx.size != K:
-            raise SgbError(f"{who}: fixed needs {K} entries")
         dev = init_X.device
         with torch.cuda.stream(torch.cuda.ExternalStream(self._stream, device=dev)):
             res = outputs(K, W, lambda rows, cols: torch.zeros((max(rows, 1), cols), dtype=torch.float64, device=dev)[:rows])

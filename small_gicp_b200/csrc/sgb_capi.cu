@@ -86,10 +86,7 @@ void forget_linearisation(sgb_ctx* ctx) {
   ctx->corr_seeds = false;
   ctx->b_view_ok = false;  // the target (or the pairing) it was built from may have changed
   ctx->b_dseed_ok = false;
-  ctx->align_key.clear();  // sgb_align_batch_async rebuilds its loop graph
-  ctx->joint_key.clear();  // and sgb_align_joint_async its own
-  ctx->gnc_key.clear();    // and sgb_align_batch_gnc_async its own
-  ctx->joint_gnc_key.clear();  // and sgb_align_joint_gnc_async its own
+  for (LoopGraph* g : {&ctx->align_loop, &ctx->joint_loop, &ctx->gnc_loop, &ctx->joint_gnc_loop}) g->key.clear();  // every async align rebuilds its loop
 }
 
 }  // namespace
@@ -645,14 +642,10 @@ void sgb_destroy(sgb_ctx* ctx) {
   if (ctx->ev_entry) cudaEventDestroy(ctx->ev_entry);
   for (int k = 0; k < sgb_ctx::kUploadChunks; k++)
     if (ctx->ev_upload[k]) cudaEventDestroy(ctx->ev_upload[k]);
-  if (ctx->align_exec) cudaGraphExecDestroy(ctx->align_exec);
-  if (ctx->joint_exec) cudaGraphExecDestroy(ctx->joint_exec);
-  if (ctx->gnc_exec) cudaGraphExecDestroy(ctx->gnc_exec);
-  if (ctx->joint_gnc_exec) cudaGraphExecDestroy(ctx->joint_gnc_exec);
   if (ctx->cap_stream) cudaStreamDestroy(ctx->cap_stream);
   if (ctx->cap_stream_nested) cudaStreamDestroy(ctx->cap_stream_nested);
   if (ctx->own_stream) cudaStreamDestroy(ctx->own_stream);
-  delete ctx;  // every DevBuf member frees its allocation (the context's device is current)
+  delete ctx;  // every DevBuf and LoopGraph member frees what it owns (the context's device is current)
 }
 
 const char* sgb_last_error(const sgb_ctx* ctx) { return ctx ? ctx->err.c_str() : g_create_error.c_str(); }

@@ -10,6 +10,7 @@
 #include <cmath>
 #include <cstdio>
 #include <cstring>
+#include <initializer_list>
 #include <string>
 #include <vector>
 
@@ -278,6 +279,24 @@ int round_kernels(sgb_ctx* ctx, const LinParams& P, const BatchParams& Bp, const
   return 0;
 }
 
+// What a linearize leaves in the context: the members of the mask (null: every member) linearised against the current target, their
+// correspondences usable as seeds, and its factor and robust kernel for error()
+void mark_linearised(sgb_ctx* ctx, int factor, int robust, double robust_c, const uint8_t* members) {
+  // a new target (or none linearised yet) invalidates every member's cached state; sgb_drop_seeds only the seeds
+  if (!ctx->have_lin) std::fill(ctx->b_lin.begin(), ctx->b_lin.end(), 0);
+  if (!ctx->corr_seeds) std::fill(ctx->b_seeded.begin(), ctx->b_seeded.end(), 0);
+  for (size_t m = 0; m < ctx->b_lin.size(); m++) {
+    if (members && !members[m]) continue;
+    ctx->b_lin[m] = 1;
+    ctx->b_seeded[m] = 1;
+  }
+  ctx->have_lin = true;
+  ctx->corr_seeds = true;
+  ctx->lin_factor = factor;
+  ctx->lin_robust = robust;
+  ctx->lin_c = robust_c;
+}
+
 // One linearize of the active members (arguments checked by the caller) into b_out, asynchronous.  T = nullptr: poses already in b_poses.
 // rows: the factor kernel's per-point rows too (the rows it does not reach are the caller's to clear: point_rows).
 int linearize_round(sgb_ctx* ctx, int factor, int robust, double robust_c, int rejector, double max_dist_sq, const double* T, const uint8_t* active,
@@ -285,7 +304,7 @@ int linearize_round(sgb_ctx* ctx, int factor, int robust, double robust_c, int r
   const size_t B = batch_members(ctx);
   CU(cudaSetDevice(ctx->device));
   const bool voxel = voxel_target(ctx);
-  // a new target (or none linearised yet) invalidates every member's cached state; sgb_drop_seeds only the seeds
+  // the same reset as mark_linearised's, here because batch_tables reads the seed flags
   if (!ctx->have_lin) std::fill(ctx->b_lin.begin(), ctx->b_lin.end(), 0);
   if (!ctx->corr_seeds) std::fill(ctx->b_seeded.begin(), ctx->b_seeded.end(), 0);
   uint32_t n_tiles = 0, n_virtual = 0;
@@ -310,16 +329,7 @@ int linearize_round(sgb_ctx* ctx, int factor, int robust, double robust_c, int r
   }
   CU(launch_batch_segment(Bp, static_cast<uint32_t>(B), true, nullptr, ctx->b_out.as<double>(), ctx->stream));
   ctx->launches += 1;
-  for (size_t m = 0; m < B; m++) {
-    if (active && !active[m]) continue;
-    ctx->b_lin[m] = 1;
-    ctx->b_seeded[m] = 1;
-  }
-  ctx->have_lin = true;
-  ctx->corr_seeds = true;
-  ctx->lin_factor = factor;
-  ctx->lin_robust = robust;
-  ctx->lin_c = robust_c;
+  mark_linearised(ctx, factor, robust, robust_c, active);
   return 0;
 }
 
@@ -566,32 +576,29 @@ auto round_loop(sgb_ctx* ctx, const sgb_align_options* o, Step step) {
 }
 
 // One launch of a device loop on ctx->stream.  While the stream is captured the WHILE node joins the capture (capture_loop); otherwise
-// the instantiated graph cached in exec under cached_key is launched, rebuilt first when key (everything the loop captured) differs from it.
+// the instantiated graph cached in graph is launched, rebuilt first when key (everything the loop captured) differs from graph's.
 template <typename Body>
-int launch_loop(sgb_ctx* ctx, const char* who, bool capturing, std::vector<unsigned char> key, cudaGraphExec_t& exec, std::vector<unsigned char>& cached_key,
-                Body body) {
+int launch_loop(sgb_ctx* ctx, const char* who, bool capturing, std::vector<unsigned char> key, LoopGraph& graph, Body body) {
   if (capturing) {
     cudaGraphConditionalHandle h;
     if (int rc = loop_handle(ctx, who, nullptr, &h)) return rc;
     return capture_loop(ctx, h, body);
   }
-  if (!exec || key != cached_key) {
-    if (exec) cudaGraphExecDestroy(exec);
-    exec = nullptr;
-    cached_key.clear();
+  if (!graph.exec || key != graph.key) {
+    graph.drop();
     cudaGraph_t g = nullptr;
     CU(cudaGraphCreate(&g, 0));
     cudaGraphConditionalHandle h;
     cudaGraphNode_t w = nullptr;
     int rc = loop_handle(ctx, who, g, &h);
     if (!rc) rc = add_loop(ctx, g, {}, h, &w, body);
-    const cudaError_t e = rc ? cudaSuccess : cudaGraphInstantiate(&exec, g, 0);
+    const cudaError_t e = rc ? cudaSuccess : cudaGraphInstantiate(&graph.exec, g, 0);
     cudaGraphDestroy(g);
     if (rc) return rc;
     CU(e);
-    cached_key.swap(key);
+    graph.key.swap(key);
   }
-  CU(cudaGraphLaunch(exec, ctx->stream));
+  CU(cudaGraphLaunch(graph.exec, ctx->stream));
   return 0;
 }
 
@@ -649,11 +656,26 @@ bool on_device(const sgb_ctx* ctx, const void* p) {
   return e == cudaSuccess && a.type == cudaMemoryTypeDevice && a.device == ctx->device;
 }
 
-// the same as a check of who's argument; what names p in the message
-int device_pointer(sgb_ctx* ctx, const char* who, const void* p, const char* what) {
-  if (!on_device(ctx, p))
-    return fail(ctx, 1, std::string(who) + ": " + what + " must be device memory of the context's GPU (cuda:" + std::to_string(ctx->device) +
-                            "); host, page-locked and managed memory are refused");
+// The check of who's device-memory arguments: each given one (a required one always) must be device memory of the context's GPU
+struct DeviceArg {
+  const void* p;
+  const char* name;
+  bool required;
+};
+int device_pointers(sgb_ctx* ctx, const std::string& who, std::initializer_list<DeviceArg> args) {
+  for (const DeviceArg& a : args)
+    if ((a.required || a.p) && !on_device(ctx, a.p))
+      return fail(ctx, 1, who + ": " + a.name + " must be device memory of the context's GPU (cuda:" + std::to_string(ctx->device) +
+                              "); host, page-locked and managed memory are refused");
+  return 0;
+}
+
+// Whether ctx->stream is being captured (an invalidated capture fails who's call)
+int capture_state(sgb_ctx* ctx, const std::string& who, bool* capturing) {
+  cudaStreamCaptureStatus capture = cudaStreamCaptureStatusNone;
+  CU(cudaStreamIsCapturing(ctx->stream, &capture));
+  if (capture == cudaStreamCaptureStatusInvalidated) return fail(ctx, 1, who + ": the context's stream is in an invalidated capture");
+  *capturing = capture == cudaStreamCaptureStatusActive;
   return 0;
 }
 
@@ -802,8 +824,9 @@ int align_start(sgb_ctx* ctx, const AlignOptions& ao, const double* init_T, std:
   return 0;
 }
 
-// The outputs of an align from the members' final state; gnc (or null): the iterations of their earlier GNC stages are added
-void align_results(const std::vector<MemberState>& state, const GncState* gnc, double* out_T, double* out_info, double* out_Hb) {
+// The outputs of an align from the members' final state; gnc (or null): the iterations of their earlier GNC stages are added, and
+// out_gnc2 (or null) gets each member's stages and mu
+void align_results(const std::vector<MemberState>& state, const GncState* gnc, double* out_T, double* out_info, double* out_Hb, double* out_gnc2) {
   for (size_t m = 0; m < state.size(); m++) {
     const MemberState& s = state[m];
     std::memcpy(out_T + 16 * m, s.T, 16 * sizeof(double));
@@ -815,6 +838,10 @@ void align_results(const std::vector<MemberState>& state, const GncState* gnc, d
     if (out_Hb) {
       std::memcpy(out_Hb + 42 * m, s.H, 36 * sizeof(double));
       std::memcpy(out_Hb + 42 * m + 36, s.b, 6 * sizeof(double));
+    }
+    if (out_gnc2) {
+      out_gnc2[2 * m] = gnc[m].stages;
+      out_gnc2[2 * m + 1] = gnc[m].mu;
     }
   }
 }
@@ -880,17 +907,43 @@ int gnc_checks(sgb_ctx* ctx, const std::string& who, const sgb_align_options* o,
 
 // A synchronous GNC call refuses a captured stream: it synchronises at every round and stage to plan the next one
 int gnc_capture_check(sgb_ctx* ctx, const std::string& who) {
-  cudaStreamCaptureStatus capture = cudaStreamCaptureStatusNone;
-  CU(cudaStreamIsCapturing(ctx->stream, &capture));
-  if (capture != cudaStreamCaptureStatusNone)
+  bool capturing = false;
+  if (int rc = capture_state(ctx, who, &capturing)) return rc;
+  if (capturing)
     return fail(ctx, 1, who + ": the context's stream is being captured, and the call synchronises at every round and stage to plan the next one; call it "
                               "outside the capture");
   return 0;
 }
 
-// the bytes of g_w, g_e and g_state a GNC align of the batch uses
+// the bytes of g_w and g_e (a double per member point) and of g_state (GncState | live flag per unit) a GNC align of n_units units
+// (members or windows) uses
 size_t gnc_w_bytes(const sgb_ctx* ctx) { return std::max<size_t>(batch_points(ctx), 1) * sizeof(double); }
-size_t gnc_state_bytes(const sgb_ctx* ctx) { return batch_members(ctx) * (sizeof(GncState) + 1); }
+size_t gnc_state_bytes(size_t n_units) { return n_units * (sizeof(GncState) + 1); }
+bool gnc_allocates(const sgb_ctx* ctx, size_t n_units) {
+  return ctx->g_w.cap < gnc_w_bytes(ctx) || ctx->g_e.cap < gnc_w_bytes(ctx) || ctx->g_state.cap < gnc_state_bytes(n_units);
+}
+int reserve_gnc(sgb_ctx* ctx, size_t n_units) {
+  CU(ctx->g_w.reserve(gnc_w_bytes(ctx)));
+  CU(ctx->g_e.reserve(gnc_w_bytes(ctx)));
+  CU(ctx->g_state.reserve(gnc_state_bytes(n_units)));
+  return 0;
+}
+
+// A stream-ordered align's first-use allocations, which a capture cannot hold: the packet search's queue (queue), the capture stream of
+// its loop (loops = 1) and of a loop nested in it (loops = 2), and the GNC buffers of gnc_units units (0: none).  extra: the call's own
+// (an upload of its tables).  Inside a capture a call that needs any fails with who + refusal; outside, the queue and the GNC buffers
+// are reserved here (add_loop makes the streams).
+int loop_allocations(sgb_ctx* ctx, const std::string& who, bool capturing, bool extra, bool queue, int loops, size_t gnc_units, const char* refusal) {
+  const bool no_queue = queue && ctx->use_packet_queue && !ctx->packet_queue.p;
+  const bool allocates = extra || no_queue || (loops > 0 && !ctx->cap_stream) || (loops > 1 && !ctx->cap_stream_nested) ||
+                         (gnc_units && gnc_allocates(ctx, gnc_units));
+  if (capturing && allocates) return fail(ctx, 1, who + refusal);
+  if (no_queue) {
+    CU(ctx->packet_queue.reserve(2 * sizeof(uint32_t)));
+    CU(cudaMemsetAsync(ctx->packet_queue.p, 0, 2 * sizeof(uint32_t), ctx->stream));
+  }
+  return gnc_units ? reserve_gnc(ctx, gnc_units) : 0;
+}
 
 // The GNC kernels' parameters of a call over g_w, g_e and g_state (reserved for the batch)
 GncParams gnc_params(sgb_ctx* ctx, const sgb_gnc_options* gnc) {
@@ -909,6 +962,33 @@ GncParams gnc_params(sgb_ctx* ctx, const sgb_gnc_options* gnc) {
   gp.gnc = ctx->g_state.as<GncState>();
   gp.live = reinterpret_cast<uint8_t*>(gp.gnc + gp.n_members);
   return gp;
+}
+
+// Every one of n_units units starts its stage 0: zero GNC state (r2max = 0, no stage begun, no iterations), live
+int gnc_begin(sgb_ctx* ctx, const GncParams& p, size_t n_units) {
+  CU(cudaMemsetAsync(p.gnc, 0, n_units * sizeof(GncState), ctx->stream));
+  CU(cudaMemsetAsync(p.live, 1, n_units, ctx->stream));
+  return 0;
+}
+
+// the rows of a reweighting round: each point's e into g_e
+BatchRows gnc_rows(const GncParams& p) {
+  BatchRows rows = {};
+  rows.member_off = p.member_off;
+  rows.perm = p.perm;
+  rows.e = p.e;
+  return rows;
+}
+
+// The GNC part of a stage loop's key: the GNC options and every buffer the GNC kernels use (more: the call's own)
+void gnc_key(std::vector<unsigned char>& k, const GncParams& p, std::initializer_list<const void*> more) {
+  for (int v : {p.kind, p.max_stages, p.stage_iterations}) key_add(k, v);
+  key_add(k, p.c2);
+  for (const void* v : {static_cast<const void*>(p.member_off), static_cast<const void*>(p.perm), static_cast<const void*>(p.corr),
+                        static_cast<const void*>(p.e), static_cast<const void*>(p.w), static_cast<const void*>(p.wstage), static_cast<const void*>(p.gnc),
+                        static_cast<const void*>(p.live)})
+    key_add(k, v);
+  for (const void* v : more) key_add(k, v);
 }
 
 }  // namespace
@@ -1149,7 +1229,7 @@ int sgb_align_batch(sgb_ctx* ctx, const sgb_align_options* o, const double* init
     return rc;
   CU(cudaMemcpyAsync(state.data(), ctx->b_state.p, B * sizeof(MemberState), cudaMemcpyDeviceToHost, ctx->stream));
   CU(cudaStreamSynchronize(ctx->stream));
-  align_results(state, nullptr, out_T, out_info, out_Hb);
+  align_results(state, nullptr, out_T, out_info, out_Hb, nullptr);
   return 0;
 }
 
@@ -1164,21 +1244,13 @@ int sgb_align_batch_gnc(sgb_ctx* ctx, const sgb_align_options* o, const sgb_gnc_
   const size_t B = batch_members(ctx), n = batch_points(ctx);
   if (B == 0) return 0;
   if (int rc = pair_view(ctx)) return rc;
-  CU(ctx->g_w.reserve(gnc_w_bytes(ctx)));
-  CU(ctx->g_e.reserve(gnc_w_bytes(ctx)));
-  CU(ctx->g_state.reserve(gnc_state_bytes(ctx)));
+  if (int rc = reserve_gnc(ctx, B)) return rc;
   std::vector<MemberState> state;
   std::vector<uint8_t> phase;
   if (int rc = align_start(ctx, ao, init_T, state, phase)) return rc;
-  // every member starts its stage 0: zero GNC state (r2max = 0, no stage begun), live
-  std::vector<unsigned char> g0(B * (sizeof(GncState) + 1), 0);
-  std::fill(g0.begin() + B * sizeof(GncState), g0.end(), 1);
-  CU(cudaMemcpyAsync(ctx->g_state.p, g0.data(), g0.size(), cudaMemcpyHostToDevice, ctx->stream));
   const GncParams gp = gnc_params(ctx, gnc);
-  BatchRows rows = {};
-  rows.member_off = gp.member_off;
-  rows.perm = gp.perm;
-  rows.e = gp.e;
+  if (int rc = gnc_begin(ctx, gp, B)) return rc;
+  const BatchRows rows = gnc_rows(gp);
   RoundWeights weights(ctx);
   std::vector<uint8_t> live(B, 1);
   for (int stage = 0; std::find(live.begin(), live.end(), 1) != live.end(); stage++) {
@@ -1209,13 +1281,7 @@ int sgb_align_batch_gnc(sgb_ctx* ctx, const sgb_align_options* o, const sgb_gnc_
   CU(cudaMemcpyAsync(g.data(), gp.gnc, B * sizeof(GncState), cudaMemcpyDeviceToHost, ctx->stream));
   if (out_point_w && n) CU(cudaMemcpyAsync(out_point_w, gp.e, n * sizeof(double), cudaMemcpyDefault, ctx->stream));
   CU(cudaStreamSynchronize(ctx->stream));
-  align_results(state, g.data(), out_T, out_info, out_Hb);
-  if (out_gnc2) {
-    for (size_t m = 0; m < B; m++) {
-      out_gnc2[2 * m] = g[m].stages;
-      out_gnc2[2 * m + 1] = g[m].mu;
-    }
-  }
+  align_results(state, g.data(), out_T, out_info, out_Hb, out_gnc2);
   return 0;
 }
 
@@ -1228,41 +1294,18 @@ int sgb_align_batch_gnc_async(sgb_ctx* ctx, const sgb_align_options* o, const sg
   const size_t B = batch_members(ctx), n = batch_points(ctx);
   if (B == 0) return 0;
   CU(cudaSetDevice(ctx->device));
-  if (int rc = device_pointer(ctx, who, d_init_T, "init_T16xB")) return rc;
-  if (int rc = device_pointer(ctx, who, d_out_T, "out_T16xB")) return rc;
-  if (int rc = device_pointer(ctx, who, d_out_info, "out_info4xB")) return rc;
-  if (d_out_Hb) {
-    if (int rc = device_pointer(ctx, who, d_out_Hb, "out_Hb42xB")) return rc;
-  }
-  if (d_out_gnc2) {
-    if (int rc = device_pointer(ctx, who, d_out_gnc2, "out_gnc2xB")) return rc;
-  }
-  if (d_out_point_w) {
-    if (int rc = device_pointer(ctx, who, d_out_point_w, "out_point_w")) return rc;
-  }
-  cudaStreamCaptureStatus capture = cudaStreamCaptureStatusNone;
-  CU(cudaStreamIsCapturing(ctx->stream, &capture));
-  if (capture == cudaStreamCaptureStatusInvalidated) return fail(ctx, 1, std::string(who) + ": the context's stream is in an invalidated capture");
-  const bool capturing = capture == cudaStreamCaptureStatusActive;
-  // A capture can hold no allocation: the GNC buffers, the packet queue and both capture streams (the stages' loop and the rounds' loop
-  // nested in it) must come from an earlier call
-  const bool allocates = ctx->g_w.cap < gnc_w_bytes(ctx) || ctx->g_e.cap < gnc_w_bytes(ctx) || ctx->g_state.cap < gnc_state_bytes(ctx) ||
-                         (ctx->use_packet_queue && !ctx->packet_queue.p) || !ctx->cap_stream || !ctx->cap_stream_nested;
-  if (capturing && allocates)
-    return fail(ctx, 1, std::string(who) + ": this call needs an allocation, which a capture cannot hold; call it once outside the capture first");
-  if (ctx->use_packet_queue && !ctx->packet_queue.p) {
-    CU(ctx->packet_queue.reserve(2 * sizeof(uint32_t)));
-    CU(cudaMemsetAsync(ctx->packet_queue.p, 0, 2 * sizeof(uint32_t), ctx->stream));
-  }
-  CU(ctx->g_w.reserve(gnc_w_bytes(ctx)));
-  CU(ctx->g_e.reserve(gnc_w_bytes(ctx)));
-  CU(ctx->g_state.reserve(gnc_state_bytes(ctx)));
+  if (int rc = device_pointers(ctx, who, {{d_init_T, "init_T16xB", true}, {d_out_T, "out_T16xB", true}, {d_out_info, "out_info4xB", true},
+                                          {d_out_Hb, "out_Hb42xB", false}, {d_out_gnc2, "out_gnc2xB", false}, {d_out_point_w, "out_point_w", false}}))
+    return rc;
+  bool capturing = false;
+  if (int rc = capture_state(ctx, who, &capturing)) return rc;
+  // the GNC buffers, the packet queue and both capture streams (the stages' loop and the rounds' loop nested in it)
+  if (int rc = loop_allocations(ctx, who, capturing, false, true, 2, B,
+                                ": this call needs an allocation, which a capture cannot hold; call it once outside the capture first"))
+    return rc;
   if (int rc = pair_view(ctx)) return rc;
   const GncParams gp = gnc_params(ctx, gnc);
-  BatchRows rows = {};
-  rows.member_off = gp.member_off;
-  rows.perm = gp.perm;
-  rows.e = gp.e;
+  const BatchRows rows = gnc_rows(gp);
   const uint32_t nb = static_cast<uint32_t>(B);
   MemberState* state = ctx->b_state.as<MemberState>();
   double* poses = ctx->b_poses.as<double>();
@@ -1270,8 +1313,7 @@ int sgb_align_batch_gnc_async(sgb_ctx* ctx, const sgb_align_options* o, const sg
   // sgb_align_batch_gnc's initial state: every member's align_init at its initial pose, zero GNC state, every member live (the seed flags
   // kept as sgb_align_batch_async keeps them)
   CU(launch_batch_align_init(ao, nb, d_init_T, state, poses, phase, ctx->b_dseed.as<uint8_t>(), ctx->corr_seeds && ctx->b_dseed_ok, ctx->stream));
-  CU(cudaMemsetAsync(gp.gnc, 0, B * sizeof(GncState), ctx->stream));
-  CU(cudaMemsetAsync(gp.live, 1, B, ctx->stream));
+  if (int rc = gnc_begin(ctx, gp, B)) return rc;
   ctx->launches += 3;  // the initial state here, the outputs below
   // One stage per iteration of the outer loop, in sgb_align_batch_gnc's order: the reweighting linearize of the members in the stage
   // (planned by batch_plan_kernel from their phases), the stage kernels, then the stage's align as an inner loop of rounds.  After
@@ -1298,14 +1340,9 @@ int sgb_align_batch_gnc_async(sgb_ctx* ctx, const sgb_align_options* o, const sg
   std::vector<unsigned char> key;
   if (!capturing) {  // loop_key, plus the GNC options and every buffer the GNC kernels use
     key = loop_key(ctx, o);
-    for (int v : {gp.kind, gp.max_stages, gp.stage_iterations}) key_add(key, v);
-    key_add(key, gp.c2);
-    for (const void* v : {static_cast<const void*>(gp.member_off), static_cast<const void*>(gp.perm), static_cast<const void*>(gp.corr),
-                          static_cast<const void*>(gp.e), static_cast<const void*>(gp.w), static_cast<const void*>(gp.wstage),
-                          static_cast<const void*>(gp.gnc)})
-      key_add(key, v);
+    gnc_key(key, gp, {});
   }
-  if (int rc = launch_loop(ctx, who, capturing, std::move(key), ctx->gnc_exec, ctx->gnc_key, stage)) return rc;
+  if (int rc = launch_loop(ctx, who, capturing, std::move(key), ctx->gnc_loop, stage)) return rc;
   ctx->launches += 1;
   if (int rc = clear_search_counters(ctx)) return rc;
   CU(launch_batch_align_finish(nb, state, d_out_T, d_out_info, d_out_Hb, ctx->stream));
@@ -1313,13 +1350,7 @@ int sgb_align_batch_gnc_async(sgb_ctx* ctx, const sgb_align_options* o, const sg
   if (d_out_point_w && n) CU(cudaMemcpyAsync(d_out_point_w, gp.e, n * sizeof(double), cudaMemcpyDeviceToDevice, ctx->stream));
   ctx->b_dseed_ok = true;
   // stage 0's reweighting round linearised every member, as sgb_align_batch_gnc's does; every round since used robust_kind (NONE)
-  std::fill(ctx->b_lin.begin(), ctx->b_lin.end(), 1);
-  std::fill(ctx->b_seeded.begin(), ctx->b_seeded.end(), 1);
-  ctx->have_lin = true;
-  ctx->corr_seeds = true;
-  ctx->lin_factor = o->factor_kind;
-  ctx->lin_robust = o->robust_kind;
-  ctx->lin_c = o->robust_c;
+  mark_linearised(ctx, o->factor_kind, o->robust_kind, o->robust_c, nullptr);
   return 0;
 }
 
@@ -1534,6 +1565,25 @@ int joint_async_tables(sgb_ctx* ctx, const JointLayout& L, bool upload) {
   return 0;
 }
 
+// The outputs of a joint align from the frames' final X and the windows' final state, a fixed frame's X as init_X gives it; gnc (or
+// null): the iterations of the windows' earlier GNC stages are added, and out_gnc2 (or null) gets each window's stages and mu
+void joint_results(const JointLayout& L, const double* init_X, const std::vector<double>& X, const std::vector<WindowState>& state, const GncState* gnc,
+                   double* out_X, double* out_info, double* out_gnc2) {
+  const int32_t* freeidx = L.free();
+  for (size_t k = 0; k < L.K; k++) std::memcpy(out_X + 16 * k, freeidx[k] < 0 ? init_X + 16 * k : X.data() + 16 * k, 16 * sizeof(double));
+  for (size_t w = 0; w < L.W; w++) {
+    double* info = out_info + 4 * w;
+    info[0] = state[w].converged ? 1.0 : 0.0;
+    info[1] = state[w].iterations + (gnc ? gnc[w].iterations : 0);
+    info[2] = state[w].inliers;
+    info[3] = state[w].e;
+    if (out_gnc2) {
+      out_gnc2[2 * w] = gnc[w].stages;
+      out_gnc2[2 * w + 1] = gnc[w].mu;
+    }
+  }
+}
+
 }  // namespace
 
 extern "C" {
@@ -1573,15 +1623,7 @@ int sgb_align_joint(sgb_ctx* ctx, const sgb_align_options* o, size_t n_windows, 
   if (K) CU(cudaMemcpyAsync(X.data(), ctx->joint.X.p, K * 16 * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
   if (W) CU(cudaMemcpyAsync(state.data(), ctx->joint.state.p, W * sizeof(WindowState), cudaMemcpyDeviceToHost, ctx->stream));
   CU(cudaStreamSynchronize(ctx->stream));
-  const int32_t* freeidx = L.free();
-  for (size_t k = 0; k < K; k++) std::memcpy(out_X + 16 * k, freeidx[k] < 0 ? init_X + 16 * k : X.data() + 16 * k, 16 * sizeof(double));
-  for (size_t w = 0; w < W; w++) {
-    double* info = out_info + 4 * w;
-    info[0] = state[w].converged ? 1.0 : 0.0;
-    info[1] = state[w].iterations;
-    info[2] = state[w].inliers;
-    info[3] = state[w].e;
-  }
+  joint_results(L, init_X, X, state, nullptr, out_X, out_info, nullptr);
   return 0;
 }
 
@@ -1628,26 +1670,19 @@ int sgb_align_joint_gnc(sgb_ctx* ctx, const sgb_align_options* o, const sgb_gnc_
   if (E) {
     if (int rc = pair_view(ctx)) return rc;
   }
-  CU(ctx->g_w.reserve(gnc_w_bytes(ctx)));
-  CU(ctx->g_e.reserve(gnc_w_bytes(ctx)));
-  CU(ctx->g_state.reserve(W * (sizeof(GncState) + 1)));
+  if (int rc = reserve_gnc(ctx, W)) return rc;
   if (int rc = joint_upload(ctx, L, init_X)) return rc;
   const JointParams J = joint_params(ctx, ctx->joint, W, E);
   const uint32_t* member_win = ctx->joint.tables.as<uint32_t>() + L.member_win_at();
   // the GNC state per window: p for the point kernels (over the edges' points), pw for the window kernels; every window starts its
-  // stage 0 with zero GNC and window state (r2max = 0, no stage begun, no iterations), live
+  // stage 0 with zero GNC and window state, live
   GncParams p = gnc_params(ctx, gnc);
   p.live = reinterpret_cast<uint8_t*>(p.gnc + W);
   GncParams pw = p;
   pw.n_members = static_cast<uint32_t>(W);
-  std::vector<unsigned char> g0(W * (sizeof(GncState) + 1), 0);
-  std::fill(g0.begin() + W * sizeof(GncState), g0.end(), 1);
-  CU(cudaMemcpyAsync(ctx->g_state.p, g0.data(), g0.size(), cudaMemcpyHostToDevice, ctx->stream));
+  if (int rc = gnc_begin(ctx, p, W)) return rc;
   CU(cudaMemsetAsync(ctx->joint.state.p, 0, W * sizeof(WindowState), ctx->stream));
-  BatchRows rows = {};
-  rows.member_off = p.member_off;
-  rows.perm = p.perm;
-  rows.e = p.e;
+  const BatchRows rows = gnc_rows(p);
   RoundWeights weights(ctx);
   const uint32_t* edge_member = L.edge_member();
   const uint32_t* edge_win = L.edge_win();
@@ -1691,19 +1726,7 @@ int sgb_align_joint_gnc(sgb_ctx* ctx, const sgb_align_options* o, const sgb_gnc_
   CU(cudaMemcpyAsync(g.data(), p.gnc, W * sizeof(GncState), cudaMemcpyDeviceToHost, ctx->stream));
   if (out_point_w && n) CU(cudaMemcpyAsync(out_point_w, p.e, n * sizeof(double), cudaMemcpyDefault, ctx->stream));
   CU(cudaStreamSynchronize(ctx->stream));
-  const int32_t* freeidx = L.free();
-  for (size_t k = 0; k < K; k++) std::memcpy(out_X + 16 * k, freeidx[k] < 0 ? init_X + 16 * k : X.data() + 16 * k, 16 * sizeof(double));
-  for (size_t w = 0; w < W; w++) {
-    double* info = out_info + 4 * w;
-    info[0] = state[w].converged ? 1.0 : 0.0;
-    info[1] = state[w].iterations + g[w].iterations;
-    info[2] = state[w].inliers;
-    info[3] = state[w].e;
-    if (out_gnc2) {
-      out_gnc2[2 * w] = g[w].stages;
-      out_gnc2[2 * w + 1] = g[w].mu;
-    }
-  }
+  joint_results(L, init_X, X, state, g.data(), out_X, out_info, out_gnc2);
   return 0;
 }
 
@@ -1715,22 +1738,15 @@ int sgb_align_batch_async(sgb_ctx* ctx, const sgb_align_options* o, const double
   const size_t B = batch_members(ctx);
   if (B == 0) return 0;
   CU(cudaSetDevice(ctx->device));
-  if (int rc = device_pointer(ctx, who, d_init_T, "init_T16xB")) return rc;
-  if (int rc = device_pointer(ctx, who, d_out_T, "out_T16xB")) return rc;
-  if (int rc = device_pointer(ctx, who, d_out_info, "out_info4xB")) return rc;
-  if (d_out_Hb) {
-    if (int rc = device_pointer(ctx, who, d_out_Hb, "out_Hb42xB")) return rc;
-  }
-  cudaStreamCaptureStatus capture = cudaStreamCaptureStatusNone;
-  CU(cudaStreamIsCapturing(ctx->stream, &capture));
-  if (capture == cudaStreamCaptureStatusInvalidated) return fail(ctx, 1, std::string(who) + ": the context's stream is in an invalidated capture");
-  const bool capturing = capture == cudaStreamCaptureStatusActive;
-  // nothing below allocates: a cudaMalloc may not run while the stream is captured (reserve_members sized everything for the batch)
-  if (ctx->use_packet_queue && !ctx->packet_queue.p) {
-    if (capturing) return fail(ctx, 1, std::string(who) + ": the first batched call of a context cannot be captured (it allocates); call it once before capturing");
-    CU(ctx->packet_queue.reserve(2 * sizeof(uint32_t)));
-    CU(cudaMemsetAsync(ctx->packet_queue.p, 0, 2 * sizeof(uint32_t), ctx->stream));
-  }
+  if (int rc = device_pointers(ctx, who, {{d_init_T, "init_T16xB", true}, {d_out_T, "out_T16xB", true}, {d_out_info, "out_info4xB", true},
+                                          {d_out_Hb, "out_Hb42xB", false}}))
+    return rc;
+  bool capturing = false;
+  if (int rc = capture_state(ctx, who, &capturing)) return rc;
+  // nothing else allocates: a cudaMalloc may not run while the stream is captured (reserve_members sized everything for the batch)
+  if (int rc = loop_allocations(ctx, who, capturing, false, true, 0, 0,
+                                ": the first batched call of a context cannot be captured (it allocates); call it once before capturing"))
+    return rc;
   if (int rc = pair_view(ctx)) return rc;
   const uint32_t nb = static_cast<uint32_t>(B);
   // the device's seed flags are kept while the host's are valid (the same target, the cached correspondences not dropped)
@@ -1743,23 +1759,15 @@ int sgb_align_batch_async(sgb_ctx* ctx, const sgb_align_options* o, const double
                            ctx->b_phase.as<uint8_t>(), ctx->stream));
       return 0;
     };
-    if (int rc = launch_loop(ctx, who, capturing, capturing ? std::vector<unsigned char>() : loop_key(ctx, o), ctx->align_exec, ctx->align_key,
-                             round_loop(ctx, o, step)))
+    if (int rc = launch_loop(ctx, who, capturing, capturing ? std::vector<unsigned char>() : loop_key(ctx, o), ctx->align_loop, round_loop(ctx, o, step)))
       return rc;
     ctx->launches += 1;
     if (int rc = clear_search_counters(ctx)) return rc;
   }
   CU(launch_batch_align_finish(nb, ctx->b_state.as<MemberState>(), d_out_T, d_out_info, d_out_Hb, ctx->stream));
   ctx->b_dseed_ok = true;
-  if (o->max_iterations > 0) {  // round 1 linearised every member, as sgb_align_batch's does
-    std::fill(ctx->b_lin.begin(), ctx->b_lin.end(), 1);
-    std::fill(ctx->b_seeded.begin(), ctx->b_seeded.end(), 1);
-    ctx->have_lin = true;
-    ctx->corr_seeds = true;
-    ctx->lin_factor = o->factor_kind;
-    ctx->lin_robust = o->robust_kind;
-    ctx->lin_c = o->robust_c;
-  }
+  // round 1 linearised every member, as sgb_align_batch's does
+  if (o->max_iterations > 0) mark_linearised(ctx, o->factor_kind, o->robust_kind, o->robust_c, nullptr);
   return 0;
 }
 
@@ -1773,20 +1781,17 @@ int sgb_align_joint_async(sgb_ctx* ctx, const sgb_align_options* o, size_t n_win
   const size_t W = L.W, K = L.K, E = L.E;
   if (W == 0) return 0;
   CU(cudaSetDevice(ctx->device));
-  if (int rc = device_pointer(ctx, who, d_init_X, "init_X16xK")) return rc;
-  if (int rc = device_pointer(ctx, who, d_out_X, "out_X16xK")) return rc;
-  if (int rc = device_pointer(ctx, who, d_out_info, "out_info4xW")) return rc;
-  cudaStreamCaptureStatus capture = cudaStreamCaptureStatusNone;
-  CU(cudaStreamIsCapturing(ctx->stream, &capture));
-  if (capture == cudaStreamCaptureStatusInvalidated) return fail(ctx, 1, std::string(who) + ": the context's stream is in an invalidated capture");
-  const bool capturing = capture == cudaStreamCaptureStatusActive;
+  if (int rc = device_pointers(ctx, who, {{d_init_X, "init_X16xK", true}, {d_out_X, "out_X16xK", true}, {d_out_info, "out_info4xW", true}})) return rc;
+  bool capturing = false;
+  if (int rc = capture_state(ctx, who, &capturing)) return rc;
   const bool loop = o->max_iterations > 0 && E > 0;
   // A capture can hold neither an allocation nor an upload from pageable memory: the buffers, the capture stream and the window tables
   // must come from an earlier call.  Outside a capture the tables are uploaded only when they changed (windows, fixed flags or pairing).
   const bool upload = joint_async_stale(ctx, L);
-  if (capturing && (upload || (loop && !ctx->cap_stream)))
-    return fail(ctx, 1, std::string(who) + ": these windows need an allocation or an upload of their tables, which a capture cannot hold; call it once "
-                                           "outside the capture first");
+  if (int rc = loop_allocations(ctx, who, capturing, upload, false, loop ? 1 : 0, 0,
+                                ": these windows need an allocation or an upload of their tables, which a capture cannot hold; call it once outside the "
+                                "capture first"))
+    return rc;
   if (int rc = joint_async_tables(ctx, L, upload)) return rc;
   if (E) {
     if (int rc = pair_view(ctx)) return rc;
@@ -1808,7 +1813,7 @@ int sgb_align_joint_async(sgb_ctx* ctx, const sgb_align_options* o, size_t n_win
       key_add(key, J);
       for (size_t v : {K, static_cast<size_t>(L.max_free)}) key_add(key, v);
     }
-    if (int rc = launch_loop(ctx, who, capturing, std::move(key), ctx->joint_exec, ctx->joint_key, round_loop(ctx, o, step))) return rc;
+    if (int rc = launch_loop(ctx, who, capturing, std::move(key), ctx->joint_loop, round_loop(ctx, o, step))) return rc;
     ctx->launches += 1;
     if (int rc = clear_search_counters(ctx)) return rc;
   }
@@ -1816,23 +1821,13 @@ int sgb_align_joint_async(sgb_ctx* ctx, const sgb_align_options* o, size_t n_win
   ctx->b_dseed_ok = true;
   // Round 1 linearised the edges of every window that started in kPhaseLinearize (one with a free frame and an edge), as sgb_align_joint's
   // first round does; no other edge was ever linearised.  Their flags are set as linearize_round sets them, the others left as they were.
-  const uint32_t* edge_member = L.edge_member();
-  const uint32_t* edge_win = L.edge_win();
-  bool any = false;
-  for (size_t q = 0; loop && q < E && !any; q++) any = L.n_free[edge_win[q]] > 0;
-  if (any) {
-    if (!ctx->have_lin) std::fill(ctx->b_lin.begin(), ctx->b_lin.end(), 0);
-    if (!ctx->corr_seeds) std::fill(ctx->b_seeded.begin(), ctx->b_seeded.end(), 0);
-    for (size_t q = 0; q < E; q++) {
-      if (!L.n_free[edge_win[q]]) continue;
-      ctx->b_lin[edge_member[q]] = 1;
-      ctx->b_seeded[edge_member[q]] = 1;
-    }
-    ctx->have_lin = true;
-    ctx->corr_seeds = true;
-    ctx->lin_factor = o->factor_kind;
-    ctx->lin_robust = o->robust_kind;
-    ctx->lin_c = o->robust_c;
+  if (loop) {
+    const uint32_t* edge_member = L.edge_member();
+    const uint32_t* edge_win = L.edge_win();
+    std::vector<uint8_t> linearised(E, 0);
+    bool any = false;
+    for (size_t q = 0; q < E; q++) any |= (linearised[edge_member[q]] = L.n_free[edge_win[q]] > 0) != 0;
+    if (any) mark_linearised(ctx, o->factor_kind, o->robust_kind, o->robust_c, linearised.data());
   }
   return 0;
 }
@@ -1848,36 +1843,19 @@ int sgb_align_joint_gnc_async(sgb_ctx* ctx, const sgb_align_options* o, const sg
   const size_t W = L.W, K = L.K, E = L.E, n = batch_points(ctx);
   if (W == 0) return 0;
   CU(cudaSetDevice(ctx->device));
-  if (int rc = device_pointer(ctx, who.c_str(), d_init_X, "init_X16xK")) return rc;
-  if (int rc = device_pointer(ctx, who.c_str(), d_out_X, "out_X16xK")) return rc;
-  if (int rc = device_pointer(ctx, who.c_str(), d_out_info, "out_info4xW")) return rc;
-  if (d_out_gnc2) {
-    if (int rc = device_pointer(ctx, who.c_str(), d_out_gnc2, "out_gnc2xW")) return rc;
-  }
-  if (d_out_point_w) {
-    if (int rc = device_pointer(ctx, who.c_str(), d_out_point_w, "out_point_w")) return rc;
-  }
-  cudaStreamCaptureStatus capture = cudaStreamCaptureStatusNone;
-  CU(cudaStreamIsCapturing(ctx->stream, &capture));
-  if (capture == cudaStreamCaptureStatusInvalidated) return fail(ctx, 1, who + ": the context's stream is in an invalidated capture");
-  const bool capturing = capture == cudaStreamCaptureStatusActive;
+  if (int rc = device_pointers(ctx, who, {{d_init_X, "init_X16xK", true}, {d_out_X, "out_X16xK", true}, {d_out_info, "out_info4xW", true},
+                                          {d_out_gnc2, "out_gnc2xW", false}, {d_out_point_w, "out_point_w", false}}))
+    return rc;
+  bool capturing = false;
+  if (int rc = capture_state(ctx, who, &capturing)) return rc;
   // A capture can hold neither an allocation nor an upload from pageable memory: the GNC buffers for W windows, the window tables and
   // buffers (uploaded only when they changed, as sgb_align_joint_async's), and with an edge the first batched call's search queue and both
   // capture streams (the stages' loop and the rounds' loop nested in it) must come from an earlier call
-  const size_t w_bytes = gnc_w_bytes(ctx), state_bytes = W * (sizeof(GncState) + 1);
   const bool upload = joint_async_stale(ctx, L);
-  const bool allocates = upload || ctx->g_w.cap < w_bytes || ctx->g_e.cap < w_bytes || ctx->g_state.cap < state_bytes ||
-                         (E && ((ctx->use_packet_queue && !ctx->packet_queue.p) || !ctx->cap_stream || !ctx->cap_stream_nested));
-  if (capturing && allocates)
-    return fail(ctx, 1, who + ": this call needs an allocation or an upload of its window tables, which a capture cannot hold; call it once outside the "
-                              "capture first");
-  if (E && ctx->use_packet_queue && !ctx->packet_queue.p) {
-    CU(ctx->packet_queue.reserve(2 * sizeof(uint32_t)));
-    CU(cudaMemsetAsync(ctx->packet_queue.p, 0, 2 * sizeof(uint32_t), ctx->stream));
-  }
-  CU(ctx->g_w.reserve(w_bytes));
-  CU(ctx->g_e.reserve(w_bytes));
-  CU(ctx->g_state.reserve(state_bytes));
+  if (int rc = loop_allocations(ctx, who, capturing, upload, E > 0, E ? 2 : 0, W,
+                                ": this call needs an allocation or an upload of its window tables, which a capture cannot hold; call it once outside "
+                                "the capture first"))
+    return rc;
   if (int rc = joint_async_tables(ctx, L, upload)) return rc;
   if (E) {
     if (int rc = pair_view(ctx)) return rc;
@@ -1894,8 +1872,7 @@ int sgb_align_joint_gnc_async(sgb_ctx* ctx, const sgb_align_options* o, const sg
   // every window live; the device's seed flags kept as sgb_align_joint_async keeps them
   if (K) CU(cudaMemcpyAsync(J.X, d_init_X, K * 16 * sizeof(double), cudaMemcpyDeviceToDevice, ctx->stream));
   CU(cudaMemsetAsync(J.state, 0, W * sizeof(WindowState), ctx->stream));
-  CU(cudaMemsetAsync(p.gnc, 0, W * sizeof(GncState), ctx->stream));
-  CU(cudaMemsetAsync(p.live, 1, W, ctx->stream));
+  if (int rc = gnc_begin(ctx, p, W)) return rc;
   if (E && !(ctx->corr_seeds && ctx->b_dseed_ok)) CU(cudaMemsetAsync(ctx->b_dseed.p, 0, E, ctx->stream));
   if (!E) {
     // No edge, so no point: sgb_align_joint_gnc's one stage of the stage kernels (r_max^2 = 0 makes it every window's last; the largest
@@ -1908,10 +1885,7 @@ int sgb_align_joint_gnc_async(sgb_ctx* ctx, const sgb_align_options* o, const sg
     // linearize of the edges of the windows in the stage (planned by batch_plan_kernel from their member phases), the stage kernels, then
     // the stage's joint align as an inner loop of rounds.  After joint_gnc_init, joint_gnc_loops gives every edge its window's phase and
     // sets both conditions: the stages' while a window has a stage to go, the rounds' while a window's align has a round to go.
-    BatchRows rows = {};
-    rows.member_off = p.member_off;
-    rows.perm = p.perm;
-    rows.e = p.e;
+    const BatchRows rows = gnc_rows(p);
     RoundWeights weights(ctx);
     const auto stage = [&](cudaGraphConditionalHandle stages) {
       cudaGraphConditionalHandle rounds;
@@ -1933,18 +1907,13 @@ int sgb_align_joint_gnc_async(sgb_ctx* ctx, const sgb_align_options* o, const sg
                           }));
     };
     std::vector<unsigned char> key;
-    if (!capturing) {  // loop_key, plus the GNC options, JointParams, the frame count, max_free and every buffer the GNC kernels use
+    if (!capturing) {  // loop_key, plus the GNC options, every buffer the GNC kernels use, JointParams, the frame count and max_free
       key = loop_key(ctx, o);
-      for (int v : {p.kind, p.max_stages, p.stage_iterations}) key_add(key, v);
-      key_add(key, p.c2);
+      gnc_key(key, p, {member_win});
       key_add(key, J);
       for (size_t v : {K, static_cast<size_t>(L.max_free)}) key_add(key, v);
-      for (const void* v : {static_cast<const void*>(p.member_off), static_cast<const void*>(p.perm), static_cast<const void*>(p.corr),
-                            static_cast<const void*>(p.e), static_cast<const void*>(p.w), static_cast<const void*>(p.wstage),
-                            static_cast<const void*>(p.gnc), static_cast<const void*>(p.live), static_cast<const void*>(member_win)})
-        key_add(key, v);
     }
-    if (int rc = launch_loop(ctx, who.c_str(), capturing, std::move(key), ctx->joint_gnc_exec, ctx->joint_gnc_key, stage)) return rc;
+    if (int rc = launch_loop(ctx, who.c_str(), capturing, std::move(key), ctx->joint_gnc_loop, stage)) return rc;
     ctx->launches += 1;
     if (int rc = clear_search_counters(ctx)) return rc;
   }
@@ -1956,13 +1925,7 @@ int sgb_align_joint_gnc_async(sgb_ctx* ctx, const sgb_align_options* o, const sg
     ctx->b_dseed_ok = true;
     // stage 0's reweighting round linearised every edge (every window is in stage 0), as sgb_align_joint_gnc's does; every round since used
     // robust_kind (NONE)
-    std::fill(ctx->b_lin.begin(), ctx->b_lin.end(), 1);
-    std::fill(ctx->b_seeded.begin(), ctx->b_seeded.end(), 1);
-    ctx->have_lin = true;
-    ctx->corr_seeds = true;
-    ctx->lin_factor = o->factor_kind;
-    ctx->lin_robust = o->robust_kind;
-    ctx->lin_c = o->robust_c;
+    mark_linearised(ctx, o->factor_kind, o->robust_kind, o->robust_c, nullptr);
   }
   return 0;
 }

@@ -47,6 +47,22 @@ struct DevBuf {
   }
 };
 
+/// The instantiated graph of a stream-ordered align's device loop and the key it was built under (launch_loop in sgb_capi_batch.cu):
+/// an empty key matches no call, so the next one rebuilds the graph.  Owns the graph: destroyed with the context.
+struct LoopGraph {
+  cudaGraphExec_t exec = nullptr;
+  std::vector<unsigned char> key;
+  LoopGraph() = default;
+  LoopGraph(const LoopGraph&) = delete;
+  LoopGraph& operator=(const LoopGraph&) = delete;
+  ~LoopGraph() { drop(); }
+  void drop() {
+    if (exec) cudaGraphExecDestroy(exec);
+    exec = nullptr;
+    key.clear();
+  }
+};
+
 /// The device side of a joint window align (JointParams in sgb_batch.h): the window / edge tables, the frames' poses, candidates and
 /// steps, the edges' last sums, the windows' WindowState and phase
 struct JointBufs {
@@ -229,27 +245,18 @@ struct sgb_ctx {
   std::vector<uint32_t> b_sub_off, b_sub_maps;
   sgb::DevBuf s_tables, s_entries, s_centres, b_centry;
   // sgb_align_batch_async: the round the planner made (BatchRound), the device's copy of b_seeded (b_dseed_ok: it never claims a seed
-  // the host's flags would not allow; cleared with them), the stream a round is captured on, and the instantiated loop with its key
+  // the host's flags would not allow; cleared with them) and the stream a round is captured on
   sgb::DevBuf b_round, b_dseed;
   bool b_dseed_ok = false;
   cudaStream_t cap_stream = nullptr;
   cudaStream_t cap_stream_nested = nullptr;  // the stream the body of a loop nested in a loop's body is captured on
-  cudaGraphExec_t align_exec = nullptr;
-  std::vector<unsigned char> align_key;
   // sgb_align_joint: the buffers of its JointParams.  sgb_align_joint_async has its own (joint_async), which no other call writes: its
-  // tables are uploaded only when they differ from ja_tab, the host copy of what joint_async.tables holds.  Its instantiated loop is
-  // cached with its key beside align_exec's.
+  // tables are uploaded only when they differ from ja_tab, the host copy of what joint_async.tables holds.
   sgb::JointBufs joint, joint_async;
   std::vector<uint32_t> ja_tab;
-  cudaGraphExec_t joint_exec = nullptr;
-  std::vector<unsigned char> joint_key;
-  // sgb_align_batch_gnc_async: its instantiated loop of stages, with its key (it uses g_w, g_e and g_state as sgb_align_batch_gnc does)
-  cudaGraphExec_t gnc_exec = nullptr;
-  std::vector<unsigned char> gnc_key;
-  // sgb_align_joint_gnc_async: its instantiated loop of stages, with its key (it uses g_w, g_e and g_state as sgb_align_joint_gnc does, and
-  // joint_async with its ja_tab as sgb_align_joint_async does)
-  cudaGraphExec_t joint_gnc_exec = nullptr;
-  std::vector<unsigned char> joint_gnc_key;
+  // The instantiated loops of sgb_align_batch_async, sgb_align_joint_async and the loops of stages of sgb_align_batch_gnc_async and
+  // sgb_align_joint_gnc_async (the GNC calls use g_w, g_e and g_state as their synchronous twins do; the joint ones joint_async)
+  sgb::LoopGraph align_loop, joint_loop, gnc_loop, joint_gnc_loop;
 };
 
 namespace sgb {
