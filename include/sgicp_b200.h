@@ -403,9 +403,11 @@ int sgb_align_batch(sgb_ctx* ctx, const sgb_align_options* options, const double
  * sgb_linearize_batch_points, the formulas, sgb_source_set_weights(w * g), sgb_align_batch (the exact-FP32-tie caveat above applies).
  * Afterwards the context is as sgb_align_batch leaves it after each member's last stage (sgb_correspondences_batch, sgb_error_batch), and
  * the weights in force are unchanged: the stage weights live in a buffer of the call.
- * Launches per stage: the reweighting linearize round (its search launches, the factor kernel, the segment kernel), 1 for the largest
- * residual (stage 0 only), 3 (mu and last stage, weights, align_init), then the align's rounds as in sgb_align_batch, each ending with one
- * step launch.  The host reads one byte per member per round, and one more per member per stage ("still in GNC").
+ * The call runs sgb_align_batch_gnc_async on its poses and outputs staged in device memory: every stage and round on the device, one
+ * upload of the poses, one copy of the outputs and one host synchronisation per call.  So it needs conditional graph nodes (CUDA 12.4 or
+ * later, driver included) as that call does, and keeps the device's seed flags as it does (a call after they were cleared starts
+ * unseeded; the exact-FP32-tie caveat above applies).  sgb_kernel_launches counts 4 per call (initial state, one launch of the graph, two
+ * for the outputs), whatever the stage and round counts, plus 1 when the pairing's view of the target is rebuilt.
  * Fails with a message, enqueuing nothing, for robust_kind != SGB_ROBUST_NONE (the GNC weights are the robust kernel), an invalid kind,
  * noise_bound_sq not finite or <= 0, max_stages < 1, stage_iterations < 1, while the context's stream is being captured (the call
  * synchronises), and for everything sgb_align_batch refuses. */
@@ -471,11 +473,12 @@ int sgb_joint_edge_poses(sgb_ctx* ctx, size_t n_windows, const size_t* window_of
  * no edge, which no such context can hold, returns its initial poses, not converged, 0 iterations, and the stage count and mu of r_max^2 =
  * 0 (GM: 1 stage, mu 1; TLS: 1 stage, mu 0).  Afterwards the context is as sgb_align_joint leaves it after each window's last stage
  * (sgb_correspondences_batch, sgb_error_batch on the edges), and the weights in force are unchanged.
- * Launches: per stage 1 for the edge poses (whenever the call has an edge, even at a stage whose windows have none), the reweighting
- * linearize round of the edges of the windows in the stage (its search launches, the factor kernel, the segment kernel; none when those
- * windows have no edge), 1 for the largest residual (stage 0 only), 3 (mu and last stage, weights, joint_init), then the joint align's
- * rounds as in sgb_align_joint, each ending with one joint step launch; plus 1 when the pairing's view of the target is rebuilt.  The host
- * reads one byte per window per round, and one more per window per stage ("still in GNC").
+ * The call runs sgb_align_joint_gnc_async on its frames and outputs staged in device memory, with window tables of its own (uploaded at
+ * every call, never those the asynchronous calls cache): every stage and joint round on the device, one copy of the outputs and one host
+ * synchronisation per call.  So it needs conditional graph nodes (CUDA 12.4 or later, driver included) as that call does, and keeps the
+ * device's seed flags as it does (the exact-FP32-tie caveat above applies).  sgb_kernel_launches counts 3 per call with at least one
+ * edge (one launch of the graph, two for the outputs) and 4 without (the stage kernels of the one stage, two for the outputs), whatever
+ * the stage and round counts, plus 1 when the pairing's view of the target is rebuilt.
  * Fails with a message, enqueuing nothing, where sgb_align_batch_gnc refuses its GNC options (robust_kind != SGB_ROBUST_NONE, an invalid
  * kind, noise_bound_sq not finite or <= 0, max_stages < 1, stage_iterations < 1), while the context's stream is being captured, and for
  * everything sgb_align_joint refuses. */
@@ -554,8 +557,8 @@ int sgb_align_batch_gnc_async(sgb_ctx* ctx, const sgb_align_options* options, co
  *     distance ties, as above), fixed frames come back bit for bit from d_init_X16xK, the context is left as it leaves it
  *     (sgb_correspondences_batch, sgb_error_batch and sgb_linearize_batch on the edges behave alike afterwards), and the weights in force
  *     are unchanged.  Errors of the enqueued work surface at the next synchronising call of the context.
- *   - The window tables are those of sgb_align_joint_async, cached in the context once for both calls: a call whose tables are unchanged
- *     uploads nothing; one whose tables changed uploads them once.
+ *   - The window tables are those of sgb_align_joint_async, cached in the context once for both calls and apart from the synchronous
+ *     joint calls': a call whose tables are unchanged uploads nothing; one whose tables changed uploads them once.
  *   - While the context's stream is being captured the whole GNC is added to the capture: each replay re-runs it from what d_init_X16xK
  *     and the weights in force hold at replay time.  A call that would have to allocate or upload (the GNC buffers for its windows, the
  *     first batched call's search queue, the capture streams, window tables that differ from the cached ones) fails with a message

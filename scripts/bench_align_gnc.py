@@ -13,11 +13,14 @@ Initial poses: ground truth times 0.5 degree of yaw and 0.1 m.  Arms, alternated
   host_tls   the same TLS loop driven from Python with public calls on a context holding one member (tests/np_gnc.host_gnc), timed on the
              first --host-members members only: what the host round trips cost per pair.
 c^2: the 90th percentile of r^2 = 2 e over the matched points of the uncorrupted pairs at ground truth (one value per size).
+--fresh-key runs one other case instead, the worst for the call's cached graph of its device loop: before every timed call a new batch
+(clutter30) whose first source frame has lost a different number of points (set_source_batch, untimed), so that every call builds and
+instantiates its graph, as in odometry, where every frame brings a new point count; gnc_gm and gnc_tls alternated, --sizes 1,8,64 say.
 Reported per workload and arm: median and worst rotation [deg] and translation [m] error against ground truth, converged count, median
 and maximum stages (GNC), and ms per pair (the median of --reps timed calls after one warm-up, each ending in a device synchronise).
 The card's name, power limit and maximum SM clock are read with nvidia-smi (read-only) in the same run and written next to the numbers.
 
-    python scripts/bench_align_gnc.py [--sizes 64,512] [--reps 3] [--host-members 8] [--out FILE]
+    python scripts/bench_align_gnc.py [--sizes 64,512] [--reps 3] [--host-members 8] [--fresh-key] [--out FILE]
 """
 import argparse
 import json
@@ -59,6 +62,7 @@ def main():
     ap.add_argument("--reps", type=int, default=3)
     ap.add_argument("--host-members", type=int, default=8)
     ap.add_argument("--corruptions", default=",".join(CORRUPTIONS))
+    ap.add_argument("--fresh-key", action="store_true")
     ap.add_argument("--out", default="")
     args = ap.parse_args()
     sizes = [int(x) for x in args.sizes.split(",")]
@@ -100,6 +104,29 @@ def main():
         t = ctx.linearize_batch_points(gt[:B], factor=sg.FACTOR_GICP, max_dist_sq=1.0, hessians=False)
         matched = np.concatenate(ctx.correspondences_batch()) != sg.NO_CORRESPONDENCE
         c2 = float(np.quantile(2.0 * t.point_e[matched], 0.9))
+        if args.fresh_key:
+            rng = np.random.default_rng(B)
+            src = [corrupt(p, "clutter30", rng) for p in frames[1 : B + 1]]
+            scov = [cov(p) for p in src]
+            arms = {"gnc_gm": sg.GNC_GEMAN_MCCLURE, "gnc_tls": sg.GNC_TLS}
+            times = {k: [] for k in arms}
+            calls = 0
+            for rep in range(args.reps + 1):  # the first is the warm-up
+                for k, gnc in arms.items():
+                    calls += 1
+                    batch(ctx, B, [src[0][:-calls]] + src[1:], [scov[0][:-calls]] + scov[1:])
+                    torch.cuda.synchronize()
+                    t0 = time.perf_counter()
+                    ctx.align_batch_gnc(inits[:B], c2, gnc=gnc, **kw)
+                    torch.cuda.synchronize()
+                    if rep:
+                        times[k].append(time.perf_counter() - t0)
+            rec = {"workload": "fresh_key clutter30", "B": B, "c2": c2, **info}
+            rec.update({k: {"ms_per_call": 1e3 * float(np.median(t)), "ms_per_call_max": 1e3 * float(np.max(t))} for k, t in times.items()})
+            print(json.dumps(rec), flush=True)
+            results.append(rec)
+            ctx.close()
+            continue
         for corr in args.corruptions.split(","):
             rng = np.random.default_rng(B)
             src = [corrupt(p, corr, rng) for p in frames[1 : B + 1]]

@@ -15,13 +15,16 @@ Arms, alternated call by call, median of --reps timed calls after one warm-up, e
   host_tls   the TLS loop of align_joint_gnc driven from Python with public calls (tests/np_joint_gnc.host_joint_gnc) on contexts holding
              one window, over the first --host-windows windows, its X checked bit-identical to gnc_tls's before it is timed.
 c^2: the 90th percentile of r^2 = 2 e over the matched points of the uncorrupted edges (c = 2) at ground truth, once per K and target kind.
+--fresh-key runs one other case instead, the worst for the call's cached graph of its device loop: windows of the first --window size,
+the first --edges count, clutter30, and before every timed call a new batch whose first frame has lost a different number of points
+(set_source_batch and set_source_pairs, untimed), so that every call builds and instantiates its graph; gnc_gm and gnc_tls alternated.
 Reported per workload and arm: median and worst rotation [deg] and translation [m] error of the free frames against ground truth,
 converged windows (edges for pairs_gnc), median and maximum stages (GNC), and ms per window; for gnc_tls also the share of its device
 time spent in the joint step kernel and the joint rounds it ran (torch.profiler, one call of its own).  The card's name, power limit and
 maximum SM clock are read with nvidia-smi (read-only) in the same run and written next to the numbers.
 
     python scripts/bench_align_joint_gnc.py [--frames 64,512] [--window 8,16] [--edges 2,4] [--kinds kdtree,voxelmap]
-                                            [--corruptions moved15,...] [--reps 5] [--host-windows 2] [--out FILE]
+                                            [--corruptions moved15,...] [--reps 5] [--host-windows 2] [--fresh-key] [--out FILE]
 """
 import argparse
 import json
@@ -53,6 +56,7 @@ def main():
     ap.add_argument("--corruptions", default=",".join(CORRUPTIONS))
     ap.add_argument("--reps", type=int, default=5)
     ap.add_argument("--host-windows", type=int, default=2)
+    ap.add_argument("--fresh-key", action="store_true")
     ap.add_argument("--out", default="")
     args = ap.parse_args()
 
@@ -109,6 +113,37 @@ def main():
             matched = np.concatenate(clean.correspondences_batch()) != sg.NO_CORRESPONDENCE
             c2 = float(np.quantile(2.0 * t.point_e[matched], 0.9))
             clean.close()
+            if args.fresh_key:
+                pts = [corrupt(p, "clutter30", np.random.default_rng(K)) for p in frames[:K]]
+                cv = [cov(p) for p in pts]
+                W, c = int(args.window.split(",")[0]), int(args.edges.split(",")[0])
+                woff = list(range(0, K, W)) + [K]
+                first, edges = window_edges(K, W, c)
+                X0 = np.array([Gt[k] if k == first[k] else Gt[k] @ noise[k] for k in range(K)])
+                ctx = context(kind, pts, cv, edges)
+                arms = {"gnc_gm": sg.GNC_GEMAN_MCCLURE, "gnc_tls": sg.GNC_TLS}
+                times = {k: [] for k in arms}
+                calls = 0
+                for rep in range(args.reps + 1):  # the first is the warm-up
+                    for k, gnc in arms.items():
+                        calls += 1
+                        p0 = [pts[0][:-calls]] + pts[1:]
+                        off = np.zeros(K + 1, dtype=np.int64)
+                        off[1:] = np.cumsum([len(p) for p in p0])
+                        ctx.set_source_batch((np.concatenate(p0), off), np.concatenate([cv[0][:-calls]] + cv[1:]))
+                        ctx.set_source_pairs(np.array([e[0] for e in edges], dtype=np.uint32), np.array([e[1] for e in edges], dtype=np.uint32))
+                        torch.cuda.synchronize()
+                        t0 = time.perf_counter()
+                        ctx.align_joint_gnc(X0, c2, windows=woff, gnc=gnc, **kw)
+                        torch.cuda.synchronize()
+                        if rep:
+                            times[k].append(time.perf_counter() - t0)
+                rec = {"workload": f"fresh_key K={K} W={W} c={c} {kind} clutter30", "windows": len(woff) - 1, "edges": len(edges), "c2": c2, **info}
+                rec.update({k: {"ms_per_call": 1e3 * float(np.median(t)), "ms_per_call_max": 1e3 * float(np.max(t))} for k, t in times.items()})
+                print(json.dumps(rec), flush=True)
+                results.append(rec)
+                ctx.close()
+                continue
             for corr in args.corruptions.split(","):
                 crng = np.random.default_rng(K)
                 pts = [corrupt(p, corr, crng) for p in frames[:K]]

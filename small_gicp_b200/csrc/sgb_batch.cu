@@ -20,17 +20,15 @@
 //   joint_step_kernel       joint windows: one CTA per window, its system assembled from its edges' sums and solved, its state machine,
 //                           its edges' next poses (sgb_align_joint; joint_align_init_kernel / joint_align_finish_kernel: the asynchronous
 //                           call's set-up and outputs)
-//   gnc_*_kernel            sgb_align_batch_gnc: the largest residual of stage 0, each member's mu and last-stage decision, each point's
-//                           GNC weight from its row of the reweighting linearize, each stage's align_init, and the step with each member's
-//                           stage iterations (sgb_align_batch_gnc_async: gnc_reweigh_kernel / gnc_loops_kernel / gnc_finish_kernel,
-//                           each stage's phases, the loops' conditions and the outputs)
-//   joint_gnc_*_kernel      sgb_align_joint_gnc: the same GNC with the window as its unit (each point's window through its edge), each
-//                           window's stage start (joint_init) and the joint step with each window's stage iterations
-//                           (sgb_align_joint_gnc_async: joint_gnc_reweigh_kernel / joint_gnc_loops_kernel / joint_gnc_finish_kernel, each
-//                           stage's edge phases, the loops' conditions and the outputs)
+//   gnc_*_kernel            sgb_align_batch_gnc(_async): the largest residual of stage 0, each member's mu and last-stage decision, each
+//                           point's GNC weight from its row of the reweighting linearize, each stage's align_init, the step with each
+//                           member's stage iterations, each stage's phases, the loops' conditions and the outputs
+//   joint_gnc_*_kernel      sgb_align_joint_gnc(_async): the same GNC with the window as its unit (each point's window through its edge),
+//                           each window's stage start (joint_init), the joint step with each window's stage iterations, each stage's edge
+//                           phases, the loops' conditions and the outputs
 // The transform, factor, segment and step kernels serve the rounds the host plans (sgb_{linearize,error,align}_batch, sgb_align_joint) and,
-// with ROUND / kModeRound, the rounds batch_plan_kernel plans on the device (sgb_align_batch_async, sgb_align_joint_async,
-// sgb_align_batch_gnc_async, sgb_align_joint_gnc_async).
+// with ROUND / kModeRound, the rounds batch_plan_kernel plans on the device (sgb_align_batch_async, sgb_align_joint_async and both GNC
+// aligns of each, whose rounds are all planned on the device).
 // A member's sums depend on its own points, pose and correspondences only, added in an order fixed by its size: bit-identical whatever
 // else is in the batch.
 #include <algorithm>
@@ -711,24 +709,23 @@ struct GncWindowUnit {
   __device__ __forceinline__ uint32_t operator()(uint32_t m) const { return __ldg(&win[m]); }
 };
 
-// every unit's largest r^2 over its points (the loop of gnc_rmax_kernel and joint_gnc_rmax_kernel)
-template <bool ROUND, typename Unit>
+// every unit's largest r^2 over its points before its stage 0 (no stage begun; the loop of gnc_rmax_kernel and joint_gnc_rmax_kernel,
+// launched at every stage of the stage loop)
+template <typename Unit>
 __device__ __forceinline__ void gnc_rmax_points(const GncParams& p, Unit unit) {
   for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < p.n; i += gridDim.x * blockDim.x) {
     const uint32_t m = owner_of(p.member_off, p.n_members, i);
     const uint32_t u = unit(m);
     if (!p.live[u] || p.corr[i] == kNone) continue;
-    if (ROUND && p.gnc[u].stages != 0) continue;
+    if (p.gnc[u].stages != 0) continue;
     const double r2 = rn_mul(2.0, p.e[batch_row(p.member_off, p.perm, m, i)]);
     // a non-negative double orders as its bit pattern; -0.0, rounding's tiny negatives and NaN never enter
     if (r2 > 0.0) atomicMax(reinterpret_cast<unsigned long long*>(&p.gnc[u].r2max), static_cast<unsigned long long>(__double_as_longlong(r2)));
   }
 }
 
-// ROUND (sgb_align_batch_gnc_async, launched at every stage of its loop): only the members before their stage 0 (no stage begun)
-template <bool ROUND>
 __global__ void gnc_rmax_kernel(const GncParams p) {
-  gnc_rmax_points<ROUND>(p, GncMemberUnit{});
+  gnc_rmax_points(p, GncMemberUnit{});
 }
 
 __global__ void __launch_bounds__(kStepBlock) gnc_stage_kernel(const GncParams p) {
@@ -792,23 +789,17 @@ __global__ void __launch_bounds__(kStepBlock) gnc_init_kernel(const GncParams p,
   }
   phase[m] = static_cast<uint8_t>(s.phase);
 }
-// ROUND: a round of a stage of sgb_align_batch_gnc_async, its kind read from `round`; `loop` becomes 1 while a member has a round to go
-template <bool ROUND>
-__global__ void __launch_bounds__(kStepBlock) gnc_step_kernel(const GncParams p, const __grid_constant__ AlignOptions o, bool linearize, const double* __restrict__ out,
+// A round of a stage, its kind read from `round`; `loop` becomes 1 while a member has a round to go
+__global__ void __launch_bounds__(kStepBlock) gnc_step_kernel(const GncParams p, const __grid_constant__ AlignOptions o, const double* __restrict__ out,
                                                               MemberState* __restrict__ state, double* __restrict__ poses, uint8_t* __restrict__ phase,
                                                               const BatchRound* __restrict__ round, cudaGraphConditionalHandle loop) {
   const uint32_t m = blockIdx.x * kStepBlock + threadIdx.x;
-  if constexpr (ROUND) {
-    int more = 0;
-    if (m < p.n_members) {
-      batch_step_member(gnc_stage_options(o, p, m), m, round->lin != 0u, out, state, poses, phase);
-      more = phase[m] == kPhaseLinearize || phase[m] == kPhaseTrial;
-    }
-    if (__syncthreads_or(more) && threadIdx.x == 0) cudaGraphSetConditional(loop, 1u);
-  } else {
-    if (m >= p.n_members) return;
-    batch_step_member(gnc_stage_options(o, p, m), m, linearize, out, state, poses, phase);
+  int more = 0;
+  if (m < p.n_members) {
+    batch_step_member(gnc_stage_options(o, p, m), m, round->lin != 0u, out, state, poses, phase);
+    more = phase[m] == kPhaseLinearize || phase[m] == kPhaseTrial;
   }
+  if (__syncthreads_or(more) && threadIdx.x == 0) cudaGraphSetConditional(loop, 1u);
 }
 
 // ---- sgb_align_batch_gnc_async (DESIGN.md §11 "Asynchronous graduated non-convexity") ----
@@ -849,11 +840,8 @@ __global__ void __launch_bounds__(kStepBlock) gnc_finish_kernel(uint32_t n_membe
   }
 }
 
-cudaError_t launch_gnc_rmax(const GncParams& p, bool round, int sm_count, cudaStream_t st) {
-  if (round)
-    gnc_rmax_kernel<true><<<gnc_point_grid(p.n, sm_count), 256, 0, st>>>(p);
-  else
-    gnc_rmax_kernel<false><<<gnc_point_grid(p.n, sm_count), 256, 0, st>>>(p);
+cudaError_t launch_gnc_rmax(const GncParams& p, int sm_count, cudaStream_t st) {
+  gnc_rmax_kernel<<<gnc_point_grid(p.n, sm_count), 256, 0, st>>>(p);
   return cudaGetLastError();
 }
 
@@ -875,13 +863,9 @@ cudaError_t launch_gnc_init(const GncParams& p, const AlignOptions& o, MemberSta
   return cudaGetLastError();
 }
 
-cudaError_t launch_gnc_step(const GncParams& p, const AlignOptions& o, bool linearize, const BatchRound* round, cudaGraphConditionalHandle loop, const double* out,
+cudaError_t launch_gnc_step(const GncParams& p, const AlignOptions& o, const BatchRound* round, cudaGraphConditionalHandle loop, const double* out,
                             MemberState* state, double* poses, uint8_t* phase, cudaStream_t st) {
-  const uint32_t grid = (p.n_members + kStepBlock - 1) / kStepBlock;
-  if (round)
-    gnc_step_kernel<true><<<grid, kStepBlock, 0, st>>>(p, o, linearize, out, state, poses, phase, round, loop);
-  else
-    gnc_step_kernel<false><<<grid, kStepBlock, 0, st>>>(p, o, linearize, out, state, poses, phase, nullptr, loop);
+  gnc_step_kernel<<<(p.n_members + kStepBlock - 1) / kStepBlock, kStepBlock, 0, st>>>(p, o, out, state, poses, phase, round, loop);
   return cudaGetLastError();
 }
 
@@ -1053,10 +1037,8 @@ cudaError_t launch_joint_align_finish(const JointParams& J, uint32_t n_frames, c
 // ---- sgb_align_joint_gnc (DESIGN.md §11 "Graduated non-convexity for joint windows"): the GNC unit is the window.  p.gnc and p.live are
 // per window; the point kernels reach a point's window through its member (edge), member_win[m] ----
 
-// ROUND (sgb_align_joint_gnc_async, launched at every stage of its loop): only the windows before their stage 0 (no stage begun)
-template <bool ROUND>
 __global__ void joint_gnc_rmax_kernel(const GncParams p, const uint32_t* __restrict__ member_win) {
-  gnc_rmax_points<ROUND>(p, GncWindowUnit{member_win});
+  gnc_rmax_points(p, GncWindowUnit{member_win});
 }
 
 template <int KIND>
@@ -1085,24 +1067,16 @@ __global__ void __launch_bounds__(kStepBlock) joint_gnc_init_kernel(const GncPar
   J.phase[w] = static_cast<uint8_t>(s.phase);
 }
 
-// joint_step_kernel for a round of a GNC stage: each window steps with its stage's max_iterations (as joint_gnc_init_kernel chose).  ROUND: a
-// round of a stage of sgb_align_joint_gnc_async, as joint_step_kernel<true> (its kind read from `round`, each stepped window's phase to its
-// edges' member_phase, `loop` set to 1 while a window has a round to go)
-template <bool ROUND>
-__global__ void __launch_bounds__(kJointBlock) joint_gnc_step_kernel(const __grid_constant__ AlignOptions o, const __grid_constant__ JointParams J, bool linearize,
+// joint_step_kernel<true> for a round of a GNC stage (its kind read from `round`, each stepped window's phase to its edges' member_phase,
+// `loop` set to 1 while a window has a round to go): each window steps with its stage's max_iterations (as joint_gnc_init_kernel chose)
+__global__ void __launch_bounds__(kJointBlock) joint_gnc_step_kernel(const __grid_constant__ AlignOptions o, const __grid_constant__ JointParams J,
                                                                      const double* __restrict__ out, const GncParams p, const BatchRound* __restrict__ round,
                                                                      cudaGraphConditionalHandle loop, uint8_t* __restrict__ member_phase) {
-  if constexpr (ROUND)
-    joint_step_window<true>(gnc_stage_options(o, p, blockIdx.x), J, linearize, out, round, loop, member_phase);
-  else
-    joint_step_window<false>(gnc_stage_options(o, p, blockIdx.x), J, linearize, out, nullptr, 0, nullptr);
+  joint_step_window<true>(gnc_stage_options(o, p, blockIdx.x), J, false, out, round, loop, member_phase);  // (the kind is the round's)
 }
 
-cudaError_t launch_joint_gnc_rmax(const GncParams& p, const uint32_t* member_win, bool round, int sm_count, cudaStream_t st) {
-  if (round)
-    joint_gnc_rmax_kernel<true><<<gnc_point_grid(p.n, sm_count), 256, 0, st>>>(p, member_win);
-  else
-    joint_gnc_rmax_kernel<false><<<gnc_point_grid(p.n, sm_count), 256, 0, st>>>(p, member_win);
+cudaError_t launch_joint_gnc_rmax(const GncParams& p, const uint32_t* member_win, int sm_count, cudaStream_t st) {
+  joint_gnc_rmax_kernel<<<gnc_point_grid(p.n, sm_count), 256, 0, st>>>(p, member_win);
   return cudaGetLastError();
 }
 
@@ -1119,13 +1093,12 @@ cudaError_t launch_joint_gnc_init(const GncParams& pw, const AlignOptions& o, co
   return cudaGetLastError();
 }
 
-cudaError_t launch_joint_gnc_step(const AlignOptions& o, const JointParams& J, int max_free, bool linearize, const double* out, const GncParams& pw,
-                                  const BatchRound* round, cudaGraphConditionalHandle loop, uint8_t* member_phase, cudaStream_t st) {
-  const auto kernel = round ? joint_gnc_step_kernel<true> : joint_gnc_step_kernel<false>;
+cudaError_t launch_joint_gnc_step(const AlignOptions& o, const JointParams& J, int max_free, const double* out, const GncParams& pw, const BatchRound* round,
+                                  cudaGraphConditionalHandle loop, uint8_t* member_phase, cudaStream_t st) {
   const size_t smem = joint_step_smem(max_free);
-  const cudaError_t e = allow_dynamic_smem(kernel, smem);
+  const cudaError_t e = allow_dynamic_smem(joint_gnc_step_kernel, smem);
   if (e != cudaSuccess) return e;
-  kernel<<<J.n_windows, kJointBlock, smem, st>>>(o, J, linearize, out, pw, round, loop, member_phase);
+  joint_gnc_step_kernel<<<J.n_windows, kJointBlock, smem, st>>>(o, J, out, pw, round, loop, member_phase);
   return cudaGetLastError();
 }
 

@@ -163,7 +163,7 @@ cudaError_t launch_batch_align_init(const AlignOptions& o, uint32_t n_members, c
 /// sgb_align_batch's outputs from the members' final state: T (16, column-major), info (converged, iterations, inliers, error), H | b (or null)
 cudaError_t launch_batch_align_finish(uint32_t n_members, const MemberState* state, double* out_T16, double* out_info4, double* out_Hb42, cudaStream_t st);
 
-// ---- sgb_align_batch_gnc (DESIGN.md §11 "Graduated non-convexity"): the stages' reweighting between host-planned aligns ----
+// ---- sgb_align_batch_gnc (DESIGN.md §11 "Graduated non-convexity"): the stages' reweighting between the stages' aligns ----
 /// What the GNC kernels of one stage share.  The members in the stage are those with live[m] = 1.  e: [rows] in the row layout of BatchRows
 /// (member_off, perm): the reweighting linearize's e rows in, each point's g of the stage out.  corr: BatchParams::corr after that
 /// linearize.  w: the weights in force in stored order (null: none); wstage: [points] w_i g_i in stored order, the weights of the stage's align.
@@ -180,9 +180,9 @@ struct GncParams {
   GncState* gnc;   // [members]
   uint8_t* live;   // [members] in: in this stage; the init kernel leaves 1 for a member with a stage to go
 };
-/// stage 0: every member's largest r^2 = 2 e_i > 0 over its points with a correspondence (gnc[m].r2max, cleared by the caller).  round:
-/// launched at every stage of the device loop, for the members that have begun no stage only
-cudaError_t launch_gnc_rmax(const GncParams& p, bool round, int sm_count, cudaStream_t st);
+/// stage 0: every member's largest r^2 = 2 e_i > 0 over its points with a correspondence (gnc[m].r2max, cleared by the caller).  Launched
+/// at every stage of the device loop: the members that have begun no stage only
+cudaError_t launch_gnc_rmax(const GncParams& p, int sm_count, cudaStream_t st);
 /// one thread per member in the stage: gnc_stage_begin
 cudaError_t launch_gnc_stage(const GncParams& p, cudaStream_t st);
 /// one thread per stored point of a member in the stage: its g (0 without a correspondence) to e, w_i g_i to wstage, TLS's not_binary flag
@@ -191,9 +191,9 @@ cudaError_t launch_gnc_weight(const GncParams& p, int sm_count, cudaStream_t st)
 /// the previous stage's iterations and starts its align from its current pose (align_init of o with max_iterations = stage_iterations
 /// unless last; pose and phase as the align's rounds read them); every other member is left done
 cudaError_t launch_gnc_init(const GncParams& p, const AlignOptions& o, MemberState* state, double* poses, uint8_t* phase, cudaStream_t st);
-/// launch_batch_step for a round of a GNC stage: each member steps with its stage's max_iterations (as launch_gnc_init chose).  round = null:
-/// a host-planned round; else a round planned on the device, its kind read from `round`, `loop` set to 1 while a member has a round to go
-cudaError_t launch_gnc_step(const GncParams& p, const AlignOptions& o, bool linearize, const BatchRound* round, cudaGraphConditionalHandle loop, const double* out,
+/// launch_batch_step for a round of a GNC stage planned on the device: each member steps with its stage's max_iterations (as launch_gnc_init
+/// chose), the round's kind read from `round`, `loop` set to 1 while a member has a round to go
+cudaError_t launch_gnc_step(const GncParams& p, const AlignOptions& o, const BatchRound* round, cudaGraphConditionalHandle loop, const double* out,
                             MemberState* state, double* poses, uint8_t* phase, cudaStream_t st);
 
 // ---- sgb_align_batch_gnc_async (DESIGN.md §11 "Asynchronous graduated non-convexity"): the stages and their rounds on the device ----
@@ -244,17 +244,17 @@ cudaError_t launch_joint_align_finish(const JointParams& J, uint32_t n_frames, c
 // GNC unit.  GncState and live flags per window: p (the point kernels) has n_members = the edges, each point's window member_win[its edge];
 // pw (the window kernels, and launch_gnc_stage) the same with n_members = the windows. ----
 /// stage 0: every window's largest r^2 = 2 e_i > 0 over its edges' points with a correspondence (gnc[w].r2max, cleared by the caller).
-/// round: launched at every stage of the device loop, for the windows that have begun no stage only
-cudaError_t launch_joint_gnc_rmax(const GncParams& p, const uint32_t* member_win, bool round, int sm_count, cudaStream_t st);
+/// Launched at every stage of the device loop: the windows that have begun no stage only
+cudaError_t launch_joint_gnc_rmax(const GncParams& p, const uint32_t* member_win, int sm_count, cudaStream_t st);
 /// launch_gnc_weight with each point's window's mu (TLS: not_binary per window)
 cudaError_t launch_joint_gnc_weight(const GncParams& p, const uint32_t* member_win, int sm_count, cudaStream_t st);
 /// launch_gnc_init per window: joint_init of a window in the stage from its current X (max_iterations = stage_iterations unless last),
 /// its phase to J.phase; every other window is left done
 cudaError_t launch_joint_gnc_init(const GncParams& pw, const AlignOptions& o, const JointParams& J, cudaStream_t st);
-/// launch_joint_step for a round of a GNC stage: each window steps with its stage's max_iterations.  round = null: a host-planned round;
-/// else a round planned on the device, as launch_joint_step's (member_phase, loop)
-cudaError_t launch_joint_gnc_step(const AlignOptions& o, const JointParams& J, int max_free, bool linearize, const double* out, const GncParams& pw,
-                                  const BatchRound* round, cudaGraphConditionalHandle loop, uint8_t* member_phase, cudaStream_t st);
+/// launch_joint_step for a round of a GNC stage planned on the device (member_phase, loop as there): each window steps with its stage's
+/// max_iterations
+cudaError_t launch_joint_gnc_step(const AlignOptions& o, const JointParams& J, int max_free, const double* out, const GncParams& pw, const BatchRound* round,
+                                  cudaGraphConditionalHandle loop, uint8_t* member_phase, cudaStream_t st);
 
 // ---- sgb_align_joint_gnc_async (DESIGN.md §11 "Asynchronous graduated non-convexity for joint windows"): the stages and their joint rounds
 // on the device, the edges the members of the rounds ----

@@ -86,7 +86,8 @@ void forget_linearisation(sgb_ctx* ctx) {
   ctx->corr_seeds = false;
   ctx->b_view_ok = false;  // the target (or the pairing) it was built from may have changed
   ctx->b_dseed_ok = false;
-  for (LoopGraph* g : {&ctx->align_loop, &ctx->joint_loop, &ctx->gnc_loop, &ctx->joint_gnc_loop}) g->key.clear();  // every async align rebuilds its loop
+  for (LoopGraph* g : {&ctx->align_loop, &ctx->joint_loop, &ctx->gnc_loop, &ctx->joint_gnc_loop, &ctx->joint_gnc_sync_loop})
+    g->key.clear();  // every stream-ordered loop is rebuilt
 }
 
 }  // namespace

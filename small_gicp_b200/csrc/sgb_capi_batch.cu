@@ -272,7 +272,7 @@ int round_kernels(sgb_ctx* ctx, const LinParams& P, const BatchParams& Bp, const
     if (int rc = round ? point_search_round(ctx, Q, &round->n_search, depth) : launch_point_search(ctx, Q, depth)) return rc;
     ctx->launches += counted;
   }
-  // the weights in force (sgb_source_set_weights), or those of an sgb_align_batch_gnc round (RoundWeights)
+  // the weights in force (sgb_source_set_weights), or those of a GNC align's round (RoundWeights)
   const double* weights = ctx->b_wround ? ctx->b_wuse : ctx->b_weighted ? ctx->b_weights.as<double>() : nullptr;
   CU(launch_batch_factor(Bp, kind, factor, robust, err, round, n_tiles, err ? nullptr : vcorr, centres, regions, S, rows, weights, ctx->stream));
   ctx->launches += counted;
@@ -806,7 +806,7 @@ int error_batch(sgb_ctx* ctx, const char* who, bool points, const double* T, con
   return copy_out(ctx, out, B);
 }
 
-// The initial state and poses of sgb_align_batch (and of stage 0 of sgb_align_batch_gnc): the only upload of poses in the whole align
+// The initial state and poses of sgb_align_batch: the only upload of poses in the whole align
 int align_start(sgb_ctx* ctx, const AlignOptions& ao, const double* init_T, std::vector<MemberState>& state, std::vector<uint8_t>& phase) {
   const size_t B = batch_members(ctx);
   state.resize(B);
@@ -824,24 +824,19 @@ int align_start(sgb_ctx* ctx, const AlignOptions& ao, const double* init_T, std:
   return 0;
 }
 
-// The outputs of an align from the members' final state; gnc (or null): the iterations of their earlier GNC stages are added, and
-// out_gnc2 (or null) gets each member's stages and mu
-void align_results(const std::vector<MemberState>& state, const GncState* gnc, double* out_T, double* out_info, double* out_Hb, double* out_gnc2) {
+// The outputs of an align from the members' final state
+void align_results(const std::vector<MemberState>& state, double* out_T, double* out_info, double* out_Hb) {
   for (size_t m = 0; m < state.size(); m++) {
     const MemberState& s = state[m];
     std::memcpy(out_T + 16 * m, s.T, 16 * sizeof(double));
     double* info = out_info + 4 * m;
     info[0] = s.converged ? 1.0 : 0.0;
-    info[1] = s.iterations + (gnc ? gnc[m].iterations : 0);
+    info[1] = s.iterations;
     info[2] = s.inliers;
     info[3] = s.e;
     if (out_Hb) {
       std::memcpy(out_Hb + 42 * m, s.H, 36 * sizeof(double));
       std::memcpy(out_Hb + 42 * m + 36, s.b, 6 * sizeof(double));
-    }
-    if (out_gnc2) {
-      out_gnc2[2 * m] = gnc[m].stages;
-      out_gnc2[2 * m + 1] = gnc[m].mu;
     }
   }
 }
@@ -874,7 +869,7 @@ int align_rounds(sgb_ctx* ctx, const sgb_align_options* o, std::vector<uint8_t>&
   }
 }
 
-// sgb_align_batch_gnc: the weights its rounds use in place of those in force, until the call returns however it returns
+// A GNC align: the weights its rounds use in place of those in force, until the call returns however it returns
 struct RoundWeights {
   sgb_ctx* ctx;
   explicit RoundWeights(sgb_ctx* c) : ctx(c) { ctx->b_wround = true; }
@@ -905,13 +900,13 @@ int gnc_checks(sgb_ctx* ctx, const std::string& who, const sgb_align_options* o,
   return gnc_option_checks(ctx, who, o, gnc);
 }
 
-// A synchronous GNC call refuses a captured stream: it synchronises at every round and stage to plan the next one
+// A synchronous GNC call refuses a captured stream: it copies its poses in and its outputs out of host memory and waits for them
 int gnc_capture_check(sgb_ctx* ctx, const std::string& who) {
   bool capturing = false;
   if (int rc = capture_state(ctx, who, &capturing)) return rc;
   if (capturing)
-    return fail(ctx, 1, who + ": the context's stream is being captured, and the call synchronises at every round and stage to plan the next one; call it "
-                              "outside the capture");
+    return fail(ctx, 1, who + ": the context's stream is being captured, and the call copies host memory and waits for its results; call it outside the "
+                              "capture (or use the _async call)");
   return 0;
 }
 
@@ -989,6 +984,80 @@ void gnc_key(std::vector<unsigned char>& k, const GncParams& p, std::initializer
                         static_cast<const void*>(p.live)})
     key_add(k, v);
   for (const void* v : more) key_add(k, v);
+}
+
+// The stream-ordered GNC of both batch GNC aligns, after their checks (who names the caller; capturing: ctx->stream is being captured):
+// the stages and their rounds as one device loop from the poses at d_init_T, the outputs to d_out_T, d_out_info and, unless null, d_out_Hb,
+// d_out_gnc2 (device memory) and out_point_w (host or device memory).
+int batch_gnc_enqueue(sgb_ctx* ctx, const char* who, bool capturing, const sgb_align_options* o, const sgb_gnc_options* gnc, const AlignOptions& ao,
+                      const double* d_init_T, double* d_out_T, double* d_out_info, double* d_out_Hb, double* d_out_gnc2, double* out_point_w) {
+  const size_t B = batch_members(ctx), n = batch_points(ctx);
+  // the GNC buffers, the packet queue and both capture streams (the stages' loop and the rounds' loop nested in it)
+  if (int rc = loop_allocations(ctx, who, capturing, false, true, 2, B,
+                                ": this call needs an allocation, which a capture cannot hold; call it once outside the capture first"))
+    return rc;
+  if (int rc = pair_view(ctx)) return rc;
+  const GncParams gp = gnc_params(ctx, gnc);
+  const BatchRows rows = gnc_rows(gp);
+  const uint32_t nb = static_cast<uint32_t>(B);
+  MemberState* state = ctx->b_state.as<MemberState>();
+  double* poses = ctx->b_poses.as<double>();
+  uint8_t* phase = ctx->b_phase.as<uint8_t>();
+  // the initial state: every member's align_init at its initial pose, zero GNC state, every member live (the seed flags kept as
+  // sgb_align_batch_async keeps them)
+  CU(launch_batch_align_init(ao, nb, d_init_T, state, poses, phase, ctx->b_dseed.as<uint8_t>(), ctx->corr_seeds && ctx->b_dseed_ok, ctx->stream));
+  if (int rc = gnc_begin(ctx, gp, B)) return rc;
+  ctx->launches += 3;  // the initial state here, the outputs below
+  // One stage per iteration of the outer loop: the reweighting linearize of the members in the stage (planned by batch_plan_kernel from
+  // their phases), the stage kernels, then the stage's align as an inner loop of rounds.  After gnc_init, gnc_loops sets both conditions:
+  // the stages' while a member has a stage to go, the rounds' while a member's align has a round to go.
+  RoundWeights weights(ctx);
+  const auto stage = [&](cudaGraphConditionalHandle stages) {
+    cudaGraphConditionalHandle rounds;
+    if (int rc = loop_handle(ctx, who, nullptr, &rounds)) return rc;
+    CU(launch_gnc_reweigh(nb, gp.live, phase, rounds, ctx->stream));
+    weights.use(nullptr);
+    if (int rc = round_head(ctx, o, stages, &rows)) return rc;
+    CU(launch_gnc_rmax(gp, ctx->sm_count, ctx->stream));
+    CU(launch_gnc_stage(gp, ctx->stream));
+    CU(launch_gnc_weight(gp, ctx->sm_count, ctx->stream));
+    CU(launch_gnc_init(gp, ao, state, poses, phase, ctx->stream));
+    CU(launch_gnc_loops(nb, gp.live, phase, stages, rounds, ctx->stream));
+    weights.use(gp.wstage);
+    return capture_loop(ctx, rounds, round_loop(ctx, o, [&](cudaGraphConditionalHandle h) {
+                          CU(launch_gnc_step(gp, ao, ctx->b_round.as<BatchRound>(), h, ctx->b_out.as<double>(), state, poses, phase, ctx->stream));
+                          return 0;
+                        }));
+  };
+  std::vector<unsigned char> key;
+  if (!capturing) {  // loop_key, plus the GNC options and every buffer the GNC kernels use
+    key = loop_key(ctx, o);
+    gnc_key(key, gp, {});
+  }
+  if (int rc = launch_loop(ctx, who, capturing, std::move(key), ctx->gnc_loop, stage)) return rc;
+  ctx->launches += 1;
+  if (int rc = clear_search_counters(ctx)) return rc;
+  CU(launch_batch_align_finish(nb, state, d_out_T, d_out_info, d_out_Hb, ctx->stream));
+  CU(launch_gnc_finish(nb, state, gp.gnc, d_out_info, d_out_gnc2, ctx->stream));
+  if (out_point_w && n) CU(cudaMemcpyAsync(out_point_w, gp.e, n * sizeof(double), cudaMemcpyDefault, ctx->stream));
+  ctx->b_dseed_ok = true;
+  // stage 0's reweighting round linearised every member; every round since used robust_kind (NONE)
+  mark_linearised(ctx, o->factor_kind, o->robust_kind, o->robust_c, nullptr);
+  return 0;
+}
+
+// The outputs of a synchronous GNC align from where it staged them to the caller's (host or device memory; a null one is skipped), then
+// the call's one synchronisation
+struct Staged {
+  double* out;
+  const double* staged;
+  size_t doubles;
+};
+int copy_staged(sgb_ctx* ctx, std::initializer_list<Staged> outputs) {
+  for (const Staged& s : outputs)
+    if (s.out) CU(cudaMemcpyAsync(s.out, s.staged, s.doubles * sizeof(double), cudaMemcpyDefault, ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));
+  return 0;
 }
 
 }  // namespace
@@ -1229,7 +1298,7 @@ int sgb_align_batch(sgb_ctx* ctx, const sgb_align_options* o, const double* init
     return rc;
   CU(cudaMemcpyAsync(state.data(), ctx->b_state.p, B * sizeof(MemberState), cudaMemcpyDeviceToHost, ctx->stream));
   CU(cudaStreamSynchronize(ctx->stream));
-  align_results(state, nullptr, out_T, out_info, out_Hb, nullptr);
+  align_results(state, out_T, out_info, out_Hb);
   return 0;
 }
 
@@ -1241,48 +1310,16 @@ int sgb_align_batch_gnc(sgb_ctx* ctx, const sgb_align_options* o, const sgb_gnc_
   if (int rc = gnc_checks(ctx, who, o, gnc, init_T, out_T, out_info, ao)) return rc;
   CU(cudaSetDevice(ctx->device));
   if (int rc = gnc_capture_check(ctx, who)) return rc;
-  const size_t B = batch_members(ctx), n = batch_points(ctx);
+  const size_t B = batch_members(ctx);
   if (B == 0) return 0;
-  if (int rc = pair_view(ctx)) return rc;
-  if (int rc = reserve_gnc(ctx, B)) return rc;
-  std::vector<MemberState> state;
-  std::vector<uint8_t> phase;
-  if (int rc = align_start(ctx, ao, init_T, state, phase)) return rc;
-  const GncParams gp = gnc_params(ctx, gnc);
-  if (int rc = gnc_begin(ctx, gp, B)) return rc;
-  const BatchRows rows = gnc_rows(gp);
-  RoundWeights weights(ctx);
-  std::vector<uint8_t> live(B, 1);
-  for (int stage = 0; std::find(live.begin(), live.end(), 1) != live.end(); stage++) {
-    // the reweighting linearize of the members in the stage at their current pose: unweighted, no robust kernel, its e rows to g_e
-    weights.use(nullptr);
-    if (int rc = linearize_round(ctx, o->factor_kind, SGB_ROBUST_NONE, o->robust_c, o->rejector_kind, o->max_dist_sq, nullptr, live.data(), &rows)) return rc;
-    if (stage == 0) {
-      CU(launch_gnc_rmax(gp, false, ctx->sm_count, ctx->stream));
-      ctx->launches += 1;
-    }
-    CU(launch_gnc_stage(gp, ctx->stream));
-    CU(launch_gnc_weight(gp, ctx->sm_count, ctx->stream));
-    CU(launch_gnc_init(gp, ao, ctx->b_state.as<MemberState>(), ctx->b_poses.as<double>(), ctx->b_phase.as<uint8_t>(), ctx->stream));
-    ctx->launches += 3;
-    CU(cudaMemcpyAsync(phase.data(), ctx->b_phase.p, B, cudaMemcpyDeviceToHost, ctx->stream));
-    CU(cudaMemcpyAsync(live.data(), gp.live, B, cudaMemcpyDeviceToHost, ctx->stream));
-    CU(cudaStreamSynchronize(ctx->stream));
-    // the stage's align with its weights
-    weights.use(gp.wstage);
-    if (int rc = align_rounds(ctx, o, phase, [&](bool lin) {
-          return launch_gnc_step(gp, ao, lin, nullptr, 0, ctx->b_out.as<double>(), ctx->b_state.as<MemberState>(), ctx->b_poses.as<double>(),
-                                 ctx->b_phase.as<uint8_t>(), ctx->stream);
-        }))
-      return rc;
-  }
-  std::vector<GncState> g(B);
-  CU(cudaMemcpyAsync(state.data(), ctx->b_state.p, B * sizeof(MemberState), cudaMemcpyDeviceToHost, ctx->stream));
-  CU(cudaMemcpyAsync(g.data(), gp.gnc, B * sizeof(GncState), cudaMemcpyDeviceToHost, ctx->stream));
-  if (out_point_w && n) CU(cudaMemcpyAsync(out_point_w, gp.e, n * sizeof(double), cudaMemcpyDefault, ctx->stream));
-  CU(cudaStreamSynchronize(ctx->stream));
-  align_results(state, g.data(), out_T, out_info, out_Hb, out_gnc2);
-  return 0;
+  // sgb_align_batch_gnc_async on the poses and outputs staged in device memory: init_T | T | info | H|b | gnc2, 80 doubles per member
+  CU(ctx->stage_pts.reserve(80 * B * sizeof(double)));
+  double* d_init_T = ctx->stage_pts.as<double>();
+  double *d_T = d_init_T + 16 * B, *d_info = d_T + 16 * B, *d_Hb = d_info + 4 * B, *d_gnc2 = d_Hb + 42 * B;
+  CU(cudaMemcpyAsync(d_init_T, init_T, 16 * B * sizeof(double), cudaMemcpyDefault, ctx->stream));
+  if (int rc = batch_gnc_enqueue(ctx, who.c_str(), false, o, gnc, ao, d_init_T, d_T, d_info, out_Hb ? d_Hb : nullptr, out_gnc2 ? d_gnc2 : nullptr, out_point_w))
+    return rc;
+  return copy_staged(ctx, {{out_T, d_T, 16 * B}, {out_info, d_info, 4 * B}, {out_Hb, d_Hb, 42 * B}, {out_gnc2, d_gnc2, 2 * B}});
 }
 
 int sgb_align_batch_gnc_async(sgb_ctx* ctx, const sgb_align_options* o, const sgb_gnc_options* gnc, const double* d_init_T, double* d_out_T, double* d_out_info,
@@ -1291,67 +1328,14 @@ int sgb_align_batch_gnc_async(sgb_ctx* ctx, const sgb_align_options* o, const sg
   const char* who = "sgb_align_batch_gnc_async";
   AlignOptions ao;
   if (int rc = gnc_checks(ctx, who, o, gnc, d_init_T, d_out_T, d_out_info, ao)) return rc;
-  const size_t B = batch_members(ctx), n = batch_points(ctx);
-  if (B == 0) return 0;
+  if (batch_members(ctx) == 0) return 0;
   CU(cudaSetDevice(ctx->device));
   if (int rc = device_pointers(ctx, who, {{d_init_T, "init_T16xB", true}, {d_out_T, "out_T16xB", true}, {d_out_info, "out_info4xB", true},
                                           {d_out_Hb, "out_Hb42xB", false}, {d_out_gnc2, "out_gnc2xB", false}, {d_out_point_w, "out_point_w", false}}))
     return rc;
   bool capturing = false;
   if (int rc = capture_state(ctx, who, &capturing)) return rc;
-  // the GNC buffers, the packet queue and both capture streams (the stages' loop and the rounds' loop nested in it)
-  if (int rc = loop_allocations(ctx, who, capturing, false, true, 2, B,
-                                ": this call needs an allocation, which a capture cannot hold; call it once outside the capture first"))
-    return rc;
-  if (int rc = pair_view(ctx)) return rc;
-  const GncParams gp = gnc_params(ctx, gnc);
-  const BatchRows rows = gnc_rows(gp);
-  const uint32_t nb = static_cast<uint32_t>(B);
-  MemberState* state = ctx->b_state.as<MemberState>();
-  double* poses = ctx->b_poses.as<double>();
-  uint8_t* phase = ctx->b_phase.as<uint8_t>();
-  // sgb_align_batch_gnc's initial state: every member's align_init at its initial pose, zero GNC state, every member live (the seed flags
-  // kept as sgb_align_batch_async keeps them)
-  CU(launch_batch_align_init(ao, nb, d_init_T, state, poses, phase, ctx->b_dseed.as<uint8_t>(), ctx->corr_seeds && ctx->b_dseed_ok, ctx->stream));
-  if (int rc = gnc_begin(ctx, gp, B)) return rc;
-  ctx->launches += 3;  // the initial state here, the outputs below
-  // One stage per iteration of the outer loop, in sgb_align_batch_gnc's order: the reweighting linearize of the members in the stage
-  // (planned by batch_plan_kernel from their phases), the stage kernels, then the stage's align as an inner loop of rounds.  After
-  // gnc_init, gnc_loops sets both conditions: the stages' while a member has a stage to go, the rounds' while a member's align has a round
-  // to go.
-  RoundWeights weights(ctx);
-  const auto stage = [&](cudaGraphConditionalHandle stages) {
-    cudaGraphConditionalHandle rounds;
-    if (int rc = loop_handle(ctx, who, nullptr, &rounds)) return rc;
-    CU(launch_gnc_reweigh(nb, gp.live, phase, rounds, ctx->stream));
-    weights.use(nullptr);
-    if (int rc = round_head(ctx, o, stages, &rows)) return rc;
-    CU(launch_gnc_rmax(gp, true, ctx->sm_count, ctx->stream));
-    CU(launch_gnc_stage(gp, ctx->stream));
-    CU(launch_gnc_weight(gp, ctx->sm_count, ctx->stream));
-    CU(launch_gnc_init(gp, ao, state, poses, phase, ctx->stream));
-    CU(launch_gnc_loops(nb, gp.live, phase, stages, rounds, ctx->stream));
-    weights.use(gp.wstage);
-    return capture_loop(ctx, rounds, round_loop(ctx, o, [&](cudaGraphConditionalHandle h) {
-                          CU(launch_gnc_step(gp, ao, true, ctx->b_round.as<BatchRound>(), h, ctx->b_out.as<double>(), state, poses, phase, ctx->stream));
-                          return 0;
-                        }));
-  };
-  std::vector<unsigned char> key;
-  if (!capturing) {  // loop_key, plus the GNC options and every buffer the GNC kernels use
-    key = loop_key(ctx, o);
-    gnc_key(key, gp, {});
-  }
-  if (int rc = launch_loop(ctx, who, capturing, std::move(key), ctx->gnc_loop, stage)) return rc;
-  ctx->launches += 1;
-  if (int rc = clear_search_counters(ctx)) return rc;
-  CU(launch_batch_align_finish(nb, state, d_out_T, d_out_info, d_out_Hb, ctx->stream));
-  CU(launch_gnc_finish(nb, state, gp.gnc, d_out_info, d_out_gnc2, ctx->stream));
-  if (d_out_point_w && n) CU(cudaMemcpyAsync(d_out_point_w, gp.e, n * sizeof(double), cudaMemcpyDeviceToDevice, ctx->stream));
-  ctx->b_dseed_ok = true;
-  // stage 0's reweighting round linearised every member, as sgb_align_batch_gnc's does; every round since used robust_kind (NONE)
-  mark_linearised(ctx, o->factor_kind, o->robust_kind, o->robust_c, nullptr);
-  return 0;
+  return batch_gnc_enqueue(ctx, who, capturing, o, gnc, ao, d_init_T, d_out_T, d_out_info, d_out_Hb, d_out_gnc2, d_out_point_w);
 }
 
 }  // extern "C"
@@ -1527,14 +1511,15 @@ int joint_rounds(sgb_ctx* ctx, const sgb_align_options* o, const JointLayout& L,
   }
 }
 
-// The window tables of layout L and the frames' X (host memory, column-major) uploaded to ctx->joint, its buffers reserved for L
+// The window tables of layout L and the frames' X (host memory, column-major; null: left to the caller) uploaded to ctx->joint, its
+// buffers reserved for L
 int joint_upload(sgb_ctx* ctx, const JointLayout& L, const double* X) {
   const std::vector<size_t> bytes = joint_bytes(L);
   const std::vector<DevBuf*> bufs = joint_buffers(ctx->joint);
   for (size_t i = 0; i < bufs.size(); i++) CU(bufs[i]->reserve(bytes[i]));
   // pageable host memory: the copies are staged before cudaMemcpyAsync returns
   CU(cudaMemcpyAsync(ctx->joint.tables.p, L.tab.data(), L.tab.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
-  if (L.K) CU(cudaMemcpyAsync(ctx->joint.X.p, X, L.K * 16 * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
+  if (L.K && X) CU(cudaMemcpyAsync(ctx->joint.X.p, X, L.K * 16 * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
   return 0;
 }
 
@@ -1549,39 +1534,123 @@ bool joint_async_stale(sgb_ctx* ctx, const JointLayout& L) {
   return L.tab != ctx->ja_tab;
 }
 
-// joint_async reserved for layout L, and its tables uploaded when upload (joint_async_stale).  ja_tab claims what joint_async.tables holds.
-// The claim is dropped before anything that can replace or lose that content: a reservation frees the old buffer before it allocates the
-// new one, and any step below may fail.  So a failed call leaves no claim behind, and the next call uploads its tables again.
-int joint_async_tables(sgb_ctx* ctx, const JointLayout& L, bool upload) {
+// joint_async reserved for layout L and its tables uploaded (when joint_async_stale: otherwise both are as L needs them already).  ja_tab
+// claims what joint_async.tables holds.  The claim is dropped before anything that can replace or lose that content: a reservation frees
+// the old buffer before it allocates the new one, and any step below may fail.  So a failed call leaves no claim behind, and the next call
+// uploads its tables again.
+int joint_async_tables(sgb_ctx* ctx, const JointLayout& L) {
   const std::vector<size_t> bytes = joint_bytes(L);
   const std::vector<DevBuf*> bufs = joint_buffers(ctx->joint_async);
-  if (upload) ctx->ja_tab.clear();
+  ctx->ja_tab.clear();
   for (size_t i = 0; i < bufs.size(); i++) CU(bufs[i]->reserve(bytes[i]));
-  if (upload) {
-    // pageable host memory: the copy is staged before cudaMemcpyAsync returns
-    CU(cudaMemcpyAsync(ctx->joint_async.tables.p, L.tab.data(), L.tab.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
-    ctx->ja_tab = L.tab;
-  }
+  // pageable host memory: the copy is staged before cudaMemcpyAsync returns
+  CU(cudaMemcpyAsync(ctx->joint_async.tables.p, L.tab.data(), L.tab.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
+  ctx->ja_tab = L.tab;
   return 0;
 }
 
-// The outputs of a joint align from the frames' final X and the windows' final state, a fixed frame's X as init_X gives it; gnc (or
-// null): the iterations of the windows' earlier GNC stages are added, and out_gnc2 (or null) gets each window's stages and mu
-void joint_results(const JointLayout& L, const double* init_X, const std::vector<double>& X, const std::vector<WindowState>& state, const GncState* gnc,
-                   double* out_X, double* out_info, double* out_gnc2) {
+// The outputs of a joint align from the frames' final X and the windows' final state, a fixed frame's X as init_X gives it
+void joint_results(const JointLayout& L, const double* init_X, const std::vector<double>& X, const std::vector<WindowState>& state, double* out_X,
+                   double* out_info) {
   const int32_t* freeidx = L.free();
   for (size_t k = 0; k < L.K; k++) std::memcpy(out_X + 16 * k, freeidx[k] < 0 ? init_X + 16 * k : X.data() + 16 * k, 16 * sizeof(double));
   for (size_t w = 0; w < L.W; w++) {
     double* info = out_info + 4 * w;
     info[0] = state[w].converged ? 1.0 : 0.0;
-    info[1] = state[w].iterations + (gnc ? gnc[w].iterations : 0);
+    info[1] = state[w].iterations;
     info[2] = state[w].inliers;
     info[3] = state[w].e;
-    if (out_gnc2) {
-      out_gnc2[2 * w] = gnc[w].stages;
-      out_gnc2[2 * w + 1] = gnc[w].mu;
-    }
   }
+}
+
+// The stream-ordered GNC of both joint GNC aligns, after their checks (who names the caller; capturing: ctx->stream is being captured):
+// the stages and their joint rounds as one device loop on the window buffers b, its graph cached in `graph`, from the frames at
+// d_init_X, the outputs to d_out_X, d_out_info and, unless null, d_out_gnc2 (device memory) and out_point_w (host or device memory).  b's
+// tables hold L's already, or (upload: b is joint_async and joint_async_stale) are uploaded here.  The loop key holds every address of b,
+// so each set of buffers keeps a graph of its own.
+int joint_gnc_enqueue(sgb_ctx* ctx, const char* who, bool capturing, bool upload, const sgb_align_options* o, const sgb_gnc_options* gnc, const AlignOptions& ao,
+                      const JointLayout& L, JointBufs& b, LoopGraph& graph, const double* d_init_X, double* d_out_X, double* d_out_info, double* d_out_gnc2,
+                      double* out_point_w) {
+  const size_t W = L.W, K = L.K, E = L.E, n = batch_points(ctx);
+  // A capture can hold neither an allocation nor an upload from pageable memory: the GNC buffers for W windows, joint_async's tables and
+  // buffers (uploaded only when they changed, as sgb_align_joint_async's), and with an edge the first batched call's search queue and both
+  // capture streams (the stages' loop and the rounds' loop nested in it) must come from an earlier call
+  if (int rc = loop_allocations(ctx, who, capturing, upload, E > 0, E ? 2 : 0, W,
+                                ": this call needs an allocation or an upload of its window tables, which a capture cannot hold; call it once outside "
+                                "the capture first"))
+    return rc;
+  if (upload) {
+    if (int rc = joint_async_tables(ctx, L)) return rc;
+  }
+  if (E) {
+    if (int rc = pair_view(ctx)) return rc;
+  }
+  const JointParams J = joint_params(ctx, b, W, E);
+  const uint32_t* member_win = b.tables.as<uint32_t>() + L.member_win_at();
+  // the GNC state per window: p for the point kernels (over the edges' points), pw for the window kernels
+  GncParams p = gnc_params(ctx, gnc);
+  p.live = reinterpret_cast<uint8_t*>(p.gnc + W);
+  GncParams pw = p;
+  pw.n_members = static_cast<uint32_t>(W);
+  uint8_t* member_phase = ctx->b_phase.as<uint8_t>();
+  // the initial state: the frames' X from d_init_X, zero window and GNC state (r2max = 0, no stage begun, no iterations), every window
+  // live; the device's seed flags kept as sgb_align_joint_async keeps them
+  if (K) CU(cudaMemcpyAsync(J.X, d_init_X, K * 16 * sizeof(double), cudaMemcpyDeviceToDevice, ctx->stream));
+  CU(cudaMemsetAsync(J.state, 0, W * sizeof(WindowState), ctx->stream));
+  if (int rc = gnc_begin(ctx, p, W)) return rc;
+  if (E && !(ctx->corr_seeds && ctx->b_dseed_ok)) CU(cudaMemsetAsync(ctx->b_dseed.p, 0, E, ctx->stream));
+  if (!E) {
+    // No edge, so no point: one stage of the stage kernels (r_max^2 = 0 makes it every window's last; the largest residual and the
+    // weights have nothing to visit) and no round
+    CU(launch_gnc_stage(pw, ctx->stream));
+    CU(launch_joint_gnc_init(pw, ao, J, ctx->stream));
+    ctx->launches += 2;
+  } else {
+    // One stage per iteration of the outer loop: the edge poses of every window's X, the reweighting linearize of the edges of the
+    // windows in the stage (planned by batch_plan_kernel from their member phases), the stage kernels, then the stage's joint align as an
+    // inner loop of rounds.  After joint_gnc_init, joint_gnc_loops gives every edge its window's phase and sets both conditions: the
+    // stages' while a window has a stage to go, the rounds' while a window's align has a round to go.
+    const BatchRows rows = gnc_rows(p);
+    RoundWeights weights(ctx);
+    const auto stage = [&](cudaGraphConditionalHandle stages) {
+      cudaGraphConditionalHandle rounds;
+      if (int rc = loop_handle(ctx, who, nullptr, &rounds)) return rc;
+      CU(launch_joint_edge_poses(J, ctx->stream));
+      CU(launch_joint_gnc_reweigh(J, p.live, member_phase, rounds, ctx->stream));
+      weights.use(nullptr);
+      if (int rc = round_head(ctx, o, stages, &rows)) return rc;
+      CU(launch_joint_gnc_rmax(p, member_win, ctx->sm_count, ctx->stream));
+      CU(launch_gnc_stage(pw, ctx->stream));
+      CU(launch_joint_gnc_weight(p, member_win, ctx->sm_count, ctx->stream));
+      CU(launch_joint_gnc_init(pw, ao, J, ctx->stream));
+      CU(launch_joint_gnc_loops(J, p.live, member_phase, stages, rounds, ctx->stream));
+      weights.use(p.wstage);
+      return capture_loop(ctx, rounds, round_loop(ctx, o, [&](cudaGraphConditionalHandle h) {
+                            CU(launch_joint_gnc_step(ao, J, L.max_free, ctx->b_out.as<double>(), pw, ctx->b_round.as<BatchRound>(), h, member_phase, ctx->stream));
+                            return 0;
+                          }));
+    };
+    std::vector<unsigned char> key;
+    if (!capturing) {  // loop_key, plus the GNC options, every buffer the GNC kernels use, JointParams, the frame count and max_free
+      key = loop_key(ctx, o);
+      gnc_key(key, p, {member_win});
+      key_add(key, J);
+      for (size_t v : {K, static_cast<size_t>(L.max_free)}) key_add(key, v);
+    }
+    if (int rc = launch_loop(ctx, who, capturing, std::move(key), graph, stage)) return rc;
+    ctx->launches += 1;
+    if (int rc = clear_search_counters(ctx)) return rc;
+  }
+  CU(launch_joint_align_finish(J, static_cast<uint32_t>(K), d_init_X, d_out_X, d_out_info, ctx->stream));
+  CU(launch_joint_gnc_finish(J, p.gnc, d_out_info, d_out_gnc2, ctx->stream));
+  ctx->launches += 2;
+  if (out_point_w && n) CU(cudaMemcpyAsync(out_point_w, p.e, n * sizeof(double), cudaMemcpyDefault, ctx->stream));
+  if (E) {
+    ctx->b_dseed_ok = true;
+    // stage 0's reweighting round linearised every edge (every window is in stage 0); every round since used robust_kind (NONE)
+    mark_linearised(ctx, o->factor_kind, o->robust_kind, o->robust_c, nullptr);
+  }
+  return 0;
 }
 
 }  // namespace
@@ -1623,7 +1692,7 @@ int sgb_align_joint(sgb_ctx* ctx, const sgb_align_options* o, size_t n_windows, 
   if (K) CU(cudaMemcpyAsync(X.data(), ctx->joint.X.p, K * 16 * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
   if (W) CU(cudaMemcpyAsync(state.data(), ctx->joint.state.p, W * sizeof(WindowState), cudaMemcpyDeviceToHost, ctx->stream));
   CU(cudaStreamSynchronize(ctx->stream));
-  joint_results(L, init_X, X, state, nullptr, out_X, out_info, nullptr);
+  joint_results(L, init_X, X, state, out_X, out_info);
   return 0;
 }
 
@@ -1665,69 +1734,19 @@ int sgb_align_joint_gnc(sgb_ctx* ctx, const sgb_align_options* o, const sgb_gnc_
   if (int rc = gnc_option_checks(ctx, who, o, gnc)) return rc;
   CU(cudaSetDevice(ctx->device));
   if (int rc = gnc_capture_check(ctx, who)) return rc;
-  const size_t W = L.W, K = L.K, E = L.E, n = batch_points(ctx);
+  const size_t W = L.W, K = L.K;
   if (W == 0) return 0;
-  if (E) {
-    if (int rc = pair_view(ctx)) return rc;
-  }
-  if (int rc = reserve_gnc(ctx, W)) return rc;
-  if (int rc = joint_upload(ctx, L, init_X)) return rc;
-  const JointParams J = joint_params(ctx, ctx->joint, W, E);
-  const uint32_t* member_win = ctx->joint.tables.as<uint32_t>() + L.member_win_at();
-  // the GNC state per window: p for the point kernels (over the edges' points), pw for the window kernels; every window starts its
-  // stage 0 with zero GNC and window state, live
-  GncParams p = gnc_params(ctx, gnc);
-  p.live = reinterpret_cast<uint8_t*>(p.gnc + W);
-  GncParams pw = p;
-  pw.n_members = static_cast<uint32_t>(W);
-  if (int rc = gnc_begin(ctx, p, W)) return rc;
-  CU(cudaMemsetAsync(ctx->joint.state.p, 0, W * sizeof(WindowState), ctx->stream));
-  const BatchRows rows = gnc_rows(p);
-  RoundWeights weights(ctx);
-  const uint32_t* edge_member = L.edge_member();
-  const uint32_t* edge_win = L.edge_win();
-  std::vector<uint8_t> live(W, 1), phase(W), active(E);
-  for (int stage = 0; std::find(live.begin(), live.end(), 1) != live.end(); stage++) {
-    // the edge poses of every window's X, then the reweighting linearize of the edges of the windows in the stage at them: unweighted,
-    // no robust kernel, its e rows to g_e
-    bool any = false;
-    for (size_t q = 0; q < E; q++) any |= (active[edge_member[q]] = live[edge_win[q]]) != 0;
-    if (E) {
-      CU(launch_joint_edge_poses(J, ctx->stream));
-      ctx->launches += 1;
-    }
-    weights.use(nullptr);
-    if (any) {
-      if (int rc = linearize_round(ctx, o->factor_kind, SGB_ROBUST_NONE, o->robust_c, o->rejector_kind, o->max_dist_sq, nullptr, active.data(), &rows)) return rc;
-    }
-    if (stage == 0) {
-      CU(launch_joint_gnc_rmax(p, member_win, false, ctx->sm_count, ctx->stream));
-      ctx->launches += 1;
-    }
-    CU(launch_gnc_stage(pw, ctx->stream));
-    CU(launch_joint_gnc_weight(p, member_win, ctx->sm_count, ctx->stream));
-    CU(launch_joint_gnc_init(pw, ao, J, ctx->stream));
-    ctx->launches += 3;
-    CU(cudaMemcpyAsync(phase.data(), ctx->joint.phase.p, W, cudaMemcpyDeviceToHost, ctx->stream));
-    CU(cudaMemcpyAsync(live.data(), p.live, W, cudaMemcpyDeviceToHost, ctx->stream));
-    CU(cudaStreamSynchronize(ctx->stream));
-    // the stage's joint align with its weights
-    weights.use(p.wstage);
-    if (int rc = joint_rounds(ctx, o, L, phase, [&](bool lin) {
-          return launch_joint_gnc_step(ao, J, L.max_free, lin, ctx->b_out.as<double>(), pw, nullptr, 0, nullptr, ctx->stream);
-        }))
-      return rc;
-  }
-  std::vector<double> X(16 * K);
-  std::vector<WindowState> state(W);
-  std::vector<GncState> g(W);
-  if (K) CU(cudaMemcpyAsync(X.data(), ctx->joint.X.p, K * 16 * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
-  CU(cudaMemcpyAsync(state.data(), ctx->joint.state.p, W * sizeof(WindowState), cudaMemcpyDeviceToHost, ctx->stream));
-  CU(cudaMemcpyAsync(g.data(), p.gnc, W * sizeof(GncState), cudaMemcpyDeviceToHost, ctx->stream));
-  if (out_point_w && n) CU(cudaMemcpyAsync(out_point_w, p.e, n * sizeof(double), cudaMemcpyDefault, ctx->stream));
-  CU(cudaStreamSynchronize(ctx->stream));
-  joint_results(L, init_X, X, state, g.data(), out_X, out_info, out_gnc2);
-  return 0;
+  // sgb_align_joint_gnc_async on the window tables of ctx->joint (never joint_async, which a captured asynchronous call may read) and the
+  // frames and outputs staged in device memory: init_X | X [frames][16] | info [windows][4] | gnc2 [windows][2]
+  CU(ctx->stage_pts.reserve((32 * K + 6 * W) * sizeof(double)));
+  double* d_init_X = ctx->stage_pts.as<double>();
+  double *d_X = d_init_X + 16 * K, *d_info = d_X + 16 * K, *d_gnc2 = d_info + 4 * W;
+  if (K) CU(cudaMemcpyAsync(d_init_X, init_X, 16 * K * sizeof(double), cudaMemcpyDefault, ctx->stream));
+  if (int rc = joint_upload(ctx, L, nullptr)) return rc;
+  if (int rc = joint_gnc_enqueue(ctx, who.c_str(), false, false, o, gnc, ao, L, ctx->joint, ctx->joint_gnc_sync_loop, d_init_X, d_X, d_info,
+                                 out_gnc2 ? d_gnc2 : nullptr, out_point_w))
+    return rc;
+  return copy_staged(ctx, {{out_X, d_X, 16 * K}, {out_info, d_info, 4 * W}, {out_gnc2, d_gnc2, 2 * W}});
 }
 
 int sgb_align_batch_async(sgb_ctx* ctx, const sgb_align_options* o, const double* d_init_T, double* d_out_T, double* d_out_info, double* d_out_Hb) {
@@ -1792,7 +1811,9 @@ int sgb_align_joint_async(sgb_ctx* ctx, const sgb_align_options* o, size_t n_win
                                 ": these windows need an allocation or an upload of their tables, which a capture cannot hold; call it once outside the "
                                 "capture first"))
     return rc;
-  if (int rc = joint_async_tables(ctx, L, upload)) return rc;
+  if (upload) {
+    if (int rc = joint_async_tables(ctx, L)) return rc;
+  }
   if (E) {
     if (int rc = pair_view(ctx)) return rc;
   }
@@ -1840,94 +1861,15 @@ int sgb_align_joint_gnc_async(sgb_ctx* ctx, const sgb_align_options* o, const sg
   JointLayout L;
   if (int rc = joint_layout(ctx, who, o, n_windows, window_off, fixed, d_init_X, d_out_X, d_out_info, ao, L)) return rc;
   if (int rc = gnc_option_checks(ctx, who, o, gnc)) return rc;
-  const size_t W = L.W, K = L.K, E = L.E, n = batch_points(ctx);
-  if (W == 0) return 0;
+  if (L.W == 0) return 0;
   CU(cudaSetDevice(ctx->device));
   if (int rc = device_pointers(ctx, who, {{d_init_X, "init_X16xK", true}, {d_out_X, "out_X16xK", true}, {d_out_info, "out_info4xW", true},
                                           {d_out_gnc2, "out_gnc2xW", false}, {d_out_point_w, "out_point_w", false}}))
     return rc;
   bool capturing = false;
   if (int rc = capture_state(ctx, who, &capturing)) return rc;
-  // A capture can hold neither an allocation nor an upload from pageable memory: the GNC buffers for W windows, the window tables and
-  // buffers (uploaded only when they changed, as sgb_align_joint_async's), and with an edge the first batched call's search queue and both
-  // capture streams (the stages' loop and the rounds' loop nested in it) must come from an earlier call
-  const bool upload = joint_async_stale(ctx, L);
-  if (int rc = loop_allocations(ctx, who, capturing, upload, E > 0, E ? 2 : 0, W,
-                                ": this call needs an allocation or an upload of its window tables, which a capture cannot hold; call it once outside "
-                                "the capture first"))
-    return rc;
-  if (int rc = joint_async_tables(ctx, L, upload)) return rc;
-  if (E) {
-    if (int rc = pair_view(ctx)) return rc;
-  }
-  const JointParams J = joint_params(ctx, ctx->joint_async, W, E);
-  const uint32_t* member_win = ctx->joint_async.tables.as<uint32_t>() + L.member_win_at();
-  // the GNC state per window, as sgb_align_joint_gnc's: p for the point kernels (over the edges' points), pw for the window kernels
-  GncParams p = gnc_params(ctx, gnc);
-  p.live = reinterpret_cast<uint8_t*>(p.gnc + W);
-  GncParams pw = p;
-  pw.n_members = static_cast<uint32_t>(W);
-  uint8_t* member_phase = ctx->b_phase.as<uint8_t>();
-  // sgb_align_joint_gnc's initial state: the frames' X from d_init_X, zero window and GNC state (r2max = 0, no stage begun, no iterations),
-  // every window live; the device's seed flags kept as sgb_align_joint_async keeps them
-  if (K) CU(cudaMemcpyAsync(J.X, d_init_X, K * 16 * sizeof(double), cudaMemcpyDeviceToDevice, ctx->stream));
-  CU(cudaMemsetAsync(J.state, 0, W * sizeof(WindowState), ctx->stream));
-  if (int rc = gnc_begin(ctx, p, W)) return rc;
-  if (E && !(ctx->corr_seeds && ctx->b_dseed_ok)) CU(cudaMemsetAsync(ctx->b_dseed.p, 0, E, ctx->stream));
-  if (!E) {
-    // No edge, so no point: sgb_align_joint_gnc's one stage of the stage kernels (r_max^2 = 0 makes it every window's last; the largest
-    // residual and the weights have nothing to visit) and no round
-    CU(launch_gnc_stage(pw, ctx->stream));
-    CU(launch_joint_gnc_init(pw, ao, J, ctx->stream));
-    ctx->launches += 2;
-  } else {
-    // One stage per iteration of the outer loop, in sgb_align_joint_gnc's order: the edge poses of every window's X, the reweighting
-    // linearize of the edges of the windows in the stage (planned by batch_plan_kernel from their member phases), the stage kernels, then
-    // the stage's joint align as an inner loop of rounds.  After joint_gnc_init, joint_gnc_loops gives every edge its window's phase and
-    // sets both conditions: the stages' while a window has a stage to go, the rounds' while a window's align has a round to go.
-    const BatchRows rows = gnc_rows(p);
-    RoundWeights weights(ctx);
-    const auto stage = [&](cudaGraphConditionalHandle stages) {
-      cudaGraphConditionalHandle rounds;
-      if (int rc = loop_handle(ctx, who.c_str(), nullptr, &rounds)) return rc;
-      CU(launch_joint_edge_poses(J, ctx->stream));
-      CU(launch_joint_gnc_reweigh(J, p.live, member_phase, rounds, ctx->stream));
-      weights.use(nullptr);
-      if (int rc = round_head(ctx, o, stages, &rows)) return rc;
-      CU(launch_joint_gnc_rmax(p, member_win, true, ctx->sm_count, ctx->stream));
-      CU(launch_gnc_stage(pw, ctx->stream));
-      CU(launch_joint_gnc_weight(p, member_win, ctx->sm_count, ctx->stream));
-      CU(launch_joint_gnc_init(pw, ao, J, ctx->stream));
-      CU(launch_joint_gnc_loops(J, p.live, member_phase, stages, rounds, ctx->stream));
-      weights.use(p.wstage);
-      return capture_loop(ctx, rounds, round_loop(ctx, o, [&](cudaGraphConditionalHandle h) {
-                            CU(launch_joint_gnc_step(ao, J, L.max_free, true, ctx->b_out.as<double>(), pw, ctx->b_round.as<BatchRound>(), h, member_phase,
-                                                     ctx->stream));
-                            return 0;
-                          }));
-    };
-    std::vector<unsigned char> key;
-    if (!capturing) {  // loop_key, plus the GNC options, every buffer the GNC kernels use, JointParams, the frame count and max_free
-      key = loop_key(ctx, o);
-      gnc_key(key, p, {member_win});
-      key_add(key, J);
-      for (size_t v : {K, static_cast<size_t>(L.max_free)}) key_add(key, v);
-    }
-    if (int rc = launch_loop(ctx, who.c_str(), capturing, std::move(key), ctx->joint_gnc_loop, stage)) return rc;
-    ctx->launches += 1;
-    if (int rc = clear_search_counters(ctx)) return rc;
-  }
-  CU(launch_joint_align_finish(J, static_cast<uint32_t>(K), d_init_X, d_out_X, d_out_info, ctx->stream));
-  CU(launch_joint_gnc_finish(J, p.gnc, d_out_info, d_out_gnc2, ctx->stream));
-  ctx->launches += 2;
-  if (d_out_point_w && n) CU(cudaMemcpyAsync(d_out_point_w, p.e, n * sizeof(double), cudaMemcpyDeviceToDevice, ctx->stream));
-  if (E) {
-    ctx->b_dseed_ok = true;
-    // stage 0's reweighting round linearised every edge (every window is in stage 0), as sgb_align_joint_gnc's does; every round since used
-    // robust_kind (NONE)
-    mark_linearised(ctx, o->factor_kind, o->robust_kind, o->robust_c, nullptr);
-  }
-  return 0;
+  return joint_gnc_enqueue(ctx, who.c_str(), capturing, joint_async_stale(ctx, L), o, gnc, ao, L, ctx->joint_async, ctx->joint_gnc_loop, d_init_X, d_out_X,
+                           d_out_info, d_out_gnc2, d_out_point_w);
 }
 
 int sgb_correspondences_batch(sgb_ctx* ctx, uint64_t* out) {

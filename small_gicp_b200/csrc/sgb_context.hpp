@@ -168,7 +168,8 @@ struct sgb_ctx {
   int src_tree_depth = 0;
 
   // ---- scratch: contents do not outlive the call that writes them ----
-  sgb::DevBuf stage_pts, stage_normals, stage_covs;  // raw double uploads
+  // raw double uploads, and the host poses and outputs of sgb_align_batch_gnc / sgb_align_joint_gnc staged in device memory (stage_pts)
+  sgb::DevBuf stage_pts, stage_normals, stage_covs;
   sgb::DevBuf keys_in, keys_out, vals_in, sort_temp;
   sgb::DevBuf corr, partials, ticket, corr64;
   sgb::DevBuf knn_tables;  // the set / entry tables of sgb_target_batch_knn_maps / _submaps
@@ -250,13 +251,14 @@ struct sgb_ctx {
   bool b_dseed_ok = false;
   cudaStream_t cap_stream = nullptr;
   cudaStream_t cap_stream_nested = nullptr;  // the stream the body of a loop nested in a loop's body is captured on
-  // sgb_align_joint: the buffers of its JointParams.  sgb_align_joint_async has its own (joint_async), which no other call writes: its
-  // tables are uploaded only when they differ from ja_tab, the host copy of what joint_async.tables holds.
+  // sgb_align_joint and sgb_align_joint_gnc: the buffers of their JointParams.  sgb_align_joint_async and sgb_align_joint_gnc_async have
+  // their own (joint_async), which no synchronous call writes: its tables are uploaded only when they differ from ja_tab, the host copy of
+  // what joint_async.tables holds.
   sgb::JointBufs joint, joint_async;
   std::vector<uint32_t> ja_tab;
-  // The instantiated loops of sgb_align_batch_async, sgb_align_joint_async and the loops of stages of sgb_align_batch_gnc_async and
-  // sgb_align_joint_gnc_async (the GNC calls use g_w, g_e and g_state as their synchronous twins do; the joint ones joint_async)
-  sgb::LoopGraph align_loop, joint_loop, gnc_loop, joint_gnc_loop;
+  // The instantiated loops of sgb_align_batch_async, sgb_align_joint_async and the loops of stages of both batch GNC aligns (gnc_loop: its
+  // graph reads no caller pointer), of sgb_align_joint_gnc_async (on joint_async) and of sgb_align_joint_gnc (joint_gnc_sync_loop, on joint)
+  sgb::LoopGraph align_loop, joint_loop, gnc_loop, joint_gnc_loop, joint_gnc_sync_loop;
 };
 
 namespace sgb {

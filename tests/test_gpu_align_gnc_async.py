@@ -1,21 +1,23 @@
 """Stream-ordered graduated non-convexity (sgb_align_batch_gnc_async, Context.align_batch_gnc_async): every stage and round on the device.
 
-  1. equality: T, info, H | b, stages, mu and every point's g are bit-identical to align_batch_gnc on a second context prepared alike, and
-     so are correspondences_batch and error_batch afterwards, over every target kind, factor, optimiser, GNC kind, with and without caller
-     weights, stage_iterations 1 and 3, max_iterations 0, 1 and 20;
-  2. degenerate schedules: TLS without outliers, max_stages = 1, an empty target;
-  3. batch sizes 1, 17 and 1024, and a permuted batch;
-  4. no host wait; capture in torch.cuda.graph and replay from new poses and new weights; calls in sequence never replay a stale graph;
-     the launch counter does not depend on the stage count;
+  1. model equality: every member's T, info, H | b, stages, mu and per-point g, and the correspondences and error_batch afterwards, are
+     bit-identical to the loop driven from the host with public calls on a context holding that member alone (np_gnc.host_gnc), over every
+     target kind, factor, optimiser, GNC kind, with and without caller weights, stage_iterations 1 and 3, max_iterations 0, 1 and 20;
+  2. degenerate schedules: TLS without outliers, max_stages = 1, an empty target, against the same model;
+  3. batch sizes 1, 17 and 1024, and a permuted batch, against the same model;
+  4. no host wait; capture in torch.cuda.graph and replay from new poses and new weights, and calls in sequence, each bit-identical to
+     align_batch_gnc on a second context prepared alike; calls in sequence never replay a stale graph; the launch counter does not
+     depend on the stage count;
   5. misuse fails with a message, enqueues nothing and leaves the weights in force."""
 import ctypes
 import itertools
+from types import SimpleNamespace
 
 import numpy as np
 import pytest
 
 import np_gnc as G
-from test_gpu_align_gnc import C2, KINDS, PLANE_KINDS, members, pair, poses, target
+from test_gpu_align_gnc import C2, FIELDS, KINDS, PLANE_KINDS, _rows, check_member, members, pair, poses, target
 from test_gpu_batch_points import LEAF, Scene
 from test_gpu_batch_weights import random_weights
 
@@ -77,6 +79,35 @@ def check(sync_ctx, async_ctx, T0, T1, c2, tag, **kw):
     return r, a
 
 
+def check_model(ctx, solo, member, T0, T1, c2, tag, w=None, **kw):
+    """align_batch_gnc_async on ctx with the weights w in force against np_gnc.host_gnc on solo, once per distinct member (member(p) pairs
+    solo with member p alone and names its cloud; a member without points is skipped, as the host loop has none to run): every member's
+    outputs bit for bit, and the correspondences and error_batch each leaves behind"""
+    ctx.set_source_weights(w)
+    a = ctx.align_batch_gnc_async(_dev(T0), c2, point_weights=True, **kw)
+    ctx.synchronize()
+    r = SimpleNamespace(**{f: getattr(a, f).cpu().numpy() for f in FIELDS + ("stages", "mu", "point_w")})
+    corr, e1 = ctx.correspondences_batch(), ctx.error_batch(T1)
+    model = dict(kw)
+    gnc = model.pop("gnc", G.TLS)
+    models = {}
+    for p in range(len(T0)):
+        rows = _rows(ctx, p)
+        if rows.start == rows.stop:
+            continue
+        ws = None if w is None else w[rows].copy()
+        cloud = member(p)
+        key = (cloud, T0[p].tobytes(), T1[p].tobytes(), None if ws is None else ws.tobytes())
+        if key not in models:
+            m = G.host_gnc(solo, T0[p], c2, kind=gnc, w=ws, **model)
+            models[key] = m, solo.correspondences_batch()[0], solo.error_batch(T1[p : p + 1])[0]
+        m, m_corr, m_e1 = models[key]
+        check_member(r, p, m, rows, tag)
+        assert np.array_equal(corr[p], m_corr), (tag, "correspondences", p)
+        _bits(e1[p], m_e1, (tag, "error_batch", p))
+    return r
+
+
 def compare(r, a, tag):
     """a GncAlignResult against an AsyncGncAlignResult, bit for bit"""
     for f in ("T_target_source", "H", "b", "error", "mu"):
@@ -94,17 +125,30 @@ def twins(s, kind):
     return c1, c2
 
 
-# ---- 1. equality with the synchronous call ----
+def solo_of(s, kind):
+    """a context holding the kind's target, and the member(p) of check_model that pairs it with member p of the kind's batch"""
+    solo = target(s, kind)
+
+    def member(p):
+        pair(solo, s, kind, p)
+        return p
+
+    return solo, member
+
+
+# ---- 1. equality with the host loop ----
 COMBOS = list(itertools.product((GN, LM), (G.GM, G.TLS), (False, True), (1, 3), (20, 1, 0)))
 
 
 @pytest.mark.parametrize("kind", KINDS)
-def test_equals_align_batch_gnc(scene, kind):
+def test_equals_the_host_loop(scene, kind):
     s = scene
-    c1, c2 = twins(s, kind)
+    ctx = _bind(target(s, kind))
+    pair(ctx, s, kind)
+    solo, member = solo_of(s, kind)
     cl = members(kind)
     T0, T1 = poses(s, cl), poses(s, cl, 1)
-    n = int(c1._batch_offsets[-1])
+    n = int(ctx._batch_offsets[-1])
     factors = (ICP, PLANE, GICP) if kind in PLANE_KINDS else (ICP, GICP)
     stages = []
     for fi, factor in enumerate(factors):
@@ -112,10 +156,8 @@ def test_equals_align_batch_gnc(scene, kind):
             opt, gnc, weighted, si, it = COMBOS[(7 * fi + 11 * ci + 3 * len(kind)) % len(COMBOS)]
             tag = (kind, factor, opt, gnc, weighted, si, it)
             w = random_weights(n, 5 + ci) if weighted else None
-            c1.set_source_weights(w)
-            c2.set_source_weights(w)
-            r, _ = check(c1, c2, T0, T1, C2[factor], tag, gnc=gnc, max_stages=40, stage_iterations=si, factor=factor, optimizer=opt,
-                         max_dist_sq=0.25, max_iterations=it)
+            r = check_model(ctx, solo, member, T0, T1, C2[factor], tag, w=w, gnc=gnc, max_stages=40, stage_iterations=si, factor=factor,
+                            optimizer=opt, max_dist_sq=0.25, max_iterations=it)
             stages.append(r.stages)
     st = np.concatenate(stages)
     print(kind, "stages: min", st.min(), "max", st.max())
@@ -125,16 +167,18 @@ def test_equals_align_batch_gnc(scene, kind):
 # ---- 2. degenerate schedules ----
 def test_degenerate_schedules(scene):
     s = scene
-    c1, c2 = twins(s, "kdtree")
+    ctx = _bind(target(s, "kdtree"))
+    solo, member = solo_of(s, "kdtree")
     cl = members("kdtree")
     T0, T1 = poses(s, cl), poses(s, cl, 1)
     # TLS without outliers: one stage of weights 1
     for factor, opt in ((ICP, GN), (GICP, LM), (PLANE, LM)):
-        r, _ = check(c1, c2, T0, T1, 1e30, ("tls without outliers", factor), gnc=G.TLS, factor=factor, optimizer=opt, max_dist_sq=1e6, max_iterations=10)
+        r = check_model(ctx, solo, member, T0, T1, 1e30, ("tls without outliers", factor), gnc=G.TLS, factor=factor, optimizer=opt, max_dist_sq=1e6,
+                        max_iterations=10)
         assert np.all(r.stages == 1) and np.all(r.mu == 0.0)
     # one stage
     for gnc in (G.GM, G.TLS):
-        r, _ = check(c1, c2, T0, T1, C2[GICP], ("one stage", gnc), gnc=gnc, max_stages=1, factor=GICP, max_dist_sq=0.25)
+        r = check_model(ctx, solo, member, T0, T1, C2[GICP], ("one stage", gnc), gnc=gnc, max_stages=1, factor=GICP, max_dist_sq=0.25)
         assert np.all(r.stages == 1)
 
 
@@ -147,28 +191,39 @@ def test_empty_target(scene):
         ctx.build_target_kdtree()
         ctx.set_source_batch(s.srcs, s.scovs)
         ctxs.append(ctx)
-    _bind(ctxs[1])
+    ctx, solo = _bind(ctxs[0]), ctxs[1]
+
+    def member(p):
+        solo.set_source_pairs([p])
+        return p
+
     cl = list(range(len(s.srcs)))
     for gnc in (G.GM, G.TLS):
-        check(ctxs[0], ctxs[1], poses(s, cl), poses(s, cl, 1), C2[GICP], ("empty target", gnc), gnc=gnc, factor=GICP, max_dist_sq=0.25)
+        check_model(ctx, solo, member, poses(s, cl), poses(s, cl, 1), C2[GICP], ("empty target", gnc), gnc=gnc, factor=GICP, max_dist_sq=0.25)
 
 
 # ---- 3. batch sizes ----
 @pytest.mark.parametrize("B", [1, 17, 1024])
 def test_batch_sizes(scene, B):
+    """every replica of a cloud at the cloud's poses and weights: one host loop per cloud is the model of all its replicas"""
     s = scene
-    c1, c2 = twins(s, "kdtree")
+    ctx = _bind(target(s, "kdtree"))
+    solo = target(s, "kdtree")
     rng = np.random.default_rng(B)
-    cl = [0, 1, 2, 4] if B == 1 else list(rng.permutation(np.resize([0, 1, 2, 4], B)))  # a permuted batch
-    cl = cl[:B]
-    c1.set_source_pairs(cl)
-    c2.set_source_pairs(cl)
-    n = int(c1._batch_offsets[-1])
-    w = random_weights(n, 3)
+    clouds = [0, 1, 2, 4]
+    cl = clouds[:B] if B == 1 else list(rng.permutation(np.resize(clouds, B)))  # a permuted batch
+    ctx.set_source_pairs(cl)
+
+    def member(p):
+        pair(solo, s, "kdtree", cl[p])
+        return cl[p]
+
+    T0, T1 = (dict(zip(clouds, poses(s, clouds, k))) for k in (0, 1))
+    cw = {c: random_weights(len(s.srcs[c]), 3 + c) for c in clouds}
+    w = np.concatenate([cw[c] for c in cl])
     for gnc, weights in ((G.TLS, None), (G.GM, w)):
-        c1.set_source_weights(weights)
-        c2.set_source_weights(weights)
-        check(c1, c2, poses(s, cl), poses(s, cl, 1), C2[GICP], ("B", B, gnc), gnc=gnc, factor=GICP, max_dist_sq=0.25)
+        check_model(ctx, solo, member, np.array([T0[c] for c in cl]), np.array([T1[c] for c in cl]), C2[GICP], ("B", B, gnc), w=weights, gnc=gnc,
+                    factor=GICP, max_dist_sq=0.25)
 
 
 # ---- 4. behaviour around the call ----

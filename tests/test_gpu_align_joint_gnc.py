@@ -8,7 +8,7 @@
   2. cross-checks: one free frame and one edge is align_batch_gnc of that edge; TLS without outliers is align_joint; max_stages = 1;
   3. windows are independent of the call (1, 17 and 1024 windows, permuted) and finish at their own stages;
   4. degenerate windows: no edge, no free frame, an edge-less free frame, every window done from the start;
-  5. state afterwards: the weights in force, also after a failing call; the launch counts of the documented formula;
+  5. state afterwards: the weights in force, also after a failing call; the documented launch count, 3 whatever the stages;
   6. misuse fails with a message, enqueues nothing and leaves the context usable;
   7. joint_edge_poses: a few ulps from numpy's X_j^-1 X_i, refused alike with align_joint;
   8. recovery: a LiDAR window with 30-50 % of every frame corrupted ends closer to ground truth under GNC than under align_joint."""
@@ -335,33 +335,8 @@ def test_weights_in_force_are_kept(scene):
         assert _bits(a, b)
 
 
-def _model_launches(solo, X, c2, gnc, fixed, **kw):
-    """the header's count from the host loop's own calls: per stage the edge poses (1), the reweighting linearize and the joint align's
-    rounds (align_joint's launches less its own edge-pose launch), plus 3; plus 1 for the largest residual"""
-    counts = []
-    calls = {k: getattr(solo, k) for k in ("joint_edge_poses", "linearize_batch_points", "align_joint")}
-
-    def count(f):
-        def g(*a, **k):
-            n0 = solo.kernel_launches
-            out = f(*a, **k)
-            counts.append(solo.kernel_launches - n0)
-            return out
-
-        return g
-
-    for k, f in calls.items():
-        setattr(solo, k, count(f))
-    try:
-        m = host_joint_gnc(solo, X, c2, fixed=fixed, kind=gnc, **kw)
-    finally:
-        for k in calls:
-            delattr(solo, k)
-    return m, sum(counts) - m.stages + 3 * m.stages + 1
-
-
 @pytest.mark.parametrize("kind", ["kdtree", "voxelmap1"])
-def test_launch_counts(scene, kind):
+def test_launch_count_is_constant(scene, kind):
     s = scene
     solo = s.context(WB.idx, kind, WB.edges)
     model = s.context(WB.idx, kind, WB.edges)
@@ -372,9 +347,8 @@ def test_launch_counts(scene, kind):
         n0 = solo.kernel_launches
         r = solo.align_joint_gnc(X, C2[GICP], fixed=WB.fixed, gnc=G.TLS, **align)
         got = solo.kernel_launches - n0
-        model.align_joint(X, fixed=WB.fixed, factor=GICP, max_dist_sq=1.0)  # (warm the model's context alike)
-        m, want = _model_launches(model, X, C2[GICP], G.TLS, WB.fixed, **align)
-        assert r.stages[0] == m.stages and got == want, (kind, kw, got, want, m.stages)
+        m = host_joint_gnc(model, X, C2[GICP], fixed=WB.fixed, kind=G.TLS, **align)
+        assert r.stages[0] == m.stages and got == 3, (kind, kw, got, m.stages)
 
 
 # ---- 6. misuse ----

@@ -1,25 +1,30 @@
 """Stream-ordered graduated non-convexity for joint windows (sgb_align_joint_gnc_async, Context.align_joint_gnc_async): every stage and
 joint round on the device.
 
-  1. equality: X, info, stages, mu and every edge point's g are bit-identical to align_joint_gnc on a second context prepared alike, and
-     so are correspondences_batch and error_batch afterwards, over many kd-trees and many voxel maps (1 and 7 offsets), ICP / point-to-plane
-     / GICP, GN and LM, GM and TLS, with and without caller weights, stage_iterations 1 and 3, max_iterations 0, 1 and 20, a DoF mask, and
-     windows of 3, 8 and 32 frames with a fixed frame that is not the first, edges both ways and a duplicate edge;
-  2. window counts 1, 17 and 1024 (permuted), windows finishing at different stages in one call;
-  3. degenerate windows: no edge, no free frame, an edge-less free frame, every window done from the start, a call with no edge at all;
-  4. no host wait; capture in torch.cuda.graph and replay from new poses and new weights, refusals inside a capture; calls in sequence
-     (options, windows, fixed flags, pairing, target, interleaved align_joint_async and align_batch_gnc_async) never replay a stale graph;
-     the launch counter does not depend on the stage count;
+  1. model equality: every window's X, info, stages, mu and per-point g, and the correspondences and error_batch afterwards, are
+     bit-identical to the loop driven from the host with public calls on a context holding that window alone (np_joint_gnc.host_joint_gnc),
+     over many kd-trees and many voxel maps (1 and 7 offsets), ICP / point-to-plane / GICP, GN and LM, GM and TLS, with and without caller
+     weights, stage_iterations 1 and 3, max_iterations 0, 1 and 20, a DoF mask, and windows of 3, 8 and 32 frames with a fixed frame that
+     is not the first, edges both ways and a duplicate edge;
+  2. window counts 1, 17 and 1024 (permuted), windows finishing at different stages in one call, against the same model;
+  3. degenerate windows: no edge, no free frame, an edge-less free frame, every window done from the start, a call with no edge at all:
+     the same model for a window with an edge, the stated result for one without;
+  4. no host wait; capture in torch.cuda.graph and replay from new poses and new weights, refusals inside a capture, and calls in sequence,
+     each bit-identical to align_joint_gnc on a second context prepared alike; calls in sequence (options, windows, fixed flags, pairing,
+     target, interleaved align_joint_async and align_batch_gnc_async) never replay a stale graph; the launch counter does not depend on
+     the stage count;
   5. misuse fails with a message, enqueues nothing and leaves the weights in force."""
 import ctypes
 import itertools
+from types import SimpleNamespace
 
 import numpy as np
 import pytest
 
 import np_gnc as G
 from test_gpu_align_joint import _perturbed
-from test_gpu_align_joint_gnc import C2, KINDS, MASK, WA, WB, WC, Scene, Window, multi
+from np_joint_gnc import host_joint_gnc
+from test_gpu_align_joint_gnc import C2, KINDS, MASK, WA, WB, WC, Scene, Window, _rows, check_window, multi
 from test_gpu_batch_weights import random_weights
 
 pytestmark = pytest.mark.gpu
@@ -91,6 +96,57 @@ def check(c1, c2, X, c2_, off, fixed, tag, **kw):
     return r, a
 
 
+def check_model(ctx, X, c2, off, fixed, er, solo, tag, w=None, **kw):
+    """align_joint_gnc_async on ctx with the weights w in force against np_joint_gnc.host_joint_gnc, once per distinct window: solo(k) is a
+    context holding window k alone and that window's name, or None for a window without an edge (no context can hold it alone: its result
+    is the stated one, X as given, no iteration, one stage at the first mu).  er: each window's edge range.  Every window's outputs bit for
+    bit, and the correspondences and error_batch at other edge poses each leaves behind."""
+    ctx.set_source_weights(w)
+    a = ctx.align_joint_gnc_async(_dev(X), c2, windows=off, fixed=fixed, point_weights=True, **kw)
+    ctx.synchronize()
+    r = SimpleNamespace(**{f: getattr(a, f).cpu().numpy() for f in ("X", "converged", "iterations", "num_inliers", "error", "stages", "mu", "point_w")})
+    corr = ctx.correspondences_batch()
+    E = ctx._batch_offsets.size - 1
+    T1 = ctx.joint_edge_poses(r.X, windows=off) if E else None
+    e1 = ctx.error_batch(T1) if E else None
+    model = dict(kw)
+    gnc = model.pop("gnc", G.TLS)
+    models = {}
+    for k, (e0, e1_) in enumerate(er):
+        f0, f1 = off[k], off[k + 1]
+        if e0 == e1_:
+            _bits(r.X[f0:f1], X[f0:f1], (tag, k, "X of a window without an edge"))
+            assert not r.converged[k] and r.iterations[k] == 0 and r.error[k] == 0 and r.num_inliers[k] == 0, (tag, k)
+            assert r.stages[k] == 1 and r.mu[k] == (1.0 if gnc == G.GM else 0.0), (tag, k)
+            continue
+        solo_ctx, name = solo(k)
+        rows = _rows(ctx, e0, e1_)
+        ws = None if w is None else w[rows].copy()
+        key = (name, X[f0:f1].tobytes(), T1[e0:e1_].tobytes(), None if ws is None else ws.tobytes())
+        if key not in models:
+            m = host_joint_gnc(solo_ctx, X[f0:f1], c2, fixed=list(fixed[f0:f1]), kind=gnc, w=ws, **model)
+            models[key] = m, solo_ctx.correspondences_batch(), solo_ctx.error_batch(T1[e0:e1_])
+        m, m_corr, m_e1 = models[key]
+        check_window(r, k, off, m, rows, tag)
+        for q, (x, y) in enumerate(zip(corr[e0:e1_], m_corr)):
+            assert np.array_equal(x, y), (tag, "correspondences", k, q)
+        _bits(e1[e0:e1_], m_e1, (tag, "error_batch", k))
+    return r
+
+
+def solos(s, wins, kind):
+    """solo(k) of check_model for the windows wins of multi(s, wins, kind): one context per distinct window"""
+    ctxs = {}
+
+    def solo(k):
+        w = wins[k]
+        if id(w) not in ctxs:
+            ctxs[id(w)] = s.context(w.idx, kind, w.edges)
+        return ctxs[id(w)], id(w)
+
+    return solo
+
+
 def twins(s, wins, kind):
     """two contexts holding the windows' frames and edges, the second bound to the current stream; the call's offsets, X and fixed flags"""
     c1, off, X, fixed, er = multi(s, wins, kind)
@@ -98,15 +154,18 @@ def twins(s, wins, kind):
     return c1, c2, off, X, fixed, er
 
 
-# ---- 1. equality with the synchronous call ----
+# ---- 1. equality with the host loop ----
 COMBOS = list(itertools.product((GN, LM), (G.GM, G.TLS), (False, True), (1, 3), (20, 1, 0), (None, MASK)))
 
 
 @pytest.mark.parametrize("kind", KINDS)
-def test_equals_align_joint_gnc(scene, kind):
+def test_equals_the_host_loop(scene, kind):
     s = scene
-    c1, c2, off, X, fixed, er = twins(s, (WA, WB, WC), kind)
-    n = int(c1._batch_offsets[-1])
+    wins = (WA, WB, WC)
+    ctx, off, X, fixed, er = multi(s, wins, kind)
+    _bind(ctx)
+    solo = solos(s, wins, kind)
+    n = int(ctx._batch_offsets[-1])
     factors = (ICP, PLANE, GICP) if kind == "kdtree" else (ICP, GICP)
     stages = []
     for fi, factor in enumerate(factors):
@@ -114,10 +173,8 @@ def test_equals_align_joint_gnc(scene, kind):
             opt, gnc, weighted, si, it, mask = COMBOS[(13 * fi + 29 * ci + 7 * KINDS.index(kind)) % len(COMBOS)]
             tag = (kind, factor, opt, gnc, weighted, si, it, mask)
             w = random_weights(n, 5 + ci) if weighted else None
-            c1.set_source_weights(w)
-            c2.set_source_weights(w)
-            r, _ = check(c1, c2, X, C2[factor], off, fixed, tag, gnc=gnc, stage_iterations=si, factor=factor, optimizer=opt, max_dist_sq=1.0,
-                         max_iterations=it, dof_mask=mask)
+            r = check_model(ctx, X, C2[factor], off, fixed, er, solo, tag, w=w, gnc=gnc, stage_iterations=si, factor=factor, optimizer=opt,
+                            max_dist_sq=1.0, max_iterations=it, dof_mask=mask)
             stages += list(r.stages)
     print(kind, "stages: min", min(stages), "max", max(stages))
     assert max(stages) > 10  # the schedules ran many stages
@@ -125,29 +182,35 @@ def test_equals_align_joint_gnc(scene, kind):
 
 def test_max_iterations_zero_and_one_stage(scene):
     s = scene
-    c1, c2, off, X, fixed, er = twins(s, (WA, WB), "kdtree")
+    wins = (WA, WB)
+    ctx, off, X, fixed, er = multi(s, wins, "kdtree")
+    _bind(ctx)
+    solo = solos(s, wins, "kdtree")
     for gnc in (G.GM, G.TLS):
         for kw in (dict(max_iterations=0), dict(max_stages=1), dict(max_stages=1, max_iterations=0), dict(stage_iterations=1, max_iterations=0)):
-            r, _ = check(c1, c2, X, C2[GICP], off, fixed, ("schedule", gnc, kw), gnc=gnc, factor=GICP, max_dist_sq=1.0, **kw)
+            r = check_model(ctx, X, C2[GICP], off, fixed, er, solo, ("schedule", gnc, kw), gnc=gnc, factor=GICP, max_dist_sq=1.0, **kw)
             if kw.get("max_stages") == 1:
                 assert np.all(r.stages == 1)
     # TLS without outliers: one stage of weights 1
-    r, _ = check(c1, c2, X, 1e30, off, fixed, "tls without outliers", gnc=G.TLS, factor=GICP, max_dist_sq=1e6, max_iterations=10)
+    r = check_model(ctx, X, 1e30, off, fixed, er, solo, "tls without outliers", gnc=G.TLS, factor=GICP, max_dist_sq=1e6, max_iterations=10)
     assert np.all(r.stages == 1) and np.all(r.mu == 0.0)
 
 
 # ---- 2. window counts ----
 @pytest.mark.parametrize("count,pool", [(1, "B"), (17, "ABD"), (1024, "D")])
 def test_window_counts(scene, count, pool):
+    """every window of a shape with that shape's weights: one host loop per shape is the model of all its windows"""
     s = scene
     shapes = {"A": WA, "B": WB, "D": Window([20, 21], [(1, 0)], [1, 0], 24)}
     names = [pool[i] for i in np.random.default_rng(count).integers(len(pool), size=count)]  # a permuted pairing of window shapes
-    c1, c2, off, X, fixed, er = twins(s, [shapes[k] for k in names], "kdtree")
-    w = random_weights(int(c1._batch_offsets[-1]), 3)
+    wins = [shapes[k] for k in names]
+    ctx, off, X, fixed, er = multi(s, wins, "kdtree")
+    _bind(ctx)
+    rows = {k: _rows(ctx, *r) for k, r in zip(names, er)}
+    sw = {k: random_weights(rows[k].stop - rows[k].start, 3 + i) for i, k in enumerate(shapes) if k in rows}
+    w = np.concatenate([sw[k] for k in names])
     for gnc, weights in ((G.TLS, None), (G.GM, w)):
-        c1.set_source_weights(weights)
-        c2.set_source_weights(weights)
-        r, _ = check(c1, c2, X, C2[GICP], off, fixed, (count, gnc), gnc=gnc, factor=GICP, max_dist_sq=1.0)
+        r = check_model(ctx, X, C2[GICP], off, fixed, er, solos(s, wins, "kdtree"), (count, gnc), w=weights, gnc=gnc, factor=GICP, max_dist_sq=1.0)
         if count == 17:
             assert len(set(r.stages)) > 1  # windows finished at different stages in one call
 
@@ -157,12 +220,22 @@ def test_degenerate_windows(scene):
     s = scene
     idx = [5, 6, 7, 8, 9, 10]
     X = _perturbed(s.fr, idx, 4)
-    c1, c2 = s.context(idx, "kdtree", [(1, 0), (4, 3)]), _bind(s.context(idx, "kdtree", [(1, 0), (4, 3)]))
+    ctx = _bind(s.context(idx, "kdtree", [(1, 0), (4, 3)]))
+    # each window with an edge alone, by its first frame: frames 0 .. 2 or 3 .. 4 of idx and its one edge 1 -> 0 (local)
+    alone = {f0: s.context(idx[f0:f1], "kdtree", [(1, 0)]) for f0, f1 in ((0, 3), (3, 5))}
+
+    def solo(off):
+        return lambda k: (alone[off[k]], off[k])
+
     for gnc in (G.GM, G.TLS):
         # windows: [] (empty) | [0, 1, 2] with edge 1 -> 0 and the edge-less free frame 2 | [3, 4] all fixed with an edge | [5] alone
-        check(c1, c2, X, C2[GICP], [0, 0, 3, 5, 6], [1, 0, 0, 1, 1, 0], ("degenerate", gnc), gnc=gnc, factor=GICP, max_dist_sq=1.0)
+        off = [0, 0, 3, 5, 6]
+        check_model(ctx, X, C2[GICP], off, [1, 0, 0, 1, 1, 0], [(0, 0), (0, 1), (1, 2), (2, 2)], solo(off), ("degenerate", gnc), gnc=gnc, factor=GICP,
+                    max_dist_sq=1.0)
         # every window done from the start
-        r, _ = check(c1, c2, X, C2[GICP], [0, 3, 5, 6], [1, 1, 1, 1, 1, 0], ("all done", gnc), gnc=gnc, factor=GICP, max_dist_sq=1.0)
+        off = [0, 3, 5, 6]
+        r = check_model(ctx, X, C2[GICP], off, [1, 1, 1, 1, 1, 0], [(0, 1), (1, 2), (2, 2)], solo(off), ("all done", gnc), gnc=gnc, factor=GICP,
+                        max_dist_sq=1.0)
         assert np.all(r.iterations == 0)
 
 
@@ -172,13 +245,12 @@ def test_call_without_edges(scene):
     idx = [11, 12, 13]
     X = _perturbed(s.fr, idx, 5)
     none = np.zeros(0, dtype=np.uint32)
-    c1, c2 = s.context(idx, "voxelmap1", [(1, 0)]), _bind(s.context(idx, "voxelmap1", [(1, 0)]))
-    for c in (c1, c2):
-        c.set_source_pairs(none, none)
+    ctx = _bind(s.context(idx, "voxelmap1", [(1, 0)]))
+    ctx.set_source_pairs(none, none)
     for gnc, mu in ((G.GM, 1.0), (G.TLS, 0.0)):
-        n0 = c2.kernel_launches
-        r, a = check(c1, c2, X, C2[GICP], [0, 2, 3], [1, 0, 0], ("no edge", gnc), gnc=gnc, factor=GICP, max_dist_sq=1.0)
-        assert c2.kernel_launches - n0 == 4
+        n0 = ctx.kernel_launches
+        r = check_model(ctx, X, C2[GICP], [0, 2, 3], [1, 0, 0], [(0, 0), (0, 0)], None, ("no edge", gnc), gnc=gnc, factor=GICP, max_dist_sq=1.0)
+        assert ctx.kernel_launches - n0 == 4
         _bits(r.X, X, "initial poses")
         assert np.all(r.stages == 1) and np.all(r.mu == mu) and np.all(r.iterations == 0) and not np.any(r.converged)
 
